@@ -199,7 +199,7 @@ def run(args, ClockSampler):
                       "autocast": "bf16", "memory_format": "channels_last",
                       "torch": torch.__version__, "torchvision": torchvision.__version__,
                       "cudnn": torch.backends.cudnn.version(),
-                      "l2": "no flush: per-step activations (GBs) exceed the 126 MB L2"},
+                      "l2": "no flush: per-step activations (GBs) exceed the 50 MB L2"},
            "clocks": clocks, "gpu_launches": 0, "final_loss": float(loss_buf)}
     if e2e is not None:
       out["e2e"] = e2e

@@ -10,9 +10,9 @@ Metric / config: BASELINE.json - ResNet-50, ImageNet-shaped synthetic data
 Timed region: exactly K training steps (decode/normalise -> forward -> loss ->
 backward -> fused all-reduce + optimizer) bracketed by barrier + synchronize,
 timed with CUDA events on the launching stream, max over ranks.  The step is
-replayed from a CUDA graph; every kernel in it is one of this repo's sm_100a
+replayed from a CUDA graph; every kernel in it is one of this repo's sm_90a
 kernels (no cuDNN / cuBLAS / NCCL call inside the timed region).  Activations
-(GBs per step) far exceed the 126 MB L2, so no explicit L2 flush is needed.
+(GBs per step) far exceed the 50 MB L2 of an H100, so no explicit L2 flush is needed.
 
 `e2e`: the same metric through the public trainer API with, every step, the
 host->device copy of that step's batch from pinned host memory (side stream,
@@ -51,8 +51,35 @@ def parse_args():
   p.add_argument("--no-graph", action="store_true")
   p.add_argument("--no-e2e", action="store_true")
   p.add_argument("--profile-step", action="store_true",
-                 help="run a few eager steps only (for ncu captures)")
+                 help="run a few eager steps only (for profiler captures)")
+  p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                 help="after the timed steps, write what the last timed step computed as "
+                      "DIR/<name>.npy (float32): the loss, the logits, a fixed seeded sample of the "
+                      "updated fp32 master weights and the batch-norm running statistics")
   return p.parse_args()
+
+
+DUMP_WEIGHT_SAMPLE = 1 << 22   # 16 MB of fp32 master weights (ResNet-50 has 25.6 M parameters)
+
+
+def dump_outputs(net, out_dir):
+  """What a caller of ResNetTrainer.train_step receives from the last timed step: the step's loss
+  and logits and the parameters it updated.  The weight sample uses fixed indices (seed 0) so two
+  builds can be compared element for element."""
+  import numpy as np
+  import torch
+  os.makedirs(out_dir, exist_ok=True)
+  master = net.store.master.detach()
+  n = master.numel()
+  if n > DUMP_WEIGHT_SAMPLE:
+    g = torch.Generator(device="cpu")
+    g.manual_seed(0)
+    idx = torch.randperm(n, generator=g)[:DUMP_WEIGHT_SAMPLE].sort().values.to(master.device)
+    master = master[idx]
+  arrays = {"loss": net.loss_sum, "logits": net.logits, "master_weights_sample": master,
+            "bn_running_stats": net.running.tensor()}
+  for name, t in arrays.items():
+    np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 class ClockSampler(object):
@@ -105,7 +132,7 @@ class ClockSampler(object):
 
 def measured_baseline(n_gpus, key="value"):
   """Same-box NCCL + cuDNN comparator numbers (baseline/nccl_cudnn_measured.json, written from
-  `bench.py --impl nccl-cudnn` runs on the B200 pod; BASELINE.md section 4).  The reference
+  `bench.py --impl nccl-cudnn` runs on the same machine; BASELINE.md section 4).  The reference
   publishes no numbers, so this is the BASELINE.md figure `vs_baseline` divides by."""
   try:
     with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "baseline",
@@ -283,6 +310,8 @@ def main():
   clocks = sampler.stop()
   ms = ev0.elapsed_time(ev1)
   loss = float(net.loss_sum)
+  if args.dump_outputs and rank == 0:
+    dump_outputs(net, args.dump_outputs)
   t = torch.tensor([ms], device=dev)
   if dist is not None:
     dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -398,7 +427,7 @@ def main():
         "steps": args.steps, "warmup": max(3, args.warmup), "ms_per_step": ms_per_step,
         "higher_is_better": True, "scaling": "weak",
         "vs_baseline": (value / base) if base else None, "dtype": "bf16",
-        "baseline": {"what": "stock torchvision + cuDNN + DDP/NCCL on the same pod "
+        "baseline": {"what": "stock torchvision + cuDNN + DDP/NCCL on the same machine "
                              "(bench.py --impl nccl-cudnn; BASELINE.md section 4)",
                      "images_per_s": base, "e2e_images_per_s": measured_baseline(world, "e2e")},
         "data": "synthetic (uint8 224x224x3 ImageNet-shaped, random-init weights)",
@@ -408,7 +437,7 @@ def main():
                    "parallelism": "dp{}".format(world),
                    "optimizer": "momentum-sgd fused with the gradient all-reduce",
                    "cuda_graph": not args.no_graph,
-                   "l2": "no flush: per-step activations (GBs) exceed the 126 MB L2"},
+                   "l2": "no flush: per-step activations (GBs) exceed the 50 MB L2"},
         "clocks": clocks, "gpu_launches": launches_per_step * args.steps,
         "launches_per_step": launches_per_step, "final_loss": loss,
     }
@@ -430,7 +459,7 @@ def main():
 
 
 def supervised_main():
-  """Single-process runs (the driver's N = 1 arm, `python bench.py ...`) are executed in a child
+  """Single-process runs (`python bench.py ...`) are executed in a child
   process under a timeout and retried once: a stalled box must cost one retry, not the headline
   number.  torchrun ranks (WORLD_SIZE set) and the reference arm run directly."""
   args = parse_args()

@@ -1,5 +1,5 @@
 """Batch inference of ResNet-50 THROUGH ``pipeline.TFModel.transform`` (BASELINE.json config
-"TFParallel batch inference ResNet-50 on 8xB200 (pipeline.TFModel)"; reference hot loop:
+"TFParallel batch inference ResNet-50 on 8xH100 (pipeline.TFModel)"; reference hot loop:
 tensorflowonspark/pipeline.py:618-645 and TFModel.scala:245-292).
 
 A DataFrame with one binary column (a uint8 224x224x3 image per row) is transformed by a TFModel

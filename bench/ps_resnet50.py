@@ -2,7 +2,7 @@
 parameters, the optimizer state (momentum) and a bf16 serving copy + (N-1) workers that pull with
 peer loads and push gradients into their slots on the PS GPU with one-way NVLink stores; no
 barrier between workers (BASELINE.json config "ResNet-50 async parameter-server (1 PS + 7
-workers) on 8xB200"; reference: ParameterServerStrategy in
+workers) on 8xH100"; reference: ParameterServerStrategy in
 examples/mnist/estimator/mnist_spark_streaming.py:86,139 - any optimizer, state on the ps).
 
   python bench/ps_resnet50.py --gpus 8 --batch 256 --steps 20
@@ -137,7 +137,7 @@ def run(gpus, batch=256, steps=20, warmup=3, lr=0.01, optimizer="momentum"):
       "config": {"model": "resnet50_v1.5", "global_batch": batch * workers, "per_gpu_batch": batch,
                  "parallelism": "async parameter server: 1 ps + {} workers".format(workers),
                  "optimizer": "{} with state resident on the ps GPU (slot mode)".format(optimizer),
-                 "cuda_graph": False, "l2": "no flush: per-step activations exceed the 126 MB L2"},
+                 "cuda_graph": False, "l2": "no flush: per-step activations exceed the 50 MB L2"},
       "clocks": {"sm_mhz": min(sm) if sm else None, "sm_max_mhz": max(
           [r["clocks"].get("sm_max_mhz") or 0 for r in res]), "reasons": reasons},
       "gpu_launches": None,

@@ -1,7 +1,7 @@
 """Segmentation U-Net fed through InputMode.SPARK: rows travel RDD -> feeder task -> shared-memory
 ring (page-locked by the consumer) -> ``cudaMemcpyAsync`` straight from the ring slot on the copy
 stream -> native U-Net step, all through ``TFNode.DataFeed`` (BASELINE.json config "segmentation
-U-Net InputMode.SPARK DataFeed queue on 8xB200"; the reference's loop being replaced is
+U-Net InputMode.SPARK DataFeed queue on 8xH100"; the reference's loop being replaced is
 tensorflowonspark/TFSparkNode.py:500-502 feeder side, TFNode.py:278-300 consumer side).
 
   python bench/unet_datafeed.py --gpus 8 --batch 64 --steps 60

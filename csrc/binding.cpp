@@ -1,4 +1,4 @@
-// Python bindings (torch extension) for the sm_100a kernels.  Only this file
+// Python bindings (torch extension) for the sm_90a kernels.  Only this file
 // includes torch headers; the .cu files are plain CUDA so they rebuild in
 // seconds.  Every op runs on the caller's current CUDA stream.
 #include <ATen/cuda/CUDAContext.h>
@@ -43,7 +43,7 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    TORCH_CHECK(n > 0, "no CUDA device: cannot query the SM count");
   }
   return n;
 }
@@ -169,7 +169,6 @@ int64_t plan_wgrad(const py::dict& a, const py::dict& b, const py::dict& g, int 
   fill_ints(g, "acc_box", w.acc_box, tfos::kMaxTaps);
   fill_ints(g, "acc_row", w.acc_row, tfos::kMaxTaps);
   fill_ints(g, "box_dw", w.box_dw, 3);
-  w.wide = geti<int>(g, "wide", 0);
   w.dw = reinterpret_cast<float*>(geti<uint64_t>(g, "dw", 0));
   TORCH_CHECK(w.dw != nullptr && w.ldw > 0, "igemm wgrad: dw/ldw");
   char err[512] = {0};
@@ -194,7 +193,6 @@ py::dict plan_info(int64_t h) {
   d["bn"] = p->bn;
   d["grid"] = p->grid;
   d["total_work"] = p->total_work;
-  d["cta_group"] = p->cta_group;
   return d;
 }
 
@@ -646,7 +644,7 @@ Tensor tensor_from_ptr(uint64_t ptr, std::vector<int64_t> sizes, const std::stri
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "tensorflowonspark_b200 native sm_100a kernels";
+  m.doc() = "tensorflowonspark_b200 native sm_90a kernels";
   m.def("igemm_plan_fwd", &plan_fwd);
   m.def("igemm_plan_wgrad", &plan_wgrad);
   m.def("igemm_run", &plan_run);

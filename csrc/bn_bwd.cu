@@ -33,7 +33,7 @@ __device__ __forceinline__ float2 masked_g(int relu, uint32_t gw, float2 xv, uin
                                            uint32_t mbits, int j, float2 fs, float2 fh) {
   float2 g = up2(gw);
   if (relu == 2) {
-    const float2 pre = __ffma2_rn(xv, fs, fh);
+    const float2 pre = ffma2_rn(xv, fs, fh);
     g.x = pre.x > 0.f ? g.x : 0.f;
     g.y = pre.y > 0.f ? g.y : 0.f;
   } else if (relu == 1) {
@@ -109,8 +109,8 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
           for (int j = 0; j < 4; ++j) {
             const float2 xv = up2(xw[j]);
             const float2 gj = masked_g(relu, gw[j], xv, yw[j], mq[k], j, fs[j], fh[j]);
-            a0[j] = __ffma2_rn(gj, __fadd2_rn(xv, nmu[j]), a0[j]);
-            a1[j] = __fadd2_rn(a1[j], gj);
+            a0[j] = ffma2_rn(gj, fadd2_rn(xv, nmu[j]), a0[j]);
+            a1[j] = fadd2_rn(a1[j], gj);
           }
         }
       }
@@ -229,7 +229,7 @@ bn_bwd_apply_kernel(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x
         for (int j = 0; j < 4; ++j) {
           const float2 xv = up2(xw[j]);
           const float2 gj = masked_g(relu, gw[j], xv, yw[j], mq[k], j, fs[j], fh[j]);
-          const float2 ov = __ffma2_rn(cA[j], gj, __ffma2_rn(cB[j], xv, cK[j]));
+          const float2 ov = ffma2_rn(cA[j], gj, ffma2_rn(cB[j], xv, cK[j]));
           ow[j] = pack_bf16x2(ov.x, ov.y);
           rw[j] = pack_bf16x2(gj.x, gj.y);
         }
@@ -318,11 +318,11 @@ bn_fwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __
         uint32_t ow[4], bits = 0;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          float2 v = __ffma2_rn(make_float2(__uint_as_float(xw[j] << 16),
+          float2 v = ffma2_rn(make_float2(__uint_as_float(xw[j] << 16),
                                             __uint_as_float(xw[j] & 0xffff0000u)),
                                 sc[j], sh[j]);
           if (has_res)
-            v = __fadd2_rn(v, make_float2(__uint_as_float(rw[j] << 16),
+            v = fadd2_rn(v, make_float2(__uint_as_float(rw[j] << 16),
                                           __uint_as_float(rw[j] & 0xffff0000u)));
           bits |= (v.x > 0.f ? 1u : 0u) << (2 * j);
           bits |= (v.y > 0.f ? 1u : 0u) << (2 * j + 1);
@@ -339,7 +339,7 @@ bn_fwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __
 
 // L2 hand-over hint (see bn_set_row_reverse in ops.h): the next launches walk the rows from the
 // END of the tensor - that is where the kernel that produced (or last read) it stopped, so the
-// first ~L2-size worth of reads hit the 126 MB L2 instead of HBM.  Host state, read at launch
+// first ~L2-size worth of reads hit the 50 MB L2 instead of HBM.  Host state, read at launch
 // time (and therefore baked into a captured CUDA graph).
 int g_row_reverse = 0;
 
@@ -349,13 +349,13 @@ inline dim3 red_grid(long long P, int C, int waves) {
   const int rl = kThreads / cg;
   long long bx = (P + rl - 1) / rl;
   const int gy = (groups + cg - 1) / cg;
-  const long long cap = (148 * waves + gy - 1) / gy;
+  const long long cap = (kSmCount * waves + gy - 1) / gy;
   if (bx > cap) bx = cap;
   if (bx < 1) bx = 1;
   return dim3(static_cast<unsigned>(bx), static_cast<unsigned>(gy));
 }
 
-// grid = resident blocks per SM (launch bounds: 2) x 148 SMs x waves; tunable for experiments
+// grid = resident blocks per SM (launch bounds: 2) x kSmCount SMs x waves; tunable for experiments
 inline int env_waves(const char* name, int dflt) {
   const char* v = getenv(name);
   return v != nullptr && atoi(v) > 0 ? atoi(v) : dflt;

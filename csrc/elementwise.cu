@@ -662,7 +662,7 @@ inline int grid_for(long long work, int threads, int max_blocks) {
   if (b < 1) b = 1;
   return static_cast<int>(b < max_blocks ? b : max_blocks);
 }
-constexpr int kMaxBlocks = 148 * 8;
+constexpr int kMaxBlocks = kSmCount * 8;
 
 inline dim3 red_grid(long long P, int C, int waves = 4) {
   const int groups = C >> 3;
@@ -670,7 +670,7 @@ inline dim3 red_grid(long long P, int C, int waves = 4) {
   const int rl = kRedThreads / cg;
   long long bx = (P + rl - 1) / rl;
   const int gy = (groups + cg - 1) / cg;
-  const long long cap = (148 * waves + gy - 1) / gy;
+  const long long cap = (kSmCount * waves + gy - 1) / gy;
   if (bx > cap) bx = cap;
   if (bx < 1) bx = 1;
   return dim3(static_cast<unsigned>(bx), static_cast<unsigned>(gy));

@@ -1,6 +1,6 @@
-// tcgen05 / TMEM / TMA implicit-GEMM kernels for sm_100a: the "forward-like" kernel
-// (fprop, dgrad, transposed conv, dense GEMM) and the host-side plan code.  The
-// weight-gradient kernel lives in igemm_wgrad.cu.
+// wgmma / TMA implicit-GEMM kernels for sm_90a: the "forward-like" kernel (fprop,
+// dgrad, transposed conv, dense GEMM) and the host-side plan code.  The
+// weight-gradient kernels live in igemm_wgrad.cu.
 //
 // Replaces what the reference reaches through TensorFlow -> cuDNN/cuBLAS for
 // its example models (SURVEY.md section 2.6(b): conv fprop/dgrad/wgrad, dense
@@ -8,21 +8,18 @@
 // examples/resnet/resnet_cifar_dist.py:208, examples/segmentation/
 // segmentation_spark.py:67-119).
 //
-// Structure: 320 threads = 10 warps, one CTA per SM, persistent over a static
-// round-robin tile list.
-//   warp 0   : TMA producer  (one lane issues cp.async.bulk.tensor into a smem ring)
-//   warp 1   : TMEM allocator + MMA issuer (one lane issues tcgen05.mma; the
-//              accumulator lives in TMEM, double-buffered across tiles)
-//   warps 2-9: epilogue.  Two warps share each TMEM lane quarter and split the
-//              64-column slabs between them (two warps per scheduler: the epilogue
-//              is instruction-latency bound with one).  tcgen05.ld -> bias / ReLU /
-//              bf16 rounding -> XOR-swizzled smem slab -> (a) per-column sum and
-//              sum of squares for the fused batch-norm statistics, read back
-//              column-wise, (b) coalesced global stores, 4 rows x 128 B per warp
-//              instruction, with optional read-modify-write accumulation.
-// Pipelines: smem full/empty mbarriers between TMA and MMA; TMEM full/empty
-// mbarriers between MMA and epilogue, so the epilogue of tile i overlaps the
-// main loop of tile i+1.
+// Structure: 384 threads = 3 warpgroups, one CTA per SM, persistent over a static
+// round-robin tile list of 128 x BN output tiles.
+//   warpgroup 0   : TMA producer (one lane issues cp.async.bulk.tensor into a smem ring)
+//   warpgroups 1-2: consumers.  Warpgroup g owns rows [64 g, 64 g + 64) of the tile: it
+//                   issues wgmma m64nBNk16 on the shared A / B stages, keeps its fp32
+//                   accumulator in registers and runs the epilogue straight from them
+//                   (bias / ReLU / bf16 rounding / read-modify-write accumulation / fused
+//                   per-column statistics, see igemm.h).
+// Pipeline: smem full/empty mbarriers between the producer and the consumers; a stage is
+// released as soon as the wgmma group that read it has retired, so the producer runs up to
+// a ring ahead - across tile boundaries, i.e. the next tile's operands arrive during the
+// epilogue of the current one.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -38,34 +35,27 @@ cudaError_t igemm_run_wgrad(const IGemmPlan* p, cudaStream_t s);  // igemm_wgrad
 
 namespace {
 
-constexpr int kThreads = 320;
-constexpr int kEpiWarps = 8;
-constexpr int kEpiThreads = kEpiWarps * 32;
+constexpr int kThreads = 384;
+constexpr int kConsumerThreads = 256;
 constexpr int kBlockM = 128;
 constexpr int kABytes = kBlockM * 128;  // 128 rows x 64 bf16
 
-// CG = 2: CTA pair (cta_group::2, see ptx.cuh): each CTA stages its own 128 A rows and HALF of the
-// B tile, the leader issues M = 256 MMAs - half the B bytes per MAC from shared memory and from
-// the L2 -> SM fabric, which is what bounds the 3x3 layers (profiles/ncu_l3c2_r1.txt).
-template <int BN, int CG = 1>
+template <int BN>
 struct FwdCfg {
-  static constexpr int kBBytes = BN * 128 / CG;
+  static constexpr int kBBytes = BN * 128;
   static constexpr int kStage = kABytes + kBBytes;
-  static constexpr int kStages = (BN <= 64) ? 8 : (BN <= 128 ? 6 : (CG == 2 ? 6 : 4));
-  static constexpr int kTmemCols = 2 * BN;  // double-buffered fp32 accumulator
+  static constexpr int kStages = (BN <= 64) ? 8 : (BN <= 128 ? 6 : 4);
   static constexpr int kStatBytes = BN * 2 * 4;
-  static constexpr int kOutStageBytes = kEpiWarps * 4096;  // per warp: 32 rows x 128 B
-  static constexpr int kSmem = kStages * kStage + kStatBytes + kOutStageBytes + 256;
+  static constexpr int kSmem = kStages * kStage + kStatBytes + 256;
 };
 // Weight-stationary mode: when all K blocks of a CTA's B (filter) tile fit next to >= 4 A stages,
 // B is loaded once per CTA and only A streams - the per-tile L2 traffic of the small-K layers
-// (1x1 convolutions, 64-channel 3x3) drops by the B share (up to 2/3), which matters because
-// those layers are bound by the ~6 KB/clk L2->SM fabric, not by HBM or the tensor pipe.
+// (1x1 convolutions, 64-channel 3x3) drops by the B share (up to 2/3).
 constexpr int kMaxStages = 12;
 constexpr int kMinAStages = 4;
 // Stem mode (ResNet 7x7/2 on the window-row layout, ops/igemm.py): a tile is 8 x 16 output
 // pixels; its A stage is ONE TMA box of 8 window columns x 37 input rows (2*16 + 5) from which
-// all seven filter rows are read through the UMMA descriptor - filter row r of output row j is
+// all seven filter rows are read through the wgmma descriptor - filter row r of output row j is
 // box row 2j + r, so the 8-row core-matrix groups sit 2 box rows (2048 B) apart (SBO) and the
 // filter row only shifts the start address by 1024 B.  L2 -> SM traffic per tile: 37 KB instead
 // of 7 x 16 KB of A plus 7 x 8 KB of B (the filter is resident).
@@ -75,6 +65,28 @@ constexpr int kStemStage = kStemBoxW * kStemRows * 128;  // 37888 B, a multiple 
 __device__ __forceinline__ void red_shared_add(float* p, float v) {
   asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(smem_u32(p)), "f"(v) : "memory");
 }
+__device__ __forceinline__ void consumer_sync() {
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+}
+
+// Per-column partial sums of the 16 rows a warp holds: lanes with the same (lane % 4) own the same
+// column pair; after the butterfly lanes 0..3 hold the warp totals and add them to shared memory.
+__device__ __forceinline__ void warp_col_pair_reduce(float* stat, int col, int lane, float2 s,
+                                                     float2 q) {
+#pragma unroll
+  for (int m = 4; m <= 16; m <<= 1) {
+    s.x += __shfl_xor_sync(0xffffffff, s.x, m);
+    s.y += __shfl_xor_sync(0xffffffff, s.y, m);
+    q.x += __shfl_xor_sync(0xffffffff, q.x, m);
+    q.y += __shfl_xor_sync(0xffffffff, q.y, m);
+  }
+  if (lane < 4) {
+    red_shared_add(stat + col * 2 + 0, s.x);
+    red_shared_add(stat + col * 2 + 1, q.x);
+    red_shared_add(stat + col * 2 + 2, s.y);
+    red_shared_add(stat + col * 2 + 3, q.y);
+  }
+}
 
 // EPI selects a compile-time epilogue so the common cases carry no per-element flag tests:
 //   0 plain store, 1 fused BN statistics, 2 read-modify-write accumulate,
@@ -82,43 +94,30 @@ __device__ __forceinline__ void red_shared_add(float* p, float v) {
 //   8 (with 0 or 2) fused batch-norm backward reduction over the stored gradient tile.
 constexpr int kEpiPlain = 0, kEpiStats = 1, kEpiAccum = 2, kEpiGeneric = 4, kEpiBnRed = 8;
 
-template <int BN, bool B_MN, int EPI, int CG = 1>
+template <int BN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(kThreads, 1)
 igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const FwdArgs a, const int total_tiles) {
-  using Cfg = FwdCfg<BN, CG>;
-  constexpr bool k2 = CG == 2;
-  // CTA pair: rank in the pair, the leader issues the MMAs; a "tile" is then a PAIR of pixel boxes
-  const uint32_t crank = k2 ? cluster_ctarank() : 0u;
-  const bool leader = crank == 0u;
-  const int tile0 = k2 ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int tstep = k2 ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  using Cfg = FwdCfg<BN>;
+  constexpr int kAcc = BN / 2;   // fp32 accumulator registers per consumer thread (64 x BN / 128)
+  const int tile0 = static_cast<int>(blockIdx.x);
+  const int tstep = static_cast<int>(gridDim.x);
   const int m_boxes = a.tiles_w * a.tiles_h * a.tiles_n;
-  // pixel box of (pair-)tile `tile` for this CTA; the odd tail box of a pair may lie outside the
-  // tensor: TMA then zero-fills and the epilogue finds no valid row
   auto box_of = [&](int tile) {
-    int mt = tile / a.n_tiles;
-    if (k2) {
-      if (a.reverse) mt = (m_boxes + 1) / 2 - 1 - mt;
-      return 2 * mt + static_cast<int>(crank);
-    }
+    const int mt = tile / a.n_tiles;
     return a.reverse ? m_boxes - 1 - mt : mt;
   };
   extern __shared__ __align__(1024) uint8_t smem[];
   float* stat_smem = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStage);
-  uint8_t* out_stage = smem + Cfg::kStages * Cfg::kStage + Cfg::kStatBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(out_stage + Cfg::kOutStageBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStage + Cfg::kStatBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + kMaxStages;
-  uint64_t* tfull = bars + 2 * kMaxStages;
-  uint64_t* tempty = tfull + 2;
-  uint64_t* bfull = tempty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bfull + 1);
+  uint64_t* bfull = bars + 2 * kMaxStages;
 
   const int warp = __shfl_sync(0xffffffff, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) {  // SWIZZLE_128B operands need 1024-byte alignment
       printf("tfos: dynamic shared memory is not 1024-byte aligned\n");
       __trap();
@@ -127,34 +126,13 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < kMaxStages; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      // 64-column tiles are one slab wide: the two warps of a lane quarter then take ALTERNATE
-      // tiles (= alternate TMEM buffers) instead of one of them idling, see the epilogue
-      mbar_init(&tempty[i], k2 ? 2 * kEpiWarps
-                                : ((BN == 64 && a.n_tiles == 1) ? kEpiWarps / 2 : kEpiWarps));
+      mbar_init(&empty[i], 2);   // one arrive per consumer warpgroup
     }
     mbar_init(bfull, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if (k2) {   // both CTAs of the pair allocate (same columns in both TMEMs)
-      tmem_alloc_2cta(tmem_slot, Cfg::kTmemCols);
-      tmem_relinquish_2cta();
-    } else {
-      tmem_alloc(tmem_slot, Cfg::kTmemCols);
-      tmem_relinquish();
-    }
-  }
-  if (threadIdx.x >= 64)
-    for (int i = threadIdx.x - 64; i < BN * 2; i += kEpiThreads) stat_smem[i] = 0.f;
-  tc_fence_before();
-  if (k2) cluster_sync_all();   // the peer's barriers and TMEM exist before anyone signals them
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  for (int i = threadIdx.x; i < BN * 2; i += kThreads) stat_smem[i] = 0.f;
+  __syncthreads();
 
   const int k_iters = a.num_taps * a.k_chunks;
   const int rows = a.box_w * a.box_h * a.box_n;
@@ -166,26 +144,14 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const uint32_t stage_tx =
       stem ? kStemStage
            : static_cast<uint32_t>(rows) * 128u + (resident ? 0u : Cfg::kBBytes);
-  // (CTA pair: host guarantees !resident && !stem; the leader's barrier counts both CTAs' bytes)
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       auto load_b = [&](uint8_t* sB, uint64_t* bar, int nt, int t, int kc) {
-        if (k2) {   // this CTA's half of the B tile: columns / rows [crank * BN/2, +BN/2)
-          if (B_MN) {
-#pragma unroll
-            for (int j = 0; j < BN / 128; ++j)
-              tma_load_2d_2cta(sB + j * 8192, &tmB, bar,
-                               nt * BN + (static_cast<int>(crank) * (BN / 128) + j) * 64 + a.tap_bn[t],
-                               a.tap_bk[t] + kc * 64);
-          } else {
-            tma_load_2d_2cta(sB, &tmB, bar, a.tap_bk[t] + kc * 64,
-                             nt * BN + static_cast<int>(crank) * (BN / 2));
-          }
-        } else if (B_MN) {
+        if (B_MN) {
 #pragma unroll
           for (int j = 0; j < BN / 64; ++j)
             tma_load_2d(sB + j * 8192, &tmB, bar, nt * BN + j * 64 + a.tap_bn[t],
@@ -226,19 +192,10 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const int t = it / a.k_chunks, kc = it - t * a.k_chunks;
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* sA = ring + stage * stage_stride;
-          if (k2) {
-            // only the leader arms the (leader's) barrier, with the bytes of BOTH CTAs; the
-            // peer's TMA completions are counted there too (barrier address, peer bit cleared)
-            if (leader) mbar_expect_tx(&full[stage], 2 * stage_tx);
-            tma_load_4d_2cta(sA, &tmA, &full[stage], kc * 64 + a.tap_dc[t], cw + a.tap_dw[t],
-                             ch + a.tap_dh[t], cn);
-            load_b(sA + kABytes, &full[stage], nt, t, kc);
-          } else {
-            mbar_expect_tx(&full[stage], stage_tx);
-            tma_load_4d(sA, &tmA, &full[stage], kc * 64 + a.tap_dc[t], cw + a.tap_dw[t],
-                        ch + a.tap_dh[t], cn);
-            if (!resident) load_b(sA + kABytes, &full[stage], nt, t, kc);
-          }
+          mbar_expect_tx(&full[stage], stage_tx);
+          tma_load_4d(sA, &tmA, &full[stage], kc * 64 + a.tap_dc[t], cw + a.tap_dw[t],
+                      ch + a.tap_dh[t], cn);
+          if (!resident) load_b(sA + kABytes, &full[stage], nt, t, kc);
           if (++stage == nstages) {
             stage = 0;
             phase ^= 1;
@@ -246,456 +203,225 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // -------------------------------------------------------------- MMA issuer
-    if (lane == 0 && (!k2 || leader)) {
-      constexpr uint32_t idesc = umma_idesc_bf16(k2 ? 2 * kBlockM : kBlockM, BN, false, B_MN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      if (resident && tile0 < total_tiles) mbar_wait(bfull, 0);
-      for (int tile = tile0; tile < total_tiles; tile += tstep) {
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        if (stem) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_base = smem_u32(ring + stage * stage_stride);
-          const uint64_t ad0 = umma_desc_sw128(a_base, 16, 2 * kStemBoxW * 128);
-          const uint64_t bd0 = umma_desc_sw128(smem_u32(smem), 16, 1024);
-          for (int r = 0; r < 7; ++r) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_bf16(d_tmem, ad0 + r * ((kStemBoxW * 128) >> 4) + k * 2,
-                        bd0 + r * (Cfg::kBBytes >> 4) + k * 2, idesc, (r | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == nstages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        for (int it = 0; it < (stem ? 0 : k_iters); ++it) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_base = smem_u32(ring + stage * stage_stride);
-          const uint32_t b_base =
-              resident ? smem_u32(smem + it * Cfg::kBBytes) : a_base + kABytes;
-          // descriptors advance by 64-bit adds (start address = low field, 16-byte units)
-          const uint64_t ad0 = umma_desc_sw128(a_base, 16, 1024);
-          const uint64_t bd0 =
-              B_MN ? umma_desc_sw128(b_base, 8192, 1024) : umma_desc_sw128(b_base, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            if (k2)
-              umma_bf16_2cta(d_tmem, ad0 + k * 2, bd0 + k * (B_MN ? 128 : 2), idesc,
-                             (it | k) != 0 ? 1u : 0u);
-            else
-              umma_bf16(d_tmem, ad0 + k * 2, bd0 + k * (B_MN ? 128 : 2), idesc,
-                        (it | k) != 0 ? 1u : 0u);
-          }
-          if (k2) umma_commit_2cta(&empty[stage], 0x3);   // both producers may refill the stage
-          else umma_commit(&empty[stage]);
-          if (++stage == nstages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (k2) umma_commit_2cta(&tfull[acc], 0x3);       // both epilogues may read their rows
-        else umma_commit(&tfull[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else {
-    // ---------------------------------------------------------------- epilogue
-    const int ew = warp - 2;    // 0..7
-    const int q = warp & 3;     // TMEM lane quarter this warp may read
-    const int half = ew >> 2;   // which column slabs / chunks this warp takes
-    const int et = threadIdx.x - 64;
-    constexpr bool kGeneric = (EPI & kEpiGeneric) != 0;
-    const bool do_stats = kGeneric ? (a.col_sum != nullptr) : ((EPI & kEpiStats) != 0);
-    const bool acc_on = kGeneric ? (a.accumulate != 0) : ((EPI & kEpiAccum) != 0);
-    const bool bias_on = kGeneric && a.bias != nullptr;
-    const bool relu_on = kGeneric && a.relu != 0;
-    constexpr bool red_on = (EPI & kEpiBnRed) != 0;   // fused BN backward reduction (igemm.h)
-    const uint32_t stg = smem_u32(out_stage + ew * 4096);
-    const bool split = BN == 64 && a.n_tiles == 1;   // half-groups own alternate tiles
-    // position of this thread's accumulator row inside the pixel box: tile independent
-    const int row = q * 32 + lane;
-    const int iw = row % a.box_w;
-    const int ih = (row / a.box_w) % a.box_h;
-    const int in_ = row / (a.box_w * a.box_h);
-    // fused statistics: lane l keeps the running sums of columns (2l, 2l+1) of its slabs in
-    // registers for as long as the CTA stays on one n tile; they meet in shared memory only
-    // when the n tile changes or the CTA runs out of tiles (see the flush below)
-    constexpr int kSlabs = BN >= 128 ? BN / 128 : 1;
-    float2 rs[kSlabs], rq[kSlabs];
-#pragma unroll
-    for (int i = 0; i < kSlabs; ++i) rs[i] = rq[i] = make_float2(0.f, 0.f);
-    auto flush_stats = [&](int nt) {
-      // registers -> shared (the row quarters / half-groups meet per column) -> global atomics
-#pragma unroll
-      for (int ci = 0; ci < kSlabs; ++ci) {
-        const int c = split ? ci : half + 2 * ci;
-        if (c < BN / 64) {
-          float* st = stat_smem + (c * 64 + 2 * lane) * 2;
-          red_shared_add(st + 0, rs[ci].x);
-          red_shared_add(st + 1, rq[ci].x);
-          red_shared_add(st + 2, rs[ci].y);
-          red_shared_add(st + 3, rq[ci].y);
-        }
-        rs[ci] = rq[ci] = make_float2(0.f, 0.f);
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int c = et; c < BN; c += kEpiThreads) {
-        const int col = nt * BN + c;
-        if (col < a.n_valid) {
-          atomicAdd(a.col_sum + col, stat_smem[c * 2 + 0]);
-          atomicAdd(a.col_sumsq + col, stat_smem[c * 2 + 1]);
-        }
-        stat_smem[c * 2 + 0] = 0.f;
-        stat_smem[c * 2 + 1] = 0.f;
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-    };
-    // fused BN backward reduction: lane (r, sg) of the store phase owns the 8 columns of segment
-    // sg for its 8 rows; per slab 8 x (sum g, sum g*x) live in registers until the n tile changes
-    float2 bg[red_on ? kSlabs : 1][4], bgx[red_on ? kSlabs : 1][4];
-#pragma unroll
-    for (int i = 0; i < (red_on ? kSlabs : 1); ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) bg[i][j] = bgx[i][j] = make_float2(0.f, 0.f);
-    auto flush_red = [&](int nt) {
-#pragma unroll
-      for (int ci = 0; ci < (red_on ? kSlabs : 1); ++ci) {
-        const int c = split ? ci : half + 2 * ci;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float2 g2 = bg[ci][j], x2 = bgx[ci][j];
-#pragma unroll
-          for (int m = 8; m <= 16; m <<= 1) {   // the four row lanes of a segment meet
-            g2.x += __shfl_xor_sync(0xffffffff, g2.x, m), g2.y += __shfl_xor_sync(0xffffffff, g2.y, m);
-            x2.x += __shfl_xor_sync(0xffffffff, x2.x, m), x2.y += __shfl_xor_sync(0xffffffff, x2.y, m);
-          }
-          if (lane < 8 && c < BN / 64) {
-            float* st = stat_smem + (c * 64 + lane * 8 + 2 * j) * 2;
-            red_shared_add(st + 0, g2.x);
-            red_shared_add(st + 1, x2.x);
-            red_shared_add(st + 2, g2.y);
-            red_shared_add(st + 3, x2.y);
-          }
-          bg[ci][j] = bgx[ci][j] = make_float2(0.f, 0.f);
-        }
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int c = et; c < BN; c += kEpiThreads) {
-        const int col = nt * BN + c;
-        if (col < a.n_valid) {
-          atomicAdd(a.col_sum + col, stat_smem[c * 2 + 0]);
-          atomicAdd(a.col_sumsq + col, stat_smem[c * 2 + 1]);
-        }
-        stat_smem[c * 2 + 0] = 0.f;
-        stat_smem[c * 2 + 1] = 0.f;
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-    };
-    int it = -1;
-    for (int tile = tile0; tile < total_tiles; tile += tstep) {
-      ++it;
-      if (split && (it & 1) != half) continue;   // the other half-group owns this tile
-      const int acc = it & 1;                    // TMEM buffer / barrier pair of this tile
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int nt = tile % a.n_tiles;
-      int mt = box_of(tile);
-      const int tw = mt % a.tiles_w;
-      mt /= a.tiles_w;
-      const int th = mt % a.tiles_h;
-      const int tn = mt / a.tiles_h;
-      const int w = tw * a.box_w + iw, h = th * a.box_h + ih, n = tn * a.box_n + in_;
-      const bool valid = row < rows && w < a.lim_w && h < a.lim_h && n < a.lim_n;
-      const long long pix =
-          (static_cast<long long>(n) * a.OH + (h * a.osh + a.ooh)) * a.OW + (w * a.osw + a.oow);
-      const long long off = pix * a.ldo + static_cast<long long>(nt) * BN;
-      const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
-
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const bool fast = !a.out_fp32 && (nt * BN + BN <= a.n_valid) && (a.ldo & 7) == 0;
-      if (fast) {
-        __nv_bfloat16* obase = reinterpret_cast<__nv_bfloat16*>(a.out);
-        const bool relu_early = relu_on && !acc_on;
-        // per-tile row bookkeeping for the coalesced store phase: lane handles rows
-        // i*4 + (lane >> 3), i = 0..7; fetch their offsets / validity once, not per slab
-        const uint32_t vmask = __ballot_sync(0xffffffff, valid);
-        const bool zero_invalid = do_stats && vmask != 0xffffffffu;
-        long long roffs[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) roffs[i] = __shfl_sync(0xffffffff, off, i * 4 + (lane >> 3));
-#pragma unroll
-        for (int ci = 0; ci < kSlabs; ++ci) {
-          const int c = split ? ci : half + 2 * ci;
-          if (c >= BN / 64) break;
-          // accumulate mode: the previous values do not depend on the MMA - issue all eight
-          // 16-byte loads of this slab now so their latency overlaps the TMEM read + staging
-          uint4 prev[8];
-          uint32_t pmask[8];
-          if (acc_on) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int r2 = i * 4 + (lane >> 3);
-              prev[i] = make_uint4(0u, 0u, 0u, 0u);
-              pmask[i] = 0xffu;
-              if ((vmask >> r2) & 1u) {
-                const long long e = roffs[i] + c * 64 + (lane & 7) * 8;
-                prev[i] = *reinterpret_cast<const uint4*>(obase + e);
-                if (a.acc_mask != nullptr) pmask[i] = a.acc_mask[e >> 3];
-              }
-            }
-          }
-          // fused BN reduction: x of the batch norm below and its ReLU bits, same rows / segment.
-          // Issued before the TMEM read (latency hidden behind it) unless the accumulate operands
-          // already occupy that slot - prev[] + xq[] + the 64 accumulator words would spill -
-          // then right after the tile has been staged.
-          uint4 xq[red_on ? 8 : 1];
-          uint32_t mq[red_on ? 8 : 1];
-          auto load_red = [&]() {
-            const __nv_bfloat16* xb = reinterpret_cast<const __nv_bfloat16*>(a.red_x);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int r2 = i * 4 + (lane >> 3);
-              xq[i] = make_uint4(0u, 0u, 0u, 0u);
-              mq[i] = 0xffu;
-              if ((vmask >> r2) & 1u) {
-                const long long e = roffs[i] + c * 64 + (lane & 7) * 8;
-                xq[i] = *reinterpret_cast<const uint4*>(xb + e);
-                if (a.red_mask != nullptr) mq[i] = a.red_mask[e >> 3];
-              }
-            }
-          };
-          if (red_on && !acc_on) load_red();
-          uint32_t v[64];
-          {
-            uint32_t (&lo)[32] = *reinterpret_cast<uint32_t (*)[32]>(&v[0]);
-            uint32_t (&hi)[32] = *reinterpret_cast<uint32_t (*)[32]>(&v[32]);
-            tmem_ld_32x32(tbase + c * 64, lo);
-            tmem_ld_32x32(tbase + c * 64 + 32, hi);
-            tmem_ld_wait();
-          }
-          const int col0 = nt * BN + c * 64;
-          uint32_t pk[32];
-#pragma unroll
-          for (int j = 0; j < 64; j += 2) {
-            float f0 = __uint_as_float(v[j]), f1 = __uint_as_float(v[j + 1]);
-            if (bias_on) {
-              f0 += __ldg(a.bias + col0 + j);
-              f1 += __ldg(a.bias + col0 + j + 1);
-            }
-            if (relu_early) {
-              f0 = fmaxf(f0, 0.f);
-              f1 = fmaxf(f1, 0.f);
-              if (a.relu == 2) {  // ReLU6 (MobileNetV2 encoder)
-                f0 = fminf(f0, 6.f);
-                f1 = fminf(f1, 6.f);
-              }
-            }
-            pk[j >> 1] = pack_bf16x2(f0, f1);
-          }
-          if (zero_invalid && !valid) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) pk[j] = 0u;
-          }
-#pragma unroll
-          for (int sgm = 0; sgm < 8; ++sgm) {
-            const uint32_t addr = stg + lane * 128 + ((sgm ^ (lane & 7)) << 4);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(pk[sgm * 4]),
-                         "r"(pk[sgm * 4 + 1]), "r"(pk[sgm * 4 + 2]), "r"(pk[sgm * 4 + 3])
-                         : "memory");
-          }
-          if (red_on && acc_on) load_red();
-          __syncwarp();
-          if (do_stats) {
-            // lane l owns columns (2l, 2l+1) of the slab: word (l & 3) of segment (l >> 2);
-            // all lanes read the same row -> 32 distinct banks.  Statistics are taken of the
-            // rounded values that are stored; rows outside the tensor were zeroed above.
-            float2 sacc = make_float2(0.f, 0.f), qacc = make_float2(0.f, 0.f);
-            const uint32_t lbase = stg + ((lane & 3) << 2);
-#pragma unroll
-            for (int r = 0; r < 32; ++r) {
-              uint32_t wv;
-              const uint32_t addr = lbase + r * 128 + (((lane >> 2) ^ (r & 7)) << 4);
-              asm volatile("ld.shared.b32 %0, [%1];" : "=r"(wv) : "r"(addr));
-              const float2 xy = make_float2(__uint_as_float(wv << 16),
-                                            __uint_as_float(wv & 0xffff0000u));
-              sacc = __fadd2_rn(sacc, xy);        // packed fp32x2 pipe (sm_100)
-              qacc = __ffma2_rn(xy, xy, qacc);
-            }
-            rs[ci] = __fadd2_rn(rs[ci], sacc);
-            rq[ci] = __fadd2_rn(rq[ci], qacc);
-          }
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int r2 = i * 4 + (lane >> 3), sg2 = lane & 7;
-            uint4 val;
-            const uint32_t addr = stg + r2 * 128 + ((sg2 ^ (r2 & 7)) << 4);
-            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
-                         : "=r"(val.x), "=r"(val.y), "=r"(val.z), "=r"(val.w)
-                         : "r"(addr));
-            const long long roff = roffs[i];
-            if ((vmask >> r2) & 1u) {
-              __nv_bfloat16* o = obase + roff + c * 64 + sg2 * 8;
-              if (acc_on) {
-                const uint4 p = prev[i];
-                float2 n0 = unpack_bf16x2(val.x), n1 = unpack_bf16x2(val.y),
-                       n2 = unpack_bf16x2(val.z), n3 = unpack_bf16x2(val.w);
-                const float2 p0 = unpack_bf16x2(p.x), p1 = unpack_bf16x2(p.y),
-                             p2 = unpack_bf16x2(p.z), p3 = unpack_bf16x2(p.w);
-                const uint32_t pm = pmask[i];   // bit j: element j of this 16-byte group counts
-                n0.x += (pm & 1u) ? p0.x : 0.f, n0.y += (pm & 2u) ? p0.y : 0.f;
-                n1.x += (pm & 4u) ? p1.x : 0.f, n1.y += (pm & 8u) ? p1.y : 0.f;
-                n2.x += (pm & 16u) ? p2.x : 0.f, n2.y += (pm & 32u) ? p2.y : 0.f;
-                n3.x += (pm & 64u) ? p3.x : 0.f, n3.y += (pm & 128u) ? p3.y : 0.f;
-                if (relu_on) {
-                  n0.x = fmaxf(n0.x, 0.f), n0.y = fmaxf(n0.y, 0.f), n1.x = fmaxf(n1.x, 0.f);
-                  n1.y = fmaxf(n1.y, 0.f), n2.x = fmaxf(n2.x, 0.f), n2.y = fmaxf(n2.y, 0.f);
-                  n3.x = fmaxf(n3.x, 0.f), n3.y = fmaxf(n3.y, 0.f);
-                }
-                val.x = pack_bf16x2(n0.x, n0.y), val.y = pack_bf16x2(n1.x, n1.y);
-                val.z = pack_bf16x2(n2.x, n2.y), val.w = pack_bf16x2(n3.x, n3.y);
-              }
-              *reinterpret_cast<uint4*>(o) = val;
-              if (red_on) {   // statistics of the ROUNDED gradient that was just stored
-                const uint32_t gw[4] = {val.x, val.y, val.z, val.w};
-                const uint32_t xw[4] = {xq[i].x, xq[i].y, xq[i].z, xq[i].w};
-                const uint32_t mb = mq[i];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  float2 g2 = unpack_bf16x2(gw[j]);
-                  g2.x = ((mb >> (2 * j)) & 1u) ? g2.x : 0.f;
-                  g2.y = ((mb >> (2 * j + 1)) & 1u) ? g2.y : 0.f;
-                  bg[ci][j] = __fadd2_rn(bg[ci][j], g2);
-                  bgx[ci][j] = __ffma2_rn(g2, unpack_bf16x2(xw[j]), bgx[ci][j]);
-                }
-              }
-            }
-          }
-          __syncwarp();
-        }
-      } else {
-        // general path: fp32 output, ragged N, or unaligned pitch (dense heads, tails)
-#pragma unroll 1
-        for (int c = split ? 0 : half; c < BN / 32; c += split ? 1 : 2) {
-          uint32_t v[32];
-          tmem_ld_32x32(tbase + c * 32, v);
-          tmem_ld_wait();
-          const int col0 = nt * BN + c * 32;
-          float f[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-          if (a.bias != nullptr) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (col0 + j < a.n_valid) f[j] += __ldg(a.bias + col0 + j);
-          }
-          if (a.out_fp32) {
-            float* o = reinterpret_cast<float*>(a.out) + off + c * 32;
-            if (valid) {
-              if (a.accumulate) {
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                  if (col0 + j < a.n_valid) f[j] += o[j];
-              }
-              if (a.relu) {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.f);
-              }
-              if (col0 + 32 <= a.n_valid && (a.ldo & 3) == 0) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                  *reinterpret_cast<float4*>(o + j) =
-                      make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-              } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                  if (col0 + j < a.n_valid) o[j] = f[j];
-              }
-            }
-          } else {
-            __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(a.out) + off + c * 32;
-            if (valid && a.accumulate) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (col0 + j < a.n_valid) f[j] += __bfloat162float(o[j]);
-            }
-            if (a.relu) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.f);
-              if (a.relu == 2) {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) f[j] = fminf(f[j], 6.f);
-              }
-            }
-#pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = __bfloat162float(__float2bfloat16_rn(f[j]));
-            if (valid) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (col0 + j < a.n_valid) o[j] = __float2bfloat16_rn(f[j]);
-            }
-          }
-          if (do_stats) {
-            // transpose-reduce butterfly: after 5 steps lane j holds the totals of column j
-            float s[32], ss[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float x = valid ? f[j] : 0.f;
-              s[j] = x;
-              ss[j] = x * x;
-            }
-#pragma unroll
-            for (int step = 16; step >= 1; step >>= 1) {
-              const bool upper = (lane & step) != 0;
-#pragma unroll
-              for (int j = 0; j < step; ++j) {
-                const float send_s = upper ? s[j] : s[j + step];
-                const float send_q = upper ? ss[j] : ss[j + step];
-                const float recv_s = __shfl_xor_sync(0xffffffff, send_s, step);
-                const float recv_q = __shfl_xor_sync(0xffffffff, send_q, step);
-                s[j] = (upper ? s[j + step] : s[j]) + recv_s;
-                ss[j] = (upper ? ss[j + step] : ss[j]) + recv_q;
-              }
-            }
-            red_shared_add(stat_smem + (c * 32 + lane) * 2 + 0, s[0]);
-            red_shared_add(stat_smem + (c * 32 + lane) * 2 + 1, ss[0]);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (k2 && !leader) mbar_arrive_cluster(&tempty[acc], 0);   // the leader owns tempty
-        else mbar_arrive(&tempty[acc]);
-      }
-      const int next_tile = tile + tstep;
-      if (!split && do_stats && (next_tile >= total_tiles || next_tile % a.n_tiles != nt))
-        flush_stats(nt);
-      if (!split && red_on && (next_tile >= total_tiles || next_tile % a.n_tiles != nt))
-        flush_red(nt);
-    }
-    // split mode: the half-groups skip each other's tiles, so they meet only here (one n tile)
-    if (split && do_stats && tile0 < total_tiles) flush_stats(0);
-    if (split && red_on && tile0 < total_tiles) flush_red(0);
+    return;
   }
 
-  tc_fence_before();
-  if (k2) {
-    cluster_sync_all();   // the peer's barriers / TMEM are signalled until both CTAs are done
-    if (warp == 1) tmem_dealloc_2cta(tmem_base, Cfg::kTmemCols);
-  } else {
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, Cfg::kTmemCols);
+  // ------------------------------------------------------------------ consumers
+  const int wg = (warp >> 2) - 1;   // 0 / 1: rows [64 wg, 64 wg + 64) of the tile
+  const int wq = warp & 3;          // warp inside the warpgroup: rows 16 wq .. 16 wq + 15
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  constexpr bool kGeneric = (EPI & kEpiGeneric) != 0;
+  const bool do_stats = kGeneric ? (a.col_sum != nullptr) : ((EPI & kEpiStats) != 0);
+  const bool acc_on = kGeneric ? (a.accumulate != 0) : ((EPI & kEpiAccum) != 0);
+  const bool bias_on = kGeneric && a.bias != nullptr;
+  const bool relu_on = kGeneric && a.relu != 0;
+  constexpr bool red_on = (EPI & kEpiBnRed) != 0;   // fused BN backward reduction (igemm.h)
+  // the two accumulator rows of this thread, inside the tile / pixel box: tile independent
+  int prow[2], iw[2], ih[2], in_[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    prow[h] = 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
+    iw[h] = prow[h] % a.box_w;
+    ih[h] = (prow[h] / a.box_w) % a.box_h;
+    in_[h] = prow[h] / (a.box_w * a.box_h);
+  }
+  const int cpair = 2 * (lane & 3);   // first of the two columns of each 8-column block
+
+  float acc[kAcc];
+#pragma unroll
+  for (int i = 0; i < kAcc; ++i) acc[i] = 0.f;
+
+  int stage = 0;
+  uint32_t phase = 0;
+  if (resident && tile0 < total_tiles) mbar_wait(bfull, 0);
+  for (int tile = tile0; tile < total_tiles; tile += tstep) {
+    // ------------------------------------------------------------ main loop
+    int prev_stage = -1;
+    auto release_prev = [&]() {
+      if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty[prev_stage]);
+    };
+    wgmma_fence_regs(acc);
+    if (stem) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t a_base = smem_u32(ring + stage * stage_stride) + wg * (8 * 2 * kStemBoxW * 128);
+      const uint64_t ad0 = wgmma_desc_sw128(a_base, 16, 2 * kStemBoxW * 128);
+      const uint64_t bd0 = wgmma_desc_sw128(smem_u32(smem), 16, 1024);
+      wgmma_fence();
+#pragma unroll 1
+      for (int r = 0; r < 7; ++r) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          Wgmma<BN>::template mma<0, 0>(acc, ad0 + r * ((kStemBoxW * 128) >> 4) + k * 2,
+                                        bd0 + r * (Cfg::kBBytes >> 4) + k * 2,
+                                        (r | k) != 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      prev_stage = stage;
+      if (++stage == nstages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    for (int it = 0; it < (stem ? 0 : k_iters); ++it) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t a_base = smem_u32(ring + stage * stage_stride);
+      const uint32_t b_base = resident ? smem_u32(smem + it * Cfg::kBBytes) : a_base + kABytes;
+      // descriptors advance by 64-bit adds (start address = low field, 16-byte units)
+      const uint64_t ad0 = wgmma_desc_sw128(a_base + wg * (64 * 128), 16, 1024);
+      const uint64_t bd0 =
+          B_MN ? wgmma_desc_sw128(b_base, 8192, 1024) : wgmma_desc_sw128(b_base, 16, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        Wgmma<BN>::template mma<0, B_MN ? 1 : 0>(acc, ad0 + k * 2, bd0 + k * (B_MN ? 128 : 2),
+                                                 (it | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      // the group issued one stage earlier has retired: its stage may be refilled
+      wgmma_wait<1>();
+      release_prev();
+      prev_stage = stage;
+      if (++stage == nstages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    release_prev();
+
+    // ------------------------------------------------------------- epilogue
+    const int nt = tile % a.n_tiles;
+    int mt = box_of(tile);
+    const int tw = mt % a.tiles_w;
+    mt /= a.tiles_w;
+    const int th = mt % a.tiles_h;
+    const int tn = mt / a.tiles_h;
+    bool valid[2];
+    long long off[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int w = tw * a.box_w + iw[h], hh = th * a.box_h + ih[h], n = tn * a.box_n + in_[h];
+      valid[h] = prow[h] < rows && w < a.lim_w && hh < a.lim_h && n < a.lim_n;
+      const long long pix =
+          (static_cast<long long>(n) * a.OH + (hh * a.osh + a.ooh)) * a.OW + (w * a.osw + a.oow);
+      off[h] = pix * a.ldo + static_cast<long long>(nt) * BN;
+    }
+    const bool fast = !a.out_fp32 && (nt * BN + BN <= a.n_valid) && (a.ldo & 7) == 0;
+    if (fast) {
+      __nv_bfloat16* obase = reinterpret_cast<__nv_bfloat16*>(a.out);
+      const bool relu_early = relu_on && !acc_on;
+#pragma unroll 4
+      for (int jb = 0; jb < BN / 8; ++jb) {
+        const int c = jb * 8 + cpair;   // column inside the tile
+        float2 s2 = make_float2(0.f, 0.f), q2 = make_float2(0.f, 0.f);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float f0 = acc[4 * jb + 2 * h], f1 = acc[4 * jb + 2 * h + 1];
+          if (bias_on) {
+            f0 += __ldg(a.bias + nt * BN + c);
+            f1 += __ldg(a.bias + nt * BN + c + 1);
+          }
+          if (relu_early) {
+            f0 = fmaxf(f0, 0.f);
+            f1 = fmaxf(f1, 0.f);
+            if (a.relu == 2) {  // ReLU6 (MobileNetV2 encoder)
+              f0 = fminf(f0, 6.f);
+              f1 = fminf(f1, 6.f);
+            }
+          }
+          uint32_t val = pack_bf16x2(f0, f1);
+          if (do_stats && valid[h]) {
+            // statistics of the rounded values that are stored; rows outside the tensor add 0
+            const float2 r = unpack_bf16x2(val);
+            s2 = fadd2_rn(s2, r);
+            q2 = ffma2_rn(r, r, q2);
+          }
+          if (valid[h]) {
+            const long long e = off[h] + c;
+            if (acc_on) {
+              const uint32_t pw = *reinterpret_cast<const uint32_t*>(obase + e);
+              const uint32_t pm = a.acc_mask != nullptr ? (a.acc_mask[e >> 3] >> (e & 7)) : 3u;
+              float2 n2 = unpack_bf16x2(val);
+              const float2 p2 = unpack_bf16x2(pw);
+              n2.x += (pm & 1u) ? p2.x : 0.f;
+              n2.y += (pm & 2u) ? p2.y : 0.f;
+              if (relu_on) {
+                n2.x = fmaxf(n2.x, 0.f);
+                n2.y = fmaxf(n2.y, 0.f);
+              }
+              val = pack_bf16x2(n2.x, n2.y);
+            }
+            *reinterpret_cast<uint32_t*>(obase + e) = val;
+            if (red_on) {   // statistics of the ROUNDED gradient that was just stored
+              const uint32_t mb = a.red_mask != nullptr ? (a.red_mask[e >> 3] >> (e & 7)) : 3u;
+              float2 g2 = unpack_bf16x2(val);
+              g2.x = (mb & 1u) ? g2.x : 0.f;
+              g2.y = (mb & 2u) ? g2.y : 0.f;
+              const float2 x2 = unpack_bf16x2(
+                  *reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(a.red_x) + e));
+              s2 = fadd2_rn(s2, g2);
+              q2 = ffma2_rn(g2, x2, q2);
+            }
+          }
+        }
+        if (do_stats || red_on) warp_col_pair_reduce(stat_smem, c, lane, s2, q2);
+      }
+    } else {
+      // general path: fp32 output, ragged N, or unaligned pitch (dense heads, tails)
+#pragma unroll 4
+      for (int jb = 0; jb < BN / 8; ++jb) {
+        const int c = jb * 8 + cpair;
+        float2 s2 = make_float2(0.f, 0.f), q2 = make_float2(0.f, 0.f);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float f[2] = {acc[4 * jb + 2 * h], acc[4 * jb + 2 * h + 1]};
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const int col = nt * BN + c + j;
+            const bool cv = col < a.n_valid;
+            const long long e = off[h] + c + j;
+            if (a.bias != nullptr && cv) f[j] += __ldg(a.bias + col);
+            if (a.out_fp32) {
+              float* o = reinterpret_cast<float*>(a.out);
+              if (valid[h]) {
+                if (a.accumulate && cv) f[j] += o[e];
+                if (a.relu) f[j] = fmaxf(f[j], 0.f);
+                if (cv) o[e] = f[j];
+              }
+            } else {
+              __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(a.out);
+              if (valid[h] && a.accumulate && cv) f[j] += __bfloat162float(o[e]);
+              if (a.relu) {
+                f[j] = fmaxf(f[j], 0.f);
+                if (a.relu == 2) f[j] = fminf(f[j], 6.f);
+              }
+              f[j] = __bfloat162float(__float2bfloat16_rn(f[j]));
+              if (valid[h] && cv) o[e] = __float2bfloat16_rn(f[j]);
+            }
+          }
+          if (do_stats && valid[h]) {
+            s2 = fadd2_rn(s2, make_float2(f[0], f[1]));
+            q2 = ffma2_rn(make_float2(f[0], f[1]), make_float2(f[0], f[1]), q2);
+          }
+        }
+        if (do_stats) warp_col_pair_reduce(stat_smem, c, lane, s2, q2);
+      }
+    }
+    // the per-column sums meet in shared memory for as long as the CTA stays on one n tile
+    const int next_tile = tile + tstep;
+    if ((do_stats || red_on) && (next_tile >= total_tiles || next_tile % a.n_tiles != nt)) {
+      consumer_sync();
+      for (int c = threadIdx.x - 128; c < BN; c += kConsumerThreads) {
+        const int col = nt * BN + c;
+        if (col < a.n_valid) {
+          atomicAdd(a.col_sum + col, stat_smem[c * 2 + 0]);
+          atomicAdd(a.col_sumsq + col, stat_smem[c * 2 + 1]);
+        }
+        stat_smem[c * 2 + 0] = 0.f;
+        stat_smem[c * 2 + 1] = 0.f;
+      }
+      consumer_sync();
+    }
   }
 }
 
@@ -751,52 +477,18 @@ bool encode(const TmapDesc& d, CUtensorMap* out, char* err, int errlen) {
 }
 
 template <int BN, bool B_MN, int EPI>
-cudaError_t launch_fwd_epi1(const IGemmPlan* p, cudaStream_t s) {
+cudaError_t launch_fwd_epi(const IGemmPlan* p, cudaStream_t s) {
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(igemm_fwd_kernel<BN, B_MN, EPI, 1>,
+    cudaError_t e = cudaFuncSetAttribute(igemm_fwd_kernel<BN, B_MN, EPI>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          FwdCfg<BN>::kSmem);
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  igemm_fwd_kernel<BN, B_MN, EPI, 1><<<p->grid, kThreads, FwdCfg<BN>::kSmem, s>>>(
+  igemm_fwd_kernel<BN, B_MN, EPI><<<p->grid, kThreads, FwdCfg<BN>::kSmem, s>>>(
       p->tmA, p->tmB, p->fa, p->total_work);
   return cudaGetLastError();
-}
-
-// CTA-pair variant: cluster (2,1,1) launch; only N = 256 tiles are built that way
-template <bool B_MN, int EPI>
-cudaError_t launch_fwd_epi2(const IGemmPlan* p, cudaStream_t s) {
-  auto kern = igemm_fwd_kernel<256, B_MN, EPI, 2>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         FwdCfg<256, 2>::kSmem);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(p->grid);
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = FwdCfg<256, 2>::kSmem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kern, p->tmA, p->tmB, p->fa, p->total_work);
-}
-
-template <int BN, bool B_MN, int EPI>
-cudaError_t launch_fwd_epi(const IGemmPlan* p, cudaStream_t s) {
-  if constexpr (BN == 256) {
-    if (p->cta_group == 2) return launch_fwd_epi2<B_MN, EPI>(p, s);
-  }
-  return launch_fwd_epi1<BN, B_MN, EPI>(p, s);
 }
 
 template <int BN, bool B_MN>
@@ -851,28 +543,7 @@ IGemmPlan* igemm_plan_fwd(const TmapDesc& a, const TmapDesc& b, const FwdArgs& a
   IGemmPlan* p = new (std::nothrow) IGemmPlan();
   if (!p) return nullptr;
   memset(p, 0, sizeof(*p));
-  // CTA pairs (cta_group::2) for N = 256 tiles that stream B: the 3x3 layers and the deep 1x1
-  // layers, which are bound by operand traffic (weight-stationary problems keep B resident in
-  // one CTA and gain nothing).  TFOS_IGEMM_2CTA=0 disables, =1 forces it wherever it is legal.
-  static const int mode_2cta = [] {
-    const char* e = getenv("TFOS_IGEMM_2CTA");
-    return e == nullptr ? 2 : atoi(e);   // 2 = automatic
-  }();
-  const int k_iters0 = args.num_taps * args.k_chunks;
-  const long long m_boxes = static_cast<long long>(args.tiles_w) * args.tiles_h * args.tiles_n;
-  const long long b_bytes0 = static_cast<long long>(k_iters0) * bn * 128;
-  const bool would_be_resident =
-      args.n_tiles <= 8 && args.n_tiles * m_boxes >= 2 * num_sms &&
-      b_bytes0 + kMinAStages * kABytes <= static_cast<long long>(FwdCfg<256>::kStages) * FwdCfg<256>::kStage;
-  const bool legal_2cta = bn == 256 && !args.stem && m_boxes >= 2 && args.n_valid % 256 == 0 &&
-                          (b_mn || true);
-  const bool want_2cta = mode_2cta == 1 ? legal_2cta
-                         : (mode_2cta == 2 ? (legal_2cta && !would_be_resident &&
-                                              args.n_tiles * ((m_boxes + 1) / 2) >= num_sms / 2)
-                                           : false);
-  TmapDesc b2 = b;
-  if (want_2cta && !b_mn) b2.box[1] = bn / 2;   // K-major B: each CTA loads half of the N rows
-  if (!encode(a, &p->tmA, err, errlen) || !encode(b2, &p->tmB, err, errlen)) {
+  if (!encode(a, &p->tmA, err, errlen) || !encode(b, &p->tmB, err, errlen)) {
     delete p;
     return nullptr;
   }
@@ -880,20 +551,7 @@ IGemmPlan* igemm_plan_fwd(const TmapDesc& a, const TmapDesc& b, const FwdArgs& a
   p->kind = 0;
   p->bn = bn;
   p->b_mn = b_mn;
-  p->cta_group = want_2cta ? 2 : 1;
   p->total_work = args.n_tiles * args.tiles_w * args.tiles_h * args.tiles_n;
-  if (want_2cta) {
-    const int pairs_avail = num_sms / 2;
-    p->total_work = args.n_tiles * static_cast<int>((m_boxes + 1) / 2);
-    int pairs = p->total_work < pairs_avail ? p->total_work : pairs_avail;
-    // pairs pinned to one n tile keep the fused statistics in registers (as for single CTAs)
-    if (args.n_tiles > 1 && args.n_tiles <= 8 && p->total_work >= 2 * pairs_avail)
-      pairs = pairs_avail - pairs_avail % args.n_tiles;
-    p->grid = 2 * pairs;
-    p->fa.b_resident = 0;
-    p->fa.a_stages = 0;
-    return p;
-  }
   p->grid = p->total_work < num_sms ? p->total_work : num_sms;
   // a grid that is a multiple of n_tiles pins every CTA to one n tile: the fused statistics
   // then stay in registers until the CTA is done, and the filter tile can stay resident
@@ -956,14 +614,6 @@ IGemmPlan* igemm_plan_wgrad(const TmapDesc& a, const TmapDesc& b, const WgradArg
   p->kind = 1;
   p->bn = bn;
   p->total_work = args.num_taps * args.m_tiles * args.n_tiles * args.k_splits;
-  if (args.wide) {  // igemm_wgrad_wide_kernel: two m tiles x 256 columns per work item
-    if (bn != 256 || args.box_rows > 64) {
-      snprintf(err, errlen, "wide wgrad: needs bn 256 and pixel boxes of at most 64 rows");
-      delete p;
-      return nullptr;
-    }
-    p->total_work = args.num_taps * ((args.m_tiles + 1) / 2) * args.n_tiles * args.k_splits;
-  }
   if (args.stem) {  // igemm_wgrad_halo_kernel: several taps per pass over the pixels
     const long long b_box = static_cast<long long>(args.box_w) * args.halo_rows * 128;
     const long long stage = 128 * 128 + args.halo_boxes * b_box;

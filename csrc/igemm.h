@@ -1,4 +1,4 @@
-// Implicit-GEMM plans for the tcgen05 kernels in igemm.cu.
+// Implicit-GEMM plans for the wgmma kernels in igemm.cu / igemm_wgrad.cu.
 //
 // One kernel family covers dense layers, 1x1 / 3x3 / strided convolutions,
 // their data gradients (and therefore transposed convolutions) and their
@@ -87,7 +87,6 @@ struct WgradArgs {
   int halo_jmul, halo_rowbytes;   // K slice j of accumulator t reads B at (j*jmul + acc_row[t]) * rowbytes
   int halo_nacc, halo_stages;
   int acc_box[kMaxTaps], acc_row[kMaxTaps], box_dw[3];
-  int wide;                       // 256 x 256 tile per CTA (igemm_wgrad_wide_kernel), boxes <= 64 px
 };
 
 struct IGemmPlan {
@@ -99,7 +98,6 @@ struct IGemmPlan {
   int b_mn;  // fwd-like only: B is MN-major ([K rows, N cols])
   int grid;
   int total_work;
-  int cta_group;  // fwd-like only: 2 = CTA pairs (cluster launch, M = 256 per MMA), else 1
 };
 
 // Returns nullptr and fills err on failure.

@@ -1,6 +1,6 @@
-// Weight-gradient tcgen05 kernel (split out of igemm.cu): dW[m, tap, n] += sum over pixels.
-// See igemm.cu for the structure shared by both kernels (TMA producer warp, single-thread
-// MMA issuer with TMEM accumulators, epilogue warps).
+// Weight-gradient wgmma kernels (split out of igemm.cu): dW[m, tap, n] += sum over pixels.
+// See igemm.cu for the structure shared by all of them (a TMA producer warpgroup, two consumer
+// warpgroups that issue wgmma and keep the fp32 accumulators in registers).
 #include <stdio.h>
 #include <string.h>
 
@@ -11,20 +11,53 @@ namespace tfos {
 
 namespace {
 
-constexpr int kThreads = 192;
-constexpr int kBlockM = 128;
+constexpr int kThreads = 384;
+
+// Stage ring shared by the weight-gradient kernels: one elected producer thread, two consumer
+// warpgroups releasing each stage once the wgmma group that read it has retired.
+struct Ring {
+  uint64_t* full;
+  uint64_t* empty;
+  int n, stage;
+  uint32_t phase;
+  __device__ void advance() {
+    if (++stage == n) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+};
+
+__device__ __forceinline__ void init_ring_bars(uint64_t* full, uint64_t* empty, int n) {
+  for (int i = 0; i < n; ++i) {
+    mbar_init(&full[i], 1);
+    mbar_init(&empty[i], 2);   // one arrive per consumer warpgroup
+  }
+  fence_mbar_init();
+}
+
+// adds a thread's accumulator pair (columns col, col + 1) of one dW row
+__device__ __forceinline__ void red_pair(float* o, int col, int n_valid, bool vec_ok, float x,
+                                         float y) {
+  if (vec_ok && col + 1 < n_valid) {
+    red_add_f32x2(o, x, y);
+  } else {
+    if (col < n_valid) atomicAdd(o, x);
+    if (col + 1 < n_valid) atomicAdd(o + 1, y);
+  }
+}
 
 // ------------------------------------------------------------------- wgrad
 // dW[m, tap, n] += sum_pixels dY[pixel, m] * X[pixel + tap, n].  Both operands
 // are MN-major in shared memory (the contiguous global dimension is channels,
 // the reduction runs over pixel rows), one TMA box of <=128 pixels per stage.
+// Warpgroup g computes output rows [64 g, 64 g + 64) of the 128 x BN tile.
 template <int BN>
 struct WgCfg {
   static constexpr int kAStage = 2 * 128 * 128;          // two 64-channel boxes, <=128 pixels
   static constexpr int kBStage = (BN / 64) * 128 * 128;
   static constexpr int kStage = kAStage + kBStage;
   static constexpr int kStages = (BN <= 64) ? 4 : (BN <= 128 ? 3 : 2);
-  static constexpr int kTmemCols = 2 * BN;
   static constexpr int kSmem = kStages * kStage + 256 + 1024;
 };
 
@@ -37,36 +70,17 @@ igemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStage);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + Cfg::kStages;
-  uint64_t* tfull = bars + 2 * Cfg::kStages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  Ring ring{bars, bars + Cfg::kStages, Cfg::kStages, 0, 0};
 
   const int warp = __shfl_sync(0xffffffff, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < Cfg::kStages; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 4);
-    }
-    fence_mbar_init();
+    init_ring_bars(ring.full, ring.empty, Cfg::kStages);
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int total_boxes = a.tiles_w * a.tiles_h * a.tiles_n;
   const int boxes_per_split = (total_boxes + a.k_splits - 1) / a.k_splits;
@@ -86,10 +100,8 @@ igemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     b1 = min(b0 + boxes_per_split, total_boxes);
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+  if (warp < 4) {
+    if (threadIdx.x == 0) {
       for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
         int t, mt, nt, b0, b1;
         decode(work, t, mt, nt, b0, b1);
@@ -98,102 +110,71 @@ igemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
           const int th = (b / a.tiles_w) % a.tiles_h;
           const int tn = b / (a.tiles_w * a.tiles_h);
           const int pw = tw * a.box_w, ph = th * a.box_h, pn = tn * a.box_n;
-          mbar_wait(&empty[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * Cfg::kStage;
+          mbar_wait(&ring.empty[ring.stage], ring.phase ^ 1);
+          uint8_t* sA = smem + ring.stage * Cfg::kStage;
           uint8_t* sB = sA + Cfg::kAStage;
-          mbar_expect_tx(&full[stage], stage_tx);
+          uint64_t* bar = &ring.full[ring.stage];
+          mbar_expect_tx(bar, stage_tx);
 #pragma unroll
           for (int j = 0; j < 2; ++j)
-            tma_load_4d(sA + j * box_bytes, &tmA, &full[stage], mt * 128 + j * 64, pw, ph, pn);
+            tma_load_4d(sA + j * box_bytes, &tmA, bar, mt * 128 + j * 64, pw, ph, pn);
 #pragma unroll
           for (int j = 0; j < BN / 64; ++j)
-            tma_load_4d(sB + j * box_bytes, &tmB, &full[stage], nt * BN + j * 64 + a.tap_dc[t],
+            tma_load_4d(sB + j * box_bytes, &tmB, bar, nt * BN + j * 64 + a.tap_dc[t],
                         pw * a.mul_w + a.tap_dw[t], ph * a.mul_h + a.tap_dh[t], pn);
-          if (++stage == Cfg::kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
+          ring.advance();
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(kBlockM, BN, true, true);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      const int mmas = a.box_rows / 16;
-      for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
-        int t, mt, nt, b0, b1;
-        decode(work, t, mt, nt, b0, b1);
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int b = b0; b < b1; ++b) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_base = smem_u32(smem + stage * Cfg::kStage);
-          const uint32_t b_base = a_base + Cfg::kAStage;
-          // one thread issues every MMA: keep its per-MMA work to two 64-bit adds (the start
-          // address is the low field of the descriptor; 2048 B = 128 units of 16 B)
-          const uint64_t ad0 = umma_desc_sw128(a_base, box_bytes, 1024);
-          const uint64_t bd0 = umma_desc_sw128(b_base, box_bytes, 1024);
-          for (int k = 0; k < mmas; ++k)
-            umma_bf16(d_tmem, ad0 + k * 128, bd0 + k * 128, idesc, (b > b0 || k > 0) ? 1u : 0u);
-          umma_commit(&empty[stage]);
-          if (++stage == Cfg::kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tfull[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
-      int t, mt, nt, b0, b1;
-      decode(work, t, mt, nt, b0, b1);
-      const int m = mt * 128 + q * 32 + lane;
-      const bool valid = m < a.m_valid && b1 > b0;
-      float* o = a.dw + static_cast<long long>(m) * a.ldw + a.tap_out[t] + nt * BN;
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN + c * 32, v);
-        tmem_ld_wait();
-        const int col0 = nt * BN + c * 32;
-        if (valid) {
-          if (col0 + 32 <= a.n_valid && (a.ldw & 3) == 0 && (a.tap_out[t] & 3) == 0) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              red_add_f32x4(o + c * 32 + j, __uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                            __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (col0 + j < a.n_valid) atomicAdd(o + c * 32 + j, __uint_as_float(v[j]));
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, Cfg::kTmemCols);
+  const int wg = (warp >> 2) - 1;
+  const int wq = warp & 3;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const int mmas = a.box_rows / 16;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
+    int t, mt, nt, b0, b1;
+    decode(work, t, mt, nt, b0, b1);
+    int prev = -1;
+    wgmma_fence_regs(acc);
+    for (int b = b0; b < b1; ++b) {
+      mbar_wait(&ring.full[ring.stage], ring.phase);
+      const uint32_t a_base = smem_u32(smem + ring.stage * Cfg::kStage);
+      const uint32_t b_base = a_base + Cfg::kAStage;
+      const uint64_t ad0 = wgmma_desc_sw128(a_base + wg * box_bytes, box_bytes, 1024);
+      const uint64_t bd0 = wgmma_desc_sw128(b_base, box_bytes, 1024);
+      wgmma_fence();
+      for (int k = 0; k < mmas; ++k)   // 16 pixels = 2048 B = 128 units of 16 B per step
+        Wgmma<BN>::template mma<1, 1>(acc, ad0 + k * 128, bd0 + k * 128,
+                                      (b > b0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && wg_leader) mbar_arrive(&ring.empty[prev]);
+      prev = ring.stage;
+      ring.advance();
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    if (prev >= 0 && wg_leader) mbar_arrive(&ring.empty[prev]);
+    if (b1 <= b0) continue;
+    const bool vec_ok = (a.ldw & 1) == 0 && (a.tap_out[t] & 1) == 0;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = mt * 128 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+      if (m >= a.m_valid) continue;
+      float* o = a.dw + static_cast<long long>(m) * a.ldw + a.tap_out[t] + nt * BN;
+#pragma unroll
+      for (int jb = 0; jb < BN / 8; ++jb) {
+        const int c = jb * 8 + 2 * (lane & 3);
+        red_pair(o + c, nt * BN + c, a.n_valid, vec_ok, acc[4 * jb + 2 * h],
+                 acc[4 * jb + 2 * h + 1]);
+      }
+    }
+  }
 }
 
 // ------------------------------------------------------------- halo wgrad
@@ -205,18 +186,18 @@ igemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 //       rows above / below; accumulator t multiplies K slice j (16 pixels = 2048 B of A) with the
 //       B rows at (j * jmul + acc_row[t]) * rowbytes of box acc_box[t] - a filter tap only moves
 //       the descriptor's start address, by a multiple of 1024 B (SWIZZLE_128B atoms stay aligned).
-// Each accumulator is 64 TMEM columns (up to 8 of them = 512 columns, single-buffered).
+// Each accumulator is 64 x 64 fp32; consumer warpgroup g keeps accumulators g, g + 2, g + 4, g + 6
+// in registers (up to 8 of them).
 //   stem 7x7/2 (window-row layout, ops/igemm.py): 16 x 8 pixels, one 16 x 21 box, 7 accumulators
 //     (filter rows), K slice j = output row j, B row 2j + r;          3.9x fewer bytes than 7 passes
 //   3x3/1 64->64: 8 x 16 pixels, three 8 x 18 boxes (dw = -1, 0, +1), 8 accumulators (all taps but
 //     the centre, which the generic kernel adds), K slice j = output rows 2j, 2j+1 (2 x 1024 B),
 //     B row 2j + dh + 1;                                              4x fewer bytes than 9 passes
-// The MMA is M = 128 wide; rows 64..127 of every accumulator are scratch (their A "half" is
-// whatever follows the dY box in shared memory) and are never read.
 constexpr int kHaloA = 128 * 128;                    // dY box: 128 pixels x 64 channels x 2 B
 constexpr int kHaloMaxStages = 3;
 constexpr int kHaloSmemData = 216 * 1024;            // stem 3 x 58 KB, 3x3 3 x 70 KB
 constexpr int kHaloSmem = kHaloSmemData + 256 + 1024;
+constexpr int kHaloAccPerWg = kMaxTaps / 2;          // 4 (8 accumulators at most, see igemm.cu)
 
 __global__ void __launch_bounds__(kThreads, 1)
 igemm_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA,
@@ -226,326 +207,110 @@ igemm_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA,
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kHaloSmemData);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + kHaloMaxStages;
-  uint64_t* tfull = bars + 2 * kHaloMaxStages;
-  uint64_t* tempty = tfull + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 1);
+  Ring ring{bars, bars + kHaloMaxStages, a.halo_stages, 0, 0};
 
   const int warp = __shfl_sync(0xffffffff, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < kHaloMaxStages; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    mbar_init(tfull, 1);
-    mbar_init(tempty, 4);
-    fence_mbar_init();
+    init_ring_bars(ring.full, ring.empty, kHaloMaxStages);
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int total_boxes = a.tiles_w * a.tiles_h * a.tiles_n;
   const int per_split = (total_boxes + a.k_splits - 1) / a.k_splits;
   const uint32_t b_box = static_cast<uint32_t>(a.box_w) * a.halo_rows * 128u;   // one halo box
   const uint32_t stage_bytes = kHaloA + a.halo_boxes * b_box;                   // multiple of 1024
-  const int nstages = a.halo_stages;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+  if (warp < 4) {
+    if (threadIdx.x == 0) {
       for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
         const int b0 = work * per_split, b1 = min(b0 + per_split, total_boxes);
         for (int b = b0; b < b1; ++b) {
           const int tw = b % a.tiles_w;
           const int th = (b / a.tiles_w) % a.tiles_h;
           const int tn = b / (a.tiles_w * a.tiles_h);
-          mbar_wait(&empty[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * stage_bytes;
-          mbar_expect_tx(&full[stage], stage_bytes);
-          tma_load_4d(sA, &tmA, &full[stage], 0, tw * a.box_w, th * a.box_h, tn);
+          mbar_wait(&ring.empty[ring.stage], ring.phase ^ 1);
+          uint8_t* sA = smem + ring.stage * stage_bytes;
+          uint64_t* bar = &ring.full[ring.stage];
+          mbar_expect_tx(bar, stage_bytes);
+          tma_load_4d(sA, &tmA, bar, 0, tw * a.box_w, th * a.box_h, tn);
           for (int i = 0; i < a.halo_boxes; ++i)
-            tma_load_4d(sA + kHaloA + i * b_box, &tmB, &full[stage], 0, tw * a.box_w + a.box_dw[i],
+            tma_load_4d(sA + kHaloA + i * b_box, &tmB, bar, 0, tw * a.box_w + a.box_dw[i],
                         th * a.box_h * a.halo_hmul + a.halo_h0, tn);
-          if (++stage == nstages) {
-            stage = 0;
-            phase ^= 1;
-          }
+          ring.advance();
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(kBlockM, 64, true, true);
-      int stage = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      uint32_t acc_off[kMaxTaps];   // descriptor offset (16-byte units) of each accumulator's B rows
-      for (int t = 0; t < kMaxTaps; ++t)
-        acc_off[t] = (a.acc_box[t] * b_box + a.acc_row[t] * a.halo_rowbytes) >> 4;
-      const uint32_t jstep = (a.halo_jmul * a.halo_rowbytes) >> 4;
-      for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
-        const int b0 = work * per_split, b1 = min(b0 + per_split, total_boxes);
-        mbar_wait(tempty, acc_phase ^ 1);
-        tc_fence_after();
-        for (int b = b0; b < b1; ++b) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_base = smem_u32(smem + stage * stage_bytes);
-          const uint32_t b_base = a_base + kHaloA;
-          // A: second 64-row half = kHaloA bytes further on (scratch rows, see above).  One thread
-          // issues all 56-64 MMAs of a stage: descriptors advance by plain 64-bit adds.
-          const uint64_t ad0 = umma_desc_sw128(a_base, kHaloA, 1024);
-          const uint64_t bd0 = umma_desc_sw128(b_base, 2048, 1024);
-          const uint32_t first = (b > b0) ? 1u : 0u;
-          for (int t = 0; t < a.halo_nacc; ++t) {
-            const uint64_t bt = bd0 + acc_off[t];
-            const uint32_t d = tmem_base + t * 64;
-            umma_bf16(d, ad0, bt, idesc, first);
-#pragma unroll
-            for (int j = 1; j < 8; ++j) umma_bf16(d, ad0 + j * 128, bt + j * jstep, idesc, 1u);
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == nstages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(tfull);
-        acc_phase ^= 1;
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    uint32_t acc_phase = 0;
-    for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
-      const int b0 = work * per_split, b1 = min(b0 + per_split, total_boxes);
-      const int m = q * 32 + lane;
-      const bool valid = m < a.m_valid && m < 64 && b1 > b0;
-      mbar_wait(tfull, acc_phase);
-      tc_fence_after();
-      if (q < 2) {
-#pragma unroll 1
-        for (int c = 0; c < 2 * a.halo_nacc; ++c) {  // accumulators x two 32-column chunks
-          uint32_t v[32];
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c * 32, v);
-          tmem_ld_wait();
-          if (valid) {
-            float* o = a.dw + static_cast<long long>(m) * a.ldw + a.tap_out[c >> 1] + (c & 1) * 32;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              red_add_f32x4(o + j, __uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                            __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty);
-      acc_phase ^= 1;
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
-}
+  const int wg = (warp >> 2) - 1;
+  const int wq = warp & 3;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  uint32_t acc_off[kHaloAccPerWg];   // descriptor offset (16-byte units) of each accumulator's B rows
+#pragma unroll
+  for (int i = 0; i < kHaloAccPerWg; ++i) {
+    const int t = 2 * i + wg;
+    acc_off[i] = t < a.halo_nacc ? (a.acc_box[t] * b_box + a.acc_row[t] * a.halo_rowbytes) >> 4 : 0;
+  }
+  const uint32_t jstep = (a.halo_jmul * a.halo_rowbytes) >> 4;
+  float acc[kHaloAccPerWg][32];
+#pragma unroll
+  for (int i = 0; i < kHaloAccPerWg; ++i)
+#pragma unroll
+    for (int j = 0; j < 32; ++j) acc[i][j] = 0.f;
 
-// ------------------------------------------------------------- wide wgrad
-// 256 x 256 output tile per CTA (two 128-row accumulators x 256 columns = all 512 TMEM columns):
-// the generic kernel's 128 x 128 tile needs (128+128) channels x 2 B of operands per pixel for
-// 16 K MACs and is bound by the L2 -> SM fabric (profiles/ncu_l3c2_r1.txt: 10.3 TB/s of L2 reads at
-// 33 % tensor activity); this tile needs (256+256) x 2 B for 64 K MACs - half the bytes per MAC.
-// Stages are 64 pixels (4 + 4 boxes of 8 KB) so that three of them fit; the accumulators are
-// single-buffered (a work item's K loop is long, its epilogue short).
-constexpr int kWideBox = 64 * 128;                  // 64 pixels x 64 channels x 2 B
-constexpr int kWideStage = 8 * kWideBox;            // A: 2 m-tiles x 2 halves, B: 4 column blocks
-constexpr int kWideStages = 3;
-constexpr int kWideSmem = kWideStages * kWideStage + 256 + 1024;
-
-__global__ void __launch_bounds__(kThreads, 1)
-igemm_wgrad_wide_kernel(const __grid_constant__ CUtensorMap tmA,
-                        const __grid_constant__ CUtensorMap tmB, const WgradArgs a,
-                        const int total_work) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWideStages * kWideStage);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + kWideStages;
-  uint64_t* tfull = bars + 2 * kWideStages;
-  uint64_t* tempty = tfull + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 1);
-
-  const int warp = __shfl_sync(0xffffffff, threadIdx.x >> 5, 0);
-  const int lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < kWideStages; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
+  for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
+    const int b0 = work * per_split, b1 = min(b0 + per_split, total_boxes);
+    int prev = -1;
+#pragma unroll
+    for (int i = 0; i < kHaloAccPerWg; ++i) wgmma_fence_regs(acc[i]);
+    for (int b = b0; b < b1; ++b) {
+      mbar_wait(&ring.full[ring.stage], ring.phase);
+      const uint32_t a_base = smem_u32(smem + ring.stage * stage_bytes);
+      const uint64_t ad0 = wgmma_desc_sw128(a_base, kHaloA, 1024);
+      const uint64_t bd0 = wgmma_desc_sw128(a_base + kHaloA, 2048, 1024);
+      const uint32_t first = (b > b0) ? 1u : 0u;
+      wgmma_fence();
+#pragma unroll
+      for (int i = 0; i < kHaloAccPerWg; ++i) {
+        if (2 * i + wg < a.halo_nacc) {
+          const uint64_t bt = bd0 + acc_off[i];
+          Wgmma<64>::mma<1, 1>(acc[i], ad0, bt, first);
+#pragma unroll
+          for (int j = 1; j < 8; ++j) Wgmma<64>::mma<1, 1>(acc[i], ad0 + j * 128, bt + j * jstep, 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && wg_leader) mbar_arrive(&ring.empty[prev]);
+      prev = ring.stage;
+      ring.advance();
     }
-    mbar_init(tfull, 1);
-    mbar_init(tempty, 4);
-    fence_mbar_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  const int total_boxes = a.tiles_w * a.tiles_h * a.tiles_n;
-  const int boxes_per_split = (total_boxes + a.k_splits - 1) / a.k_splits;
-  const uint32_t box_bytes = static_cast<uint32_t>(a.box_rows) * 128u;   // <= kWideBox
-  const uint32_t stage_tx = box_bytes * 8u;
-  const int m_pairs = (a.m_tiles + 1) / 2;
-
-  auto decode = [&](int work, int& t, int& mp, int& nt, int& b0, int& b1) {
-    const int ks = work % a.k_splits;
-    int r = work / a.k_splits;
-    nt = r % a.n_tiles;
-    r /= a.n_tiles;
-    mp = r % m_pairs;
-    t = r / m_pairs;
-    b0 = ks * boxes_per_split;
-    b1 = min(b0 + boxes_per_split, total_boxes);
-  };
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
-        int t, mp, nt, b0, b1;
-        decode(work, t, mp, nt, b0, b1);
-        for (int b = b0; b < b1; ++b) {
-          const int tw = b % a.tiles_w;
-          const int th = (b / a.tiles_w) % a.tiles_h;
-          const int tn = b / (a.tiles_w * a.tiles_h);
-          const int pw = tw * a.box_w, ph = th * a.box_h, pn = tn * a.box_n;
-          mbar_wait(&empty[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * kWideStage;
-          uint8_t* sB = sA + 4 * kWideBox;
-          mbar_expect_tx(&full[stage], stage_tx);
+    wgmma_wait<0>();
 #pragma unroll
-          for (int j = 0; j < 4; ++j)   // channels beyond Cout are zero-filled by TMA
-            tma_load_4d(sA + j * box_bytes, &tmA, &full[stage], mp * 256 + j * 64, pw, ph, pn);
+    for (int i = 0; i < kHaloAccPerWg; ++i) wgmma_fence_regs(acc[i]);
+    if (prev >= 0 && wg_leader) mbar_arrive(&ring.empty[prev]);
+    if (b1 <= b0) continue;
 #pragma unroll
-          for (int j = 0; j < 4; ++j)
-            tma_load_4d(sB + j * box_bytes, &tmB, &full[stage], nt * 256 + j * 64 + a.tap_dc[t],
-                        pw * a.mul_w + a.tap_dw[t], ph * a.mul_h + a.tap_dh[t], pn);
-          if (++stage == kWideStages) {
-            stage = 0;
-            phase ^= 1;
-          }
+    for (int h = 0; h < 2; ++h) {
+      const int m = wq * 16 + (lane >> 2) + 8 * h;
+      if (m >= a.m_valid) continue;
+#pragma unroll
+      for (int i = 0; i < kHaloAccPerWg; ++i) {
+        const int t = 2 * i + wg;
+        if (t >= a.halo_nacc) continue;
+        float* o = a.dw + static_cast<long long>(m) * a.ldw + a.tap_out[t];
+#pragma unroll
+        for (int jb = 0; jb < 8; ++jb) {
+          const int c = jb * 8 + 2 * (lane & 3);
+          red_add_f32x2(o + c, acc[i][4 * jb + 2 * h], acc[i][4 * jb + 2 * h + 1]);
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(kBlockM, 256, true, true);
-      int stage = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      const int mmas = a.box_rows / 16;
-      for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
-        int t, mp, nt, b0, b1;
-        decode(work, t, mp, nt, b0, b1);
-        mbar_wait(tempty, acc_phase ^ 1);
-        tc_fence_after();
-        for (int b = b0; b < b1; ++b) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_base = smem_u32(smem + stage * kWideStage);
-          const uint32_t b_base = a_base + 4 * kWideBox;
-          const uint64_t ad0 = umma_desc_sw128(a_base, box_bytes, 1024);
-          const uint64_t ad1 = umma_desc_sw128(a_base + 2 * box_bytes, box_bytes, 1024);
-          const uint64_t bd0 = umma_desc_sw128(b_base, box_bytes, 1024);
-          for (int k = 0; k < mmas; ++k) {
-            const uint32_t accf = (b > b0 || k > 0) ? 1u : 0u;
-            umma_bf16(tmem_base, ad0 + k * 128, bd0 + k * 128, idesc, accf);
-            umma_bf16(tmem_base + 256, ad1 + k * 128, bd0 + k * 128, idesc, accf);
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == kWideStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(tfull);
-        acc_phase ^= 1;
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    uint32_t acc_phase = 0;
-    for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
-      int t, mp, nt, b0, b1;
-      decode(work, t, mp, nt, b0, b1);
-      mbar_wait(tfull, acc_phase);
-      tc_fence_after();
-      const bool vec_ok = (a.ldw & 3) == 0 && (a.tap_out[t] & 3) == 0;
-#pragma unroll 1
-      for (int mt = 0; mt < 2; ++mt) {
-        const int m = mp * 256 + mt * 128 + q * 32 + lane;
-        const bool valid = m < a.m_valid && b1 > b0;
-        float* o = a.dw + static_cast<long long>(m) * a.ldw + a.tap_out[t] + nt * 256;
-#pragma unroll 1
-        for (int c = 0; c < 8; ++c) {
-          uint32_t v[32];
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + mt * 256 + c * 32, v);
-          tmem_ld_wait();
-          const int col0 = nt * 256 + c * 32;
-          if (valid) {
-            if (col0 + 32 <= a.n_valid && vec_ok) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4)
-                red_add_f32x4(o + c * 32 + j, __uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                              __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (col0 + j < a.n_valid) atomicAdd(o + c * 32 + j, __uint_as_float(v[j]));
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty);
-      acc_phase ^= 1;
-    }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
-}
-
-cudaError_t launch_wgrad_wide(const IGemmPlan* p, cudaStream_t s) {
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(igemm_wgrad_wide_kernel,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, kWideSmem);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
-  igemm_wgrad_wide_kernel<<<p->grid, kThreads, kWideSmem, s>>>(p->tmA, p->tmB, p->wa,
-                                                              p->total_work);
-  return cudaGetLastError();
 }
 
 cudaError_t launch_wgrad_stem(const IGemmPlan* p, cudaStream_t s) {
@@ -580,7 +345,6 @@ cudaError_t launch_wgrad(const IGemmPlan* p, cudaStream_t s) {
 
 cudaError_t igemm_run_wgrad(const IGemmPlan* p, cudaStream_t s) {
   if (p->wa.stem) return launch_wgrad_stem(p, s);
-  if (p->wa.wide) return launch_wgrad_wide(p, s);
   switch (p->bn) {
     case 64: return launch_wgrad<64>(p, s);
     case 128: return launch_wgrad<128>(p, s);

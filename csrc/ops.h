@@ -1,4 +1,4 @@
-// C++ entry points of the non-GEMM sm_100a kernels (elementwise.cu,
+// C++ entry points of the non-GEMM sm_90a kernels (elementwise.cu,
 // optim_comm.cu, feed.cu).  All functions enqueue on the given stream and
 // return the launch status; none of them synchronises.
 #pragma once

@@ -589,7 +589,7 @@ cudaError_t flag_barrier(const BcastArgs& a, cudaStream_t s) {
 cudaError_t ps_push_dense(float* w_ps, const float* g, long long n, const float* hyper,
                           cudaStream_t s) {
   long long blocks = (n / 4 + 255) / 256;
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > kSmCount * 4) blocks = kSmCount * 4;
   if (blocks < 1) blocks = 1;
   ps_push_dense_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(w_ps, g, n, hyper);
   return cudaGetLastError();
@@ -597,7 +597,7 @@ cudaError_t ps_push_dense(float* w_ps, const float* g, long long n, const float*
 cudaError_t ps_push_sparse(float* w_ps, const float* g_rows, const int* idx, int nrows, int width,
                            const float* hyper, cudaStream_t s) {
   long long blocks = (static_cast<long long>(nrows) * width / ((width & 3) == 0 ? 4 : 1) + 255) / 256;
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > kSmCount * 4) blocks = kSmCount * 4;
   if (blocks < 1) blocks = 1;
   ps_push_sparse_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(w_ps, g_rows, idx, nrows,
                                                                      width, hyper);
@@ -605,7 +605,7 @@ cudaError_t ps_push_sparse(float* w_ps, const float* g_rows, const int* idx, int
 }
 cudaError_t ps_apply(const PsApplyArgs& a, int opt, cudaStream_t s) {
   if ((a.n & 7) != 0 || (a.lo & 7) != 0) return cudaErrorInvalidValue;
-  const int grid = 148 * 2;
+  const int grid = kSmCount * 2;
   switch (opt) {
     case kOptSgd: ps_apply_kernel<kOptSgd><<<grid, 512, 0, s>>>(a); break;
     case kOptMomentum: ps_apply_kernel<kOptMomentum><<<grid, 512, 0, s>>>(a); break;
@@ -627,7 +627,7 @@ cudaError_t ps_pull_model(const PsPullArgs& a, int grid, cudaStream_t s) {
 }
 cudaError_t ps_pull(const float* w_ps, float* w_local, void* w_bf16, long long n, cudaStream_t s) {
   long long blocks = (n / 4 + 255) / 256;
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > kSmCount * 4) blocks = kSmCount * 4;
   if (blocks < 1) blocks = 1;
   ps_pull_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
       w_ps, w_local, static_cast<__nv_bfloat16*>(w_bf16), n);

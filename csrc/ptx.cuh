@@ -1,7 +1,7 @@
-// Thin inline-PTX wrappers for the sm_100a programming model: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and the
-// system-scope acquire/release accessors used by the cross-GPU kernels.
-// Everything in here is sm_100a-only by design: there is no fallback path.
+// Thin inline-PTX wrappers for the sm_90a programming model: mbarrier, TMA
+// (cp.async.bulk.tensor), wgmma and the system-scope acquire/release
+// accessors used by the cross-GPU kernels.
+// Everything in here is sm_90a-only by design: there is no fallback path.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -10,6 +10,9 @@
 #include <stdio.h>
 
 namespace tfos {
+
+// SMs of an H100 SXM: the grid-size caps of the grid-stride streaming kernels are multiples of it
+constexpr int kSmCount = 132;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -61,7 +64,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Bounded wait: a protocol bug must trap (and surface as a CUDA error through
-// the node's error queue) instead of hanging the GPU box.
+// the node's error queue) instead of hanging the GPU.  No printf here: a call
+// inside the wait would make ptxas serialize the wgmma pipeline around it.
 #ifndef TFOS_MBAR_TIMEOUT_NS
 #define TFOS_MBAR_TIMEOUT_NS 4000000000ull
 #endif
@@ -70,11 +74,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint64_t t0 = globaltimer_ns();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > TFOS_MBAR_TIMEOUT_NS) {
-      printf("tfos: mbarrier timeout block=%d thread=%d parity=%u\n", blockIdx.x, threadIdx.x,
-             parity);
-      __trap();
-    }
+    if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > TFOS_MBAR_TIMEOUT_NS) __trap();
   }
 }
 
@@ -99,158 +99,128 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ----------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
+// ------------------------------------------------------------------ wgmma
+// Warpgroup MMA (sm_90a): the four warps of a warpgroup issue one wgmma together and receive a
+// 64 x N fp32 accumulator in registers.  Thread t of warp w holds rows 16 w + t / 4 and
+// 16 w + t / 4 + 8; for each 8-column block j, d[4 j + 0, 1] are columns 8 j + 2 (t % 4) + {0, 1}
+// of the first row and d[4 j + 2, 3] the same columns of the second.
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 -> fp32, issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once every previously issued tcgen05.mma has retired.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-// ------------------------------------------------ CTA pairs (cta_group::2)
-// Two CTAs of a cluster on the two SMs of a TPC execute ONE tcgen05.mma with M = 256: CTA r owns
-// accumulator rows [128 r, 128 r + 128) in ITS TMEM, supplies its own 128 rows of A and HALF of
-// the B tile from its own shared memory; the leader (cluster rank 0) issues the instruction.
-constexpr uint32_t kLeaderCtaMask = 0xFEFFFFFFu;  // shared::cluster address -> the pair's even CTA
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::
-                   : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2cta() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// TMA loads whose completion is counted on the LEADER's barrier (same offset, peer bit cleared)
-__device__ __forceinline__ void tma_load_4d_2cta(void* dst, const CUtensorMap* m, uint64_t* bar,
-                                                 int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kLeaderCtaMask), "r"(c0), "r"(c1),
-      "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2cta(void* dst, const CUtensorMap* m, uint64_t* bar,
-                                                 int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kLeaderCtaMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2cta(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                               uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (count 1) on the same-offset barrier of every CTA in `mask` once the MMAs issued so far
-// by this thread have retired
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64"
-      " [%0], %1;" ::"r"(smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-// arrive on the barrier at the same offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// 32 lanes x 32 columns of fp32: thread t of the warp gets lane (base+t), 32 consecutive columns.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-      " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+// D (+)= A[smem] * B[smem] for a 64 x N x 16 bf16 step.  TA / TB = 1: the operand is MN-major
+// in shared memory (the M / N index is the contiguous one), else K-major.
+template <int N>
+struct Wgmma;
+template <>
+struct Wgmma<64> {
+  template <int TA, int TB>
+  __device__ __forceinline__ static void mma(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+template <>
+struct Wgmma<128> {
+  template <int TA, int TB>
+  __device__ __forceinline__ static void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+template <>
+struct Wgmma<256> {
+  template <int TA, int TB>
+  __device__ __forceinline__ static void mma(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+        "}, %128, %129, p, 1, 1, %131, %132;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
 
-// UMMA shared-memory matrix descriptor (sm_100 "version 1"), SWIZZLE_128B.
+// wgmma shared-memory matrix descriptor, SWIZZLE_128B.
 //   bits [0,14)  start address >> 4      bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4 bits [46,48) version = 1
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes,
-                                                    uint32_t sbo_bytes) {
+//   bits [32,46) stride byte offset >> 4 bits [62,64) layout type (1 = SWIZZLE_128B)
+// K-major: SBO = 1024 (8 rows of 128 B), LBO unused.  MN-major: LBO = distance between 64-element
+// blocks of the M / N dimension, SBO = distance between groups of 8 K rows (1024).
+// Operand tiles start on 1024-byte boundaries; a 16-element K step inside a 128-byte row adds 2
+// to the start-address field, a 16-row K step of an MN-major tile adds 128.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes,
+                                                     uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3ffff) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3fff) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3fff) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 accumulate.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, bool a_mn_major,
-                                                       bool b_mn_major) {
-  return (1u << 4)                         // D format = F32
-         | (1u << 7)                       // A format = BF16
-         | (1u << 10)                      // B format = BF16
-         | ((a_mn_major ? 1u : 0u) << 15)  // A major
-         | ((b_mn_major ? 1u : 0u) << 16)  // B major
-         | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
 
 // ------------------------------------------------ system-scope sync (NVLink)
 __device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) {
@@ -289,10 +259,21 @@ __device__ __forceinline__ void st_relaxed_sys_v4(void* p, uint4 v) {
                "r"(v.y), "r"(v.z), "r"(v.w)
                : "memory");
 }
+__device__ __forceinline__ void red_add_f32x2(float* p, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
+}
 __device__ __forceinline__ void red_add_f32x4(float* p, float a, float b, float c, float d) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c),
                "f"(d)
                : "memory");
+}
+
+// fp32x2 arithmetic, one lane at a time (sm_90 has no packed fp32 pipe), round-to-nearest
+__device__ __forceinline__ float2 fadd2_rn(float2 a, float2 b) {
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {

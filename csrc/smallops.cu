@@ -156,7 +156,7 @@ depthwise3x3_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16
 inline int blocks_for(long long work) {
   long long b = (work + 255) / 256;
   if (b < 1) b = 1;
-  return static_cast<int>(b < 148 * 16 ? b : 148 * 16);
+  return static_cast<int>(b < kSmCount * 16 ? b : kSmCount * 16);
 }
 
 }  // namespace
@@ -173,7 +173,7 @@ cudaError_t conv3x3_c1_wgrad(const void* x, const void* dy, float* dw, float* db
                              int W, int Cout, cudaStream_t s) {
   const long long P = static_cast<long long>(N) * (H - 2) * (W - 2);
   long long blocks = (P + 63) / 64;
-  if (blocks > 148 * 2) blocks = 148 * 2;
+  if (blocks > kSmCount * 2) blocks = kSmCount * 2;
   if (blocks < 1) blocks = 1;
   conv3x3_c1_wgrad_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
       static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(dy), dw, dbias, N, H,

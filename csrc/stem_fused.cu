@@ -302,7 +302,7 @@ stem_pool_bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, const uint8_
 
 inline unsigned grid_blocks(long long threads) {
   long long b = (threads + 255) / 256;
-  const long long cap = 148ll * 8;
+  const long long cap = static_cast<long long>(kSmCount) * 8;
   if (b > cap) b = cap;
   return static_cast<unsigned>(b < 1 ? 1 : b);
 }

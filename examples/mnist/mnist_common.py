@@ -1,5 +1,5 @@
 """Shared pieces of the MNIST examples: one training loop that runs the torch module on CPU
-executors (gloo) and the native sm_100a trainer on B200 executors (fused all-reduce + SGD)."""
+executors (gloo) and the native sm_90a trainer on H100 executors (fused all-reduce + SGD)."""
 import time
 
 
@@ -26,7 +26,7 @@ class Trainer(object):
         comm.broadcast("aux32", root=0)
       self.xh = torch.zeros(batch_size, 784, dtype=torch.float32).pin_memory()
       self.yh = torch.zeros(batch_size, dtype=torch.int32).pin_memory()
-      self.desc = "native sm_100a trainer, world {}".format(world)
+      self.desc = "native sm_90a trainer, world {}".format(world)
     else:
       if world > 1:
         ctx.init_process_group(backend="gloo")

@@ -1,5 +1,5 @@
 """Streaming + asynchronous parameter server: a DStream of CSV micro-batches feeds the workers,
-parameters live on a 'ps' node (its GPU on B200) and are updated without barriers
+parameters live on a 'ps' node (its GPU on H100) and are updated without barriers
 (reference: examples/mnist/estimator/mnist_spark_streaming.py:86-142, ParameterServerStrategy with
 num_ps=1, feed_timeout=86400, ``cluster.shutdown(ssc)``; stop it with examples/utils/stop_streaming.py).
 

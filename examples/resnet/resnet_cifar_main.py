@@ -1,4 +1,4 @@
-"""ResNet-56 / CIFAR-10 on ONE B200 (no Spark): the single-node entry point of the reference's
+"""ResNet-56 / CIFAR-10 on ONE H100 (no Spark): the single-node entry point of the reference's
 ResNet example trio (examples/resnet/resnet_cifar_main.py; flags and schedule from
 resnet_cifar_dist.py:35-66,133-148,196-257).  ``main_fun(argv, ctx)`` is shared with
 ``resnet_cifar_dist.py`` (one process per GPU under torchrun) and ``resnet_cifar_spark.py``.

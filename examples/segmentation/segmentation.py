@@ -1,4 +1,4 @@
-"""Image segmentation U-Net on ONE B200, no Spark (reference: examples/segmentation/
+"""Image segmentation U-Net on ONE H100, no Spark (reference: examples/segmentation/
 segmentation.py - the notebook-derived single-node script; model at segmentation_spark.py:67-119):
 frozen MobileNetV2 encoder, four transposed-conv up-blocks, per-pixel softmax cross-entropy, Adam.
 Checkpoints every epoch (the reference's ModelCheckpoint callback) and reports pixel accuracy of

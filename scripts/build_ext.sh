@@ -1,5 +1,5 @@
 #!/bin/sh
-# Compile every CUDA/C++ source under csrc/ for sm_100a into tensorflowonspark_b200/_ext/ (in-tree).
+# Compile every CUDA/C++ source under csrc/ for sm_90a into tensorflowonspark_b200/_ext/ (in-tree).
 # Works on a machine without a GPU: nvcc cross-compiles.
 set -e
 cd "$(dirname "$0")/.."

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Bring a multi-host GPU cluster up or down over SSH - the role the reference gives to its
 vendored ``scripts/spark_ec2.py`` (launch / destroy / login / stop / start / get-master /
-reboot-slaves on EC2 through boto).  There is no cloud API on a B200 pod, so the unit of
+reboot-slaves on EC2 through boto).  There is no cloud API on a GPU machine, so the unit of
 provisioning here is a list of hosts you can ssh to:
 
   scripts/cluster_launch.py --hosts b200-0,b200-1 --spark-home /opt/spark launch
@@ -10,7 +10,7 @@ provisioning here is a list of hosts you can ssh to:
   scripts/cluster_launch.py --hosts b200-0,b200-1 stop | start | destroy
   scripts/cluster_launch.py --hosts ... --dry-run launch            # print the commands only
 
-``launch`` rsyncs this repository to every host, builds the sm_100a extension there, starts a
+``launch`` rsyncs this repository to every host, builds the sm_90a extension there, starts a
 Spark Standalone master on the first host and one worker per GPU on every host (with Spark's GPU
 resource discovery, so TFSparkNode takes its device from ``TaskContext.resources()``).
 ``stop`` / ``start`` stop and restart the daemons; ``destroy`` also removes the deployed copy.

@@ -1,6 +1,6 @@
 """Packaging for tensorflowonspark_b200 (counterpart of the reference's setup.py / setup.cfg).
 
-The CUDA extension is NOT built through setuptools' build_ext: it is compiled in-tree for sm_100a
+The CUDA extension is NOT built through setuptools' build_ext: it is compiled in-tree for sm_90a
 by ``tensorflowonspark_b200/_build.py`` (``python -c "import __graft_entry__ as g; g.build()"`` or
 ``scripts/build_ext.sh``) so that the resulting ``_ext/_tfos_b200_C.so`` sits next to the sources
 and travels with a checkout; ``pip install -e .`` then only registers the packages.
@@ -10,7 +10,7 @@ from setuptools import find_packages, setup
 setup(
     name="tensorflowonspark-b200",
     version="0.2.0",
-    description="B200-native (sm_100a) framework with the capabilities of TensorFlowOnSpark",
+    description="Hopper-native (sm_90a) framework with the capabilities of TensorFlowOnSpark",
     packages=find_packages(include=["tensorflowonspark_b200*", "tensorflowonspark*"]),
     package_data={"tensorflowonspark_b200": ["_ext/*.so"]},
     python_requires=">=3.10",

@@ -1,5 +1,5 @@
 """Import-compatibility alias: ``import tensorflowonspark`` / ``from tensorflowonspark import
-TFCluster, TFNode, ...`` resolve to the B200-native implementation in ``tensorflowonspark_b200``
+TFCluster, TFNode, ...`` resolve to the Hopper-native implementation in ``tensorflowonspark_b200``
 so programs written against yahoo/TensorFlowOnSpark only change the body of their ``map_fun``."""
 import importlib
 import sys

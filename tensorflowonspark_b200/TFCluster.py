@@ -2,9 +2,9 @@
 
 Public surface identical to tensorflowonspark/TFCluster.py (``InputMode``, ``run``, and the
 ``TFCluster`` object with ``train`` / ``inference`` / ``shutdown`` / ``tensorboard_url``); what
-a "node" is differs: each Spark executor hosts one PyTorch rank bound to one B200 (see
+a "node" is differs: each Spark executor hosts one PyTorch rank bound to one H100 (see
 TFSparkNode.py) and the gradient / broadcast / parameter-server traffic runs through the
-sm_100a kernels in csrc/optim_comm.cu instead of TensorFlow's runtime.
+sm_90a kernels in csrc/optim_comm.cu instead of TensorFlow's runtime.
 """
 import logging
 import os
@@ -184,7 +184,7 @@ def run(sc, map_fun, tf_args, num_executors, num_ps, tensorboard=False,
     map_fun: user function ``map_fun(tf_args, ctx)`` run on every node.
     tf_args: argparse namespace / dict / argv list handed to ``map_fun`` (an argv list also
       becomes ``sys.argv`` on the node).
-    num_executors: total number of nodes (= Spark executors = GPUs on one B200 box).
+    num_executors: total number of nodes (= Spark executors = GPUs on one H100 box).
     num_ps: how many of them are parameter servers.
     tensorboard: launch TensorBoard on the first worker.
     input_mode: :class:`InputMode`.

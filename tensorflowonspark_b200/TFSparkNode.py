@@ -50,7 +50,7 @@ class TFNodeContext(object):
     self.working_dir = working_dir
     self.mgr = mgr
     self.tmp_socket = tmp_socket
-    # B200 runtime additions
+    # H100 runtime additions
     self.rank = -1            # rank among master/chief/worker nodes (-1 for ps / evaluator)
     self.world_size = self.num_workers
     self.local_rank = 0
@@ -78,7 +78,7 @@ class TFNodeContext(object):
     """See :func:`TFNode.release_port`."""
     return TFNode.release_port(self)
 
-  # ------------------------------------------------------------- B200 runtime
+  # ------------------------------------------------------------- H100 runtime
   @property
   def device(self):
     """torch device of this node (the assigned GPU is always cuda:0; 'cpu' without one)."""

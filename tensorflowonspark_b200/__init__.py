@@ -1,4 +1,4 @@
-"""tensorflowonspark_b200: a Blackwell-native framework with the capabilities and
+"""tensorflowonspark_b200: a Hopper-native framework with the capabilities and
 public API of yahoo/TensorFlowOnSpark (reference: tensorflowonspark/__init__.py:1-5)."""
 import logging
 

@@ -1,7 +1,7 @@
 """``python -m tensorflowonspark_b200 <command>`` - the operational entry points in one place.
 
   info                      versions, extension status, visible GPUs
-  build                     compile csrc/ for sm_100a into tensorflowonspark_b200/_ext/
+  build                     compile csrc/ for sm_90a into tensorflowonspark_b200/_ext/
   inference ...             the batch-inference application (same options as the reference's JVM
                             ``Inference`` CLI, src/main/scala/.../Inference.scala:30-43)
   stop-streaming HOST PORT  ask a streaming job to stop through its reservation server

@@ -1,9 +1,9 @@
-"""In-tree build and loading of the native sm_100a extension.
+"""In-tree build and loading of the native sm_90a extension.
 
 The extension (`csrc/*.cu`, `csrc/*.cc`, `csrc/binding.cpp`) is compiled with
-``-gencode arch=compute_100a,code=sm_100a`` into
+``-gencode arch=compute_90a,code=sm_90a`` into
 ``tensorflowonspark_b200/_ext/_tfos_b200_C.so``.  The ``.so`` is git-ignored but
-travels to the GPU box with the working tree, so nothing is JIT-compiled there.
+is loaded from the tree as built, so nothing is JIT-compiled at run time.
 
 GPU ops fail loudly when the extension is missing; there is no eager fallback
 for them.  (Host-only helpers - TFRecord codec, the shared-memory ring - have a
@@ -25,7 +25,7 @@ EXT_DIR = os.path.join(PKG_DIR, "_ext")
 
 SOURCES = ["binding.cpp", "igemm.cu", "igemm_wgrad.cu", "elementwise.cu", "bn_bwd.cu", "stem_fused.cu",
            "smallops.cu", "optim_comm.cu", "feed.cc", "tfrecord.cc", "vmm.cc"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--expt-relaxed-constexpr", "--use_fast_math"]
 
 _lock = threading.Lock()

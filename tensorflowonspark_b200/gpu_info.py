@@ -57,7 +57,7 @@ def _inventory():
     pass
   gpus = []
   for line in _smi("--list-gpus").splitlines():
-    # "GPU 0: NVIDIA B200 (UUID: GPU-xxxx)"
+    # "GPU 0: NVIDIA H100 (UUID: GPU-xxxx)"
     if not line.startswith("GPU "):
       continue
     idx = int(line[4:line.index(":")])

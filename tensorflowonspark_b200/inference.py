@@ -1,6 +1,6 @@
 """Batch-inference CLI: TFRecords -> exported model -> JSON, on the executors' GPUs.
 
-The Python/B200 counterpart of the JVM application in the reference
+The Python/H100 counterpart of the JVM application in the reference
 (src/main/scala/com/yahoo/tensorflowonspark/Inference.scala:17-80): same options
 (``--export_dir --input --schema_hint --input_mapping --output_mapping --output --verbose``),
 same flow (``DFUtil.loadTFRecords`` -> ``TFModel.transform`` -> ``write.json``).

@@ -8,7 +8,7 @@ captured once into a CUDA graph.  Parameters live in three flat buffers
 all-reduce and the optimizer are one fused kernel over contiguous ranges
 (parallel/fused_optim.py).
 
-This is the B200-native stand-in for what the reference delegates to Keras /
+This is the Hopper-native stand-in for what the reference delegates to Keras /
 tf.distribute in its example programs (e.g. examples/mnist/keras/mnist_spark.py:
 11-66, examples/resnet/resnet_cifar_dist.py:196-257).
 """
@@ -232,7 +232,7 @@ class BatchNorm(object):
 
   def forward(self, x_raw, y, residual=None, act=1, training=True, fused_stats=True, rev=False):
     """``rev``: walk the rows last-to-first.  The convolution that produced ``x_raw`` wrote its
-    tiles first-to-last, so the END of the tensor is what the 126 MB L2 still holds; the apply
+    tiles first-to-last, so the END of the tensor is what the 50 MB L2 still holds; the apply
     kernel then finishes at the START of ``y``, which is where the next convolution begins."""
     count = x_raw.numel() // self.C
     ops.C().bn_set_row_reverse(bool(rev))

@@ -5,8 +5,8 @@ cross-entropy, SGD lr 1e-3, batch 64.
 Two implementations with identical parameters:
 * :class:`MnistCNN` - a plain ``torch.nn`` module; used on CPU executors (BASELINE config #1:
   "MNIST InputMode.SPARK sync SGD local[2] on CPU") and as the numerical reference;
-* :class:`MnistTrainer` - the native-engine version for B200: direct Cin=1 convolution kernel,
-  tcgen05 GEMMs with fused bias/ReLU for the dense layers, fused softmax-CE, fused
+* :class:`MnistTrainer` - the native-engine version for H100: direct Cin=1 convolution kernel,
+  wgmma GEMMs with fused bias/ReLU for the dense layers, fused softmax-CE, fused
   all-reduce + SGD (parallel/fused_optim.py).
 """
 import torch
@@ -55,7 +55,7 @@ def build_served(state):
 
 
 class MnistTrainer(object):
-  """Native sm_100a MNIST CNN with static buffers (batch B), NHWC bf16 activations."""
+  """Native sm_90a MNIST CNN with static buffers (batch B), NHWC bf16 activations."""
 
   V, VP = 10, 16  # classes, padded to a multiple of 8 for 16-byte rows
 

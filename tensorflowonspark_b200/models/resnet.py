@@ -1,5 +1,5 @@
 """ResNet (v1.5 bottleneck: 50/101/152; basic-block CIFAR variants 20/32/56) on the
-native engine: NHWC bf16 activations, tcgen05 implicit-GEMM convolutions with
+native engine: NHWC bf16 activations, wgmma implicit-GEMM convolutions with
 batch-norm statistics fused into their epilogues, fused BN+ReLU(+residual)
 apply/backward kernels, fused all-reduce + momentum-SGD optimizer.
 
@@ -180,8 +180,8 @@ class ResNetTrainer(object):
       self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, momentum=momentum,
                                   weight_decay=weight_decay, buckets=buckets)
     # opt-in (TFOS_WGRAD_STREAM=1): weight gradients on a side stream, concurrent with the BN
-    # kernels (engine.py).  Measured on B200: 20.13 vs 20.17 ms/step - the two kernel families do
-    # co-reside on the SMs but share the same L2 -> SM fabric ceiling, so nothing is gained.
+    # kernels (engine.py).  Off by default: the two kernel families co-reside on the SMs but
+    # compete for the same L2 -> SM bandwidth.
     self.wg_stream = None
     if tr and dev.type == "cuda" and os.environ.get("TFOS_WGRAD_STREAM", "0") == "1":
       self.wg_stream = torch.cuda.Stream(device=dev)
@@ -194,7 +194,7 @@ class ResNetTrainer(object):
   def _assign_directions(self):
     """L2 hand-over ("serpentine") schedule, TFOS_L2_SERPENTINE=0 disables it.
 
-    Activations are 13 - 411 MB per tensor at batch 256, the L2 holds 126 MB: a kernel that walks
+    Activations are 13 - 411 MB per tensor at batch 256, the L2 holds 50 MB: a kernel that walks
     a tensor front to back leaves its TAIL in L2.  Every memory-bound kernel of the chain
     therefore starts at the end where its predecessor stopped:
       forward   conv (tiles ascending) -> BN apply (rows descending) -> next conv (ascending) ...
@@ -255,7 +255,7 @@ class ResNetTrainer(object):
   # ------------------------------------------------- broadcast fused with use
   def bind_broadcast_root(self, root=0):
     """Prepare the fused startup broadcast: forward plans whose filters are read by TMA
-    straight out of the ROOT rank's weight buffer over NVLink (tile by tile, as the tcgen05
+    straight out of the ROOT rank's weight buffer over NVLink (tile by tile, as the wgmma
     main loop consumes them), while `bcast_pull` fills the local copy on a side stream."""
     comm = self.comm
     flat = ops.C().tensor_from_ptr(comm.peer_ptrs("weights")[root], [self.store.total], "bf16")
@@ -418,7 +418,7 @@ class ResNetTrainer(object):
     (w' = w * gamma / sqrt(var + eps) per output channel, bias = beta - mean * that scale, from
     the fp32 masters and the running statistics), ReLU and the residual add run in the conv
     epilogues (bias / ReLU / accumulate), identity blocks accumulate IN PLACE into their input.
-    The forward pass is then 53 tcgen05 convolutions + 2 pools + the dense head: none of the 53
+    The forward pass is then 53 wgmma convolutions + 2 pools + the dense head: none of the 53
     batch-norm passes (2/3 of the inference-time HBM traffic) remains.  Call again after the
     parameters or running statistics change (``fold_batch_norms``)."""
     assert not self.training, "folded inference is built on a training=False trainer"

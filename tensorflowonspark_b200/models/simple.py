@@ -100,7 +100,7 @@ def build_rowsum(state):
 
 def allreduce_mean_grads(module, world_size):
   """Plain torch.distributed gradient averaging (the CPU/gloo plumbing path and the NCCL
-  baseline; the B200 product path is parallel/fused_optim.py)."""
+  baseline; the H100 product path is parallel/fused_optim.py)."""
   import torch.distributed as dist
   if world_size <= 1:
     return

@@ -4,7 +4,7 @@ native engine: frozen MobileNetV2 encoder (128x128x3 input, five skip taps) + fo
 + a final Conv2DTranspose to the class logits; Adam, per-pixel sparse cross-entropy.
 
 Kernel mapping:
-  encoder   1x1 expand / project convs -> tcgen05 GEMM with folded inference-BN bias and fused
+  encoder   1x1 expand / project convs -> wgmma GEMM with folded inference-BN bias and fused
             ReLU6; 3x3 depthwise -> depthwise3x3 kernel (bias + ReLU6 fused); stem 3x3/s2 ->
             implicit GEMM.  Forward only (``layer.trainable = False`` in the reference, :83).
   decoder   Conv2DTranspose forward = the stride-2 *data-gradient* implicit GEMM (four output

@@ -1,5 +1,5 @@
-"""Native sm_100a ops.  ``ops.C()`` is the loaded extension module (csrc/binding.cpp);
-``ops.igemm`` builds tcgen05 implicit-GEMM plans; everything else is a thin call
+"""Native sm_90a ops.  ``ops.C()`` is the loaded extension module (csrc/binding.cpp);
+``ops.igemm`` builds wgmma implicit-GEMM plans; everything else is a thin call
 into a fused elementwise / reduction / collective kernel.
 
 No op here falls back to eager PyTorch: if the extension is missing the call

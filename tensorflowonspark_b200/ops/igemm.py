@@ -1,4 +1,4 @@
-"""Plans for the tcgen05 implicit-GEMM kernels (csrc/igemm.cu).
+"""Plans for the wgmma implicit-GEMM kernels (csrc/igemm.cu, csrc/igemm_wgrad.cu).
 
 A *plan* binds fixed device buffers to one kernel launch: two TMA tensor maps
 plus the tile/tap tables.  Layers build their plans once (buffers are static,
@@ -26,7 +26,8 @@ _WGRAD_WORK = int(os.environ.get("TFOS_WGRAD_WORK", "0"))  # 0: per-layer heuris
 _STEM_HALO = os.environ.get("TFOS_STEM_HALO", "1") == "1"
 _WGRAD_HALO = os.environ.get("TFOS_WGRAD_HALO", "1") == "1"
 _WGRAD_HALO_MIN_PIXELS = int(os.environ.get("TFOS_WGRAD_HALO_MIN_PIXELS", "16384"))
-_STEM_SPLITS = int(os.environ.get("TFOS_STEM_SPLITS", "148"))
+_SMS = 132   # H100 SXM; the split-K work-item counts below are multiples of it
+_STEM_SPLITS = int(os.environ.get("TFOS_STEM_SPLITS", str(_SMS)))
 
 
 def launch_count():
@@ -284,17 +285,10 @@ def _wgrad_plan(dy, dy_whn, Cout, x, x_whn, Cin, dw, ldw, taps, mul, es, box=Non
                 tap_dc=None, tap_out=None, n_valid=None):
   OW, OH, N = dy_whn
   n_valid = Cin if n_valid is None else n_valid
-  # 256 x 256 tile per CTA (igemm_wgrad_wide_kernel): half the L2 -> SM bytes per MAC; needs
-  # 64-pixel stages, so it only pays when both channel counts fill the tile
-  # (measured, tools/bench_igemm.py: 14x14 layers -15...25 %; 7x7 layers lose to box padding)
+  # 128 x 256 tile per CTA (wgmma N = 256): fewer operand bytes per MAC than 128 x 128; it only
+  # pays when both channel counts fill the tile and there are enough pixels to split over
   wide = (_WGRAD_WIDE and Cout % 256 == 0 and n_valid % 256 == 0 and es == 1 and c_box_b is None
           and OW * OH * N >= _WGRAD_WIDE_MIN_PIXELS)
-  if wide:
-    if box is None:
-      box = choose_box(OW, OH, N, multiple_of=16, allow_pad=True, max_rows=64, min_rows=64)
-    elif box[0] * box[1] * box[2] > 64:   # caller's 128-row GEMM box: halve it
-      assert box[1] == 1 and box[2] == 1
-      box = (64, 1, 1, -(-OW // 64), 1, 1)
   if box is None:
     box = choose_box(OW, OH, N, multiple_of=16, allow_pad=True)
   bw, bh, bnn, tw, th, tn = box
@@ -308,20 +302,20 @@ def _wgrad_plan(dy, dy_whn, Cout, x, x_whn, Cin, dw, ldw, taps, mul, es, box=Non
   else:
     tb = _tmap4(x, x_whn, Cin, (bw * es, bh * es, bnn), es=(es, es, 1))
   m_tiles, n_tiles = -(-Cout // 128), -(-n_valid // bn)
-  out_tiles = len(taps) * (-(-m_tiles // 2) if wide else m_tiles) * n_tiles
+  out_tiles = len(taps) * m_tiles * n_tiles
   total_boxes = tw * th * tn
   # split-K work items (measured, tools/bench_igemm.py --kind wgrad): the HBM-bound 1x1 layers
   # with many pixels want one wave (fewer fp32 atomics), everything else two to four
   work = _WGRAD_WORK
   if work == 0 and wide:
-    # 256 KB of fp32 atomics per work item and no epilogue overlap: one wave for the memory
-    # bound 1x1 layers, two for the 3x3 ones
-    work = 148 if len(taps) == 1 else 296
+    # 128 KB of fp32 atomics per work item: one wave for the memory bound 1x1 layers, two for the
+    # 3x3 ones
+    work = _SMS if len(taps) == 1 else 2 * _SMS
   if work == 0:
     if len(taps) == 1:
-      work = 148 if total_boxes >= 1024 else 592
+      work = _SMS if total_boxes >= 1024 else 4 * _SMS
     else:
-      work = 592 if Cout <= 64 else 296
+      work = 4 * _SMS if Cout <= 64 else 2 * _SMS
   k_splits = max(1, min(-(-work // out_tiles), max(1, total_boxes // 2)))
   g = {
       "tiles_w": tw, "tiles_h": th, "tiles_n": tn, "box_w": bw, "box_h": bh, "box_n": bnn,
@@ -330,7 +324,7 @@ def _wgrad_plan(dy, dy_whn, Cout, x, x_whn, Cin, dw, ldw, taps, mul, es, box=Non
       "tap_dc": tap_dc if tap_dc is not None else [0] * len(taps),
       "tap_out": tap_out if tap_out is not None else [t[2] for t in taps],
       "m_tiles": m_tiles, "n_tiles": n_tiles, "k_splits": k_splits,
-      "m_valid": Cout, "n_valid": n_valid, "ldw": ldw, "dw": dw.data_ptr(), "wide": int(wide),
+      "m_valid": Cout, "n_valid": n_valid, "ldw": ldw, "dw": dw.data_ptr(),
   }
   h = _C().igemm_plan_wgrad(ta, tb, g, bn)
   return Plan([h], (dy, x, dw), "wgrad{} {}->{} taps{} splits{}".format(
@@ -462,7 +456,7 @@ def stem_wgrad(dy, xp, dw):
   _, H, Wp, _ = xp.shape
   if Cout <= 64 and _STEM_HALO:
     # all seven filter rows from one 16 x 21 halo box per 16 x 8 output pixels
-    # (csrc/igemm_wgrad.cu igemm_wgrad_stem_kernel)
+    # (csrc/igemm_wgrad.cu igemm_wgrad_halo_kernel)
     ta = _tmap4(dy, (OW, OH, N), Cout, (16, 8, 1))
     tb = _stem_halo_tmap(xp, N, H, Wp, OW, 16, 2 * 8 + 5)
     tw, th = -(-OW // 16), -(-OH // 8)
@@ -481,7 +475,7 @@ def stem_wgrad(dy, xp, dw):
   ta = _tmap4(dy, (OW, OH, N), Cout, (bw, bh, bnn))
   tb = _stem_tmap(xp, N, H, Wp, OW, (bw, bh, bnn), 2)
   out_tiles = 7
-  k_splits = max(1, min(-(-296 // out_tiles), max(1, tw * th * tn // 2)))
+  k_splits = max(1, min(-(-2 * _SMS // out_tiles), max(1, tw * th * tn // 2)))
   g = {
       "tiles_w": tw, "tiles_h": th, "tiles_n": tn, "box_w": bw, "box_h": bh, "box_n": bnn,
       "mul_w": 1, "mul_h": 2, "num_taps": 7,

@@ -66,7 +66,7 @@ class FusedOptimizer(object):
     import os
     env_grid = int(os.environ.get("TFOS_AR_GRID", "0"))   # CTAs of the fused kernel (experiments)
     grid = grid or env_grid or None
-    self.grid = grid or (148 if self.world == 1 else 64)
+    self.grid = grid or (132 if self.world == 1 else 64)
     n = store.total
     if not buckets:
       buckets = [(0, n, None)]

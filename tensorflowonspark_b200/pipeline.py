@@ -97,7 +97,7 @@ HasOutputMapping = _make_mixin("HasOutputMapping", [
      _NO_DEFAULT)])
 HasProtocol = _make_mixin("HasProtocol", [
     ("protocol", "Protocol", "Interconnect for the collectives (grpc|rdma accepted for "
-     "compatibility; NVLink peer access is always used on B200)", _S, "grpc")])
+     "compatibility; NVLink peer access is always used on H100)", _S, "grpc")])
 HasReaders = _make_mixin("HasReaders", [
     ("readers", "Readers", "number of reader/enqueue threads", _I, 1)])
 HasSteps = _make_mixin("HasSteps", [
@@ -234,7 +234,7 @@ class TFEstimator(Estimator, TFParams, HasInputMapping, HasClusterSize, HasNumPS
 class TFModel(Model, TFParams, HasInputMapping, HasOutputMapping, HasBatchSize, HasModelDir,
               HasExportDir, HasSignatureDefKey, HasTagSet):
   """Spark ML Model running an exported model over a DataFrame, one independent replica per
-  executor (one per GPU on a B200 box), batches of ``batch_size`` rows."""
+  executor (one per GPU on an H100 box), batches of ``batch_size`` rows."""
 
   def __init__(self, tf_args):
     super(TFModel, self).__init__()

@@ -7,7 +7,7 @@ with two deliberate differences:
 
 * frames are ``>I`` length + **msgpack** (pickle of bytes received from the network is
   not deserialised here);
-* a tiny key/value board (``PUT`` / ``GET``) rides on the same connection.  The B200
+* a tiny key/value board (``PUT`` / ``GET``) rides on the same connection.  The H100
   runtime uses it to exchange CUDA IPC memory handles for the symmetric buffers of the
   fused collectives (parallel/symm.py) - the reference only ever exchanged host:port.
 """

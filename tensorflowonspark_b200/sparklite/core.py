@@ -4,9 +4,9 @@ The reference needs Apache Spark only as a process launcher and partition
 feeder (SURVEY.md section 1, layer L0) and explicitly requires executors that are
 *separate long-lived processes* (reference tests/README.md:10: Spark local mode
 is unsupported because TFoS needs one python worker per executor).  pyspark and
-a JVM are not installed on the B200 image, so this module provides that
+a JVM are not installed on the H100 image, so this module provides that
 substrate: ``SparkContext('local[N]')`` forks N persistent executor processes
-(one per GPU on an 8xB200 box), each with its own working directory, running
+(one per GPU on an 8xH100 box), each with its own working directory, running
 one task at a time, with python-worker reuse semantics.
 
 Only the pyspark surface that TensorFlowOnSpark touches is implemented (see the

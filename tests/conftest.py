@@ -6,7 +6,7 @@ Tiers (mirrors the reference's strategy, SURVEY.md section 4):
     (gloo where a collective is needed) - the stand-in for the reference's 2-worker
     Spark Standalone cluster;
   * ``@pytest.mark.gpu`` - native-kernel numerics vs plain PyTorch fp32 and end-to-end
-    training on a real B200 (run by the driver with ``-m gpu``).
+    training on a real H100 (``pytest -m gpu``).
 """
 import os
 import sys
@@ -20,7 +20,7 @@ import torch  # noqa: E402,F401  (imported before executors fork so they inherit
 
 
 def pytest_configure(config):
-  config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+  config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100 box)")
 
 
 def pytest_collection_modifyitems(config, items):

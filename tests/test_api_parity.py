@@ -1,65 +1,59 @@
 """Every public module / function / class / method / constant of the reference python package
 exists here under the same name, and reference argument names can be used as keywords.
-(Parsed with ``ast`` - the reference is never imported; skipped when the checkout is absent.)"""
-import ast
+(The reference's public surface - names and positional argument lists, parsed from its sources
+with ``ast`` - is stored in tests/golden/reference_api.json; the reference is never imported.)"""
 import importlib
 import inspect
+import json
 import os
 
 import pytest
 
-REF = "/root/reference/tensorflowonspark"
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_api.json")
 
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not mounted")
-
-
-def _modules():
-  return sorted(f[:-3] for f in os.listdir(REF) if f.endswith(".py") and f != "__init__.py")
+with open(GOLDEN) as _f:
+  REF_API = json.load(_f)
 
 
-@pytest.mark.parametrize("mod", _modules() if os.path.isdir(REF) else [])
+@pytest.mark.parametrize("mod", sorted(REF_API))
 def test_public_surface(mod):
-  tree = ast.parse(open(os.path.join(REF, mod + ".py")).read())
+  ref = REF_API[mod]
   m = importlib.import_module("tensorflowonspark_b200." + mod)
   alias = importlib.import_module("tensorflowonspark." + mod)   # reference-style import path
   assert alias is m or alias.__dict__.keys() >= {k for k in m.__dict__ if not k.startswith("_")}
   missing, renamed = [], []
 
-  def check_sig(owner, node, label):
-    obj = getattr(owner, node.name)
+  def check_sig(owner, name, want, label):
+    obj = getattr(owner, name)
     try:
       sig = inspect.signature(obj)
     except (TypeError, ValueError):
       return
     mine = [p.name for p in sig.parameters.values()
             if p.kind in (p.POSITIONAL_ONLY, p.POSITIONAL_OR_KEYWORD)]
-    want = [a.arg for a in node.args.args]
     if inspect.isclass(owner) and want[:1] in (["self"], ["cls"]) and mine[:1] not in (["self"], ["cls"]):
       want = want[1:]
     if mine[:len(want)] != want:
       renamed.append((label, want, mine))
 
-  for node in tree.body:
-    if isinstance(node, ast.Assign):
-      for t in node.targets:
-        if isinstance(t, ast.Name) and t.id.isupper() and not hasattr(m, t.id):
-          missing.append(t.id)
-    if isinstance(node, ast.FunctionDef) and not node.name.startswith("_"):
-      if not hasattr(m, node.name):
-        missing.append(node.name)
+  for const in ref["constants"]:
+    if not hasattr(m, const):
+      missing.append(const)
+  for name, args in sorted(ref["functions"].items()):
+    if not hasattr(m, name):
+      missing.append(name)
+    else:
+      check_sig(m, name, args, name)
+  for cname, methods in sorted(ref["classes"].items()):
+    if not hasattr(m, cname):
+      missing.append(cname)
+      continue
+    cls = getattr(m, cname)
+    for name, args in sorted(methods.items()):
+      if not hasattr(cls, name):
+        missing.append(cname + "." + name)
       else:
-        check_sig(m, node, node.name)
-    if isinstance(node, ast.ClassDef) and not node.name.startswith("_"):
-      if not hasattr(m, node.name):
-        missing.append(node.name)
-        continue
-      cls = getattr(m, node.name)
-      for sub in node.body:
-        if isinstance(sub, ast.FunctionDef) and (not sub.name.startswith("_") or sub.name == "__init__"):
-          if not hasattr(cls, sub.name):
-            missing.append(node.name + "." + sub.name)
-          else:
-            check_sig(cls, sub, node.name + "." + sub.name)
+        check_sig(cls, name, args, cname + "." + name)
   assert not missing, "missing from tensorflowonspark_b200.{}: {}".format(mod, missing)
   assert not renamed, "argument names differ in {}: {}".format(mod, renamed)
 

@@ -1,6 +1,6 @@
 """Driver logic of the GPU-only example programs, dry-run on CPU.
 
-examples/resnet/{resnet_spark,resnet_cifar_main}.py can only train on a B200, but everything
+examples/resnet/{resnet_spark,resnet_cifar_main}.py can only train on an H100, but everything
 around the trainer - flag parsing, communicator selection and initial broadcast, resume from
 ``model_dir``, LR schedule, periodic checkpoints, JSONL metrics and TensorBoard events - is plain
 Python.  Here the native trainers are replaced by a stand-in with the same surface, so that a typo

@@ -1,5 +1,5 @@
 """GPU tier: whole programs through TFCluster on a real device (1 executor = 1 GPU):
-MNIST via InputMode.SPARK with the native sm_100a trainer -> export -> TFParallel inference, and
+MNIST via InputMode.SPARK with the native sm_90a trainer -> export -> TFParallel inference, and
 the segmentation U-Net fed through DataFeed -> pinned staging -> async H2D."""
 import os
 import re
@@ -29,7 +29,7 @@ def test_mnist_spark_train_export_infer_on_gpu():
   out = _run(["examples/mnist/mnist_spark.py", "--cluster_size", "1", "--images_labels",
               d + "/data/csv/train", "--epochs", "3", "--learning_rate", "0.05", "--export_dir",
               d + "/export", "--model_dir", d + "/model"])
-  assert "native sm_100a trainer" in out          # not the CPU fallback
+  assert "native sm_90a trainer" in out          # not the CPU fallback
   assert os.path.exists(d + "/export/weights.pt")
   out = _run(["examples/mnist/mnist_inference.py", "--cluster_size", "1", "--images_labels",
               d + "/data/tfr/test", "--export_dir", d + "/export", "--output", d + "/pred"])

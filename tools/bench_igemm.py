@@ -1,10 +1,10 @@
-"""Per-layer timing of the tcgen05 implicit-GEMM kernels on ResNet-50 shapes (batch 256).
+"""Per-layer timing of the wgmma implicit-GEMM kernels on ResNet-50 shapes (batch 256).
 
   python tools/bench_igemm.py               # table: time, TFLOP/s, GB/s, fraction of measured peaks
   python tools/bench_igemm.py --only l1c3   # one case, few iterations (for an ncu capture)
 
 CUDA-event timing after warm-up; every case cycles through enough distinct buffers to exceed
-the 126 MB L2.  Peaks come from MEASURED_PEAKS.json when present.
+the 50 MB L2.  Peaks come from MEASURED_PEAKS.json when present.
 """
 import argparse
 import json

@@ -1,7 +1,6 @@
-"""Committed SASS evidence: `cuobjdump -sass` listing of every hot kernel of the shipped extension,
-one file per kernel under profiles/sass/, plus a mnemonic summary (UTC*MMA = tcgen05.mma, `.2CTA`
-= cta_group::2, UTMALDG = TMA, LDTM = tcgen05.ld, UTCBAR = tcgen05.commit, LDGMC = multimem
-ld_reduce, SYNCS = mbarrier, FFMA2 = packed fp32x2; /opt/skills/guides/B200_PROFILING.md).
+"""SASS evidence: `cuobjdump -sass` listing of every hot kernel of the built extension, one file
+per kernel under profiles/sass/, plus a mnemonic summary (HGMMA = wgmma, UTMALDG = TMA,
+WARPGROUP = wgmma fences / waits, LDGMC = multimem ld_reduce, SYNCS = mbarrier).
 
   python tools/dump_sass.py            # needs only the built .so and cuobjdump (no GPU)
 """
@@ -17,13 +16,12 @@ OUT = os.path.join(ROOT, "profiles", "sass")
 
 # (file stem, regex on the demangled name)
 KERNELS = [
-    ("igemm_fwd_256_fprop_stats_2cta", r"igemm_fwd_kernel<256, false, 1, 2>"),
-    ("igemm_fwd_256_fprop_stats_1cta", r"igemm_fwd_kernel<256, false, 1, 1>"),
-    ("igemm_fwd_256_dgrad_accum_bnred_1cta", r"igemm_fwd_kernel<256, true, 10, 1>"),
-    ("igemm_fwd_256_dgrad_bnred_2cta", r"igemm_fwd_kernel<256, true, 8, 2>"),
-    ("igemm_fwd_64_fprop_stats", r"igemm_fwd_kernel<64, false, 1, 1>"),
+    ("igemm_fwd_256_fprop_stats", r"igemm_fwd_kernel<256, false, 1>"),
+    ("igemm_fwd_256_dgrad_accum_bnred", r"igemm_fwd_kernel<256, true, 10>"),
+    ("igemm_fwd_256_dgrad_bnred", r"igemm_fwd_kernel<256, true, 8>"),
+    ("igemm_fwd_64_fprop_stats", r"igemm_fwd_kernel<64, false, 1>"),
     ("igemm_wgrad_128", r"igemm_wgrad_kernel<128>"),
-    ("igemm_wgrad_wide", r"igemm_wgrad_wide_kernel"),
+    ("igemm_wgrad_256", r"igemm_wgrad_kernel<256>"),
     ("igemm_wgrad_halo", r"igemm_wgrad_halo_kernel"),
     ("allreduce_opt_momentum_nvls", r"allreduce_opt_kernel<1, true, 0>"),
     ("allreduce_opt_momentum_p2p", r"allreduce_opt_kernel<1, false, 0>"),
@@ -35,13 +33,12 @@ KERNELS = [
     ("stem_bn_relu_pool_fwd", r"stem_bn_relu_pool_fwd_kernel"),
     ("stem_pool_bn_bwd_reduce", r"stem_pool_bn_bwd_reduce_kernel"),
     ("stem_pool_bn_bwd_apply", r"stem_pool_bn_bwd_apply_kernel"),
-    ("igemm_fwd_256_generic_bias_relu_accumulate", r"igemm_fwd_kernel<256, false, 4, 1>"),
+    ("igemm_fwd_256_generic_bias_relu_accumulate", r"igemm_fwd_kernel<256, false, 4>"),
     ("bn_fwd_apply_finalize", r"bn_fwd_apply_kernel<true>"),
     ("bn_bwd_apply", r"bn_bwd_apply_kernel"),
     ("bn_bwd_reduce", r"bn_bwd_reduce_kernel"),
 ]
-KEY = ("UTCHMMA", "UTMALDG", "LDTM", "UTCBAR", "UTCCP", "LDGMC", "SYNCS", "FFMA2", "HMMA", "RED", "ATOM",
-       "UCGABAR", "ST.E", "STG", "LDG")
+KEY = ("HGMMA", "UTMALDG", "WARPGROUP", "LDGMC", "SYNCS", "HMMA", "RED", "ATOM", "ST.E", "STG", "LDG")
 
 
 def main():

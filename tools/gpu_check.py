@@ -105,7 +105,7 @@ def gemm_wgrad():
   from tensorflowonspark_b200.ops import igemm
   ok = True
   for (M, Co, Ci) in [(1024, 128, 64), (4096, 256, 128), (2000, 1000, 2048), (512, 64, 64),
-                      (4096, 512, 256), (1000, 256, 768)]:  # the last two: wide 256x256 tiles
+                      (4096, 512, 256), (1000, 256, 768)]:  # the last two: wide 128x256 tiles
     dy = torch.randn(M, Co, device="cuda").bfloat16()
     x = torch.randn(M, Ci, device="cuda").bfloat16()
     dw = torch.zeros(Co, Ci, device="cuda")
@@ -222,7 +222,7 @@ def conv_wgrad():
 
 @check
 def wgrad_wide():
-  """The 256 x 256-tile weight-gradient kernel, forced on for small problems too."""
+  """The 128 x 256-tile weight-gradient plans, forced on for small problems too."""
   import torch
   from tensorflowonspark_b200.ops import igemm
   old = igemm._WGRAD_WIDE_MIN_PIXELS
@@ -647,7 +647,7 @@ def _rel_l2(a, b):
 @check
 def resnet50_grad_parity():
   """Whole-network bar (reference: tests/test_pipeline.py:149-172 is end-to-end too): the native
-  ResNet-50 (bf16 activations, tcgen05 convolutions, fused BN) against a torchvision ResNet-50 in
+  ResNet-50 (bf16 activations, wgmma convolutions, fused BN) against a torchvision ResNet-50 in
   fp32 holding the SAME parameters and fed the SAME batch: logits, loss, the gradient of every
   conv / BN / FC parameter and the weights after one momentum-SGD step.  Error metric: relative L2
   per tensor; budgets are stated per tensor class below (bf16 activation rounding accumulates
