@@ -45,8 +45,14 @@ struct FwdCfg {
   static constexpr int kBBytes = BN * 128;
   static constexpr int kStage = kABytes + kBBytes;
   static constexpr int kStages = (BN <= 64) ? 8 : (BN <= 128 ? 6 : 4);
+  static constexpr int kRing = kStages * kStage;
+  // epilogue stage: per consumer warpgroup 64 rows x kOutCols bf16 (BN = 256 drains in two
+  // passes), 16-byte chunks XOR-swizzled by row so that stmatrix and the row reads are conflict free
+  static constexpr int kOutCols = BN < 128 ? BN : 128;
+  static constexpr int kOutWgBytes = 64 * kOutCols * 2;
   static constexpr int kStatBytes = BN * 2 * 4;
-  static constexpr int kSmem = kStages * kStage + kStatBytes + 256;
+  static constexpr int kSmem = kRing + 2 * kOutWgBytes + kStatBytes + 256;
+  static_assert(kSmem <= 232448, "over the sm_90 opt-in shared memory limit");
 };
 // Weight-stationary mode: when all K blocks of a CTA's B (filter) tile fit next to >= 4 A stages,
 // B is loaded once per CTA and only A streams - the per-tile L2 traffic of the small-K layers
@@ -65,28 +71,16 @@ constexpr int kStemStage = kStemBoxW * kStemRows * 128;  // 37888 B, a multiple 
 __device__ __forceinline__ void red_shared_add(float* p, float v) {
   asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(smem_u32(p)), "f"(v) : "memory");
 }
-__device__ __forceinline__ void consumer_sync() {
-  asm volatile("bar.sync 1, 256;" ::: "memory");
+// barrier 1: both consumer warpgroups; 2 + wg: one consumer warpgroup (its epilogue stage)
+__device__ __forceinline__ void consumer_sync() { named_bar_sync(1, 256); }
+__device__ __forceinline__ void warpgroup_sync(int wg) { named_bar_sync(2 + wg, 128); }
+
+__host__ __device__ __forceinline__ bool aligned16(const void* p) {
+  return (reinterpret_cast<uintptr_t>(p) & 15) == 0;
 }
 
-// Per-column partial sums of the 16 rows a warp holds: lanes with the same (lane % 4) own the same
-// column pair; after the butterfly lanes 0..3 hold the warp totals and add them to shared memory.
-__device__ __forceinline__ void warp_col_pair_reduce(float* stat, int col, int lane, float2 s,
-                                                     float2 q) {
-#pragma unroll
-  for (int m = 4; m <= 16; m <<= 1) {
-    s.x += __shfl_xor_sync(0xffffffff, s.x, m);
-    s.y += __shfl_xor_sync(0xffffffff, s.y, m);
-    q.x += __shfl_xor_sync(0xffffffff, q.x, m);
-    q.y += __shfl_xor_sync(0xffffffff, q.y, m);
-  }
-  if (lane < 4) {
-    red_shared_add(stat + col * 2 + 0, s.x);
-    red_shared_add(stat + col * 2 + 1, q.x);
-    red_shared_add(stat + col * 2 + 2, s.y);
-    red_shared_add(stat + col * 2 + 3, q.y);
-  }
-}
+// register split of the 384-thread CTA: 128 x 40 + 256 x 232 <= 64 K
+constexpr uint32_t kProducerRegs = 40, kConsumerRegs = 232;
 
 // EPI selects a compile-time epilogue so the common cases carry no per-element flag tests:
 //   0 plain store, 1 fused BN statistics, 2 read-modify-write accumulate,
@@ -108,8 +102,9 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     return a.reverse ? m_boxes - 1 - mt : mt;
   };
   extern __shared__ __align__(1024) uint8_t smem[];
-  float* stat_smem = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStage);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStage + Cfg::kStatBytes);
+  float* stat_smem = reinterpret_cast<float*>(smem + Cfg::kRing + 2 * Cfg::kOutWgBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kRing + 2 * Cfg::kOutWgBytes +
+                                               Cfg::kStatBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + kMaxStages;
   uint64_t* bfull = bars + 2 * kMaxStages;
@@ -147,6 +142,7 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
   if (warp < 4) {
     // ------------------------------------------------------------ TMA producer
+    setmaxnreg_dec<kProducerRegs>();
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -207,6 +203,7 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 
   // ------------------------------------------------------------------ consumers
+  setmaxnreg_inc<kConsumerRegs>();
   const int wg = (warp >> 2) - 1;   // 0 / 1: rows [64 wg, 64 wg + 64) of the tile
   const int wq = warp & 3;          // warp inside the warpgroup: rows 16 wq .. 16 wq + 15
   const bool wg_leader = (threadIdx.x & 127) == 0;
@@ -216,15 +213,43 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const bool bias_on = kGeneric && a.bias != nullptr;
   const bool relu_on = kGeneric && a.relu != 0;
   constexpr bool red_on = (EPI & kEpiBnRed) != 0;   // fused BN backward reduction (igemm.h)
-  // the two accumulator rows of this thread, inside the tile / pixel box: tile independent
-  int prow[2], iw[2], ih[2], in_[2];
+  // Staged epilogue (bf16 output, whole column tiles, 16-byte aligned rows): the warpgroup packs
+  // its 64 x BN accumulator to bf16 into its shared-memory stage, kOutCols columns per pass, and
+  // drains the stage row-major: thread ct owns the 8-column chunk ct % kChunks of rows
+  // ct / kChunks + kRowStep i.  The per-column statistics are summed in that pass into registers
+  // that live as long as the CTA stays on one n tile.
+  constexpr int kOutCols = Cfg::kOutCols;
+  constexpr int kChunks = kOutCols / 8;
+  constexpr int kRowStep = 128 / kChunks;
+  constexpr int kRowsPer = 64 / kRowStep;
+  constexpr int kPasses = BN / kOutCols;
+  // rows whose read-modify-write operands are in flight together: fewer where both operands are
+  // read next to the second half of a BN = 256 accumulator, to stay within kConsumerRegs
+  constexpr int kRowBatch =
+      BN == 256 && (kGeneric || (EPI & (kEpiAccum | kEpiBnRed)) == (kEpiAccum | kEpiBnRed)) ? 2 : 4;
+  const uint32_t ostage = smem_u32(smem + Cfg::kRing + wg * Cfg::kOutWgBytes);
+  // stmatrix: lanes 8 q .. 8 q + 7 address matrix q = (8-column block + q / 2, row half q % 2)
+  const int sm_row = 16 * wq + (lane & 7) + 8 * ((lane >> 3) & 1);
+  const uint32_t sm_addr = ostage + sm_row * (kOutCols * 2);
+  const int ct = threadIdx.x & 127;
+  const int ochunk = ct % kChunks, orow0 = ct / kChunks;
+  // the stage row r holds chunk c at position c ^ (r & 7); r & 7 == orow0 & 7 for all rows of ct
+  const uint32_t o_addr = ostage + orow0 * (kOutCols * 2) + ((ochunk ^ (orow0 & 7)) << 4);
+  // pixel of each copy-out row inside the box (iw | ih << 8 | in << 16), ~0u past the box
+  uint32_t opix[kRowsPer];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    prow[h] = 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
-    iw[h] = prow[h] % a.box_w;
-    ih[h] = (prow[h] / a.box_w) % a.box_h;
-    in_[h] = prow[h] / (a.box_w * a.box_h);
+  for (int i = 0; i < kRowsPer; ++i) {
+    const int pr = 64 * wg + orow0 + kRowStep * i;
+    opix[i] = pr < rows ? static_cast<uint32_t>(pr % a.box_w) |
+                              static_cast<uint32_t>((pr / a.box_w) % a.box_h) << 8 |
+                              static_cast<uint32_t>(pr / (a.box_w * a.box_h)) << 16
+                        : ~0u;
   }
+  float csum[kPasses][8], csq[kPasses][8];   // column sums of chunk ochunk of each pass
+#pragma unroll
+  for (int p = 0; p < kPasses; ++p)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) csum[p][j] = csq[p][j] = 0.f;
   const int cpair = 2 * (lane & 3);   // first of the two columns of each 8-column block
 
   float acc[kAcc];
@@ -296,82 +321,132 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     mt /= a.tiles_w;
     const int th = mt % a.tiles_h;
     const int tn = mt / a.tiles_h;
-    bool valid[2];
-    long long off[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int w = tw * a.box_w + iw[h], hh = th * a.box_h + ih[h], n = tn * a.box_n + in_[h];
-      valid[h] = prow[h] < rows && w < a.lim_w && hh < a.lim_h && n < a.lim_n;
+    auto pixel_off = [&](int iw, int ih, int in_, long long* off) {   // false: outside the tensor
+      const int w = tw * a.box_w + iw, hh = th * a.box_h + ih, n = tn * a.box_n + in_;
       const long long pix =
           (static_cast<long long>(n) * a.OH + (hh * a.osh + a.ooh)) * a.OW + (w * a.osw + a.oow);
-      off[h] = pix * a.ldo + static_cast<long long>(nt) * BN;
-    }
-    const bool fast = !a.out_fp32 && (nt * BN + BN <= a.n_valid) && (a.ldo & 7) == 0;
-    if (fast) {
+      *off = pix * a.ldo + static_cast<long long>(nt) * BN;
+      return w < a.lim_w && hh < a.lim_h && n < a.lim_n;
+    };
+    // non-generic instances are only launched with whole, aligned bf16 tiles (launch_fwd)
+    const bool staged = !kGeneric || (!a.out_fp32 && nt * BN + BN <= a.n_valid &&
+                                      (a.ldo & 7) == 0 && aligned16(a.out));
+    if (staged) {
       __nv_bfloat16* obase = reinterpret_cast<__nv_bfloat16*>(a.out);
       const bool relu_early = relu_on && !acc_on;
-#pragma unroll 4
-      for (int jb = 0; jb < BN / 8; ++jb) {
-        const int c = jb * 8 + cpair;   // column inside the tile
-        float2 s2 = make_float2(0.f, 0.f), q2 = make_float2(0.f, 0.f);
+      // ReLU6 (MobileNetV2 encoder) as a clamp without a branch; f is never NaN after the fmaxf
+      const float relu_cap = a.relu == 2 ? 6.f : INFINITY;
+      // bias of this thread's first column; formed as an integer because a.bias may be null
+      const float* const bias_p = reinterpret_cast<const float*>(
+          reinterpret_cast<uintptr_t>(a.bias) + sizeof(float) * (nt * BN + cpair));
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float f0 = acc[4 * jb + 2 * h], f1 = acc[4 * jb + 2 * h + 1];
-          if (bias_on) {
-            f0 += __ldg(a.bias + nt * BN + c);
-            f1 += __ldg(a.bias + nt * BN + c + 1);
-          }
-          if (relu_early) {
-            f0 = fmaxf(f0, 0.f);
-            f1 = fmaxf(f1, 0.f);
-            if (a.relu == 2) {  // ReLU6 (MobileNetV2 encoder)
-              f0 = fminf(f0, 6.f);
-              f1 = fminf(f1, 6.f);
+      for (int p = 0; p < kPasses; ++p) {
+        warpgroup_sync(wg);   // the previous drain of the stage is complete
+#pragma unroll
+        for (int jj = 0; jj < kChunks; jj += 2) {
+          uint32_t v[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const int jb = p * kChunks + jj + (q >> 1), h = q & 1;
+            float f0 = acc[4 * jb + 2 * h], f1 = acc[4 * jb + 2 * h + 1];
+            if (bias_on) {   // plain loads: an __ldg may be hoisted above the main loop
+              f0 += bias_p[jb * 8];
+              f1 += bias_p[jb * 8 + 1];
             }
+            if (relu_early) {
+              f0 = fminf(fmaxf(f0, 0.f), relu_cap);
+              f1 = fminf(fmaxf(f1, 0.f), relu_cap);
+            }
+            v[q] = pack_bf16x2(f0, f1);
           }
-          uint32_t val = pack_bf16x2(f0, f1);
-          if (do_stats && valid[h]) {
-            // statistics of the rounded values that are stored; rows outside the tensor add 0
-            const float2 r = unpack_bf16x2(val);
-            s2 = fadd2_rn(s2, r);
-            q2 = ffma2_rn(r, r, q2);
+          const int chunk = jj + (lane >> 4);
+          stmatrix_x4(sm_addr + ((chunk ^ (sm_row & 7)) << 4), v[0], v[1], v[2], v[3]);
+        }
+        warpgroup_sync(wg);   // the stage holds columns [p kOutCols, p kOutCols + kOutCols)
+        const int c = p * kOutCols + ochunk * 8;   // first column of the chunk inside the tile
+#pragma unroll
+        for (int i0 = 0; i0 < kRowsPer; i0 += kRowBatch) {
+        // element offsets of the rows (-1: outside the tensor), then their read-modify-write
+        // operands, so that the load latencies overlap
+        long long eo[kRowBatch];
+        uint4 prev[kRowBatch], xr[kRowBatch];
+        uint32_t pmask[kRowBatch], rmask[kRowBatch];
+#pragma unroll
+        for (int b = 0; b < kRowBatch; ++b) {
+          const uint32_t px = opix[i0 + b];
+          long long o = -1;
+          if (px == ~0u || !pixel_off(px & 0xff, (px >> 8) & 0xff, px >> 16, &o)) o = -1;
+          eo[b] = o < 0 ? -1 : o + c;
+          if (eo[b] < 0) continue;
+          const long long e = eo[b];
+          if (acc_on) {
+            prev[b] = *reinterpret_cast<const uint4*>(obase + e);
+            pmask[b] = a.acc_mask != nullptr ? a.acc_mask[e >> 3] : 0xffu;
           }
-          if (valid[h]) {
-            const long long e = off[h] + c;
-            if (acc_on) {
-              const uint32_t pw = *reinterpret_cast<const uint32_t*>(obase + e);
-              const uint32_t pm = a.acc_mask != nullptr ? (a.acc_mask[e >> 3] >> (e & 7)) : 3u;
-              float2 n2 = unpack_bf16x2(val);
-              const float2 p2 = unpack_bf16x2(pw);
+          if (red_on) {
+            xr[b] = ld_nc_v4(reinterpret_cast<const __nv_bfloat16*>(a.red_x) + e);
+            rmask[b] = a.red_mask != nullptr ? a.red_mask[e >> 3] : 0xffu;
+          }
+        }
+#pragma unroll
+        for (int b = 0; b < kRowBatch; ++b) {
+          const uint4 sv = ld_shared_v4(o_addr + (i0 + b) * kRowStep * (kOutCols * 2));
+          if (eo[b] < 0) continue;
+          uint32_t w[4] = {sv.x, sv.y, sv.z, sv.w};
+          const uint32_t pw[4] = {prev[b].x, prev[b].y, prev[b].z, prev[b].w};
+          const uint32_t xw[4] = {xr[b].x, xr[b].y, xr[b].z, xr[b].w};
+          const uint32_t pmask_i = pmask[b], rmask_i = rmask[b];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            if (do_stats) {   // statistics of the rounded values that are stored
+              const float2 r = unpack_bf16x2(w[k]);
+              csum[p][2 * k] = __fadd_rn(csum[p][2 * k], r.x);
+              csum[p][2 * k + 1] = __fadd_rn(csum[p][2 * k + 1], r.y);
+              csq[p][2 * k] = __fmaf_rn(r.x, r.x, csq[p][2 * k]);
+              csq[p][2 * k + 1] = __fmaf_rn(r.y, r.y, csq[p][2 * k + 1]);
+            }
+            if (acc_on) {   // the rounded product plus the previous value, rounded again
+              const uint32_t pm = pmask_i >> (2 * k);
+              float2 n2 = unpack_bf16x2(w[k]);
+              const float2 p2 = unpack_bf16x2(pw[k]);
               n2.x += (pm & 1u) ? p2.x : 0.f;
               n2.y += (pm & 2u) ? p2.y : 0.f;
               if (relu_on) {
                 n2.x = fmaxf(n2.x, 0.f);
                 n2.y = fmaxf(n2.y, 0.f);
               }
-              val = pack_bf16x2(n2.x, n2.y);
+              w[k] = pack_bf16x2(n2.x, n2.y);
             }
-            *reinterpret_cast<uint32_t*>(obase + e) = val;
-            if (red_on) {   // statistics of the ROUNDED gradient that was just stored
-              const uint32_t mb = a.red_mask != nullptr ? (a.red_mask[e >> 3] >> (e & 7)) : 3u;
-              float2 g2 = unpack_bf16x2(val);
+            if (red_on) {   // statistics of the ROUNDED gradient that is stored
+              const uint32_t mb = rmask_i >> (2 * k);
+              float2 g2 = unpack_bf16x2(w[k]);
               g2.x = (mb & 1u) ? g2.x : 0.f;
               g2.y = (mb & 2u) ? g2.y : 0.f;
-              const float2 x2 = unpack_bf16x2(
-                  *reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(a.red_x) + e));
-              s2 = fadd2_rn(s2, g2);
-              q2 = ffma2_rn(g2, x2, q2);
+              const float2 x2 = unpack_bf16x2(xw[k]);
+              csum[p][2 * k] = __fadd_rn(csum[p][2 * k], g2.x);
+              csum[p][2 * k + 1] = __fadd_rn(csum[p][2 * k + 1], g2.y);
+              csq[p][2 * k] = __fmaf_rn(g2.x, x2.x, csq[p][2 * k]);
+              csq[p][2 * k + 1] = __fmaf_rn(g2.y, x2.y, csq[p][2 * k + 1]);
             }
           }
+          *reinterpret_cast<uint4*>(obase + eo[b]) = make_uint4(w[0], w[1], w[2], w[3]);
         }
-        if (do_stats || red_on) warp_col_pair_reduce(stat_smem, c, lane, s2, q2);
+        }
       }
     } else {
-      // general path: fp32 output, ragged N, or unaligned pitch (dense heads, tails)
-#pragma unroll 4
+      // direct path: fp32 output, ragged N, or unaligned pitch (dense heads, tails)
+      bool valid[2];
+      long long off[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int prow = 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
+        valid[h] = pixel_off(prow % a.box_w, (prow / a.box_w) % a.box_h,
+                             prow / (a.box_w * a.box_h), &off[h]) &&
+                   prow < rows;
+      }
+#pragma unroll
       for (int jb = 0; jb < BN / 8; ++jb) {
         const int c = jb * 8 + cpair;
-        float2 s2 = make_float2(0.f, 0.f), q2 = make_float2(0.f, 0.f);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           float f[2] = {acc[4 * jb + 2 * h], acc[4 * jb + 2 * h + 1]};
@@ -380,7 +455,7 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             const int col = nt * BN + c + j;
             const bool cv = col < a.n_valid;
             const long long e = off[h] + c + j;
-            if (a.bias != nullptr && cv) f[j] += __ldg(a.bias + col);
+            if (a.bias != nullptr && cv) f[j] += a.bias[col];
             if (a.out_fp32) {
               float* o = reinterpret_cast<float*>(a.out);
               if (valid[h]) {
@@ -398,18 +473,28 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               f[j] = __bfloat162float(__float2bfloat16_rn(f[j]));
               if (valid[h] && cv) o[e] = __float2bfloat16_rn(f[j]);
             }
-          }
-          if (do_stats && valid[h]) {
-            s2 = fadd2_rn(s2, make_float2(f[0], f[1]));
-            q2 = ffma2_rn(make_float2(f[0], f[1]), make_float2(f[0], f[1]), q2);
+            if (do_stats && valid[h] && cv) {
+              red_shared_add(stat_smem + (c + j) * 2 + 0, f[j]);
+              red_shared_add(stat_smem + (c + j) * 2 + 1, f[j] * f[j]);
+            }
           }
         }
-        if (do_stats) warp_col_pair_reduce(stat_smem, c, lane, s2, q2);
       }
     }
     // the per-column sums meet in shared memory for as long as the CTA stays on one n tile
     const int next_tile = tile + tstep;
     if ((do_stats || red_on) && (next_tile >= total_tiles || next_tile % a.n_tiles != nt)) {
+#pragma unroll
+      for (int p = 0; p < kPasses; ++p)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int c = p * kOutCols + ochunk * 8 + j;
+          if (csum[p][j] != 0.f || csq[p][j] != 0.f) {
+            red_shared_add(stat_smem + c * 2 + 0, csum[p][j]);
+            red_shared_add(stat_smem + c * 2 + 1, csq[p][j]);
+          }
+          csum[p][j] = csq[p][j] = 0.f;
+        }
       consumer_sync();
       for (int c = threadIdx.x - 128; c < BN; c += kConsumerThreads) {
         const int col = nt * BN + c;
@@ -494,7 +579,8 @@ cudaError_t launch_fwd_epi(const IGemmPlan* p, cudaStream_t s) {
 template <int BN, bool B_MN>
 cudaError_t launch_fwd(const IGemmPlan* p, cudaStream_t s) {
   const FwdArgs& f = p->fa;
-  const bool ragged = f.out_fp32 || (f.ldo & 7) != 0 || (f.n_valid % BN) != 0;
+  const bool ragged = f.out_fp32 || (f.ldo & 7) != 0 || (f.n_valid % BN) != 0 ||
+                      !aligned16(f.out);
   const bool generic = ragged || f.bias != nullptr || f.relu != 0 ||
                        (f.col_sum != nullptr && f.accumulate && f.red_x == nullptr);
   if (generic) return launch_fwd_epi<BN, B_MN, kEpiGeneric>(p, s);
@@ -525,8 +611,10 @@ IGemmPlan* igemm_plan_fwd(const TmapDesc& a, const TmapDesc& b, const FwdArgs& a
     return nullptr;
   }
   if (args.acc_mask != nullptr &&
-      (!args.accumulate || args.out_fp32 || (args.ldo & 7) != 0 || args.n_valid % bn != 0)) {
-    snprintf(err, errlen, "acc_mask needs accumulate, bf16 output and whole column tiles");
+      (!args.accumulate || args.out_fp32 || (args.ldo & 7) != 0 || args.n_valid % bn != 0 ||
+       !aligned16(args.out))) {
+    snprintf(err, errlen,
+             "acc_mask needs accumulate, 16-byte aligned bf16 output and whole column tiles");
     return nullptr;
   }
   if (args.col_sum != nullptr && args.accumulate && args.red_x == nullptr) {
@@ -535,9 +623,11 @@ IGemmPlan* igemm_plan_fwd(const TmapDesc& a, const TmapDesc& b, const FwdArgs& a
   }
   if (args.red_x != nullptr &&
       (!b_mn || args.col_sum == nullptr || args.col_sumsq == nullptr || args.out_fp32 ||
-       (args.ldo & 7) != 0 || args.n_valid % bn != 0 || args.bias != nullptr || args.relu != 0)) {
-    snprintf(err, errlen, "fused BN reduction needs a data-gradient plan with bf16 output, whole "
-                          "column tiles, no bias / ReLU and both accumulators");
+       (args.ldo & 7) != 0 || args.n_valid % bn != 0 || args.bias != nullptr || args.relu != 0 ||
+       !aligned16(args.out) || !aligned16(args.red_x))) {
+    snprintf(err, errlen, "fused BN reduction needs a data-gradient plan with 16-byte aligned bf16 "
+                          "output and input, whole column tiles, no bias / ReLU and both "
+                          "accumulators");
     return nullptr;
   }
   IGemmPlan* p = new (std::nothrow) IGemmPlan();
@@ -566,9 +656,9 @@ IGemmPlan* igemm_plan_fwd(const TmapDesc& a, const TmapDesc& b, const FwdArgs& a
     return e == nullptr || atoi(e) != 0;
   }();
   const int k_iters = args.num_taps * args.k_chunks;
-  const long long ring_bytes = bn == 64    ? FwdCfg<64>::kStages * FwdCfg<64>::kStage
-                               : bn == 128 ? FwdCfg<128>::kStages * FwdCfg<128>::kStage
-                                           : FwdCfg<256>::kStages * FwdCfg<256>::kStage;
+  const long long ring_bytes = bn == 64    ? FwdCfg<64>::kRing
+                               : bn == 128 ? FwdCfg<128>::kRing
+                                           : FwdCfg<256>::kRing;
   const long long b_bytes = static_cast<long long>(k_iters) * bn * 128;
   if (args.stem) {
     if (bn != 64 || b_mn || args.num_taps != 7 || args.k_chunks != 1 || args.n_tiles != 1 ||

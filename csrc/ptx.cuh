@@ -204,6 +204,39 @@ struct Wgmma<256> {
   }
 };
 
+// Warp-specialised register split: the warps of a warpgroup hand registers back to (dec) or take
+// them from (inc) the CTA's pool; N is the new per-thread count, a multiple of 8 in [24, 256].
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+
+// Four 8 x 8 bf16 matrices from the fragments of a warp (register i of lane t: row t / 4, columns
+// 2 (t % 4) + {0, 1} of matrix i) to shared memory; lanes 8 i .. 8 i + 7 give the row addresses of
+// matrix i.  This is the layout of a wgmma accumulator's 8-column block after bf16 packing.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2,
+                                            uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr),
+               "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+               : "memory");
+}
+__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
+  uint4 r;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
+               : "r"(addr)
+               : "memory");
+  return r;
+}
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 // wgmma shared-memory matrix descriptor, SWIZZLE_128B.
 //   bits [0,14)  start address >> 4      bits [16,30) leading byte offset >> 4
 //   bits [32,46) stride byte offset >> 4 bits [62,64) layout type (1 = SWIZZLE_128B)

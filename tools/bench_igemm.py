@@ -4,7 +4,8 @@
   python tools/bench_igemm.py --only l1c3   # one case, few iterations (for an ncu capture)
 
 CUDA-event timing after warm-up; every case cycles through enough distinct buffers to exceed
-the 50 MB L2.  Peaks come from MEASURED_PEAKS.json when present.
+the 50 MB L2.  Peaks come from MEASURED_PEAKS.json when present, else from the H100 SXM data
+sheet (3,350 GB/s HBM3, 989 TFLOP/s dense bf16 at up to 700 W): a ceiling, not a reached rate.
 """
 import argparse
 import json
@@ -34,6 +35,13 @@ CASES = [
     ("l1c3_dgrad", "dgrad", (56, 56, 64, 256, 1, 1)),
     ("l1c1_dgrad", "dgrad", (56, 56, 256, 64, 1, 1)),
     ("l3c2_dgrad", "dgrad", (14, 14, 256, 256, 3, 1)),
+    # the batch-norm backward epilogues of the data gradients: fused reduction (EPI 8), masked
+    # residual accumulate (EPI 2 + acc_mask) and both (EPI 10)
+    ("l1c1_dgrad_red", "dgrad_red", (56, 56, 256, 64, 1, 1)),
+    ("l1c1_dgrad_acc", "dgrad_acc", (56, 56, 256, 64, 1, 1)),
+    ("l1c1_dgrad_accred", "dgrad_accred", (56, 56, 256, 64, 1, 1)),
+    ("l2c1_dgrad_red", "dgrad_red", (28, 28, 512, 128, 1, 1)),
+    ("l1c2_dgrad_red", "dgrad_red", (56, 56, 64, 64, 3, 1)),
     ("l1c2_wgrad", "wgrad", (56, 56, 64, 64, 3, 1)),
     ("l1c3_wgrad", "wgrad", (56, 56, 64, 256, 1, 1)),
     ("l1c1_wgrad", "wgrad", (56, 56, 256, 64, 1, 1)),
@@ -52,7 +60,7 @@ def peaks():
   if os.path.exists(p):
     d = json.load(open(p))
     return d["hbm_gbs"], d["bf16_tflops"], "measured"
-  return 6650.0, 1590.0, "fallback"
+  return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 def build(kind, shape, nbuf, stats=True):
@@ -70,6 +78,15 @@ def build(kind, shape, nbuf, stats=True):
       plans.append(igemm.conv_fprop(x, w, y, s, pad, stats=st))
     elif kind == "dgrad":
       plans.append(igemm.conv_dgrad(y, w, x, s, pad))
+    elif kind.startswith("dgrad_"):
+      acc = "acc" in kind
+      mask = torch.randint(0, 256, (B * H * W * Ci // 8,), device=dev, dtype=torch.uint8)
+      red = None
+      if "red" in kind:
+        red = (torch.randn(B, H, W, Ci, device=dev).bfloat16(), mask,
+               torch.zeros(Ci, device=dev), torch.zeros(Ci, device=dev))
+      plans.append(igemm.conv_dgrad(y, w, x, s, pad, accumulate=acc,
+                                    acc_mask=mask if acc else None, bn_reduce=red))
     else:
       dw = torch.zeros(Co, k, k, Ci, device=dev)
       plans.append(igemm.conv_wgrad(y, x, dw, s, pad))
@@ -83,7 +100,8 @@ def main():
   ap.add_argument("--only", default=None)
   ap.add_argument("--iters", type=int, default=20)
   ap.add_argument("--no-stats", action="store_true")
-  ap.add_argument("--kind", default=None, help="fprop | dgrad | wgrad")
+  ap.add_argument("--kind", default=None,
+                  help="fprop | dgrad | dgrad_red | dgrad_acc | dgrad_accred | wgrad")
   args = ap.parse_args()
   hbm, tf, src = peaks()
   print("peaks ({}): HBM {:.0f} GB/s, bf16 {:.0f} TFLOP/s".format(src, hbm, tf))
