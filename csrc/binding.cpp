@@ -127,6 +127,7 @@ int64_t plan_fwd(const py::dict& a, const py::dict& b, const py::dict& g, int bn
   f.out = reinterpret_cast<void*>(geti<uint64_t>(g, "out", 0));
   f.red_x = reinterpret_cast<const void*>(geti<uint64_t>(g, "red_x", 0));
   f.red_mask = reinterpret_cast<const uint8_t*>(geti<uint64_t>(g, "red_mask", 0));
+  f.epi_prefetch = geti<int>(g, "epi_prefetch", 1);
   TORCH_CHECK(f.out != nullptr && f.ldo > 0 && f.n_valid > 0, "igemm fwd: out/ldo/n_valid");
   char err[512] = {0};
   tfos::IGemmPlan* p =
@@ -193,6 +194,7 @@ py::dict plan_info(int64_t h) {
   d["bn"] = p->bn;
   d["grid"] = p->grid;
   d["total_work"] = p->total_work;
+  if (p->kind == 0) d["epi_prefetch"] = p->fa.epi_prefetch;
   return d;
 }
 

@@ -40,19 +40,59 @@ constexpr int kConsumerThreads = 256;
 constexpr int kBlockM = 128;
 constexpr int kABytes = kBlockM * 128;  // 128 rows x 64 bf16
 
-template <int BN>
+// EPI selects a compile-time epilogue so the common cases carry no per-element flag tests:
+//   0 plain store, 1 fused BN statistics, 2 read-modify-write accumulate,
+//   4 generic (bias / ReLU / ReLU6 / statistics / accumulate decided at run time).
+//   8 (with 0 or 2) fused batch-norm backward reduction over the stored gradient tile.
+//  16 (with 2, 8 or 10, data gradients) the operands the epilogue reads - the previous value,
+//     red_x and the two masks - are prefetched into shared memory (see the consumer code).
+constexpr int kEpiPlain = 0, kEpiStats = 1, kEpiAccum = 2, kEpiGeneric = 4, kEpiBnRed = 8,
+              kEpiPrefetch = 16;
+constexpr int kSmemLimit = 232448;   // sm_90 opt-in shared memory per block
+
+// copy-out geometry of the staged epilogue: a consumer warpgroup drains 64 rows x kOutCols columns
+// per pass; each of its 128 threads owns one 8-column chunk of kRowsPer of those rows
+__host__ __device__ constexpr int fwd_out_cols(int bn) { return bn < 128 ? bn : 128; }
+__host__ __device__ constexpr int fwd_rows_per(int bn) { return fwd_out_cols(bn) / 16; }
+// prefetch buffer: per consumer warpgroup two slots, each holding half of every thread's copy-out
+// rows of one pass - per row and operand 16 bytes of data and the 4-byte word holding its mask byte
+__host__ __device__ constexpr int fwd_pf_ops(int epi) {
+  return (epi & kEpiPrefetch) == 0 ? 0 : ((epi & kEpiAccum) ? 1 : 0) + ((epi & kEpiBnRed) ? 1 : 0);
+}
+// slots per warpgroup = units per pass; 4 or 8 smaller units measured slower (per-unit overhead)
+constexpr int kPfSlots = 2;
+__host__ __device__ constexpr int fwd_pf_slot_bytes(int bn, int epi) {
+  return fwd_rows_per(bn) / kPfSlots * 128 * fwd_pf_ops(epi) * (16 + 4);
+}
+// everything but the ring: two epilogue stages, the column statistics, the barriers, the prefetch
+// buffer
+__host__ __device__ constexpr int fwd_fixed_bytes(int bn, int epi) {
+  return 2 * (64 * fwd_out_cols(bn) * 2) + bn * 2 * 4 + 256 + 2 * kPfSlots * fwd_pf_slot_bytes(bn, epi);
+}
+// ring stages: as many as fit, up to 8 / 6 / 4 for BN = 64 / 128 / 256
+__host__ __device__ constexpr int fwd_stages(int bn, int epi) {
+  return (kSmemLimit - fwd_fixed_bytes(bn, epi)) / (kABytes + bn * 128) <
+                 ((bn <= 64) ? 8 : (bn <= 128 ? 6 : 4))
+             ? (kSmemLimit - fwd_fixed_bytes(bn, epi)) / (kABytes + bn * 128)
+             : ((bn <= 64) ? 8 : (bn <= 128 ? 6 : 4));
+}
+
+template <int BN, int EPI>
 struct FwdCfg {
   static constexpr int kBBytes = BN * 128;
   static constexpr int kStage = kABytes + kBBytes;
-  static constexpr int kStages = (BN <= 64) ? 8 : (BN <= 128 ? 6 : 4);
+  static constexpr int kStages = fwd_stages(BN, EPI);
   static constexpr int kRing = kStages * kStage;
   // epilogue stage: per consumer warpgroup 64 rows x kOutCols bf16 (BN = 256 drains in two
   // passes), 16-byte chunks XOR-swizzled by row so that stmatrix and the row reads are conflict free
-  static constexpr int kOutCols = BN < 128 ? BN : 128;
+  static constexpr int kOutCols = fwd_out_cols(BN);
   static constexpr int kOutWgBytes = 64 * kOutCols * 2;
   static constexpr int kStatBytes = BN * 2 * 4;
-  static constexpr int kSmem = kRing + 2 * kOutWgBytes + kStatBytes + 256;
-  static_assert(kSmem <= 232448, "over the sm_90 opt-in shared memory limit");
+  static constexpr int kPfSlotBytes = fwd_pf_slot_bytes(BN, EPI);
+  static constexpr int kPfOff = kRing + 2 * kOutWgBytes + kStatBytes + 256;
+  static constexpr int kSmem = kRing + fwd_fixed_bytes(BN, EPI);
+  static_assert(kStages >= 2, "the ring needs two stages");
+  static_assert(kSmem <= kSmemLimit, "over the sm_90 opt-in shared memory limit");
 };
 // Weight-stationary mode: when all K blocks of a CTA's B (filter) tile fit next to >= 4 A stages,
 // B is loaded once per CTA and only A streams - the per-tile L2 traffic of the small-K layers
@@ -82,17 +122,11 @@ __host__ __device__ __forceinline__ bool aligned16(const void* p) {
 // register split of the 384-thread CTA: 128 x 40 + 256 x 232 <= 64 K
 constexpr uint32_t kProducerRegs = 40, kConsumerRegs = 232;
 
-// EPI selects a compile-time epilogue so the common cases carry no per-element flag tests:
-//   0 plain store, 1 fused BN statistics, 2 read-modify-write accumulate,
-//   4 generic (bias / ReLU / ReLU6 / statistics / accumulate decided at run time).
-//   8 (with 0 or 2) fused batch-norm backward reduction over the stored gradient tile.
-constexpr int kEpiPlain = 0, kEpiStats = 1, kEpiAccum = 2, kEpiGeneric = 4, kEpiBnRed = 8;
-
 template <int BN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(kThreads, 1)
 igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const FwdArgs a, const int total_tiles) {
-  using Cfg = FwdCfg<BN>;
+  using Cfg = FwdCfg<BN, EPI>;
   constexpr int kAcc = BN / 2;   // fp32 accumulator registers per consumer thread (64 x BN / 128)
   const int tile0 = static_cast<int>(blockIdx.x);
   const int tstep = static_cast<int>(gridDim.x);
@@ -223,10 +257,25 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   constexpr int kRowStep = 128 / kChunks;
   constexpr int kRowsPer = 64 / kRowStep;
   constexpr int kPasses = BN / kOutCols;
+  static_assert(kRowsPer == fwd_rows_per(BN), "copy-out geometry");
+  // Operand prefetch: each thread copies the read-modify-write operands of its own copy-out rows
+  // into shared memory with cp.async - it alone writes and reads them, so no barrier is involved.
+  // A unit is half of the thread's rows of one pass; unit j of every tile goes to slot j % 2, and
+  // a slot is refilled as soon as its unit has been read, with the unit two ahead (during the last
+  // pass: the next tile's first units).  One or two units are in flight at all times: during the
+  // main loop, the stmatrix packing and the other unit's copy-out.
+  constexpr bool kPrefetch = (EPI & kEpiPrefetch) != 0;
+  constexpr int kUnits = kPfSlots * kPasses;
+  constexpr int kPfOps = fwd_pf_ops(EPI);
+  constexpr int kOpX = (EPI & kEpiAccum) ? 1 : 0;   // operand 0: previous value, then red_x
+  constexpr int kUnitRows = kRowsPer / kPfSlots;
   // rows whose read-modify-write operands are in flight together: fewer where both operands are
-  // read next to the second half of a BN = 256 accumulator, to stay within kConsumerRegs
+  // read next to the second half of a BN = 256 accumulator, to stay within kConsumerRegs; with the
+  // prefetch, the rows of one unit (their operands are read from shared memory row by row)
   constexpr int kRowBatch =
-      BN == 256 && (kGeneric || (EPI & (kEpiAccum | kEpiBnRed)) == (kEpiAccum | kEpiBnRed)) ? 2 : 4;
+      kPrefetch ? kUnitRows
+      : BN == 256 && (kGeneric || (EPI & (kEpiAccum | kEpiBnRed)) == (kEpiAccum | kEpiBnRed)) ? 2
+                                                                                              : 4;
   const uint32_t ostage = smem_u32(smem + Cfg::kRing + wg * Cfg::kOutWgBytes);
   // stmatrix: lanes 8 q .. 8 q + 7 address matrix q = (8-column block + q / 2, row half q % 2)
   const int sm_row = 16 * wq + (lane & 7) + 8 * ((lane >> 3) & 1);
@@ -251,6 +300,70 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
     for (int j = 0; j < 8; ++j) csum[p][j] = csq[p][j] = 0.f;
   const int cpair = 2 * (lane & 3);   // first of the two columns of each 8-column block
+  // where a tile's box sits: its first pixel and the offset of its first column.  Computed once
+  // per tile: the divisions are long dependent chains, and the epilogue has two warps per scheduler
+  // to hide them.
+  struct TileOrg {
+    int w0, h0, n0;
+    long long col0;
+  };
+  auto tile_org = [&](int tile) {
+    int mt = box_of(tile);
+    const int tw = mt % a.tiles_w;
+    mt /= a.tiles_w;
+    return TileOrg{tw * a.box_w, (mt % a.tiles_h) * a.box_h, (mt / a.tiles_h) * a.box_n,
+                   static_cast<long long>(tile % a.n_tiles) * BN};
+  };
+  // element offset of pixel (iw, ih, in_) of a tile's box at the tile's first column; false: the
+  // pixel is outside the tensor
+  auto org_pixel_off = [&](const TileOrg& t, int iw, int ih, int in_, long long* off) {
+    const int w = t.w0 + iw, hh = t.h0 + ih, n = t.n0 + in_;
+    const long long pix =
+        (static_cast<long long>(n) * a.OH + (hh * a.osh + a.ooh)) * a.OW + (w * a.osw + a.oow);
+    *off = pix * a.ldo + t.col0;
+    return w < a.lim_w && hh < a.lim_h && n < a.lim_n;
+  };
+  __nv_bfloat16* const obase = reinterpret_cast<__nv_bfloat16*>(a.out);
+  // prefetch slot s of this warpgroup: 16-byte operand vectors [o][b][ct], then the 4-byte words
+  // holding the mask bytes [o][b][ct] (the plan checked that the masks are 4-byte aligned and that
+  // ldo % 32 == 0, so every word lies inside the mask tensor)
+  const uint32_t pf_base = smem_u32(smem + Cfg::kPfOff) + wg * kPfSlots * Cfg::kPfSlotBytes;
+  auto pf_vec = [&](int s, int o, int b) {
+    return pf_base + s * Cfg::kPfSlotBytes + ((o * kUnitRows + b) * 128 + ct) * 16;
+  };
+  auto pf_mask = [&](int s, int o, int b) {
+    return pf_base + s * Cfg::kPfSlotBytes + kPfOps * kUnitRows * 128 * 16 +
+           ((o * kUnitRows + b) * 128 + ct) * 4;
+  };
+  auto mask_word = [](const uint8_t* m, long long e) {
+    return reinterpret_cast<const void*>(m + ((e >> 3) & ~3ll));
+  };
+  // queue unit j of tile t (nothing past the last tile, but always one commit group per unit)
+  auto pf_issue = [&](int t, const TileOrg& org, int j) {
+    if (t < total_tiles) {
+      const int s = j % kPfSlots, c = (j / kPfSlots) * kOutCols + ochunk * 8;
+#pragma unroll
+      for (int b = 0; b < kUnitRows; ++b) {
+        const uint32_t px = opix[s * kUnitRows + b];
+        long long o = -1;
+        if (px == ~0u || !org_pixel_off(org, px & 0xff, (px >> 8) & 0xff, px >> 16, &o)) continue;
+        const long long e = o + c;
+        if (EPI & kEpiAccum) {
+          cp_async_16(pf_vec(s, 0, b), obase + e);
+          if (a.acc_mask != nullptr) cp_async_4(pf_mask(s, 0, b), mask_word(a.acc_mask, e));
+        }
+        if (red_on) {
+          cp_async_16(pf_vec(s, kOpX, b), reinterpret_cast<const __nv_bfloat16*>(a.red_x) + e);
+          if (a.red_mask != nullptr) cp_async_4(pf_mask(s, kOpX, b), mask_word(a.red_mask, e));
+        }
+      }
+    }
+    cp_async_commit();
+  };
+  if (kPrefetch) {
+#pragma unroll
+    for (int j = 0; j < kPfSlots; ++j) pf_issue(tile0, tile_org(tile0), j);
+  }
 
   float acc[kAcc];
 #pragma unroll
@@ -259,6 +372,7 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   int stage = 0;
   uint32_t phase = 0;
   if (resident && tile0 < total_tiles) mbar_wait(bfull, 0);
+  TileOrg org = tile_org(tile0);   // of `tile`; carried over so that each tile computes one
   for (int tile = tile0; tile < total_tiles; tile += tstep) {
     // ------------------------------------------------------------ main loop
     int prev_stage = -1;
@@ -316,23 +430,14 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
     // ------------------------------------------------------------- epilogue
     const int nt = tile % a.n_tiles;
-    int mt = box_of(tile);
-    const int tw = mt % a.tiles_w;
-    mt /= a.tiles_w;
-    const int th = mt % a.tiles_h;
-    const int tn = mt / a.tiles_h;
+    const TileOrg next_org = tile_org(tile + tstep);
     auto pixel_off = [&](int iw, int ih, int in_, long long* off) {   // false: outside the tensor
-      const int w = tw * a.box_w + iw, hh = th * a.box_h + ih, n = tn * a.box_n + in_;
-      const long long pix =
-          (static_cast<long long>(n) * a.OH + (hh * a.osh + a.ooh)) * a.OW + (w * a.osw + a.oow);
-      *off = pix * a.ldo + static_cast<long long>(nt) * BN;
-      return w < a.lim_w && hh < a.lim_h && n < a.lim_n;
+      return org_pixel_off(org, iw, ih, in_, off);
     };
     // non-generic instances are only launched with whole, aligned bf16 tiles (launch_fwd)
     const bool staged = !kGeneric || (!a.out_fp32 && nt * BN + BN <= a.n_valid &&
                                       (a.ldo & 7) == 0 && aligned16(a.out));
     if (staged) {
-      __nv_bfloat16* obase = reinterpret_cast<__nv_bfloat16*>(a.out);
       const bool relu_early = relu_on && !acc_on;
       // ReLU6 (MobileNetV2 encoder) as a clamp without a branch; f is never NaN after the fmaxf
       const float relu_cap = a.relu == 2 ? 6.f : INFINITY;
@@ -371,6 +476,8 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         long long eo[kRowBatch];
         uint4 prev[kRowBatch], xr[kRowBatch];
         uint32_t pmask[kRowBatch], rmask[kRowBatch];
+        const int s = i0 / kRowBatch;   // prefetch: unit 2 p + s, in slot s
+        if (kPrefetch) cp_async_wait<kPfSlots - 1>();   // that unit has landed; later ones may be pending
 #pragma unroll
         for (int b = 0; b < kRowBatch; ++b) {
           const uint32_t px = opix[i0 + b];
@@ -378,6 +485,7 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (px == ~0u || !pixel_off(px & 0xff, (px >> 8) & 0xff, px >> 16, &o)) o = -1;
           eo[b] = o < 0 ? -1 : o + c;
           if (eo[b] < 0) continue;
+          if (kPrefetch) continue;
           const long long e = eo[b];
           if (acc_on) {
             prev[b] = *reinterpret_cast<const uint4*>(obase + e);
@@ -392,6 +500,18 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int b = 0; b < kRowBatch; ++b) {
           const uint4 sv = ld_shared_v4(o_addr + (i0 + b) * kRowStep * (kOutCols * 2));
           if (eo[b] < 0) continue;
+          if (kPrefetch) {
+            // the mask byte of element e sits at byte (e >> 3) & 3 of its word
+            const int msh = static_cast<int>((eo[b] >> 3) & 3) * 8;
+            if (acc_on) {
+              prev[b] = ld_shared_v4(pf_vec(s, 0, b));
+              pmask[b] = a.acc_mask != nullptr ? ld_shared_u32(pf_mask(s, 0, b)) >> msh : 0xffu;
+            }
+            if (red_on) {
+              xr[b] = ld_shared_v4(pf_vec(s, kOpX, b));
+              rmask[b] = a.red_mask != nullptr ? ld_shared_u32(pf_mask(s, kOpX, b)) >> msh : 0xffu;
+            }
+          }
           uint32_t w[4] = {sv.x, sv.y, sv.z, sv.w};
           const uint32_t pw[4] = {prev[b].x, prev[b].y, prev[b].z, prev[b].w};
           const uint32_t xw[4] = {xr[b].x, xr[b].y, xr[b].z, xr[b].w};
@@ -430,6 +550,13 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
           }
           *reinterpret_cast<uint4*>(obase + eo[b]) = make_uint4(w[0], w[1], w[2], w[3]);
+        }
+        if (kPrefetch) {   // refill the slot with the unit two ahead
+          const int j = kPfSlots * p + s + kPfSlots;
+          if (j < kUnits)
+            pf_issue(tile, org, j);
+          else
+            pf_issue(tile + tstep, next_org, j - kUnits);
         }
         }
       }
@@ -507,6 +634,7 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
       consumer_sync();
     }
+    org = next_org;
   }
 }
 
@@ -567,34 +695,65 @@ cudaError_t launch_fwd_epi(const IGemmPlan* p, cudaStream_t s) {
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(igemm_fwd_kernel<BN, B_MN, EPI>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         FwdCfg<BN>::kSmem);
+                                         FwdCfg<BN, EPI>::kSmem);
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  igemm_fwd_kernel<BN, B_MN, EPI><<<p->grid, kThreads, FwdCfg<BN>::kSmem, s>>>(
+  igemm_fwd_kernel<BN, B_MN, EPI><<<p->grid, kThreads, FwdCfg<BN, EPI>::kSmem, s>>>(
       p->tmA, p->tmB, p->fa, p->total_work);
   return cudaGetLastError();
 }
 
-template <int BN, bool B_MN>
-cudaError_t launch_fwd(const IGemmPlan* p, cudaStream_t s) {
-  const FwdArgs& f = p->fa;
-  const bool ragged = f.out_fp32 || (f.ldo & 7) != 0 || (f.n_valid % BN) != 0 ||
+// The epilogue instance (EPI of igemm_fwd_kernel) of a plan; `prefetch` asks for the operand
+// prefetch where the instance has one.
+int fwd_epi(const FwdArgs& f, int bn, bool b_mn, bool prefetch) {
+  const bool ragged = f.out_fp32 || (f.ldo & 7) != 0 || (f.n_valid % bn) != 0 ||
                       !aligned16(f.out);
   const bool generic = ragged || f.bias != nullptr || f.relu != 0 ||
                        (f.col_sum != nullptr && f.accumulate && f.red_x == nullptr);
-  if (generic) return launch_fwd_epi<BN, B_MN, kEpiGeneric>(p, s);
-  if (B_MN) {  // data gradients: plain or accumulate (statistics only through the generic path)
+  if (generic) return kEpiGeneric;
+  if (b_mn) {  // data gradients: plain or accumulate (statistics only through the generic path)
+    int epi;
     if (f.red_x != nullptr)   // fused BN backward reduction (validated in igemm_plan_fwd)
-      return f.accumulate ? launch_fwd_epi<BN, B_MN, kEpiAccum | kEpiBnRed>(p, s)
-                          : launch_fwd_epi<BN, B_MN, kEpiBnRed>(p, s);
-    if (f.col_sum != nullptr) return launch_fwd_epi<BN, B_MN, kEpiGeneric>(p, s);
-    return f.accumulate ? launch_fwd_epi<BN, B_MN, kEpiAccum>(p, s)
-                        : launch_fwd_epi<BN, B_MN, kEpiPlain>(p, s);
+      epi = f.accumulate ? kEpiAccum | kEpiBnRed : kEpiBnRed;
+    else if (f.col_sum != nullptr)
+      return kEpiGeneric;
+    else
+      epi = f.accumulate ? kEpiAccum : kEpiPlain;
+    return prefetch && epi != kEpiPlain ? epi | kEpiPrefetch : epi;
   }
-  if (f.accumulate) return launch_fwd_epi<BN, B_MN, kEpiGeneric>(p, s);
-  return f.col_sum != nullptr ? launch_fwd_epi<BN, B_MN, kEpiStats>(p, s)
-                              : launch_fwd_epi<BN, B_MN, kEpiPlain>(p, s);
+  if (f.accumulate) return kEpiGeneric;
+  return f.col_sum != nullptr ? kEpiStats : kEpiPlain;
+}
+
+template <int BN, bool B_MN>
+cudaError_t launch_fwd(const IGemmPlan* p, cudaStream_t s) {
+  switch (p->epi) {
+    case kEpiPlain: return launch_fwd_epi<BN, B_MN, kEpiPlain>(p, s);
+    case kEpiStats: return launch_fwd_epi<BN, B_MN, kEpiStats>(p, s);
+    case kEpiGeneric: return launch_fwd_epi<BN, B_MN, kEpiGeneric>(p, s);
+    default: break;
+  }
+  if constexpr (B_MN) {
+    switch (p->epi) {
+      case kEpiAccum: return launch_fwd_epi<BN, B_MN, kEpiAccum>(p, s);
+      case kEpiBnRed: return launch_fwd_epi<BN, B_MN, kEpiBnRed>(p, s);
+      case kEpiAccum | kEpiBnRed: return launch_fwd_epi<BN, B_MN, kEpiAccum | kEpiBnRed>(p, s);
+      default: break;
+    }
+  }
+  if constexpr (B_MN && BN >= 128) {   // igemm_plan_fwd: no prefetch at BN = 64
+    switch (p->epi) {
+      case kEpiPrefetch | kEpiAccum:
+        return launch_fwd_epi<BN, B_MN, kEpiPrefetch | kEpiAccum>(p, s);
+      case kEpiPrefetch | kEpiBnRed:
+        return launch_fwd_epi<BN, B_MN, kEpiPrefetch | kEpiBnRed>(p, s);
+      case kEpiPrefetch | kEpiAccum | kEpiBnRed:
+        return launch_fwd_epi<BN, B_MN, kEpiPrefetch | kEpiAccum | kEpiBnRed>(p, s);
+      default: break;
+    }
+  }
+  return cudaErrorInvalidValue;
 }
 
 }  // namespace
@@ -641,6 +800,17 @@ IGemmPlan* igemm_plan_fwd(const TmapDesc& a, const TmapDesc& b, const FwdArgs& a
   p->kind = 0;
   p->bn = bn;
   p->b_mn = b_mn;
+  // the operand prefetch reads each mask byte through the aligned 4-byte word that holds it: that
+  // word stays inside the mask tensor when the tensor is 4-byte aligned and ldo % 32 == 0
+  auto words_inside = [&](const uint8_t* m) {
+    return m == nullptr || ((reinterpret_cast<uintptr_t>(m) & 3) == 0 && args.ldo % 32 == 0);
+  };
+  // At BN = 64 the prefetch buffer costs a ring stage and the copy-out is short: measured slower
+  // (tools/bench_igemm.py l1c2_dgrad_red), so those plans keep the loads in the copy-out pass.
+  const bool prefetch = args.epi_prefetch != 0 && bn >= 128 && words_inside(args.acc_mask) &&
+                        words_inside(args.red_mask);
+  p->epi = fwd_epi(args, bn, b_mn != 0, prefetch);
+  p->fa.epi_prefetch = (p->epi & kEpiPrefetch) != 0;
   p->total_work = args.n_tiles * args.tiles_w * args.tiles_h * args.tiles_n;
   p->grid = p->total_work < num_sms ? p->total_work : num_sms;
   // a grid that is a multiple of n_tiles pins every CTA to one n tile: the fused statistics
@@ -656,9 +826,9 @@ IGemmPlan* igemm_plan_fwd(const TmapDesc& a, const TmapDesc& b, const FwdArgs& a
     return e == nullptr || atoi(e) != 0;
   }();
   const int k_iters = args.num_taps * args.k_chunks;
-  const long long ring_bytes = bn == 64    ? FwdCfg<64>::kRing
-                               : bn == 128 ? FwdCfg<128>::kRing
-                                           : FwdCfg<256>::kRing;
+  // the ring of the instance this plan runs (the prefetch instances have fewer stages)
+  const long long ring_bytes =
+      static_cast<long long>(fwd_stages(bn, p->epi)) * (kABytes + bn * 128);
   const long long b_bytes = static_cast<long long>(k_iters) * bn * 128;
   if (args.stem) {
     if (bn != 64 || b_mn || args.num_taps != 7 || args.k_chunks != 1 || args.n_tiles != 1 ||

@@ -65,6 +65,11 @@ struct FwdArgs {
   // (a full read of dY and x) disappears.
   const void* red_x;
   const uint8_t* red_mask;
+  // data-gradient epilogues that read operands (accumulate, fused BN reduction): 0 reads them from
+  // global memory in the copy-out pass; otherwise igemm_plan_fwd picks the instance that prefetches
+  // them into shared memory while the main loop runs, where the plan allows it (igemm.cu), and
+  // sets this to 1 if it did, 0 if not
+  int epi_prefetch;
 };
 
 // weight-gradient problems: K = pixels, M = Cout, N = Cin (per tap).
@@ -96,6 +101,7 @@ struct IGemmPlan {
   int kind;  // 0 = fwd-like, 1 = wgrad
   int bn;    // 64 / 128 / 256
   int b_mn;  // fwd-like only: B is MN-major ([K rows, N cols])
+  int epi;   // fwd-like only: the epilogue instance (igemm.cu, EPI of igemm_fwd_kernel)
   int grid;
   int total_work;
 };

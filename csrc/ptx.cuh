@@ -232,6 +232,26 @@ __device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
                : "memory");
   return r;
 }
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t r;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(addr) : "memory");
+  return r;
+}
+// cp.async: global -> shared copies that complete in the background; a thread sees its own copies
+// after cp_async_wait<N> (at most N of its most recent commit groups still pending)
+__device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_4(uint32_t dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() {
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
 // named barrier over `count` threads (id 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");

@@ -28,6 +28,10 @@ _WGRAD_HALO = os.environ.get("TFOS_WGRAD_HALO", "1") == "1"
 _WGRAD_HALO_MIN_PIXELS = int(os.environ.get("TFOS_WGRAD_HALO_MIN_PIXELS", "16384"))
 _SMS = 132   # H100 SXM; the split-K work-item counts below are multiples of it
 _STEM_SPLITS = int(os.environ.get("TFOS_STEM_SPLITS", str(_SMS)))
+# data gradients with an accumulate / fused-BN-reduction epilogue prefetch the operands that
+# epilogue reads into shared memory during the main loop (csrc/igemm.cu); 0 reads them in the
+# copy-out pass instead
+_DGRAD_EPI_PREFETCH = os.environ.get("TFOS_DGRAD_EPI_PREFETCH", "1") == "1"
 
 
 def launch_count():
@@ -170,6 +174,7 @@ def gemm(a, b, out, b_layout="nk", bias=None, relu=False, accumulate=False, stat
       "ldo": out.shape[1], "n_valid": N, "relu": int(relu),
       "out_fp32": int(out.dtype == torch.float32), "accumulate": int(accumulate),
       "bias": bias.data_ptr() if bias is not None else 0, "out": out.data_ptr(),
+      "epi_prefetch": int(_DGRAD_EPI_PREFETCH),   # 'kn' + accumulate: see conv_dgrad
   }
   _stats_args(g, stats)
   h = _C().igemm_plan_fwd(ta, tb, g, bn, b_layout == "kn")
@@ -221,7 +226,7 @@ def conv_fprop(x, w, y, stride=1, pad=0, bias=None, relu=False, stats=None, accu
 
 
 def conv_dgrad(dy, w, dx, stride=1, pad=0, accumulate=False, relu=False, bias=None, stats=None,
-               acc_mask=None, bn_reduce=None):
+               acc_mask=None, bn_reduce=None, epi_prefetch=None):
   """dx[N,H,W,Cin] (=|+=) conv_transpose(dy[N,OH,OW,Cout], w[Cout,R,S,Cin]).
 
   Also the forward of a transposed convolution (Keras Conv2DTranspose) when
@@ -233,7 +238,14 @@ def conv_dgrad(dy, w, dx, stride=1, pad=0, accumulate=False, relu=False, bias=No
   norm whose input was ``x_raw`` (shape of dx); the epilogue accumulates the two per-channel sums
   of that batch norm's backward reduction while it stores dx (csrc/igemm.h: red_x).  Requires
   that this call writes EVERY pixel of dx (raises ValueError otherwise: a strided 1x1 does not).
+
+  ``epi_prefetch``: whether the accumulate / ``bn_reduce`` epilogue prefetches the values it reads
+  into shared memory while the main loop runs (False: it loads them in the copy-out pass).  Both
+  give the same dx bit for bit.  None: on unless TFOS_DGRAD_EPI_PREFETCH=0.  The plan falls back
+  to the loads in the copy-out pass where it cannot prefetch (``Plan.info()``: ``epi_prefetch``).
   """
+  if epi_prefetch is None:
+    epi_prefetch = _DGRAD_EPI_PREFETCH
   N, OH, OW, Cout = dy.shape
   _, R, S, Cin = w.shape
   _, H, W, _ = dx.shape
@@ -267,6 +279,7 @@ def conv_dgrad(dy, w, dx, stride=1, pad=0, accumulate=False, relu=False, bias=No
         "ldo": Cin, "n_valid": Cin, "accumulate": int(accumulate), "relu": int(relu),
         "acc_mask": acc_mask.data_ptr() if acc_mask is not None else 0,
         "bias": bias.data_ptr() if bias is not None else 0, "out": dx.data_ptr(),
+        "epi_prefetch": int(bool(epi_prefetch)),
     }
     _stats_args(g, stats)  # transposed-conv *forward* feeding a batch norm
     if bn_reduce is not None:

@@ -41,7 +41,13 @@ CASES = [
     ("l1c1_dgrad_acc", "dgrad_acc", (56, 56, 256, 64, 1, 1)),
     ("l1c1_dgrad_accred", "dgrad_accred", (56, 56, 256, 64, 1, 1)),
     ("l2c1_dgrad_red", "dgrad_red", (28, 28, 512, 128, 1, 1)),
+    ("l2c1_dgrad_accred", "dgrad_accred", (28, 28, 512, 128, 1, 1)),
+    ("l3c1_dgrad_accred", "dgrad_accred", (14, 14, 1024, 256, 1, 1)),
+    ("l4c1_dgrad_accred", "dgrad_accred", (7, 7, 2048, 512, 1, 1)),
     ("l1c2_dgrad_red", "dgrad_red", (56, 56, 64, 64, 3, 1)),
+    ("l3c2_dgrad_red", "dgrad_red", (14, 14, 256, 256, 3, 1)),
+    ("l3c3_dgrad_red", "dgrad_red", (14, 14, 256, 1024, 1, 1)),
+    ("l4c3_dgrad_red", "dgrad_red", (7, 7, 512, 2048, 1, 1)),
     ("l1c2_wgrad", "wgrad", (56, 56, 64, 64, 3, 1)),
     ("l1c3_wgrad", "wgrad", (56, 56, 64, 256, 1, 1)),
     ("l1c1_wgrad", "wgrad", (56, 56, 256, 64, 1, 1)),
@@ -63,7 +69,7 @@ def peaks():
   return 3350.0, 989.0, "H100 SXM data sheet"
 
 
-def build(kind, shape, nbuf, stats=True):
+def build(kind, shape, nbuf, stats=True, epi_prefetch=None):
   H, W, Ci, Co, k, s = shape
   pad = k // 2
   OH, OW = (H + 2 * pad - k) // s + 1, (W + 2 * pad - k) // s + 1
@@ -86,12 +92,16 @@ def build(kind, shape, nbuf, stats=True):
         red = (torch.randn(B, H, W, Ci, device=dev).bfloat16(), mask,
                torch.zeros(Ci, device=dev), torch.zeros(Ci, device=dev))
       plans.append(igemm.conv_dgrad(y, w, x, s, pad, accumulate=acc,
-                                    acc_mask=mask if acc else None, bn_reduce=red))
+                                    acc_mask=mask if acc else None, bn_reduce=red,
+                                    epi_prefetch=epi_prefetch))
     else:
       dw = torch.zeros(Co, k, k, Ci, device=dev)
       plans.append(igemm.conv_wgrad(y, x, dw, s, pad))
   flops = 2.0 * B * OH * OW * Co * Ci * k * k
   byts = 2.0 * B * (H * W * Ci + OH * OW * Co) + 2.0 * Co * Ci * k * k
+  # the epilogue's reads: the previous dx (accumulate) and red_x, each with its bit mask
+  byts += ("acc" in kind) * B * H * W * Ci * (2 + 1 / 8.0)
+  byts += ("red" in kind) * B * H * W * Ci * (2 + 1 / 8.0)
   return plans, flops, byts
 
 
@@ -100,6 +110,8 @@ def main():
   ap.add_argument("--only", default=None)
   ap.add_argument("--iters", type=int, default=20)
   ap.add_argument("--no-stats", action="store_true")
+  ap.add_argument("--epi-prefetch", type=int, choices=(0, 1), default=None,
+                  help="dgrad_* kinds: prefetch the epilogue operands (default: the plan's choice)")
   ap.add_argument("--kind", default=None,
                   help="fprop | dgrad | dgrad_red | dgrad_acc | dgrad_accred | wgrad")
   args = ap.parse_args()
@@ -113,7 +125,8 @@ def main():
     H, W, Ci, Co, k, s = shape
     per = 2.0 * B * (H * W * Ci + H * W * Co)
     nbuf = 1 if args.only else max(2, int(400e6 // per) + 1)
-    plans, flops, byts = build(kind, shape, nbuf, not args.no_stats)
+    plans, flops, byts = build(kind, shape, nbuf, not args.no_stats,
+                               None if args.epi_prefetch is None else bool(args.epi_prefetch))
     iters = 3 if args.only else args.iters
     for p in plans[:2]:
       p.run()
