@@ -164,8 +164,8 @@ int64_t plan_wgrad(const py::dict& a, const py::dict& b, const py::dict& g, int 
   w.halo_rows = geti<int>(g, "halo_rows", 21);
   w.halo_hmul = geti<int>(g, "halo_hmul", 2);
   w.halo_h0 = geti<int>(g, "halo_h0", 0);
-  w.halo_jmul = geti<int>(g, "halo_jmul", 2);
   w.halo_rowbytes = geti<int>(g, "halo_rowbytes", 2048);
+  fill_ints(g, "halo_jrow", w.halo_jrow, 8);
   w.halo_nacc = geti<int>(g, "halo_nacc", 7);
   fill_ints(g, "acc_box", w.acc_box, tfos::kMaxTaps);
   fill_ints(g, "acc_row", w.acc_row, tfos::kMaxTaps);

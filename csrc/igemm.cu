@@ -875,19 +875,28 @@ IGemmPlan* igemm_plan_wgrad(const TmapDesc& a, const TmapDesc& b, const WgradArg
   p->bn = bn;
   p->total_work = args.num_taps * args.m_tiles * args.n_tiles * args.k_splits;
   if (args.stem) {  // igemm_wgrad_halo_kernel: several taps per pass over the pixels
-    const long long b_box = static_cast<long long>(args.box_w) * args.halo_rows * 128;
+    const long long b_box = static_cast<long long>(args.box_w) * args.halo_rows * args.box_n * 128;
     const long long stage = 128 * 128 + args.halo_boxes * b_box;
-    const bool geo_ok = (args.box_w == 16 && args.box_h == 8) || (args.box_w == 8 && args.box_h == 16);
-    if (bn != 64 || !geo_ok || args.box_n != 1 || args.m_valid > 64 || args.m_tiles != 1 ||
-        args.n_tiles != 1 || args.halo_nacc < 1 || args.halo_nacc > 8 || args.halo_boxes < 1 ||
-        args.halo_boxes > 3 || stage % 1024 != 0 || stage * 2 > 216 * 1024 ||
-        args.halo_rowbytes % 1024 != 0) {
-      snprintf(err, errlen, "halo wgrad: bad geometry (bn 64, 16x8 or 8x16 box, Cout <= 64, <= 8 taps)");
+    const int kslices = args.box_rows / 16;
+    bool rows_ok = args.box_w * 128 == args.halo_rowbytes;
+    for (int j = 0; j < kslices && rows_ok; ++j)   // every accumulator's 16 B rows inside its box
+      for (int t = 0; t < args.halo_nacc && rows_ok; ++t) {
+        const long long r = static_cast<long long>(args.halo_jrow[j] + args.acc_row[t]) *
+                            args.halo_rowbytes;
+        rows_ok = args.halo_jrow[j] >= 0 && args.acc_row[t] >= 0 && r + 2048 <= b_box &&
+                  args.acc_box[t] >= 0 && args.acc_box[t] < args.halo_boxes;
+      }
+    if (bn != 64 || (args.box_w != 8 && args.box_w != 16) || args.m_valid > 64 * args.m_tiles ||
+        args.n_valid != 64 * args.n_tiles || args.halo_nacc < 1 || args.halo_nacc > kMaxTaps ||
+        args.halo_boxes < 1 || args.halo_boxes > 3 || stage % 1024 != 0 ||
+        stage * 2 > 216 * 1024 || args.halo_rowbytes % 1024 != 0 || !rows_ok) {
+      snprintf(err, errlen, "halo wgrad: bad geometry (bn 64, 8- or 16-pixel rows, 64-channel "
+               "slices, <= 9 taps, two stages in 216 KB)");
       delete p;
       return nullptr;
     }
     p->wa.halo_stages = static_cast<int>((216 * 1024) / stage > 3 ? 3 : (216 * 1024) / stage);
-    p->total_work = args.k_splits;
+    p->total_work = args.m_tiles * args.n_tiles * args.k_splits;
   }
   p->grid = p->total_work < num_sms ? p->total_work : num_sms;
   return p;

@@ -86,10 +86,12 @@ struct WgradArgs {
   int ldw;                        // dW row pitch in elements (= taps * Cin)
   float* dw;                      // fp32, accumulated with red.global.add
   int stem;                       // halo mode (igemm_wgrad_halo_kernel): 1 = 7x7/2 stem, 2 = 3x3
-  // halo mode geometry (filled by the plan builder, see igemm_wgrad.cu)
-  int halo_boxes, halo_rows;      // B boxes per stage (w shifts) and input rows per box
+  // halo mode geometry (filled by the plan builder, see igemm_wgrad.cu); m_tiles / n_tiles count
+  // 64-channel slices of Cout / Cin
+  int halo_boxes, halo_rows;      // B boxes per stage (w shifts) and input rows per box and image
   int halo_hmul, halo_h0;         // B row origin = tile row * box_h * hmul + h0
-  int halo_jmul, halo_rowbytes;   // K slice j of accumulator t reads B at (j*jmul + acc_row[t]) * rowbytes
+  int halo_rowbytes;              // bytes of one B row
+  int halo_jrow[8];               // K slice j of accumulator t reads B rows from halo_jrow[j] + acc_row[t]
   int halo_nacc, halo_stages;
   int acc_box[kMaxTaps], acc_row[kMaxTaps], box_dw[3];
 };

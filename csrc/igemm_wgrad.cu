@@ -178,26 +178,31 @@ igemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 }
 
 // ------------------------------------------------------------- halo wgrad
-// Several filter taps from ONE pass over the pixels, for layers whose Cout x Cin tile is so small
-// (64 x 64) that the generic kernel - one pass per tap - is bound by re-reading the same pixels
-// through the L2 -> SM fabric.  Per stage of 128 output pixels:
-//   A = dY box [128 pixels][64 channels], 16 KB (MN-major, M = Cout = 64)
-//   B = 1 or 3 X halo boxes (the box's w origin shifted by box_dw[i]) that also cover the input
-//       rows above / below; accumulator t multiplies K slice j (16 pixels = 2048 B of A) with the
-//       B rows at (j * jmul + acc_row[t]) * rowbytes of box acc_box[t] - a filter tap only moves
-//       the descriptor's start address, by a multiple of 1024 B (SWIZZLE_128B atoms stay aligned).
-// Each accumulator is 64 x 64 fp32; consumer warpgroup g keeps accumulators g, g + 2, g + 4, g + 6
-// in registers (up to 8 of them).
+// Several filter taps from ONE pass over the pixels.  The generic kernel above makes the tap part
+// of the work item, so a 3x3 layer streams dY and X through the L2 -> SM fabric nine times; here a
+// work item is (64-channel Cout slice mt, 64-channel Cin slice nt, pixel split) and every stage of
+// at most 128 output pixels feeds all taps:
+//   A = dY box [box_rows pixels][64 channels of slice mt] (MN-major, M = Cout), in a 16 KB slot
+//   B = 1 or 3 X halo boxes of slice nt (the box's w origin shifted by box_dw[i]) that also cover
+//       the input rows above / below; accumulator t multiplies K slice j (16 pixels = 2048 B of A)
+//       with the B rows at (halo_jrow[j] + acc_row[t]) * rowbytes of box acc_box[t] - a filter tap
+//       only moves the descriptor's start address, by a multiple of 1024 B (SWIZZLE_128B atoms
+//       stay aligned).
+// Each accumulator is 64 x 64 fp32; consumer warpgroup g keeps accumulators g, g + 2, ... in
+// registers (up to 5 of them: 160 registers, which setmaxnreg makes room for).
 //   stem 7x7/2 (window-row layout, ops/igemm.py): 16 x 8 pixels, one 16 x 21 box, 7 accumulators
 //     (filter rows), K slice j = output row j, B row 2j + r;          3.9x fewer bytes than 7 passes
-//   3x3/1 64->64: 8 x 16 pixels, three 8 x 18 boxes (dw = -1, 0, +1), 8 accumulators (all taps but
-//     the centre, which the generic kernel adds), K slice j = output rows 2j, 2j+1 (2 x 1024 B),
-//     B row 2j + dh + 1;                                              4x fewer bytes than 9 passes
-constexpr int kHaloA = 128 * 128;                    // dY box: 128 pixels x 64 channels x 2 B
+//   3x3/1, Cin and Cout multiples of 64: 8 x bh x bn pixels (bh even; bn > 1 images only when one
+//     image fits in bh rows), three 8 x (bh + 2) x bn boxes (dw = -1, 0, +1), 9 accumulators,
+//     K slice j = output rows 2j', 2j'+1 of image i (j = i * bh / 2 + j'),
+//     B row i * (bh + 2) + 2j' + dh + 1                    (ops/igemm.py _wgrad3x3_onepass_plan)
+constexpr int kHaloA = 128 * 128;                    // dY slot: 128 pixels x 64 channels x 2 B
 constexpr int kHaloMaxStages = 3;
-constexpr int kHaloSmemData = 216 * 1024;            // stem 3 x 58 KB, 3x3 3 x 70 KB
+constexpr int kHaloSmemData = 216 * 1024;            // stem 3 x 58 KB, 3x3 3 x <= 70 KB
 constexpr int kHaloSmem = kHaloSmemData + 256 + 1024;
-constexpr int kHaloAccPerWg = kMaxTaps / 2;          // 4 (8 accumulators at most, see igemm.cu)
+constexpr int kHaloAccPerWg = (kMaxTaps + 1) / 2;    // 5 (9 accumulators at most, see igemm.cu)
+constexpr int kHaloKSlices = 8;                      // 16-pixel K slices per stage, at most
+constexpr uint32_t kHaloProducerRegs = 40, kHaloConsumerRegs = 232;
 
 __global__ void __launch_bounds__(kThreads, 1)
 igemm_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA,
@@ -220,13 +225,27 @@ igemm_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA,
 
   const int total_boxes = a.tiles_w * a.tiles_h * a.tiles_n;
   const int per_split = (total_boxes + a.k_splits - 1) / a.k_splits;
-  const uint32_t b_box = static_cast<uint32_t>(a.box_w) * a.halo_rows * 128u;   // one halo box
+  const int pairs = a.m_tiles * a.n_tiles;
+  const uint32_t b_box = static_cast<uint32_t>(a.box_w) * a.halo_rows * a.box_n * 128u;
   const uint32_t stage_bytes = kHaloA + a.halo_boxes * b_box;                   // multiple of 1024
+  const uint32_t stage_tx = a.box_rows * 128u + a.halo_boxes * b_box;
+
+  // work item -> (Cout slice, Cin slice, pixel split); the slice pair varies fastest, so the CTAs
+  // running at the same time read the same pixels (each dY / X box comes from HBM about once)
+  auto decode = [&](int work, int& mt, int& nt, int& b0, int& b1) {
+    const int pair = work % pairs;
+    mt = pair / a.n_tiles;
+    nt = pair - mt * a.n_tiles;
+    b0 = (work / pairs) * per_split;
+    b1 = min(b0 + per_split, total_boxes);
+  };
 
   if (warp < 4) {
+    setmaxnreg_dec<kHaloProducerRegs>();
     if (threadIdx.x == 0) {
       for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
-        const int b0 = work * per_split, b1 = min(b0 + per_split, total_boxes);
+        int mt, nt, b0, b1;
+        decode(work, mt, nt, b0, b1);
         for (int b = b0; b < b1; ++b) {
           const int tw = b % a.tiles_w;
           const int th = (b / a.tiles_w) % a.tiles_h;
@@ -234,11 +253,11 @@ igemm_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA,
           mbar_wait(&ring.empty[ring.stage], ring.phase ^ 1);
           uint8_t* sA = smem + ring.stage * stage_bytes;
           uint64_t* bar = &ring.full[ring.stage];
-          mbar_expect_tx(bar, stage_bytes);
-          tma_load_4d(sA, &tmA, bar, 0, tw * a.box_w, th * a.box_h, tn);
+          mbar_expect_tx(bar, stage_tx);
+          tma_load_4d(sA, &tmA, bar, mt * 64, tw * a.box_w, th * a.box_h, tn * a.box_n);
           for (int i = 0; i < a.halo_boxes; ++i)
-            tma_load_4d(sA + kHaloA + i * b_box, &tmB, bar, 0, tw * a.box_w + a.box_dw[i],
-                        th * a.box_h * a.halo_hmul + a.halo_h0, tn);
+            tma_load_4d(sA + kHaloA + i * b_box, &tmB, bar, nt * 64, tw * a.box_w + a.box_dw[i],
+                        th * a.box_h * a.halo_hmul + a.halo_h0, tn * a.box_n);
           ring.advance();
         }
       }
@@ -246,16 +265,20 @@ igemm_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA,
     return;
   }
 
+  setmaxnreg_inc<kHaloConsumerRegs>();
   const int wg = (warp >> 2) - 1;
   const int wq = warp & 3;
   const bool wg_leader = (threadIdx.x & 127) == 0;
+  const int kslices = a.box_rows / 16;
   uint32_t acc_off[kHaloAccPerWg];   // descriptor offset (16-byte units) of each accumulator's B rows
 #pragma unroll
   for (int i = 0; i < kHaloAccPerWg; ++i) {
     const int t = 2 * i + wg;
     acc_off[i] = t < a.halo_nacc ? (a.acc_box[t] * b_box + a.acc_row[t] * a.halo_rowbytes) >> 4 : 0;
   }
-  const uint32_t jstep = (a.halo_jmul * a.halo_rowbytes) >> 4;
+  uint32_t j_off[kHaloKSlices];      // descriptor offset of K slice j's B rows
+#pragma unroll
+  for (int j = 0; j < kHaloKSlices; ++j) j_off[j] = (a.halo_jrow[j] * a.halo_rowbytes) >> 4;
   float acc[kHaloAccPerWg][32];
 #pragma unroll
   for (int i = 0; i < kHaloAccPerWg; ++i)
@@ -263,7 +286,8 @@ igemm_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA,
     for (int j = 0; j < 32; ++j) acc[i][j] = 0.f;
 
   for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
-    const int b0 = work * per_split, b1 = min(b0 + per_split, total_boxes);
+    int mt, nt, b0, b1;
+    decode(work, mt, nt, b0, b1);
     int prev = -1;
 #pragma unroll
     for (int i = 0; i < kHaloAccPerWg; ++i) wgmma_fence_regs(acc[i]);
@@ -280,7 +304,8 @@ igemm_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA,
           const uint64_t bt = bd0 + acc_off[i];
           Wgmma<64>::mma<1, 1>(acc[i], ad0, bt, first);
 #pragma unroll
-          for (int j = 1; j < 8; ++j) Wgmma<64>::mma<1, 1>(acc[i], ad0 + j * 128, bt + j * jstep, 1u);
+          for (int j = 1; j < kHaloKSlices; ++j)
+            if (j < kslices) Wgmma<64>::mma<1, 1>(acc[i], ad0 + j * 128, bt + j_off[j], 1u);
         }
       }
       wgmma_commit();
@@ -296,13 +321,13 @@ igemm_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA,
     if (b1 <= b0) continue;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int m = wq * 16 + (lane >> 2) + 8 * h;
+      const int m = mt * 64 + wq * 16 + (lane >> 2) + 8 * h;
       if (m >= a.m_valid) continue;
 #pragma unroll
       for (int i = 0; i < kHaloAccPerWg; ++i) {
         const int t = 2 * i + wg;
         if (t >= a.halo_nacc) continue;
-        float* o = a.dw + static_cast<long long>(m) * a.ldw + a.tap_out[t];
+        float* o = a.dw + static_cast<long long>(m) * a.ldw + a.tap_out[t] + nt * 64;
 #pragma unroll
         for (int jb = 0; jb < 8; ++jb) {
           const int c = jb * 8 + 2 * (lane & 3);

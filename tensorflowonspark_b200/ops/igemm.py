@@ -24,8 +24,10 @@ _WGRAD_WIDE = os.environ.get("TFOS_WGRAD_WIDE", "1") == "1"
 _WGRAD_WIDE_MIN_PIXELS = int(os.environ.get("TFOS_WGRAD_WIDE_MIN_PIXELS", "32768"))
 _WGRAD_WORK = int(os.environ.get("TFOS_WGRAD_WORK", "0"))  # 0: per-layer heuristic
 _STEM_HALO = os.environ.get("TFOS_STEM_HALO", "1") == "1"
+# 3x3 / stride 1 weight gradients with 64-channel multiples: all nine taps from one pass over the
+# pixels (_wgrad3x3_onepass_plan) once the layer has this many output pixels
 _WGRAD_HALO = os.environ.get("TFOS_WGRAD_HALO", "1") == "1"
-_WGRAD_HALO_MIN_PIXELS = int(os.environ.get("TFOS_WGRAD_HALO_MIN_PIXELS", "16384"))
+_WGRAD_HALO_MIN_PIXELS = int(os.environ.get("TFOS_WGRAD_HALO_MIN_PIXELS", "8192"))
 _SMS = 132   # H100 SXM; the split-K work-item counts below are multiples of it
 _STEM_SPLITS = int(os.environ.get("TFOS_STEM_SPLITS", str(_SMS)))
 # data gradients with an accumulate / fused-BN-reduction epilogue prefetch the operands that
@@ -344,29 +346,65 @@ def _wgrad_plan(dy, dy_whn, Cout, x, x_whn, Cin, dw, ldw, taps, mul, es, box=Non
       " wide" if wide else "", Cin, Cout, len(taps), k_splits))
 
 
-def _wgrad3x3_halo_plan(dy, x, dw):
-  """3x3 / stride 1 / pad 1 with Cin = 64, Cout <= 64: eight taps in one pass over the pixels
-  (csrc/igemm_wgrad.cu igemm_wgrad_halo_kernel), the centre tap by the generic kernel."""
+# three ring stages of igemm_wgrad_halo_kernel: the 7 x 7 layers measured 17 % slower with two stages
+# of 8 x 8 x 2 pixels than with three of 8 x 8 x 1
+_HALO_STAGE_BYTES = 216 * 1024 // 3
+
+
+def onepass_box(OW, OH, N):
+  """dY box (8, bh, bn) of the one-pass 3x3 weight gradient: 8 x bh pixels (bh even: a K slice is
+  two 8-pixel rows) of bn images, several images only when one image fits in bh rows.  Picks the
+  largest fraction of useful (non-padding) pixels, then the most pixels per stage.
+  Returns (bh, bn, tiles_w, tiles_h, tiles_n, useful fraction)."""
+  best = None
+  tw = -(-OW // 8)
+  for bh in range(2, 17, 2):
+    th = -(-OH // bh)
+    for bn in range(1, 128 // (8 * bh) + 1):
+      if bn > N or (bn > 1 and th > 1):
+        break
+      if 16384 + 3 * 8 * (bh + 2) * bn * 128 > _HALO_STAGE_BYTES:
+        break
+      tn = -(-N // bn)
+      useful = float(OW * OH * N) / (tw * 8 * th * bh * tn * bn)
+      key = (round(useful, 4), bh * bn)
+      if best is None or key > best[0]:
+        best = (key, (bh, bn, tw, th, tn, useful))
+  return best[1]
+
+
+def _wgrad3x3_onepass_plan(dy, x, dw):
+  """3x3 / stride 1 / pad 1 with Cin and Cout multiples of 64: all nine taps from one pass over the
+  pixels (csrc/igemm_wgrad.cu igemm_wgrad_halo_kernel).  A work item is a 64 x 64 channel slice
+  pair and a range of pixel boxes; each box of dY comes with three w-shifted X boxes (dw = -1, 0,
+  +1) that also hold the rows above and below, and a filter tap selects rows of one of them."""
   N, OH, OW, Cout = dy.shape
   _, H, W, Cin = x.shape
-  ta = _tmap4(dy, (OW, OH, N), Cout, (8, 16, 1))
-  tb = _tmap4(x, (W, H, N), Cin, (8, 16 + 2, 1))
-  taps = [(dh, dw_) for dh in (-1, 0, 1) for dw_ in (-1, 0, 1) if (dh, dw_) != (0, 0)]
-  tw, th = -(-OW // 8), -(-OH // 16)
+  bh, bn, tw, th, tn, useful = onepass_box(OW, OH, N)
+  ta = _tmap4(dy, (OW, OH, N), Cout, (8, bh, bn))
+  tb = _tmap4(x, (W, H, N), Cin, (8, bh + 2, bn))
+  taps = [(dh, dw_) for dh in (-1, 0, 1) for dw_ in (-1, 0, 1)]
+  # K slice j (16 pixels: output rows 2j', 2j'+1 of image i) reads the B rows of image i starting
+  # at output row 2j' (+ dh + 1 for the tap)
+  jpi = bh // 2
+  pairs = (Cout // 64) * (Cin // 64)
+  total_boxes = tw * th * tn
+  # one wave of work items: two waves measured 3-10 % slower (twice the fp32 atomics of dW)
+  k_splits = max(1, min((_WGRAD_WORK or _SMS) // pairs, total_boxes // 2))
   g = {
-      "tiles_w": tw, "tiles_h": th, "tiles_n": N, "box_w": 8, "box_h": 16, "box_n": 1,
+      "tiles_w": tw, "tiles_h": th, "tiles_n": tn, "box_w": 8, "box_h": bh, "box_n": bn,
       "num_taps": 1, "stem": 2,
-      "halo_boxes": 3, "box_dw": [-1, 0, 1], "halo_rows": 16 + 2, "halo_hmul": 1, "halo_h0": -1,
-      "halo_jmul": 2, "halo_rowbytes": 1024, "halo_nacc": 8,
+      "halo_boxes": 3, "box_dw": [-1, 0, 1], "halo_rows": bh + 2, "halo_hmul": 1, "halo_h0": -1,
+      "halo_rowbytes": 1024, "halo_nacc": 9,
+      "halo_jrow": [(j // jpi) * (bh + 2) + 2 * (j % jpi) for j in range(bh * bn // 2)],
       "acc_box": [d + 1 for (_, d) in taps], "acc_row": [dh + 1 for (dh, _) in taps],
       "tap_out": [((dh + 1) * 3 + (d + 1)) * Cin for (dh, d) in taps],
-      "m_tiles": 1, "n_tiles": 1, "k_splits": max(1, min(_STEM_SPLITS, tw * th * N)),
-      "m_valid": Cout, "n_valid": 64, "ldw": 9 * Cin, "dw": dw.data_ptr(),
+      "m_tiles": Cout // 64, "n_tiles": Cin // 64, "k_splits": k_splits,
+      "m_valid": Cout, "n_valid": Cin, "ldw": 9 * Cin, "dw": dw.data_ptr(),
   }
-  halo = _C().igemm_plan_wgrad(ta, tb, g, 64)
-  centre = _wgrad_plan(dy, (OW, OH, N), Cout, x, (W, H, N), Cin, dw, 9 * Cin, [(0, 0, 4 * Cin)], 1, 1)
-  handles, centre.handles = [halo] + centre.handles, []   # this plan owns (and frees) them all
-  return Plan(handles, (dy, x, dw), "wgrad 3x3 halo {}->{}".format(Cin, Cout))
+  h = _C().igemm_plan_wgrad(ta, tb, g, 64)
+  return Plan([h], (dy, x, dw), "wgrad 3x3 onepass {}->{} box 8x{}x{} useful {:.0%} splits{}".format(
+      Cin, Cout, bh, bn, useful, k_splits))
 
 
 def conv_wgrad(dy, x, dw, stride=1, pad=0):
@@ -376,9 +414,9 @@ def conv_wgrad(dy, x, dw, stride=1, pad=0):
   _, R, S, _ = dw.shape
   if R == 1 and S == 1 and stride == 1 and pad == 0:
     return gemm_wgrad(dy.view(-1, Cout), x.view(-1, Cin), dw.view(Cout, Cin))
-  if (_WGRAD_HALO and R == 3 and S == 3 and stride == 1 and pad == 1 and Cin == 64 and Cout <= 64
-      and Cout % 8 == 0 and N * OH * OW >= _WGRAD_HALO_MIN_PIXELS):
-    return _wgrad3x3_halo_plan(dy, x, dw)
+  if (_WGRAD_HALO and R == 3 and S == 3 and stride == 1 and pad == 1 and Cin % 64 == 0
+      and Cout % 64 == 0 and N * OH * OW >= _WGRAD_HALO_MIN_PIXELS):
+    return _wgrad3x3_onepass_plan(dy, x, dw)
   taps = [(s - pad, r - pad, (r * S + s) * Cin) for r in range(R) for s in range(S)]
   return _wgrad_plan(dy, (OW, OH, N), Cout, x, (W, H, N), Cin, dw, R * S * Cin, taps, stride,
                      stride)
@@ -477,7 +515,8 @@ def stem_wgrad(dy, xp, dw):
         "tiles_w": tw, "tiles_h": th, "tiles_n": N, "box_w": 16, "box_h": 8, "box_n": 1,
         "num_taps": 1, "stem": 1,
         "halo_boxes": 1, "box_dw": [0], "halo_rows": 2 * 8 + 5, "halo_hmul": 2,
-        "halo_h0": -STEM_PAD, "halo_jmul": 2, "halo_rowbytes": 2048, "halo_nacc": 7,
+        "halo_h0": -STEM_PAD, "halo_jrow": [2 * j for j in range(8)], "halo_rowbytes": 2048,
+        "halo_nacc": 7,
         "acc_box": [0] * 7, "acc_row": list(range(7)), "tap_out": [r * 64 for r in range(7)],
         "m_tiles": 1, "n_tiles": 1, "k_splits": max(1, min(_STEM_SPLITS, tw * th * N)),
         "m_valid": Cout, "n_valid": 64, "ldw": 7 * 64, "dw": dw.data_ptr(),

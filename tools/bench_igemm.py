@@ -57,6 +57,10 @@ CASES = [
     ("l3c3_wgrad", "wgrad", (14, 14, 256, 1024, 1, 1)),
     ("l3c2_wgrad", "wgrad", (14, 14, 256, 256, 3, 1)),
     ("l4c2_wgrad", "wgrad", (7, 7, 512, 512, 3, 1)),
+    # the first block of layer2-4: stride 2 in the 3x3 (torchvision v1.5)
+    ("l2c2s2_wgrad", "wgrad", (56, 56, 128, 128, 3, 2)),
+    ("l3c2s2_wgrad", "wgrad", (28, 28, 256, 256, 3, 2)),
+    ("l4c2s2_wgrad", "wgrad", (14, 14, 512, 512, 3, 2)),
     ("l4c3_wgrad", "wgrad", (7, 7, 512, 2048, 1, 1)),
 ]
 
@@ -67,6 +71,13 @@ def peaks():
     d = json.load(open(p))
     return d["hbm_gbs"], d["bf16_tflops"], "measured"
   return 3350.0, 989.0, "H100 SXM data sheet"
+
+
+def device_line():
+  import subprocess
+  q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm",
+                      "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+  return "{} ({})".format(torch.cuda.get_device_name(0), q or "power limit / max SM clock unknown")
 
 
 def build(kind, shape, nbuf, stats=True, epi_prefetch=None):
@@ -112,10 +123,16 @@ def main():
   ap.add_argument("--no-stats", action="store_true")
   ap.add_argument("--epi-prefetch", type=int, choices=(0, 1), default=None,
                   help="dgrad_* kinds: prefetch the epilogue operands (default: the plan's choice)")
+  ap.add_argument("--wgrad-onepass", type=int, choices=(0, 1), default=None,
+                  help="3x3 wgrad: all nine taps from one pass over the pixels (default: the "
+                       "plan's choice, TFOS_WGRAD_HALO)")
   ap.add_argument("--kind", default=None,
                   help="fprop | dgrad | dgrad_red | dgrad_acc | dgrad_accred | wgrad")
   args = ap.parse_args()
+  if args.wgrad_onepass is not None:
+    igemm._WGRAD_HALO = bool(args.wgrad_onepass)
   hbm, tf, src = peaks()
+  print(device_line())
   print("peaks ({}): HBM {:.0f} GB/s, bf16 {:.0f} TFLOP/s".format(src, hbm, tf))
   print("{:12s} {:6s} {:>9s} {:>9s} {:>9s} {:>7s} {:>7s}".format(
       "case", "kind", "us", "TFLOP/s", "GB/s", "%flops", "%hbm"))
@@ -138,9 +155,9 @@ def main():
     e1.record()
     torch.cuda.synchronize()
     us = e0.elapsed_time(e1) * 1e3 / iters
-    print("{:12s} {:6s} {:9.1f} {:9.1f} {:9.1f} {:6.1f}% {:6.1f}%".format(
+    print("{:12s} {:6s} {:9.1f} {:9.1f} {:9.1f} {:6.1f}% {:6.1f}%  {}".format(
         name, kind, us, flops / us / 1e6, byts / us / 1e3, 100 * flops / us / 1e6 / tf,
-        100 * byts / us / 1e3 / hbm))
+        100 * byts / us / 1e3 / hbm, plans[0].desc))
     del plans
     torch.cuda.empty_cache()
 
