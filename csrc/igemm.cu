@@ -20,6 +20,7 @@
 // released as soon as the wgmma group that read it has retired, so the producer runs up to
 // a ring ahead - across tile boundaries, i.e. the next tile's operands arrive during the
 // epilogue of the current one.
+#include <limits.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -873,7 +874,15 @@ IGemmPlan* igemm_plan_wgrad(const TmapDesc& a, const TmapDesc& b, const WgradArg
   p->wa = args;
   p->kind = 1;
   p->bn = bn;
-  p->total_work = args.num_taps * args.m_tiles * args.n_tiles * args.k_splits;
+  // generic kernel: total_work counts (output tile, pixel box) iterations, split evenly over the grid
+  const long long iters = static_cast<long long>(args.num_taps) * args.m_tiles * args.n_tiles *
+                          args.tiles_w * args.tiles_h * args.tiles_n;
+  if (iters < 1 || iters > INT_MAX) {
+    snprintf(err, errlen, "wgrad: %lld (tile, pixel box) iterations", iters);
+    delete p;
+    return nullptr;
+  }
+  p->total_work = static_cast<int>(iters);
   if (args.stem) {  // igemm_wgrad_halo_kernel: several taps per pass over the pixels
     const long long b_box = static_cast<long long>(args.box_w) * args.halo_rows * args.box_n * 128;
     const long long stage = 128 * 128 + args.halo_boxes * b_box;

@@ -81,7 +81,9 @@ struct WgradArgs {
   int num_taps;
   int tap_dw[kMaxTaps], tap_dh[kMaxTaps], tap_dc[kMaxTaps];
   int tap_out[kMaxTaps];          // element offset of the tap inside a dW row
-  int m_tiles, n_tiles, k_splits;
+  int m_tiles, n_tiles;
+  int k_splits;                   // halo mode: pixel splits per slice pair (the generic kernel
+                                  // splits the pixels evenly over the grid, igemm_wgrad.cu)
   int m_valid, n_valid;           // Cout, Cin
   int ldw;                        // dW row pitch in elements (= taps * Cin)
   float* dw;                      // fp32, accumulated with red.global.add

@@ -52,6 +52,14 @@ __device__ __forceinline__ void red_pair(float* o, int col, int n_valid, bool ve
 // are MN-major in shared memory (the contiguous global dimension is channels,
 // the reduction runs over pixel rows), one TMA box of <=128 pixels per stage.
 // Warpgroup g computes output rows [64 g, 64 g + 64) of the 128 x BN tile.
+//
+// The (output tile, pixel box) iterations of a launch form one flat range, tiles outermost
+// (tile = (tap, m tile, n tile), n tile fastest) and a tile's boxes consecutive; total_work is its
+// length.  CTA c of G takes iterations [c * total_work / G, (c + 1) * total_work / G), so slices
+// differ by at most one box however the count falls against the SM count, and it adds its partial
+// dW at every tile boundary it crosses and at the end of its slice.  CTAs with neighbouring slices
+// stream disjoint pixels of the same tile at the same time (its X and dY boxes are shared in L2).
+// ops/igemm.py _wgrad_slices is the same split.
 template <int BN>
 struct WgCfg {
   static constexpr int kAStage = 2 * 128 * 128;          // two 64-channel boxes, <=128 pixels
@@ -82,29 +90,35 @@ igemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   }
   __syncthreads();
 
-  const int total_boxes = a.tiles_w * a.tiles_h * a.tiles_n;
-  const int boxes_per_split = (total_boxes + a.k_splits - 1) / a.k_splits;
+  const int boxes = a.tiles_w * a.tiles_h * a.tiles_n;   // pixel boxes per output tile
   const uint32_t box_bytes = static_cast<uint32_t>(a.box_rows) * 128u;
   const uint32_t stage_tx = box_bytes * (2 + BN / 64);
+  const int s0 = static_cast<int>(static_cast<long long>(blockIdx.x) * total_work / gridDim.x);
+  const int s1 = static_cast<int>(static_cast<long long>(blockIdx.x + 1) * total_work / gridDim.x);
 
-  // work item -> (tap, m tile, n tile, k split); splits vary fastest so that
-  // concurrently running CTAs stream disjoint pixels of the same tile.
-  auto decode = [&](int work, int& t, int& mt, int& nt, int& b0, int& b1) {
-    const int ks = work % a.k_splits;
-    int r = work / a.k_splits;
+  // the segment of this CTA's slice that ends at iteration end: boxes [b0, b1) of tile
+  // (tap t, m tile mt, n tile nt); returns its start, where the previous segment ends.  The
+  // segments run last first, so a slice that crosses into a tile starts on that tile's first
+  // boxes: when there are about as many tiles as CTAs, all CTAs then stream about the same pixels
+  // at the same time instead of points spread over the whole tensor.  The producer and the
+  // consumers walk the same segments, so their ring stages and phases stay in step.
+  auto segment = [&](int end, int& t, int& mt, int& nt, int& b0, int& b1) {
+    int r = (end - 1) / boxes;
+    const int base = r * boxes;
+    b0 = max(s0, base) - base;
+    b1 = end - base;
     nt = r % a.n_tiles;
     r /= a.n_tiles;
     mt = r % a.m_tiles;
     t = r / a.m_tiles;
-    b0 = ks * boxes_per_split;
-    b1 = min(b0 + boxes_per_split, total_boxes);
+    return base + b0;
   };
 
   if (warp < 4) {
     if (threadIdx.x == 0) {
-      for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
+      for (int it = s1; it > s0;) {
         int t, mt, nt, b0, b1;
-        decode(work, t, mt, nt, b0, b1);
+        it = segment(it, t, mt, nt, b0, b1);
         for (int b = b0; b < b1; ++b) {
           const int tw = b % a.tiles_w;
           const int th = (b / a.tiles_w) % a.tiles_h;
@@ -136,9 +150,9 @@ igemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
+  for (int it = s1; it > s0;) {
     int t, mt, nt, b0, b1;
-    decode(work, t, mt, nt, b0, b1);
+    it = segment(it, t, mt, nt, b0, b1);
     int prev = -1;
     wgmma_fence_regs(acc);
     for (int b = b0; b < b1; ++b) {
@@ -160,7 +174,6 @@ igemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     wgmma_wait<0>();
     wgmma_fence_regs(acc);
     if (prev >= 0 && wg_leader) mbar_arrive(&ring.empty[prev]);
-    if (b1 <= b0) continue;
     const bool vec_ok = (a.ldw & 1) == 0 && (a.tap_out[t] & 1) == 0;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -179,7 +192,7 @@ igemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 
 // ------------------------------------------------------------- halo wgrad
 // Several filter taps from ONE pass over the pixels.  The generic kernel above makes the tap part
-// of the work item, so a 3x3 layer streams dY and X through the L2 -> SM fabric nine times; here a
+// of the output tile, so a 3x3 layer streams dY and X through the L2 -> SM fabric nine times; here a
 // work item is (64-channel Cout slice mt, 64-channel Cin slice nt, pixel split) and every stage of
 // at most 128 output pixels feeds all taps:
 //   A = dY box [box_rows pixels][64 channels of slice mt] (MN-major, M = Cout), in a 16 KB slot

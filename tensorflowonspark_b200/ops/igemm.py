@@ -22,13 +22,15 @@ _launches = 0
 # weight-gradient tiling knobs (tools/bench_igemm.py sweeps them)
 _WGRAD_WIDE = os.environ.get("TFOS_WGRAD_WIDE", "1") == "1"
 _WGRAD_WIDE_MIN_PIXELS = int(os.environ.get("TFOS_WGRAD_WIDE_MIN_PIXELS", "32768"))
-_WGRAD_WORK = int(os.environ.get("TFOS_WGRAD_WORK", "0"))  # 0: per-layer heuristic
+# work items of the one-pass 3x3 plan (_wgrad3x3_onepass_plan); 0: one wave.  The generic kernel
+# splits its pixels evenly over the SMs (_wgrad_slices) and has no such knob.
+_WGRAD_WORK = int(os.environ.get("TFOS_WGRAD_WORK", "0"))
 _STEM_HALO = os.environ.get("TFOS_STEM_HALO", "1") == "1"
 # 3x3 / stride 1 weight gradients with 64-channel multiples: all nine taps from one pass over the
 # pixels (_wgrad3x3_onepass_plan) once the layer has this many output pixels
 _WGRAD_HALO = os.environ.get("TFOS_WGRAD_HALO", "1") == "1"
 _WGRAD_HALO_MIN_PIXELS = int(os.environ.get("TFOS_WGRAD_HALO_MIN_PIXELS", "8192"))
-_SMS = 132   # H100 SXM; the split-K work-item counts below are multiples of it
+_SMS = 132   # H100 SXM; the halo kernels' work-item counts below are multiples of it
 _STEM_SPLITS = int(os.environ.get("TFOS_STEM_SPLITS", str(_SMS)))
 # data gradients with an accumulate / fused-BN-reduction epilogue prefetch the operands that
 # epilogue reads into shared memory during the main loop (csrc/igemm.cu); 0 reads them in the
@@ -317,33 +319,50 @@ def _wgrad_plan(dy, dy_whn, Cout, x, x_whn, Cin, dw, ldw, taps, mul, es, box=Non
   else:
     tb = _tmap4(x, x_whn, Cin, (bw * es, bh * es, bnn), es=(es, es, 1))
   m_tiles, n_tiles = -(-Cout // 128), -(-n_valid // bn)
-  out_tiles = len(taps) * m_tiles * n_tiles
-  total_boxes = tw * th * tn
-  # split-K work items (measured, tools/bench_igemm.py --kind wgrad): the HBM-bound 1x1 layers
-  # with many pixels want one wave (fewer fp32 atomics), everything else two to four
-  work = _WGRAD_WORK
-  if work == 0 and wide:
-    # 128 KB of fp32 atomics per work item: one wave for the memory bound 1x1 layers, two for the
-    # 3x3 ones
-    work = _SMS if len(taps) == 1 else 2 * _SMS
-  if work == 0:
-    if len(taps) == 1:
-      work = _SMS if total_boxes >= 1024 else 4 * _SMS
-    else:
-      work = 4 * _SMS if Cout <= 64 else 2 * _SMS
-  k_splits = max(1, min(-(-work // out_tiles), max(1, total_boxes // 2)))
   g = {
       "tiles_w": tw, "tiles_h": th, "tiles_n": tn, "box_w": bw, "box_h": bh, "box_n": bnn,
       "mul_w": mul, "mul_h": mul, "num_taps": len(taps),
       "tap_dw": [t[0] for t in taps], "tap_dh": [t[1] for t in taps],
       "tap_dc": tap_dc if tap_dc is not None else [0] * len(taps),
       "tap_out": tap_out if tap_out is not None else [t[2] for t in taps],
-      "m_tiles": m_tiles, "n_tiles": n_tiles, "k_splits": k_splits,
+      "m_tiles": m_tiles, "n_tiles": n_tiles,
       "m_valid": Cout, "n_valid": n_valid, "ldw": ldw, "dw": dw.data_ptr(),
   }
   h = _C().igemm_plan_wgrad(ta, tb, g, bn)
-  return Plan([h], (dy, x, dw), "wgrad{} {}->{} taps{} splits{}".format(
-      " wide" if wide else "", Cin, Cout, len(taps), k_splits))
+  return Plan([h], (dy, x, dw), "wgrad{} {}->{} taps{} {}".format(
+      " wide" if wide else "", Cin, Cout, len(taps),
+      _slices_desc(len(taps) * m_tiles * n_tiles, tw * th * tn, _C().igemm_info(h)["grid"])))
+
+
+def _wgrad_slices(tiles, boxes, ctas):
+  """The pixel split of the generic weight-gradient kernel (csrc/igemm_wgrad.cu,
+  igemm_wgrad_kernel).  The ``tiles * boxes`` (output tile, pixel box) iterations, tiles outermost,
+  go to ``min(ctas, tiles * boxes)`` CTAs in contiguous slices whose lengths differ by at most one
+  box.  Returns one list per CTA of the segments ``(tile, first box, end box)`` of its slice, one
+  per tile it touches, in the order the CTA walks them: last first.  The CTA adds its partial dW
+  to the tile once per segment."""
+  total = tiles * boxes
+  grid = min(ctas, total)
+  out = []
+  for c in range(grid):
+    start, it = c * total // grid, (c + 1) * total // grid
+    segs = []
+    while it > start:
+      t = (it - 1) // boxes
+      b0 = max(start, t * boxes) - t * boxes
+      segs.append((t, b0, it - t * boxes))
+      it = t * boxes + b0
+    out.append(segs)
+  return out
+
+
+def _slices_desc(tiles, boxes, ctas):
+  slices = _wgrad_slices(tiles, boxes, ctas)
+  lens = [sum(b1 - b0 for (_, b0, b1) in s) for s in slices]
+  lo, hi = min(lens), max(lens)
+  mid = sum(1 for s in slices if s[-1][1] != 0)
+  return "slice {} boxes, {}/{} CTAs start mid-tile".format(
+      lo if lo == hi else "{}-{}".format(lo, hi), mid, len(slices))
 
 
 # three ring stages of igemm_wgrad_halo_kernel: the 7 x 7 layers measured 17 % slower with two stages
@@ -526,14 +545,12 @@ def stem_wgrad(dy, xp, dw):
   bw, bh, bnn, tw, th, tn = choose_box(OW, OH, N, multiple_of=16, allow_pad=True)
   ta = _tmap4(dy, (OW, OH, N), Cout, (bw, bh, bnn))
   tb = _stem_tmap(xp, N, H, Wp, OW, (bw, bh, bnn), 2)
-  out_tiles = 7
-  k_splits = max(1, min(-(-2 * _SMS // out_tiles), max(1, tw * th * tn // 2)))
   g = {
       "tiles_w": tw, "tiles_h": th, "tiles_n": tn, "box_w": bw, "box_h": bh, "box_n": bnn,
       "mul_w": 1, "mul_h": 2, "num_taps": 7,
       "tap_dw": [0] * 7, "tap_dh": [r - STEM_PAD for r in range(7)], "tap_dc": [0] * 7,
       "tap_out": [r * 64 for r in range(7)],
-      "m_tiles": -(-Cout // 128), "n_tiles": 1, "k_splits": k_splits,
+      "m_tiles": -(-Cout // 128), "n_tiles": 1,
       "m_valid": Cout, "n_valid": 64, "ldw": 7 * 64, "dw": dw.data_ptr(),
   }
   h = _C().igemm_plan_wgrad(ta, tb, g, 64)

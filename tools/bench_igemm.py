@@ -62,6 +62,12 @@ CASES = [
     ("l3c2s2_wgrad", "wgrad", (28, 28, 256, 256, 3, 2)),
     ("l4c2s2_wgrad", "wgrad", (14, 14, 512, 512, 3, 2)),
     ("l4c3_wgrad", "wgrad", (7, 7, 512, 2048, 1, 1)),
+    ("l4c1_wgrad", "wgrad", (7, 7, 2048, 512, 1, 1)),
+    ("l4c1b1_wgrad", "wgrad", (14, 14, 1024, 512, 1, 1)),   # first block of layer4
+    # projection shortcuts of the first blocks: 1x1, stride 2
+    ("l2ds_wgrad", "wgrad", (56, 56, 256, 512, 1, 2)),
+    ("l3ds_wgrad", "wgrad", (28, 28, 512, 1024, 1, 2)),
+    ("l4ds_wgrad", "wgrad", (14, 14, 1024, 2048, 1, 2)),
 ]
 
 
