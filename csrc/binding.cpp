@@ -496,9 +496,40 @@ void allreduce_opt(const py::dict& d) {
   a.grads_mc = reinterpret_cast<const float*>(geti<uint64_t>(d, "grads_mc", 0));
   a.weights_mc = reinterpret_cast<__nv_bfloat16*>(geti<uint64_t>(d, "weights_mc", 0));
   a.aux32_mc = reinterpret_cast<float*>(geti<uint64_t>(d, "aux32_mc", 0));
+  a.lars_off = reinterpret_cast<const long long*>(geti<uint64_t>(d, "lars_off", 0));
+  a.lars_norms = reinterpret_cast<const float*>(geti<uint64_t>(d, "lars_norms", 0));
+  a.lars_t0 = geti<int>(d, "lars_t0", 0);
+  a.lars_nt = geti<int>(d, "lars_nt", 0);
+  a.lars_T = geti<int>(d, "lars_T", 0);
   const int opt = geti<int>(d, "opt", 0);
   const int grid = geti<int>(d, "grid", 32);
   check(tfos::allreduce_opt(a, opt, grid, cur_stream(), geti<int>(d, "phase", 0)), "allreduce_opt");
+}
+
+void lars_norms(const py::dict& d) {
+  tfos::LarsNormArgs a;
+  std::memset(&a, 0, sizeof(a));
+  a.grads = reinterpret_cast<const float*>(d["grads"].cast<uint64_t>());
+  a.master = reinterpret_cast<const float*>(d["master"].cast<uint64_t>());
+  a.seg = reinterpret_cast<const long long*>(geti<uint64_t>(d, "seg", 0));
+  a.tseg = reinterpret_cast<const int*>(d["tseg"].cast<uint64_t>());
+  a.partial = reinterpret_cast<float*>(geti<uint64_t>(d, "partial", 0));
+  a.nseg = geti<int>(d, "nseg", 0);
+  a.t0 = geti<int>(d, "t0", 0);
+  a.nt = geti<int>(d, "nt", 0);
+  a.T = geti<int>(d, "T", 0);
+  a.world = geti<int>(d, "world", 1);
+  a.rank = geti<int>(d, "rank", 0);
+  a.slot = geti<int>(d, "slot", 0);
+  TORCH_CHECK(a.world >= 1 && a.world <= tfos::kMaxRanks, "lars_norms: world out of range");
+  fill_ptrs(d["norms"].cast<std::vector<uint64_t>>(), reinterpret_cast<void**>(a.norms), a.world);
+  a.norms_mc = reinterpret_cast<float*>(geti<uint64_t>(d, "norms_mc", 0));
+  if (a.world > 1) {
+    fill_ptrs(d["flags"].cast<std::vector<uint64_t>>(), reinterpret_cast<void**>(a.flags), a.world);
+    a.epoch = reinterpret_cast<uint32_t*>(d["epoch"].cast<uint64_t>());
+  }
+  a.block_counter = reinterpret_cast<uint32_t*>(d["block_counter"].cast<uint64_t>());
+  check(tfos::lars_norms(a, cur_stream()), "lars_norms");
 }
 
 tfos::BcastArgs parse_bcast(const py::dict& d) {
@@ -683,6 +714,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("copy_channels", &copy_channels);
   m.def("pixel_xent", &pixel_xent);
   m.def("allreduce_opt", &allreduce_opt);
+  m.def("lars_norms", &lars_norms);
   m.def("bcast_pull", &bcast_pull);
   m.def("flag_barrier", &flag_barrier);
   m.def("set_flag_timeout_ms", &set_flag_timeout_ms);

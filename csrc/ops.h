@@ -74,13 +74,16 @@ cudaError_t pixel_xent(const void* logits, const int* labels, void* dlogits, flo
 
 // ---- optim_comm.cu
 constexpr int kMaxRanks = 8;
-constexpr int kOptSgd = 0, kOptMomentum = 1, kOptAdam = 2;
+constexpr int kOptSgd = 0, kOptMomentum = 1, kOptAdam = 2, kOptLars = 3;
+// LARS: most adapted tensors one shard of a bucket may intersect (the update kernel keeps their
+// start offsets and trust ratios in shared memory); ResNet-152 has 156 adapted tensors
+constexpr int kLarsMaxTensors = 256;
 
 struct AllreduceOptArgs {
   float* master;       // fp32 master weights (full length; a rank only touches its shards)
-  float* state1;       // momentum / Adam m
+  float* state1;       // momentum / Adam m / LARS velocity (lr and trust ratio applied inside)
   float* state2;       // Adam v
-  const float* hyper;  // device: lr, momentum, wd, grad_scale, beta1, beta2, eps, step
+  const float* hyper;  // device: lr, momentum, wd, grad_scale, beta1 | LARS eta, beta2, eps, step
   long long begin, end;  // element range of this bucket (begin % 8 == 0)
   long long decay_end;   // elements [0, decay_end) receive weight decay
   long long state_offset;
@@ -95,9 +98,39 @@ struct AllreduceOptArgs {
   float* aux32_mc;
   uint32_t* epoch;          // local, one word per slot
   uint32_t* block_counter;  // local, one word per slot
+  // LARS only.  The adapted tensors (the decayed head) tile [0, decay_end): tensor t is
+  // [lars_off[t], lars_off[t + 1]).  This rank's shard intersects [lars_t0, lars_t0 + lars_nt).
+  // lars_norms is the local [world][lars_T] table of {sum g^2, sum w^2, 0, 0} that
+  // lars_norms() filled, row r with rank r's partial sums.
+  const long long* lars_off;
+  const float* lars_norms;
+  int lars_t0, lars_nt, lars_T;
 };
 // phase: 0 = fused; 1 = intra-host reduce-scatter only; 2 = update + all-gather only (optim_comm.cu)
+// kOptLars with world > 1 runs as phase 1 -> lars_norms -> phase 2 (phase 0 is refused)
 cudaError_t allreduce_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStream_t s, int phase = 0);
+
+// LARS per-tensor norms of one rank's shard of one bucket (deterministic: no float atomics).
+// seg[2 s], seg[2 s + 1] bound segment s; the segments of local tensor j are
+// [tseg[j], tseg[j + 1]).  Each CTA reduces whole segments into partial[2 s .. 2 s + 1]; the
+// last CTA sums every tensor's segments in order and stores {sum g^2, sum w^2} into row `rank`
+// of every local peer's norms table (multimem.st when norms_mc is set), then runs the same
+// release / acquire exit barrier as allreduce_opt on flag slot `slot`.
+struct LarsNormArgs {
+  const float* grads;    // this rank's reduced gradients (unscaled sum)
+  const float* master;
+  const long long* seg;
+  const int* tseg;
+  float* partial;        // [2 nseg] scratch, overwritten every launch
+  float* norms[kMaxRanks];
+  float* norms_mc;
+  int nseg, t0, nt, T;
+  int world, rank, slot;
+  uint32_t* flags[kMaxRanks];
+  uint32_t* epoch;
+  uint32_t* block_counter;  // back at 0 when the kernel completes
+};
+cudaError_t lars_norms(const LarsNormArgs& a, cudaStream_t s);
 
 struct BcastArgs {
   int world, rank, root, slot;

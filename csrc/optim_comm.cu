@@ -14,6 +14,8 @@
 //                   updated bf16 weights into every rank's weight buffer - the
 //                   "all-gather" half of the all-reduce carries the new
 //                   parameters instead of the reduced gradients.
+//   lars_norms    : LARS per-tensor norms of a rank's reduced shard, exchanged among the local
+//                   peers between the reduce-scatter and update halves of allreduce_opt.
 //   bcast_pull    : startup broadcast, every rank pulls the root's parameters.
 //   ps_*          : asynchronous parameter server: workers apply gradients to
 //                   PS-resident weights with remote red.add (no barrier) and
@@ -71,7 +73,8 @@ __device__ __forceinline__ void multimem_st_b32x4(void* mc, uint4 v) {
 }
 
 // hyper[]: 0 lr, 1 momentum, 2 weight_decay, 3 grad_scale (1/world * loss scale),
-//          4 beta1, 5 beta2, 6 eps, 7 step (Adam bias correction)
+//          4 beta1 (Adam) | trust coefficient eta (LARS), 5 beta2, 6 eps, 7 step (Adam bias
+//          correction)
 template <int OPT>
 __device__ __forceinline__ float opt_update(float w, float g, float& s1, float& s2,
                                             const float* h, bool decay) {
@@ -93,6 +96,16 @@ __device__ __forceinline__ float opt_update(float w, float g, float& s1, float& 
   return w - h[0] * g;
 }
 
+// LARS.  lrt = lr * trust ratio of the element's tensor for the adapted (decayed) head, where
+// v = m v + lr trust (g + wd w); the tail (BN scale/offset, biases) takes v = m v + lr g.  Unlike
+// momentum, the velocity carries lr: w = w - v.
+__device__ __forceinline__ float lars_update(float w, float g, float& v, const float* h,
+                                             bool adapted, float lrt) {
+  g *= h[3];
+  v = adapted ? h[1] * v + lrt * (g + h[2] * w) : h[1] * v + h[0] * g;
+  return w - v;
+}
+
 // PHASE splits the kernel for the hierarchical (several hosts) all-reduce: 1 = intra-host
 // reduce-scatter only (the sum over the local peers of this rank's shard replaces that shard of
 // the rank's OWN gradient buffer - peers only ever read the other shards of it); 2 = update +
@@ -111,6 +124,30 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
       st_release_sys(a.flags[threadIdx.x] + a.slot * 32 + rank, e);
     if (threadIdx.x < world) wait_flag(my + threadIdx.x, e);
   }
+  // LARS: start offsets and trust ratios of the shard's adapted tensors.  Every rank sums the
+  // rows of the norms table in rank order, so ranks whose shards split one tensor derive the
+  // same ratio bit for bit.
+  const long long* t_off = nullptr;
+  const float* t_trust = nullptr;
+  if constexpr (OPT == kOptLars) {
+    __shared__ long long s_off[kLarsMaxTensors + 1];
+    __shared__ float s_trust[kLarsMaxTensors];
+    for (int j = threadIdx.x; j <= a.lars_nt; j += blockDim.x) s_off[j] = a.lars_off[a.lars_t0 + j];
+    for (int j = threadIdx.x; j < a.lars_nt; j += blockDim.x) {
+      float g2 = 0.f, w2 = 0.f;
+      for (int r = 0; r < world; ++r) {
+        const uint4 v = ld_relaxed_sys_v4(
+            a.lars_norms + (static_cast<long long>(r) * a.lars_T + a.lars_t0 + j) * 4);
+        g2 += __uint_as_float(v.x);
+        w2 += __uint_as_float(v.y);
+      }
+      const float gn = sqrtf(g2) * fabsf(a.hyper[3]), wn = sqrtf(w2);
+      s_trust[j] = (wn > 0.f && gn > 0.f) ? a.hyper[4] * wn / (gn + a.hyper[2] * wn) : 1.f;
+    }
+    t_off = s_off;
+    t_trust = s_trust;
+  }
+  int tj = 0;  // this thread's current tensor: its elements are visited in ascending order
   __syncthreads();
 
   const long long n = a.end - a.begin;
@@ -126,7 +163,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
   for (long long i0 = lo + (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 8;
        i0 < hi; i0 += stride * kU) {
    float4 mg0[kU], mg1[kU];
-   if (MULTIMEM) {
+   if (MULTIMEM && PHASE != 2) {
 #pragma unroll
      for (int u = 0; u < kU; ++u) {
        const long long iu = i0 + u * stride;
@@ -197,8 +234,20 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
       s2[0] = m0.x, s2[1] = m0.y, s2[2] = m0.z, s2[3] = m0.w;
       s2[4] = m1.x, s2[5] = m1.y, s2[6] = m1.z, s2[7] = m1.w;
     }
+    if constexpr (OPT == kOptLars) {
+      // tensors are padded to multiples of 8 elements: the group lies inside one tensor
+      const bool adapted = i < a.decay_end;
+      float lrt = 0.f;
+      if (adapted) {
+        while (tj + 1 < a.lars_nt && t_off[tj + 1] <= i) ++tj;
+        lrt = h[0] * t_trust[tj];
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) w[j] = lars_update(w[j], g[j], s1[j], h, adapted, lrt);
+    } else {
 #pragma unroll
     for (int j = 0; j < 8; ++j) w[j] = opt_update<OPT>(w[j], g[j], s1[j], s2[j], h, i + j < a.decay_end);
+    }
     *reinterpret_cast<float4*>(a.master + li) = make_float4(w[0], w[1], w[2], w[3]);
     *reinterpret_cast<float4*>(a.master + li + 4) = make_float4(w[4], w[5], w[6], w[7]);
     if (OPT != kOptSgd) {
@@ -342,6 +391,94 @@ __global__ void flag_barrier_kernel(const BcastArgs a) {
   }
   __syncthreads();
   if (threadIdx.x == 0) *a.epoch = e;
+}
+
+// LARS norm pass (see LarsNormArgs in ops.h).  Segments are reduced in a fixed thread -> element
+// mapping and a fixed tree, tensors sum their segments in order: the result does not depend on
+// which CTA takes which segment, and replicas that see the same gradients get the same bits.
+constexpr int kLarsNormThreads = 256;
+__global__ void __launch_bounds__(kLarsNormThreads) lars_norms_kernel(const LarsNormArgs a) {
+  __shared__ float red[2][kLarsNormThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int s = blockIdx.x; s < a.nseg; s += gridDim.x) {
+    const long long lo = a.seg[2 * s], hi = a.seg[2 * s + 1];
+    float g2 = 0.f, w2 = 0.f;
+    for (long long i = lo + threadIdx.x * 8; i < hi; i += kLarsNormThreads * 8) {
+      const float4 g0 = *reinterpret_cast<const float4*>(a.grads + i);
+      const float4 g1 = *reinterpret_cast<const float4*>(a.grads + i + 4);
+      const float4 w0 = *reinterpret_cast<const float4*>(a.master + i);
+      const float4 w1 = *reinterpret_cast<const float4*>(a.master + i + 4);
+      g2 += g0.x * g0.x + g0.y * g0.y + g0.z * g0.z + g0.w * g0.w;
+      g2 += g1.x * g1.x + g1.y * g1.y + g1.z * g1.z + g1.w * g1.w;
+      w2 += w0.x * w0.x + w0.y * w0.y + w0.z * w0.z + w0.w * w0.w;
+      w2 += w1.x * w1.x + w1.y * w1.y + w1.z * w1.z + w1.w * w1.w;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      g2 += __shfl_xor_sync(0xffffffffu, g2, o);
+      w2 += __shfl_xor_sync(0xffffffffu, w2, o);
+    }
+    if (lane == 0) red[0][warp] = g2, red[1][warp] = w2;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float sg = 0.f, sw = 0.f;
+      for (int k = 0; k < kLarsNormThreads / 32; ++k) sg += red[0][k], sw += red[1][k];
+      a.partial[2 * s] = sg;
+      a.partial[2 * s + 1] = sw;
+    }
+    __syncthreads();
+  }
+  // the last CTA to finish sums the partials (threadFenceReduction pattern)
+  __shared__ uint32_t is_last;
+  if (threadIdx.x == 0) {
+    __threadfence();
+    is_last = (atomicAdd(a.block_counter, 1u) == gridDim.x - 1) ? 1u : 0u;
+  }
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  const int world = a.world, rank = a.rank;
+  // one warp per tensor: lane l takes segments l, l + 32, ... then a fixed shuffle tree
+  for (int j = warp; j < a.nt; j += kLarsNormThreads / 32) {
+    double sg = 0.0, sw = 0.0;
+    for (int s = a.tseg[j] + lane; s < a.tseg[j + 1]; s += 32) {
+      sg += __ldcg(a.partial + 2 * s);
+      sw += __ldcg(a.partial + 2 * s + 1);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      sg += __shfl_xor_sync(0xffffffffu, sg, o);
+      sw += __shfl_xor_sync(0xffffffffu, sw, o);
+    }
+    if (lane != 0) continue;
+    uint4 v;
+    v.x = __float_as_uint(static_cast<float>(sg));
+    v.y = __float_as_uint(static_cast<float>(sw));
+    v.z = v.w = 0u;
+    const long long off = (static_cast<long long>(rank) * a.T + a.t0 + j) * 4;
+    if (world == 1) {
+      *reinterpret_cast<uint4*>(a.norms[0] + off) = v;
+    } else if (a.norms_mc != nullptr) {
+      multimem_st_b32x4(a.norms_mc + off, v);
+    } else {
+#pragma unroll
+      for (int p = 0; p < kMaxRanks; ++p)
+        if (p < world) st_relaxed_sys_v4(a.norms[(rank + p) % world] + off, v);
+    }
+  }
+  if (world > 1) {
+    // exit barrier: when this kernel completes on a rank, every peer's row is visible there
+    const uint32_t e = *a.epoch + 1;
+    __threadfence_system();
+    __syncthreads();
+    if (threadIdx.x < world) {
+      st_release_sys(a.flags[threadIdx.x] + a.slot * 32 + 16 + rank, e);
+      wait_flag(a.flags[rank] + a.slot * 32 + 16 + threadIdx.x, e);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) *a.epoch = e;
+  }
+  if (threadIdx.x == 0) *a.block_counter = 0;
 }
 
 // ------------------------------------------------------- parameter server
@@ -563,6 +700,31 @@ cudaError_t launch_ar(const AllreduceOptArgs& a, int grid, cudaStream_t s, int p
   return cudaGetLastError();
 }
 
+// LARS needs whole-tensor norms of the reduced gradient between the two halves, so with peers it
+// always runs split; on a one-host NVLS communicator both halves use the multicast paths
+cudaError_t launch_lars(const AllreduceOptArgs& a, int grid, cudaStream_t s, int phase) {
+  if (a.lars_nt < 0 || a.lars_nt > kLarsMaxTensors) return cudaErrorInvalidValue;
+  if (a.lars_nt > 0 && (a.lars_off == nullptr || a.lars_norms == nullptr))
+    return cudaErrorInvalidValue;
+  const bool nvls = a.grads_mc != nullptr && a.weights_mc != nullptr && a.world > 1;
+  if (phase == 1) {
+    if (nvls)
+      allreduce_opt_kernel<kOptSgd, true, 1><<<grid, 512, 0, s>>>(a);
+    else
+      allreduce_opt_kernel<kOptSgd, false, 1><<<grid, 512, 0, s>>>(a);
+  } else if (phase == 2) {
+    if (nvls)
+      allreduce_opt_kernel<kOptLars, true, 2><<<grid, 512, 0, s>>>(a);
+    else
+      allreduce_opt_kernel<kOptLars, false, 2><<<grid, 512, 0, s>>>(a);
+  } else if (a.world == 1) {
+    allreduce_opt_kernel<kOptLars, false><<<grid, 512, 0, s>>>(a);
+  } else {
+    return cudaErrorInvalidValue;
+  }
+  return cudaGetLastError();
+}
+
 }  // namespace
 
 cudaError_t allreduce_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStream_t s, int phase) {
@@ -572,8 +734,16 @@ cudaError_t allreduce_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStre
     case kOptSgd: return launch_ar<kOptSgd>(a, grid, s, phase);
     case kOptMomentum: return launch_ar<kOptMomentum>(a, grid, s, phase);
     case kOptAdam: return launch_ar<kOptAdam>(a, grid, s, phase);
+    case kOptLars: return launch_lars(a, grid, s, phase);
     default: return cudaErrorInvalidValue;
   }
+}
+cudaError_t lars_norms(const LarsNormArgs& a, cudaStream_t s) {
+  if (a.world < 1 || a.world > kMaxRanks || a.nseg < 0 || a.nt < 0) return cudaErrorInvalidValue;
+  int grid = a.nseg < kSmCount * 4 ? a.nseg : kSmCount * 4;
+  if (grid < 1) grid = 1;
+  lars_norms_kernel<<<grid, kLarsNormThreads, 0, s>>>(a);
+  return cudaGetLastError();
 }
 cudaError_t set_flag_timeout_ns(unsigned long long ns) {
   return cudaMemcpyToSymbol(g_flag_timeout_ns, &ns, sizeof(ns));

@@ -8,6 +8,11 @@ CIFAR-10 network the reference actually trains.
 
   python examples/resnet/resnet_spark.py --cluster_size 8 --model resnet50 --batch_size 256 \
       --train_steps 100
+
+Large global batches: ``--optimizer lars`` (per-layer trust ratios, parallel/fused_optim.py) with
+a linear warm-up over ``--warmup_steps`` and polynomial decay to 0 at the last step
+(``resnet.poly_warmup_lr``), peaking at ``--base_lr`` (default: the linear-scaling rule
+0.1 * global batch / 256).
 """
 import argparse
 import os
@@ -29,6 +34,11 @@ def parse(argv):
   p.add_argument("--no_graph", action="store_true")
   p.add_argument("--tensorboard", action="store_true")
   p.add_argument("--metrics", default=None, help="JSONL file for per-step metrics")
+  p.add_argument("--optimizer", default="momentum", choices=["momentum", "lars"])
+  p.add_argument("--base_lr", type=float, default=None,
+                 help="peak learning rate (default: 0.1 * global batch / 256; resnet56: piecewise_lr)")
+  p.add_argument("--warmup_steps", type=int, default=0, help="lars: linear warm-up steps")
+  p.add_argument("--trust_coefficient", type=float, default=0.001, help="lars: eta")
   p.add_argument("--metrics_port", type=int, default=None,
                  help="serve the same fields on a Prometheus /metrics endpoint (port + rank; 0: any free port)")
   return p.parse_args(argv)
@@ -44,13 +54,18 @@ def main_fun(argv, ctx):
   torch.cuda.set_device(0)  # the node runtime made the assigned GPU device 0
   comm = ctx.gradient_comm() if ctx.world_size > 1 else None   # one host: P2P/NVLS kernels; several: NCCL
   B = args.batch_size
+  lars = args.optimizer == "lars"
   if args.model == "resnet56":
-    net = resnet.CifarResNetTrainer(depth=56, batch=B, device="cuda:0", comm=comm,
-                                    lr=resnet.piecewise_lr(0, B * ctx.world_size))
+    base_lr = args.base_lr if args.base_lr is not None else resnet.piecewise_lr(0, B * ctx.world_size)
+  else:
+    base_lr = args.base_lr if args.base_lr is not None else 0.1 * B * ctx.world_size / 256.0
+  opt = dict(optimizer=args.optimizer, trust_coefficient=args.trust_coefficient) if lars else {}
+  if args.model == "resnet56":
+    net = resnet.CifarResNetTrainer(depth=56, batch=B, device="cuda:0", comm=comm, lr=base_lr, **opt)
   else:
     depth = int(args.model.replace("resnet", ""))
     net = resnet.ResNetTrainer(depth=depth, batch=B, image=args.image or 224, device="cuda:0",
-                               comm=comm, lr=0.1 * B * ctx.world_size / 256.0)
+                               comm=comm, lr=base_lr, **opt)
   if comm is not None:
     comm.broadcast("weights", root=0)   # the chief's initial variables win
     comm.broadcast("aux32", root=0)
@@ -77,8 +92,11 @@ def main_fun(argv, ctx):
     events = summary.SummaryWriter(ctx.absolute_path(args.model_dir))
   torch.cuda.synchronize()
   t0 = time.time()
-  for step in range(start, start + args.train_steps):
-    if args.epochs_per_step:
+  total_steps = start + args.train_steps
+  for step in range(start, total_steps):
+    if lars:   # hyper-parameters live in device memory: this works under graph replay
+      net.set_lr(resnet.poly_warmup_lr(step, total_steps, base_lr, args.warmup_steps))
+    elif args.epochs_per_step:
       net.set_lr(resnet.piecewise_lr(int(step * args.epochs_per_step), B * ctx.world_size))
     fault.maybe_inject(ctx.rank, step)      # TFOS_FAULT_INJECT (resilience tests), no-op otherwise
     loss = net.train_step()

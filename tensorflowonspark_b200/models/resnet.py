@@ -43,7 +43,9 @@ class ResNetTrainer(object):
 
   def __init__(self, depth=50, batch=256, image=224, num_classes=1000, device="cuda:0",
                lr=0.1, momentum=0.9, weight_decay=1e-4, comm=None, training=True, seed=1234,
-               optimizer="momentum"):
+               optimizer="momentum", trust_coefficient=0.001):
+    """``optimizer``: sgd | momentum | adam | lars (``trust_coefficient`` is LARS's eta; see
+    parallel/fused_optim.py)."""
     assert depth in self.CFG, "bottleneck depths: 50/101/152"
     self.device = torch.device(device)
     self.B, self.image, self.num_classes, self.depth = batch, image, num_classes, depth
@@ -178,7 +180,8 @@ class ResNetTrainer(object):
       from ..parallel.fused_optim import FusedOptimizer
       buckets = self._comm_buckets() if (comm is not None and comm.world > 1) else None
       self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, momentum=momentum,
-                                  weight_decay=weight_decay, buckets=buckets)
+                                  weight_decay=weight_decay, buckets=buckets,
+                                  trust_coefficient=trust_coefficient)
     # opt-in (TFOS_WGRAD_STREAM=1): weight gradients on a side stream, concurrent with the BN
     # kernels (engine.py).  Off by default: the two kernel families co-reside on the SMs but
     # compete for the same L2 -> SM bandwidth.
@@ -651,7 +654,8 @@ class CifarResNetTrainer(object):
   momentum SGD, batch 128, weight decay 2e-4)."""
 
   def __init__(self, depth=56, batch=128, num_classes=10, device="cuda:0", lr=0.1, momentum=0.9,
-               weight_decay=2e-4, comm=None, seed=1234):
+               weight_decay=2e-4, comm=None, seed=1234, optimizer="momentum",
+               trust_coefficient=0.001):
     assert (depth - 2) % 6 == 0
     n = (depth - 2) // 6
     self.device = dev = torch.device(device)
@@ -713,8 +717,8 @@ class CifarResNetTrainer(object):
     self.correct = torch.zeros(1, dtype=torch.float32, device=dev)
     self.fc.build(self.avg, self.logits, self.dlogits, self.g_avg)
     from ..parallel.fused_optim import FusedOptimizer
-    self.optim = FusedOptimizer(st, comm=comm, opt="momentum", lr=lr, momentum=momentum,
-                                weight_decay=weight_decay)
+    self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, momentum=momentum,
+                                weight_decay=weight_decay, trust_coefficient=trust_coefficient)
     self.graph = None
     self.mean, self.std = [0.4914, 0.4822, 0.4465], [0.2470, 0.2435, 0.2616]
 
@@ -769,3 +773,15 @@ def piecewise_lr(epoch, batch_size, base=0.1, boundaries=(91, 136, 182), factors
     if epoch >= b:
       lr = base * batch_size / 128.0 * f
   return lr
+
+
+def poly_warmup_lr(step, total_steps, base_lr, warmup_steps, end_lr=0.0, power=2.0):
+  """Large-batch (LARS) schedule: linear warm-up from 0 to ``base_lr`` over ``warmup_steps``
+  steps (``step`` 0 .. ``warmup_steps - 1`` take ``base_lr * (step + 1) / warmup_steps``), then
+  polynomial decay ``end_lr + (base_lr - end_lr) * (1 - p) ** power``, where p runs from 0 at
+  ``step = warmup_steps`` to 1 at ``step = total_steps``."""
+  if step < warmup_steps:
+    return base_lr * (step + 1) / float(warmup_steps)
+  decay_steps = max(1, total_steps - warmup_steps)
+  p = min(1.0, float(step - warmup_steps) / decay_steps)
+  return end_lr + (base_lr - end_lr) * (1.0 - p) ** power

@@ -20,20 +20,92 @@ Across hosts (``comm`` is a parallel/group_comm.GroupComm) the peer loads are re
 form with scale 1 / world, replicated on every rank.  The collective is not recorded into a
 CUDA graph: while a trainer captures its step, ``finish()`` only notes that the update is due,
 and ``after_replay()`` - called by the trainers after every graph replay - runs it eagerly.
+
+LARS (``opt="lars"``) gives every adapted tensor - the decayed head: conv and dense weights -
+its own trust ratio ``eta * |w| / (|g| + wd * |w|)`` from the norms of its fp32 master and of
+its AVERAGED gradient, and runs momentum with lr * trust applied inside the velocity:
+``v = m v + lr trust (g + wd w); w = w - v``.  The non-decayed tail takes ``v = m v + lr g``.
+``state1`` holds that velocity (momentum's ``state1`` does not carry lr, so a momentum checkpoint
+does not continue under LARS).  The norms need the whole reduced tensor, so every bucket runs a
+separate, deterministic norm pass (csrc/optim_comm.cu ``lars_norms``) between the reduce-scatter
+and the update: ``[PHASE 1 ->] norms (+ exchange of per-tensor partials among the local peers)
+-> update [+ all-gather]``.  A bucket bound must not cut an adapted tensor.
 """
+import bisect
+
 import torch
 
 from .. import ops
 
-OPTS = {"sgd": 0, "momentum": 1, "adam": 2}
+OPTS = {"sgd": 0, "momentum": 1, "adam": 2, "lars": 3}
+# csrc/ops.h kLarsMaxTensors: adapted tensors one shard of a bucket may intersect
+LARS_MAX_TENSORS = 256
+# elements per work item of the LARS norm pass (one CTA reduces one segment at a time)
+LARS_SEGMENT = 16384
+
+
+def _shard(b, e, world, rank):
+  """[lo, hi) of ``rank``'s shard of bucket [b, e) - the arithmetic of allreduce_opt_kernel."""
+  n = e - b
+  chunk = ((n + world - 1) // world + 7) // 8 * 8
+  return b + min(n, chunk * rank), b + min(n, chunk * (rank + 1))
+
+
+def lars_tables(bounds, buckets, world, seg_len=LARS_SEGMENT):
+  """Work tables of the LARS norm pass.
+
+  ``bounds``: the adapted tensors tile ``[0, bounds[-1])`` (= ``decay_end``), tensor ``t`` being
+  ``[bounds[t], bounds[t + 1])``.  ``buckets``: ``(begin, end, ...)`` element ranges.  Returns,
+  per bucket and per rank, ``{"t0", "nt", "seg", "tseg"}``: the shard intersects tensors
+  ``t0 .. t0 + nt - 1``; ``seg`` lists ``(lo, hi)`` segments of at most ``seg_len`` elements, each
+  inside one tensor and the shard, tensor after tensor; ``tseg[j] .. tseg[j + 1]`` are local
+  tensor ``j``'s segments.  Raises ValueError when a bucket bound falls inside an adapted tensor
+  or a shard intersects more than LARS_MAX_TENSORS of them."""
+  assert seg_len % 8 == 0 and seg_len > 0
+  decay_end = bounds[-1]
+  starts = set(bounds)
+  out = []
+  for bi, bk in enumerate(buckets):
+    b, e = bk[0], bk[1]
+    for x in (b, e):
+      if 0 < x < decay_end and x not in starts:
+        raise ValueError("LARS: bucket {} bound {} falls inside an adapted tensor (each tensor's "
+                         "norm must come from one bucket)".format(bi, x))
+    per_rank = []
+    for r in range(world):
+      lo, hi = _shard(b, e, world, r)
+      ahi = min(hi, decay_end)
+      tab = {"t0": 0, "nt": 0, "seg": [], "tseg": [0]}
+      if lo < ahi:
+        t0 = bisect.bisect_right(bounds, lo) - 1
+        t1 = bisect.bisect_left(bounds, ahi)
+        if t1 - t0 > LARS_MAX_TENSORS:
+          raise ValueError("LARS: rank {}'s shard of bucket {} intersects {} adapted tensors; the "
+                           "update kernel holds at most {} (split the bucket)".format(
+                               r, bi, t1 - t0, LARS_MAX_TENSORS))
+        tab["t0"], tab["nt"] = t0, t1 - t0
+        for t in range(t0, t1):
+          s, stop = max(bounds[t], lo), min(bounds[t + 1], ahi)
+          while s < stop:
+            tab["seg"].append((s, min(stop, s + seg_len)))
+            s += seg_len
+          tab["tseg"].append(len(tab["seg"]))
+      per_rank.append(tab)
+    out.append(per_rank)
+  return out
 
 
 class FusedOptimizer(object):
 
   def __init__(self, store, comm=None, opt="momentum", lr=0.1, momentum=0.9, weight_decay=0.0,
-               beta1=0.9, beta2=0.999, eps=1e-7, buckets=None, grid=None):
+               beta1=0.9, beta2=0.999, eps=1e-7, buckets=None, grid=None, trust_coefficient=0.001):
+    """``trust_coefficient``: LARS eta (``opt="lars"``; it takes the slot of Adam's beta1 in
+    the hyper-parameter vector, which LARS does not use)."""
     self.store, self.comm = store, comm
     self.opt = OPTS[opt]
+    self.lars = self.opt == OPTS["lars"]
+    if self.lars:
+      beta1 = trust_coefficient
     dev = store.master.device
     self.device = dev
     # group mode: gradients travel through torch.distributed, the kernel sees a world of one
@@ -73,6 +145,9 @@ class FusedOptimizer(object):
     for b, e, _ in buckets:
       assert b % 8 == 0 and b < e <= n, "bucket bounds must be multiples of 8 inside the vector"
     self.buckets = list(buckets)
+    if self.lars:   # (validates the buckets before anything is allocated)
+      self._lars_bounds = [s["offset"] for s in store.order if s["decay"]] + [store.decay_end]
+      self._lars_tab = lars_tables(self._lars_bounds, self.buckets, self.world)
     self._args = []
     for slot, (b, e, tag) in enumerate(self.buckets):
       d = {
@@ -106,6 +181,8 @@ class FusedOptimizer(object):
           d["grid"] = grid or 48
       self._args.append(d)
     self.nvls = bool(self._args and self._args[0].get("grads_mc"))
+    if self.lars:
+      self._build_lars(store, comm)
     self._by_tag = {}
     for i, (_, _, tag) in enumerate(self.buckets):
       self._by_tag.setdefault(tag, []).append(i)
@@ -117,6 +194,42 @@ class FusedOptimizer(object):
       self._ev_ready = [torch.cuda.Event() for _ in self.buckets]
       self._ev_wait0 = torch.cuda.Event(enable_timing=True)
       self._ev_wait1 = torch.cuda.Event(enable_timing=True)
+
+  def _build_lars(self, store, comm):
+    """Device tables of the norm pass and the norms table: ``world`` rows of ``T`` entries
+    {sum g^2, sum w^2, 0, 0}, row r written by rank r (symmetric with peers, multicast on NVLS).
+    Entries of tensors outside a rank's shards stay 0, so every rank may sum all rows."""
+    dev = self.device
+    T = len(self._lars_bounds) - 1
+    n_norms = self.world * max(1, T) * 4
+    if comm is not None and self.world > 1:
+      self.lars_norms = comm.alloc("lars_norms", n_norms, torch.float32, multicast=self.nvls)
+      self.lars_norms.zero_()
+      norms = comm.peer_ptrs("lars_norms")
+      norms_mc = comm.mc_ptr("lars_norms") if self.nvls else 0
+    else:
+      self.lars_norms = torch.zeros(n_norms, dtype=torch.float32, device=dev)
+      norms, norms_mc = [self.lars_norms.data_ptr()], 0
+    self._lars_off = torch.tensor(self._lars_bounds, dtype=torch.int64, device=dev)
+    self._lars_bufs, self._lars_args, self._lars_phase = [], [], []
+    for i, d in enumerate(self._args):
+      tab = self._lars_tab[i][self.rank]
+      seg = torch.tensor([x for s in tab["seg"] for x in s] or [0, 0], dtype=torch.int64, device=dev)
+      tseg = torch.tensor(tab["tseg"], dtype=torch.int32, device=dev)
+      partial = torch.zeros(max(2, 2 * len(tab["seg"])), dtype=torch.float32, device=dev)
+      counter = torch.zeros(1, dtype=torch.int32, device=dev)
+      self._lars_bufs.append((seg, tseg, partial, counter))
+      d.update(lars_off=self._lars_off.data_ptr(), lars_norms=self.lars_norms.data_ptr(),
+               lars_t0=tab["t0"], lars_nt=tab["nt"], lars_T=T)
+      nd = {"grads": d["grads"][self.rank if self.world > 1 else 0], "master": store.master.data_ptr(),
+            "seg": seg.data_ptr(), "tseg": tseg.data_ptr(), "partial": partial.data_ptr(),
+            "nseg": len(tab["seg"]), "t0": tab["t0"], "nt": tab["nt"], "T": T,
+            "world": self.world, "rank": self.rank, "slot": i, "norms": norms,
+            "norms_mc": norms_mc, "block_counter": counter.data_ptr()}
+      if self.world > 1:
+        nd.update(flags=d["flags"], epoch=d["epoch"])
+      self._lars_args.append(nd)
+      self._lars_phase.append((dict(d, phase=1), dict(d, phase=2)))
 
   def set_lr(self, lr):
     self.hyper[0:1].fill_(float(lr))
@@ -206,6 +319,8 @@ class FusedOptimizer(object):
       self._run_bucket(i)
 
   def _run_bucket(self, i):
+    if self.lars:
+      return self._run_bucket_lars(i)
     if self.hier_mode:
       d = self._args[i]
       if self.world > 1:
@@ -219,6 +334,30 @@ class FusedOptimizer(object):
       b, e, _ = self.buckets[i]
       self.comm.all_reduce(self.store.grads[b:e])     # SUM; the kernel scales by 1 / world
     ops.K.allreduce_opt(self._args[i])
+
+  def _run_bucket_lars(self, i):
+    """reduce-scatter -> per-tensor norms (+ exchange among the local peers) -> update +
+    all-gather, all on the bucket's flag slot.  Without peers: norms -> one-pass update."""
+    phase1, phase2 = self._lars_phase[i]
+    if self.hier_mode:
+      if self.world > 1:
+        ops.K.allreduce_opt(phase1)
+      lo, hi = self.shard_bounds(i, self.rank)
+      if hi > lo:
+        self.comm.all_reduce_inter(self.store.grads[lo:hi])
+      ops.K.lars_norms(self._lars_args[i])
+      ops.K.allreduce_opt(phase2)
+      return
+    if self.group_mode:
+      b, e, _ = self.buckets[i]
+      self.comm.all_reduce(self.store.grads[b:e])
+    if self.world > 1:
+      ops.K.allreduce_opt(phase1)
+      ops.K.lars_norms(self._lars_args[i])
+      ops.K.allreduce_opt(phase2)
+    else:
+      ops.K.lars_norms(self._lars_args[i])
+      ops.K.allreduce_opt(self._args[i])
 
   def _capturing_group(self):
     return ((self.group_mode or self.hier_mode) and self.device.type == "cuda"
