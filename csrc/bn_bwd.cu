@@ -14,7 +14,6 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "ops.h"
 #include "ptx.cuh"
@@ -355,11 +354,10 @@ inline dim3 red_grid(long long P, int C, int waves) {
   return dim3(static_cast<unsigned>(bx), static_cast<unsigned>(gy));
 }
 
-// grid = resident blocks per SM (launch bounds: 2) x kSmCount SMs x waves; tunable for experiments
-inline int env_waves(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return v != nullptr && atoi(v) > 0 ? atoi(v) : dflt;
-}
+// grid = resident blocks per SM (launch bounds: 2) x kSmCount SMs x waves
+constexpr int kWavesFwd = 3;
+constexpr int kWavesReduce = 2;
+constexpr int kWavesApply = 2;
 
 }  // namespace
 
@@ -367,8 +365,7 @@ void bn_set_row_reverse(int flag) { g_row_reverse = flag ? 1 : 0; }
 
 cudaError_t bn_apply(const void* x, const void* residual, const float* scale, const float* shift,
                      void* y, uint8_t* mask, long long P, int C, int act, cudaStream_t s) {
-  static const int waves = env_waves("TFOS_BN_WAVES_FWD", 3);
-  bn_fwd_apply_kernel<false><<<red_grid(P, C, waves), kThreads, 0, s>>>(
+  bn_fwd_apply_kernel<false><<<red_grid(P, C, kWavesFwd), kThreads, 0, s>>>(
       static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(residual), scale,
       shift, static_cast<__nv_bfloat16*>(y), mask, P, C, act, BnFinalize(), g_row_reverse);
   return cudaGetLastError();
@@ -376,8 +373,7 @@ cudaError_t bn_apply(const void* x, const void* residual, const float* scale, co
 
 cudaError_t bn_apply_finalize(const void* x, const void* residual, void* y, uint8_t* mask,
                               long long P, int C, int act, const BnFinalize& fin, cudaStream_t s) {
-  static const int waves = env_waves("TFOS_BN_WAVES_FWD", 3);
-  bn_fwd_apply_kernel<true><<<red_grid(P, C, waves), kThreads, 0, s>>>(
+  bn_fwd_apply_kernel<true><<<red_grid(P, C, kWavesFwd), kThreads, 0, s>>>(
       static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(residual), nullptr,
       nullptr, static_cast<__nv_bfloat16*>(y), mask, P, C, act, fin, g_row_reverse);
   return cudaGetLastError();
@@ -387,8 +383,7 @@ cudaError_t bn_bwd_reduce(const void* dy, const void* x, const void* y, const fl
                           const float* invstd, const float* fscale, const float* fshift,
                           long long P, int C, int relu, float* dgamma, float* dbeta,
                           cudaStream_t s) {
-  static const int waves = env_waves("TFOS_BN_WAVES_REDUCE", 2);
-  bn_bwd_reduce_kernel<<<red_grid(P, C, waves), kThreads, 0, s>>>(
+  bn_bwd_reduce_kernel<<<red_grid(P, C, kWavesReduce), kThreads, 0, s>>>(
       static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x),
       static_cast<const __nv_bfloat16*>(y), mean, invstd, fscale, fshift, P, C, relu, dgamma,
       dbeta, g_row_reverse);
@@ -400,8 +395,7 @@ cudaError_t bn_bwd_apply(const void* dy, const void* x, const void* y, const flo
                          float* dbeta, const float* fscale, const float* fshift, void* dx,
                          void* dres, long long P, int C, int relu, const float* sum_g,
                          const float* sum_gx, cudaStream_t s) {
-  static const int waves = env_waves("TFOS_BN_WAVES_APPLY", 2);
-  bn_bwd_apply_kernel<<<red_grid(P, C, waves), kThreads, 0, s>>>(
+  bn_bwd_apply_kernel<<<red_grid(P, C, kWavesApply), kThreads, 0, s>>>(
       static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x),
       static_cast<const __nv_bfloat16*>(y), gamma, mean, invstd, dgamma, dbeta, fscale, fshift,
       static_cast<__nv_bfloat16*>(dx), static_cast<__nv_bfloat16*>(dres), P, C, relu,

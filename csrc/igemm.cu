@@ -822,10 +822,6 @@ IGemmPlan* igemm_plan_fwd(const TmapDesc& a, const TmapDesc& b, const FwdArgs& a
   // tile list (grid multiple of n_tiles) and run several tiles so that the B load amortises
   p->fa.b_resident = 0;
   p->fa.a_stages = 0;
-  static const bool allow_resident = [] {
-    const char* e = getenv("TFOS_B_RESIDENT");
-    return e == nullptr || atoi(e) != 0;
-  }();
   const int k_iters = args.num_taps * args.k_chunks;
   // the ring of the instance this plan runs (the prefetch instances have fewer stages)
   const long long ring_bytes =
@@ -840,7 +836,7 @@ IGemmPlan* igemm_plan_fwd(const TmapDesc& a, const TmapDesc& b, const FwdArgs& a
     }
     p->fa.b_resident = 1;
     p->fa.a_stages = static_cast<int>((ring_bytes - b_bytes) / kStemStage);
-  } else if (allow_resident && args.n_tiles <= 8 && p->total_work >= 2 * num_sms &&
+  } else if (args.n_tiles <= 8 && p->total_work >= 2 * num_sms &&
       b_bytes + kMinAStages * kABytes <= ring_bytes) {
     const int grid = num_sms - num_sms % args.n_tiles;
     if (grid > 0) {

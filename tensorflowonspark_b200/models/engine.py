@@ -114,36 +114,11 @@ def normal(std):
   return lambda shape, gen: torch.randn(shape, generator=gen) * std
 
 
-# Weight gradients are needed by nobody until the optimizer runs, read only buffers that the rest
-# of the backward pass never rewrites, and are bound by the L2 -> SM fabric (profiles/): issued on
-# a side stream they overlap the HBM-bound batch-norm kernels of the layers below instead of
-# standing in the critical path.  A trainer opts in with set_wgrad_stream(); the optimizer joins
-# the stream before it consumes the gradients (FusedOptimizer.add_producer_stream).
-_wgrad_stream = None
-
-
-def set_wgrad_stream(stream):
-  global _wgrad_stream
-  _wgrad_stream = stream
-
-
 def _run_wgrad(layer):
-  """wgrad (+ bias gradient) of a Conv / Dense layer, on the side stream when one is set."""
-  def body():
-    layer.wgrad.run()
-    if layer.sbias is not None:
-      ops.K.colsum(layer.dy, layer.store.g(layer.sbias))
-  side = _wgrad_stream
-  if side is None:
-    return body()
-  main = torch.cuda.current_stream(side.device)
-  ev = getattr(layer, "_ev_dy", None)
-  if ev is None:
-    ev = layer._ev_dy = torch.cuda.Event()
-  ev.record(main)          # dy (and this step's zeroed gradient buffer) are final here
-  side.wait_event(ev)
-  with torch.cuda.stream(side):
-    body()
+  """wgrad (+ bias gradient) of a Conv / Dense layer."""
+  layer.wgrad.run()
+  if layer.sbias is not None:
+    ops.K.colsum(layer.dy, layer.store.g(layer.sbias))
 
 
 class StatsArena(object):
@@ -230,7 +205,7 @@ class BatchNorm(object):
   def stats(self):
     return (self.sum, self.sumsq)
 
-  def forward(self, x_raw, y, residual=None, act=1, training=True, fused_stats=True, rev=False):
+  def forward(self, x_raw, y, residual=None, act=1, training=True, rev=False):
     """``rev``: walk the rows last-to-first.  The convolution that produced ``x_raw`` wrote its
     tiles first-to-last, so the END of the tensor is what the 50 MB L2 still holds; the apply
     kernel then finishes at the START of ``y``, which is where the next convolution begins."""
@@ -245,15 +220,13 @@ class BatchNorm(object):
       self.mask = self.ensure_mask(x_raw.numel(), x_raw.device)
     else:
       self.mask = None
-    if training and fused_stats and getattr(self, "arena", None) is not None:
+    if training and getattr(self, "arena", None) is not None:
       ops.K.bn_apply_finalize(x_raw, residual, y, act, self.mask, self.sum, self.sumsq, self.gamma,
                               self.beta, self.running_mean, self.running_var, self.mean,
                               self.invstd, self.scale, self.shift, float(count), self.eps,
                               self.momentum)
       return
     if training:
-      if not fused_stats:
-        ops.K.bn_stats(x_raw, self.sum, self.sumsq)
       ops.K.bn_finalize(self.sum, self.sumsq, self.gamma, self.beta, self.running_mean,
                         self.running_var, self.mean, self.invstd, self.scale, self.shift,
                         float(count), self.eps, self.momentum)

@@ -85,25 +85,20 @@ class ResNetTrainer(object):
     self.xp = _buf((B, image, Wp, 8), dev)
     self.labels = torch.zeros(B, dtype=torch.int32, device=dev)
     self.stem_raw = _buf((B, OH, OW, 64), dev)
-    self.stem_act = None   # allocated below unless the fused stem tail makes it unnecessary
     PH, PW = (OH + 2 - 3) // 2 + 1, (OW + 2 - 3) // 2 + 1
     self.pool = _buf((B, PH, PW, 64), dev)
     self.pool_idx = _buf((B, PH, PW, 64), dev, torch.uint8)
     tr = training
     # all batch-norm statistics accumulators live in one arena that is zeroed once per step;
     # finalisation is folded into the apply kernels (engine.BatchNorm.build)
-    self.stats_arena = engine.StatsArena(dev) if (tr and dev.type == "cuda" and os.environ.get(
-        "TFOS_BN_FUSED_FINALIZE", "1") != "0") else None
+    self.stats_arena = engine.StatsArena(dev) if tr else None
     self.running = engine.RunningArena(dev)   # all BN running statistics, one flat buffer
     self.stem_bn.build(dev, self.stats_arena, self.running)
-    self.fuse_stem = (tr and self.stats_arena is not None and dev.type == "cuda"
-                      and os.environ.get("TFOS_FUSE_STEM", "1") != "0")
-    if not self.fuse_stem:
-      self.stem_act = _buf((B, OH, OW, 64), dev)
+    # training fuses the stem's BN + ReLU + max pool (_forward): the activation is never stored
+    self.stem_act = None if tr else _buf((B, OH, OW, 64), dev)
     self.p_stem = igemm.stem_fprop(self.xp, st.w(self.stem_w), self.stem_raw,
                                    stats=self.stem_bn.stats if tr else None)
     if tr:
-      self.g_stem_act = None if self.fuse_stem else _buf((B, OH, OW, 64), dev)
       self.g_stem_raw = _buf((B, OH, OW, 64), dev)
       self.p_stem_wgrad = igemm.stem_wgrad(self.g_stem_raw, self.xp, st.g(self.stem_w))
 
@@ -135,15 +130,14 @@ class ResNetTrainer(object):
       # the block output's ReLU mask (one bit per element, written by bn3's forward): identity
       # blocks fold "mask * dY" into conv1's accumulating dgrad instead of materialising it
       omask = b.u3.bn.ensure_mask(b.out.numel(), dev) if tr else None
-      # Fused batch-norm backward reductions (TFOS_BN_FUSED_REDUCE=0 disables): the data gradient
-      # that WRITES a batch norm's dy also accumulates that batch norm's sum(g), sum(g x):
+      # Fused batch-norm backward reductions: the data gradient that WRITES a batch norm's dy
+      # also accumulates that batch norm's sum(g), sum(g x):
       #   conv3.dgrad -> g_a2 = dy of bn2        conv2.dgrad -> g_a1 = dy of bn1
       #   identity block: conv1.dgrad (accumulating) completes g_x = dy of the PREVIOUS block's bn3
-      fr = tr and self.stats_arena is not None and os.environ.get("TFOS_BN_FUSED_REDUCE", "1") != "0"
-      red1 = (b.u1.bn, b.r1, b.u1.bn.ensure_mask(b.a1.numel(), dev)) if fr else None
-      red2 = (b.u2.bn, b.r2, b.u2.bn.ensure_mask(b.a2.numel(), dev)) if fr else None
+      red1 = (b.u1.bn, b.r1, b.u1.bn.ensure_mask(b.a1.numel(), dev)) if tr else None
+      red2 = (b.u2.bn, b.r2, b.u2.bn.ensure_mask(b.a2.numel(), dev)) if tr else None
       redp = None
-      if fr and ident and prev_block is not None:
+      if tr and ident and prev_block is not None:
         redp = (prev_block.u3.bn, prev_block.r3, prev_block.u3.bn.ensure_mask(
             prev_block.out.numel(), dev))
       b.u1.conv.build(x, b.r1, b.g_r1, b.g_x, stats=b.u1.bn.stats, dx_accumulate=ident,
@@ -182,20 +176,13 @@ class ResNetTrainer(object):
       self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, momentum=momentum,
                                   weight_decay=weight_decay, buckets=buckets,
                                   trust_coefficient=trust_coefficient)
-    # opt-in (TFOS_WGRAD_STREAM=1): weight gradients on a side stream, concurrent with the BN
-    # kernels (engine.py).  Off by default: the two kernel families co-reside on the SMs but
-    # compete for the same L2 -> SM bandwidth.
-    self.wg_stream = None
-    if tr and dev.type == "cuda" and os.environ.get("TFOS_WGRAD_STREAM", "0") == "1":
-      self.wg_stream = torch.cuda.Stream(device=dev)
-      self.optim.add_producer_stream(self.wg_stream)
     self.graph = None
     self.mean = [0.485, 0.456, 0.406]
     self.std = [0.229, 0.224, 0.225]
     self._assign_directions()
 
   def _assign_directions(self):
-    """L2 hand-over ("serpentine") schedule, TFOS_L2_SERPENTINE=0 disables it.
+    """L2 hand-over ("serpentine") schedule.
 
     Activations are 13 - 411 MB per tensor at batch 256, the L2 holds 50 MB: a kernel that walks
     a tensor front to back leaves its TAIL in L2.  Every memory-bound kernel of the chain
@@ -203,17 +190,15 @@ class ResNetTrainer(object):
       forward   conv (tiles ascending) -> BN apply (rows descending) -> next conv (ascending) ...
       backward  BN reduce (d) -> BN apply (not d) -> the unit's dgrad (d) -> next unit (not d) ...
     Only the ORDER in which tiles / rows are visited changes; results are identical."""
-    self.serpentine = self.device.type == "cuda" and os.environ.get("TFOS_L2_SERPENTINE", "1") == "1"
     d = False
     for b in reversed(self.blocks):
       for u in (b.u3, b.u2, b.u1):
-        u.rev = (d, not d) if self.serpentine else (False, False)
-        if self.serpentine and u.conv.dgrad is not None:
+        u.rev = (d, not d)
+        if u.conv.dgrad is not None:
           u.conv.dgrad.set_reverse(d)
         d = not d
       if b.ds is not None:
-        b.ds.rev = (False, True) if self.serpentine else (False, False)
-    self.stem_rev = (d, not d) if self.serpentine else (False, False)
+        b.ds.rev = (False, True)
 
   def _comm_buckets(self):
     """Gradient buckets for overlapping the fused all-reduce with backward: (begin, end, tag)
@@ -299,8 +284,7 @@ class ResNetTrainer(object):
       self.stats_arena.zero()   # the fused conv epilogues accumulate from zero every pass
     K.decode_normalize(self.in_u8, self.xp, igemm.STEM_PAD, self.mean, self.std)
     (self.p_stem_remote if remote else self.p_stem).run()
-    rv = self.serpentine
-    if training and self.fuse_stem:
+    if training:
       # BN + ReLU + max pool in one pass over the raw conv output (csrc/stem_fused.cu): the
       # 411 MB stem activation is never written
       bn = self.stem_bn
@@ -314,15 +298,15 @@ class ResNetTrainer(object):
     for b in self.blocks:
       for u, raw, act in ((b.u1, b.r1, b.a1), (b.u2, b.r2, b.a2)):
         run(u.conv)
-        u.bn.forward(raw, act, None, 1, training, rev=rv)
+        u.bn.forward(raw, act, None, 1, training, rev=True)
       run(b.u3.conv)
       if b.ds is not None:
         run(b.ds.conv)
-        b.ds.bn.forward(b.rd, b.idn, None, 0, training, rev=rv)
+        b.ds.bn.forward(b.rd, b.idn, None, 0, training, rev=True)
         idn = b.idn
       else:
         idn = b.x
-      b.u3.bn.forward(b.r3, b.out, idn, 1, training, rev=rv)
+      b.u3.bn.forward(b.r3, b.out, idn, 1, training, rev=True)
     K.avgpool_fwd(self.last, self.avg)
     run(self.fc)
 
@@ -336,13 +320,6 @@ class ResNetTrainer(object):
   def _backward(self):
     K = ops.K
     self.optim.zero_grads()
-    engine.set_wgrad_stream(self.wg_stream)
-    try:
-      self._backward_layers(K)
-    finally:
-      engine.set_wgrad_stream(None)
-
-  def _backward_layers(self, K):
     self.fc.backward()
     K.avgpool_bwd(self.g_avg, self.g_last)
     for bi in reversed(range(len(self.blocks))):
@@ -359,17 +336,12 @@ class ResNetTrainer(object):
         b.ds.bn.backward(b.g_out, b.rd, None, b.g_rd, relu=True, mask=b.u3.bn.mask, rev=b.ds.rev)
         b.ds.conv.backward()  # accumulates into g_x
       self.optim.launch(bi)   # buckets that became final start their all-reduce now
-    if self.fuse_stem:
-      # max-pool backward recomputed inside the BN reduction and the BN apply: the gradient of
-      # the stem activation (411 MB) is never written or read
-      bn = self.stem_bn
-      K.stem_pool_bn_bwd(self.g_pool, self.pool_idx, self.stem_raw, bn.gamma, bn.mean, bn.invstd,
-                         bn.scale, bn.shift, bn.dgamma, bn.dbeta, self.g_stem_raw)
-      ops.count()   # two launches
-    else:
-      K.maxpool_bwd(self.g_pool, self.pool_idx, self.g_stem_act, 3, 2, 1)
-      self.stem_bn.backward(self.g_stem_act, self.stem_raw, self.stem_act, self.g_stem_raw,
-                            relu=True, rev=self.stem_rev)
+    # max-pool backward recomputed inside the BN reduction and the BN apply: the gradient of the
+    # stem activation (411 MB) is never written or read
+    bn = self.stem_bn
+    K.stem_pool_bn_bwd(self.g_pool, self.pool_idx, self.stem_raw, bn.gamma, bn.mean, bn.invstd,
+                       bn.scale, bn.shift, bn.dgamma, bn.dbeta, self.g_stem_raw)
+    ops.count()   # two launches
     self.p_stem_wgrad.run()
 
   # ------------------------------------------------------------------ API

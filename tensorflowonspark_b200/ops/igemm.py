@@ -12,30 +12,17 @@ Layout conventions (all bf16 unless noted):
 These replace the cuDNN/cuBLAS calls the reference reaches through TensorFlow
 (SURVEY.md section 2.6(b)).
 """
-import os
-
 from .. import _build
 
 BLOCK_M = 128
 BLOCK_K = 64
 _launches = 0
-# weight-gradient tiling knobs (tools/bench_igemm.py sweeps them)
-_WGRAD_WIDE = os.environ.get("TFOS_WGRAD_WIDE", "1") == "1"
-_WGRAD_WIDE_MIN_PIXELS = int(os.environ.get("TFOS_WGRAD_WIDE_MIN_PIXELS", "32768"))
-# work items of the one-pass 3x3 plan (_wgrad3x3_onepass_plan); 0: one wave.  The generic kernel
-# splits its pixels evenly over the SMs (_wgrad_slices) and has no such knob.
-_WGRAD_WORK = int(os.environ.get("TFOS_WGRAD_WORK", "0"))
-_STEM_HALO = os.environ.get("TFOS_STEM_HALO", "1") == "1"
+# 128 x 256-tile weight gradients from this many pixels on (_wgrad_plan)
+_WGRAD_WIDE_MIN_PIXELS = 32768
 # 3x3 / stride 1 weight gradients with 64-channel multiples: all nine taps from one pass over the
 # pixels (_wgrad3x3_onepass_plan) once the layer has this many output pixels
-_WGRAD_HALO = os.environ.get("TFOS_WGRAD_HALO", "1") == "1"
-_WGRAD_HALO_MIN_PIXELS = int(os.environ.get("TFOS_WGRAD_HALO_MIN_PIXELS", "8192"))
+_WGRAD_HALO_MIN_PIXELS = 8192
 _SMS = 132   # H100 SXM; the halo kernels' work-item counts below are multiples of it
-_STEM_SPLITS = int(os.environ.get("TFOS_STEM_SPLITS", str(_SMS)))
-# data gradients with an accumulate / fused-BN-reduction epilogue prefetch the operands that
-# epilogue reads into shared memory during the main loop (csrc/igemm.cu); 0 reads them in the
-# copy-out pass instead
-_DGRAD_EPI_PREFETCH = os.environ.get("TFOS_DGRAD_EPI_PREFETCH", "1") == "1"
 
 
 def launch_count():
@@ -178,7 +165,6 @@ def gemm(a, b, out, b_layout="nk", bias=None, relu=False, accumulate=False, stat
       "ldo": out.shape[1], "n_valid": N, "relu": int(relu),
       "out_fp32": int(out.dtype == torch.float32), "accumulate": int(accumulate),
       "bias": bias.data_ptr() if bias is not None else 0, "out": out.data_ptr(),
-      "epi_prefetch": int(_DGRAD_EPI_PREFETCH),   # 'kn' + accumulate: see conv_dgrad
   }
   _stats_args(g, stats)
   h = _C().igemm_plan_fwd(ta, tb, g, bn, b_layout == "kn")
@@ -230,7 +216,7 @@ def conv_fprop(x, w, y, stride=1, pad=0, bias=None, relu=False, stats=None, accu
 
 
 def conv_dgrad(dy, w, dx, stride=1, pad=0, accumulate=False, relu=False, bias=None, stats=None,
-               acc_mask=None, bn_reduce=None, epi_prefetch=None):
+               acc_mask=None, bn_reduce=None, epi_prefetch=True):
   """dx[N,H,W,Cin] (=|+=) conv_transpose(dy[N,OH,OW,Cout], w[Cout,R,S,Cin]).
 
   Also the forward of a transposed convolution (Keras Conv2DTranspose) when
@@ -245,11 +231,9 @@ def conv_dgrad(dy, w, dx, stride=1, pad=0, accumulate=False, relu=False, bias=No
 
   ``epi_prefetch``: whether the accumulate / ``bn_reduce`` epilogue prefetches the values it reads
   into shared memory while the main loop runs (False: it loads them in the copy-out pass).  Both
-  give the same dx bit for bit.  None: on unless TFOS_DGRAD_EPI_PREFETCH=0.  The plan falls back
-  to the loads in the copy-out pass where it cannot prefetch (``Plan.info()``: ``epi_prefetch``).
+  give the same dx bit for bit.  The plan falls back to the loads in the copy-out pass where it
+  cannot prefetch (``Plan.info()``: ``epi_prefetch``).
   """
-  if epi_prefetch is None:
-    epi_prefetch = _DGRAD_EPI_PREFETCH
   N, OH, OW, Cout = dy.shape
   _, R, S, Cin = w.shape
   _, H, W, _ = dx.shape
@@ -298,19 +282,17 @@ def conv_dgrad(dy, w, dx, stride=1, pad=0, accumulate=False, relu=False, bias=No
                                                       " +bnred" if bn_reduce is not None else ""))
 
 
-def _wgrad_plan(dy, dy_whn, Cout, x, x_whn, Cin, dw, ldw, taps, mul, es, box=None, c_box_b=None,
-                tap_dc=None, tap_out=None, n_valid=None):
+def _wgrad_plan(dy, dy_whn, Cout, x, x_whn, Cin, dw, ldw, taps, mul, es, box=None):
   OW, OH, N = dy_whn
-  n_valid = Cin if n_valid is None else n_valid
   # 128 x 256 tile per CTA (wgmma N = 256): fewer operand bytes per MAC than 128 x 128; it only
   # pays when both channel counts fill the tile and there are enough pixels to split over
-  wide = (_WGRAD_WIDE and Cout % 256 == 0 and n_valid % 256 == 0 and es == 1 and c_box_b is None
+  wide = (Cout % 256 == 0 and Cin % 256 == 0 and es == 1
           and OW * OH * N >= _WGRAD_WIDE_MIN_PIXELS)
   if box is None:
     box = choose_box(OW, OH, N, multiple_of=16, allow_pad=True)
   bw, bh, bnn, tw, th, tn = box
   assert (bw * bh * bnn) % 16 == 0 and bw * bh * bnn <= 128
-  bn = 64 if n_valid <= 64 else 128
+  bn = 64 if Cin <= 64 else 128
   if wide:
     bn = 256
   ta = _tmap4(dy, dy_whn, Cout, (bw, bh, bnn))
@@ -318,15 +300,14 @@ def _wgrad_plan(dy, dy_whn, Cout, x, x_whn, Cin, dw, ldw, taps, mul, es, box=Non
     tb = _tmap4(x, x_whn, Cin, (bw, bh, bnn))
   else:
     tb = _tmap4(x, x_whn, Cin, (bw * es, bh * es, bnn), es=(es, es, 1))
-  m_tiles, n_tiles = -(-Cout // 128), -(-n_valid // bn)
+  m_tiles, n_tiles = -(-Cout // 128), -(-Cin // bn)
   g = {
       "tiles_w": tw, "tiles_h": th, "tiles_n": tn, "box_w": bw, "box_h": bh, "box_n": bnn,
       "mul_w": mul, "mul_h": mul, "num_taps": len(taps),
       "tap_dw": [t[0] for t in taps], "tap_dh": [t[1] for t in taps],
-      "tap_dc": tap_dc if tap_dc is not None else [0] * len(taps),
-      "tap_out": tap_out if tap_out is not None else [t[2] for t in taps],
+      "tap_out": [t[2] for t in taps],
       "m_tiles": m_tiles, "n_tiles": n_tiles,
-      "m_valid": Cout, "n_valid": n_valid, "ldw": ldw, "dw": dw.data_ptr(),
+      "m_valid": Cout, "n_valid": Cin, "ldw": ldw, "dw": dw.data_ptr(),
   }
   h = _C().igemm_plan_wgrad(ta, tb, g, bn)
   return Plan([h], (dy, x, dw), "wgrad{} {}->{} taps{} {}".format(
@@ -409,7 +390,7 @@ def _wgrad3x3_onepass_plan(dy, x, dw):
   pairs = (Cout // 64) * (Cin // 64)
   total_boxes = tw * th * tn
   # one wave of work items: two waves measured 3-10 % slower (twice the fp32 atomics of dW)
-  k_splits = max(1, min((_WGRAD_WORK or _SMS) // pairs, total_boxes // 2))
+  k_splits = max(1, min(_SMS // pairs, total_boxes // 2))
   g = {
       "tiles_w": tw, "tiles_h": th, "tiles_n": tn, "box_w": 8, "box_h": bh, "box_n": bn,
       "num_taps": 1, "stem": 2,
@@ -433,7 +414,7 @@ def conv_wgrad(dy, x, dw, stride=1, pad=0):
   _, R, S, _ = dw.shape
   if R == 1 and S == 1 and stride == 1 and pad == 0:
     return gemm_wgrad(dy.view(-1, Cout), x.view(-1, Cin), dw.view(Cout, Cin))
-  if (_WGRAD_HALO and R == 3 and S == 3 and stride == 1 and pad == 1 and Cin % 64 == 0
+  if (R == 3 and S == 3 and stride == 1 and pad == 1 and Cin % 64 == 0
       and Cout % 64 == 0 and N * OH * OW >= _WGRAD_HALO_MIN_PIXELS):
     return _wgrad3x3_onepass_plan(dy, x, dw)
   taps = [(s - pad, r - pad, (r * S + s) * Cin) for r in range(R) for s in range(S)]
@@ -458,17 +439,6 @@ def stem_geometry(H, W):
   return OH, OW, Wp
 
 
-def _stem_tmap(xp, N, H, Wp, OW, box, es_h):
-  bw, bh, bnn = box
-  return {
-      "base": xp.data_ptr(),
-      "dims": [64, OW, H, N],
-      "strides": [2 * STEM_CP * 2, Wp * STEM_CP * 2, H * Wp * STEM_CP * 2],
-      "box": [64, bw, bh * es_h, bnn],
-      "elem_strides": [1, 1, es_h, 1],
-  }
-
-
 def _stem_halo_tmap(xp, N, H, Wp, OW, bw, rows):
   """Window-row view of xp with input rows at stride 1: one box = bw window columns x rows."""
   return {
@@ -484,77 +454,51 @@ def stem_fprop(xp, w, y, bias=None, relu=False, stats=None):
   N, H, Wp, _ = xp.shape
   Cout = w.shape[0]
   _, OH, OW, _ = y.shape
-  bn = _bn_for(Cout)
-  if Cout <= 64 and _STEM_HALO:
-    # halo mode (csrc/igemm.cu "stem mode"): 8 x 16 output pixels per tile, one 8 x 37 box of
-    # input rows serves all seven filter rows, the packed filter stays resident in smem
-    ta = _stem_halo_tmap(xp, N, H, Wp, OW, 8, 2 * 16 + 5)
-    tb = _tmap2(w, Cout, 7 * 64, bn)
-    g = {
-        "tiles_w": -(-OW // 8), "tiles_h": -(-OH // 16), "tiles_n": N, "n_tiles": 1,
-        "box_w": 8, "box_h": 16, "box_n": 1, "mul_w": 1, "mul_h": 2,
-        "num_taps": 7, "k_chunks": 1, "stem": 1,
-        "tap_dw": [0] * 7, "tap_dh": [-STEM_PAD] * 7, "tap_bk": [r * 64 for r in range(7)],
-        "lim_w": OW, "lim_h": OH, "lim_n": N, "OW": OW, "OH": OH,
-        "ldo": Cout, "n_valid": Cout, "relu": int(relu),
-        "bias": bias.data_ptr() if bias is not None else 0, "out": y.data_ptr(),
-    }
-    _stats_args(g, stats)
-    h = _C().igemm_plan_fwd(ta, tb, g, bn, False)
-    return Plan([h], (xp, w, y, bias, stats), "stem fprop (halo)")
-  bw, bh, bnn, tw, th, tn = choose_box(OW, OH, N)
-  ta = _stem_tmap(xp, N, H, Wp, OW, (bw, bh, bnn), 2)
-  tb = _tmap2(w, Cout, 7 * 64, bn)
+  if Cout > 64:
+    raise ValueError("stem_fprop: Cout {} > 64 (the stem kernel computes one 64-channel tile)"
+                     .format(Cout))
+  # halo mode (csrc/igemm.cu "stem mode"): 8 x 16 output pixels per tile, one 8 x 37 box of
+  # input rows serves all seven filter rows, the packed filter stays resident in smem
+  ta = _stem_halo_tmap(xp, N, H, Wp, OW, 8, 2 * 16 + 5)
+  tb = _tmap2(w, Cout, 7 * 64, 64)
   g = {
-      "tiles_w": tw, "tiles_h": th, "tiles_n": tn, "n_tiles": -(-Cout // bn),
-      "box_w": bw, "box_h": bh, "box_n": bnn, "mul_w": 1, "mul_h": 2,
-      "num_taps": 7, "k_chunks": 1,
-      "tap_dw": [0] * 7, "tap_dh": [r - STEM_PAD for r in range(7)],
-      "tap_bk": [r * 64 for r in range(7)],
+      "tiles_w": -(-OW // 8), "tiles_h": -(-OH // 16), "tiles_n": N, "n_tiles": 1,
+      "box_w": 8, "box_h": 16, "box_n": 1, "mul_w": 1, "mul_h": 2,
+      "num_taps": 7, "k_chunks": 1, "stem": 1,
+      "tap_dw": [0] * 7, "tap_dh": [-STEM_PAD] * 7, "tap_bk": [r * 64 for r in range(7)],
       "lim_w": OW, "lim_h": OH, "lim_n": N, "OW": OW, "OH": OH,
       "ldo": Cout, "n_valid": Cout, "relu": int(relu),
       "bias": bias.data_ptr() if bias is not None else 0, "out": y.data_ptr(),
   }
   _stats_args(g, stats)
-  h = _C().igemm_plan_fwd(ta, tb, g, bn, False)
-  return Plan([h], (xp, w, y, bias, stats), "stem fprop")
+  h = _C().igemm_plan_fwd(ta, tb, g, 64, False)
+  return Plan([h], (xp, w, y, bias, stats), "stem fprop (halo)")
 
 
 def stem_wgrad(dy, xp, dw):
   """dw [Cout, 7, 64] fp32 += dy[N,OH,OW,Cout]^T windows(xp)."""
   N, OH, OW, Cout = dy.shape
   _, H, Wp, _ = xp.shape
-  if Cout <= 64 and _STEM_HALO:
-    # all seven filter rows from one 16 x 21 halo box per 16 x 8 output pixels
-    # (csrc/igemm_wgrad.cu igemm_wgrad_halo_kernel)
-    ta = _tmap4(dy, (OW, OH, N), Cout, (16, 8, 1))
-    tb = _stem_halo_tmap(xp, N, H, Wp, OW, 16, 2 * 8 + 5)
-    tw, th = -(-OW // 16), -(-OH // 8)
-    g = {
-        "tiles_w": tw, "tiles_h": th, "tiles_n": N, "box_w": 16, "box_h": 8, "box_n": 1,
-        "num_taps": 1, "stem": 1,
-        "halo_boxes": 1, "box_dw": [0], "halo_rows": 2 * 8 + 5, "halo_hmul": 2,
-        "halo_h0": -STEM_PAD, "halo_jrow": [2 * j for j in range(8)], "halo_rowbytes": 2048,
-        "halo_nacc": 7,
-        "acc_box": [0] * 7, "acc_row": list(range(7)), "tap_out": [r * 64 for r in range(7)],
-        "m_tiles": 1, "n_tiles": 1, "k_splits": max(1, min(_STEM_SPLITS, tw * th * N)),
-        "m_valid": Cout, "n_valid": 64, "ldw": 7 * 64, "dw": dw.data_ptr(),
-    }
-    h = _C().igemm_plan_wgrad(ta, tb, g, 64)
-    return Plan([h], (dy, xp, dw), "stem wgrad (halo)")
-  bw, bh, bnn, tw, th, tn = choose_box(OW, OH, N, multiple_of=16, allow_pad=True)
-  ta = _tmap4(dy, (OW, OH, N), Cout, (bw, bh, bnn))
-  tb = _stem_tmap(xp, N, H, Wp, OW, (bw, bh, bnn), 2)
+  if Cout > 64:
+    raise ValueError("stem_wgrad: Cout {} > 64 (the stem kernel computes one 64-channel tile)"
+                     .format(Cout))
+  # all seven filter rows from one 16 x 21 halo box per 16 x 8 output pixels
+  # (csrc/igemm_wgrad.cu igemm_wgrad_halo_kernel)
+  ta = _tmap4(dy, (OW, OH, N), Cout, (16, 8, 1))
+  tb = _stem_halo_tmap(xp, N, H, Wp, OW, 16, 2 * 8 + 5)
+  tw, th = -(-OW // 16), -(-OH // 8)
   g = {
-      "tiles_w": tw, "tiles_h": th, "tiles_n": tn, "box_w": bw, "box_h": bh, "box_n": bnn,
-      "mul_w": 1, "mul_h": 2, "num_taps": 7,
-      "tap_dw": [0] * 7, "tap_dh": [r - STEM_PAD for r in range(7)], "tap_dc": [0] * 7,
-      "tap_out": [r * 64 for r in range(7)],
-      "m_tiles": -(-Cout // 128), "n_tiles": 1,
+      "tiles_w": tw, "tiles_h": th, "tiles_n": N, "box_w": 16, "box_h": 8, "box_n": 1,
+      "num_taps": 1, "stem": 1,
+      "halo_boxes": 1, "box_dw": [0], "halo_rows": 2 * 8 + 5, "halo_hmul": 2,
+      "halo_h0": -STEM_PAD, "halo_jrow": [2 * j for j in range(8)], "halo_rowbytes": 2048,
+      "halo_nacc": 7,
+      "acc_box": [0] * 7, "acc_row": list(range(7)), "tap_out": [r * 64 for r in range(7)],
+      "m_tiles": 1, "n_tiles": 1, "k_splits": max(1, min(_SMS, tw * th * N)),
       "m_valid": Cout, "n_valid": 64, "ldw": 7 * 64, "dw": dw.data_ptr(),
   }
   h = _C().igemm_plan_wgrad(ta, tb, g, 64)
-  return Plan([h], (dy, xp, dw), "stem wgrad")
+  return Plan([h], (dy, xp, dw), "stem wgrad (halo)")
 
 
 def pack_stem_weight(w_krsc):

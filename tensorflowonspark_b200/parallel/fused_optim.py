@@ -98,7 +98,7 @@ def lars_tables(bounds, buckets, world, seg_len=LARS_SEGMENT):
 class FusedOptimizer(object):
 
   def __init__(self, store, comm=None, opt="momentum", lr=0.1, momentum=0.9, weight_decay=0.0,
-               beta1=0.9, beta2=0.999, eps=1e-7, buckets=None, grid=None, trust_coefficient=0.001):
+               beta1=0.9, beta2=0.999, eps=1e-7, buckets=None, trust_coefficient=0.001):
     """``trust_coefficient``: LARS eta (``opt="lars"``; it takes the slot of Adam's beta1 in
     the hyper-parameter vector, which LARS does not use)."""
     self.store, self.comm = store, comm
@@ -135,10 +135,8 @@ class FusedOptimizer(object):
     self.state1 = _state("state1") if self.opt != 0 else None
     self.state2 = _state("state2") if self.opt == 2 else None
     self.step_count = 0
-    import os
-    env_grid = int(os.environ.get("TFOS_AR_GRID", "0"))   # CTAs of the fused kernel (experiments)
-    grid = grid or env_grid or None
-    self.grid = grid or (132 if self.world == 1 else 64)
+    # CTAs of the fused kernel: one per SM alone, 64 peer-to-peer, 48 with NVLS (below)
+    self.grid = 132 if self.world == 1 else 64
     n = store.total
     if not buckets:
       buckets = [(0, n, None)]
@@ -178,7 +176,7 @@ class FusedOptimizer(object):
           d["grads_mc"] = comm.mc_ptr("grads")
           d["weights_mc"] = comm.mc_ptr("weights")
           d["aux32_mc"] = comm.mc_ptr("aux32")
-          d["grid"] = grid or 48
+          d["grid"] = 48
       self._args.append(d)
     self.nvls = bool(self._args and self._args[0].get("grads_mc"))
     if self.lars:
@@ -245,21 +243,6 @@ class FusedOptimizer(object):
       self.hyper[7:8].add_(1.0)
 
   # ---------------------------------------------------------------- overlap
-  def add_producer_stream(self, stream):
-    """Gradients are also written by kernels on ``stream`` (the weight-gradient side stream):
-    every consumer of the gradient buffer waits for it."""
-    if not hasattr(self, "_producers"):
-      self._producers = []
-    self._producers.append((stream, {}))
-
-  def _join_producers(self, consumer, key):
-    for stream, events in getattr(self, "_producers", []):
-      ev = events.get(key)
-      if ev is None:
-        ev = events[key] = torch.cuda.Event()
-      ev.record(stream)
-      consumer.wait_event(ev)
-
   def launch(self, tag):
     """Gradients of every bucket tagged ``tag`` are final on the current stream: run their
     fused all-reduce + update on the communication stream now."""
@@ -273,7 +256,6 @@ class FusedOptimizer(object):
         continue
       self._ev_ready[i].record(main)
       self.comm_stream.wait_event(self._ev_ready[i])
-      self._join_producers(self.comm_stream, i)
       with torch.cuda.stream(self.comm_stream):
         self._run_bucket(i)
       self._launched.add(i)
@@ -284,8 +266,6 @@ class FusedOptimizer(object):
       self.deferred = True      # the collective stays outside the graph: after_replay() runs it
       return
     if not self.overlap:
-      if self.device.type == "cuda":
-        self._join_producers(torch.cuda.current_stream(self.device), "finish")
       return self.step()
     for tag in list(self._by_tag):
       self.launch(tag)

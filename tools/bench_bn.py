@@ -27,8 +27,6 @@ def timeit(fn, iters=10):
 
 
 def main():
-  print("waves reduce={} apply={}".format(os.environ.get("TFOS_BN_WAVES_REDUCE", "dflt"),
-                                          os.environ.get("TFOS_BN_WAVES_APPLY", "dflt")))
   tot = {}
   for P, C in SHAPES:
     x = torch.randn(P, C, device="cuda").bfloat16()

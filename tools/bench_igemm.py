@@ -86,7 +86,7 @@ def device_line():
   return "{} ({})".format(torch.cuda.get_device_name(0), q or "power limit / max SM clock unknown")
 
 
-def build(kind, shape, nbuf, stats=True, epi_prefetch=None):
+def build(kind, shape, nbuf, stats=True, epi_prefetch=True):
   H, W, Ci, Co, k, s = shape
   pad = k // 2
   OH, OW = (H + 2 * pad - k) // s + 1, (W + 2 * pad - k) // s + 1
@@ -127,16 +127,11 @@ def main():
   ap.add_argument("--only", default=None)
   ap.add_argument("--iters", type=int, default=20)
   ap.add_argument("--no-stats", action="store_true")
-  ap.add_argument("--epi-prefetch", type=int, choices=(0, 1), default=None,
-                  help="dgrad_* kinds: prefetch the epilogue operands (default: the plan's choice)")
-  ap.add_argument("--wgrad-onepass", type=int, choices=(0, 1), default=None,
-                  help="3x3 wgrad: all nine taps from one pass over the pixels (default: the "
-                       "plan's choice, TFOS_WGRAD_HALO)")
+  ap.add_argument("--epi-prefetch", type=int, choices=(0, 1), default=1,
+                  help="dgrad_* kinds: prefetch the epilogue operands where the plan can")
   ap.add_argument("--kind", default=None,
                   help="fprop | dgrad | dgrad_red | dgrad_acc | dgrad_accred | wgrad")
   args = ap.parse_args()
-  if args.wgrad_onepass is not None:
-    igemm._WGRAD_HALO = bool(args.wgrad_onepass)
   hbm, tf, src = peaks()
   print(device_line())
   print("peaks ({}): HBM {:.0f} GB/s, bf16 {:.0f} TFLOP/s".format(src, hbm, tf))
@@ -148,8 +143,7 @@ def main():
     H, W, Ci, Co, k, s = shape
     per = 2.0 * B * (H * W * Ci + H * W * Co)
     nbuf = 1 if args.only else max(2, int(400e6 // per) + 1)
-    plans, flops, byts = build(kind, shape, nbuf, not args.no_stats,
-                               None if args.epi_prefetch is None else bool(args.epi_prefetch))
+    plans, flops, byts = build(kind, shape, nbuf, not args.no_stats, bool(args.epi_prefetch))
     iters = 3 if args.only else args.iters
     for p in plans[:2]:
       p.run()
