@@ -412,6 +412,42 @@ void decode_normalize(const Tensor& in, Tensor out, int wofs, std::vector<double
                                cur_stream()),
         "decode_normalize");
 }
+void bn_fold(const Tensor& tab, const Tensor& eps, const Tensor& row0, int64_t rows, const Tensor& w,
+             const Tensor& aux32, const Tensor& running, Tensor wf, Tensor bias) {
+  need(tab, torch::kInt64, "tab");
+  need(eps, torch::kFloat32, "eps");
+  need(row0, torch::kInt64, "row0");
+  need(w, torch::kBFloat16, "w");
+  need(aux32, torch::kFloat32, "aux32");
+  need(running, torch::kFloat32, "running");
+  need(wf, torch::kBFloat16, "wf");
+  need(bias, torch::kFloat32, "bias");
+  const int units = tab.size(0);
+  TORCH_CHECK(tab.dim() == 2 && tab.size(1) == tfos::kFoldCols && units > 0 &&
+                  eps.numel() == units && row0.numel() == units + 1,
+              "bn_fold: table shapes");
+  TORCH_CHECK(wf.numel() == w.numel(), "bn_fold: wf must have the layout of w");
+  TORCH_CHECK(rows > 0, "bn_fold: rows (= row0[units], the total output channels)");
+  check(tfos::bn_fold(static_cast<const long long*>(tab.data_ptr()), eps.data_ptr<float>(),
+                      static_cast<const long long*>(row0.data_ptr()),
+                      units, rows, w.data_ptr(), aux32.data_ptr<float>(), running.data_ptr<float>(),
+                      wf.data_ptr(), bias.data_ptr<float>(), cur_stream()),
+        "bn_fold");
+}
+void eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& n_valid, Tensor acc,
+                  int V) {
+  need(logits, torch::kFloat32, "logits");
+  need(labels, torch::kInt32, "labels");
+  need(n_valid, torch::kInt32, "n_valid");
+  need(acc, torch::kFloat64, "acc");
+  TORCH_CHECK(logits.dim() == 2 && V >= 1 && V <= logits.size(1), "eval_metrics: V in [1, ld]");
+  TORCH_CHECK(labels.numel() >= logits.size(0), "eval_metrics: fewer labels than rows");
+  TORCH_CHECK(acc.numel() >= tfos::kEvalSlots, "eval_metrics: acc needs 8 slots");
+  check(tfos::eval_metrics(logits.data_ptr<float>(), labels.data_ptr<int>(),
+                           n_valid.data_ptr<int>(), acc.data_ptr<double>(), logits.size(0),
+                           logits.size(1), V, cur_stream()),
+        "eval_metrics");
+}
 void cast_f32_bf16(const Tensor& in, Tensor out) {
   need(in, torch::kFloat32, "in");
   need(out, torch::kBFloat16, "out");
@@ -708,6 +744,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("softmax_xent", &softmax_xent);
   m.def("decode_normalize", &decode_normalize);
   m.def("cast_f32_bf16", &cast_f32_bf16);
+  m.def("bn_fold", &bn_fold);
+  m.def("eval_metrics", &eval_metrics);
   m.def("conv3x3_c1_fwd", &conv3x3_c1_fwd);
   m.def("conv3x3_c1_wgrad", &conv3x3_c1_wgrad);
   m.def("depthwise3x3_fwd", &depthwise3x3_fwd);

@@ -206,4 +206,22 @@ cudaError_t conv3x3_c1_wgrad(const void* x, const void* dy, float* dw, float* db
 cudaError_t depthwise3x3_fwd(const void* x, const void* w, const float* bias, void* y, int N,
                              int H, int W, int C, int stride, int act, cudaStream_t s);
 
+// ---- held-out evaluation (eval.cu)
+// bn_fold: row u of tab [units][kFoldCols] describes one convolution + batch norm.  Offsets are
+// element offsets into the flat bf16 weights (filter), aux32 (gamma, beta), the running-statistics
+// buffer (mean, var) and the fp32 bias output; every output channel's filter row holds
+// per_channel contiguous elements (multiple of 8, like the filter offset).  row0 [units + 1] is
+// the prefix sum of Cout.  wf has the layout of w.
+constexpr int kFoldWeight = 0, kFoldCout = 1, kFoldPerChannel = 2, kFoldGamma = 3, kFoldBeta = 4,
+              kFoldMean = 5, kFoldVar = 6, kFoldBias = 7, kFoldCols = 8;
+cudaError_t bn_fold(const long long* tab, const float* eps, const long long* row0, int units,
+                    long long rows, const void* w, const float* aux32, const float* running,
+                    void* wf, float* bias, cudaStream_t s);
+// eval_metrics: acc[kEval*] += totals of rows [0, *n_valid) of fp32 logits [rows, ld], columns
+// [0, V) only (deterministic: one CTA, fixed-order sums)
+constexpr int kEvalCount = 0, kEvalTop1 = 1, kEvalTop5 = 2, kEvalInvalid = 3, kEvalLoss = 4,
+              kEvalUsedSlots = 5, kEvalSlots = 8;
+cudaError_t eval_metrics(const float* logits, const int* labels, const int* n_valid, double* acc,
+                         int rows, int ld, int V, cudaStream_t s);
+
 }  // namespace tfos

@@ -13,6 +13,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 NUM_TRAIN, NUM_EVAL = 50000, 10000
+EVAL_SEED = 1 << 20   # synthetic held-out batches: above every training seed (the rank)
 
 
 def define_flags():
@@ -27,6 +28,8 @@ def define_flags():
   p.add_argument("--model_dir", default=None)
   p.add_argument("--epochs_between_evals", type=int, default=10)
   p.add_argument("--skip_eval", action="store_true")
+  p.add_argument("--eval_steps", type=int, default=0,
+                 help="synthetic data: held-out batches per rank and evaluation (0: no evaluation)")
   # distribution flags of the reference; here every replica is one process on one GPU and the
   # gradient all-reduce is always fused with the optimizer: the flags select what they still can
   p.add_argument("--ds", "--distribution_strategy", dest="ds", default="multi_worker_mirrored",
@@ -99,6 +102,33 @@ def main_fun(argv, ctx):
   if args.train_steps:
     total = min(total, args.train_steps)
   rng = np.random.RandomState(1234 + ctx.rank)
+  # held-out set (the reference's validation_freq = epochs_between_evals): CIFAR-10's test batch,
+  # sharded over the ranks like the training set, or synthetic batches from disjoint seeds
+  eval_set = None
+  if not args.skip_eval:
+    if not synthetic:
+      ex, ey = read_cifar(args.data_dir, False)
+      ex, ey = ex[ctx.rank::world], ey[ctx.rank::world].astype(np.int32)
+      eval_set = [(ex[i:i + B], ey[i:i + B]) for i in range(0, len(ex), B)]
+    elif args.eval_steps:
+      eval_set = [net.synthetic_batch(seed=EVAL_SEED + ctx.rank * args.eval_steps + i)
+                  for i in range(args.eval_steps)]
+  eval_events = None
+  if eval_set is not None and args.model_dir and ctx.is_chief:
+    from tensorflowonspark_b200.utils import summary
+    eval_events = summary.SummaryWriter(os.path.join(ctx.absolute_path(args.model_dir), "eval"))
+
+  def evaluate(step, epoch):
+    res = net.evaluate(eval_set)
+    if ctx.is_chief:
+      print("eval: epoch {} loss {:.4f} top1 {:.4f} top5 {:.4f} ({} images)".format(
+          epoch, res["loss"], res["top1"], res["top5"], res["count"]))
+    if eval_events:
+      eval_events.add_scalars({"loss": res["loss"], "accuracy": res["top1"],
+                               "top5_accuracy": res["top5"]}, step)
+      eval_events.flush()
+
+  every = steps_per_epoch * max(1, args.epochs_between_evals)
   if synthetic:
     net.set_input(x, y)
     net.train_step()
@@ -128,7 +158,12 @@ def main_fun(argv, ctx):
         1, args.epochs_between_evals)) == 0:
       checkpoint.save(ctx.absolute_path(args.model_dir), step + 1,
                       {"params": net.state_dict(), "optim": net.optim.state_dict()})
+    if eval_set is not None and ((step + 1) % every == 0 or step + 1 == total):
+      evaluate(step + 1, (step + 1) // steps_per_epoch)
+      t0, seen = time.time(), 0
   torch.cuda.synchronize()
+  if eval_events:
+    eval_events.close()
   if args.model_dir and ctx.is_chief:
     checkpoint.save(ctx.absolute_path(args.model_dir), total,
                     {"params": net.state_dict(), "optim": net.optim.state_dict()})

@@ -13,12 +13,20 @@ Large global batches: ``--optimizer lars`` (per-layer trust ratios, parallel/fus
 a linear warm-up over ``--warmup_steps`` and polynomial decay to 0 at the last step
 (``resnet.poly_warmup_lr``), peaking at ``--base_lr`` (default: the linear-scaling rule
 0.1 * global batch / 256).
+
+Held-out evaluation: ``--eval_steps N`` scores N synthetic ImageNet-shaped batches per rank
+(drawn from seeds disjoint from the training batch) every ``--eval_every K`` steps and after the
+last step (``K = 0``: only after the last step), through the trainer's folded forward pass on its
+own buffers (``ResNetTrainer.evaluate``).  The totals are summed over all ranks; the eval fields
+go to the JSONL metrics, TensorBoard and the Prometheus exporter next to the training fields.
 """
 import argparse
 import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+
+EVAL_SEED = 1 << 20   # synthetic held-out batches: above every training seed (the rank)
 
 
 def parse(argv):
@@ -39,6 +47,10 @@ def parse(argv):
                  help="peak learning rate (default: 0.1 * global batch / 256; resnet56: piecewise_lr)")
   p.add_argument("--warmup_steps", type=int, default=0, help="lars: linear warm-up steps")
   p.add_argument("--trust_coefficient", type=float, default=0.001, help="lars: eta")
+  p.add_argument("--eval_steps", type=int, default=0,
+                 help="synthetic held-out batches per rank and evaluation (0: no evaluation)")
+  p.add_argument("--eval_every", type=int, default=0,
+                 help="evaluate every K steps (0: only after the last step)")
   p.add_argument("--metrics_port", type=int, default=None,
                  help="serve the same fields on a Prometheus /metrics endpoint (port + rank; 0: any free port)")
   return p.parse_args(argv)
@@ -90,6 +102,25 @@ def main_fun(argv, ctx):
   if args.model_dir and ctx.is_chief:     # TensorBoard scalars next to the checkpoints
     from tensorflowonspark_b200.utils import summary
     events = summary.SummaryWriter(ctx.absolute_path(args.model_dir))
+  eval_batches = []
+
+  def evaluate(step):
+    if not eval_batches:   # seeds disjoint from the training batch's (seed = rank)
+      eval_batches.extend(net.synthetic_batch(seed=EVAL_SEED + ctx.rank * args.eval_steps + i)
+                          for i in range(args.eval_steps))
+    res = net.evaluate(eval_batches)
+    if ctx.is_chief:
+      print("eval: step {} loss {:.4f} top1 {:.4f} top5 {:.4f} ({} images)".format(
+          step, res["loss"], res["top1"], res["top5"], res["count"]))
+    fields = {"eval_loss": res["loss"], "eval_top1": res["top1"], "eval_top5": res["top5"],
+              "eval_count": res["count"]}
+    if log:
+      log.log(step=step, **fields)
+    if events:
+      events.add_scalars(fields, step)
+    if exporter and not log:
+      exporter.update(step=step, **fields)
+
   torch.cuda.synchronize()
   t0 = time.time()
   total_steps = start + args.train_steps
@@ -116,6 +147,10 @@ def main_fun(argv, ctx):
     if args.model_dir and args.save_steps and (step + 1) % args.save_steps == 0 and ctx.is_chief:
       checkpoint.save(ctx.absolute_path(args.model_dir), step + 1,
                       {"params": net.state_dict(), "optim": net.optim.state_dict()})
+    if args.eval_steps and ((args.eval_every and (step + 1) % args.eval_every == 0) or
+                            step + 1 == total_steps):
+      evaluate(step + 1)
+      t0 = time.time()
   torch.cuda.synchronize()
   if events:
     events.close()

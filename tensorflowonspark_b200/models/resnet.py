@@ -35,6 +35,186 @@ def _buf(shape, device, dtype=torch.bfloat16):
   return torch.zeros(shape, dtype=dtype, device=device)
 
 
+# columns of the bn_fold table (csrc/ops.h kFold*)
+FOLD_WEIGHT, FOLD_COUT, FOLD_PER_CHANNEL, FOLD_GAMMA, FOLD_BETA, FOLD_MEAN, FOLD_VAR, FOLD_BIAS = \
+    range(8)
+
+
+def fold_table(store, units, running):
+  """Host table that drives the ``bn_fold`` kernel: one int64 row per (filter spec, BatchNorm) of
+  ``units`` with the filter's offset in ``store.weights``, Cout, the elements per output channel,
+  gamma / beta offsets in ``store.aux32``, running mean / var offsets in ``running``'s buffer
+  (engine.RunningArena) and the unit's slot in the fp32 bias vector (each padded to 8).
+  Returns (table [U, 8] int64, eps [U] fp32, row0 [U + 1] int64: prefix sums of Cout, bias length)."""
+  rows, eps, row0, boff = [], [], [0], 0
+  base = running.buf.data_ptr()
+  for spec, bn in units:
+    cout = spec["shape"][0]
+    per = spec["numel"] // cout
+    if bn.C != cout or per % 8 or spec["offset"] % 8:
+      raise ValueError("bn_fold: {} does not fold into {}".format(bn.name, spec["name"]))
+    rows.append([spec["offset"], cout, per, bn.sg["offset"] - store.decay_end,
+                 bn.sb["offset"] - store.decay_end,
+                 (bn.running_mean.data_ptr() - base) // 4, (bn.running_var.data_ptr() - base) // 4,
+                 boff])
+    eps.append(bn.eps)
+    row0.append(row0[-1] + cout)
+    boff += (cout + 7) // 8 * 8
+  return (torch.tensor(rows, dtype=torch.int64), torch.tensor(eps, dtype=torch.float32),
+          torch.tensor(row0, dtype=torch.int64), boff)
+
+
+class _Evaluator(object):
+  """Held-out evaluation on a trainer's own buffers (``eval_begin`` / ``eval_step`` /
+  ``eval_end`` of both ResNet trainers).
+
+  The forward pass is the folded network of ``build_folded_inference`` (bias, ReLU and the
+  residual add in the convolution epilogues) run on the trainer's activation buffers: the next
+  training forward rewrites all of them, and backward reads only what its own forward wrote.  The
+  filters are folded from the bf16 ``weights`` and ``aux32``, which are complete and identical on
+  every rank (the fp32 masters are only current for a rank's own shard), with rank 0's running
+  statistics - the ones its checkpoint and exports carry - so every rank scores the same model.
+  Only the uint8 input batch, labels, folded filters and biases are extra memory, allocated on the
+  first ``eval_begin``."""
+
+  def __init__(self, net):
+    st, dev, comm = net.store, net.device, net.comm
+    self.net, self.comm = net, comm
+    units = net._fold_units()
+    tab, eps, row0, nbias = fold_table(st, units, net.running)
+    self.tab, self.eps, self.row0 = tab.to(dev), eps.to(dev), row0.to(dev)
+    self.rows = int(row0[-1])
+    self.wf = torch.zeros_like(st.weights)
+    self.bf = torch.zeros(nbias, dtype=torch.float32, device=dev)
+    bias = {id(bn): self.bf[int(tab[i, FOLD_BIAS]):int(tab[i, FOLD_BIAS]) + bn.C]
+            for i, (_, bn) in enumerate(units)}
+    self.u8 = torch.zeros_like(net.in_u8)         # never in_u8: drivers stage a batch and replay
+    self.labels = torch.zeros_like(net.labels)
+    self.n_valid = torch.zeros(1, dtype=torch.int32, device=dev)
+    self.acc = torch.zeros(8, dtype=torch.float64, device=dev)
+    self.V = net.num_classes
+    self.kind = None if comm is None else (
+        "group" if getattr(comm, "cross_host", False) else
+        "hier" if getattr(comm, "hierarchical", False) else "symm")
+    if comm is None:
+      self.running = net.running.tensor()
+    else:
+      self.running = comm.alloc("eval_running", net.running.used, torch.float32)
+    self.totals = self.peers = None
+    if self.kind in ("symm", "hier"):
+      # fp64[8] in a symmetric fp32 buffer: every rank sums all ranks' copies in rank order
+      self.totals = comm.alloc("eval_totals", 16, torch.float32).view(torch.float64)
+    self._forward = net._eval_forward(lambda spec: st._view(self.wf, spec), bias, self.u8)
+    self.graph, self.calls = None, 0
+    self.feeder = None
+
+  def begin(self):
+    net, comm = self.net, self.comm
+    self.acc.zero_()
+    if comm is not None:
+      self.running.copy_(net.running.tensor())
+      comm.broadcast("eval_running", 0)
+    st = net.store
+    ops.K.bn_fold(self.tab, self.eps, self.row0, self.rows, st.weights, st.aux32, self.running,
+                  self.wf, self.bf)
+
+  def _run(self):
+    self._forward()
+    ops.K.eval_metrics(self.net.logits, self.labels, self.n_valid, self.acc, self.V)
+
+  def step(self, images_u8, labels):
+    n = len(images_u8)
+    if n > self.net.B:
+      raise ValueError("batch of {} rows exceeds the trainer's batch size {}".format(n, self.net.B))
+    if n:
+      x = torch.as_tensor(images_u8)
+      self.u8[:n].copy_(x.reshape((n,) + tuple(self.u8.shape[1:])), non_blocking=True)
+      self.labels[:n].copy_(torch.as_tensor(labels).reshape(n), non_blocking=True)
+    self.n_valid.fill_(n)
+    if self.graph is None and self.calls >= 1:
+      self._capture()
+    if self.graph is not None:
+      self.graph.replay()
+    else:
+      self._run()
+    self.calls += 1
+
+  def _capture(self):
+    """The evaluation forward + metric as one CUDA graph (after one eager call, like
+    ServedResNet._capture); thread-local capture under a cross-host communicator, as in
+    ResNetTrainer.capture."""
+    g = torch.cuda.CUDAGraph()
+    mode = "thread_local" if getattr(self.net.optim, "group_mode", False) else "global"
+    with torch.cuda.graph(g, capture_error_mode=mode):
+      self._run()
+    self.graph = g
+
+  def run(self, batches):
+    """eval_step over (images, labels) pairs; host batches are staged in page-locked memory one
+    batch ahead of the forward pass."""
+    import numpy as np
+    pending = []
+
+    def flush():
+      n = pending.pop(0)
+      dx, dy = self.feeder.pop()
+      self.step(dx[:n], dy[:n])
+      self.feeder.release()
+
+    for images, labels in batches:
+      if isinstance(images, torch.Tensor) and images.is_cuda:
+        while pending:
+          flush()
+        self.step(images, labels)
+        continue
+      if self.feeder is None:
+        from ..feed import DevicePrefetcher
+        self.feeder = DevicePrefetcher([(tuple(self.u8.shape), torch.uint8),
+                                        ((self.net.B,), torch.int32)], self.net.device, depth=2)
+      x = images.numpy() if isinstance(images, torch.Tensor) else np.asarray(images)
+      y = labels.numpy() if isinstance(labels, torch.Tensor) else np.asarray(labels)
+      n = len(x)
+      if n > self.net.B:
+        raise ValueError("batch of {} rows exceeds the trainer's batch size {}".format(
+            n, self.net.B))
+      hx, hy = self.feeder.acquire_host()
+      hx.numpy()[:n] = x.reshape((n,) + tuple(self.u8.shape[1:]))
+      hy.numpy()[:n] = y.reshape(n)
+      self.feeder.push_host()
+      pending.append(n)
+      if len(pending) > 1:   # batch i + 1 is on its way: run batch i
+        flush()
+    while pending:
+      flush()
+
+  def end(self):
+    comm = self.comm
+    if self.kind is None:
+      tot = self.acc
+    elif self.kind == "group":
+      tot = self.acc.clone()
+      comm.all_reduce(tot)
+    else:
+      if self.peers is None:
+        C = ops.C()
+        self.peers = [C.tensor_from_ptr(p, [16], "f32").view(torch.float64)
+                      for p in comm.peer_ptrs("eval_totals")]
+      self.totals.copy_(self.acc)
+      comm.barrier()              # every rank's totals are written
+      tot = self.peers[0].clone()
+      for p in self.peers[1:]:
+        tot += p
+      comm.barrier()              # every rank has read them before the next pass rewrites them
+      if self.kind == "hier":
+        comm.all_reduce_inter(tot)
+    h = tot.cpu().tolist()
+    if h[3] > 0:
+      raise ValueError("evaluation saw {} label(s) outside [0, {})".format(int(h[3]), self.V))
+    count = int(h[0])
+    mean = (lambda v: v / count) if count else (lambda v: float("nan"))
+    return {"count": count, "loss": mean(h[4]), "top1": mean(h[1]), "top5": mean(h[2])}
+
+
 class ResNetTrainer(object):
   """Static-buffer ResNet.  ``train_step(images_u8 | normalized, labels)`` runs
   forward, backward and the fused optimizer; ``forward_only`` serves inference."""
@@ -398,20 +578,30 @@ class ResNetTrainer(object):
     parameters or running statistics change (``fold_batch_norms``)."""
     assert not self.training, "folded inference is built on a training=False trainer"
     st, dev = self.store, self.device
-    units = [("stem", self.stem_w, self.stem_bn)]
-    for b in self.blocks:
-      for u in (b.u1, b.u2, b.u3) + ((b.ds,) if b.ds is not None else ()):
-        units.append((u, u.conv.sw, u.bn))
-    self._fold_units = units
+    units = self._fold_units()
     self.wf = torch.zeros_like(st.weights)        # folded bf16 filters, same layout as weights
-    self.bf = torch.zeros(sum((bn.C + 7) // 8 * 8 for _, _, bn in units), dtype=torch.float32,
+    self.bf = torch.zeros(sum((bn.C + 7) // 8 * 8 for _, bn in units), dtype=torch.float32,
                           device=dev)
     bias, off = {}, 0
-    for key, _, bn in units:
+    for _, bn in units:
       bias[id(bn)] = self.bf[off:off + bn.C]
       off += (bn.C + 7) // 8 * 8
-    wv = lambda spec: st._view(self.wf, spec)  # noqa: E731
-    plans = [igemm.stem_fprop(self.xp, wv(self.stem_w), self.stem_act, bias=bias[id(self.stem_bn)],
+    self._f_plans, self._f_last = self._folded_plans(lambda spec: st._view(self.wf, spec), bias,
+                                                     self.stem_act)
+    self.fold_batch_norms()
+
+  def _fold_units(self):
+    """(filter spec, batch norm) of every convolution followed by a batch norm, stem first."""
+    units = [(self.stem_w, self.stem_bn)]
+    for b in self.blocks:
+      for u in (b.u1, b.u2, b.u3) + ((b.ds,) if b.ds is not None else ()):
+        units.append((u.conv.sw, u.bn))
+    return units
+
+  def _folded_plans(self, wv, bias, stem_out):
+    """The folded network's convolutions: ``wv(spec)`` is a folded filter, ``bias[id(bn)]`` the
+    folded batch norm's bias; the stem writes ``stem_out``.  Returns (plans, last activation)."""
+    plans = [igemm.stem_fprop(self.xp, wv(self.stem_w), stem_out, bias=bias[id(self.stem_bn)],
                               relu=True)]
     cur = self.pool
     for b in self.blocks:
@@ -429,13 +619,28 @@ class ResNetTrainer(object):
       plans.append(igemm.conv_fprop(b.a2, wv(b.u3.conv.sw), target, 1, 0, bias=bias[id(b.u3.bn)],
                                     relu=True, accumulate=True))
       cur = target
-    self._f_plans, self._f_last = plans, cur
-    self.fold_batch_norms()
+    return plans, cur
+
+  def _eval_forward(self, wv, bias, u8):
+    """Evaluation forward pass on this trainer's activation buffers (see _Evaluator): the stem
+    writes ``stem_raw``, which a training trainer has too."""
+    plans, last = self._folded_plans(wv, bias, self.stem_raw)
+    K = ops.K
+
+    def run():
+      K.decode_normalize(u8, self.xp, igemm.STEM_PAD, self.mean, self.std)
+      plans[0].run()
+      K.maxpool_fwd(self.stem_raw, self.pool, self.pool_idx, 3, 2, 1)
+      for p in plans[1:]:
+        p.run()
+      K.avgpool_fwd(last, self.avg)
+      self.fc.forward()
+    return run
 
   def fold_batch_norms(self):
     st = self.store
     off = 0
-    for key, spec, bn in self._fold_units:
+    for spec, bn in self._fold_units():
       scale = st.m(bn.sg) * torch.rsqrt(bn.running_var + bn.eps)
       w = st.m(spec).float()
       st._view(self.wf, spec).copy_(w * scale.view(-1, *([1] * (w.dim() - 1))))
@@ -453,6 +658,39 @@ class ResNetTrainer(object):
     K.avgpool_fwd(self._f_last, self.avg)
     self.fc.forward()
     return self.logits
+
+  # ------------------------------------------------------- held-out evaluation
+  def eval_begin(self):
+    """Start an evaluation pass: zero the totals, take rank 0's running statistics and fold every
+    batch norm into a copy of the current bf16 filters (one launch).  Stream-ordered after the
+    last ``train_step``; the first call allocates the evaluation buffers and plans."""
+    if getattr(self, "_evaluator", None) is None:
+      self._evaluator = _Evaluator(self)
+    self._evaluator.begin()
+
+  def eval_step(self, images_u8, labels):
+    """Add the top-1 / top-5 / loss totals of n <= B images (host or device, uint8 NHWC) and their
+    labels.  Runs the folded network on the training buffers, leaving ``in_u8`` / ``labels`` and
+    the training state untouched; ``logits`` then holds the batch's logits.  No host sync."""
+    self._eval_state().step(images_u8, labels)
+
+  def eval_end(self):
+    """Totals summed over all ranks (identical on every rank): {"count", "loss", "top1", "top5"};
+    the last three are means over ``count`` (NaN when it is 0).  Raises ValueError on every rank
+    when any rank saw a label outside [0, num_classes)."""
+    return self._eval_state().end()
+
+  def evaluate(self, batches):
+    """eval_begin + eval_step over ``(images, labels)`` pairs + eval_end.  Host batches go through
+    page-locked staging: the copy of batch i + 1 overlaps the forward pass of batch i."""
+    self.eval_begin()
+    self._evaluator.run(batches)
+    return self.eval_end()
+
+  def _eval_state(self):
+    if getattr(self, "_evaluator", None) is None:
+      raise RuntimeError("eval_begin() has not been called")
+    return self._evaluator
 
   def set_lr(self, lr):
     self.optim.set_lr(lr)
@@ -632,6 +870,7 @@ class CifarResNetTrainer(object):
     n = (depth - 2) // 6
     self.device = dev = torch.device(device)
     self.B, self.image, self.num_classes = batch, 32, num_classes
+    self.comm = comm
     self.VP = (num_classes + 7) // 8 * 8
     B = batch
     st = self.store = ParamStore()
@@ -701,6 +940,44 @@ class CifarResNetTrainer(object):
   capture = ResNetTrainer.capture
   train_step = ResNetTrainer.train_step
   set_lr = ResNetTrainer.set_lr
+  eval_begin = ResNetTrainer.eval_begin
+  eval_step = ResNetTrainer.eval_step
+  eval_end = ResNetTrainer.eval_end
+  evaluate = ResNetTrainer.evaluate
+  _eval_state = ResNetTrainer._eval_state
+
+  def _fold_units(self):
+    """(filter spec, batch norm) of every convolution followed by a batch norm, stem first."""
+    units = [(self.stem.conv.sw, self.stem.bn)]
+    for b in self.blocks:
+      for u in (b.u1, b.u2) + ((b.ds,) if b.ds is not None else ()):
+        units.append((u.conv.sw, u.bn))
+    return units
+
+  def _eval_forward(self, wv, bias, u8):
+    """Folded basic-block network on the training buffers (see _Evaluator): bias + ReLU in every
+    epilogue, the shortcut into ``out``, conv2 accumulating the residual into ``out`` (projection
+    blocks) or in place into the block input (identity blocks)."""
+    conv = lambda x, u, y, **kw: igemm.conv_fprop(  # noqa: E731
+        x, wv(u.conv.sw), y, u.conv.stride, u.conv.pad, bias=bias[id(u.bn)], **kw)
+    cur = self.stem_act
+    plans = [conv(self.x8, self.stem, cur, relu=True)]
+    for b in self.blocks:
+      plans.append(conv(cur, b.u1, b.a1, relu=True))
+      if b.ds is not None:
+        plans.append(conv(cur, b.ds, b.out))
+        cur = b.out
+      plans.append(conv(b.a1, b.u2, cur, relu=True, accumulate=True))
+    last = cur
+    K = ops.K
+
+    def run():
+      K.decode_normalize(u8, self.x8, 0, self.mean, self.std)
+      for p in plans:
+        p.run()
+      K.avgpool_fwd(last, self.avg)
+      self.fc.forward()
+    return run
 
   def step_kernels(self):
     K = ops.K
