@@ -448,6 +448,31 @@ void eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& n_va
                            logits.size(1), V, cur_stream()),
         "eval_metrics");
 }
+int64_t seg_eval_scratch(int64_t pixels) {
+  return static_cast<int64_t>(tfos::seg_eval_grid(pixels)) * tfos::kSegEvalSlots;
+}
+void seg_eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& n_valid,
+                      Tensor acc, Tensor partial, Tensor counter, int V) {
+  need(logits, torch::kBFloat16, "logits");
+  need(labels, torch::kInt32, "labels");
+  need(n_valid, torch::kInt32, "n_valid");
+  need(acc, torch::kFloat64, "acc");
+  need(partial, torch::kFloat64, "partial");
+  need(counter, torch::kInt32, "counter");
+  TORCH_CHECK(logits.dim() >= 2 && logits.size(0) > 0 && logits.size(-1) == 8 && V >= 1 && V <= 8,
+              "seg_eval_metrics: logits [B, ..., 8] and V in [1, 8]");
+  const int64_t images = logits.size(0), pixels = logits.numel() / 8;
+  TORCH_CHECK(labels.numel() == pixels, "seg_eval_metrics: one label per pixel");
+  TORCH_CHECK(acc.numel() >= tfos::kSegEvalSlots, "seg_eval_metrics: acc needs 68 slots");
+  TORCH_CHECK(partial.numel() >= seg_eval_scratch(pixels),
+              "seg_eval_metrics: partial needs seg_eval_scratch(pixels) doubles");
+  TORCH_CHECK(counter.numel() >= 1, "seg_eval_metrics: counter");
+  check(tfos::seg_eval_metrics(logits.data_ptr(), labels.data_ptr<int>(), n_valid.data_ptr<int>(),
+                               acc.data_ptr<double>(), partial.data_ptr<double>(),
+                               reinterpret_cast<unsigned int*>(counter.data_ptr<int>()),
+                               static_cast<int>(images), pixels / images, V, cur_stream()),
+        "seg_eval_metrics");
+}
 void cast_f32_bf16(const Tensor& in, Tensor out) {
   need(in, torch::kFloat32, "in");
   need(out, torch::kBFloat16, "out");
@@ -746,6 +771,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("cast_f32_bf16", &cast_f32_bf16);
   m.def("bn_fold", &bn_fold);
   m.def("eval_metrics", &eval_metrics);
+  m.def("seg_eval_scratch", &seg_eval_scratch);
+  m.def("seg_eval_metrics", &seg_eval_metrics);
   m.def("conv3x3_c1_fwd", &conv3x3_c1_fwd);
   m.def("conv3x3_c1_wgrad", &conv3x3_c1_wgrad);
   m.def("depthwise3x3_fwd", &depthwise3x3_fwd);

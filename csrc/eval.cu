@@ -7,6 +7,10 @@
 //                   added to an fp64 accumulator by ONE CTA with a fixed row-to-warp assignment
 //                   and a fixed-order reduction: no floating-point atomics, so the totals are
 //                   bitwise reproducible across runs and graph replays.
+//  * seg_eval_metrics : the same for the U-Net's per-pixel bf16 logits (models/unet.py): count,
+//                   correct, invalid labels, loss and the V x V confusion matrix of every pixel of
+//                   the valid images.  Many CTAs, each over a fixed contiguous pixel range; the
+//                   last CTA to finish sums the per-CTA partials in a fixed order.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -114,7 +118,158 @@ eval_metrics_kernel(const float* __restrict__ logits, const int* __restrict__ la
   }
 }
 
+constexpr int kSegThreads = 512;
+constexpr int kSegWarps = kSegThreads / 32;
+constexpr int kSegMaxGrid = kSmCount * 2;
+constexpr int kSegUnroll = 4;        // pixels per thread in flight
+constexpr int kSegStep = kSegThreads * kSegUnroll;
+constexpr int kSegBins = 8 * 8 + 1;  // confusion cells y * 8 + pred, then "invalid label"
+
+// One pixel: its bin (y * 8 + pred, kSegBins - 1 for a label outside [0, V)) and loss.  pred is
+// pixel_xent_kernel's arg-max (strict > over j < V from l[0]: the lowest index wins ties), so an
+// evaluation's "correct" counts exactly what training's does.
+__device__ __forceinline__ int seg_score(const uint4 v, const int y, const int V, double& loss) {
+  if (y < 0 || y >= V) return kSegBins - 1;
+  const float2 a = unpack_bf16x2(v.x), b = unpack_bf16x2(v.y), c = unpack_bf16x2(v.z),
+               d = unpack_bf16x2(v.w);
+  const float l[8] = {a.x, a.y, b.x, b.y, c.x, c.y, d.x, d.y};
+  float mx = l[0];
+  int am = 0;
+#pragma unroll
+  for (int j = 1; j < 8; ++j)
+    if (j < V && l[j] > mx) mx = l[j], am = j;
+  float se = 0.f, ly = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    if (j < V) se += __expf(l[j] - mx);
+    if (j == y) ly = l[j];
+  }
+  loss += static_cast<double>(__logf(se) + mx - ly);
+  return y * 8 + am;
+}
+
+// Pixels [0, n_valid * ppi) of bf16 logits [P, 8] and int32 labels [P].  CTA b owns the pixel
+// range [b * chunk, (b + 1) * chunk) (chunk a multiple of kSegStep); each pass over kSegStep
+// pixels loads pixels u * kSegThreads + t (u < kSegUnroll) into thread t first, then scores
+// them, so every warp runs the same number of iterations and the full-mask warp intrinsics are
+// safe.
+// Bins are integer counts (warp-aggregated shared-memory atomics: exact); the loss is a
+// per-thread fp64 sum reduced in a fixed tree.  The CTA writes its partials slot-major
+// (partial[s * grid + b]); the last CTA to finish sums each slot over the CTAs with a fixed
+// lane -> CTA assignment and shuffle tree.  So the totals are bitwise reproducible.
+__global__ void __launch_bounds__(kSegThreads)
+seg_eval_metrics_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                        const int* __restrict__ n_valid, double* __restrict__ acc,
+                        double* __restrict__ partial, unsigned int* __restrict__ counter,
+                        int images, long long ppi, long long chunk, int V) {
+  __shared__ int bins[kSegWarps][kSegBins];
+  __shared__ int cells[kSegBins];
+  __shared__ double wloss[kSegWarps];
+  __shared__ unsigned int is_last;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int i = threadIdx.x; i < kSegWarps * kSegBins; i += kSegThreads) (&bins[0][0])[i] = 0;
+  __syncthreads();
+  int n = *n_valid;
+  n = n < 0 ? 0 : (n > images ? images : n);
+  const long long limit = static_cast<long long>(n) * ppi;
+  const long long lo = static_cast<long long>(blockIdx.x) * chunk;
+  const long long hi = lo + chunk < limit ? lo + chunk : limit;
+  double loss = 0.0;
+  for (long long base = lo; base < hi; base += kSegStep) {
+    uint4 v[kSegUnroll];
+    int y[kSegUnroll];
+#pragma unroll
+    for (int u = 0; u < kSegUnroll; ++u) {
+      const long long p = base + u * kSegThreads + threadIdx.x;
+      if (p < hi) {
+        y[u] = __ldcs(labels + p);
+        v[u] = __ldcs(reinterpret_cast<const uint4*>(logits + p * 8));  // the pixel's 16 bytes
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < kSegUnroll; ++u) {
+      const long long p = base + u * kSegThreads + threadIdx.x;
+      const int bin = p < hi ? seg_score(v[u], y[u], V, loss) : -1;
+      const unsigned same = __match_any_sync(0xffffffffu, bin);
+      if (bin >= 0 && lane == __ffs(same) - 1) atomicAdd(&bins[warp][bin], __popc(same));
+    }
+  }
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) loss += __shfl_xor_sync(0xffffffffu, loss, o);
+  if (lane == 0) wloss[warp] = loss;
+  __syncthreads();
+  // CTA partial of [count, correct, invalid, loss, confusion[64]]: the bins summed over the
+  // warps, count and correct from them (integer shuffles, exact), the loss in warp order
+  if (threadIdx.x < kSegBins) {
+    int c = 0;
+    for (int w = 0; w < kSegWarps; ++w) c += bins[w][threadIdx.x];
+    cells[threadIdx.x] = c;
+  }
+  __syncthreads();
+  const int grid = gridDim.x;
+  double* mine = partial + blockIdx.x;
+  if (warp == 0) {
+    int cnt = cells[lane] + cells[lane + 32], hit = lane < 8 ? cells[lane * 9] : 0;
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) {
+      cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+      hit += __shfl_xor_sync(0xffffffffu, hit, o);
+    }
+    if (lane == 0) {
+      double l = 0.0;
+      for (int w = 0; w < kSegWarps; ++w) l += wloss[w];
+      mine[static_cast<long long>(kSegEvalCount) * grid] = cnt;
+      mine[static_cast<long long>(kSegEvalCorrect) * grid] = hit;
+      mine[static_cast<long long>(kSegEvalInvalid) * grid] = cells[kSegBins - 1];
+      mine[static_cast<long long>(kSegEvalLoss) * grid] = l;
+      __threadfence();
+    }
+  } else if (threadIdx.x >= 32 && threadIdx.x < 32 + 64) {
+    const int k = threadIdx.x - 32;
+    mine[static_cast<long long>(kSegEvalConfusion + k) * grid] = cells[k];
+    __threadfence();
+  }
+  __syncthreads();
+  // the last CTA to finish adds up the partials (threadFenceReduction pattern)
+  if (threadIdx.x == 0) is_last = (atomicAdd(counter, 1u) == gridDim.x - 1) ? 1u : 0u;
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  for (int s = warp; s < kSegEvalSlots; s += kSegWarps) {   // one warp per slot
+    const double* row = partial + static_cast<long long>(s) * grid;
+    double t = 0.0;
+#pragma unroll
+    for (int k = 0; k < (kSegMaxGrid + 31) / 32; ++k) {   // lane -> CTAs lane, lane + 32, ...
+      const int b = lane + 32 * k;
+      if (b < grid) t += __ldcg(row + b);
+    }
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if (lane == 0) acc[s] += t;
+  }
+  if (threadIdx.x == 0) *counter = 0;  // ready for the next launch or graph replay
+}
+
 }  // namespace
+
+int seg_eval_grid(long long pixels) {
+  long long blocks = (pixels + kSegStep - 1) / kSegStep;
+  if (blocks > kSegMaxGrid) blocks = kSegMaxGrid;
+  return blocks < 1 ? 1 : static_cast<int>(blocks);
+}
+
+cudaError_t seg_eval_metrics(const void* logits, const int* labels, const int* n_valid,
+                             double* acc, double* partial, unsigned int* counter, int images,
+                             long long ppi, int V, cudaStream_t s) {
+  const long long pixels = static_cast<long long>(images) * ppi;
+  const int grid = seg_eval_grid(pixels);
+  // a multiple of one pass: only the CTA at the end of the valid range has a partial pass
+  const long long chunk = ((pixels + grid - 1) / grid + kSegStep - 1) / kSegStep * kSegStep;
+  seg_eval_metrics_kernel<<<grid, kSegThreads, 0, s>>>(
+      static_cast<const __nv_bfloat16*>(logits), labels, n_valid, acc, partial, counter, images,
+      ppi, chunk, V);
+  return cudaGetLastError();
+}
 
 cudaError_t bn_fold(const long long* tab, const float* eps, const long long* row0, int units,
                     long long rows, const void* w, const float* aux32, const float* running,

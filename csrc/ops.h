@@ -223,5 +223,17 @@ constexpr int kEvalCount = 0, kEvalTop1 = 1, kEvalTop5 = 2, kEvalInvalid = 3, kE
               kEvalUsedSlots = 5, kEvalSlots = 8;
 cudaError_t eval_metrics(const float* logits, const int* labels, const int* n_valid, double* acc,
                          int rows, int ld, int V, cudaStream_t s);
+// seg_eval_metrics: acc[kSegEval*] += totals of the pixels of images [0, *n_valid) of bf16
+// logits [images * ppi, 8] (channels [0, V) only) and int32 labels [images * ppi]: count,
+// correct, invalid labels, loss and confusion[y * 8 + pred].  partial holds seg_eval_grid(pixels)
+// x kSegEvalSlots doubles; counter is one zeroed uint32 that the kernel leaves at zero.
+// Deterministic: a fixed grid and pixel ranges, integer bins, the partials summed in a fixed
+// order by the last CTA to finish.
+constexpr int kSegEvalCount = 0, kSegEvalCorrect = 1, kSegEvalInvalid = 2, kSegEvalLoss = 3,
+              kSegEvalConfusion = 4, kSegEvalSlots = 4 + 8 * 8;
+int seg_eval_grid(long long pixels);
+cudaError_t seg_eval_metrics(const void* logits, const int* labels, const int* n_valid,
+                             double* acc, double* partial, unsigned int* counter, int images,
+                             long long ppi, int V, cudaStream_t s);
 
 }  // namespace tfos

@@ -1,8 +1,9 @@
 """Image segmentation U-Net on ONE H100, no Spark (reference: examples/segmentation/
 segmentation.py - the notebook-derived single-node script; model at segmentation_spark.py:67-119):
 frozen MobileNetV2 encoder, four transposed-conv up-blocks, per-pixel softmax cross-entropy, Adam.
-Checkpoints every epoch (the reference's ModelCheckpoint callback) and reports pixel accuracy of
-``predict`` on a held-out synthetic batch.
+Checkpoints every epoch (the reference's ModelCheckpoint callback) and evaluates every epoch on
+``--eval_steps`` held-out synthetic batches per rank (the reference's ``validation_data``):
+validation loss, pixel accuracy and mean IoU.
 
   python examples/segmentation/segmentation.py --epochs 2 --steps_per_epoch 50
 """
@@ -13,6 +14,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 IMG = 128
+EVAL_SEED = 99991   # held-out batches: seeds apart from the training batches' 1000 * rank + i
 
 
 def define_flags():
@@ -21,6 +23,8 @@ def define_flags():
   p.add_argument("--epochs", type=int, default=2)
   p.add_argument("--steps_per_epoch", type=int, default=57, help="3680 training images / 64")
   p.add_argument("--learning_rate", type=float, default=1e-3)
+  p.add_argument("--eval_steps", type=int, default=1,
+                 help="held-out batches per rank evaluated after every epoch (0: no evaluation)")
   p.add_argument("--model_dir", default=None)
   p.add_argument("--export_dir", default=None)
   return p
@@ -46,11 +50,17 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
   if args.model_dir:
     start, state = checkpoint.load(args.model_dir)
     if state is not None:
-      net.store.load_state_dict(state["params"])
+      net.load_state_dict(state["params"])
       net.optim.load_state_dict(state["optim"])
       print("resumed from step", start)
   batches = [net.synthetic_batch(seed=1000 * rank + i)[0] for i in range(4)]
-  held_out = net.synthetic_batch(seed=99991)[0]
+  # this rank's shard of the held-out set: batch i of rank r is held-out batch i * world + r
+  held_out = [net.synthetic_batch(seed=EVAL_SEED + i * world + rank)[0]
+              for i in range(getattr(args, "eval_steps", 1))]
+  eval_events = None
+  if held_out and args.model_dir and is_chief:
+    from tensorflowonspark_b200.utils import summary
+    eval_events = summary.SummaryWriter(os.path.join(args.model_dir, "eval"))
   step = start
   for epoch in range(args.epochs):
     t0 = time.time()
@@ -60,16 +70,25 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
       loss = net.train_step()
       step += 1
     torch.cuda.synchronize()
+    rate = args.steps_per_epoch * B * world / (time.time() - t0)
+    res = net.evaluate([(x, labels_of(x)) for x in held_out]) if held_out else None  # collective
     if is_chief:
-      pred = net.predict(held_out).float().argmax(-1)   # logits [B,128,128,3] -> class ids
-      acc = float((pred.to(torch.int32) == labels_of(held_out)).float().mean())
-      print("epoch {} loss {:.4f} held-out pixel accuracy {:.4f}  {:.0f} images/s".format(
-          epoch + 1, float(loss), acc, args.steps_per_epoch * B * world / (time.time() - t0)))
+      line = "epoch {} loss {:.4f}".format(epoch + 1, float(loss))
+      if res is not None:
+        line += " val_loss {:.4f} val_accuracy {:.4f} val_mean_iou {:.4f}".format(
+            res["loss"], res["accuracy"], res["mean_iou"])
+      print(line + "  {:.0f} images/s".format(rate))
+      if eval_events is not None:
+        eval_events.add_scalars({"loss": res["loss"], "accuracy": res["accuracy"],
+                                 "mean_iou": res["mean_iou"]}, step)
+        eval_events.flush()
       if args.model_dir:
         checkpoint.save(args.model_dir, step,
-                        {"params": net.store.state_dict(), "optim": net.optim.state_dict()})
+                        {"params": net.state_dict(), "optim": net.optim.state_dict()})
+  if eval_events is not None:
+    eval_events.close()
   if args.export_dir and is_chief:
-    checkpoint.export_model(net.store.state_dict(), args.export_dir)
+    checkpoint.export_model(net.state_dict(), args.export_dir)
   return net
 
 

@@ -6,6 +6,10 @@ are provided here: ``--input_mode tf`` (each worker synthesises / reads its own 
 ``--input_mode spark`` (BASELINE.json config #4: the images travel RDD -> shared-memory pinned
 ring -> ``cudaMemcpyAsync`` on a copy stream -> device, through ``TFNode.DataFeed``).
 
+Held-out evaluation (the reference's ``validation_data``): ``--eval_steps N`` scores N synthetic
+batches per rank every ``--eval_every K`` steps and after the last step, in either input mode
+(``UNetTrainer.evaluate``: loss, pixel accuracy and mean IoU summed over all ranks).
+
   python examples/segmentation/segmentation_spark.py --cluster_size 8 --batch_size 64 --steps 100
 """
 import argparse
@@ -15,6 +19,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 IMG = 128
+EVAL_SEED = 99991   # held-out batches (--eval_steps): seeds apart from the training batches'
 
 
 def synth_rows(n, seed):
@@ -44,7 +49,27 @@ def main_fun(args, ctx):
   if comm is not None:
     comm.broadcast("weights", root=0)
     comm.broadcast("aux32", root=0)
+  # held-out evaluation (off unless --eval_steps): every --eval_every steps and after the last one
+  eval_steps, eval_every = getattr(args, "eval_steps", 0), getattr(args, "eval_every", 0)
+  held_out, evaluated = [], [0]
+
+  def evaluate(step):
+    if not held_out:   # this rank's shard, seeds apart from the training batches' (seed = rank)
+      for i in range(eval_steps):
+        x, _ = net.synthetic_batch(seed=EVAL_SEED + i * ctx.world_size + ctx.rank)
+        held_out.append((x, ((x[..., 0] > 127).to(torch.uint8) + (x[..., 1] > 200).to(torch.uint8))))
+    res = net.evaluate(held_out)   # collective: every rank evaluates
+    evaluated[0] = step
+    if ctx.is_chief:
+      print("eval: step {} val_loss={:.4f} val_accuracy={:.4f} val_mean_iou={:.4f} ({} images)".format(
+          step, res["loss"], res["accuracy"], res["mean_iou"], res["images"]), flush=True)
+
+  def after_step(done):
+    if eval_steps and eval_every and done % eval_every == 0:
+      evaluate(done)
+
   t0, seen = time.time(), 0
+  done = 0
   if args.input_mode == "spark":
     feed = ctx.get_data_feed(train_mode=True)
     feed.pin_ring()   # ring slots become DMA sources: no staging copy between feeder and GPU
@@ -71,6 +96,7 @@ def main_fun(args, ctx):
       h4 = time.time()
       for k, d in enumerate((h1 - h0, h2 - h1, h3 - h2, h4 - h3)):
         host[k] += d
+      done += 1
       if step == 0:
         net.capture()          # static buffers: later steps replay one CUDA graph
         torch.cuda.synchronize()
@@ -80,6 +106,7 @@ def main_fun(args, ctx):
         torch.cuda.synchronize()
         print("step {:4d} loss {:.4f} {:.0f} images/s".format(
             step + 1, float(loss), seen * ctx.num_workers / (time.time() - t0)))
+      after_step(done)
     print("rank {} ran {} steps ({} rows); host ms/step: feed {:.2f} staging {:.2f} hand-over {:.2f} "
           "launch {:.2f}; H2D tensors straight from the ring {} / staged {}".format(
               ctx.rank, step + 1, seen + B, *([1e3 * h / (step + 1) for h in host]
@@ -96,10 +123,14 @@ def main_fun(args, ctx):
     for step in range(args.steps):
       fault.maybe_inject(ctx.rank, step)
       loss = net.train_step()
+      done += 1
       if (step + 1) % 10 == 0 and ctx.is_chief:
         torch.cuda.synchronize()
         print("step {:4d} loss {:.4f} {:.0f} images/s".format(
             step + 1, float(loss), (step + 1) * B * ctx.world_size / (time.time() - t0)))
+      after_step(done)
+  if eval_steps and evaluated[0] != done:
+    evaluate(done)
   torch.cuda.synchronize()
 
 
@@ -115,6 +146,10 @@ if __name__ == "__main__":
   parser.add_argument("--learning_rate", type=float, default=1e-3)
   parser.add_argument("--input_mode", default="tf", choices=["tf", "spark"])
   parser.add_argument("--num_examples", type=int, default=2048)
+  parser.add_argument("--eval_steps", type=int, default=0,
+                      help="synthetic held-out batches per rank and evaluation (0: no evaluation)")
+  parser.add_argument("--eval_every", type=int, default=0,
+                      help="evaluate every K steps (0: only after the last step)")
   args = parser.parse_args()
   conf = SparkConf().setAppName("segmentation_spark") \
       .set("spark.executor.instances", str(args.cluster_size)) \

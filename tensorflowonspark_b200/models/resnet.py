@@ -14,7 +14,7 @@ import torch
 
 from .. import ops
 from ..ops import igemm
-from . import engine
+from . import engine, evaluation
 from .engine import BatchNorm, Conv, Dense, ParamStore, normal
 
 
@@ -93,20 +93,14 @@ class _Evaluator(object):
     self.n_valid = torch.zeros(1, dtype=torch.int32, device=dev)
     self.acc = torch.zeros(8, dtype=torch.float64, device=dev)
     self.V = net.num_classes
-    self.kind = None if comm is None else (
-        "group" if getattr(comm, "cross_host", False) else
-        "hier" if getattr(comm, "hierarchical", False) else "symm")
     if comm is None:
       self.running = net.running.tensor()
     else:
       self.running = comm.alloc("eval_running", net.running.used, torch.float32)
-    self.totals = self.peers = None
-    if self.kind in ("symm", "hier"):
-      # fp64[8] in a symmetric fp32 buffer: every rank sums all ranks' copies in rank order
-      self.totals = comm.alloc("eval_totals", 16, torch.float32).view(torch.float64)
+    self.rank_sum = evaluation.RankSum(comm, "eval_totals", 8)
     self._forward = net._eval_forward(lambda spec: st._view(self.wf, spec), bias, self.u8)
     self.graph, self.calls = None, 0
-    self.feeder = None
+    self.staging = evaluation.HostStaging(dev, net.B, self.u8.shape[1:], ())
 
   def begin(self):
     net, comm = self.net, self.comm
@@ -152,62 +146,10 @@ class _Evaluator(object):
   def run(self, batches):
     """eval_step over (images, labels) pairs; host batches are staged in page-locked memory one
     batch ahead of the forward pass."""
-    import numpy as np
-    pending = []
-
-    def flush():
-      n = pending.pop(0)
-      dx, dy = self.feeder.pop()
-      self.step(dx[:n], dy[:n])
-      self.feeder.release()
-
-    for images, labels in batches:
-      if isinstance(images, torch.Tensor) and images.is_cuda:
-        while pending:
-          flush()
-        self.step(images, labels)
-        continue
-      if self.feeder is None:
-        from ..feed import DevicePrefetcher
-        self.feeder = DevicePrefetcher([(tuple(self.u8.shape), torch.uint8),
-                                        ((self.net.B,), torch.int32)], self.net.device, depth=2)
-      x = images.numpy() if isinstance(images, torch.Tensor) else np.asarray(images)
-      y = labels.numpy() if isinstance(labels, torch.Tensor) else np.asarray(labels)
-      n = len(x)
-      if n > self.net.B:
-        raise ValueError("batch of {} rows exceeds the trainer's batch size {}".format(
-            n, self.net.B))
-      hx, hy = self.feeder.acquire_host()
-      hx.numpy()[:n] = x.reshape((n,) + tuple(self.u8.shape[1:]))
-      hy.numpy()[:n] = y.reshape(n)
-      self.feeder.push_host()
-      pending.append(n)
-      if len(pending) > 1:   # batch i + 1 is on its way: run batch i
-        flush()
-    while pending:
-      flush()
+    self.staging.run(self.step, batches)
 
   def end(self):
-    comm = self.comm
-    if self.kind is None:
-      tot = self.acc
-    elif self.kind == "group":
-      tot = self.acc.clone()
-      comm.all_reduce(tot)
-    else:
-      if self.peers is None:
-        C = ops.C()
-        self.peers = [C.tensor_from_ptr(p, [16], "f32").view(torch.float64)
-                      for p in comm.peer_ptrs("eval_totals")]
-      self.totals.copy_(self.acc)
-      comm.barrier()              # every rank's totals are written
-      tot = self.peers[0].clone()
-      for p in self.peers[1:]:
-        tot += p
-      comm.barrier()              # every rank has read them before the next pass rewrites them
-      if self.kind == "hier":
-        comm.all_reduce_inter(tot)
-    h = tot.cpu().tolist()
+    h = self.rank_sum(self.acc)
     if h[3] > 0:
       raise ValueError("evaluation saw {} label(s) outside [0, {})".format(int(h[3]), self.V))
     count = int(h[0])

@@ -16,11 +16,13 @@ which leaves shapes, FLOPs and memory traffic - everything the benchmarks measur
 """
 import math
 
+import numpy as np
 import torch
 
 from .. import ops
 from ..ops import igemm
-from .engine import BatchNorm, ParamStore, constant, he_normal
+from . import evaluation
+from .engine import BatchNorm, ParamStore, RunningArena, constant, he_normal
 
 # (expansion t, out channels c, repeats n, stride s) - MobileNetV2, width 1.0
 MBV2 = [(1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1), (6, 160, 3, 2),
@@ -47,6 +49,7 @@ class _FrozenConv(object):
     self.k, self.stride, self.act = k, stride, act
 
   def build(self, x, y):
+    self.x, self.y = x, y
     self.plan = igemm.conv_fprop(x, self.w, y, self.stride, self.k // 2, bias=self.bias,
                                  relu=self.act)
 
@@ -140,20 +143,33 @@ class _Upsample(object):
     self.sw = store.register(name + ".w", (cin, 3, 3, cout), True, he_normal(9 * cin))
     self.bn = BatchNorm(store, name + ".bn", cout)
 
-  def build(self, x, raw, act_out, g_act, g_raw, g_x, dev):
-    """x [B,h,w,cin] -> raw/act_out [B,2h,2w,cout]; g_* are the matching gradient buffers."""
+  def build(self, x, raw, act_out, g_act, g_raw, g_x, dev, running):
+    """x [B,h,w,cin] -> raw/act_out [B,2h,2w,cout]; g_* are the matching gradient buffers;
+    ``running`` (engine.RunningArena) holds the batch norm's running statistics."""
     st = self.store
-    self.bn.build(dev)
+    self.bn.build(dev, running=running)
     self.x, self.raw, self.act = x, raw, act_out
     self.g_act, self.g_raw = g_act, g_raw
     # BN statistics are fused into every parity-class launch of the transposed conv
     self.fwd = igemm.conv_dgrad(x, st.w(self.sw), raw, 2, 1, stats=self.bn.stats)
+    # inference (predict, evaluation): the same convolution without the statistics, so that it
+    # leaves nothing in the accumulators that the next training step's bn_finalize would read
+    self.fwd_inference = igemm.conv_dgrad(x, st.w(self.sw), raw, 2, 1)
     self.wgrad = igemm.conv_wgrad(x, g_raw, st.g(self.sw), 2, 1)
     self.dgrad = igemm.conv_fprop(g_raw, st.w(self.sw), g_x, 2, 1) if g_x is not None else None
 
   def forward(self, training=True):
-    self.fwd.run()
+    (self.fwd if training else self.fwd_inference).run()
     self.bn.forward(self.raw, self.act, None, 1, training)
+
+  def forward_eval(self, mean, var, scale, shift):
+    """Inference forward with the running statistics ``mean`` / ``var`` (rank 0's copy during an
+    evaluation); the batch norm's coefficients go to ``scale`` / ``shift``, the evaluator's own."""
+    self.fwd_inference.run()
+    bn = self.bn
+    ops.K.bn_inference_coeffs(bn.gamma, bn.beta, mean, var, scale, shift, bn.eps)
+    ops.C().bn_set_row_reverse(False)
+    ops.K.bn_apply(self.raw, None, scale, shift, self.act, 1, None)
 
   def backward(self):
     self.bn.backward(self.g_act, self.raw, self.act, self.g_raw, relu=True)
@@ -171,6 +187,7 @@ class UNetTrainer(object):
     assert classes <= 8
     self.device = dev = torch.device(device)
     self.B, self.image, self.classes = batch, image, classes
+    self.comm = comm
     B = batch
     self.encoder = MobileNetV2Encoder(batch, image, dev)
     skips = self.encoder.skips  # [64x64x96, 32x32x144, 16x16x192, 8x8x576, 4x4x320]
@@ -186,13 +203,15 @@ class UNetTrainer(object):
 
     x, h = skips[-1], skips[-1].shape[1]
     g_x = None  # the encoder is frozen: no gradient flows into it
+    # the decoder batch norms' running statistics, one flat buffer (checkpoints, evaluation)
+    self.running = RunningArena(dev, capacity=2 * sum(self.UP))
     self.cats, self.g_cats = [], []
     for i, up in enumerate(self.ups):
       f, skip = self.UP[i], skips[-2 - i]
       h *= 2
       raw, act = _buf((B, h, h, f), dev), _buf((B, h, h, f), dev)
       g_act, g_raw = _buf((B, h, h, f), dev), _buf((B, h, h, f), dev)
-      up.build(x, raw, act, g_act, g_raw, g_x, dev)
+      up.build(x, raw, act, g_act, g_raw, g_x, dev, self.running)
       cat = _buf((B, h, h, f + skip.shape[-1]), dev)
       g_cat = _buf(cat.shape, dev)
       self.cats.append((cat, act, skip, f))
@@ -227,13 +246,19 @@ class UNetTrainer(object):
       self.labels.copy_(labels.reshape(self.labels.shape), non_blocking=True)
 
   # ------------------------------------------------------------------ step
-  def _forward(self, training=True):
+  def _forward(self, training=True, u8=None, bn=None):
+    """Forward pass of the image batch in ``u8`` (default ``in_u8``).  ``bn``: one
+    (mean, var, scale, shift) per decoder block for an evaluation forward (_Upsample.forward_eval)."""
     K = ops.K
     # [0, 255] -> [-1, 1] (the reference normalises with x / 127.5 - 1... here (x/255 - .5)/.5)
-    K.decode_normalize(self.in_u8, self.encoder.x, 0, [0.5, 0.5, 0.5], [0.5, 0.5, 0.5])
+    K.decode_normalize(self.in_u8 if u8 is None else u8, self.encoder.x, 0, [0.5, 0.5, 0.5],
+                       [0.5, 0.5, 0.5])
     self.encoder.forward()
-    for up, (cat, act, skip, f) in zip(self.ups, self.cats):
-      up.forward(training)
+    for i, (up, (cat, act, skip, f)) in enumerate(zip(self.ups, self.cats)):
+      if bn is None:
+        up.forward(training)
+      else:
+        up.forward_eval(*bn[i])
       K.copy_channels(act, cat, f, 0, 0)
       K.copy_channels(skip, cat, skip.shape[-1], 0, f)
     self.p_last.run()
@@ -283,7 +308,191 @@ class UNetTrainer(object):
     return self.loss_sum
 
   def predict(self, images_u8=None):
+    """Logits [B, H, W, classes] of ``images_u8`` (staged into ``in_u8``), with the decoder batch
+    norms on their running statistics; accumulates no batch statistics."""
     if images_u8 is not None:
       self.set_input(images_u8)
     self._forward(False)
     return self.logits[..., :self.classes]
+
+  # ------------------------------------------------------------------ state
+  def state_dict(self):
+    """Parameters (fp32 masters, assembled across ranks when sharded) + the decoder batch norms'
+    running statistics: everything inference or a resumed run needs."""
+    sd = dict(self.store.state_dict())
+    sd["__running__"] = self.running.tensor().detach().cpu().clone()
+    return sd
+
+  def load_state_dict(self, sd):
+    """Inverse of state_dict(); a parameters-only dict (no ``__running__``) keeps the current
+    running statistics."""
+    sd = dict(sd)
+    running = sd.pop("__running__", None)
+    self.store.load_state_dict(sd)
+    if running is not None:
+      self.running.tensor().copy_(running.to(self.device))
+
+  # ------------------------------------------------------- held-out evaluation
+  def eval_begin(self):
+    """Start an evaluation pass: zero the totals and take rank 0's running statistics.
+    Stream-ordered after the last ``train_step``; the first call allocates the evaluation
+    buffers."""
+    if getattr(self, "_evaluator", None) is None:
+      self._evaluator = _SegEvaluator(self)
+    self._evaluator.begin()
+
+  def eval_step(self, images_u8, masks):
+    """Add the totals of n <= B images (uint8 [n, H, W, 3]) and their masks ([n, H, W], uint8 or
+    int32, host or device; widened on the device, out-of-range values count as invalid).  Runs
+    the forward pass on the training buffers with the running statistics, leaving ``in_u8`` /
+    ``labels`` and the training state untouched; ``logits`` then holds the batch's logits.  No
+    host sync."""
+    self._eval_state().step(images_u8, masks)
+
+  def eval_end(self):
+    """Totals summed over all ranks (identical on every rank), see seg_eval_result.  Raises
+    ValueError on every rank when any rank saw a mask value outside [0, classes)."""
+    return self._eval_state().end()
+
+  def evaluate(self, batches):
+    """eval_begin + eval_step over ``(images, masks)`` pairs + eval_end.  Host batches go through
+    page-locked staging: the copy of batch i + 1 overlaps the forward pass of batch i."""
+    self.eval_begin()
+    self._evaluator.run(batches)
+    return self.eval_end()
+
+  def _eval_state(self):
+    if getattr(self, "_evaluator", None) is None:
+      raise RuntimeError("eval_begin() has not been called")
+    return self._evaluator
+
+
+# accumulator slots of seg_eval_metrics (csrc/ops.h kSegEval*); slot SEG_IMAGES counts images
+SEG_COUNT, SEG_CORRECT, SEG_INVALID, SEG_LOSS, SEG_CONFUSION, SEG_SLOTS = 0, 1, 2, 3, 4, 68
+SEG_IMAGES, SEG_ACC = 68, 72
+
+
+def seg_eval_result(totals, classes):
+  """Host metrics from the summed accumulator ``totals`` (a sequence of SEG_ACC floats):
+  {"count": scored pixels, "images", "loss", "accuracy", "mean_iou", "iou": [classes values]}.
+  IoU of class c = cm[c, c] / (row_c + col_c - cm[c, c]) of the confusion matrix cm[label, pred];
+  a class with an empty union has IoU NaN and is left out of mean_iou (NaN when every class is).
+  loss and accuracy are means over the scored pixels (NaN when there are none).  Raises
+  ValueError when any mask value was outside [0, classes)."""
+  h = [float(v) for v in totals]
+  if h[SEG_INVALID] > 0:
+    raise ValueError("evaluation saw {} mask value(s) outside [0, {})".format(
+        int(h[SEG_INVALID]), classes))
+  count = int(h[SEG_COUNT])
+  cm = [h[SEG_CONFUSION + 8 * y:SEG_CONFUSION + 8 * y + 8] for y in range(8)]
+  iou = []
+  for c in range(classes):
+    inter = cm[c][c]
+    union = sum(cm[c][:classes]) + sum(cm[y][c] for y in range(classes)) - inter
+    iou.append(inter / union if union > 0 else float("nan"))
+  seen = [v for v in iou if v == v]
+  mean = (lambda v: v / count) if count else (lambda v: float("nan"))
+  return {"count": count, "images": int(h[SEG_IMAGES]), "loss": mean(h[SEG_LOSS]),
+          "accuracy": mean(h[SEG_CORRECT]),
+          "mean_iou": sum(seen) / len(seen) if seen else float("nan"), "iou": iou}
+
+
+def _widen(masks):
+  """Mask values as int32 without narrowing any of them: values beyond the int32 range are
+  clamped, which keeps them outside [0, classes) and so invalid."""
+  m = torch.as_tensor(masks)
+  if m.dtype in (torch.uint8, torch.int32):
+    return m
+  return m.long().clamp(-1, 2 ** 31 - 1)
+
+
+class _SegEvaluator(object):
+  """Held-out evaluation on a UNetTrainer's own buffers (eval_begin / eval_step / eval_end).
+
+  The forward pass is the inference network (transposed convolutions without batch statistics,
+  batch norms on running statistics) on the trainer's activation buffers: the next training
+  forward rewrites all of them, and backward reads only what its own forward wrote.  The bf16
+  filters and aux32 are identical on every rank; the running statistics are rank 0's - the ones
+  its checkpoint carries - so every rank scores the same model.  Only the uint8 images, int32
+  masks, per-block batch-norm coefficients and the metric accumulators are extra memory,
+  allocated on the first eval_begin."""
+
+  def __init__(self, net):
+    dev, comm = net.device, net.comm
+    self.net, self.comm, self.V = net, comm, net.classes
+    self.u8 = torch.zeros_like(net.in_u8)         # never in_u8: drivers stage a batch and replay
+    self.labels = torch.zeros_like(net.labels)
+    self.n_valid = torch.zeros(1, dtype=torch.int32, device=dev)
+    self.acc = torch.zeros(SEG_ACC, dtype=torch.float64, device=dev)
+    self.partial = torch.zeros(ops.C().seg_eval_scratch(self.labels.numel()), dtype=torch.float64,
+                               device=dev)
+    self.counter = torch.zeros(1, dtype=torch.int32, device=dev)
+    if comm is None:
+      self.running = net.running.tensor()
+    else:
+      self.running = comm.alloc("seg_eval_running", net.running.used, torch.float32)
+    base = net.running.buf.data_ptr()
+    view = lambda t: self.running[(t.data_ptr() - base) // 4:][:t.numel()]  # noqa: E731
+    self.bn = [(view(up.bn.running_mean), view(up.bn.running_var),
+                torch.zeros(up.cout, dtype=torch.float32, device=dev),
+                torch.zeros(up.cout, dtype=torch.float32, device=dev)) for up in net.ups]
+    self.rank_sum = evaluation.RankSum(comm, "seg_eval_totals", SEG_ACC)
+    self.staging = evaluation.HostStaging(dev, net.B, self.u8.shape[1:], self.labels.shape[1:])
+    self.graph, self.calls, self.images = None, 0, 0
+
+  def begin(self):
+    net, comm = self.net, self.comm
+    self.acc.zero_()
+    self.images = 0
+    if comm is not None:
+      self.running.copy_(net.running.tensor())
+      comm.broadcast("seg_eval_running", 0)
+
+  def _run(self):
+    self.net._forward(False, self.u8, self.bn)
+    ops.K.seg_eval_metrics(self.net.logits, self.labels, self.n_valid, self.acc, self.partial,
+                           self.counter, self.V)
+
+  def step(self, images_u8, masks):
+    n = len(images_u8)
+    if n > self.net.B:
+      raise ValueError("batch of {} images exceeds the trainer's batch size {}".format(
+          n, self.net.B))
+    if n:
+      x = torch.as_tensor(images_u8)
+      self.u8[:n].copy_(x.reshape((n,) + tuple(self.u8.shape[1:])), non_blocking=True)
+      self.labels[:n].copy_(_widen(masks).reshape((n,) + tuple(self.labels.shape[1:])),
+                            non_blocking=True)
+    self.n_valid.fill_(n)
+    if self.graph is None and self.calls >= 1:
+      self._capture()
+    if self.graph is not None:
+      self.graph.replay()
+    else:
+      self._run()
+    self.calls += 1
+    self.images += n
+
+  def _capture(self):
+    """The evaluation forward + metric as one CUDA graph, after one eager call; thread-local
+    capture under a cross-host communicator, as in UNetTrainer.capture."""
+    g = torch.cuda.CUDAGraph()
+    mode = "thread_local" if getattr(self.net.optim, "group_mode", False) else "global"
+    with torch.cuda.graph(g, capture_error_mode=mode):
+      self._run()
+    self.graph = g
+
+  def run(self, batches):
+    """eval_step over (images, masks) pairs; host masks are staged as uint8 when they are uint8,
+    as int32 otherwise."""
+    def host(pairs):
+      for x, y in pairs:
+        if not (isinstance(x, torch.Tensor) and x.is_cuda):
+          y = _widen(y.numpy() if isinstance(y, torch.Tensor) else np.asarray(y))
+        yield x, y
+    self.staging.run(self.step, host(batches),
+                     lambda y: torch.uint8 if y.dtype == np.uint8 else torch.int32)
+
+  def end(self):
+    self.acc[SEG_IMAGES].fill_(self.images)
+    return seg_eval_result(self.rank_sum(self.acc), self.V)
