@@ -473,6 +473,26 @@ void seg_eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& 
                                static_cast<int>(images), pixels / images, V, cur_stream()),
         "seg_eval_metrics");
 }
+void seg_predict(const Tensor& logits, Tensor mask, c10::optional<Tensor> out, int V) {
+  need(logits, torch::kBFloat16, "logits");
+  need(mask, torch::kUInt8, "mask");
+  TORCH_CHECK(logits.dim() >= 2 && logits.size(-1) == 8 && V >= 1 && V <= 8,
+              "seg_predict: logits [B, ..., 8] and V in [1, 8]");
+  const int64_t pixels = logits.numel() / 8;
+  TORCH_CHECK(mask.numel() == pixels, "seg_predict: one mask byte per pixel");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(mask.data_ptr()) % 16 == 0,
+              "seg_predict: mask must be 16-byte aligned");
+  float* o = nullptr;
+  if (out.has_value() && out->defined()) {
+    need(*out, torch::kFloat32, "out");
+    TORCH_CHECK(out->numel() == pixels * V, "seg_predict: out holds V floats per pixel");
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(out->data_ptr()) % 16 == 0,
+                "seg_predict: out must be 16-byte aligned");
+    o = out->data_ptr<float>();
+  }
+  check(tfos::seg_predict(logits.data_ptr(), mask.data_ptr<uint8_t>(), o, pixels, V, cur_stream()),
+        "seg_predict");
+}
 void cast_f32_bf16(const Tensor& in, Tensor out) {
   need(in, torch::kFloat32, "in");
   need(out, torch::kBFloat16, "out");
@@ -773,6 +793,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("eval_metrics", &eval_metrics);
   m.def("seg_eval_scratch", &seg_eval_scratch);
   m.def("seg_eval_metrics", &seg_eval_metrics);
+  m.def("seg_predict", &seg_predict);
   m.def("conv3x3_c1_fwd", &conv3x3_c1_fwd);
   m.def("conv3x3_c1_wgrad", &conv3x3_c1_wgrad);
   m.def("depthwise3x3_fwd", &depthwise3x3_fwd);

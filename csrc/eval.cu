@@ -125,19 +125,33 @@ constexpr int kSegUnroll = 4;        // pixels per thread in flight
 constexpr int kSegStep = kSegThreads * kSegUnroll;
 constexpr int kSegBins = 8 * 8 + 1;  // confusion cells y * 8 + pred, then "invalid label"
 
-// One pixel: its bin (y * 8 + pred, kSegBins - 1 for a label outside [0, V)) and loss.  pred is
-// pixel_xent_kernel's arg-max (strict > over j < V from l[0]: the lowest index wins ties), so an
-// evaluation's "correct" counts exactly what training's does.
-__device__ __forceinline__ int seg_score(const uint4 v, const int y, const int V, double& loss) {
-  if (y < 0 || y >= V) return kSegBins - 1;
-  const float2 a = unpack_bf16x2(v.x), b = unpack_bf16x2(v.y), c = unpack_bf16x2(v.z),
-               d = unpack_bf16x2(v.w);
-  const float l[8] = {a.x, a.y, b.x, b.y, c.x, c.y, d.x, d.y};
-  float mx = l[0];
+// The predicted class of one pixel: pixel_xent_kernel's arg-max, a strict > over j < V starting
+// from l[0], so the lowest index wins ties, a NaN never replaces the running maximum and channels
+// >= V are never read.  mx is the maximum that scan ends with.  Shared by evaluation (seg_score)
+// and serving (seg_predict), so a served mask is exactly the prediction evaluation scores.
+__device__ __forceinline__ int seg_argmax(const float (&l)[8], const int V, float& mx) {
+  mx = l[0];
   int am = 0;
 #pragma unroll
   for (int j = 1; j < 8; ++j)
     if (j < V && l[j] > mx) mx = l[j], am = j;
+  return am;
+}
+
+__device__ __forceinline__ void unpack_bf16x8(const uint4 v, float (&l)[8]) {
+  const float2 a = unpack_bf16x2(v.x), b = unpack_bf16x2(v.y), c = unpack_bf16x2(v.z),
+               d = unpack_bf16x2(v.w);
+  l[0] = a.x, l[1] = a.y, l[2] = b.x, l[3] = b.y, l[4] = c.x, l[5] = c.y, l[6] = d.x, l[7] = d.y;
+}
+
+// One pixel: its bin (y * 8 + pred, kSegBins - 1 for a label outside [0, V)) and loss.  pred is
+// seg_argmax, so an evaluation's "correct" counts exactly what training's does.
+__device__ __forceinline__ int seg_score(const uint4 v, const int y, const int V, double& loss) {
+  if (y < 0 || y >= V) return kSegBins - 1;
+  float l[8];
+  unpack_bf16x8(v, l);
+  float mx;
+  const int am = seg_argmax(l, V, mx);
   float se = 0.f, ly = 0.f;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
@@ -250,7 +264,74 @@ seg_eval_metrics_kernel(const __nv_bfloat16* __restrict__ logits, const int* __r
   if (threadIdx.x == 0) *counter = 0;  // ready for the next launch or graph replay
 }
 
+constexpr int kPredThreads = 128;
+constexpr int kPredWarps = kPredThreads / 32;
+constexpr int kPredPerThread = 16;                     // one 16-byte mask store per thread
+constexpr int kPredPerWarp = 32 * kPredPerThread;      // 512 pixels
+constexpr int kPredPerBlock = kPredWarps * kPredPerWarp;
+
+// Pixels [0, P) of bf16 logits [P, 8] -> mask[p] = seg_argmax (uint8) and, when out is not null,
+// out[p * V + j] = float(l_j) for j < V.  Warp w of the grid owns pixels [512 w, 512 w + 512):
+// load u (u < 16) reads pixel 512 w + 32 u + lane, so every load instruction covers 512
+// contiguous bytes and all 16 are in flight before the first use.  The 512 mask bytes are
+// transposed through shared memory so that each lane stores 16 consecutive bytes; the fp32
+// logits of the 32 pixels of one load go through shared memory too and leave as contiguous
+// 128-byte rows.  The last warp's range may end early (P need not be a multiple of anything).
+__global__ void __launch_bounds__(kPredThreads)
+seg_predict_kernel(const __nv_bfloat16* __restrict__ logits, uint8_t* __restrict__ mask,
+                   float* __restrict__ out, long long P, int V) {
+  __shared__ __align__(16) uint8_t cls[kPredWarps][kPredPerWarp];
+  __shared__ float vals[kPredWarps][32 * 8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long base =
+      (static_cast<long long>(blockIdx.x) * kPredWarps + warp) * kPredPerWarp;
+  if (base >= P) return;
+  const long long left = P - base;
+  const int count = left < kPredPerWarp ? static_cast<int>(left) : kPredPerWarp;
+  const uint4* src = reinterpret_cast<const uint4*>(logits) + base;
+  uint4 v[kPredPerThread];
+#pragma unroll
+  for (int u = 0; u < kPredPerThread; ++u) {
+    const int i = u * 32 + lane;
+    v[u] = i < count ? __ldcs(src + i) : make_uint4(0u, 0u, 0u, 0u);
+  }
+#pragma unroll
+  for (int u = 0; u < kPredPerThread; ++u) {
+    float l[8], mx;
+    unpack_bf16x8(v[u], l);
+    cls[warp][u * 32 + lane] = static_cast<uint8_t>(seg_argmax(l, V, mx));
+    if (out != nullptr) {
+      const int n = count - u * 32;          // pixels of this load inside the range
+      if (n <= 0) break;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (j < V) vals[warp][lane * V + j] = l[j];
+      __syncwarp();
+      float* dst = out + (base + u * 32) * V;
+      const int m = (n < 32 ? n : 32) * V;
+      for (int i = lane; i < m; i += 32) __stcs(dst + i, vals[warp][i]);
+      __syncwarp();
+    }
+  }
+  __syncwarp();
+  if (count == kPredPerWarp) {
+    __stcs(reinterpret_cast<uint4*>(mask + base) + lane,
+           reinterpret_cast<const uint4*>(cls[warp])[lane]);
+  } else {
+    for (int i = lane; i < count; i += 32) mask[base + i] = cls[warp][i];
+  }
+}
+
 }  // namespace
+
+cudaError_t seg_predict(const void* logits, uint8_t* mask, float* out, long long pixels, int V,
+                        cudaStream_t s) {
+  if (pixels <= 0) return cudaSuccess;
+  const long long blocks = (pixels + kPredPerBlock - 1) / kPredPerBlock;
+  seg_predict_kernel<<<static_cast<unsigned>(blocks), kPredThreads, 0, s>>>(
+      static_cast<const __nv_bfloat16*>(logits), mask, out, pixels, V);
+  return cudaGetLastError();
+}
 
 int seg_eval_grid(long long pixels) {
   long long blocks = (pixels + kSegStep - 1) / kSegStep;

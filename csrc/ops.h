@@ -235,5 +235,11 @@ int seg_eval_grid(long long pixels);
 cudaError_t seg_eval_metrics(const void* logits, const int* labels, const int* n_valid,
                              double* acc, double* partial, unsigned int* counter, int images,
                              long long ppi, int V, cudaStream_t s);
+// seg_predict (serving): pixels [0, pixels) of bf16 logits [pixels, 8] -> mask[p] = the class
+// seg_eval_metrics / pixel_xent predict (lowest index among the maxima of channels [0, V)) and,
+// when out is not null, out[p * V + j] = the fp32 value of channel j < V.  One pass; mask and out
+// must be 16-byte aligned.
+cudaError_t seg_predict(const void* logits, uint8_t* mask, float* out, long long pixels, int V,
+                        cudaStream_t s);
 
 }  // namespace tfos

@@ -87,8 +87,8 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
                         {"params": net.state_dict(), "optim": net.optim.state_dict()})
   if eval_events is not None:
     eval_events.close()
-  if args.export_dir and is_chief:
-    checkpoint.export_model(net.state_dict(), args.export_dir)
+  if args.export_dir and is_chief:   # servable: the artefact names unet.build_served
+    checkpoint.export_model(net, args.export_dir)
   return net
 
 

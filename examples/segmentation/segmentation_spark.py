@@ -10,6 +10,10 @@ Held-out evaluation (the reference's ``validation_data``): ``--eval_steps N`` sc
 batches per rank every ``--eval_every K`` steps and after the last step, in either input mode
 (``UNetTrainer.evaluate``: loss, pixel accuracy and mean IoU summed over all ranks).
 
+After the last step the chief checkpoints into ``--model_dir`` and exports into ``--export_dir``
+(both optional); either one serves through ``pipeline.TFModel`` (``unet.ServedUNet``), see
+segmentation_inference.py.
+
   python examples/segmentation/segmentation_spark.py --cluster_size 8 --batch_size 64 --steps 100
 """
 import argparse
@@ -132,6 +136,20 @@ def main_fun(args, ctx):
   if eval_steps and evaluated[0] != done:
     evaluate(done)
   torch.cuda.synchronize()
+  # the reference checkpoints into --model_dir and exports a SavedModel into --export_dir; here
+  # both name unet.build_served, so either one can be served by TFModel / the inference CLI
+  model_dir, export_dir = getattr(args, "model_dir", None), getattr(args, "export_dir", None)
+  if model_dir or export_dir:
+    if ctx.is_chief:
+      from tensorflowonspark_b200.utils import checkpoint
+      if model_dir:
+        checkpoint.save(ctx.absolute_path(model_dir), done, net.state_dict(), model=net)
+      if export_dir:
+        checkpoint.export_model(net, ctx.absolute_path(export_dir))
+    if comm is not None:
+      # the chief's state_dict() reads the peers' parameter shards: they stay until it is done
+      comm.barrier()
+      torch.cuda.synchronize()
 
 
 if __name__ == "__main__":
@@ -150,6 +168,10 @@ if __name__ == "__main__":
                       help="synthetic held-out batches per rank and evaluation (0: no evaluation)")
   parser.add_argument("--eval_every", type=int, default=0,
                       help="evaluate every K steps (0: only after the last step)")
+  parser.add_argument("--model_dir", default=None,
+                      help="checkpoint written by the chief after the last step (servable)")
+  parser.add_argument("--export_dir", default=None,
+                      help="inference artefact exported by the chief after the last step")
   args = parser.parse_args()
   conf = SparkConf().setAppName("segmentation_spark") \
       .set("spark.executor.instances", str(args.cluster_size)) \

@@ -38,9 +38,10 @@ class ParamStore(object):
     self._specs.append(spec)
     return spec
 
-  def finalize(self, device, alloc=None, seed=1234):
+  def finalize(self, device, alloc=None, seed=1234, grads=True):
     """alloc(nbytes_name, numel, dtype) -> tensor lets the caller place the buffers in
-    symmetric (peer-mapped) memory; default is ordinary device memory."""
+    symmetric (peer-mapped) memory; default is ordinary device memory.  ``grads=False`` (an
+    inference-only model) allocates no gradient buffer: ``g()`` then returns None."""
     order = [s for s in self._specs if s["decay"]] + [s for s in self._specs if not s["decay"]]
     off = 0
     for s in order:
@@ -54,7 +55,7 @@ class ParamStore(object):
       alloc = lambda name, n, dt: torch.zeros(n, dtype=dt, device=device)  # noqa: E731
     self.master = alloc("master", self.total, torch.float32)  # symmetric too: broadcastable
     self.weights = alloc("weights", self.total, torch.bfloat16)
-    self.grads = alloc("grads", self.total, torch.float32)
+    self.grads = alloc("grads", self.total, torch.float32) if grads else None
     # fp32 replica of the non-decayed tail (BN scale/offset are consumed in fp32)
     self.aux32 = alloc("aux32", max(8, self.total - self.decay_end), torch.float32)
     gen = torch.Generator(device="cpu")
@@ -74,7 +75,7 @@ class ParamStore(object):
     return self._view(self.weights, s)
 
   def g(self, s):
-    return self._view(self.grads, s)
+    return None if self.grads is None else self._view(self.grads, s)
 
   def m(self, s):
     return self._view(self.master, s)

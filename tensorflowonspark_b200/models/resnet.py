@@ -14,7 +14,7 @@ import torch
 
 from .. import ops
 from ..ops import igemm
-from . import engine, evaluation
+from . import engine, evaluation, serving
 from .engine import BatchNorm, Conv, Dense, ParamStore, normal
 
 
@@ -662,15 +662,14 @@ class ResNetTrainer(object):
       self.running.tensor().copy_(running.to(self.device))
 
 
-class ServedResNet(object):
+class ServedResNet(serving.Replica):
   """Inference callable behind ``pipeline.TFModel`` / ``TFParallel``: one bf16 replica on the
   executor's GPU.  ``submit(inputs)`` stages a uint8 NHWC batch in page-locked memory, copies it
-  on the copy stream and enqueues the forward pass + an async read-back of the results;
-  ``collect()`` returns the oldest submitted batch - so the H2D copy of batch i+1 and the host's
-  row handling overlap the kernels of batch i (pipeline._run_model drives it one batch ahead)."""
+  on the copy stream and enqueues the forward pass (~165 launches) + arg-max and an async
+  read-back of ``logits`` and ``prediction``; ``collect()`` returns the oldest submitted batch
+  (models/serving.Replica)."""
 
   def __init__(self, state, depth=50, image=224, num_classes=1000, batch=256, device="cuda:0"):
-    from ..feed import DevicePrefetcher
     torch.cuda.set_device(torch.device(device))
     self.net = ResNetTrainer(depth=depth, batch=batch, image=image, num_classes=num_classes,
                              device=device, training=False)
@@ -679,125 +678,22 @@ class ServedResNet(object):
     if self.folded:
       self.net.build_folded_inference()
     self._fwd = self.net.forward_folded if self.folded else (lambda: self.net._forward(False))
-    self.B, self.image, self.V = batch, image, num_classes
-    dev = self.net.device
-    self.feeder = DevicePrefetcher([((batch, image, image, 3), torch.uint8)], dev, depth=2)
-    self.h_logits = [torch.empty(batch, num_classes, dtype=torch.float32).pin_memory()
-                     for _ in range(2)]
-    self.h_pred = [torch.empty(batch, dtype=torch.int64).pin_memory() for _ in range(2)]
-    self.done = [torch.cuda.Event() for _ in range(2)]
-    self._pending = []
-    self._k = 0
-    self.pred_dev = torch.zeros(batch, dtype=torch.int64, device=dev)
-    self.graph, self._batches = None, 0
-    self.use_graph = os.environ.get("TFOS_SERVE_GRAPH", "1") == "1"
-    self.copy_threads = max(1, int(os.environ.get("TFOS_SERVE_COPY_THREADS", "4")))
-    if self.copy_threads > 1:
-      from concurrent.futures import ThreadPoolExecutor
-      self._pool = ThreadPoolExecutor(max_workers=self.copy_threads, thread_name_prefix="tfos-stage")
+    self.image, self.V = image, num_classes
+    self.pred_dev = torch.zeros(batch, dtype=torch.int64, device=self.net.device)
+    super(ServedResNet, self).__init__(
+        self.net.device, batch, (image, image, 3),
+        {"logits": self.net.logits[:, :num_classes], "prediction": self.pred_dev},
+        self.net.set_input)
 
-  def submit(self, inputs):
-    import numpy as np
-    x = inputs["image"] if isinstance(inputs, dict) else inputs
-    x = np.asarray(x)
-    n = len(x)
-    if n > self.B:
-      raise ValueError("batch of {} rows exceeds the served batch size {}".format(n, self.B))
-    x = x.reshape(n, self.image, self.image, 3)
-    if n < self.B:   # ragged tail: pad (the padded rows' outputs are dropped)
-      x = np.concatenate([x, np.zeros((self.B - n,) + x.shape[1:], dtype=x.dtype)])
-    self.feeder.push_arrays([x])
-    self._enqueue(n)
-
-  def submit_rows(self, columns):
-    """Same as :meth:`submit` for a column of raw row cells (bytes / memoryview / ndarray, one
-    uint8 HWC image each): every row is copied ONCE, straight into the page-locked staging
-    buffer the H2D copy reads - no intermediate batch array (pipeline._run_model uses this when a
-    served model offers it)."""
-    import numpy as np
-    rows = columns["image"] if isinstance(columns, dict) else columns
-    n = len(rows)
-    if n > self.B:
-      raise ValueError("batch of {} rows exceeds the served batch size {}".format(n, self.B))
-    (host,) = self.feeder.acquire_host()
-    hv = host.numpy().reshape(self.B, -1)
-
-    def fill(lo, hi):
-      for r in range(lo, hi):
-        row = rows[r]
-        hv[r] = np.frombuffer(row, dtype=np.uint8) if not isinstance(row, np.ndarray) \
-            else row.reshape(-1)
-
-    # 38.5 MB per 256-image batch: one thread copies ~5 GB/s, which is slower than the GPU
-    # consumes it (8.5 vs 6.5 ms per batch); numpy releases the GIL during the copies, so a few
-    # threads fill disjoint row ranges of the staging buffer in parallel
-    k = self.copy_threads
-    if k > 1 and n >= 4 * k:
-      step = (n + k - 1) // k
-      list(self._pool.map(lambda i: fill(i * step, min(n, (i + 1) * step)), range(k)))
-    else:
-      fill(0, n)
-    if n < self.B:
-      hv[n:] = 0
-    self.feeder.push_host()
-    self._enqueue(n)
-
-  def _capture(self):
-    """The whole forward pass (~165 launches) + arg-max as ONE CUDA graph: the host thread that
-    also fills the staging buffers spends microseconds, not a millisecond, per batch on launches."""
-    dev = self.net.device
-    cur = torch.cuda.current_stream(dev)
-    side = torch.cuda.Stream(device=dev)
-    side.wait_stream(cur)
-    with torch.cuda.stream(side):
-      self._fwd()
-      self.pred_dev.copy_(self.net.logits[:, :self.V].argmax(1))
-    cur.wait_stream(side)
-    torch.cuda.synchronize(dev)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-      self._fwd()
-      self.pred_dev.copy_(self.net.logits[:, :self.V].argmax(1))
-    self.graph = g
-
-  def _enqueue(self, n):
-    (dx,) = self.feeder.pop()
-    self.net.set_input(dx)
-    self.feeder.release()
-    if self.graph is None and self.use_graph and self._batches >= 1:
-      self._capture()
-    if self.graph is not None:
-      self.graph.replay()
-    else:
-      self._fwd()
-      self.pred_dev.copy_(self.net.logits[:, :self.V].argmax(1))
-    self._batches += 1
-    logits = self.net.logits
-    k = self._k
-    self._k ^= 1
-    self.h_logits[k].copy_(logits[:, :self.V], non_blocking=True)
-    self.h_pred[k].copy_(self.pred_dev, non_blocking=True)
-    self.done[k].record(torch.cuda.current_stream(self.net.device))
-    self._pending.append((k, n))
-
-  def collect(self):
-    k, n = self._pending.pop(0)
-    self.done[k].synchronize()
-    return {"logits": self.h_logits[k][:n].numpy().copy(),
-            "prediction": self.h_pred[k][:n].numpy().copy()}
-
-  def pending(self):
-    return len(self._pending)
-
-  def __call__(self, **inputs):
-    self.submit(inputs)
-    return self.collect()
+  def _run(self):
+    self._fwd()
+    self.pred_dev.copy_(self.net.logits[:, :self.V].argmax(1))
 
 
 def build_served(state, depth=50, image=224, num_classes=1000, batch=None, **_):
   """Export builder (utils/checkpoint.py): rebuilds the replica on the executor's GPU."""
-  batch = int(batch or os.environ.get("TFOS_SERVE_BATCH", "256"))
-  return ServedResNet(state, depth=depth, image=image, num_classes=num_classes, batch=batch)
+  return ServedResNet(state, depth=depth, image=image, num_classes=num_classes,
+                      batch=serving.serve_batch(batch))
 
 
 class CifarResNetTrainer(object):

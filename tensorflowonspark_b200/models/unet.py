@@ -21,7 +21,7 @@ import torch
 
 from .. import ops
 from ..ops import igemm
-from . import evaluation
+from . import evaluation, serving
 from .engine import BatchNorm, ParamStore, RunningArena, constant, he_normal
 
 # (expansion t, out channels c, repeats n, stride s) - MobileNetV2, width 1.0
@@ -143,18 +143,23 @@ class _Upsample(object):
     self.sw = store.register(name + ".w", (cin, 3, 3, cout), True, he_normal(9 * cin))
     self.bn = BatchNorm(store, name + ".bn", cout)
 
-  def build(self, x, raw, act_out, g_act, g_raw, g_x, dev, running):
+  def build(self, x, raw, act_out, g_act, g_raw, g_x, dev, running, training=True):
     """x [B,h,w,cin] -> raw/act_out [B,2h,2w,cout]; g_* are the matching gradient buffers;
-    ``running`` (engine.RunningArena) holds the batch norm's running statistics."""
+    ``running`` (engine.RunningArena) holds the batch norm's running statistics.
+    ``training=False``: only the inference convolution is planned (g_* are not used)."""
     st = self.store
     self.bn.build(dev, running=running)
     self.x, self.raw, self.act = x, raw, act_out
     self.g_act, self.g_raw = g_act, g_raw
-    # BN statistics are fused into every parity-class launch of the transposed conv
-    self.fwd = igemm.conv_dgrad(x, st.w(self.sw), raw, 2, 1, stats=self.bn.stats)
+    self.fwd = self.wgrad = self.dgrad = None
+    if training:
+      # BN statistics are fused into every parity-class launch of the transposed conv
+      self.fwd = igemm.conv_dgrad(x, st.w(self.sw), raw, 2, 1, stats=self.bn.stats)
     # inference (predict, evaluation): the same convolution without the statistics, so that it
     # leaves nothing in the accumulators that the next training step's bn_finalize would read
     self.fwd_inference = igemm.conv_dgrad(x, st.w(self.sw), raw, 2, 1)
+    if not training:
+      return
     self.wgrad = igemm.conv_wgrad(x, g_raw, st.g(self.sw), 2, 1)
     self.dgrad = igemm.conv_fprop(g_raw, st.w(self.sw), g_x, 2, 1) if g_x is not None else None
 
@@ -179,15 +184,19 @@ class _Upsample(object):
 
 
 class UNetTrainer(object):
-  """Static-buffer U-Net for ``batch`` images of ``image`` x ``image`` x 3 and ``classes`` labels."""
+  """Static-buffer U-Net for ``batch`` images of ``image`` x ``image`` x 3 and ``classes`` labels.
+  ``training=False`` builds only what the forward pass needs (predict, evaluate, serving): no
+  gradient buffers, no backward or statistics-fused plans and no optimizer (``optim`` is None)."""
 
   UP = (512, 256, 128, 64)
 
-  def __init__(self, batch=64, image=128, classes=3, device="cuda:0", lr=1e-3, comm=None, seed=1234):
+  def __init__(self, batch=64, image=128, classes=3, device="cuda:0", lr=1e-3, comm=None, seed=1234,
+               training=True):
     assert classes <= 8
     self.device = dev = torch.device(device)
     self.B, self.image, self.classes = batch, image, classes
     self.comm = comm
+    self.training = tr = training
     B = batch
     self.encoder = MobileNetV2Encoder(batch, image, dev)
     skips = self.encoder.skips  # [64x64x96, 32x32x144, 16x16x192, 8x8x576, 4x4x320]
@@ -199,7 +208,7 @@ class UNetTrainer(object):
       cin = f + skips[-2 - i].shape[-1]
     self.s_last = st.register("last.w", (cin, 3, 3, 8), True, he_normal(9 * cin))
     self.s_last_b = st.register("last.b", (8,), False, constant(0.0))
-    st.finalize(dev, alloc=comm.alloc if comm is not None else None, seed=seed)
+    st.finalize(dev, alloc=comm.alloc if comm is not None else None, seed=seed, grads=tr)
 
     x, h = skips[-1], skips[-1].shape[1]
     g_x = None  # the encoder is frozen: no gradient flows into it
@@ -210,25 +219,31 @@ class UNetTrainer(object):
       f, skip = self.UP[i], skips[-2 - i]
       h *= 2
       raw, act = _buf((B, h, h, f), dev), _buf((B, h, h, f), dev)
-      g_act, g_raw = _buf((B, h, h, f), dev), _buf((B, h, h, f), dev)
-      up.build(x, raw, act, g_act, g_raw, g_x, dev, self.running)
+      g_act = g_raw = g_cat = None
+      if tr:
+        g_act, g_raw = _buf((B, h, h, f), dev), _buf((B, h, h, f), dev)
+      up.build(x, raw, act, g_act, g_raw, g_x, dev, self.running, training=tr)
       cat = _buf((B, h, h, f + skip.shape[-1]), dev)
-      g_cat = _buf(cat.shape, dev)
+      if tr:
+        g_cat = _buf(cat.shape, dev)
+        self.g_cats.append((g_cat, g_act, f))
       self.cats.append((cat, act, skip, f))
-      self.g_cats.append((g_cat, g_act, f))
       x, g_x = cat, g_cat
     h *= 2
     self.logits = _buf((B, h, h, 8), dev)
-    self.dlogits = _buf((B, h, h, 8), dev)
+    self.dlogits = _buf((B, h, h, 8), dev) if tr else None
     self.labels = torch.zeros(B, h, h, dtype=torch.int32, device=dev)
     self.p_last = igemm.conv_dgrad(x, st.w(self.s_last), self.logits, 2, 1, bias=st.f32(self.s_last_b))
-    self.p_last_wgrad = igemm.conv_wgrad(x, self.dlogits, st.g(self.s_last), 2, 1)
-    self.p_last_dgrad = igemm.conv_fprop(self.dlogits, st.w(self.s_last), g_x, 2, 1)
+    self.p_last_wgrad = self.p_last_dgrad = self.optim = None
+    if tr:
+      self.p_last_wgrad = igemm.conv_wgrad(x, self.dlogits, st.g(self.s_last), 2, 1)
+      self.p_last_dgrad = igemm.conv_fprop(self.dlogits, st.w(self.s_last), g_x, 2, 1)
     self.loss_sum = torch.zeros(1, dtype=torch.float32, device=dev)
     self.correct = torch.zeros(1, dtype=torch.float32, device=dev)
     self.in_u8 = _buf((B, image, image, 3), dev, torch.uint8)
-    from ..parallel.fused_optim import FusedOptimizer
-    self.optim = FusedOptimizer(st, comm=comm, opt="adam", lr=lr, weight_decay=0.0)
+    if tr:
+      from ..parallel.fused_optim import FusedOptimizer
+      self.optim = FusedOptimizer(st, comm=comm, opt="adam", lr=lr, weight_decay=0.0)
     self.graph = None
 
   # ------------------------------------------------------------------ data
@@ -264,6 +279,8 @@ class UNetTrainer(object):
     self.p_last.run()
 
   def step_kernels(self):
+    if not self.training:
+      raise RuntimeError("this UNetTrainer was built with training=False: it cannot train")
     K = ops.K
     self._forward(True)
     self.loss_sum.zero_()
@@ -318,19 +335,48 @@ class UNetTrainer(object):
   # ------------------------------------------------------------------ state
   def state_dict(self):
     """Parameters (fp32 masters, assembled across ranks when sharded) + the decoder batch norms'
-    running statistics: everything inference or a resumed run needs."""
+    running statistics (``__running__``) + the frozen encoder (``__encoder__``: one (bf16 filter,
+    fp32 bias) pair per convolution of ``encoder.layers``, in that order, as the forward uses
+    them): everything inference or a resumed run needs, independent of the loading host's RNG."""
     sd = dict(self.store.state_dict())
     sd["__running__"] = self.running.tensor().detach().cpu().clone()
+    sd["__encoder__"] = [(c.w.detach().cpu().clone(), c.bias.detach().cpu().clone())
+                         for c in self._encoder_convs()]
     return sd
 
   def load_state_dict(self, sd):
-    """Inverse of state_dict(); a parameters-only dict (no ``__running__``) keeps the current
-    running statistics."""
+    """Inverse of state_dict(); a dict without ``__running__`` keeps the current running
+    statistics, one without ``__encoder__`` (checkpoints written before the encoder was part of
+    the state) keeps the seeded encoder."""
     sd = dict(sd)
     running = sd.pop("__running__", None)
+    encoder = sd.pop("__encoder__", None)
+    if encoder is not None:
+      convs = self._encoder_convs()
+      if len(encoder) != len(convs) or any(
+          w.shape != c.w.shape or b.shape != c.bias.shape for c, (w, b) in zip(convs, encoder)):
+        raise ValueError("__encoder__ does not match this U-Net's encoder ({} convolutions)".format(
+            len(convs)))
+      for c, (w, b) in zip(convs, encoder):
+        c.w.copy_(w.to(self.device, torch.bfloat16))
+        c.bias.copy_(b.to(self.device, torch.float32))
     self.store.load_state_dict(sd)
     if running is not None:
       self.running.tensor().copy_(running.to(self.device))
+
+  def _encoder_convs(self):
+    return [c for c in self.encoder.layers if not isinstance(c, _Residual)]
+
+  # ------------------------------------------------------------------ serving
+  export_builder = "tensorflowonspark_b200.models.unet:build_served"
+  export_signatures = {"serving_default": {
+      "inputs": {"image": "image"}, "outputs": {"mask": "mask", "logits": "logits"},
+      "input_dtypes": {"image": "uint8"},
+      "output_dtypes": {"mask": "uint8", "logits": "float32"}}}
+
+  @property
+  def export_builder_args(self):
+    return {"image": self.image, "classes": self.classes}
 
   # ------------------------------------------------------- held-out evaluation
   def eval_begin(self):
@@ -496,3 +542,42 @@ class _SegEvaluator(object):
   def end(self):
     self.acc[SEG_IMAGES].fill_(self.images)
     return seg_eval_result(self.rank_sum(self.acc), self.V)
+
+
+class ServedUNet(serving.Replica):
+  """Inference callable behind ``pipeline.TFModel`` / the inference CLI: one bf16 U-Net replica
+  (a ``training=False`` trainer) on the executor's GPU.  Input ``image``: uint8 [n, H, W, 3] (or
+  one row cell of H*W*3 bytes per image).  Outputs ``mask``: uint8 [n, H, W], the class every
+  pixel is predicted as - exactly the prediction evaluation scores (seg_predict); ``logits``:
+  fp32 [n, H, W, classes].  The forward pass + seg_predict run as one CUDA graph after the first
+  batch; ``select_outputs`` keeps the logits (12x the bytes of the mask at 3 classes) on the
+  device unless they are asked for (models/serving.Replica)."""
+
+  def __init__(self, state, image=128, classes=3, batch=256, device="cuda:0"):
+    torch.cuda.set_device(torch.device(device))
+    self.net = UNetTrainer(batch=batch, image=image, classes=classes, device=device,
+                           training=False)
+    self.net.load_state_dict(state)
+    self.image, self.V = image, classes
+    dev = self.net.device
+    self.mask = torch.zeros(batch, image, image, dtype=torch.uint8, device=dev)
+    self.logits = torch.zeros(batch, image, image, classes, dtype=torch.float32, device=dev)
+    super(ServedUNet, self).__init__(dev, batch, (image, image, 3),
+                                     {"mask": self.mask, "logits": self.logits},
+                                     self.net.set_input)
+
+  def select_outputs(self, names):
+    """Compute and read back only the outputs ``names`` (``mask`` and / or ``logits``) from the
+    next batch on; ValueError for a name the model does not offer."""
+    self._select_outputs(names)
+
+  def _run(self):
+    self.net._forward(False)
+    ops.K.seg_predict(self.net.logits, self.mask,
+                      self.logits if "logits" in self.selected else None, self.V)
+
+
+def build_served(state, image=128, classes=3, batch=None, **_):
+  """Export builder (utils/checkpoint.py): rebuilds the replica on the executor's GPU with
+  ``TFOS_SERVE_BATCH`` rows per batch unless ``batch`` is given."""
+  return ServedUNet(state, image=image, classes=classes, batch=serving.serve_batch(batch))

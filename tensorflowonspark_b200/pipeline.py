@@ -316,6 +316,11 @@ def _run_model(iterator, args, tf_args):
   out_names = [t for t, _ in sorted(args.output_mapping.items())]
   shapes = signature.get("input_shapes", {})
   dtypes = signature.get("input_dtypes", {})
+  # outputs the signature declares a dtype for travel as one bytes cell per row (a BinaryType
+  # column) - a 128x128 mask would otherwise become 16,384 Python ints per row
+  out_dtypes = signature.get("output_dtypes", {})
+  if hasattr(model, "select_outputs"):
+    model.select_outputs(out_names)
 
   def emit(outputs, n):
     if not isinstance(outputs, dict):
@@ -331,7 +336,11 @@ def _run_model(iterator, args, tf_args):
       else:
         o = np.asarray(o)
       assert len(o) == n, "output '{}' has {} rows, expected {}".format(t, len(o), n)
-      cols.append(o.tolist())   # Row cells must be plain Python values
+      if t in out_dtypes:
+        o = np.ascontiguousarray(o, dtype=out_dtypes[t])
+        cols.append([o[i].tobytes() for i in range(n)])
+      else:
+        cols.append(o.tolist())   # Row cells must be plain Python values
     return zip(*cols)
 
   pipelined = hasattr(model, "submit") and hasattr(model, "collect")
