@@ -194,7 +194,45 @@ py::dict plan_info(int64_t h) {
   d["bn"] = p->bn;
   d["grid"] = p->grid;
   d["total_work"] = p->total_work;
-  if (p->kind == 0) d["epi_prefetch"] = p->fa.epi_prefetch;
+  if (p->kind == 0) {
+    // the kernel instance the plan launches (igemm_fwd_kernel<bn, b_mn, epi>), its mode and the
+    // tile geometry: enough to name every M box and output pixel the launch covers
+    const tfos::FwdArgs& f = p->fa;
+    d["epi_prefetch"] = f.epi_prefetch;
+    d["epi"] = p->epi;
+    d["b_mn"] = p->b_mn;
+    d["b_resident"] = f.b_resident;
+    d["a_stages"] = f.a_stages;
+    d["reverse"] = f.reverse;
+    d["stem"] = f.stem;
+    d["tiles_w"] = f.tiles_w;
+    d["tiles_h"] = f.tiles_h;
+    d["tiles_n"] = f.tiles_n;
+    d["box_w"] = f.box_w;
+    d["box_h"] = f.box_h;
+    d["box_n"] = f.box_n;
+    d["n_tiles"] = f.n_tiles;
+    d["osw"] = f.osw;
+    d["oow"] = f.oow;
+    d["osh"] = f.osh;
+    d["ooh"] = f.ooh;
+    d["lim_w"] = f.lim_w;
+    d["lim_h"] = f.lim_h;
+    d["lim_n"] = f.lim_n;
+  } else {
+    const tfos::WgradArgs& w = p->wa;
+    d["stem"] = w.stem;   // 0 generic kernel, 1 stem halo, 2 one-pass 3x3 halo
+    d["k_splits"] = w.k_splits;
+    d["halo_stages"] = w.halo_stages;
+    d["m_tiles"] = w.m_tiles;
+    d["n_tiles"] = w.n_tiles;
+    // the pixel boxes the K (pixel) loop walks: with grid and total_work (generic kernel) or
+    // k_splits (halo kernels) they give how many pixels one CTA accumulates before its atomic add
+    d["box_rows"] = w.box_rows;
+    d["tiles_w"] = w.tiles_w;
+    d["tiles_h"] = w.tiles_h;
+    d["tiles_n"] = w.tiles_n;
+  }
   return d;
 }
 

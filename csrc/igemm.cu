@@ -533,8 +533,8 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               n2.x += (pm & 1u) ? p2.x : 0.f;
               n2.y += (pm & 2u) ? p2.y : 0.f;
               if (relu_on) {
-                n2.x = fmaxf(n2.x, 0.f);
-                n2.y = fmaxf(n2.y, 0.f);
+                n2.x = fminf(fmaxf(n2.x, 0.f), relu_cap);
+                n2.y = fminf(fmaxf(n2.y, 0.f), relu_cap);
               }
               w[k] = pack_bf16x2(n2.x, n2.y);
             }
@@ -588,7 +588,10 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               float* o = reinterpret_cast<float*>(a.out);
               if (valid[h]) {
                 if (a.accumulate && cv) f[j] += o[e];
-                if (a.relu) f[j] = fmaxf(f[j], 0.f);
+                if (a.relu) {
+                  f[j] = fmaxf(f[j], 0.f);
+                  if (a.relu == 2) f[j] = fminf(f[j], 6.f);
+                }
                 if (cv) o[e] = f[j];
               }
             } else {
