@@ -556,6 +556,70 @@ void depthwise3x3_fwd(const Tensor& x, const Tensor& w, c10::optional<Tensor> bi
                                x.size(1), x.size(2), x.size(3), stride, act, cur_stream()),
         "depthwise3x3_fwd");
 }
+int64_t depthwise3x3_bwd_scratch(int64_t N, int64_t H, int64_t C, int64_t stride) {
+  TORCH_CHECK(N > 0 && H > 0 && C > 0 && C % 8 == 0 && (stride == 1 || stride == 2),
+              "depthwise3x3_bwd_scratch: N, H > 0, C % 8 == 0, stride 1 or 2");
+  return tfos::depthwise3x3_bwd_scratch(N, H, C, stride);
+}
+inline bool aligned16(const Tensor& t) {
+  return reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0;
+}
+void depthwise3x3_bwd(const Tensor& x, const Tensor& w, const Tensor& y, const Tensor& dy,
+                      c10::optional<Tensor> add, int64_t add_off, Tensor dx, Tensor dw, Tensor dbias,
+                      Tensor dbias_in, Tensor scratch, int64_t stride) {
+  need(x, torch::kBFloat16, "x");
+  need(w, torch::kBFloat16, "w");
+  need(y, torch::kBFloat16, "y");
+  need(dy, torch::kBFloat16, "dy");
+  need(dx, torch::kBFloat16, "dx");
+  need(dw, torch::kFloat32, "dw");
+  need(dbias, torch::kFloat32, "dbias");
+  need(dbias_in, torch::kFloat32, "dbias_in");
+  need(scratch, torch::kFloat32, "scratch");
+  TORCH_CHECK(stride == 1 || stride == 2, "depthwise3x3_bwd: stride must be 1 or 2");
+  TORCH_CHECK(x.dim() == 4, "depthwise3x3_bwd: x must be [N, H, W, C]");
+  const int64_t N = x.size(0), H = x.size(1), W = x.size(2), C = x.size(3);
+  const int64_t OH = (H - 1) / stride + 1, OW = (W - 1) / stride + 1;
+  TORCH_CHECK(N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0,
+              "depthwise3x3_bwd: non-empty x with C % 8 == 0");
+  TORCH_CHECK(N * OH < (int64_t(1) << 31) && N * H * W * C < (int64_t(1) << 40),
+              "depthwise3x3_bwd: tensor too large");
+  TORCH_CHECK(w.sizes() == torch::IntArrayRef({9, C}), "depthwise3x3_bwd: w must be [9, C]");
+  TORCH_CHECK(y.sizes() == torch::IntArrayRef({N, OH, OW, C}) && dy.sizes() == y.sizes(),
+              "depthwise3x3_bwd: y and dy must be [N, (H-1)/s+1, (W-1)/s+1, C]");
+  TORCH_CHECK(dx.sizes() == x.sizes(), "depthwise3x3_bwd: dx must have the shape of x");
+  TORCH_CHECK(dw.sizes() == w.sizes(), "depthwise3x3_bwd: dw must be [9, C]");
+  TORCH_CHECK(dbias.numel() == C && dbias_in.numel() == C,
+              "depthwise3x3_bwd: dbias and dbias_in hold C floats");
+  TORCH_CHECK(scratch.numel() >= depthwise3x3_bwd_scratch(N, H, C, stride),
+              "depthwise3x3_bwd: scratch needs depthwise3x3_bwd_scratch(N, H, C, stride) floats");
+  for (const Tensor& t : {x, w, y, dy, dx})
+    TORCH_CHECK(aligned16(t), "depthwise3x3_bwd: bf16 tensors must be 16-byte aligned");
+  for (const Tensor& t : {w, y, dy, dx, dw, dbias, dbias_in, scratch})
+    TORCH_CHECK(t.device() == x.device(), "depthwise3x3_bwd: tensors on different devices");
+  const void* ap = nullptr;
+  int ld = 0;
+  if (add.has_value() && add->defined()) {
+    need(*add, torch::kBFloat16, "add");
+    TORCH_CHECK(add->device() == x.device(), "depthwise3x3_bwd: add on another device");
+    TORCH_CHECK(add->dim() == 4 && add->size(0) == N && add->size(1) == H && add->size(2) == W,
+                "depthwise3x3_bwd: add must be [N, H, W, ld]");
+    const int64_t L = add->size(3);
+    TORCH_CHECK(L % 8 == 0 && add_off % 8 == 0 && add_off >= 0 && add_off + C <= L,
+                "depthwise3x3_bwd: the add slice [add_off, add_off + C) must lie inside the ",
+                "channels of add, with ld and add_off multiples of 8");
+    TORCH_CHECK(aligned16(*add), "depthwise3x3_bwd: add must be 16-byte aligned");
+    ap = static_cast<const at::BFloat16*>(add->data_ptr()) + add_off;
+    ld = static_cast<int>(L);
+  } else {
+    TORCH_CHECK(add_off == 0, "depthwise3x3_bwd: add_off without add");
+  }
+  check(tfos::depthwise3x3_bwd(x.data_ptr(), w.data_ptr(), y.data_ptr(), dy.data_ptr(), ap, ld,
+                               dx.data_ptr(), dw.data_ptr<float>(), dbias.data_ptr<float>(),
+                               dbias_in.data_ptr<float>(), scratch.data_ptr<float>(), N, H, W, C,
+                               stride, cur_stream()),
+        "depthwise3x3_bwd");
+}
 void copy_channels(const Tensor& src, Tensor dst, int C, int src_off, int dst_off) {
   need(src, torch::kBFloat16, "src");
   need(dst, torch::kBFloat16, "dst");
@@ -835,6 +899,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv3x3_c1_fwd", &conv3x3_c1_fwd);
   m.def("conv3x3_c1_wgrad", &conv3x3_c1_wgrad);
   m.def("depthwise3x3_fwd", &depthwise3x3_fwd);
+  m.def("depthwise3x3_bwd_scratch", &depthwise3x3_bwd_scratch, py::arg("N"), py::arg("H"),
+        py::arg("C"), py::arg("stride"));
+  m.def("depthwise3x3_bwd", &depthwise3x3_bwd, py::arg("x"), py::arg("w"), py::arg("y"),
+        py::arg("dy"), py::arg("add"), py::arg("add_off"), py::arg("dx"), py::arg("dw"),
+        py::arg("dbias"), py::arg("dbias_in"), py::arg("scratch"), py::arg("stride"));
   m.def("copy_channels", &copy_channels);
   m.def("pixel_xent", &pixel_xent);
   m.def("allreduce_opt", &allreduce_opt);

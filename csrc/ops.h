@@ -205,6 +205,18 @@ cudaError_t conv3x3_c1_wgrad(const void* x, const void* dy, float* dw, float* db
                              int W, int Cout, cudaStream_t s);
 cudaError_t depthwise3x3_fwd(const void* x, const void* w, const float* bias, void* y, int N,
                              int H, int W, int C, int stride, int act, cudaStream_t s);
+// Backward of a depthwise 3x3 (pad 1, stride 1 or 2) whose output y and input x are both ReLU6
+// outputs, r(v) = [0 < v < 6] on the stored bf16 values, g = dy * r(y):
+//   dw[t, c] = sum g * x_tap, dbias[c] = sum g        (fp32, written)
+//   dx = bf16((sum over taps of g * w + add) * r(x)), dbias_in[c] = sum of the stored dx (fp32)
+// add (may be null): channel slice of a [N, H, W, add_ld] tensor, already offset to its first
+// channel.  scratch: depthwise3x3_bwd_scratch() floats, zero before the first launch; the kernel
+// leaves its counters at zero.  Deterministic: no float atomics, fixed reduction order.
+long long depthwise3x3_bwd_scratch(int N, int H, int C, int stride);
+cudaError_t depthwise3x3_bwd(const void* x, const void* w, const void* y, const void* dy,
+                             const void* add, int add_ld, void* dx, float* dw, float* dbias,
+                             float* dbias_in, float* scratch, int N, int H, int W, int C,
+                             int stride, cudaStream_t s);
 
 // ---- held-out evaluation (eval.cu)
 // bn_fold: row u of tab [units][kFoldCols] describes one convolution + batch norm.  Offsets are

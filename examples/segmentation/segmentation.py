@@ -1,6 +1,8 @@
 """Image segmentation U-Net on ONE H100, no Spark (reference: examples/segmentation/
 segmentation.py - the notebook-derived single-node script; model at segmentation_spark.py:67-119):
 frozen MobileNetV2 encoder, four transposed-conv up-blocks, per-pixel softmax cross-entropy, Adam.
+``--encoder_trainable_from k`` fine-tunes the encoder's blocks block_k..block_16 as well (0: the
+stem and every block), e.g. after a frozen run, resuming from its checkpoint.
 Checkpoints every epoch (the reference's ModelCheckpoint callback) and evaluates every epoch on
 ``--eval_steps`` held-out synthetic batches per rank (the reference's ``validation_data``):
 validation loss, pixel accuracy and mean IoU.
@@ -27,7 +29,35 @@ def define_flags():
                  help="held-out batches per rank evaluated after every epoch (0: no evaluation)")
   p.add_argument("--model_dir", default=None)
   p.add_argument("--export_dir", default=None)
+  p.add_argument("--encoder_trainable_from", type=int, default=None,
+                 help="fine-tune the encoder too: 0 trains the stem and every block, k in 1..16 "
+                      "blocks block_k..block_16 (default: frozen encoder)")
   return p
+
+
+def trainer_kwargs(args):
+  """Keyword arguments the trainer gets from the flags beyond the common ones: none unless the
+  encoder is fine-tuned."""
+  k = getattr(args, "encoder_trainable_from", None)
+  return {} if k is None else {"encoder_trainable_from": k}
+
+
+def resume(net, state, fine_tuning):
+  """Load a checkpoint's parameters and optimizer state.  A fine-tuning run resumed from a
+  checkpoint whose trainable encoder units differ from its own - a frozen run's (the first stage
+  of transfer learning) or one that fine-tuned other blocks - starts from that checkpoint's
+  encoder (``__encoder__``, then the ``encoder.*`` masters it has) and a fresh optimizer: the
+  saved optimizer state covers another set of parameters."""
+  params = state["params"]
+  net.load_state_dict(params)
+  if fine_tuning:
+    theirs = {k for k in params if k.startswith("encoder.")}
+    mine = {s["name"] for s in net.store.order if s["name"].startswith("encoder.")}
+    if theirs != mine:
+      print("checkpoint fine-tunes {} encoder parameters, this run {}: starting from its encoder "
+            "with a fresh optimizer state".format(len(theirs), len(mine)))
+      return
+  net.optim.load_state_dict(state["optim"])
 
 
 def labels_of(x):
@@ -41,8 +71,9 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
   from tensorflowonspark_b200.models import unet
   from tensorflowonspark_b200.utils import checkpoint
   B = args.batch_size
+  extra = trainer_kwargs(args)
   net = unet.UNetTrainer(batch=B, image=IMG, classes=3, device=device, lr=args.learning_rate,
-                         comm=comm)
+                         comm=comm, **extra)
   if comm is not None:
     comm.broadcast("weights", root=0)
     comm.broadcast("aux32", root=0)
@@ -50,8 +81,7 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
   if args.model_dir:
     start, state = checkpoint.load(args.model_dir)
     if state is not None:
-      net.load_state_dict(state["params"])
-      net.optim.load_state_dict(state["optim"])
+      resume(net, state, bool(extra))
       print("resumed from step", start)
   batches = [net.synthetic_batch(seed=1000 * rank + i)[0] for i in range(4)]
   # this rank's shard of the held-out set: batch i of rank r is held-out batch i * world + r

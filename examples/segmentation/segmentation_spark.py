@@ -48,8 +48,9 @@ def main_fun(args, ctx):
   torch.cuda.set_device(0)
   comm = ctx.gradient_comm() if ctx.world_size > 1 else None   # one host: P2P/NVLS kernels; several: NCCL
   B = args.batch_size
+  k = getattr(args, "encoder_trainable_from", None)   # None: frozen encoder, as the reference
   net = unet.UNetTrainer(batch=B, image=IMG, classes=3, device="cuda:0", lr=args.learning_rate,
-                         comm=comm)
+                         comm=comm, **({} if k is None else {"encoder_trainable_from": k}))
   if comm is not None:
     comm.broadcast("weights", root=0)
     comm.broadcast("aux32", root=0)
@@ -172,6 +173,9 @@ if __name__ == "__main__":
                       help="checkpoint written by the chief after the last step (servable)")
   parser.add_argument("--export_dir", default=None,
                       help="inference artefact exported by the chief after the last step")
+  parser.add_argument("--encoder_trainable_from", type=int, default=None,
+                      help="fine-tune the encoder too: 0 trains the stem and every block, k in "
+                           "1..16 blocks block_k..block_16 (default: frozen encoder)")
   args = parser.parse_args()
   conf = SparkConf().setAppName("segmentation_spark") \
       .set("spark.executor.instances", str(args.cluster_size)) \

@@ -6,15 +6,24 @@ native engine: frozen MobileNetV2 encoder (128x128x3 input, five skip taps) + fo
 Kernel mapping:
   encoder   1x1 expand / project convs -> wgmma GEMM with folded inference-BN bias and fused
             ReLU6; 3x3 depthwise -> depthwise3x3 kernel (bias + ReLU6 fused); stem 3x3/s2 ->
-            implicit GEMM.  Forward only (``layer.trainable = False`` in the reference, :83).
+            implicit GEMM.  Frozen by default (``layer.trainable = False`` in the reference, :83).
+  fine-tune ``UNetTrainer(encoder_trainable_from=k)`` also trains the stem and blocks (k = 0) or
+            blocks block_k..block_16: batch norm stays folded (frozen statistics), the folded
+            filters and biases are the parameters.  1x1 wgrad / dgrad and the stem wgrad are
+            implicit GEMMs; every ReLU6 sits at a depthwise conv's input or output, so one fused
+            depthwise3x3_bwd launch applies both derivatives and produces dx, dw, the depthwise
+            bias gradient and the producer's bias gradient (deterministic, no float atomics).
   decoder   Conv2DTranspose forward = the stride-2 *data-gradient* implicit GEMM (four output
             parity classes), with batch-norm statistics fused into its epilogue; its backward
             = stride-2 fprop (input gradient) + stride-2 wgrad.  Channel concatenation is a
             strided 16-byte copy into the concat buffer.
-There is no pretrained checkpoint on this box (no network): the encoder is random-initialised,
-which leaves shapes, FLOPs and memory traffic - everything the benchmarks measure - unchanged.
+There are no pretrained ImageNet weights: the encoder is random-initialised from a fixed seed,
+which leaves shapes, FLOPs and memory traffic - everything the benchmarks measure - unchanged, and
+fine-tuning is how a user improves those features.
 """
+import functools
 import math
+import numbers
 
 import numpy as np
 import torch
@@ -29,65 +38,124 @@ MBV2 = [(1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1
         (6, 320, 1, 1)]
 #: blocks whose *expansion* output is a skip tap (Keras names block_{1,3,6,13}_expand_relu)
 SKIP_BLOCKS = (1, 3, 6, 13)
+#: inverted-residual blocks block_0 .. block_16
+NUM_BLOCKS = sum(n for _, _, n, _ in MBV2)
+
+
+def encoder_depthwise_shapes(image=128):
+  """(block, H, C, stride) of the 17 depthwise layers: input H x H x C, as the encoder builds them."""
+  out, H, cin = [], image // 2, 32
+  for t, c, n, s in MBV2:
+    for i in range(n):
+      stride = s if i == 0 else 1
+      out.append((len(out), H, cin * t, stride))
+      H, cin = (H - 1) // stride + 1, c
+  return out
 
 
 def _buf(shape, dev, dtype=torch.bfloat16):
   return torch.zeros(shape, dtype=dtype, device=dev)
 
 
-class _FrozenConv(object):
-  """1x1 or 3x3 convolution + folded inference batch-norm (+ReLU6), forward only."""
+class _EncoderUnit(object):
+  """Folded filter ``w`` and bias ``bias`` of one encoder convolution.  Frozen: standalone bf16 /
+  fp32 tensors.  Trainable (fine-tuning): register() makes the folded values parameters of the
+  trainer's ParamStore (the filter decayed, the bias not, so kernels read it in fp32 from aux32)
+  and bind() points ``w`` / ``bias`` at their store views once the store is finalized."""
 
-  def __init__(self, gen, cin, cout, k, stride, act, dev):
+  def _init_values(self, w, bias, dev, trainable):
+    self.trainable = trainable
+    if trainable:
+      self.init, self.w, self.bias = (w, bias), None, None   # fp32 values the masters start from
+    else:
+      self.w = w.to(dev, torch.bfloat16).contiguous()
+      self.bias = bias.to(dev, torch.float32).contiguous()
+
+  def register(self, store, name):
+    w, b = self.init
+    self.sw = store.register(name + ".w", w.shape, True, lambda shape, gen, v=w: v.clone())
+    self.sb = store.register(name + ".b", b.shape, False, lambda shape, gen, v=b: v.clone())
+
+  def bind(self, store):
+    self.w, self.bias, self.init = store.w(self.sw), store.f32(self.sb), None
+
+
+class _FrozenConv(_EncoderUnit):
+  """1x1 or 3x3 convolution + folded inference batch-norm (+ReLU6)."""
+
+  def __init__(self, gen, cin, cout, k, stride, act, dev, trainable=False):
     w = torch.randn(cout, k, k, cin, generator=gen) * math.sqrt(2.0 / (k * k * cin))
     gamma = 1.0 + 0.1 * torch.randn(cout, generator=gen)
     beta, mean = 0.1 * torch.randn(cout, generator=gen), 0.1 * torch.randn(cout, generator=gen)
     var = 1.0 + 0.1 * torch.rand(cout, generator=gen)
     scale = gamma / torch.sqrt(var + 1e-3)
-    self.w = (w * scale.view(-1, 1, 1, 1)).to(dev, torch.bfloat16).contiguous()
-    self.bias = (beta - mean * scale).to(dev, torch.float32).contiguous()
+    self._init_values(w * scale.view(-1, 1, 1, 1), beta - mean * scale, dev, trainable)
     self.k, self.stride, self.act = k, stride, act
 
-  def build(self, x, y):
+  def zero_input_channels(self, c0):
+    """Zero the filter taps of input channels >= c0 (the stem's padding channels)."""
+    (self.init[0] if self.trainable else self.w)[..., c0:] = 0
+
+  def connect(self, x, y):
     self.x, self.y = x, y
-    self.plan = igemm.conv_fprop(x, self.w, y, self.stride, self.k // 2, bias=self.bias,
+
+  def build(self):
+    self.plan = igemm.conv_fprop(self.x, self.w, self.y, self.stride, self.k // 2, bias=self.bias,
                                  relu=self.act)
 
   def forward(self):
     self.plan.run()
 
 
-class _FrozenDepthwise(object):
+class _FrozenDepthwise(_EncoderUnit):
 
-  def __init__(self, gen, c, stride, dev):
+  def __init__(self, gen, c, stride, dev, trainable=False):
     w = torch.randn(9, c, generator=gen) * math.sqrt(2.0 / 9)
     scale = 1.0 + 0.1 * torch.randn(c, generator=gen)
-    self.w = (w * scale.view(1, -1)).to(dev, torch.bfloat16).contiguous()
-    self.bias = (0.1 * torch.randn(c, generator=gen)).to(dev, torch.float32).contiguous()
+    self._init_values(w * scale.view(1, -1), 0.1 * torch.randn(c, generator=gen), dev, trainable)
     self.stride = stride
 
-  def build(self, x, y):
+  def connect(self, x, y):
     self.x, self.y = x, y
+
+  def build(self):
+    pass
 
   def forward(self):
     ops.K.depthwise3x3_fwd(self.x, self.w, self.bias, self.y, self.stride, 2)
 
 
-class MobileNetV2Encoder(object):
-  """Frozen feature extractor returning the five skip tensors."""
+class _Block(object):
+  """One inverted-residual block: Keras index, units (expand is None for block 0), its input and
+  output buffers, and whether the input is added to the output."""
 
-  def __init__(self, batch, image, dev, seed=7):
+  def __init__(self, index, expand, dw, project, inp, out, residual):
+    self.index, self.expand, self.dw, self.project = index, expand, dw, project
+    self.inp, self.out, self.residual = inp, out, residual
+
+
+class MobileNetV2Encoder(object):
+  """Feature extractor returning the five skip tensors.
+
+  ``trainable_from`` None: every unit frozen, forward only.  k in 0..16: the units of blocks
+  k..16 (and the stem for k = 0) register in ``store``; call bind() once the store is finalized
+  (it builds the forward plans on the store views), then build_backward()."""
+
+  def __init__(self, batch, image, dev, seed=7, trainable_from=None, store=None):
     gen = torch.Generator(device="cpu")
     gen.manual_seed(seed)
     B = batch
+    self.dev, self.trainable_from = dev, trainable_from
+    trains = lambda b: trainable_from is not None and b >= trainable_from  # noqa: E731
     self.x = _buf((B, image, image, 8), dev)  # 3 real + 5 zero channels (16-byte pixels)
-    self.layers = []
+    self.layers, self.blocks = [], []
     H = image // 2
     cur = _buf((B, H, H, 32), dev)
-    stem = _FrozenConv(gen, 8, 32, 3, 2, 2, dev)
-    stem.w[..., 3:] = 0
-    stem.build(self.x, cur)
+    stem = self.stem = _FrozenConv(gen, 8, 32, 3, 2, 2, dev, trainable=trains(0))
+    stem.zero_input_channels(3)
+    stem.connect(self.x, cur)
     self.layers.append(stem)
+    units = [("encoder.stem", stem)]
     self.skips = []
     cin, block = 32, 0
     for t, c, n, s in MBV2:
@@ -95,34 +163,99 @@ class MobileNetV2Encoder(object):
         stride = s if i == 0 else 1
         inp = cur
         hidden = cin * t
+        e = None
+        name = "encoder.block{}.".format(block)
         if t != 1:
-          e = _FrozenConv(gen, cin, hidden, 1, 1, 2, dev)
+          e = _FrozenConv(gen, cin, hidden, 1, 1, 2, dev, trainable=trains(block))
           ebuf = _buf((B, H, H, hidden), dev)
-          e.build(cur, ebuf)
+          e.connect(cur, ebuf)
           self.layers.append(e)
+          units.append((name + "expand", e))
           cur = ebuf
           if block in SKIP_BLOCKS:
             self.skips.append(cur)
         H2 = (H - 1) // stride + 1
-        d = _FrozenDepthwise(gen, hidden, stride, dev)
+        d = _FrozenDepthwise(gen, hidden, stride, dev, trainable=trains(block))
         dbuf = _buf((B, H2, H2, hidden), dev)
-        d.build(cur, dbuf)
+        d.connect(cur, dbuf)
         self.layers.append(d)
-        p = _FrozenConv(gen, hidden, c, 1, 1, 0, dev)
+        p = _FrozenConv(gen, hidden, c, 1, 1, 0, dev, trainable=trains(block))
         pbuf = _buf((B, H2, H2, c), dev)
-        p.build(dbuf, pbuf)
+        p.connect(dbuf, pbuf)
         self.layers.append(p)
+        units += [(name + "dw", d), (name + "project", p)]
         cur = pbuf
-        if stride == 1 and cin == c:
+        residual = stride == 1 and cin == c
+        if residual:
           self.layers.append(_Residual(pbuf, inp))
+        self.blocks.append(_Block(block, e, d, p, inp, pbuf, residual))
         cin, H, block = c, H2, block + 1
     self.skips.append(cur)  # block_16_project, 4x4x320 at 128 input
     self.out_hw = H
+    self.trainable_units = [u for _, u in units if u.trainable]
+    for name, u in units:
+      if u.trainable:
+        u.register(store, name)
+    self.backward_ops = []
+    if trainable_from is None:
+      self._build_forward()
+
+  def _build_forward(self):
+    for layer in self.layers:
+      if not isinstance(layer, _Residual):
+        layer.build()
+
+  def bind(self, store):
+    """Point the trainable units at the finalized store's views and build the forward plans."""
+    for u in self.trainable_units:
+      u.bind(store)
+    self._build_forward()
+
+  def build_backward(self, store, g_top, skip_grads):
+    """Plan the backward of the trainable blocks, top down.  ``g_top``: gradient of block_16's
+    project output (written by the decoder); ``skip_grads``: {block index: (tensor, channel
+    offset)} - the slice of an up-block's concatenation gradient that belongs to that block's
+    expand output.  Per block: project wgrad + bias colsum + dgrad, the fused depthwise backward
+    (both ReLU6 derivatives, the skip gradient, the producer's bias gradient), expand wgrad and,
+    above the lowest trainable block, expand dgrad into the block input's gradient - accumulated
+    when the block is residual, whose input and output share one gradient buffer."""
+    st, dev, K = store, self.dev, ops.K
+    lowest = self.trainable_from
+    run = self.backward_ops
+    g_out = g_top
+    for blk in reversed(self.blocks):
+      if blk.index < lowest:
+        break
+      e, d, p = blk.expand, blk.dw, blk.project
+      g_d = _buf(d.y.shape, dev)
+      run += [igemm.conv_wgrad(g_out, d.y, st.g(p.sw)).run,
+              functools.partial(K.colsum, g_out, st.g(p.sb)),
+              igemm.conv_dgrad(g_out, p.w, g_d).run]
+      g_x = _buf(d.x.shape, dev)   # gradient of the producer's pre-activation (expand or stem)
+      producer = e if e is not None else self.stem
+      add, add_off = skip_grads.get(blk.index, (None, 0))
+      N, H, _, C = d.x.shape
+      scratch = torch.zeros(ops.C().depthwise3x3_bwd_scratch(N, H, C, d.stride),
+                            dtype=torch.float32, device=dev)
+      run.append(functools.partial(K.depthwise3x3_bwd, d.x, d.w, d.y, g_d, add, add_off, g_x,
+                                   st.g(d.sw), st.g(d.sb), st.g(producer.sb), scratch, d.stride))
+      if e is None:   # block 0: its input is the stem's output
+        run.append(igemm.conv_wgrad(g_x, self.x, st.g(self.stem.sw), 2, 1).run)
+        continue
+      run.append(igemm.conv_wgrad(g_x, blk.inp, st.g(e.sw)).run)
+      if blk.index > lowest:
+        g_in = g_out if blk.residual else _buf(blk.inp.shape, dev)
+        run.append(igemm.conv_dgrad(g_x, e.w, g_in, accumulate=blk.residual).run)
+        g_out = g_in
 
   def forward(self):
     for layer in self.layers:
       layer.forward()
     return self.skips
+
+  def backward(self):
+    for op in self.backward_ops:
+      op()
 
 
 class _Residual(object):
@@ -183,24 +316,46 @@ class _Upsample(object):
       self.dgrad.run()
 
 
+def _trainable_from(k, training):
+  """Validated ``encoder_trainable_from``: None, or a block index in 0..16 (training only)."""
+  if k is None:
+    return None
+  if isinstance(k, bool) or not isinstance(k, numbers.Integral):
+    raise ValueError("encoder_trainable_from must be None or an int in 0..16, not {!r}".format(k))
+  if not 0 <= k < NUM_BLOCKS:
+    raise ValueError("encoder_trainable_from must be in 0..16, got {}".format(k))
+  if not training:
+    raise ValueError("encoder_trainable_from needs training=True (an inference-only U-Net has no "
+                     "gradients)")
+  return int(k)
+
+
 class UNetTrainer(object):
   """Static-buffer U-Net for ``batch`` images of ``image`` x ``image`` x 3 and ``classes`` labels.
   ``training=False`` builds only what the forward pass needs (predict, evaluate, serving): no
-  gradient buffers, no backward or statistics-fused plans and no optimizer (``optim`` is None)."""
+  gradient buffers, no backward or statistics-fused plans and no optimizer (``optim`` is None).
+
+  ``encoder_trainable_from``: None (default) trains the decoder only, on a frozen encoder.  An int
+  k fine-tunes the encoder too: 0 trains the stem and all 17 inverted-residual blocks, k in 1..16
+  the Keras blocks block_k .. block_16.  Their folded (batch norm in the filter) filters and biases
+  become parameters ``encoder.stem.{w,b}`` / ``encoder.block{b}.{expand,dw,project}.{w,b}`` of the
+  store, starting from exactly the frozen network of the same seed; the optimizer and gradient
+  all-reduce cover them like every other parameter."""
 
   UP = (512, 256, 128, 64)
 
   def __init__(self, batch=64, image=128, classes=3, device="cuda:0", lr=1e-3, comm=None, seed=1234,
-               training=True):
+               training=True, encoder_trainable_from=None):
+    k = self.encoder_trainable_from = _trainable_from(encoder_trainable_from, training)
     assert classes <= 8
     self.device = dev = torch.device(device)
     self.B, self.image, self.classes = batch, image, classes
     self.comm = comm
     self.training = tr = training
     B = batch
-    self.encoder = MobileNetV2Encoder(batch, image, dev)
-    skips = self.encoder.skips  # [64x64x96, 32x32x144, 16x16x192, 8x8x576, 4x4x320]
     st = self.store = ParamStore()
+    self.encoder = MobileNetV2Encoder(batch, image, dev, trainable_from=k, store=st)
+    skips = self.encoder.skips  # [64x64x96, 32x32x144, 16x16x192, 8x8x576, 4x4x320]
     self.ups = []
     cin = skips[-1].shape[-1]
     for i, f in enumerate(self.UP):
@@ -209,9 +364,12 @@ class UNetTrainer(object):
     self.s_last = st.register("last.w", (cin, 3, 3, 8), True, he_normal(9 * cin))
     self.s_last_b = st.register("last.b", (8,), False, constant(0.0))
     st.finalize(dev, alloc=comm.alloc if comm is not None else None, seed=seed, grads=tr)
+    if k is not None:
+      self.encoder.bind(st)
 
     x, h = skips[-1], skips[-1].shape[1]
-    g_x = None  # the encoder is frozen: no gradient flows into it
+    # a frozen encoder takes no gradient; a fine-tuned one gets block_16's output gradient here
+    g_x = self.g_top = _buf(x.shape, dev) if k is not None else None
     # the decoder batch norms' running statistics, one flat buffer (checkpoints, evaluation)
     self.running = RunningArena(dev, capacity=2 * sum(self.UP))
     self.cats, self.g_cats = [], []
@@ -238,6 +396,10 @@ class UNetTrainer(object):
     if tr:
       self.p_last_wgrad = igemm.conv_wgrad(x, self.dlogits, st.g(self.s_last), 2, 1)
       self.p_last_dgrad = igemm.conv_fprop(self.dlogits, st.w(self.s_last), g_x, 2, 1)
+    if k is not None:
+      # up-block i concatenates skips[-2 - i], the expand output of SKIP_BLOCKS[-1 - i]
+      skip_grads = {SKIP_BLOCKS[-1 - i]: (g_cat, f) for i, (g_cat, _, f) in enumerate(self.g_cats)}
+      self.encoder.build_backward(st, self.g_top, skip_grads)
     self.loss_sum = torch.zeros(1, dtype=torch.float32, device=dev)
     self.correct = torch.zeros(1, dtype=torch.float32, device=dev)
     self.in_u8 = _buf((B, image, image, 3), dev, torch.uint8)
@@ -295,6 +457,7 @@ class UNetTrainer(object):
     for up, (g_cat, g_act, f) in zip(reversed(self.ups), reversed(self.g_cats)):
       K.copy_channels(g_cat, g_act, f, 0, 0)  # gradient of the decoder half of the concat
       up.backward()
+    self.encoder.backward()   # fine-tuning only: nothing to run on a frozen encoder
     self.optim.step()
 
   def capture(self):
@@ -335,9 +498,11 @@ class UNetTrainer(object):
   # ------------------------------------------------------------------ state
   def state_dict(self):
     """Parameters (fp32 masters, assembled across ranks when sharded) + the decoder batch norms'
-    running statistics (``__running__``) + the frozen encoder (``__encoder__``: one (bf16 filter,
-    fp32 bias) pair per convolution of ``encoder.layers``, in that order, as the forward uses
-    them): everything inference or a resumed run needs, independent of the loading host's RNG."""
+    running statistics (``__running__``) + the encoder (``__encoder__``: one (bf16 filter, fp32
+    bias) pair per convolution of ``encoder.layers``, in that order, as the forward uses them,
+    with their current values when the encoder is fine-tuned): everything inference or a resumed
+    run needs, independent of the loading host's RNG.  A fine-tuning trainer's parameters include
+    the fp32 masters ``encoder.*`` of its trainable units."""
     sd = dict(self.store.state_dict())
     sd["__running__"] = self.running.tensor().detach().cpu().clone()
     sd["__encoder__"] = [(c.w.detach().cpu().clone(), c.bias.detach().cpu().clone())
@@ -347,7 +512,9 @@ class UNetTrainer(object):
   def load_state_dict(self, sd):
     """Inverse of state_dict(); a dict without ``__running__`` keeps the current running
     statistics, one without ``__encoder__`` (checkpoints written before the encoder was part of
-    the state) keeps the seeded encoder."""
+    the state) keeps the seeded encoder.  ``__encoder__`` is applied first, then any ``encoder.*``
+    fp32 masters: a frozen run's checkpoint starts fine-tuning from its encoder, a fine-tuning
+    checkpoint resumes with exact masters, and a frozen trainer ignores ``encoder.*``."""
     sd = dict(sd)
     running = sd.pop("__running__", None)
     encoder = sd.pop("__encoder__", None)
@@ -357,9 +524,14 @@ class UNetTrainer(object):
           w.shape != c.w.shape or b.shape != c.bias.shape for c, (w, b) in zip(convs, encoder)):
         raise ValueError("__encoder__ does not match this U-Net's encoder ({} convolutions)".format(
             len(convs)))
+      st = self.store
       for c, (w, b) in zip(convs, encoder):
-        c.w.copy_(w.to(self.device, torch.bfloat16))
-        c.bias.copy_(b.to(self.device, torch.float32))
+        if c.trainable:   # into the masters: store.load_state_dict rounds them to the bf16 copy
+          st.m(c.sw).copy_(w.to(self.device, torch.bfloat16).float())
+          st.m(c.sb).copy_(b.to(self.device, torch.float32))
+        else:
+          c.w.copy_(w.to(self.device, torch.bfloat16))
+          c.bias.copy_(b.to(self.device, torch.float32))
     self.store.load_state_dict(sd)
     if running is not None:
       self.running.tensor().copy_(running.to(self.device))
