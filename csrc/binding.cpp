@@ -486,8 +486,23 @@ void eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& n_va
                            logits.size(1), V, cur_stream()),
         "eval_metrics");
 }
-int64_t seg_eval_scratch(int64_t pixels) {
-  return static_cast<int64_t>(tfos::seg_eval_grid(pixels)) * tfos::kSegEvalSlots;
+// The logits' padded channel count picks the kernel: 8 -> the one-load-per-pixel kernels
+// (V <= 8), 16..256 -> the wide kernels (seg_wide.cuh) with VP = ceil(V / 8) * 8.
+int64_t seg_padded_classes(int64_t V) {
+  return V <= 8 ? 8 : (V + 7) / 8 * 8;
+}
+bool seg_channels_match(const Tensor& logits, int64_t V) {
+  return logits.dim() >= 2 && V >= 1 && V <= 256 && logits.size(-1) == seg_padded_classes(V);
+}
+int64_t seg_eval_scratch(int64_t pixels, int64_t V) {
+  TORCH_CHECK(V >= 1 && V <= 256, "seg_eval_scratch: V in [1, 256]");
+  if (V <= 8) return static_cast<int64_t>(tfos::seg_eval_grid(pixels)) * tfos::kSegEvalSlots;
+  return tfos::seg_eval_wide_scratch(pixels, static_cast<int>(V));
+}
+// accumulator slots seg_eval_metrics adds to (models/unet.py: seg_eval_layout)
+int64_t seg_eval_slots(int64_t V) {
+  TORCH_CHECK(V >= 1 && V <= 256, "seg_eval_slots: V in [1, 256]");
+  return V <= 8 ? tfos::kSegEvalSlots : tfos::seg_eval_wide_slots(static_cast<int>(V));
 }
 void seg_eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& n_valid,
                       Tensor acc, Tensor partial, Tensor counter, int V) {
@@ -497,14 +512,28 @@ void seg_eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& 
   need(acc, torch::kFloat64, "acc");
   need(partial, torch::kFloat64, "partial");
   need(counter, torch::kInt32, "counter");
-  TORCH_CHECK(logits.dim() >= 2 && logits.size(0) > 0 && logits.size(-1) == 8 && V >= 1 && V <= 8,
-              "seg_eval_metrics: logits [B, ..., 8] and V in [1, 8]");
-  const int64_t images = logits.size(0), pixels = logits.numel() / 8;
+  TORCH_CHECK(seg_channels_match(logits, V), "seg_eval_metrics: logits [B, ..., VP] with V in [1, 256] and "
+              "VP = 8 for V <= 8, ceil(V / 8) * 8 above");
+  TORCH_CHECK(logits.size(0) > 0, "seg_eval_metrics: no images");
+  const int64_t VP = logits.size(-1);
+  const int64_t images = logits.size(0), pixels = logits.numel() / VP;
   TORCH_CHECK(labels.numel() == pixels, "seg_eval_metrics: one label per pixel");
-  TORCH_CHECK(acc.numel() >= tfos::kSegEvalSlots, "seg_eval_metrics: acc needs 68 slots");
-  TORCH_CHECK(partial.numel() >= seg_eval_scratch(pixels),
-              "seg_eval_metrics: partial needs seg_eval_scratch(pixels) doubles");
+  TORCH_CHECK(acc.numel() >= seg_eval_slots(V), "seg_eval_metrics: acc needs seg_eval_slots(V) = ",
+              seg_eval_slots(V), " slots");
+  TORCH_CHECK(partial.numel() >= seg_eval_scratch(pixels, V),
+              "seg_eval_metrics: partial needs seg_eval_scratch(pixels, V) doubles");
   TORCH_CHECK(counter.numel() >= 1, "seg_eval_metrics: counter");
+  if (VP > 8) {
+    for (const Tensor& t : {labels, n_valid, acc, partial, counter})
+      TORCH_CHECK(t.device() == logits.device(), "seg_eval_metrics: tensors on different devices");
+    check(tfos::seg_eval_metrics_wide(
+              logits.data_ptr(), labels.data_ptr<int>(), n_valid.data_ptr<int>(),
+              acc.data_ptr<double>(), partial.data_ptr<double>(),
+              reinterpret_cast<unsigned int*>(counter.data_ptr<int>()), static_cast<int>(images),
+              pixels / images, static_cast<int>(VP), V, cur_stream()),
+          "seg_eval_metrics");
+    return;
+  }
   check(tfos::seg_eval_metrics(logits.data_ptr(), labels.data_ptr<int>(), n_valid.data_ptr<int>(),
                                acc.data_ptr<double>(), partial.data_ptr<double>(),
                                reinterpret_cast<unsigned int*>(counter.data_ptr<int>()),
@@ -514,9 +543,10 @@ void seg_eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& 
 void seg_predict(const Tensor& logits, Tensor mask, c10::optional<Tensor> out, int V) {
   need(logits, torch::kBFloat16, "logits");
   need(mask, torch::kUInt8, "mask");
-  TORCH_CHECK(logits.dim() >= 2 && logits.size(-1) == 8 && V >= 1 && V <= 8,
-              "seg_predict: logits [B, ..., 8] and V in [1, 8]");
-  const int64_t pixels = logits.numel() / 8;
+  TORCH_CHECK(seg_channels_match(logits, V), "seg_predict: logits [B, ..., VP] with V in [1, 256] and "
+              "VP = 8 for V <= 8, ceil(V / 8) * 8 above");
+  const int64_t VP = logits.size(-1);
+  const int64_t pixels = logits.numel() / VP;
   TORCH_CHECK(mask.numel() == pixels, "seg_predict: one mask byte per pixel");
   TORCH_CHECK(reinterpret_cast<uintptr_t>(mask.data_ptr()) % 16 == 0,
               "seg_predict: mask must be 16-byte aligned");
@@ -527,6 +557,12 @@ void seg_predict(const Tensor& logits, Tensor mask, c10::optional<Tensor> out, i
     TORCH_CHECK(reinterpret_cast<uintptr_t>(out->data_ptr()) % 16 == 0,
                 "seg_predict: out must be 16-byte aligned");
     o = out->data_ptr<float>();
+  }
+  if (VP > 8) {
+    check(tfos::seg_predict_wide(logits.data_ptr(), mask.data_ptr<uint8_t>(), o, pixels,
+                                 static_cast<int>(VP), V, cur_stream()),
+          "seg_predict");
+    return;
   }
   check(tfos::seg_predict(logits.data_ptr(), mask.data_ptr<uint8_t>(), o, pixels, V, cur_stream()),
         "seg_predict");
@@ -635,6 +671,22 @@ void pixel_xent(const Tensor& logits, const Tensor& labels, c10::optional<Tensor
                 Tensor loss_sum, c10::optional<Tensor> correct, int V, double scale) {
   need(logits, torch::kBFloat16, "logits");
   need(labels, torch::kInt32, "labels");
+  if (logits.size(-1) > 8) {
+    TORCH_CHECK(seg_channels_match(logits, V), "pixel_xent: logits [B, ..., VP] with V in [1, 256] and "
+                "VP = 8 for V <= 8, ceil(V / 8) * 8 above");
+    const int64_t VP = logits.size(-1);
+    const int64_t P = logits.numel() / VP;
+    TORCH_CHECK(labels.numel() == P, "pixel_xent: one label per pixel");
+    const void* d = optptr(dlogits);
+    if (d != nullptr)
+      TORCH_CHECK(dlogits->sizes() == logits.sizes() && dlogits->scalar_type() == torch::kBFloat16,
+                  "pixel_xent: dlogits must be bf16 with the shape of logits");
+    check(tfos::pixel_xent_wide(logits.data_ptr(), labels.data_ptr<int>(), const_cast<void*>(d),
+                                loss_sum.data_ptr<float>(), optf(correct), P,
+                                static_cast<int>(VP), V, scale, cur_stream()),
+          "pixel_xent");
+    return;
+  }
   TORCH_CHECK(logits.size(-1) == 8 && V <= 8, "pixel_xent expects 8 padded channels");
   check(tfos::pixel_xent(logits.data_ptr(), labels.data_ptr<int>(),
                          const_cast<void*>(optptr(dlogits)), loss_sum.data_ptr<float>(),
@@ -893,7 +945,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("cast_f32_bf16", &cast_f32_bf16);
   m.def("bn_fold", &bn_fold);
   m.def("eval_metrics", &eval_metrics);
-  m.def("seg_eval_scratch", &seg_eval_scratch);
+  m.def("seg_eval_scratch", &seg_eval_scratch, py::arg("pixels"), py::arg("classes") = 8);
+  m.def("seg_eval_slots", &seg_eval_slots);
   m.def("seg_eval_metrics", &seg_eval_metrics);
   m.def("seg_predict", &seg_predict);
   m.def("conv3x3_c1_fwd", &conv3x3_c1_fwd);

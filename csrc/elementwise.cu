@@ -10,6 +10,7 @@
 
 #include "ops.h"
 #include "ptx.cuh"
+#include "seg_wide.cuh"
 
 namespace tfos {
 
@@ -657,6 +658,65 @@ pixel_xent_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restric
   }
 }
 
+// pixel_xent for VP = 16..256 padded channels (V = 9..256 classes): G lanes per pixel
+// (seg_wide.cuh), each lane one 16-byte chunk of the logits in registers, so every pixel's logits
+// are read once and its dlogits written once.  Warp tile t covers pixels [t * 32 / G, ...); the
+// loop bound is uniform over the warp, so the full-mask group shuffles are safe.  Channels
+// j >= V get exactly zero gradient and never enter the loss or the arg-max.  A label outside
+// [0, V) (not validated, as for the 8-channel kernel) contributes the loss mx + log(se), a
+// gradient without the one-hot term and no hit.
+template <int G>
+__global__ void __launch_bounds__(256)
+pixel_xent_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                       __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
+                       long long P, int VP, int V, float scale) {
+  constexpr int kPix = 32 / G;   // pixels per warp tile
+  const int lane = threadIdx.x & 31, sub = lane & (G - 1), c0 = sub * 8;
+  const long long nw = static_cast<long long>(gridDim.x) * (256 / 32);
+  float local = 0.f, hits = 0.f;
+  for (long long t = static_cast<long long>(blockIdx.x) * (256 / 32) + (threadIdx.x >> 5);
+       t * kPix < P; t += nw) {
+    const long long p = t * kPix + lane / G;
+    const bool in = p < P, live = in && c0 < VP;
+    float l[8];
+    if (live) {
+      load8(logits + p * VP + c0, l);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) l[k] = 0.f;
+    }
+    float mx;
+    const int am = seg_argmax_wide<G>(l, c0, V, mx);
+    const int y = in ? labels[p] : -1;
+    float e[8], se = 0.f, ly = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      e[k] = c0 + k < V ? __expf(l[k] - mx) : 0.f;
+      se += e[k];
+      if (c0 + k < V && c0 + k == y) ly = l[k];
+    }
+    se = seg_group_sum<G>(se);
+    ly = seg_group_sum<G>(ly);
+    const float inv = 1.f / se;
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      e[k] = c0 + k < V ? (e[k] * inv - (c0 + k == y ? 1.f : 0.f)) * scale : 0.f;
+    if (dlogits != nullptr && live) store8(dlogits + p * VP + c0, e);
+    if (in && sub == 0) {
+      local += -(ly - mx - __logf(se)) * scale;
+      hits += (am == y) ? 1.f : 0.f;
+    }
+  }
+  for (int o = 16; o >= 1; o >>= 1) {
+    local += __shfl_xor_sync(0xffffffff, local, o);
+    hits += __shfl_xor_sync(0xffffffff, hits, o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(loss_sum, local);
+    if (correct_sum != nullptr) atomicAdd(correct_sum, hits);
+  }
+}
+
 inline int grid_for(long long work, int threads, int max_blocks) {
   long long b = (work + threads - 1) / threads;
   if (b < 1) b = 1;
@@ -809,6 +869,29 @@ cudaError_t pixel_xent(const void* logits, const int* labels, void* dlogits, flo
   pixel_xent_kernel<<<grid_for(P, 256, kMaxBlocks), 256, 0, s>>>(
       static_cast<const __nv_bfloat16*>(logits), labels, static_cast<__nv_bfloat16*>(dlogits),
       loss_sum, correct_sum, P, V, scale);
+  TFOS_RET();
+}
+cudaError_t pixel_xent_wide(const void* logits, const int* labels, void* dlogits, float* loss_sum,
+                            float* correct_sum, long long P, int VP, int V, float scale,
+                            cudaStream_t s) {
+  const int G = seg_wide_group(VP);
+  const int grid = grid_for(P * G, 256, kMaxBlocks);
+  const auto* l = static_cast<const __nv_bfloat16*>(logits);
+  auto* d = static_cast<__nv_bfloat16*>(dlogits);
+#define TFOS_XENT_WIDE(g)                                                                     \
+  case g:                                                                                     \
+    pixel_xent_wide_kernel<g><<<grid, 256, 0, s>>>(l, labels, d, loss_sum, correct_sum, P, VP, \
+                                                   V, scale);                                 \
+    break;
+  switch (G) {
+    TFOS_XENT_WIDE(2)
+    TFOS_XENT_WIDE(4)
+    TFOS_XENT_WIDE(8)
+    TFOS_XENT_WIDE(16)
+    TFOS_XENT_WIDE(32)
+    default: return cudaErrorInvalidValue;
+  }
+#undef TFOS_XENT_WIDE
   TFOS_RET();
 }
 cudaError_t cast_f32_bf16(const float* in, void* out, long long n, cudaStream_t s) {

@@ -17,6 +17,7 @@
 
 #include "ops.h"
 #include "ptx.cuh"
+#include "seg_wide.cuh"
 
 namespace tfos {
 namespace {
@@ -322,7 +323,239 @@ seg_predict_kernel(const __nv_bfloat16* __restrict__ logits, uint8_t* __restrict
   }
 }
 
+// Wide logits (seg_wide.cuh): G lanes per pixel, kSegWarps * 32 / G pixels per CTA pass.
+constexpr int kSegWideChunk = kSegThreads;   // CTA ranges are multiples of every pass size
+constexpr int kSegWideScalars = 4;           // count, correct, invalid, loss: per-CTA partials
+// the CTA keeps its own uint32 [V, V] confusion table in shared memory up to this size
+constexpr int kSegWideSmemTable = 100 * 1024;
+
+// seg_eval_metrics_kernel for bf16 logits [P, VP], V > 8.  CTA b scores pixels
+// [b * chunk, (b + 1) * chunk) of the valid range, warp w the pixels of passes w, w + kSegWarps,
+// ...  Confusion counts: bins y * V + pred, warp-aggregated with __match_any_sync, then added to
+// the CTA's shared uint32 table (smem_table) and flushed to the global uint64 table with one
+// integer atomic per non-zero cell, or added to the global table directly when V x V does not fit.
+// Scalars: count / correct / invalid as integers, the loss as fp64, per thread, then warp-shuffle
+// and warp-order sums into the CTA's partials; the last CTA to finish sums the partials in a fixed
+// order, adds the table into acc and zeroes it.  Bitwise reproducible.
+template <int G>
+__global__ void __launch_bounds__(kSegThreads)
+seg_eval_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                     const int* __restrict__ n_valid, double* __restrict__ acc,
+                     double* __restrict__ partial, unsigned long long* __restrict__ table,
+                     unsigned int* __restrict__ counter, int images, long long ppi,
+                     long long chunk, int VP, int V, int smem_table) {
+  extern __shared__ unsigned int tab[];
+  __shared__ int wint[3][kSegWarps];
+  __shared__ double wloss[kSegWarps];
+  __shared__ unsigned int is_last;
+  constexpr int kPix = 32 / G;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, sub = lane & (G - 1), c0 = sub * 8;
+  const int cells = V * V;
+  if (smem_table)
+    for (int i = threadIdx.x; i < cells; i += kSegThreads) tab[i] = 0u;
+  __syncthreads();
+  int n = *n_valid;
+  n = n < 0 ? 0 : (n > images ? images : n);
+  const long long limit = static_cast<long long>(n) * ppi;
+  const long long lo = static_cast<long long>(blockIdx.x) * chunk;
+  const long long hi = lo + chunk < limit ? lo + chunk : limit;
+  int cnt = 0, hit = 0, bad = 0;
+  double loss = 0.0;
+  for (long long base = lo + warp * kPix; base < hi; base += kSegWarps * kPix) {
+    const long long p = base + lane / G;
+    const bool in = p < hi;
+    float l[8];
+    if (in && c0 < VP) {
+      seg_unpack8(__ldcs(reinterpret_cast<const uint4*>(logits + p * VP + c0)), l);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) l[k] = 0.f;
+    }
+    const int y = in ? __ldcs(labels + p) : -1;
+    float mx;
+    const int am = seg_argmax_wide<G>(l, c0, V, mx);
+    float se = 0.f, ly = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      if (c0 + k < V) se += __expf(l[k] - mx);
+      if (c0 + k < V && c0 + k == y) ly = l[k];
+    }
+    se = seg_group_sum<G>(se);
+    ly = seg_group_sum<G>(ly);
+    int bin = -1;
+    if (in && sub == 0) {
+      if (y < 0 || y >= V) {
+        bad += 1;
+      } else {
+        cnt += 1;
+        hit += am == y ? 1 : 0;
+        loss += static_cast<double>(__logf(se) + mx - ly);
+        bin = y * V + am;
+      }
+    }
+    const unsigned same = __match_any_sync(0xffffffffu, bin);
+    if (bin >= 0 && lane == __ffs(same) - 1) {
+      if (smem_table) atomicAdd(&tab[bin], static_cast<unsigned>(__popc(same)));
+      else atomicAdd(&table[bin], static_cast<unsigned long long>(__popc(same)));
+    }
+  }
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) {
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    hit += __shfl_xor_sync(0xffffffffu, hit, o);
+    bad += __shfl_xor_sync(0xffffffffu, bad, o);
+    loss += __shfl_xor_sync(0xffffffffu, loss, o);
+  }
+  if (lane == 0) {
+    wint[0][warp] = cnt, wint[1][warp] = hit, wint[2][warp] = bad;
+    wloss[warp] = loss;
+  }
+  __syncthreads();
+  const int grid = gridDim.x;
+  if (threadIdx.x == 0) {
+    long long c = 0, h = 0, b = 0;
+    double l = 0.0;
+    for (int w = 0; w < kSegWarps; ++w)
+      c += wint[0][w], h += wint[1][w], b += wint[2][w], l += wloss[w];
+    partial[static_cast<long long>(kSegEvalCount) * grid + blockIdx.x] = static_cast<double>(c);
+    partial[static_cast<long long>(kSegEvalCorrect) * grid + blockIdx.x] = static_cast<double>(h);
+    partial[static_cast<long long>(kSegEvalInvalid) * grid + blockIdx.x] = static_cast<double>(b);
+    partial[static_cast<long long>(kSegEvalLoss) * grid + blockIdx.x] = l;
+  }
+  if (smem_table) {
+    for (int i = threadIdx.x; i < cells; i += kSegThreads) {
+      const unsigned c = tab[i];
+      if (c) atomicAdd(&table[i], static_cast<unsigned long long>(c));
+    }
+  }
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) is_last = (atomicAdd(counter, 1u) == gridDim.x - 1) ? 1u : 0u;
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  if (warp < kSegWideScalars) {   // the four scalar slots, one warp each
+    const double* row = partial + static_cast<long long>(warp) * grid;
+    double t = 0.0;
+#pragma unroll
+    for (int k = 0; k < (kSegMaxGrid + 31) / 32; ++k) {
+      const int b = lane + 32 * k;
+      if (b < grid) t += __ldcg(row + b);
+    }
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if (lane == 0) acc[warp] += t;
+  }
+  for (int i = threadIdx.x; i < cells; i += kSegThreads) {
+    const unsigned long long c = __ldcg(table + i);
+    if (c) {
+      acc[kSegWideConfusion + i] += static_cast<double>(c);
+      table[i] = 0ull;
+    }
+  }
+  if (threadIdx.x == 0) *counter = 0;  // ready for the next launch or graph replay
+}
+
+// seg_predict_kernel for bf16 logits [P, VP], V > 8: warp tiles of 32 / G pixels over a
+// grid-stride loop; the group's first lane writes the mask byte, every lane its channels < V of
+// the compact fp32 logits.
+template <int G>
+__global__ void __launch_bounds__(256)
+seg_predict_wide_kernel(const __nv_bfloat16* __restrict__ logits, uint8_t* __restrict__ mask,
+                        float* __restrict__ out, long long P, int VP, int V) {
+  constexpr int kPix = 32 / G;
+  const int lane = threadIdx.x & 31, sub = lane & (G - 1), c0 = sub * 8;
+  const long long nw = static_cast<long long>(gridDim.x) * (256 / 32);
+  for (long long t = static_cast<long long>(blockIdx.x) * (256 / 32) + (threadIdx.x >> 5);
+       t * kPix < P; t += nw) {
+    const long long p = t * kPix + lane / G;
+    const bool in = p < P;
+    float l[8];
+    if (in && c0 < VP) {
+      seg_unpack8(__ldcs(reinterpret_cast<const uint4*>(logits + p * VP + c0)), l);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) l[k] = 0.f;
+    }
+    float mx;
+    const int am = seg_argmax_wide<G>(l, c0, V, mx);
+    if (!in) continue;
+    if (sub == 0) mask[p] = static_cast<uint8_t>(am);
+    if (out != nullptr) {
+      float* dst = out + p * V + c0;
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        if (c0 + k < V) __stcs(dst + k, l[k]);
+    }
+  }
+}
+
 }  // namespace
+
+long long seg_eval_wide_scratch(long long pixels, int V) {
+  return static_cast<long long>(seg_eval_grid(pixels)) * kSegWideScalars +
+         static_cast<long long>(V) * V;
+}
+
+cudaError_t seg_eval_metrics_wide(const void* logits, const int* labels, const int* n_valid,
+                                  double* acc, double* scratch, unsigned int* counter, int images,
+                                  long long ppi, int VP, int V, cudaStream_t s) {
+  const long long pixels = static_cast<long long>(images) * ppi;
+  const int grid = seg_eval_grid(pixels);
+  const long long chunk =
+      ((pixels + grid - 1) / grid + kSegWideChunk - 1) / kSegWideChunk * kSegWideChunk;
+  // the table first: its place does not depend on the grid, so one scratch serves any pixel count
+  auto* table = reinterpret_cast<unsigned long long*>(scratch);
+  double* partial = scratch + static_cast<long long>(V) * V;
+  const size_t tbytes = static_cast<size_t>(V) * V * sizeof(unsigned int);
+  const int smem_table = tbytes <= static_cast<size_t>(kSegWideSmemTable) ? 1 : 0;
+  const size_t smem = smem_table ? tbytes : 0;
+  const auto* l = static_cast<const __nv_bfloat16*>(logits);
+#define TFOS_SEG_EVAL_WIDE(g)                                                                   \
+  case g: {                                                                                     \
+    static const cudaError_t attr = cudaFuncSetAttribute(                                       \
+        seg_eval_wide_kernel<g>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSegWideSmemTable); \
+    if (attr != cudaSuccess) return attr;                                                       \
+    seg_eval_wide_kernel<g><<<grid, kSegThreads, smem, s>>>(l, labels, n_valid, acc, partial,   \
+                                                            table, counter, images, ppi, chunk, \
+                                                            VP, V, smem_table);                 \
+    break;                                                                                      \
+  }
+  switch (seg_wide_group(VP)) {
+    TFOS_SEG_EVAL_WIDE(2)
+    TFOS_SEG_EVAL_WIDE(4)
+    TFOS_SEG_EVAL_WIDE(8)
+    TFOS_SEG_EVAL_WIDE(16)
+    TFOS_SEG_EVAL_WIDE(32)
+    default: return cudaErrorInvalidValue;
+  }
+#undef TFOS_SEG_EVAL_WIDE
+  return cudaGetLastError();
+}
+
+cudaError_t seg_predict_wide(const void* logits, uint8_t* mask, float* out, long long pixels,
+                             int VP, int V, cudaStream_t s) {
+  if (pixels <= 0) return cudaSuccess;
+  const int G = seg_wide_group(VP);
+  long long blocks = (pixels * G + 255) / 256;
+  if (blocks > kSmCount * 8) blocks = kSmCount * 8;
+  const auto* l = static_cast<const __nv_bfloat16*>(logits);
+#define TFOS_SEG_PREDICT_WIDE(g)                                                            \
+  case g:                                                                                   \
+    seg_predict_wide_kernel<g><<<static_cast<unsigned>(blocks), 256, 0, s>>>(l, mask, out, \
+                                                                            pixels, VP, V); \
+    break;
+  switch (G) {
+    TFOS_SEG_PREDICT_WIDE(2)
+    TFOS_SEG_PREDICT_WIDE(4)
+    TFOS_SEG_PREDICT_WIDE(8)
+    TFOS_SEG_PREDICT_WIDE(16)
+    TFOS_SEG_PREDICT_WIDE(32)
+    default: return cudaErrorInvalidValue;
+  }
+#undef TFOS_SEG_PREDICT_WIDE
+  return cudaGetLastError();
+}
 
 cudaError_t seg_predict(const void* logits, uint8_t* mask, float* out, long long pixels, int V,
                         cudaStream_t s) {

@@ -71,6 +71,11 @@ cudaError_t copy_channels(const void* src, void* dst, long long P, int C, int sr
                           int dst_ld, int dst_off, cudaStream_t s);
 cudaError_t pixel_xent(const void* logits, const int* labels, void* dlogits, float* loss_sum,
                        float* correct_sum, long long P, int V, float scale, cudaStream_t s);
+// pixel_xent for bf16 logits [P, VP], VP = ceil(V / 8) * 8 in 16..256 (seg_wide.cuh): the same
+// loss, gradient (exactly zero in channels >= V) and hits, one read and one write per pixel
+cudaError_t pixel_xent_wide(const void* logits, const int* labels, void* dlogits, float* loss_sum,
+                            float* correct_sum, long long P, int VP, int V, float scale,
+                            cudaStream_t s);
 
 // ---- optim_comm.cu
 constexpr int kMaxRanks = 8;
@@ -253,5 +258,25 @@ cudaError_t seg_eval_metrics(const void* logits, const int* labels, const int* n
 // must be 16-byte aligned.
 cudaError_t seg_predict(const void* logits, uint8_t* mask, float* out, long long pixels, int V,
                         cudaStream_t s);
+// Wide logits, bf16 [pixels, VP] with VP = ceil(V / 8) * 8 in 16..256 (9 <= V <= 256).
+// seg_eval_metrics_wide: acc[kSegWide*] += the same totals; accumulator layout
+// [count, correct, invalid, loss, images, confusion V x V] (the kernel leaves images alone).
+// scratch: seg_eval_wide_scratch(pixels, V) doubles, zero before the first launch: a uint64
+// [V, V] confusion table that the CTAs add their integer counts to and the last CTA adds into acc
+// and zeroes again, then per-CTA partials of the four scalars (summed in a fixed order by the
+// last CTA).  counter as for seg_eval_metrics.  Deterministic: integer counts are exact and
+// order-independent, the scalars are summed in a fixed order.
+constexpr int kSegWideImages = 4, kSegWideConfusion = 5;
+inline long long seg_eval_wide_slots(int V) {
+  return kSegWideConfusion + static_cast<long long>(V) * V;
+}
+long long seg_eval_wide_scratch(long long pixels, int V);
+cudaError_t seg_eval_metrics_wide(const void* logits, const int* labels, const int* n_valid,
+                                  double* acc, double* scratch, unsigned int* counter, int images,
+                                  long long ppi, int VP, int V, cudaStream_t s);
+// seg_predict_wide: mask[p] = the class (seg_wide.cuh) and, when out is not null,
+// out[p * V + j] = the fp32 value of channel j < V.  One pass; any pixel count.
+cudaError_t seg_predict_wide(const void* logits, uint8_t* mask, float* out, long long pixels,
+                             int VP, int V, cudaStream_t s);
 
 }  // namespace tfos

@@ -1,0 +1,71 @@
+// Per-pixel logits wider than one 16-byte load (the segmentation U-Net with 9..256 classes):
+// bf16 logits [P, VP], VP = ceil(V / 8) * 8 in 16..256.  A pixel belongs to a group of G lanes
+// (G the power of two >= VP / 8, aligned inside the warp); lane i of the group holds channels
+// [8 i, 8 i + 8) in registers, lanes with 8 i >= VP hold nothing.  Reductions over the pixel are
+// xor-shuffles with offsets < G, which stay inside the group.  Shared by pixel_xent
+// (elementwise.cu), seg_eval_metrics and seg_predict (eval.cu), so training, evaluation and
+// serving predict the same class for every pixel.
+#pragma once
+
+#include <cuda_bf16.h>
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "ptx.cuh"
+
+namespace tfos {
+
+constexpr int kSegWideNone = 0x7fffffff;  // "no channel yet" in the arg-max scan
+
+// G for VP padded channels: the power of two >= VP / 8 (2 .. 32)
+inline int seg_wide_group(int VP) {
+  int g = 2;
+  while (g * 8 < VP) g *= 2;
+  return g;
+}
+
+__device__ __forceinline__ void seg_unpack8(const uint4 v, float (&l)[8]) {
+  const float2 a = unpack_bf16x2(v.x), b = unpack_bf16x2(v.y), c = unpack_bf16x2(v.z),
+               d = unpack_bf16x2(v.w);
+  l[0] = a.x, l[1] = a.y, l[2] = b.x, l[3] = b.y, l[4] = c.x, l[5] = c.y, l[6] = d.x, l[7] = d.y;
+}
+
+template <int G>
+__device__ __forceinline__ float seg_group_sum(float v) {
+#pragma unroll
+  for (int o = G / 2; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// The predicted class of the group's pixel, the rule of the 8-channel seg_argmax written as a
+// definition: 0 when l_0 is NaN, otherwise the lowest index of the maximum over the non-NaN
+// l_j, j < V.  Channels >= V are never read.  l: this lane's channels [c0, c0 + 8).  mx is
+// l at the result (NaN when l_0 is), the shift of the softmax.  Every lane of the group returns
+// the same values: the combine is a total order (value descending, then index ascending).
+template <int G>
+__device__ __forceinline__ int seg_argmax_wide(const float (&l)[8], const int c0, const int V,
+                                               float& mx) {
+  float m = 0.f;
+  int am = kSegWideNone;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const float v = l[k];
+    if (c0 + k < V && v == v && (am == kSegWideNone || v > m)) m = v, am = c0 + k;
+  }
+#pragma unroll
+  for (int o = G / 2; o >= 1; o >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, m, o);
+    const int a2 = __shfl_xor_sync(0xffffffffu, am, o);
+    if (a2 != kSegWideNone && (am == kSegWideNone || m2 > m || (m2 == m && a2 < am)))
+      m = m2, am = a2;
+  }
+  const float l0 = __shfl_sync(0xffffffffu, l[0], 0, G);   // the group's first lane holds l_0
+  if (l0 != l0) {
+    mx = l0;
+    return 0;
+  }
+  mx = m;
+  return am;
+}
+
+}  // namespace tfos

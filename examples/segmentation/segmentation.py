@@ -1,6 +1,8 @@
 """Image segmentation U-Net on ONE H100, no Spark (reference: examples/segmentation/
 segmentation.py - the notebook-derived single-node script; model at segmentation_spark.py:67-119):
 frozen MobileNetV2 encoder, four transposed-conv up-blocks, per-pixel softmax cross-entropy, Adam.
+``--classes V`` (1..256, default 3) sets the class count; the synthetic labels are the 3-class
+trimap, or the red channel in V bands (models/unet.synthetic_labels).
 ``--encoder_trainable_from k`` fine-tunes the encoder's blocks block_k..block_16 as well (0: the
 stem and every block), e.g. after a frozen run, resuming from its checkpoint.
 Checkpoints every epoch (the reference's ModelCheckpoint callback) and evaluates every epoch on
@@ -25,6 +27,8 @@ def define_flags():
   p.add_argument("--epochs", type=int, default=2)
   p.add_argument("--steps_per_epoch", type=int, default=57, help="3680 training images / 64")
   p.add_argument("--learning_rate", type=float, default=1e-3)
+  p.add_argument("--classes", type=int, default=3,
+                 help="segmentation classes, 1..256 (labels: the trimap at 3, else red-channel bands)")
   p.add_argument("--eval_steps", type=int, default=1,
                  help="held-out batches per rank evaluated after every epoch (0: no evaluation)")
   p.add_argument("--model_dir", default=None)
@@ -60,9 +64,11 @@ def resume(net, state, fine_tuning):
   net.optim.load_state_dict(state["optim"])
 
 
-def labels_of(x):
-  """Synthetic 3-class 'trimap' derived from the image itself (learnable, no dataset needed)."""
-  return (x[..., 0] > 127).int() + (x[..., 1] > 200).int()
+def labels_of(x, classes=3):
+  """Synthetic labels derived from the image itself (learnable, no dataset needed): the 3-class
+  'trimap' at 3 classes, red-channel bands otherwise (models/unet.synthetic_labels)."""
+  from tensorflowonspark_b200.models import unet
+  return unet.synthetic_labels(x, classes)
 
 
 def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
@@ -72,7 +78,8 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
   from tensorflowonspark_b200.utils import checkpoint
   B = args.batch_size
   extra = trainer_kwargs(args)
-  net = unet.UNetTrainer(batch=B, image=IMG, classes=3, device=device, lr=args.learning_rate,
+  V = getattr(args, "classes", 3)
+  net = unet.UNetTrainer(batch=B, image=IMG, classes=V, device=device, lr=args.learning_rate,
                          comm=comm, **extra)
   if comm is not None:
     comm.broadcast("weights", root=0)
@@ -96,12 +103,12 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
     t0 = time.time()
     for i in range(args.steps_per_epoch):
       x = batches[i % len(batches)]
-      net.set_input(x, labels_of(x))
+      net.set_input(x, labels_of(x, V))
       loss = net.train_step()
       step += 1
     torch.cuda.synchronize()
     rate = args.steps_per_epoch * B * world / (time.time() - t0)
-    res = net.evaluate([(x, labels_of(x)) for x in held_out]) if held_out else None  # collective
+    res = net.evaluate([(x, labels_of(x, V)) for x in held_out]) if held_out else None  # collective
     if is_chief:
       line = "epoch {} loss {:.4f}".format(epoch + 1, float(loss))
       if res is not None:

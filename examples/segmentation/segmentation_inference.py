@@ -19,14 +19,14 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspa
 IMG = 128
 
 
-def synth(n, seed):
-  """n synthetic (image, mask) pairs: the 3-class mask the training examples learn,
-  (red > 127) + (green > 200)."""
+def synth(n, seed, classes=3):
+  """n synthetic (image, mask) pairs: the mask the training examples learn at ``classes`` classes
+  (models/unet.synthetic_labels: the trimap (red > 127) + (green > 200) at 3)."""
   import numpy as np
+  from tensorflowonspark_b200.models import unet
   rng = np.random.RandomState(seed)
   imgs = rng.randint(0, 256, size=(n, IMG, IMG, 3), dtype=np.uint8)
-  masks = (imgs[..., 0] > 127).astype(np.uint8) + (imgs[..., 1] > 200).astype(np.uint8)
-  return imgs, masks
+  return imgs, unet.synthetic_labels(imgs, classes)
 
 
 def run(sc, args):
@@ -48,7 +48,8 @@ def run(sc, args):
   if args.output:
     preds.write.json(args.output)
   got = np.stack([np.frombuffer(r.mask, dtype=np.uint8) for r in preds.collect()])
-  want = np.concatenate([synth(per[i], i)[1] for i in range(parts)]).reshape(len(got), -1)
+  V = getattr(args, "classes", 3)
+  want = np.concatenate([synth(per[i], i, V)[1] for i in range(parts)]).reshape(len(got), -1)
   return float((got == want).mean())
 
 
@@ -60,6 +61,8 @@ if __name__ == "__main__":
   parser.add_argument("--num_images", type=int, default=1024)
   parser.add_argument("--partitions", type=int, default=4)
   parser.add_argument("--batch_size", type=int, default=64)
+  parser.add_argument("--classes", type=int, default=3,
+                      help="classes of the exported model (its synthetic masks are scored)")
   parser.add_argument("--output", default=None, help="directory for the JSON-lines predictions")
   args = parser.parse_args()
   conf = SparkConf().setAppName("segmentation_inference") \

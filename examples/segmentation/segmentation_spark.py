@@ -26,15 +26,16 @@ IMG = 128
 EVAL_SEED = 99991   # held-out batches (--eval_steps): seeds apart from the training batches'
 
 
-def synth_rows(n, seed):
+def synth_rows(n, seed, classes=3):
   """Synthetic oxford-pets-like rows: (uint8 image [128,128,3], uint8 mask [128,128]) as numpy
   arrays - the feeder packs them column-wise into the shared-memory ring without touching
-  individual pixels in Python."""
+  individual pixels in Python.  Masks: models/unet.synthetic_labels (the trimap at 3 classes)."""
   import numpy as np
+  from tensorflowonspark_b200.models import unet
   rng = np.random.RandomState(seed)
   pool = min(n, 64)   # 64 distinct random images per partition, cycled: the generator must not
   imgs = rng.randint(0, 256, size=(pool, IMG, IMG, 3), dtype=np.uint8)   # be the bottleneck
-  masks = (imgs[..., 0] > 127).astype(np.uint8) + (imgs[..., 1] > 200).astype(np.uint8)
+  masks = unet.synthetic_labels(imgs, classes)
   return [(imgs[i % pool], masks[i % pool]) for i in range(n)]
 
 
@@ -49,7 +50,8 @@ def main_fun(args, ctx):
   comm = ctx.gradient_comm() if ctx.world_size > 1 else None   # one host: P2P/NVLS kernels; several: NCCL
   B = args.batch_size
   k = getattr(args, "encoder_trainable_from", None)   # None: frozen encoder, as the reference
-  net = unet.UNetTrainer(batch=B, image=IMG, classes=3, device="cuda:0", lr=args.learning_rate,
+  V = getattr(args, "classes", 3)
+  net = unet.UNetTrainer(batch=B, image=IMG, classes=V, device="cuda:0", lr=args.learning_rate,
                          comm=comm, **({} if k is None else {"encoder_trainable_from": k}))
   if comm is not None:
     comm.broadcast("weights", root=0)
@@ -62,7 +64,7 @@ def main_fun(args, ctx):
     if not held_out:   # this rank's shard, seeds apart from the training batches' (seed = rank)
       for i in range(eval_steps):
         x, _ = net.synthetic_batch(seed=EVAL_SEED + i * ctx.world_size + ctx.rank)
-        held_out.append((x, ((x[..., 0] > 127).to(torch.uint8) + (x[..., 1] > 200).to(torch.uint8))))
+        held_out.append((x, unet.synthetic_labels(x, V).to(torch.uint8)))
     res = net.evaluate(held_out)   # collective: every rank evaluates
     evaluated[0] = step
     if ctx.is_chief:
@@ -120,7 +122,7 @@ def main_fun(args, ctx):
     feed.terminate()
   else:
     x, y = net.synthetic_batch(seed=ctx.rank)
-    net.set_input(x, (x[..., 0] > 127).int() + (x[..., 1] > 200).int())
+    net.set_input(x, unet.synthetic_labels(x, V))
     net.train_step()
     net.capture()
     torch.cuda.synchronize()
@@ -163,6 +165,8 @@ if __name__ == "__main__":
   parser.add_argument("--epochs", type=int, default=1)
   parser.add_argument("--steps", type=int, default=50)
   parser.add_argument("--learning_rate", type=float, default=1e-3)
+  parser.add_argument("--classes", type=int, default=3,
+                      help="segmentation classes, 1..256 (labels: the trimap at 3, else red-channel bands)")
   parser.add_argument("--input_mode", default="tf", choices=["tf", "spark"])
   parser.add_argument("--num_examples", type=int, default=2048)
   parser.add_argument("--eval_steps", type=int, default=0,
@@ -184,7 +188,7 @@ if __name__ == "__main__":
   if args.input_mode == "spark":
     parts = args.cluster_size * 4
     per = args.num_examples // parts
-    rdd = sc.parallelize(range(parts), parts).flatMap(lambda i: synth_rows(per, i))
+    rdd = sc.parallelize(range(parts), parts).flatMap(lambda i: synth_rows(per, i, args.classes))
     cluster = TFCluster.run(sc, main_fun, args, args.cluster_size, num_ps=0,
                             input_mode=TFCluster.InputMode.SPARK, master_node="chief")
     cluster.train(rdd, args.epochs)

@@ -330,8 +330,42 @@ def _trainable_from(k, training):
   return int(k)
 
 
+#: most classes a U-Net can have: its masks (served output, DataFeed wire format) are uint8
+MAX_CLASSES = 256
+
+
+def _classes(v):
+  """Validated class count: an int in 1..MAX_CLASSES."""
+  if isinstance(v, bool) or not isinstance(v, numbers.Integral):
+    raise ValueError("classes must be an int in 1..{}, not {!r}".format(MAX_CLASSES, v))
+  if not 1 <= v <= MAX_CLASSES:
+    raise ValueError("classes must be in 1..{}, got {}".format(MAX_CLASSES, v))
+  return int(v)
+
+
+def padded_classes(classes):
+  """Channels of the logits for ``classes`` labels: 8 up to 8 classes (one 16-byte load per
+  pixel), else the next multiple of 8 (the wide kernels, csrc/seg_wide.cuh)."""
+  return 8 if classes <= 8 else -(-classes // 8) * 8
+
+
+def synthetic_labels(x, classes=3):
+  """Learnable synthetic labels of uint8 images [..., 3] (no dataset needed): at 3 classes the
+  trimap (red > 127) + (green > 200); at any other count the red channel quantised into
+  ``classes`` equal bands, red * classes // 256, which reaches every class of [0, classes).
+  A torch tensor gives int32 labels, a numpy array uint8 ones (the DataFeed wire format)."""
+  if isinstance(x, torch.Tensor):
+    if classes == 3:
+      return (x[..., 0] > 127).int() + (x[..., 1] > 200).int()
+    return x[..., 0].int() * classes // 256
+  if classes == 3:
+    return (x[..., 0] > 127).astype(np.uint8) + (x[..., 1] > 200).astype(np.uint8)
+  return (x[..., 0].astype(np.int32) * classes // 256).astype(np.uint8)
+
+
 class UNetTrainer(object):
-  """Static-buffer U-Net for ``batch`` images of ``image`` x ``image`` x 3 and ``classes`` labels.
+  """Static-buffer U-Net for ``batch`` images of ``image`` x ``image`` x 3 and ``classes`` labels
+  (1..256).  The head's logits have padded_classes(classes) channels.
   ``training=False`` builds only what the forward pass needs (predict, evaluate, serving): no
   gradient buffers, no backward or statistics-fused plans and no optimizer (``optim`` is None).
 
@@ -346,8 +380,9 @@ class UNetTrainer(object):
 
   def __init__(self, batch=64, image=128, classes=3, device="cuda:0", lr=1e-3, comm=None, seed=1234,
                training=True, encoder_trainable_from=None):
+    classes = _classes(classes)
     k = self.encoder_trainable_from = _trainable_from(encoder_trainable_from, training)
-    assert classes <= 8
+    self.VP = VP = padded_classes(classes)
     self.device = dev = torch.device(device)
     self.B, self.image, self.classes = batch, image, classes
     self.comm = comm
@@ -361,8 +396,8 @@ class UNetTrainer(object):
     for i, f in enumerate(self.UP):
       self.ups.append(_Upsample(st, "up{}".format(i), cin, f))
       cin = f + skips[-2 - i].shape[-1]
-    self.s_last = st.register("last.w", (cin, 3, 3, 8), True, he_normal(9 * cin))
-    self.s_last_b = st.register("last.b", (8,), False, constant(0.0))
+    self.s_last = st.register("last.w", (cin, 3, 3, VP), True, he_normal(9 * cin))
+    self.s_last_b = st.register("last.b", (VP,), False, constant(0.0))
     st.finalize(dev, alloc=comm.alloc if comm is not None else None, seed=seed, grads=tr)
     if k is not None:
       self.encoder.bind(st)
@@ -388,8 +423,8 @@ class UNetTrainer(object):
       self.cats.append((cat, act, skip, f))
       x, g_x = cat, g_cat
     h *= 2
-    self.logits = _buf((B, h, h, 8), dev)
-    self.dlogits = _buf((B, h, h, 8), dev) if tr else None
+    self.logits = _buf((B, h, h, VP), dev)
+    self.dlogits = _buf((B, h, h, VP), dev) if tr else None
     self.labels = torch.zeros(B, h, h, dtype=torch.int32, device=dev)
     self.p_last = igemm.conv_dgrad(x, st.w(self.s_last), self.logits, 2, 1, bias=st.f32(self.s_last_b))
     self.p_last_wgrad = self.p_last_dgrad = self.optim = None
@@ -590,27 +625,47 @@ SEG_COUNT, SEG_CORRECT, SEG_INVALID, SEG_LOSS, SEG_CONFUSION, SEG_SLOTS = 0, 1, 
 SEG_IMAGES, SEG_ACC = 68, 72
 
 
+def seg_eval_layout(classes):
+  """(images slot, first confusion slot, confusion row stride, accumulator length) of the
+  evaluation accumulator for ``classes`` labels.  Up to 8 classes: the SEG_* layout, an 8 x 8
+  confusion matrix.  More: [count, correct, invalid, loss, images, confusion classes x classes]
+  (csrc/ops.h kSegWide*; the binding's seg_eval_slots(classes) is its length)."""
+  if classes <= 8:
+    return SEG_IMAGES, SEG_CONFUSION, 8, SEG_ACC
+  return 4, 5, classes, 5 + classes * classes
+
+
 def seg_eval_result(totals, classes):
-  """Host metrics from the summed accumulator ``totals`` (a sequence of SEG_ACC floats):
+  """Host metrics from the summed accumulator ``totals`` (seg_eval_layout(classes) floats):
   {"count": scored pixels, "images", "loss", "accuracy", "mean_iou", "iou": [classes values]}.
   IoU of class c = cm[c, c] / (row_c + col_c - cm[c, c]) of the confusion matrix cm[label, pred];
   a class with an empty union has IoU NaN and is left out of mean_iou (NaN when every class is).
   loss and accuracy are means over the scored pixels (NaN when there are none).  Raises
   ValueError when any mask value was outside [0, classes)."""
-  h = [float(v) for v in totals]
+  images, conf, ld, _ = seg_eval_layout(classes)
+  if classes <= 8:
+    h = [float(v) for v in totals]
+    cm = [h[conf + ld * y:conf + ld * y + ld] for y in range(ld)]
+    iou = []
+    for c in range(classes):
+      inter = cm[c][c]
+      union = sum(cm[c][:classes]) + sum(cm[y][c] for y in range(classes)) - inter
+      iou.append(inter / union if union > 0 else float("nan"))
+  else:   # V x V cells: numpy (the same sums, in float64, of integer-valued counts)
+    t = np.asarray(totals, dtype=np.float64)
+    h = [float(v) for v in t[:conf]]
+    cm = t[conf:conf + classes * classes].reshape(classes, classes)
+    inter = np.diagonal(cm)
+    union = cm.sum(axis=1) + cm.sum(axis=0) - inter
+    with np.errstate(invalid="ignore", divide="ignore"):
+      iou = [float(v) for v in np.where(union > 0, inter / np.where(union > 0, union, 1), np.nan)]
   if h[SEG_INVALID] > 0:
     raise ValueError("evaluation saw {} mask value(s) outside [0, {})".format(
         int(h[SEG_INVALID]), classes))
   count = int(h[SEG_COUNT])
-  cm = [h[SEG_CONFUSION + 8 * y:SEG_CONFUSION + 8 * y + 8] for y in range(8)]
-  iou = []
-  for c in range(classes):
-    inter = cm[c][c]
-    union = sum(cm[c][:classes]) + sum(cm[y][c] for y in range(classes)) - inter
-    iou.append(inter / union if union > 0 else float("nan"))
   seen = [v for v in iou if v == v]
   mean = (lambda v: v / count) if count else (lambda v: float("nan"))
-  return {"count": count, "images": int(h[SEG_IMAGES]), "loss": mean(h[SEG_LOSS]),
+  return {"count": count, "images": int(h[images]), "loss": mean(h[SEG_LOSS]),
           "accuracy": mean(h[SEG_CORRECT]),
           "mean_iou": sum(seen) / len(seen) if seen else float("nan"), "iou": iou}
 
@@ -641,9 +696,10 @@ class _SegEvaluator(object):
     self.u8 = torch.zeros_like(net.in_u8)         # never in_u8: drivers stage a batch and replay
     self.labels = torch.zeros_like(net.labels)
     self.n_valid = torch.zeros(1, dtype=torch.int32, device=dev)
-    self.acc = torch.zeros(SEG_ACC, dtype=torch.float64, device=dev)
-    self.partial = torch.zeros(ops.C().seg_eval_scratch(self.labels.numel()), dtype=torch.float64,
-                               device=dev)
+    self.images_slot, _, _, slots = seg_eval_layout(self.V)
+    self.acc = torch.zeros(slots, dtype=torch.float64, device=dev)
+    self.partial = torch.zeros(ops.C().seg_eval_scratch(self.labels.numel(), self.V),
+                               dtype=torch.float64, device=dev)
     self.counter = torch.zeros(1, dtype=torch.int32, device=dev)
     if comm is None:
       self.running = net.running.tensor()
@@ -654,7 +710,7 @@ class _SegEvaluator(object):
     self.bn = [(view(up.bn.running_mean), view(up.bn.running_var),
                 torch.zeros(up.cout, dtype=torch.float32, device=dev),
                 torch.zeros(up.cout, dtype=torch.float32, device=dev)) for up in net.ups]
-    self.rank_sum = evaluation.RankSum(comm, "seg_eval_totals", SEG_ACC)
+    self.rank_sum = evaluation.RankSum(comm, "seg_eval_totals", slots)
     self.staging = evaluation.HostStaging(dev, net.B, self.u8.shape[1:], self.labels.shape[1:])
     self.graph, self.calls, self.images = None, 0, 0
 
@@ -712,7 +768,7 @@ class _SegEvaluator(object):
                      lambda y: torch.uint8 if y.dtype == np.uint8 else torch.int32)
 
   def end(self):
-    self.acc[SEG_IMAGES].fill_(self.images)
+    self.acc[self.images_slot].fill_(self.images)
     return seg_eval_result(self.rank_sum(self.acc), self.V)
 
 
@@ -723,7 +779,9 @@ class ServedUNet(serving.Replica):
   pixel is predicted as - exactly the prediction evaluation scores (seg_predict); ``logits``:
   fp32 [n, H, W, classes].  The forward pass + seg_predict run as one CUDA graph after the first
   batch; ``select_outputs`` keeps the logits (12x the bytes of the mask at 3 classes) on the
-  device unless they are asked for (models/serving.Replica)."""
+  device unless they are asked for (models/serving.Replica).  Above 8 classes the logits'
+  device buffer (2.5 GB at batch 256 and 150 classes) is only allocated once ``logits`` is
+  selected."""
 
   def __init__(self, state, image=128, classes=3, batch=256, device="cuda:0"):
     torch.cuda.set_device(torch.device(device))
@@ -733,7 +791,9 @@ class ServedUNet(serving.Replica):
     self.image, self.V = image, classes
     dev = self.net.device
     self.mask = torch.zeros(batch, image, image, dtype=torch.uint8, device=dev)
-    self.logits = torch.zeros(batch, image, image, classes, dtype=torch.float32, device=dev)
+    self._logits_shape = (batch, image, image, classes)
+    self.logits = None if classes > 8 else torch.zeros(self._logits_shape, dtype=torch.float32,
+                                                       device=dev)
     super(ServedUNet, self).__init__(dev, batch, (image, image, 3),
                                      {"mask": self.mask, "logits": self.logits},
                                      self.net.set_input)
@@ -744,9 +804,12 @@ class ServedUNet(serving.Replica):
     self._select_outputs(names)
 
   def _run(self):
+    want = "logits" in self.selected
+    if want and self.logits is None:   # first eager batch with logits selected (never in capture)
+      self.logits = torch.zeros(self._logits_shape, dtype=torch.float32, device=self.net.device)
+      self._outputs["logits"] = self.logits
     self.net._forward(False)
-    ops.K.seg_predict(self.net.logits, self.mask,
-                      self.logits if "logits" in self.selected else None, self.V)
+    ops.K.seg_predict(self.net.logits, self.mask, self.logits if want else None, self.V)
 
 
 def build_served(state, image=128, classes=3, batch=None, **_):

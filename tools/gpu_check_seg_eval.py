@@ -1,6 +1,10 @@
 """Multi-GPU checks of the U-Net's held-out evaluation (run under torchrun, one rank per GPU):
 
-  python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 tools/gpu_check_seg_eval.py
+  python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 tools/gpu_check_seg_eval.py \
+      [--classes V]
+
+``--classes`` (default 3) sets the class count: above 8 the evaluation runs the wide kernel and
+its [count, correct, invalid, loss, images, V x V confusion] accumulator.
 
 A UNetTrainer per rank trains 3 steps on the rank's own batch (so the ranks' running statistics
 differ), then evaluates its shard of a held-out set through
@@ -12,6 +16,7 @@ Checks: (a) eval_end() is identical on every rank; (b) the summed totals (count,
 confusion matrix) equal those of a one-GPU trainer loaded with rank 0's state_dict() that scores
 the union of the shards, and the loss agrees to fp64 summation order.
 """
+import argparse
 import math
 import os
 import sys
@@ -25,6 +30,9 @@ B, IMG, N = 4, 64, 3 * 4 + 3
 
 
 def main():
+  p = argparse.ArgumentParser()
+  p.add_argument("--classes", type=int, default=3)
+  V = p.parse_args().classes
   rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
   local = int(os.environ.get("LOCAL_RANK", rank))
   torch.cuda.set_device(local)
@@ -42,17 +50,18 @@ def main():
 
   g = torch.Generator().manual_seed(99)   # the same held-out set on every rank
   X = torch.randint(0, 256, (N, IMG, IMG, 3), dtype=torch.uint8, generator=g).to(dev)
-  Y = ((X[..., 0] > 127).int() + (X[..., 1] > 200).int()).to(torch.int32)
+  Y = unet.synthetic_labels(X, V).to(torch.int32)
+  _, conf, ld, _ = unet.seg_eval_layout(V)
 
   def batches(x, y):
     return [(x[i:i + B], y[i:i + B]) for i in range(0, len(x), B)]
 
   def exact(acc):   # count, correct, invalid, confusion matrix
     a = acc.cpu()
-    return torch.cat([a[:3], a[4:68]])
+    return torch.cat([a[:3], a[conf:conf + ld * ld]])
 
   def run(tag, comm):
-    net = unet.UNetTrainer(batch=B, image=IMG, classes=3, device=dev, comm=comm, seed=5, lr=1e-3)
+    net = unet.UNetTrainer(batch=B, image=IMG, classes=V, device=dev, comm=comm, seed=5, lr=1e-3)
     comm.broadcast("weights", root=0)
     comm.broadcast("aux32", root=0)
     x, _ = net.synthetic_batch(seed=rank)         # each rank trains on its own batch
@@ -68,7 +77,7 @@ def main():
     sd = net.state_dict()                          # rank 0's parameters and running statistics
     obj = [sd if rank == 0 else None]
     dist.broadcast_object_list(obj, src=0)
-    ref = unet.UNetTrainer(batch=B, image=IMG, classes=3, device=dev, seed=5)
+    ref = unet.UNetTrainer(batch=B, image=IMG, classes=V, device=dev, seed=5)
     ref.load_state_dict(obj[0])
     union = torch.cat([torch.arange(N)[r::world] for r in range(world)])
     one = ref.evaluate(batches(X[union.to(dev)], Y[union.to(dev)]))
