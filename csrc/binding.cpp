@@ -5,6 +5,7 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
+#include <cstdint>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -504,8 +505,53 @@ int64_t seg_eval_slots(int64_t V) {
   TORCH_CHECK(V >= 1 && V <= 256, "seg_eval_slots: V in [1, 256]");
   return V <= 8 ? tfos::kSegEvalSlots : tfos::seg_eval_wide_slots(static_cast<int>(V));
 }
+// The segmentation loss options (ops.h SegLossOpts) from the optional binding arguments:
+// ignore_index an int32 value, weights fp32 with at least V entries on ref's device.
+tfos::SegLossOpts seg_loss_opts(const Tensor& ref, c10::optional<int64_t> ignore_index,
+                                const c10::optional<Tensor>& weights, int64_t V,
+                                const char* what) {
+  tfos::SegLossOpts o{0, 0, nullptr, nullptr};
+  if (ignore_index.has_value()) {
+    TORCH_CHECK(*ignore_index >= INT32_MIN && *ignore_index <= INT32_MAX, what,
+                ": ignore_index must fit in int32");
+    o.ignore = static_cast<int>(*ignore_index);
+    o.has_ignore = 1;
+  }
+  if (weights.has_value() && weights->defined()) {
+    need(*weights, torch::kFloat32, "weights");
+    TORCH_CHECK(weights->numel() >= V, what, ": weights needs one entry per class");
+    TORCH_CHECK(weights->device() == ref.device(), what, ": tensors on different devices");
+    o.weights = weights->data_ptr<float>();
+  }
+  return o;
+}
+int64_t seg_label_norm_scratch(int64_t V) {
+  TORCH_CHECK(V >= 1 && V <= 256, "seg_label_norm_scratch: V in [1, 256]");
+  return tfos::seg_label_norm_scratch(static_cast<int>(V));
+}
+// norm [3] fp64 = [sum over the labels that are not ignore_index of w[y], their count, inv]
+void seg_label_norm(const Tensor& labels, Tensor norm, Tensor scratch, int64_t V,
+                    c10::optional<int64_t> ignore_index, c10::optional<Tensor> weights) {
+  need(labels, torch::kInt32, "labels");
+  need(norm, torch::kFloat64, "norm");
+  need(scratch, torch::kInt64, "scratch");
+  TORCH_CHECK(V >= 1 && V <= 256, "seg_label_norm: V in [1, 256]");
+  TORCH_CHECK(labels.numel() > 0, "seg_label_norm: no labels");
+  TORCH_CHECK(norm.numel() >= 3, "seg_label_norm: norm needs 3 slots");
+  TORCH_CHECK(scratch.numel() >= seg_label_norm_scratch(V),
+              "seg_label_norm: scratch needs seg_label_norm_scratch(V) words");
+  for (const Tensor& t : {norm, scratch})
+    TORCH_CHECK(t.device() == labels.device(), "seg_label_norm: tensors on different devices");
+  const tfos::SegLossOpts o = seg_loss_opts(labels, ignore_index, weights, V, "seg_label_norm");
+  check(tfos::seg_label_norm(labels.data_ptr<int>(), labels.numel(), static_cast<int>(V), o,
+                             norm.data_ptr<double>(),
+                             reinterpret_cast<unsigned long long*>(scratch.data_ptr<int64_t>()),
+                             cur_stream()),
+        "seg_label_norm");
+}
 void seg_eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& n_valid,
-                      Tensor acc, Tensor partial, Tensor counter, int V) {
+                      Tensor acc, Tensor partial, Tensor counter, int V,
+                      c10::optional<int64_t> ignore_index, c10::optional<Tensor> weights) {
   need(logits, torch::kBFloat16, "logits");
   need(labels, torch::kInt32, "labels");
   need(n_valid, torch::kInt32, "n_valid");
@@ -523,6 +569,18 @@ void seg_eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& 
   TORCH_CHECK(partial.numel() >= seg_eval_scratch(pixels, V),
               "seg_eval_metrics: partial needs seg_eval_scratch(pixels, V) doubles");
   TORCH_CHECK(counter.numel() >= 1, "seg_eval_metrics: counter");
+  if (ignore_index.has_value() || (weights.has_value() && weights->defined())) {
+    for (const Tensor& t : {labels, n_valid, acc, partial, counter})
+      TORCH_CHECK(t.device() == logits.device(), "seg_eval_metrics: tensors on different devices");
+    const tfos::SegLossOpts o = seg_loss_opts(logits, ignore_index, weights, V, "seg_eval_metrics");
+    check(tfos::seg_eval_metrics_opt(
+              logits.data_ptr(), labels.data_ptr<int>(), n_valid.data_ptr<int>(),
+              acc.data_ptr<double>(), partial.data_ptr<double>(),
+              reinterpret_cast<unsigned int*>(counter.data_ptr<int>()), static_cast<int>(images),
+              pixels / images, static_cast<int>(VP), V, o, cur_stream()),
+          "seg_eval_metrics");
+    return;
+  }
   if (VP > 8) {
     for (const Tensor& t : {labels, n_valid, acc, partial, counter})
       TORCH_CHECK(t.device() == logits.device(), "seg_eval_metrics: tensors on different devices");
@@ -668,9 +726,36 @@ void copy_channels(const Tensor& src, Tensor dst, int C, int src_off, int dst_of
         "copy_channels");
 }
 void pixel_xent(const Tensor& logits, const Tensor& labels, c10::optional<Tensor> dlogits,
-                Tensor loss_sum, c10::optional<Tensor> correct, int V, double scale) {
+                Tensor loss_sum, c10::optional<Tensor> correct, int V, double scale,
+                c10::optional<int64_t> ignore_index, c10::optional<Tensor> weights,
+                c10::optional<Tensor> norm) {
   need(logits, torch::kBFloat16, "logits");
   need(labels, torch::kInt32, "labels");
+  const bool opt = ignore_index.has_value() || (weights.has_value() && weights->defined()) ||
+                   (norm.has_value() && norm->defined());
+  if (opt) {   // the loss options: scale is inv from norm (seg_label_norm of these labels)
+    TORCH_CHECK(seg_channels_match(logits, V), "pixel_xent: logits [B, ..., VP] with V in [1, 256] and "
+                "VP = 8 for V <= 8, ceil(V / 8) * 8 above");
+    TORCH_CHECK(norm.has_value() && norm->defined(), "pixel_xent: the loss options need norm");
+    need(*norm, torch::kFloat64, "norm");
+    TORCH_CHECK(norm->numel() >= 3, "pixel_xent: norm needs 3 slots");
+    const int64_t VP = logits.size(-1);
+    const int64_t P = logits.numel() / VP;
+    TORCH_CHECK(labels.numel() == P, "pixel_xent: one label per pixel");
+    const void* d = optptr(dlogits);
+    if (d != nullptr)
+      TORCH_CHECK(dlogits->sizes() == logits.sizes() && dlogits->scalar_type() == torch::kBFloat16,
+                  "pixel_xent: dlogits must be bf16 with the shape of logits");
+    TORCH_CHECK(norm->device() == logits.device() && labels.device() == logits.device(),
+                "pixel_xent: tensors on different devices");
+    tfos::SegLossOpts o = seg_loss_opts(logits, ignore_index, weights, V, "pixel_xent");
+    o.norm = norm->data_ptr<double>();
+    check(tfos::pixel_xent_opt(logits.data_ptr(), labels.data_ptr<int>(), const_cast<void*>(d),
+                               loss_sum.data_ptr<float>(), optf(correct), P, static_cast<int>(VP),
+                               V, o, cur_stream()),
+          "pixel_xent");
+    return;
+  }
   if (logits.size(-1) > 8) {
     TORCH_CHECK(seg_channels_match(logits, V), "pixel_xent: logits [B, ..., VP] with V in [1, 256] and "
                 "VP = 8 for V <= 8, ceil(V / 8) * 8 above");
@@ -947,7 +1032,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("eval_metrics", &eval_metrics);
   m.def("seg_eval_scratch", &seg_eval_scratch, py::arg("pixels"), py::arg("classes") = 8);
   m.def("seg_eval_slots", &seg_eval_slots);
-  m.def("seg_eval_metrics", &seg_eval_metrics);
+  m.def("seg_eval_metrics", &seg_eval_metrics, py::arg("logits"), py::arg("labels"),
+        py::arg("n_valid"), py::arg("acc"), py::arg("partial"), py::arg("counter"), py::arg("V"),
+        py::arg("ignore_index") = py::none(), py::arg("weights") = py::none());
+  m.def("seg_label_norm_scratch", &seg_label_norm_scratch);
+  m.def("seg_label_norm", &seg_label_norm, py::arg("labels"), py::arg("norm"), py::arg("scratch"),
+        py::arg("V"), py::arg("ignore_index") = py::none(), py::arg("weights") = py::none());
   m.def("seg_predict", &seg_predict);
   m.def("conv3x3_c1_fwd", &conv3x3_c1_fwd);
   m.def("conv3x3_c1_wgrad", &conv3x3_c1_wgrad);
@@ -958,7 +1048,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("dy"), py::arg("add"), py::arg("add_off"), py::arg("dx"), py::arg("dw"),
         py::arg("dbias"), py::arg("dbias_in"), py::arg("scratch"), py::arg("stride"));
   m.def("copy_channels", &copy_channels);
-  m.def("pixel_xent", &pixel_xent);
+  m.def("pixel_xent", &pixel_xent, py::arg("logits"), py::arg("labels"), py::arg("dlogits"),
+        py::arg("loss_sum"), py::arg("correct"), py::arg("V"), py::arg("scale"),
+        py::arg("ignore_index") = py::none(), py::arg("weights") = py::none(),
+        py::arg("norm") = py::none());
   m.def("allreduce_opt", &allreduce_opt);
   m.def("lars_norms", &lars_norms);
   m.def("bcast_pull", &bcast_pull);

@@ -615,11 +615,16 @@ copy_channels_kernel(const __nv_bfloat16* __restrict__ src, __nv_bfloat16* __res
 
 // Per-pixel softmax cross-entropy for a handful of classes (V <= 8): one thread per pixel, the
 // pixel's 8 padded logits are one 16-byte load.  loss_sum += -log p[label] * scale,
-// dlogits = (p - onehot) * scale, padded channels get zero gradient.
-__global__ void __launch_bounds__(256)
-pixel_xent_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
-                  __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
-                  long long P, int V, float scale) {
+// dlogits = (p - onehot) * scale, padded channels get zero gradient.  kOpt (pixel_xent_opt_kernel):
+// the loss options of seg_wide.cuh, scale = w[label] * inv with inv from o.norm; a pixel with
+// scale 0 (ignored, zero weight, or an empty batch) adds nothing and gets an exact zero gradient.
+template <bool kOpt>
+__device__ __forceinline__ void pixel_xent_body(const __nv_bfloat16* __restrict__ logits,
+                                                const int* __restrict__ labels,
+                                                __nv_bfloat16* __restrict__ dlogits,
+                                                float* loss_sum, float* correct_sum, long long P,
+                                                int V, float scale, const SegLossOpts& o) {
+  if (kOpt) scale = static_cast<float>(o.norm[2]);
   float local = 0.f, hits = 0.f;
   for (long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; p < P;
        p += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -637,16 +642,19 @@ pixel_xent_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restric
       se += e[j];
     }
     const int label = labels[p];
+    const bool scored = !kOpt || !seg_ignored(o, label);
+    const float s = kOpt ? (scored ? seg_weight(o, label, V) * scale : 0.f) : scale;
+    const bool live = !kOpt || s != 0.f;
     const float inv = 1.f / se;
     float lab_logit = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       if (j == label) lab_logit = l[j];
-      e[j] = j < V ? (e[j] * inv - (j == label ? 1.f : 0.f)) * scale : 0.f;
+      e[j] = j < V && live ? (e[j] * inv - (j == label ? 1.f : 0.f)) * s : 0.f;
     }
     if (dlogits != nullptr) store8(dlogits + p * 8, e);
-    local += -(lab_logit - mx - __logf(se)) * scale;
-    hits += (am == label) ? 1.f : 0.f;
+    if (live) local += -(lab_logit - mx - __logf(se)) * s;
+    hits += (scored && am == label) ? 1.f : 0.f;
   }
   for (int o = 16; o >= 1; o >>= 1) {
     local += __shfl_xor_sync(0xffffffff, local, o);
@@ -658,18 +666,36 @@ pixel_xent_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restric
   }
 }
 
+__global__ void __launch_bounds__(256)
+pixel_xent_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                  __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
+                  long long P, int V, float scale) {
+  pixel_xent_body<false>(logits, labels, dlogits, loss_sum, correct_sum, P, V, scale,
+                         SegLossOpts{});
+}
+
+__global__ void __launch_bounds__(256)
+pixel_xent_opt_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                      __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
+                      long long P, int V, const SegLossOpts o) {
+  pixel_xent_body<true>(logits, labels, dlogits, loss_sum, correct_sum, P, V, 0.f, o);
+}
+
 // pixel_xent for VP = 16..256 padded channels (V = 9..256 classes): G lanes per pixel
 // (seg_wide.cuh), each lane one 16-byte chunk of the logits in registers, so every pixel's logits
 // are read once and its dlogits written once.  Warp tile t covers pixels [t * 32 / G, ...); the
 // loop bound is uniform over the warp, so the full-mask group shuffles are safe.  Channels
 // j >= V get exactly zero gradient and never enter the loss or the arg-max.  A label outside
 // [0, V) (not validated, as for the 8-channel kernel) contributes the loss mx + log(se), a
-// gradient without the one-hot term and no hit.
-template <int G>
-__global__ void __launch_bounds__(256)
-pixel_xent_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
-                       __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
-                       long long P, int VP, int V, float scale) {
+// gradient without the one-hot term and no hit.  kOpt: the loss options, as pixel_xent_body.
+template <int G, bool kOpt>
+__device__ __forceinline__ void pixel_xent_wide_body(const __nv_bfloat16* __restrict__ logits,
+                                                     const int* __restrict__ labels,
+                                                     __nv_bfloat16* __restrict__ dlogits,
+                                                     float* loss_sum, float* correct_sum,
+                                                     long long P, int VP, int V, float scale,
+                                                     const SegLossOpts& o) {
+  if (kOpt) scale = static_cast<float>(o.norm[2]);
   constexpr int kPix = 32 / G;   // pixels per warp tile
   const int lane = threadIdx.x & 31, sub = lane & (G - 1), c0 = sub * 8;
   const long long nw = static_cast<long long>(gridDim.x) * (256 / 32);
@@ -688,6 +714,9 @@ pixel_xent_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __re
     float mx;
     const int am = seg_argmax_wide<G>(l, c0, V, mx);
     const int y = in ? labels[p] : -1;
+    const bool scored = !kOpt || (in && !seg_ignored(o, y));
+    const float s = kOpt ? (scored ? seg_weight(o, y, V) * scale : 0.f) : scale;
+    const bool weighed = !kOpt || s != 0.f;
     float e[8], se = 0.f, ly = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
@@ -700,11 +729,11 @@ pixel_xent_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __re
     const float inv = 1.f / se;
 #pragma unroll
     for (int k = 0; k < 8; ++k)
-      e[k] = c0 + k < V ? (e[k] * inv - (c0 + k == y ? 1.f : 0.f)) * scale : 0.f;
+      e[k] = c0 + k < V && weighed ? (e[k] * inv - (c0 + k == y ? 1.f : 0.f)) * s : 0.f;
     if (dlogits != nullptr && live) store8(dlogits + p * VP + c0, e);
     if (in && sub == 0) {
-      local += -(ly - mx - __logf(se)) * scale;
-      hits += (am == y) ? 1.f : 0.f;
+      if (weighed) local += -(ly - mx - __logf(se)) * s;
+      hits += (scored && am == y) ? 1.f : 0.f;
     }
   }
   for (int o = 16; o >= 1; o >>= 1) {
@@ -714,6 +743,99 @@ pixel_xent_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __re
   if ((threadIdx.x & 31) == 0) {
     atomicAdd(loss_sum, local);
     if (correct_sum != nullptr) atomicAdd(correct_sum, hits);
+  }
+}
+
+template <int G>
+__global__ void __launch_bounds__(256)
+pixel_xent_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                       __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
+                       long long P, int VP, int V, float scale) {
+  pixel_xent_wide_body<G, false>(logits, labels, dlogits, loss_sum, correct_sum, P, VP, V, scale,
+                                 SegLossOpts{});
+}
+
+template <int G>
+__global__ void __launch_bounds__(256)
+pixel_xent_wide_opt_kernel(const __nv_bfloat16* __restrict__ logits,
+                           const int* __restrict__ labels, __nv_bfloat16* __restrict__ dlogits,
+                           float* loss_sum, float* correct_sum, long long P, int VP, int V,
+                           const SegLossOpts o) {
+  pixel_xent_wide_body<G, true>(logits, labels, dlogits, loss_sum, correct_sum, P, VP, V, 0.f, o);
+}
+
+// seg_label_norm: one CTA per SM over the labels.  Each CTA counts its labels per class in shared
+// memory (warp-aggregated atomics; bin V for labels outside [0, V), ignored labels skipped) and
+// adds the non-zero bins to the global uint64 table; the last CTA to finish (ticket counter)
+// forms sum_c w_c n_c in fp64 with a fixed thread -> class assignment and reduction tree, writes
+// norm and zeroes the table and the ticket for the next launch or graph replay.
+constexpr int kNormThreads = 512;
+constexpr int kNormWarps = kNormThreads / 32;
+constexpr int kNormUnroll = 8;   // labels in flight per thread
+constexpr int kNormMaxBins = 256 + 1;
+
+__global__ void __launch_bounds__(kNormThreads)
+seg_label_norm_kernel(const int* __restrict__ labels, long long P, int V, const SegLossOpts o,
+                      double* __restrict__ norm, unsigned long long* __restrict__ table) {
+  __shared__ unsigned int bins[kNormMaxBins];
+  __shared__ double wsum[kNormWarps];
+  __shared__ unsigned long long wcnt[kNormWarps];
+  __shared__ unsigned int is_last;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int i = threadIdx.x; i <= V; i += kNormThreads) bins[i] = 0u;
+  __syncthreads();
+  const long long stride = static_cast<long long>(gridDim.x) * kNormThreads;
+  // the bound is uniform over the warp: full-mask __match_any_sync is safe
+  for (long long base = static_cast<long long>(blockIdx.x) * kNormThreads + warp * 32; base < P;
+       base += stride * kNormUnroll) {
+    int y[kNormUnroll];
+#pragma unroll
+    for (int u = 0; u < kNormUnroll; ++u) {
+      const long long p = base + u * stride + lane;
+      y[u] = p < P ? labels[p] : 0;
+    }
+#pragma unroll
+    for (int u = 0; u < kNormUnroll; ++u) {
+      const long long p = base + u * stride + lane;
+      const int bin = p >= P || seg_ignored(o, y[u]) ? -1 : (y[u] >= 0 && y[u] < V ? y[u] : V);
+      const unsigned same = __match_any_sync(0xffffffffu, bin);
+      if (bin >= 0 && lane == __ffs(same) - 1) atomicAdd(&bins[bin], __popc(same));
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i <= V; i += kNormThreads)
+    if (bins[i]) atomicAdd(&table[i], static_cast<unsigned long long>(bins[i]));
+  __threadfence();
+  __syncthreads();
+  unsigned int* counter = reinterpret_cast<unsigned int*>(table + V + 1);
+  if (threadIdx.x == 0) is_last = (atomicAdd(counter, 1u) == gridDim.x - 1) ? 1u : 0u;
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  // thread t owns bin t (kNormThreads > kNormMaxBins): a fixed order for the fp64 sum
+  const int i = threadIdx.x;
+  unsigned long long n = 0ull;
+  double w = 0.0;
+  if (i <= V) {
+    n = __ldcg(table + i);
+    table[i] = 0ull;
+    w = static_cast<double>(n) * static_cast<double>(seg_weight(o, i, V));
+  }
+#pragma unroll
+  for (int k = 16; k >= 1; k >>= 1) {
+    w += __shfl_xor_sync(0xffffffffu, w, k);
+    n += __shfl_xor_sync(0xffffffffu, n, k);
+  }
+  if (lane == 0) wsum[warp] = w, wcnt[warp] = n;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double sw = 0.0;
+    unsigned long long cnt = 0ull;
+    for (int k = 0; k < kNormWarps; ++k) sw += wsum[k], cnt += wcnt[k];
+    norm[0] = sw;
+    norm[1] = static_cast<double>(cnt);
+    norm[2] = sw > 0.0 ? static_cast<double>(static_cast<float>(1.0 / sw)) : 0.0;
+    *counter = 0u;
   }
 }
 
@@ -892,6 +1014,41 @@ cudaError_t pixel_xent_wide(const void* logits, const int* labels, void* dlogits
     default: return cudaErrorInvalidValue;
   }
 #undef TFOS_XENT_WIDE
+  TFOS_RET();
+}
+cudaError_t pixel_xent_opt(const void* logits, const int* labels, void* dlogits, float* loss_sum,
+                           float* correct_sum, long long P, int VP, int V, SegLossOpts o,
+                           cudaStream_t s) {
+  const auto* l = static_cast<const __nv_bfloat16*>(logits);
+  auto* d = static_cast<__nv_bfloat16*>(dlogits);
+  if (VP == 8) {
+    pixel_xent_opt_kernel<<<grid_for(P, 256, kMaxBlocks), 256, 0, s>>>(l, labels, d, loss_sum,
+                                                                         correct_sum, P, V, o);
+    TFOS_RET();
+  }
+  const int G = seg_wide_group(VP);
+  const int grid = grid_for(P * G, 256, kMaxBlocks);
+#define TFOS_XENT_WIDE_OPT(g)                                                                 \
+  case g:                                                                                     \
+    pixel_xent_wide_opt_kernel<g><<<grid, 256, 0, s>>>(l, labels, d, loss_sum, correct_sum, P, \
+                                                       VP, V, o);                             \
+    break;
+  switch (G) {
+    TFOS_XENT_WIDE_OPT(2)
+    TFOS_XENT_WIDE_OPT(4)
+    TFOS_XENT_WIDE_OPT(8)
+    TFOS_XENT_WIDE_OPT(16)
+    TFOS_XENT_WIDE_OPT(32)
+    default: return cudaErrorInvalidValue;
+  }
+#undef TFOS_XENT_WIDE_OPT
+  TFOS_RET();
+}
+cudaError_t seg_label_norm(const int* labels, long long P, int V, SegLossOpts o, double* norm,
+                           unsigned long long* scratch, cudaStream_t s) {
+  if (V < 1 || V > kNormMaxBins - 1) return cudaErrorInvalidValue;
+  seg_label_norm_kernel<<<grid_for(P, kNormThreads * kNormUnroll, kSmCount), kNormThreads, 0, s>>>(
+      labels, P, V, o, norm, scratch);
   TFOS_RET();
 }
 cudaError_t cast_f32_bf16(const float* in, void* out, long long n, cudaStream_t s) {

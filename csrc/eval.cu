@@ -146,8 +146,12 @@ __device__ __forceinline__ void unpack_bf16x8(const uint4 v, float (&l)[8]) {
 }
 
 // One pixel: its bin (y * 8 + pred, kSegBins - 1 for a label outside [0, V)) and loss.  pred is
-// seg_argmax, so an evaluation's "correct" counts exactly what training's does.
-__device__ __forceinline__ int seg_score(const uint4 v, const int y, const int V, double& loss) {
+// seg_argmax, so an evaluation's "correct" counts exactly what training's does.  kOpt: the loss
+// options (seg_wide.cuh): an ignored pixel has no bin (-1), the loss term is weighted by w[y].
+template <bool kOpt>
+__device__ __forceinline__ int seg_score(const uint4 v, const int y, const int V, double& loss,
+                                         const SegLossOpts& o) {
+  if (kOpt && seg_ignored(o, y)) return -1;
   if (y < 0 || y >= V) return kSegBins - 1;
   float l[8];
   unpack_bf16x8(v, l);
@@ -159,7 +163,12 @@ __device__ __forceinline__ int seg_score(const uint4 v, const int y, const int V
     if (j < V) se += __expf(l[j] - mx);
     if (j == y) ly = l[j];
   }
-  loss += static_cast<double>(__logf(se) + mx - ly);
+  if (kOpt) {
+    const float w = seg_weight(o, y, V);
+    if (w != 0.f) loss += static_cast<double>(w) * static_cast<double>(__logf(se) + mx - ly);
+  } else {
+    loss += static_cast<double>(__logf(se) + mx - ly);
+  }
   return y * 8 + am;
 }
 
@@ -172,11 +181,12 @@ __device__ __forceinline__ int seg_score(const uint4 v, const int y, const int V
 // per-thread fp64 sum reduced in a fixed tree.  The CTA writes its partials slot-major
 // (partial[s * grid + b]); the last CTA to finish sums each slot over the CTAs with a fixed
 // lane -> CTA assignment and shuffle tree.  So the totals are bitwise reproducible.
-__global__ void __launch_bounds__(kSegThreads)
-seg_eval_metrics_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
-                        const int* __restrict__ n_valid, double* __restrict__ acc,
-                        double* __restrict__ partial, unsigned int* __restrict__ counter,
-                        int images, long long ppi, long long chunk, int V) {
+template <bool kOpt>
+__device__ __forceinline__ void seg_eval_metrics_body(
+    const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+    const int* __restrict__ n_valid, double* __restrict__ acc, double* __restrict__ partial,
+    unsigned int* __restrict__ counter, int images, long long ppi, long long chunk, int V,
+    const SegLossOpts& o) {
   __shared__ int bins[kSegWarps][kSegBins];
   __shared__ int cells[kSegBins];
   __shared__ double wloss[kSegWarps];
@@ -204,7 +214,7 @@ seg_eval_metrics_kernel(const __nv_bfloat16* __restrict__ logits, const int* __r
 #pragma unroll
     for (int u = 0; u < kSegUnroll; ++u) {
       const long long p = base + u * kSegThreads + threadIdx.x;
-      const int bin = p < hi ? seg_score(v[u], y[u], V, loss) : -1;
+      const int bin = p < hi ? seg_score<kOpt>(v[u], y[u], V, loss, o) : -1;
       const unsigned same = __match_any_sync(0xffffffffu, bin);
       if (bin >= 0 && lane == __ffs(same) - 1) atomicAdd(&bins[warp][bin], __popc(same));
     }
@@ -263,6 +273,25 @@ seg_eval_metrics_kernel(const __nv_bfloat16* __restrict__ logits, const int* __r
     if (lane == 0) acc[s] += t;
   }
   if (threadIdx.x == 0) *counter = 0;  // ready for the next launch or graph replay
+}
+
+__global__ void __launch_bounds__(kSegThreads)
+seg_eval_metrics_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                        const int* __restrict__ n_valid, double* __restrict__ acc,
+                        double* __restrict__ partial, unsigned int* __restrict__ counter,
+                        int images, long long ppi, long long chunk, int V) {
+  seg_eval_metrics_body<false>(logits, labels, n_valid, acc, partial, counter, images, ppi, chunk,
+                               V, SegLossOpts{});
+}
+
+__global__ void __launch_bounds__(kSegThreads)
+seg_eval_metrics_opt_kernel(const __nv_bfloat16* __restrict__ logits,
+                            const int* __restrict__ labels, const int* __restrict__ n_valid,
+                            double* __restrict__ acc, double* __restrict__ partial,
+                            unsigned int* __restrict__ counter, int images, long long ppi,
+                            long long chunk, int V, const SegLossOpts o) {
+  seg_eval_metrics_body<true>(logits, labels, n_valid, acc, partial, counter, images, ppi, chunk,
+                              V, o);
 }
 
 constexpr int kPredThreads = 128;
@@ -456,6 +485,131 @@ seg_eval_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __rest
   if (threadIdx.x == 0) *counter = 0;  // ready for the next launch or graph replay
 }
 
+// seg_eval_wide_kernel with the loss options (seg_wide.cuh), as seg_score: an ignored pixel is
+// neither counted nor invalid and has no bin, the loss term is weighted by w[y].  A copy of
+// seg_eval_wide_kernel rather than a shared inline body: inlining a common body changes the
+// default instances' register allocation.  One CTA per SM is the register budget: without it
+// ptxas fits G = 32 into 32 registers and spills.
+template <int G>
+__global__ void __launch_bounds__(kSegThreads, 1)
+seg_eval_wide_opt_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                         const int* __restrict__ n_valid, double* __restrict__ acc,
+                         double* __restrict__ partial, unsigned long long* __restrict__ table,
+                         unsigned int* __restrict__ counter, int images, long long ppi,
+                         long long chunk, int VP, int V, int smem_table, const SegLossOpts o) {
+  extern __shared__ unsigned int tab[];
+  __shared__ int wint[3][kSegWarps];
+  __shared__ double wloss[kSegWarps];
+  __shared__ unsigned int is_last;
+  constexpr int kPix = 32 / G;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, sub = lane & (G - 1), c0 = sub * 8;
+  const int cells = V * V;
+  if (smem_table)
+    for (int i = threadIdx.x; i < cells; i += kSegThreads) tab[i] = 0u;
+  __syncthreads();
+  int n = *n_valid;
+  n = n < 0 ? 0 : (n > images ? images : n);
+  const long long limit = static_cast<long long>(n) * ppi;
+  const long long lo = static_cast<long long>(blockIdx.x) * chunk;
+  const long long hi = lo + chunk < limit ? lo + chunk : limit;
+  int cnt = 0, hit = 0, bad = 0;
+  double loss = 0.0;
+  for (long long base = lo + warp * kPix; base < hi; base += kSegWarps * kPix) {
+    const long long p = base + lane / G;
+    const bool in = p < hi;
+    float l[8];
+    if (in && c0 < VP) {
+      seg_unpack8(__ldcs(reinterpret_cast<const uint4*>(logits + p * VP + c0)), l);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) l[k] = 0.f;
+    }
+    const int y = in ? __ldcs(labels + p) : -1;
+    float mx;
+    const int am = seg_argmax_wide<G>(l, c0, V, mx);
+    float se = 0.f, ly = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      if (c0 + k < V) se += __expf(l[k] - mx);
+      if (c0 + k < V && c0 + k == y) ly = l[k];
+    }
+    se = seg_group_sum<G>(se);
+    ly = seg_group_sum<G>(ly);
+    int bin = -1;
+    if (in && sub == 0 && !seg_ignored(o, y)) {
+      if (y < 0 || y >= V) {
+        bad += 1;
+      } else {
+        cnt += 1;
+        hit += am == y ? 1 : 0;
+        const float w = seg_weight(o, y, V);
+        if (w != 0.f) loss += static_cast<double>(w) * static_cast<double>(__logf(se) + mx - ly);
+        bin = y * V + am;
+      }
+    }
+    const unsigned same = __match_any_sync(0xffffffffu, bin);
+    if (bin >= 0 && lane == __ffs(same) - 1) {
+      if (smem_table) atomicAdd(&tab[bin], static_cast<unsigned>(__popc(same)));
+      else atomicAdd(&table[bin], static_cast<unsigned long long>(__popc(same)));
+    }
+  }
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) {
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    hit += __shfl_xor_sync(0xffffffffu, hit, o);
+    bad += __shfl_xor_sync(0xffffffffu, bad, o);
+    loss += __shfl_xor_sync(0xffffffffu, loss, o);
+  }
+  if (lane == 0) {
+    wint[0][warp] = cnt, wint[1][warp] = hit, wint[2][warp] = bad;
+    wloss[warp] = loss;
+  }
+  __syncthreads();
+  const int grid = gridDim.x;
+  if (threadIdx.x == 0) {
+    long long c = 0, h = 0, b = 0;
+    double l = 0.0;
+    for (int w = 0; w < kSegWarps; ++w)
+      c += wint[0][w], h += wint[1][w], b += wint[2][w], l += wloss[w];
+    partial[static_cast<long long>(kSegEvalCount) * grid + blockIdx.x] = static_cast<double>(c);
+    partial[static_cast<long long>(kSegEvalCorrect) * grid + blockIdx.x] = static_cast<double>(h);
+    partial[static_cast<long long>(kSegEvalInvalid) * grid + blockIdx.x] = static_cast<double>(b);
+    partial[static_cast<long long>(kSegEvalLoss) * grid + blockIdx.x] = l;
+  }
+  if (smem_table) {
+    for (int i = threadIdx.x; i < cells; i += kSegThreads) {
+      const unsigned c = tab[i];
+      if (c) atomicAdd(&table[i], static_cast<unsigned long long>(c));
+    }
+  }
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) is_last = (atomicAdd(counter, 1u) == gridDim.x - 1) ? 1u : 0u;
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  if (warp < kSegWideScalars) {   // the four scalar slots, one warp each
+    const double* row = partial + static_cast<long long>(warp) * grid;
+    double t = 0.0;
+#pragma unroll
+    for (int k = 0; k < (kSegMaxGrid + 31) / 32; ++k) {
+      const int b = lane + 32 * k;
+      if (b < grid) t += __ldcg(row + b);
+    }
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if (lane == 0) acc[warp] += t;
+  }
+  for (int i = threadIdx.x; i < cells; i += kSegThreads) {
+    const unsigned long long c = __ldcg(table + i);
+    if (c) {
+      acc[kSegWideConfusion + i] += static_cast<double>(c);
+      table[i] = 0ull;
+    }
+  }
+  if (threadIdx.x == 0) *counter = 0;  // ready for the next launch or graph replay
+}
+
 // seg_predict_kernel for bf16 logits [P, VP], V > 8: warp tiles of 32 / G pixels over a
 // grid-stride loop; the group's first lane writes the mask byte, every lane its channels < V of
 // the compact fp32 logits.
@@ -497,9 +651,12 @@ long long seg_eval_wide_scratch(long long pixels, int V) {
          static_cast<long long>(V) * V;
 }
 
-cudaError_t seg_eval_metrics_wide(const void* logits, const int* labels, const int* n_valid,
-                                  double* acc, double* scratch, unsigned int* counter, int images,
-                                  long long ppi, int VP, int V, cudaStream_t s) {
+// seg_eval_metrics_wide (kOpt false) and its optioned instances: one launch geometry
+template <bool kOpt>
+cudaError_t launch_seg_eval_wide(const void* logits, const int* labels, const int* n_valid,
+                                 double* acc, double* scratch, unsigned int* counter, int images,
+                                 long long ppi, int VP, int V, const SegLossOpts& o,
+                                 cudaStream_t s) {
   const long long pixels = static_cast<long long>(images) * ppi;
   const int grid = seg_eval_grid(pixels);
   const long long chunk =
@@ -513,12 +670,22 @@ cudaError_t seg_eval_metrics_wide(const void* logits, const int* labels, const i
   const auto* l = static_cast<const __nv_bfloat16*>(logits);
 #define TFOS_SEG_EVAL_WIDE(g)                                                                   \
   case g: {                                                                                     \
-    static const cudaError_t attr = cudaFuncSetAttribute(                                       \
-        seg_eval_wide_kernel<g>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSegWideSmemTable); \
+    static const cudaError_t attr =                                                             \
+        kOpt ? cudaFuncSetAttribute(seg_eval_wide_opt_kernel<g>,                                \
+                                    cudaFuncAttributeMaxDynamicSharedMemorySize,                \
+                                    kSegWideSmemTable)                                          \
+             : cudaFuncSetAttribute(seg_eval_wide_kernel<g>,                                    \
+                                    cudaFuncAttributeMaxDynamicSharedMemorySize,                \
+                                    kSegWideSmemTable);                                         \
     if (attr != cudaSuccess) return attr;                                                       \
-    seg_eval_wide_kernel<g><<<grid, kSegThreads, smem, s>>>(l, labels, n_valid, acc, partial,   \
-                                                            table, counter, images, ppi, chunk, \
-                                                            VP, V, smem_table);                 \
+    if constexpr (kOpt)                                                                         \
+      seg_eval_wide_opt_kernel<g><<<grid, kSegThreads, smem, s>>>(                              \
+          l, labels, n_valid, acc, partial, table, counter, images, ppi, chunk, VP, V,          \
+          smem_table, o);                                                                       \
+    else                                                                                        \
+      seg_eval_wide_kernel<g><<<grid, kSegThreads, smem, s>>>(l, labels, n_valid, acc, partial, \
+                                                              table, counter, images, ppi,      \
+                                                              chunk, VP, V, smem_table);        \
     break;                                                                                      \
   }
   switch (seg_wide_group(VP)) {
@@ -531,6 +698,13 @@ cudaError_t seg_eval_metrics_wide(const void* logits, const int* labels, const i
   }
 #undef TFOS_SEG_EVAL_WIDE
   return cudaGetLastError();
+}
+
+cudaError_t seg_eval_metrics_wide(const void* logits, const int* labels, const int* n_valid,
+                                  double* acc, double* scratch, unsigned int* counter, int images,
+                                  long long ppi, int VP, int V, cudaStream_t s) {
+  return launch_seg_eval_wide<false>(logits, labels, n_valid, acc, scratch, counter, images, ppi,
+                                     VP, V, SegLossOpts{}, s);
 }
 
 cudaError_t seg_predict_wide(const void* logits, uint8_t* mask, float* out, long long pixels,
@@ -572,16 +746,33 @@ int seg_eval_grid(long long pixels) {
   return blocks < 1 ? 1 : static_cast<int>(blocks);
 }
 
+// a multiple of one pass: only the CTA at the end of the valid range has a partial pass
+static long long seg_eval_chunk(long long pixels, int grid) {
+  return ((pixels + grid - 1) / grid + kSegStep - 1) / kSegStep * kSegStep;
+}
+
 cudaError_t seg_eval_metrics(const void* logits, const int* labels, const int* n_valid,
                              double* acc, double* partial, unsigned int* counter, int images,
                              long long ppi, int V, cudaStream_t s) {
   const long long pixels = static_cast<long long>(images) * ppi;
   const int grid = seg_eval_grid(pixels);
-  // a multiple of one pass: only the CTA at the end of the valid range has a partial pass
-  const long long chunk = ((pixels + grid - 1) / grid + kSegStep - 1) / kSegStep * kSegStep;
   seg_eval_metrics_kernel<<<grid, kSegThreads, 0, s>>>(
       static_cast<const __nv_bfloat16*>(logits), labels, n_valid, acc, partial, counter, images,
-      ppi, chunk, V);
+      ppi, seg_eval_chunk(pixels, grid), V);
+  return cudaGetLastError();
+}
+
+cudaError_t seg_eval_metrics_opt(const void* logits, const int* labels, const int* n_valid,
+                                 double* acc, double* scratch, unsigned int* counter, int images,
+                                 long long ppi, int VP, int V, SegLossOpts o, cudaStream_t s) {
+  if (VP != 8)
+    return launch_seg_eval_wide<true>(logits, labels, n_valid, acc, scratch, counter, images, ppi,
+                                      VP, V, o, s);
+  const long long pixels = static_cast<long long>(images) * ppi;
+  const int grid = seg_eval_grid(pixels);
+  seg_eval_metrics_opt_kernel<<<grid, kSegThreads, 0, s>>>(
+      static_cast<const __nv_bfloat16*>(logits), labels, n_valid, acc, scratch, counter, images,
+      ppi, seg_eval_chunk(pixels, grid), V, o);
   return cudaGetLastError();
 }
 

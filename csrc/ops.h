@@ -76,6 +76,31 @@ cudaError_t pixel_xent(const void* logits, const int* labels, void* dlogits, flo
 cudaError_t pixel_xent_wide(const void* logits, const int* labels, void* dlogits, float* loss_sum,
                             float* correct_sum, long long P, int VP, int V, float scale,
                             cudaStream_t s);
+// Loss options of the segmentation U-Net (ignore_index, class weights), read by the optioned
+// instances of seg_label_norm, pixel_xent and seg_eval_metrics.  A pixel whose label equals
+// `ignore` (when has_ignore) takes no part; w[y] = weights[y] for y in [0, V) (1 when weights is
+// null), 1 for any other label.  norm: [sum w, |S|, inv] as seg_label_norm writes it (fp64;
+// inv = 1 / sum w rounded to fp32, 0 when sum w = 0).
+struct SegLossOpts {
+  int ignore;
+  int has_ignore;
+  const float* weights;
+  const double* norm;
+};
+// seg_label_norm: norm = [sum over the non-ignored labels of w[y], their count |S|, inv] from one
+// pass over int32 labels [P].  scratch: seg_label_norm_scratch(V) zeroed uint64 words (per-class
+// counts [V + 1], the last for labels outside [0, V), then the CTA ticket), left at zero, so it
+// replays in a CUDA graph with no reset.  Integer counts and a fixed-order fp64 sum: bitwise
+// reproducible.
+inline long long seg_label_norm_scratch(int V) { return V + 2; }
+cudaError_t seg_label_norm(const int* labels, long long P, int V, SegLossOpts o, double* norm,
+                           unsigned long long* scratch, cudaStream_t s);
+// pixel_xent / pixel_xent_wide with loss options: loss_sum += sum over S of w[y] l_p * inv,
+// dlogits = w[y] (p - onehot) * inv on S, exactly 0 on ignored pixels, on pixels with
+// w[y] * inv = 0 and in channels >= V; correct_sum += the hits on S.  VP = 8: the 8-channel kernel.
+cudaError_t pixel_xent_opt(const void* logits, const int* labels, void* dlogits, float* loss_sum,
+                           float* correct_sum, long long P, int VP, int V, SegLossOpts o,
+                           cudaStream_t s);
 
 // ---- optim_comm.cu
 constexpr int kMaxRanks = 8;
@@ -274,6 +299,12 @@ long long seg_eval_wide_scratch(long long pixels, int V);
 cudaError_t seg_eval_metrics_wide(const void* logits, const int* labels, const int* n_valid,
                                   double* acc, double* scratch, unsigned int* counter, int images,
                                   long long ppi, int VP, int V, cudaStream_t s);
+// seg_eval_metrics / seg_eval_metrics_wide with loss options (o.norm unused): ignored pixels
+// leave count, correct, loss and the confusion matrix and are never invalid; the loss slot adds
+// w[y] * l_p.  VP = 8: the 8-channel kernel and layout.
+cudaError_t seg_eval_metrics_opt(const void* logits, const int* labels, const int* n_valid,
+                                 double* acc, double* scratch, unsigned int* counter, int images,
+                                 long long ppi, int VP, int V, SegLossOpts o, cudaStream_t s);
 // seg_predict_wide: mask[p] = the class (seg_wide.cuh) and, when out is not null,
 // out[p * V + j] = the fp32 value of channel j < V.  One pass; any pixel count.
 cudaError_t seg_predict_wide(const void* logits, uint8_t* mask, float* out, long long pixels,

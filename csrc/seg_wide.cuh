@@ -11,11 +11,21 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "ops.h"
 #include "ptx.cuh"
 
 namespace tfos {
 
 constexpr int kSegWideNone = 0x7fffffff;  // "no channel yet" in the arg-max scan
+
+// The loss options (ops.h SegLossOpts), shared by the training, pre-pass and evaluation kernels
+// so that all three leave out the same pixels and weigh them alike.
+__device__ __forceinline__ bool seg_ignored(const SegLossOpts& o, const int y) {
+  return o.has_ignore && y == o.ignore;
+}
+__device__ __forceinline__ float seg_weight(const SegLossOpts& o, const int y, const int V) {
+  return o.weights != nullptr && y >= 0 && y < V ? __ldg(o.weights + y) : 1.f;
+}
 
 // G for VP padded channels: the power of two >= VP / 8 (2 .. 32)
 inline int seg_wide_group(int VP) {

@@ -3,6 +3,9 @@ segmentation.py - the notebook-derived single-node script; model at segmentation
 frozen MobileNetV2 encoder, four transposed-conv up-blocks, per-pixel softmax cross-entropy, Adam.
 ``--classes V`` (1..256, default 3) sets the class count; the synthetic labels are the 3-class
 trimap, or the red channel in V bands (models/unet.synthetic_labels).
+``--ignore_index k`` leaves pixels labelled k out of the loss and the evaluation (void pixels: 255
+in PASCAL VOC, Cityscapes and COCO-Stuff); ``--class_weights w0,w1,...`` weighs each class's
+pixels in the cross-entropy (one weight per class).
 ``--encoder_trainable_from k`` fine-tunes the encoder's blocks block_k..block_16 as well (0: the
 stem and every block), e.g. after a frozen run, resuming from its checkpoint.
 Checkpoints every epoch (the reference's ModelCheckpoint callback) and evaluates every epoch on
@@ -29,6 +32,10 @@ def define_flags():
   p.add_argument("--learning_rate", type=float, default=1e-3)
   p.add_argument("--classes", type=int, default=3,
                  help="segmentation classes, 1..256 (labels: the trimap at 3, else red-channel bands)")
+  p.add_argument("--ignore_index", type=int, default=None,
+                 help="label value left out of the loss and the evaluation, e.g. 255 (default: none)")
+  p.add_argument("--class_weights", type=class_weights, default=None,
+                 help="comma-separated cross-entropy weight per class (default: unweighted)")
   p.add_argument("--eval_steps", type=int, default=1,
                  help="held-out batches per rank evaluated after every epoch (0: no evaluation)")
   p.add_argument("--model_dir", default=None)
@@ -39,11 +46,16 @@ def define_flags():
   return p
 
 
+def class_weights(text):
+  """--class_weights: comma-separated numbers, one per class."""
+  return [float(v) for v in text.split(",")]
+
+
 def trainer_kwargs(args):
-  """Keyword arguments the trainer gets from the flags beyond the common ones: none unless the
-  encoder is fine-tuned."""
-  k = getattr(args, "encoder_trainable_from", None)
-  return {} if k is None else {"encoder_trainable_from": k}
+  """Keyword arguments the trainer gets from the flags beyond the common ones: only those of the
+  options that are set (encoder fine-tuning, ignore_index, class_weights)."""
+  names = ("encoder_trainable_from", "ignore_index", "class_weights")
+  return {n: getattr(args, n) for n in names if getattr(args, n, None) is not None}
 
 
 def resume(net, state, fine_tuning):
@@ -88,7 +100,7 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
   if args.model_dir:
     start, state = checkpoint.load(args.model_dir)
     if state is not None:
-      resume(net, state, bool(extra))
+      resume(net, state, "encoder_trainable_from" in extra)
       print("resumed from step", start)
   batches = [net.synthetic_batch(seed=1000 * rank + i)[0] for i in range(4)]
   # this rank's shard of the held-out set: batch i of rank r is held-out batch i * world + r

@@ -6,6 +6,9 @@ are provided here: ``--input_mode tf`` (each worker synthesises / reads its own 
 ``--input_mode spark`` (BASELINE.json config #4: the images travel RDD -> shared-memory pinned
 ring -> ``cudaMemcpyAsync`` on a copy stream -> device, through ``TFNode.DataFeed``).
 
+``--ignore_index k`` and ``--class_weights w0,w1,...`` are UNetTrainer's loss options (void pixels
+left out; per-class cross-entropy weights).
+
 Held-out evaluation (the reference's ``validation_data``): ``--eval_steps N`` scores N synthetic
 batches per rank every ``--eval_every K`` steps and after the last step, in either input mode
 (``UNetTrainer.evaluate``: loss, pixel accuracy and mean IoU summed over all ranks).
@@ -49,10 +52,12 @@ def main_fun(args, ctx):
   torch.cuda.set_device(0)
   comm = ctx.gradient_comm() if ctx.world_size > 1 else None   # one host: P2P/NVLS kernels; several: NCCL
   B = args.batch_size
-  k = getattr(args, "encoder_trainable_from", None)   # None: frozen encoder, as the reference
+  # None: frozen encoder (as the reference), no ignored label, unweighted loss
+  extra = {n: getattr(args, n) for n in ("encoder_trainable_from", "ignore_index", "class_weights")
+           if getattr(args, n, None) is not None}
   V = getattr(args, "classes", 3)
   net = unet.UNetTrainer(batch=B, image=IMG, classes=V, device="cuda:0", lr=args.learning_rate,
-                         comm=comm, **({} if k is None else {"encoder_trainable_from": k}))
+                         comm=comm, **extra)
   if comm is not None:
     comm.broadcast("weights", root=0)
     comm.broadcast("aux32", root=0)
@@ -167,6 +172,11 @@ if __name__ == "__main__":
   parser.add_argument("--learning_rate", type=float, default=1e-3)
   parser.add_argument("--classes", type=int, default=3,
                       help="segmentation classes, 1..256 (labels: the trimap at 3, else red-channel bands)")
+  parser.add_argument("--ignore_index", type=int, default=None,
+                      help="label value left out of the loss and the evaluation, e.g. 255 (default: none)")
+  parser.add_argument("--class_weights", type=lambda s: [float(v) for v in s.split(",")],
+                      default=None,
+                      help="comma-separated cross-entropy weight per class (default: unweighted)")
   parser.add_argument("--input_mode", default="tf", choices=["tf", "spark"])
   parser.add_argument("--num_examples", type=int, default=2048)
   parser.add_argument("--eval_steps", type=int, default=0,

@@ -343,6 +343,39 @@ def _classes(v):
   return int(v)
 
 
+def _ignore_index(v):
+  """Validated ``ignore_index``: None, or an int in the int32 range (labels are int32)."""
+  if v is None:
+    return None
+  if isinstance(v, bool) or not isinstance(v, numbers.Integral):
+    raise ValueError("ignore_index must be None or an int, not {!r}".format(v))
+  if not -2 ** 31 <= v < 2 ** 31:
+    raise ValueError("ignore_index must fit in int32, got {}".format(v))
+  return int(v)
+
+
+def _class_weights(v, classes):
+  """Validated ``class_weights``: None, or a tuple of ``classes`` finite, non-negative, not all
+  zero weights, rounded to fp32 as the kernels read them."""
+  if v is None:
+    return None
+  if isinstance(v, (torch.Tensor, np.ndarray)):
+    v = v.tolist()
+  if isinstance(v, (str, bytes, bool, numbers.Number)) or not hasattr(v, "__len__"):
+    raise ValueError("class_weights must be None or a sequence of {} numbers, not {!r}".format(
+        classes, v))
+  if len(v) != classes:
+    raise ValueError("class_weights needs one weight per class ({}), got {}".format(classes, len(v)))
+  if any(isinstance(w, bool) or not isinstance(w, numbers.Real) for w in v):
+    raise ValueError("class_weights must be real numbers, got {!r}".format(v))
+  w = tuple(float(np.float32(x)) for x in v)
+  if not all(math.isfinite(x) and x >= 0 for x in w):
+    raise ValueError("class_weights must be finite and non-negative, got {!r}".format(v))
+  if not any(w):
+    raise ValueError("class_weights are all zero")
+  return w
+
+
 def padded_classes(classes):
   """Channels of the logits for ``classes`` labels: 8 up to 8 classes (one 16-byte load per
   pixel), else the next multiple of 8 (the wide kernels, csrc/seg_wide.cuh)."""
@@ -374,14 +407,36 @@ class UNetTrainer(object):
   the Keras blocks block_k .. block_16.  Their folded (batch norm in the filter) filters and biases
   become parameters ``encoder.stem.{w,b}`` / ``encoder.block{b}.{expand,dw,project}.{w,b}`` of the
   store, starting from exactly the frozen network of the same seed; the optimizer and gradient
-  all-reduce cover them like every other parameter."""
+  all-reduce cover them like every other parameter.
+
+  ``ignore_index`` and ``class_weights`` are the loss options of
+  ``F.cross_entropy(logits, y, weight=class_weights, ignore_index=ignore_index)``, for training and
+  evaluation (also of a ``training=False`` trainer's ``evaluate``).  ``ignore_index``: None or an
+  int32 value; a pixel whose label equals it takes no part in the loss, the gradient, the hit
+  count ``correct`` or any evaluation total (void pixels, 255 in PASCAL VOC, Cityscapes and
+  COCO-Stuff).  It may lie inside [0, classes), as in PyTorch: that class is then never scored.
+  uint8 masks only carry 0..255, so a larger or negative value never matches one.
+  ``class_weights``: None or ``classes`` finite, non-negative weights, not all zero (rounded to
+  fp32).  With S the non-ignored pixels of a step and w[y] the weight of label y (1 without
+  weights, and for a label outside [0, classes) that is not ignored):
+  loss = sum_S w[y] l_p / sum_S w[y] and dlogits_p = w[y] (softmax_p - onehot_p) / sum_S w[y],
+  exactly 0 for ignored pixels.  When sum_S w[y] = 0 (every pixel ignored, or only zero-weight
+  classes present) the loss and the gradient are 0, where PyTorch gives NaN.  The denominator is
+  computed on the device each step (``loss_norm``), so a captured step uses its own batch's.
+  Under data parallelism each rank normalises by its own denominator and the gradient all-reduce
+  averages, as DDP does with a mean-reduced CrossEntropyLoss.  With neither option the step
+  launches exactly the kernels it did without them.  ``loss_norm`` (fp64 [3], training only) holds
+  the last step's [sum_S w[y], |S|, 1 / sum_S w[y]]: loss_sum is the mean loss and
+  correct / loss_norm[1] the pixel accuracy, without a host sync."""
 
   UP = (512, 256, 128, 64)
 
   def __init__(self, batch=64, image=128, classes=3, device="cuda:0", lr=1e-3, comm=None, seed=1234,
-               training=True, encoder_trainable_from=None):
+               training=True, encoder_trainable_from=None, ignore_index=None, class_weights=None):
     classes = _classes(classes)
     k = self.encoder_trainable_from = _trainable_from(encoder_trainable_from, training)
+    self.ignore_index = _ignore_index(ignore_index)
+    self.class_weights = _class_weights(class_weights, classes)
     self.VP = VP = padded_classes(classes)
     self.device = dev = torch.device(device)
     self.B, self.image, self.classes = batch, image, classes
@@ -437,6 +492,21 @@ class UNetTrainer(object):
       self.encoder.build_backward(st, self.g_top, skip_grads)
     self.loss_sum = torch.zeros(1, dtype=torch.float32, device=dev)
     self.correct = torch.zeros(1, dtype=torch.float32, device=dev)
+    # the loss options' device state: weights [VP] (zero in the padding channels), the
+    # pre-pass's scratch and its result; without options loss_norm is the constant denominator
+    self.weights = None
+    if self.class_weights is not None:
+      self.weights = torch.zeros(VP, dtype=torch.float32, device=dev)
+      self.weights[:classes] = torch.tensor(self.class_weights, dtype=torch.float32)
+    self.loss_opts = self.ignore_index is not None or self.class_weights is not None
+    self.loss_norm = self._norm_scratch = None
+    if tr:
+      npix = self.labels.numel()
+      self.loss_norm = torch.tensor([npix, npix, float(np.float32(1.0 / npix))],
+                                    dtype=torch.float64, device=dev)
+      if self.loss_opts:
+        self._norm_scratch = torch.zeros(ops.C().seg_label_norm_scratch(classes),
+                                         dtype=torch.int64, device=dev)
     self.in_u8 = _buf((B, image, image, 3), dev, torch.uint8)
     if tr:
       from ..parallel.fused_optim import FusedOptimizer
@@ -483,8 +553,14 @@ class UNetTrainer(object):
     self.loss_sum.zero_()
     self.correct.zero_()
     npix = self.labels.numel()
-    K.pixel_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct, self.classes,
-                 1.0 / npix)
+    if self.loss_opts:   # the denominator sum_S w[y] of this batch's labels, on the device
+      K.seg_label_norm(self.labels, self.loss_norm, self._norm_scratch, self.classes,
+                       self.ignore_index, self.weights)
+      K.pixel_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
+                   self.classes, 1.0 / npix, self.ignore_index, self.weights, self.loss_norm)
+    else:
+      K.pixel_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
+                   self.classes, 1.0 / npix)
     self.optim.zero_grads()
     self.p_last_wgrad.run()
     K.colsum(self.dlogits, self.store.g(self.s_last_b))
@@ -604,7 +680,9 @@ class UNetTrainer(object):
 
   def eval_end(self):
     """Totals summed over all ranks (identical on every rank), see seg_eval_result.  Raises
-    ValueError on every rank when any rank saw a mask value outside [0, classes)."""
+    ValueError on every rank when any rank saw a mask value outside [0, classes) that is not
+    ``ignore_index``.  With ``ignore_index`` the result also has ``"ignored"``: the pixels left
+    out.  With ``class_weights`` the loss is the weighted mean."""
     return self._eval_state().end()
 
   def evaluate(self, batches):
@@ -635,13 +713,15 @@ def seg_eval_layout(classes):
   return 4, 5, classes, 5 + classes * classes
 
 
-def seg_eval_result(totals, classes):
+def seg_eval_result(totals, classes, class_weights=None):
   """Host metrics from the summed accumulator ``totals`` (seg_eval_layout(classes) floats):
   {"count": scored pixels, "images", "loss", "accuracy", "mean_iou", "iou": [classes values]}.
   IoU of class c = cm[c, c] / (row_c + col_c - cm[c, c]) of the confusion matrix cm[label, pred];
   a class with an empty union has IoU NaN and is left out of mean_iou (NaN when every class is).
-  loss and accuracy are means over the scored pixels (NaN when there are none).  Raises
-  ValueError when any mask value was outside [0, classes)."""
+  loss and accuracy are means over the scored pixels (NaN when there are none).  With
+  ``class_weights`` (``classes`` values) the loss slot holds sum w[y] l_p and the loss is its
+  weighted mean, divided by sum_c w_c row_c (NaN when that is 0); IoU and accuracy stay
+  unweighted.  Raises ValueError when any mask value was outside [0, classes)."""
   images, conf, ld, _ = seg_eval_layout(classes)
   if classes <= 8:
     h = [float(v) for v in totals]
@@ -665,7 +745,12 @@ def seg_eval_result(totals, classes):
   count = int(h[SEG_COUNT])
   seen = [v for v in iou if v == v]
   mean = (lambda v: v / count) if count else (lambda v: float("nan"))
-  return {"count": count, "images": int(h[images]), "loss": mean(h[SEG_LOSS]),
+  loss = mean(h[SEG_LOSS])
+  if class_weights is not None:
+    rows = np.asarray(totals, dtype=np.float64)[conf:conf + ld * classes].reshape(classes, ld)
+    wsum = float(np.dot(np.asarray(class_weights, dtype=np.float64), rows[:, :classes].sum(axis=1)))
+    loss = h[SEG_LOSS] / wsum if wsum > 0 else float("nan")
+  return {"count": count, "images": int(h[images]), "loss": loss,
           "accuracy": mean(h[SEG_CORRECT]),
           "mean_iou": sum(seen) / len(seen) if seen else float("nan"), "iou": iou}
 
@@ -723,9 +808,14 @@ class _SegEvaluator(object):
       comm.broadcast("seg_eval_running", 0)
 
   def _run(self):
-    self.net._forward(False, self.u8, self.bn)
-    ops.K.seg_eval_metrics(self.net.logits, self.labels, self.n_valid, self.acc, self.partial,
-                           self.counter, self.V)
+    net = self.net
+    net._forward(False, self.u8, self.bn)
+    if net.loss_opts:
+      ops.K.seg_eval_metrics(net.logits, self.labels, self.n_valid, self.acc, self.partial,
+                             self.counter, self.V, net.ignore_index, net.weights)
+    else:
+      ops.K.seg_eval_metrics(net.logits, self.labels, self.n_valid, self.acc, self.partial,
+                             self.counter, self.V)
 
   def step(self, images_u8, masks):
     n = len(images_u8)
@@ -769,7 +859,11 @@ class _SegEvaluator(object):
 
   def end(self):
     self.acc[self.images_slot].fill_(self.images)
-    return seg_eval_result(self.rank_sum(self.acc), self.V)
+    net = self.net
+    res = seg_eval_result(self.rank_sum(self.acc), self.V, net.class_weights)
+    if net.ignore_index is not None:   # every pixel of the images is scored, invalid or ignored
+      res["ignored"] = res["images"] * net.image * net.image - res["count"]
+    return res
 
 
 class ServedUNet(serving.Replica):
