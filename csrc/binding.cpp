@@ -569,33 +569,15 @@ void seg_eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& 
   TORCH_CHECK(partial.numel() >= seg_eval_scratch(pixels, V),
               "seg_eval_metrics: partial needs seg_eval_scratch(pixels, V) doubles");
   TORCH_CHECK(counter.numel() >= 1, "seg_eval_metrics: counter");
-  if (ignore_index.has_value() || (weights.has_value() && weights->defined())) {
-    for (const Tensor& t : {labels, n_valid, acc, partial, counter})
-      TORCH_CHECK(t.device() == logits.device(), "seg_eval_metrics: tensors on different devices");
-    const tfos::SegLossOpts o = seg_loss_opts(logits, ignore_index, weights, V, "seg_eval_metrics");
-    check(tfos::seg_eval_metrics_opt(
-              logits.data_ptr(), labels.data_ptr<int>(), n_valid.data_ptr<int>(),
-              acc.data_ptr<double>(), partial.data_ptr<double>(),
-              reinterpret_cast<unsigned int*>(counter.data_ptr<int>()), static_cast<int>(images),
-              pixels / images, static_cast<int>(VP), V, o, cur_stream()),
-          "seg_eval_metrics");
-    return;
-  }
-  if (VP > 8) {
-    for (const Tensor& t : {labels, n_valid, acc, partial, counter})
-      TORCH_CHECK(t.device() == logits.device(), "seg_eval_metrics: tensors on different devices");
-    check(tfos::seg_eval_metrics_wide(
-              logits.data_ptr(), labels.data_ptr<int>(), n_valid.data_ptr<int>(),
-              acc.data_ptr<double>(), partial.data_ptr<double>(),
-              reinterpret_cast<unsigned int*>(counter.data_ptr<int>()), static_cast<int>(images),
-              pixels / images, static_cast<int>(VP), V, cur_stream()),
-          "seg_eval_metrics");
-    return;
-  }
-  check(tfos::seg_eval_metrics(logits.data_ptr(), labels.data_ptr<int>(), n_valid.data_ptr<int>(),
-                               acc.data_ptr<double>(), partial.data_ptr<double>(),
-                               reinterpret_cast<unsigned int*>(counter.data_ptr<int>()),
-                               static_cast<int>(images), pixels / images, V, cur_stream()),
+  for (const Tensor& t : {labels, n_valid, acc, partial, counter})
+    TORCH_CHECK(t.device() == logits.device(), "seg_eval_metrics: tensors on different devices");
+  const tfos::SegLossOpts o = seg_loss_opts(logits, ignore_index, weights, V, "seg_eval_metrics");
+  check(tfos::seg_eval_metrics(
+            logits.data_ptr(), labels.data_ptr<int>(), n_valid.data_ptr<int>(),
+            acc.data_ptr<double>(), partial.data_ptr<double>(),
+            reinterpret_cast<unsigned int*>(counter.data_ptr<int>()), static_cast<int>(images),
+            pixels / images, static_cast<int>(VP), V, o.has_ignore || o.weights ? &o : nullptr,
+            cur_stream()),
         "seg_eval_metrics");
 }
 void seg_predict(const Tensor& logits, Tensor mask, c10::optional<Tensor> out, int V) {
@@ -616,13 +598,8 @@ void seg_predict(const Tensor& logits, Tensor mask, c10::optional<Tensor> out, i
                 "seg_predict: out must be 16-byte aligned");
     o = out->data_ptr<float>();
   }
-  if (VP > 8) {
-    check(tfos::seg_predict_wide(logits.data_ptr(), mask.data_ptr<uint8_t>(), o, pixels,
-                                 static_cast<int>(VP), V, cur_stream()),
-          "seg_predict");
-    return;
-  }
-  check(tfos::seg_predict(logits.data_ptr(), mask.data_ptr<uint8_t>(), o, pixels, V, cur_stream()),
+  check(tfos::seg_predict(logits.data_ptr(), mask.data_ptr<uint8_t>(), o, pixels,
+                          static_cast<int>(VP), V, cur_stream()),
         "seg_predict");
 }
 void cast_f32_bf16(const Tensor& in, Tensor out) {
@@ -731,51 +708,29 @@ void pixel_xent(const Tensor& logits, const Tensor& labels, c10::optional<Tensor
                 c10::optional<Tensor> norm) {
   need(logits, torch::kBFloat16, "logits");
   need(labels, torch::kInt32, "labels");
-  const bool opt = ignore_index.has_value() || (weights.has_value() && weights->defined()) ||
-                   (norm.has_value() && norm->defined());
-  if (opt) {   // the loss options: scale is inv from norm (seg_label_norm of these labels)
-    TORCH_CHECK(seg_channels_match(logits, V), "pixel_xent: logits [B, ..., VP] with V in [1, 256] and "
-                "VP = 8 for V <= 8, ceil(V / 8) * 8 above");
+  TORCH_CHECK(seg_channels_match(logits, V), "pixel_xent: logits [B, ..., VP] with V in [1, 256] and "
+              "VP = 8 for V <= 8, ceil(V / 8) * 8 above");
+  const int64_t VP = logits.size(-1);
+  const int64_t P = logits.numel() / VP;
+  TORCH_CHECK(labels.numel() == P, "pixel_xent: one label per pixel");
+  TORCH_CHECK(labels.device() == logits.device(), "pixel_xent: tensors on different devices");
+  const void* d = optptr(dlogits);
+  if (d != nullptr)
+    TORCH_CHECK(dlogits->sizes() == logits.sizes() && dlogits->scalar_type() == torch::kBFloat16,
+                "pixel_xent: dlogits must be bf16 with the shape of logits");
+  // the loss options: scale is inv from norm (seg_label_norm of these labels)
+  tfos::SegLossOpts o = seg_loss_opts(logits, ignore_index, weights, V, "pixel_xent");
+  const bool opt = o.has_ignore || o.weights || (norm.has_value() && norm->defined());
+  if (opt) {
     TORCH_CHECK(norm.has_value() && norm->defined(), "pixel_xent: the loss options need norm");
     need(*norm, torch::kFloat64, "norm");
     TORCH_CHECK(norm->numel() >= 3, "pixel_xent: norm needs 3 slots");
-    const int64_t VP = logits.size(-1);
-    const int64_t P = logits.numel() / VP;
-    TORCH_CHECK(labels.numel() == P, "pixel_xent: one label per pixel");
-    const void* d = optptr(dlogits);
-    if (d != nullptr)
-      TORCH_CHECK(dlogits->sizes() == logits.sizes() && dlogits->scalar_type() == torch::kBFloat16,
-                  "pixel_xent: dlogits must be bf16 with the shape of logits");
-    TORCH_CHECK(norm->device() == logits.device() && labels.device() == logits.device(),
-                "pixel_xent: tensors on different devices");
-    tfos::SegLossOpts o = seg_loss_opts(logits, ignore_index, weights, V, "pixel_xent");
+    TORCH_CHECK(norm->device() == logits.device(), "pixel_xent: tensors on different devices");
     o.norm = norm->data_ptr<double>();
-    check(tfos::pixel_xent_opt(logits.data_ptr(), labels.data_ptr<int>(), const_cast<void*>(d),
-                               loss_sum.data_ptr<float>(), optf(correct), P, static_cast<int>(VP),
-                               V, o, cur_stream()),
-          "pixel_xent");
-    return;
   }
-  if (logits.size(-1) > 8) {
-    TORCH_CHECK(seg_channels_match(logits, V), "pixel_xent: logits [B, ..., VP] with V in [1, 256] and "
-                "VP = 8 for V <= 8, ceil(V / 8) * 8 above");
-    const int64_t VP = logits.size(-1);
-    const int64_t P = logits.numel() / VP;
-    TORCH_CHECK(labels.numel() == P, "pixel_xent: one label per pixel");
-    const void* d = optptr(dlogits);
-    if (d != nullptr)
-      TORCH_CHECK(dlogits->sizes() == logits.sizes() && dlogits->scalar_type() == torch::kBFloat16,
-                  "pixel_xent: dlogits must be bf16 with the shape of logits");
-    check(tfos::pixel_xent_wide(logits.data_ptr(), labels.data_ptr<int>(), const_cast<void*>(d),
-                                loss_sum.data_ptr<float>(), optf(correct), P,
-                                static_cast<int>(VP), V, scale, cur_stream()),
-          "pixel_xent");
-    return;
-  }
-  TORCH_CHECK(logits.size(-1) == 8 && V <= 8, "pixel_xent expects 8 padded channels");
-  check(tfos::pixel_xent(logits.data_ptr(), labels.data_ptr<int>(),
-                         const_cast<void*>(optptr(dlogits)), loss_sum.data_ptr<float>(),
-                         optf(correct), logits.numel() / 8, V, scale, cur_stream()),
+  check(tfos::pixel_xent(logits.data_ptr(), labels.data_ptr<int>(), const_cast<void*>(d),
+                         loss_sum.data_ptr<float>(), optf(correct), P, static_cast<int>(VP), V,
+                         static_cast<float>(scale), opt ? &o : nullptr, cur_stream()),
         "pixel_xent");
 }
 

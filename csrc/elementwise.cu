@@ -615,26 +615,23 @@ copy_channels_kernel(const __nv_bfloat16* __restrict__ src, __nv_bfloat16* __res
 
 // Per-pixel softmax cross-entropy for a handful of classes (V <= 8): one thread per pixel, the
 // pixel's 8 padded logits are one 16-byte load.  loss_sum += -log p[label] * scale,
-// dlogits = (p - onehot) * scale, padded channels get zero gradient.  kOpt (pixel_xent_opt_kernel):
-// the loss options of seg_wide.cuh, scale = w[label] * inv with inv from o.norm; a pixel with
-// scale 0 (ignored, zero weight, or an empty batch) adds nothing and gets an exact zero gradient.
+// dlogits = (p - onehot) * scale, padded channels get zero gradient.  The predicted class is
+// seg_argmax (seg_wide.cuh).  kOpt: the loss options of seg_wide.cuh, scale (the argument is
+// unused) = w[label] * inv with inv from o.norm; a pixel with scale 0 (ignored, zero weight, or
+// an empty batch) adds nothing and gets an exact zero gradient.
 template <bool kOpt>
-__device__ __forceinline__ void pixel_xent_body(const __nv_bfloat16* __restrict__ logits,
-                                                const int* __restrict__ labels,
-                                                __nv_bfloat16* __restrict__ dlogits,
-                                                float* loss_sum, float* correct_sum, long long P,
-                                                int V, float scale, const SegLossOpts& o) {
+__global__ void __launch_bounds__(256)
+pixel_xent_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                  __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
+                  long long P, int V, float scale, const SegLossOpts o) {
   if (kOpt) scale = static_cast<float>(o.norm[2]);
   float local = 0.f, hits = 0.f;
   for (long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; p < P;
        p += static_cast<long long>(gridDim.x) * blockDim.x) {
     float l[8];
     load8(logits + p * 8, l);
-    float mx = l[0];
-    int am = 0;
-#pragma unroll
-    for (int j = 1; j < 8; ++j)
-      if (j < V && l[j] > mx) mx = l[j], am = j;
+    float mx;
+    const int am = seg_argmax(l, V, mx);
     float se = 0.f, e[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -666,35 +663,18 @@ __device__ __forceinline__ void pixel_xent_body(const __nv_bfloat16* __restrict_
   }
 }
 
-__global__ void __launch_bounds__(256)
-pixel_xent_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
-                  __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
-                  long long P, int V, float scale) {
-  pixel_xent_body<false>(logits, labels, dlogits, loss_sum, correct_sum, P, V, scale,
-                         SegLossOpts{});
-}
-
-__global__ void __launch_bounds__(256)
-pixel_xent_opt_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
-                      __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
-                      long long P, int V, const SegLossOpts o) {
-  pixel_xent_body<true>(logits, labels, dlogits, loss_sum, correct_sum, P, V, 0.f, o);
-}
-
 // pixel_xent for VP = 16..256 padded channels (V = 9..256 classes): G lanes per pixel
 // (seg_wide.cuh), each lane one 16-byte chunk of the logits in registers, so every pixel's logits
 // are read once and its dlogits written once.  Warp tile t covers pixels [t * 32 / G, ...); the
 // loop bound is uniform over the warp, so the full-mask group shuffles are safe.  Channels
 // j >= V get exactly zero gradient and never enter the loss or the arg-max.  A label outside
 // [0, V) (not validated, as for the 8-channel kernel) contributes the loss mx + log(se), a
-// gradient without the one-hot term and no hit.  kOpt: the loss options, as pixel_xent_body.
+// gradient without the one-hot term and no hit.  kOpt: the loss options, as pixel_xent_kernel.
 template <int G, bool kOpt>
-__device__ __forceinline__ void pixel_xent_wide_body(const __nv_bfloat16* __restrict__ logits,
-                                                     const int* __restrict__ labels,
-                                                     __nv_bfloat16* __restrict__ dlogits,
-                                                     float* loss_sum, float* correct_sum,
-                                                     long long P, int VP, int V, float scale,
-                                                     const SegLossOpts& o) {
+__global__ void __launch_bounds__(256)
+pixel_xent_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                       __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
+                       long long P, int VP, int V, float scale, const SegLossOpts o) {
   if (kOpt) scale = static_cast<float>(o.norm[2]);
   constexpr int kPix = 32 / G;   // pixels per warp tile
   const int lane = threadIdx.x & 31, sub = lane & (G - 1), c0 = sub * 8;
@@ -744,24 +724,6 @@ __device__ __forceinline__ void pixel_xent_wide_body(const __nv_bfloat16* __rest
     atomicAdd(loss_sum, local);
     if (correct_sum != nullptr) atomicAdd(correct_sum, hits);
   }
-}
-
-template <int G>
-__global__ void __launch_bounds__(256)
-pixel_xent_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
-                       __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
-                       long long P, int VP, int V, float scale) {
-  pixel_xent_wide_body<G, false>(logits, labels, dlogits, loss_sum, correct_sum, P, VP, V, scale,
-                                 SegLossOpts{});
-}
-
-template <int G>
-__global__ void __launch_bounds__(256)
-pixel_xent_wide_opt_kernel(const __nv_bfloat16* __restrict__ logits,
-                           const int* __restrict__ labels, __nv_bfloat16* __restrict__ dlogits,
-                           float* loss_sum, float* correct_sum, long long P, int VP, int V,
-                           const SegLossOpts o) {
-  pixel_xent_wide_body<G, true>(logits, labels, dlogits, loss_sum, correct_sum, P, VP, V, 0.f, o);
 }
 
 // seg_label_norm: one CTA per SM over the labels.  Each CTA counts its labels per class in shared
@@ -986,63 +948,33 @@ cudaError_t copy_channels(const void* src, void* dst, long long P, int C, int sr
       src_off, dst_ld, dst_off);
   TFOS_RET();
 }
-cudaError_t pixel_xent(const void* logits, const int* labels, void* dlogits, float* loss_sum,
-                       float* correct_sum, long long P, int V, float scale, cudaStream_t s) {
-  pixel_xent_kernel<<<grid_for(P, 256, kMaxBlocks), 256, 0, s>>>(
-      static_cast<const __nv_bfloat16*>(logits), labels, static_cast<__nv_bfloat16*>(dlogits),
-      loss_sum, correct_sum, P, V, scale);
-  TFOS_RET();
-}
-cudaError_t pixel_xent_wide(const void* logits, const int* labels, void* dlogits, float* loss_sum,
-                            float* correct_sum, long long P, int VP, int V, float scale,
-                            cudaStream_t s) {
-  const int G = seg_wide_group(VP);
-  const int grid = grid_for(P * G, 256, kMaxBlocks);
-  const auto* l = static_cast<const __nv_bfloat16*>(logits);
-  auto* d = static_cast<__nv_bfloat16*>(dlogits);
-#define TFOS_XENT_WIDE(g)                                                                     \
-  case g:                                                                                     \
-    pixel_xent_wide_kernel<g><<<grid, 256, 0, s>>>(l, labels, d, loss_sum, correct_sum, P, VP, \
-                                                   V, scale);                                 \
-    break;
-  switch (G) {
-    TFOS_XENT_WIDE(2)
-    TFOS_XENT_WIDE(4)
-    TFOS_XENT_WIDE(8)
-    TFOS_XENT_WIDE(16)
-    TFOS_XENT_WIDE(32)
-    default: return cudaErrorInvalidValue;
-  }
-#undef TFOS_XENT_WIDE
-  TFOS_RET();
-}
-cudaError_t pixel_xent_opt(const void* logits, const int* labels, void* dlogits, float* loss_sum,
-                           float* correct_sum, long long P, int VP, int V, SegLossOpts o,
-                           cudaStream_t s) {
-  const auto* l = static_cast<const __nv_bfloat16*>(logits);
-  auto* d = static_cast<__nv_bfloat16*>(dlogits);
+// the default (kOpt false) and the option instances: one launch geometry
+template <bool kOpt>
+static cudaError_t launch_pixel_xent(const __nv_bfloat16* logits, const int* labels,
+                                     __nv_bfloat16* dlogits, float* loss_sum, float* correct_sum,
+                                     long long P, int VP, int V, float scale, const SegLossOpts& o,
+                                     cudaStream_t s) {
   if (VP == 8) {
-    pixel_xent_opt_kernel<<<grid_for(P, 256, kMaxBlocks), 256, 0, s>>>(l, labels, d, loss_sum,
-                                                                         correct_sum, P, V, o);
+    pixel_xent_kernel<kOpt><<<grid_for(P, 256, kMaxBlocks), 256, 0, s>>>(
+        logits, labels, dlogits, loss_sum, correct_sum, P, V, scale, o);
     TFOS_RET();
   }
-  const int G = seg_wide_group(VP);
-  const int grid = grid_for(P * G, 256, kMaxBlocks);
-#define TFOS_XENT_WIDE_OPT(g)                                                                 \
-  case g:                                                                                     \
-    pixel_xent_wide_opt_kernel<g><<<grid, 256, 0, s>>>(l, labels, d, loss_sum, correct_sum, P, \
-                                                       VP, V, o);                             \
-    break;
-  switch (G) {
-    TFOS_XENT_WIDE_OPT(2)
-    TFOS_XENT_WIDE_OPT(4)
-    TFOS_XENT_WIDE_OPT(8)
-    TFOS_XENT_WIDE_OPT(16)
-    TFOS_XENT_WIDE_OPT(32)
-    default: return cudaErrorInvalidValue;
-  }
-#undef TFOS_XENT_WIDE_OPT
-  TFOS_RET();
+  return seg_wide_dispatch(VP, [&](auto g) {
+    constexpr int G = decltype(g)::value;
+    pixel_xent_wide_kernel<G, kOpt><<<grid_for(P * G, 256, kMaxBlocks), 256, 0, s>>>(
+        logits, labels, dlogits, loss_sum, correct_sum, P, VP, V, scale, o);
+    TFOS_RET();
+  });
+}
+cudaError_t pixel_xent(const void* logits, const int* labels, void* dlogits, float* loss_sum,
+                       float* correct_sum, long long P, int VP, int V, float scale,
+                       const SegLossOpts* opts, cudaStream_t s) {
+  const auto* l = static_cast<const __nv_bfloat16*>(logits);
+  auto* d = static_cast<__nv_bfloat16*>(dlogits);
+  if (opts != nullptr)
+    return launch_pixel_xent<true>(l, labels, d, loss_sum, correct_sum, P, VP, V, scale, *opts, s);
+  return launch_pixel_xent<false>(l, labels, d, loss_sum, correct_sum, P, VP, V, scale,
+                                  SegLossOpts{}, s);
 }
 cudaError_t seg_label_norm(const int* labels, long long P, int V, SegLossOpts o, double* norm,
                            unsigned long long* scratch, cudaStream_t s) {

@@ -126,35 +126,18 @@ constexpr int kSegUnroll = 4;        // pixels per thread in flight
 constexpr int kSegStep = kSegThreads * kSegUnroll;
 constexpr int kSegBins = 8 * 8 + 1;  // confusion cells y * 8 + pred, then "invalid label"
 
-// The predicted class of one pixel: pixel_xent_kernel's arg-max, a strict > over j < V starting
-// from l[0], so the lowest index wins ties, a NaN never replaces the running maximum and channels
-// >= V are never read.  mx is the maximum that scan ends with.  Shared by evaluation (seg_score)
-// and serving (seg_predict), so a served mask is exactly the prediction evaluation scores.
-__device__ __forceinline__ int seg_argmax(const float (&l)[8], const int V, float& mx) {
-  mx = l[0];
-  int am = 0;
-#pragma unroll
-  for (int j = 1; j < 8; ++j)
-    if (j < V && l[j] > mx) mx = l[j], am = j;
-  return am;
-}
-
-__device__ __forceinline__ void unpack_bf16x8(const uint4 v, float (&l)[8]) {
-  const float2 a = unpack_bf16x2(v.x), b = unpack_bf16x2(v.y), c = unpack_bf16x2(v.z),
-               d = unpack_bf16x2(v.w);
-  l[0] = a.x, l[1] = a.y, l[2] = b.x, l[3] = b.y, l[4] = c.x, l[5] = c.y, l[6] = d.x, l[7] = d.y;
-}
-
 // One pixel: its bin (y * 8 + pred, kSegBins - 1 for a label outside [0, V)) and loss.  pred is
-// seg_argmax, so an evaluation's "correct" counts exactly what training's does.  kOpt: the loss
-// options (seg_wide.cuh): an ignored pixel has no bin (-1), the loss term is weighted by w[y].
+// seg_argmax (seg_wide.cuh), as in training (pixel_xent) and serving (seg_predict), so an
+// evaluation's "correct" counts exactly what training's does and a served mask is exactly the
+// prediction evaluation scores.  kOpt: the loss options (seg_wide.cuh): an ignored pixel has no
+// bin (-1), the loss term is weighted by w[y].
 template <bool kOpt>
 __device__ __forceinline__ int seg_score(const uint4 v, const int y, const int V, double& loss,
                                          const SegLossOpts& o) {
   if (kOpt && seg_ignored(o, y)) return -1;
   if (y < 0 || y >= V) return kSegBins - 1;
   float l[8];
-  unpack_bf16x8(v, l);
+  seg_unpack8(v, l);
   float mx;
   const int am = seg_argmax(l, V, mx);
   float se = 0.f, ly = 0.f;
@@ -172,6 +155,33 @@ __device__ __forceinline__ int seg_score(const uint4 v, const int y, const int V
   return y * 8 + am;
 }
 
+// The pixel range [lo, hi) of CTA blockIdx.x: its chunk of the pixels of images [0, *n_valid),
+// *n_valid clamped to [0, images].
+__device__ __forceinline__ void seg_eval_range(const int* __restrict__ n_valid, const int images,
+                                               const long long ppi, const long long chunk,
+                                               long long& lo, long long& hi) {
+  int n = *n_valid;
+  n = n < 0 ? 0 : (n > images ? images : n);
+  const long long limit = static_cast<long long>(n) * ppi;
+  lo = static_cast<long long>(blockIdx.x) * chunk;
+  hi = lo + chunk < limit ? lo + chunk : limit;
+}
+
+// One warp's sum of one row of per-CTA partials: lane -> CTAs lane, lane + 32, ... in that
+// order, then a shuffle tree.  The order is fixed, so the sum is bitwise reproducible.
+__device__ __forceinline__ double seg_partial_sum(const double* __restrict__ row, const int grid,
+                                                  const int lane) {
+  double t = 0.0;
+#pragma unroll
+  for (int k = 0; k < (kSegMaxGrid + 31) / 32; ++k) {
+    const int b = lane + 32 * k;
+    if (b < grid) t += __ldcg(row + b);
+  }
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+  return t;
+}
+
 // Pixels [0, n_valid * ppi) of bf16 logits [P, 8] and int32 labels [P].  CTA b owns the pixel
 // range [b * chunk, (b + 1) * chunk) (chunk a multiple of kSegStep); each pass over kSegStep
 // pixels loads pixels u * kSegThreads + t (u < kSegUnroll) into thread t first, then scores
@@ -181,12 +191,13 @@ __device__ __forceinline__ int seg_score(const uint4 v, const int y, const int V
 // per-thread fp64 sum reduced in a fixed tree.  The CTA writes its partials slot-major
 // (partial[s * grid + b]); the last CTA to finish sums each slot over the CTAs with a fixed
 // lane -> CTA assignment and shuffle tree.  So the totals are bitwise reproducible.
+// kOpt: the loss options, as seg_score.
 template <bool kOpt>
-__device__ __forceinline__ void seg_eval_metrics_body(
-    const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
-    const int* __restrict__ n_valid, double* __restrict__ acc, double* __restrict__ partial,
-    unsigned int* __restrict__ counter, int images, long long ppi, long long chunk, int V,
-    const SegLossOpts& o) {
+__global__ void __launch_bounds__(kSegThreads)
+seg_eval_metrics_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                        const int* __restrict__ n_valid, double* __restrict__ acc,
+                        double* __restrict__ partial, unsigned int* __restrict__ counter,
+                        int images, long long ppi, long long chunk, int V, const SegLossOpts o) {
   __shared__ int bins[kSegWarps][kSegBins];
   __shared__ int cells[kSegBins];
   __shared__ double wloss[kSegWarps];
@@ -194,11 +205,8 @@ __device__ __forceinline__ void seg_eval_metrics_body(
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int i = threadIdx.x; i < kSegWarps * kSegBins; i += kSegThreads) (&bins[0][0])[i] = 0;
   __syncthreads();
-  int n = *n_valid;
-  n = n < 0 ? 0 : (n > images ? images : n);
-  const long long limit = static_cast<long long>(n) * ppi;
-  const long long lo = static_cast<long long>(blockIdx.x) * chunk;
-  const long long hi = lo + chunk < limit ? lo + chunk : limit;
+  long long lo, hi;
+  seg_eval_range(n_valid, images, ppi, chunk, lo, hi);
   double loss = 0.0;
   for (long long base = lo; base < hi; base += kSegStep) {
     uint4 v[kSegUnroll];
@@ -261,37 +269,10 @@ __device__ __forceinline__ void seg_eval_metrics_body(
   if (!is_last) return;
   __threadfence();
   for (int s = warp; s < kSegEvalSlots; s += kSegWarps) {   // one warp per slot
-    const double* row = partial + static_cast<long long>(s) * grid;
-    double t = 0.0;
-#pragma unroll
-    for (int k = 0; k < (kSegMaxGrid + 31) / 32; ++k) {   // lane -> CTAs lane, lane + 32, ...
-      const int b = lane + 32 * k;
-      if (b < grid) t += __ldcg(row + b);
-    }
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    const double t = seg_partial_sum(partial + static_cast<long long>(s) * grid, grid, lane);
     if (lane == 0) acc[s] += t;
   }
   if (threadIdx.x == 0) *counter = 0;  // ready for the next launch or graph replay
-}
-
-__global__ void __launch_bounds__(kSegThreads)
-seg_eval_metrics_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
-                        const int* __restrict__ n_valid, double* __restrict__ acc,
-                        double* __restrict__ partial, unsigned int* __restrict__ counter,
-                        int images, long long ppi, long long chunk, int V) {
-  seg_eval_metrics_body<false>(logits, labels, n_valid, acc, partial, counter, images, ppi, chunk,
-                               V, SegLossOpts{});
-}
-
-__global__ void __launch_bounds__(kSegThreads)
-seg_eval_metrics_opt_kernel(const __nv_bfloat16* __restrict__ logits,
-                            const int* __restrict__ labels, const int* __restrict__ n_valid,
-                            double* __restrict__ acc, double* __restrict__ partial,
-                            unsigned int* __restrict__ counter, int images, long long ppi,
-                            long long chunk, int V, const SegLossOpts o) {
-  seg_eval_metrics_body<true>(logits, labels, n_valid, acc, partial, counter, images, ppi, chunk,
-                              V, o);
 }
 
 constexpr int kPredThreads = 128;
@@ -328,7 +309,7 @@ seg_predict_kernel(const __nv_bfloat16* __restrict__ logits, uint8_t* __restrict
 #pragma unroll
   for (int u = 0; u < kPredPerThread; ++u) {
     float l[8], mx;
-    unpack_bf16x8(v[u], l);
+    seg_unpack8(v[u], l);
     cls[warp][u * 32 + lane] = static_cast<uint8_t>(seg_argmax(l, V, mx));
     if (out != nullptr) {
       const int n = count - u * 32;          // pixels of this load inside the range
@@ -366,13 +347,17 @@ constexpr int kSegWideSmemTable = 100 * 1024;
 // Scalars: count / correct / invalid as integers, the loss as fp64, per thread, then warp-shuffle
 // and warp-order sums into the CTA's partials; the last CTA to finish sums the partials in a fixed
 // order, adds the table into acc and zeroes it.  Bitwise reproducible.
-template <int G>
-__global__ void __launch_bounds__(kSegThreads)
+// kOpt: the loss options (seg_wide.cuh), as seg_score: an ignored pixel is neither counted nor
+// invalid and has no bin, the loss term is weighted by w[y].  One CTA per SM is the option
+// instances' register budget: without it ptxas fits G = 32 into 32 registers and spills.  The
+// default instances state no minimum.
+template <int G, bool kOpt>
+__global__ void __launch_bounds__(kSegThreads, kOpt ? 1 : 0)
 seg_eval_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
                      const int* __restrict__ n_valid, double* __restrict__ acc,
                      double* __restrict__ partial, unsigned long long* __restrict__ table,
                      unsigned int* __restrict__ counter, int images, long long ppi,
-                     long long chunk, int VP, int V, int smem_table) {
+                     long long chunk, int VP, int V, int smem_table, const SegLossOpts o) {
   extern __shared__ unsigned int tab[];
   __shared__ int wint[3][kSegWarps];
   __shared__ double wloss[kSegWarps];
@@ -383,11 +368,8 @@ seg_eval_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __rest
   if (smem_table)
     for (int i = threadIdx.x; i < cells; i += kSegThreads) tab[i] = 0u;
   __syncthreads();
-  int n = *n_valid;
-  n = n < 0 ? 0 : (n > images ? images : n);
-  const long long limit = static_cast<long long>(n) * ppi;
-  const long long lo = static_cast<long long>(blockIdx.x) * chunk;
-  const long long hi = lo + chunk < limit ? lo + chunk : limit;
+  long long lo, hi;
+  seg_eval_range(n_valid, images, ppi, chunk, lo, hi);
   int cnt = 0, hit = 0, bad = 0;
   double loss = 0.0;
   for (long long base = lo + warp * kPix; base < hi; base += kSegWarps * kPix) {
@@ -412,13 +394,18 @@ seg_eval_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __rest
     se = seg_group_sum<G>(se);
     ly = seg_group_sum<G>(ly);
     int bin = -1;
-    if (in && sub == 0) {
+    if (in && sub == 0 && !(kOpt && seg_ignored(o, y))) {
       if (y < 0 || y >= V) {
         bad += 1;
       } else {
         cnt += 1;
         hit += am == y ? 1 : 0;
-        loss += static_cast<double>(__logf(se) + mx - ly);
+        if constexpr (kOpt) {
+          const float w = seg_weight(o, y, V);
+          if (w != 0.f) loss += static_cast<double>(w) * static_cast<double>(__logf(se) + mx - ly);
+        } else {
+          loss += static_cast<double>(__logf(se) + mx - ly);
+        }
         bin = y * V + am;
       }
     }
@@ -464,140 +451,7 @@ seg_eval_wide_kernel(const __nv_bfloat16* __restrict__ logits, const int* __rest
   if (!is_last) return;
   __threadfence();
   if (warp < kSegWideScalars) {   // the four scalar slots, one warp each
-    const double* row = partial + static_cast<long long>(warp) * grid;
-    double t = 0.0;
-#pragma unroll
-    for (int k = 0; k < (kSegMaxGrid + 31) / 32; ++k) {
-      const int b = lane + 32 * k;
-      if (b < grid) t += __ldcg(row + b);
-    }
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-    if (lane == 0) acc[warp] += t;
-  }
-  for (int i = threadIdx.x; i < cells; i += kSegThreads) {
-    const unsigned long long c = __ldcg(table + i);
-    if (c) {
-      acc[kSegWideConfusion + i] += static_cast<double>(c);
-      table[i] = 0ull;
-    }
-  }
-  if (threadIdx.x == 0) *counter = 0;  // ready for the next launch or graph replay
-}
-
-// seg_eval_wide_kernel with the loss options (seg_wide.cuh), as seg_score: an ignored pixel is
-// neither counted nor invalid and has no bin, the loss term is weighted by w[y].  A copy of
-// seg_eval_wide_kernel rather than a shared inline body: inlining a common body changes the
-// default instances' register allocation.  One CTA per SM is the register budget: without it
-// ptxas fits G = 32 into 32 registers and spills.
-template <int G>
-__global__ void __launch_bounds__(kSegThreads, 1)
-seg_eval_wide_opt_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
-                         const int* __restrict__ n_valid, double* __restrict__ acc,
-                         double* __restrict__ partial, unsigned long long* __restrict__ table,
-                         unsigned int* __restrict__ counter, int images, long long ppi,
-                         long long chunk, int VP, int V, int smem_table, const SegLossOpts o) {
-  extern __shared__ unsigned int tab[];
-  __shared__ int wint[3][kSegWarps];
-  __shared__ double wloss[kSegWarps];
-  __shared__ unsigned int is_last;
-  constexpr int kPix = 32 / G;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, sub = lane & (G - 1), c0 = sub * 8;
-  const int cells = V * V;
-  if (smem_table)
-    for (int i = threadIdx.x; i < cells; i += kSegThreads) tab[i] = 0u;
-  __syncthreads();
-  int n = *n_valid;
-  n = n < 0 ? 0 : (n > images ? images : n);
-  const long long limit = static_cast<long long>(n) * ppi;
-  const long long lo = static_cast<long long>(blockIdx.x) * chunk;
-  const long long hi = lo + chunk < limit ? lo + chunk : limit;
-  int cnt = 0, hit = 0, bad = 0;
-  double loss = 0.0;
-  for (long long base = lo + warp * kPix; base < hi; base += kSegWarps * kPix) {
-    const long long p = base + lane / G;
-    const bool in = p < hi;
-    float l[8];
-    if (in && c0 < VP) {
-      seg_unpack8(__ldcs(reinterpret_cast<const uint4*>(logits + p * VP + c0)), l);
-    } else {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) l[k] = 0.f;
-    }
-    const int y = in ? __ldcs(labels + p) : -1;
-    float mx;
-    const int am = seg_argmax_wide<G>(l, c0, V, mx);
-    float se = 0.f, ly = 0.f;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      if (c0 + k < V) se += __expf(l[k] - mx);
-      if (c0 + k < V && c0 + k == y) ly = l[k];
-    }
-    se = seg_group_sum<G>(se);
-    ly = seg_group_sum<G>(ly);
-    int bin = -1;
-    if (in && sub == 0 && !seg_ignored(o, y)) {
-      if (y < 0 || y >= V) {
-        bad += 1;
-      } else {
-        cnt += 1;
-        hit += am == y ? 1 : 0;
-        const float w = seg_weight(o, y, V);
-        if (w != 0.f) loss += static_cast<double>(w) * static_cast<double>(__logf(se) + mx - ly);
-        bin = y * V + am;
-      }
-    }
-    const unsigned same = __match_any_sync(0xffffffffu, bin);
-    if (bin >= 0 && lane == __ffs(same) - 1) {
-      if (smem_table) atomicAdd(&tab[bin], static_cast<unsigned>(__popc(same)));
-      else atomicAdd(&table[bin], static_cast<unsigned long long>(__popc(same)));
-    }
-  }
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) {
-    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    hit += __shfl_xor_sync(0xffffffffu, hit, o);
-    bad += __shfl_xor_sync(0xffffffffu, bad, o);
-    loss += __shfl_xor_sync(0xffffffffu, loss, o);
-  }
-  if (lane == 0) {
-    wint[0][warp] = cnt, wint[1][warp] = hit, wint[2][warp] = bad;
-    wloss[warp] = loss;
-  }
-  __syncthreads();
-  const int grid = gridDim.x;
-  if (threadIdx.x == 0) {
-    long long c = 0, h = 0, b = 0;
-    double l = 0.0;
-    for (int w = 0; w < kSegWarps; ++w)
-      c += wint[0][w], h += wint[1][w], b += wint[2][w], l += wloss[w];
-    partial[static_cast<long long>(kSegEvalCount) * grid + blockIdx.x] = static_cast<double>(c);
-    partial[static_cast<long long>(kSegEvalCorrect) * grid + blockIdx.x] = static_cast<double>(h);
-    partial[static_cast<long long>(kSegEvalInvalid) * grid + blockIdx.x] = static_cast<double>(b);
-    partial[static_cast<long long>(kSegEvalLoss) * grid + blockIdx.x] = l;
-  }
-  if (smem_table) {
-    for (int i = threadIdx.x; i < cells; i += kSegThreads) {
-      const unsigned c = tab[i];
-      if (c) atomicAdd(&table[i], static_cast<unsigned long long>(c));
-    }
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) is_last = (atomicAdd(counter, 1u) == gridDim.x - 1) ? 1u : 0u;
-  __syncthreads();
-  if (!is_last) return;
-  __threadfence();
-  if (warp < kSegWideScalars) {   // the four scalar slots, one warp each
-    const double* row = partial + static_cast<long long>(warp) * grid;
-    double t = 0.0;
-#pragma unroll
-    for (int k = 0; k < (kSegMaxGrid + 31) / 32; ++k) {
-      const int b = lane + 32 * k;
-      if (b < grid) t += __ldcg(row + b);
-    }
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    const double t = seg_partial_sum(partial + static_cast<long long>(warp) * grid, grid, lane);
     if (lane == 0) acc[warp] += t;
   }
   for (int i = threadIdx.x; i < cells; i += kSegThreads) {
@@ -651,95 +505,6 @@ long long seg_eval_wide_scratch(long long pixels, int V) {
          static_cast<long long>(V) * V;
 }
 
-// seg_eval_metrics_wide (kOpt false) and its optioned instances: one launch geometry
-template <bool kOpt>
-cudaError_t launch_seg_eval_wide(const void* logits, const int* labels, const int* n_valid,
-                                 double* acc, double* scratch, unsigned int* counter, int images,
-                                 long long ppi, int VP, int V, const SegLossOpts& o,
-                                 cudaStream_t s) {
-  const long long pixels = static_cast<long long>(images) * ppi;
-  const int grid = seg_eval_grid(pixels);
-  const long long chunk =
-      ((pixels + grid - 1) / grid + kSegWideChunk - 1) / kSegWideChunk * kSegWideChunk;
-  // the table first: its place does not depend on the grid, so one scratch serves any pixel count
-  auto* table = reinterpret_cast<unsigned long long*>(scratch);
-  double* partial = scratch + static_cast<long long>(V) * V;
-  const size_t tbytes = static_cast<size_t>(V) * V * sizeof(unsigned int);
-  const int smem_table = tbytes <= static_cast<size_t>(kSegWideSmemTable) ? 1 : 0;
-  const size_t smem = smem_table ? tbytes : 0;
-  const auto* l = static_cast<const __nv_bfloat16*>(logits);
-#define TFOS_SEG_EVAL_WIDE(g)                                                                   \
-  case g: {                                                                                     \
-    static const cudaError_t attr =                                                             \
-        kOpt ? cudaFuncSetAttribute(seg_eval_wide_opt_kernel<g>,                                \
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize,                \
-                                    kSegWideSmemTable)                                          \
-             : cudaFuncSetAttribute(seg_eval_wide_kernel<g>,                                    \
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize,                \
-                                    kSegWideSmemTable);                                         \
-    if (attr != cudaSuccess) return attr;                                                       \
-    if constexpr (kOpt)                                                                         \
-      seg_eval_wide_opt_kernel<g><<<grid, kSegThreads, smem, s>>>(                              \
-          l, labels, n_valid, acc, partial, table, counter, images, ppi, chunk, VP, V,          \
-          smem_table, o);                                                                       \
-    else                                                                                        \
-      seg_eval_wide_kernel<g><<<grid, kSegThreads, smem, s>>>(l, labels, n_valid, acc, partial, \
-                                                              table, counter, images, ppi,      \
-                                                              chunk, VP, V, smem_table);        \
-    break;                                                                                      \
-  }
-  switch (seg_wide_group(VP)) {
-    TFOS_SEG_EVAL_WIDE(2)
-    TFOS_SEG_EVAL_WIDE(4)
-    TFOS_SEG_EVAL_WIDE(8)
-    TFOS_SEG_EVAL_WIDE(16)
-    TFOS_SEG_EVAL_WIDE(32)
-    default: return cudaErrorInvalidValue;
-  }
-#undef TFOS_SEG_EVAL_WIDE
-  return cudaGetLastError();
-}
-
-cudaError_t seg_eval_metrics_wide(const void* logits, const int* labels, const int* n_valid,
-                                  double* acc, double* scratch, unsigned int* counter, int images,
-                                  long long ppi, int VP, int V, cudaStream_t s) {
-  return launch_seg_eval_wide<false>(logits, labels, n_valid, acc, scratch, counter, images, ppi,
-                                     VP, V, SegLossOpts{}, s);
-}
-
-cudaError_t seg_predict_wide(const void* logits, uint8_t* mask, float* out, long long pixels,
-                             int VP, int V, cudaStream_t s) {
-  if (pixels <= 0) return cudaSuccess;
-  const int G = seg_wide_group(VP);
-  long long blocks = (pixels * G + 255) / 256;
-  if (blocks > kSmCount * 8) blocks = kSmCount * 8;
-  const auto* l = static_cast<const __nv_bfloat16*>(logits);
-#define TFOS_SEG_PREDICT_WIDE(g)                                                            \
-  case g:                                                                                   \
-    seg_predict_wide_kernel<g><<<static_cast<unsigned>(blocks), 256, 0, s>>>(l, mask, out, \
-                                                                            pixels, VP, V); \
-    break;
-  switch (G) {
-    TFOS_SEG_PREDICT_WIDE(2)
-    TFOS_SEG_PREDICT_WIDE(4)
-    TFOS_SEG_PREDICT_WIDE(8)
-    TFOS_SEG_PREDICT_WIDE(16)
-    TFOS_SEG_PREDICT_WIDE(32)
-    default: return cudaErrorInvalidValue;
-  }
-#undef TFOS_SEG_PREDICT_WIDE
-  return cudaGetLastError();
-}
-
-cudaError_t seg_predict(const void* logits, uint8_t* mask, float* out, long long pixels, int V,
-                        cudaStream_t s) {
-  if (pixels <= 0) return cudaSuccess;
-  const long long blocks = (pixels + kPredPerBlock - 1) / kPredPerBlock;
-  seg_predict_kernel<<<static_cast<unsigned>(blocks), kPredThreads, 0, s>>>(
-      static_cast<const __nv_bfloat16*>(logits), mask, out, pixels, V);
-  return cudaGetLastError();
-}
-
 int seg_eval_grid(long long pixels) {
   long long blocks = (pixels + kSegStep - 1) / kSegStep;
   if (blocks > kSegMaxGrid) blocks = kSegMaxGrid;
@@ -751,29 +516,69 @@ static long long seg_eval_chunk(long long pixels, int grid) {
   return ((pixels + grid - 1) / grid + kSegStep - 1) / kSegStep * kSegStep;
 }
 
-cudaError_t seg_eval_metrics(const void* logits, const int* labels, const int* n_valid,
-                             double* acc, double* partial, unsigned int* counter, int images,
-                             long long ppi, int V, cudaStream_t s) {
+// the default (kOpt false) and the option instances: one grid and scratch layout
+template <bool kOpt>
+static cudaError_t launch_seg_eval(const __nv_bfloat16* logits, const int* labels,
+                                   const int* n_valid, double* acc, double* scratch,
+                                   unsigned int* counter, int images, long long ppi, int VP, int V,
+                                   const SegLossOpts& o, cudaStream_t s) {
   const long long pixels = static_cast<long long>(images) * ppi;
   const int grid = seg_eval_grid(pixels);
-  seg_eval_metrics_kernel<<<grid, kSegThreads, 0, s>>>(
-      static_cast<const __nv_bfloat16*>(logits), labels, n_valid, acc, partial, counter, images,
-      ppi, seg_eval_chunk(pixels, grid), V);
-  return cudaGetLastError();
+  if (VP == 8) {
+    seg_eval_metrics_kernel<kOpt><<<grid, kSegThreads, 0, s>>>(
+        logits, labels, n_valid, acc, scratch, counter, images, ppi, seg_eval_chunk(pixels, grid),
+        V, o);
+    return cudaGetLastError();
+  }
+  const long long chunk =
+      ((pixels + grid - 1) / grid + kSegWideChunk - 1) / kSegWideChunk * kSegWideChunk;
+  // the table first: its place does not depend on the grid, so one scratch serves any pixel count
+  auto* table = reinterpret_cast<unsigned long long*>(scratch);
+  double* partial = scratch + static_cast<long long>(V) * V;
+  const size_t tbytes = static_cast<size_t>(V) * V * sizeof(unsigned int);
+  const int smem_table = tbytes <= static_cast<size_t>(kSegWideSmemTable) ? 1 : 0;
+  const size_t smem = smem_table ? tbytes : 0;
+  return seg_wide_dispatch(VP, [&](auto g) {
+    auto* kernel = seg_eval_wide_kernel<decltype(g)::value, kOpt>;
+    static const cudaError_t attr = cudaFuncSetAttribute(
+        kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSegWideSmemTable);
+    if (attr != cudaSuccess) return attr;
+    kernel<<<grid, kSegThreads, smem, s>>>(logits, labels, n_valid, acc, partial, table, counter,
+                                           images, ppi, chunk, VP, V, smem_table, o);
+    return cudaGetLastError();
+  });
 }
 
-cudaError_t seg_eval_metrics_opt(const void* logits, const int* labels, const int* n_valid,
-                                 double* acc, double* scratch, unsigned int* counter, int images,
-                                 long long ppi, int VP, int V, SegLossOpts o, cudaStream_t s) {
-  if (VP != 8)
-    return launch_seg_eval_wide<true>(logits, labels, n_valid, acc, scratch, counter, images, ppi,
-                                      VP, V, o, s);
-  const long long pixels = static_cast<long long>(images) * ppi;
-  const int grid = seg_eval_grid(pixels);
-  seg_eval_metrics_opt_kernel<<<grid, kSegThreads, 0, s>>>(
-      static_cast<const __nv_bfloat16*>(logits), labels, n_valid, acc, scratch, counter, images,
-      ppi, seg_eval_chunk(pixels, grid), V, o);
-  return cudaGetLastError();
+cudaError_t seg_eval_metrics(const void* logits, const int* labels, const int* n_valid,
+                             double* acc, double* scratch, unsigned int* counter, int images,
+                             long long ppi, int VP, int V, const SegLossOpts* opts,
+                             cudaStream_t s) {
+  const auto* l = static_cast<const __nv_bfloat16*>(logits);
+  if (opts != nullptr)
+    return launch_seg_eval<true>(l, labels, n_valid, acc, scratch, counter, images, ppi, VP, V,
+                                 *opts, s);
+  return launch_seg_eval<false>(l, labels, n_valid, acc, scratch, counter, images, ppi, VP, V,
+                                SegLossOpts{}, s);
+}
+
+cudaError_t seg_predict(const void* logits, uint8_t* mask, float* out, long long pixels, int VP,
+                        int V, cudaStream_t s) {
+  if (pixels <= 0) return cudaSuccess;
+  const auto* l = static_cast<const __nv_bfloat16*>(logits);
+  if (VP == 8) {
+    const long long blocks = (pixels + kPredPerBlock - 1) / kPredPerBlock;
+    seg_predict_kernel<<<static_cast<unsigned>(blocks), kPredThreads, 0, s>>>(l, mask, out, pixels,
+                                                                              V);
+    return cudaGetLastError();
+  }
+  return seg_wide_dispatch(VP, [&](auto g) {
+    constexpr int G = decltype(g)::value;
+    long long blocks = (pixels * G + 255) / 256;
+    if (blocks > kSmCount * 8) blocks = kSmCount * 8;
+    seg_predict_wide_kernel<G><<<static_cast<unsigned>(blocks), 256, 0, s>>>(l, mask, out, pixels,
+                                                                             VP, V);
+    return cudaGetLastError();
+  });
 }
 
 cudaError_t bn_fold(const long long* tab, const float* eps, const long long* row0, int units,

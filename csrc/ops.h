@@ -69,15 +69,8 @@ cudaError_t decode_normalize(const uint8_t* in, void* out, int N, int H, int W, 
 cudaError_t cast_f32_bf16(const float* in, void* out, long long n, cudaStream_t s);
 cudaError_t copy_channels(const void* src, void* dst, long long P, int C, int src_ld, int src_off,
                           int dst_ld, int dst_off, cudaStream_t s);
-cudaError_t pixel_xent(const void* logits, const int* labels, void* dlogits, float* loss_sum,
-                       float* correct_sum, long long P, int V, float scale, cudaStream_t s);
-// pixel_xent for bf16 logits [P, VP], VP = ceil(V / 8) * 8 in 16..256 (seg_wide.cuh): the same
-// loss, gradient (exactly zero in channels >= V) and hits, one read and one write per pixel
-cudaError_t pixel_xent_wide(const void* logits, const int* labels, void* dlogits, float* loss_sum,
-                            float* correct_sum, long long P, int VP, int V, float scale,
-                            cudaStream_t s);
-// Loss options of the segmentation U-Net (ignore_index, class weights), read by the optioned
-// instances of seg_label_norm, pixel_xent and seg_eval_metrics.  A pixel whose label equals
+// Loss options of the segmentation U-Net (ignore_index, class weights), read by seg_label_norm
+// and the optioned instances of pixel_xent and seg_eval_metrics.  A pixel whose label equals
 // `ignore` (when has_ignore) takes no part; w[y] = weights[y] for y in [0, V) (1 when weights is
 // null), 1 for any other label.  norm: [sum w, |S|, inv] as seg_label_norm writes it (fp64;
 // inv = 1 / sum w rounded to fp32, 0 when sum w = 0).
@@ -95,12 +88,17 @@ struct SegLossOpts {
 inline long long seg_label_norm_scratch(int V) { return V + 2; }
 cudaError_t seg_label_norm(const int* labels, long long P, int V, SegLossOpts o, double* norm,
                            unsigned long long* scratch, cudaStream_t s);
-// pixel_xent / pixel_xent_wide with loss options: loss_sum += sum over S of w[y] l_p * inv,
-// dlogits = w[y] (p - onehot) * inv on S, exactly 0 on ignored pixels, on pixels with
-// w[y] * inv = 0 and in channels >= V; correct_sum += the hits on S.  VP = 8: the 8-channel kernel.
-cudaError_t pixel_xent_opt(const void* logits, const int* labels, void* dlogits, float* loss_sum,
-                           float* correct_sum, long long P, int VP, int V, SegLossOpts o,
-                           cudaStream_t s);
+// pixel_xent: per-pixel softmax cross-entropy of bf16 logits [P, VP] over channels [0, V) and
+// int32 labels [P].  VP = 8 (V <= 8): one 16-byte load per pixel; VP = ceil(V / 8) * 8 in 16..256
+// (V = 9..256): the wide kernels (seg_wide.cuh), one read and one write per pixel.
+// loss_sum += sum of l_p * scale, dlogits (when not null) = (p - onehot) * scale, exactly zero in
+// channels >= V; correct_sum (when not null) += the pixels whose predicted class is the label.
+// opts not null: the loss options; scale is unused, inv comes from opts->norm.  loss_sum += sum
+// over S of w[y] l_p * inv, dlogits = w[y] (p - onehot) * inv on S and exactly 0 on ignored pixels
+// and on pixels with w[y] * inv = 0; correct_sum += the hits on S.
+cudaError_t pixel_xent(const void* logits, const int* labels, void* dlogits, float* loss_sum,
+                       float* correct_sum, long long P, int VP, int V, float scale,
+                       const SegLossOpts* opts, cudaStream_t s);
 
 // ---- optim_comm.cu
 constexpr int kMaxRanks = 8;
@@ -265,49 +263,37 @@ constexpr int kEvalCount = 0, kEvalTop1 = 1, kEvalTop5 = 2, kEvalInvalid = 3, kE
               kEvalUsedSlots = 5, kEvalSlots = 8;
 cudaError_t eval_metrics(const float* logits, const int* labels, const int* n_valid, double* acc,
                          int rows, int ld, int V, cudaStream_t s);
-// seg_eval_metrics: acc[kSegEval*] += totals of the pixels of images [0, *n_valid) of bf16
-// logits [images * ppi, 8] (channels [0, V) only) and int32 labels [images * ppi]: count,
-// correct, invalid labels, loss and confusion[y * 8 + pred].  partial holds seg_eval_grid(pixels)
-// x kSegEvalSlots doubles; counter is one zeroed uint32 that the kernel leaves at zero.
-// Deterministic: a fixed grid and pixel ranges, integer bins, the partials summed in a fixed
-// order by the last CTA to finish.
+// seg_eval_metrics: acc += totals of the pixels of images [0, *n_valid) of bf16 logits
+// [images * ppi, VP] (channels [0, V) only; VP as for pixel_xent) and int32 labels [images * ppi].
+// counter is one zeroed uint32 that the kernel leaves at zero.
+// VP = 8: acc[kSegEval*] = count, correct, invalid labels, loss and confusion[y * 8 + pred];
+// scratch holds seg_eval_grid(pixels) x kSegEvalSlots doubles of per-CTA partials.
+// VP = 16..256: accumulator layout [count, correct, invalid, loss, images, confusion V x V]
+// (kSegWide*; the kernel leaves images alone).  scratch: seg_eval_wide_scratch(pixels, V) doubles,
+// zero before the first launch: a uint64 [V, V] confusion table that the CTAs add their integer
+// counts to and the last CTA adds into acc and zeroes again, then per-CTA partials of the four
+// scalars.
+// Deterministic: a fixed grid and pixel ranges, integer counts (exact and order-independent), the
+// per-CTA partials summed in a fixed order by the last CTA to finish.
+// opts not null: the loss options (opts->norm unused): ignored pixels leave count, correct, loss
+// and the confusion matrix and are never invalid; the loss slot adds w[y] * l_p.
 constexpr int kSegEvalCount = 0, kSegEvalCorrect = 1, kSegEvalInvalid = 2, kSegEvalLoss = 3,
               kSegEvalConfusion = 4, kSegEvalSlots = 4 + 8 * 8;
-int seg_eval_grid(long long pixels);
-cudaError_t seg_eval_metrics(const void* logits, const int* labels, const int* n_valid,
-                             double* acc, double* partial, unsigned int* counter, int images,
-                             long long ppi, int V, cudaStream_t s);
-// seg_predict (serving): pixels [0, pixels) of bf16 logits [pixels, 8] -> mask[p] = the class
-// seg_eval_metrics / pixel_xent predict (lowest index among the maxima of channels [0, V)) and,
-// when out is not null, out[p * V + j] = the fp32 value of channel j < V.  One pass; mask and out
-// must be 16-byte aligned.
-cudaError_t seg_predict(const void* logits, uint8_t* mask, float* out, long long pixels, int V,
-                        cudaStream_t s);
-// Wide logits, bf16 [pixels, VP] with VP = ceil(V / 8) * 8 in 16..256 (9 <= V <= 256).
-// seg_eval_metrics_wide: acc[kSegWide*] += the same totals; accumulator layout
-// [count, correct, invalid, loss, images, confusion V x V] (the kernel leaves images alone).
-// scratch: seg_eval_wide_scratch(pixels, V) doubles, zero before the first launch: a uint64
-// [V, V] confusion table that the CTAs add their integer counts to and the last CTA adds into acc
-// and zeroes again, then per-CTA partials of the four scalars (summed in a fixed order by the
-// last CTA).  counter as for seg_eval_metrics.  Deterministic: integer counts are exact and
-// order-independent, the scalars are summed in a fixed order.
 constexpr int kSegWideImages = 4, kSegWideConfusion = 5;
+int seg_eval_grid(long long pixels);
 inline long long seg_eval_wide_slots(int V) {
   return kSegWideConfusion + static_cast<long long>(V) * V;
 }
 long long seg_eval_wide_scratch(long long pixels, int V);
-cudaError_t seg_eval_metrics_wide(const void* logits, const int* labels, const int* n_valid,
-                                  double* acc, double* scratch, unsigned int* counter, int images,
-                                  long long ppi, int VP, int V, cudaStream_t s);
-// seg_eval_metrics / seg_eval_metrics_wide with loss options (o.norm unused): ignored pixels
-// leave count, correct, loss and the confusion matrix and are never invalid; the loss slot adds
-// w[y] * l_p.  VP = 8: the 8-channel kernel and layout.
-cudaError_t seg_eval_metrics_opt(const void* logits, const int* labels, const int* n_valid,
-                                 double* acc, double* scratch, unsigned int* counter, int images,
-                                 long long ppi, int VP, int V, SegLossOpts o, cudaStream_t s);
-// seg_predict_wide: mask[p] = the class (seg_wide.cuh) and, when out is not null,
-// out[p * V + j] = the fp32 value of channel j < V.  One pass; any pixel count.
-cudaError_t seg_predict_wide(const void* logits, uint8_t* mask, float* out, long long pixels,
-                             int VP, int V, cudaStream_t s);
+cudaError_t seg_eval_metrics(const void* logits, const int* labels, const int* n_valid,
+                             double* acc, double* scratch, unsigned int* counter, int images,
+                             long long ppi, int VP, int V, const SegLossOpts* opts,
+                             cudaStream_t s);
+// seg_predict (serving): pixels [0, pixels) of bf16 logits [pixels, VP] (VP as for pixel_xent) ->
+// mask[p] = the class seg_eval_metrics / pixel_xent predict (seg_wide.cuh: lowest index among the
+// maxima of channels [0, V)) and, when out is not null, out[p * V + j] = the fp32 value of
+// channel j < V.  One pass; any pixel count; mask and out must be 16-byte aligned.
+cudaError_t seg_predict(const void* logits, uint8_t* mask, float* out, long long pixels, int VP,
+                        int V, cudaStream_t s);
 
 }  // namespace tfos

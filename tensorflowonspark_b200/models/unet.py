@@ -556,11 +556,10 @@ class UNetTrainer(object):
     if self.loss_opts:   # the denominator sum_S w[y] of this batch's labels, on the device
       K.seg_label_norm(self.labels, self.loss_norm, self._norm_scratch, self.classes,
                        self.ignore_index, self.weights)
-      K.pixel_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
-                   self.classes, 1.0 / npix, self.ignore_index, self.weights, self.loss_norm)
-    else:
-      K.pixel_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
-                   self.classes, 1.0 / npix)
+    # without options ignore_index and weights are None and the scale is the host's 1 / npix
+    K.pixel_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
+                 self.classes, 1.0 / npix, self.ignore_index, self.weights,
+                 self.loss_norm if self.loss_opts else None)
     self.optim.zero_grads()
     self.p_last_wgrad.run()
     K.colsum(self.dlogits, self.store.g(self.s_last_b))
@@ -810,12 +809,8 @@ class _SegEvaluator(object):
   def _run(self):
     net = self.net
     net._forward(False, self.u8, self.bn)
-    if net.loss_opts:
-      ops.K.seg_eval_metrics(net.logits, self.labels, self.n_valid, self.acc, self.partial,
-                             self.counter, self.V, net.ignore_index, net.weights)
-    else:
-      ops.K.seg_eval_metrics(net.logits, self.labels, self.n_valid, self.acc, self.partial,
-                             self.counter, self.V)
+    ops.K.seg_eval_metrics(net.logits, self.labels, self.n_valid, self.acc, self.partial,
+                           self.counter, self.V, net.ignore_index, net.weights)
 
   def step(self, images_u8, masks):
     n = len(images_u8)

@@ -37,12 +37,12 @@ KERNELS = [
     ("bn_fwd_apply_finalize", r"bn_fwd_apply_kernel<true>"),
     ("bn_bwd_apply", r"bn_bwd_apply_kernel"),
     ("bn_bwd_reduce", r"bn_bwd_reduce_kernel"),
-    ("pixel_xent", r"pixel_xent_kernel("),
-    ("pixel_xent_wide_g4", r"pixel_xent_wide_kernel<4>"),
-    ("pixel_xent_wide_g32", r"pixel_xent_wide_kernel<32>"),
-    ("seg_eval_metrics", r"seg_eval_metrics_kernel("),
-    ("seg_eval_wide_g4", r"seg_eval_wide_kernel<4>"),
-    ("seg_eval_wide_g32", r"seg_eval_wide_kernel<32>"),
+    ("pixel_xent", r"pixel_xent_kernel<false>("),
+    ("pixel_xent_wide_g4", r"pixel_xent_wide_kernel<4, false>"),
+    ("pixel_xent_wide_g32", r"pixel_xent_wide_kernel<32, false>"),
+    ("seg_eval_metrics", r"seg_eval_metrics_kernel<false>("),
+    ("seg_eval_wide_g4", r"seg_eval_wide_kernel<4, false>"),
+    ("seg_eval_wide_g32", r"seg_eval_wide_kernel<32, false>"),
 ]
 KEY = ("HGMMA", "UTMALDG", "WARPGROUP", "LDGMC", "SYNCS", "HMMA", "RED", "ATOM", "ST.E", "STG", "LDG")
 
