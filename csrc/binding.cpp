@@ -5,6 +5,7 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
+#include <cmath>
 #include <cstdint>
 #include <cstring>
 #include <string>
@@ -418,7 +419,11 @@ void avgpool_bwd(const Tensor& dy, Tensor dx) {
         "avgpool_bwd");
 }
 void softmax_xent(const Tensor& logits, const Tensor& labels, c10::optional<Tensor> dlogits,
-                  Tensor loss_sum, c10::optional<Tensor> correct, int V, double scale) {
+                  Tensor loss_sum, c10::optional<Tensor> correct, int V, double scale,
+                  double label_smoothing) {
+  if (!(std::isfinite(label_smoothing) && label_smoothing >= 0.0 && label_smoothing <= 1.0))
+    throw py::value_error("softmax_xent: label_smoothing must be in [0, 1], got " +
+                          std::to_string(label_smoothing));
   TORCH_CHECK(logits.is_cuda() && logits.is_contiguous(), "logits");
   need(labels, torch::kInt32, "labels");
   const int ld = logits.size(-1);
@@ -434,7 +439,7 @@ void softmax_xent(const Tensor& logits, const Tensor& labels, c10::optional<Tens
   }
   check(tfos::softmax_xent(logits.data_ptr(), fp32 ? 1 : 0, labels.data_ptr<int>(), dl,
                            loss_sum.data_ptr<float>(), optf(correct), rows, V, ld, ldd, scale,
-                           cur_stream()),
+                           static_cast<float>(label_smoothing), cur_stream()),
         "softmax_xent");
 }
 void decode_normalize(const Tensor& in, Tensor out, int wofs, std::vector<double> mean,
@@ -980,7 +985,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("maxpool_bwd", &maxpool_bwd);
   m.def("avgpool_fwd", &avgpool_fwd);
   m.def("avgpool_bwd", &avgpool_bwd);
-  m.def("softmax_xent", &softmax_xent);
+  m.def("softmax_xent", &softmax_xent, py::arg("logits"), py::arg("labels"), py::arg("dlogits"),
+        py::arg("loss_sum"), py::arg("correct"), py::arg("V"), py::arg("scale"),
+        py::arg("label_smoothing") = 0.0);
   m.def("decode_normalize", &decode_normalize);
   m.def("cast_f32_bf16", &cast_f32_bf16);
   m.def("bn_fold", &bn_fold);

@@ -455,6 +455,10 @@ avgpool_bwd_kernel(const __nv_bfloat16* __restrict__ dy, __nv_bfloat16* __restri
 // One block per row: loss_sum += -log softmax(logits)[label] * scale and
 // dlogits = (softmax - onehot) * scale.  Rows = samples (classification) or
 // pixels (segmentation); ld = row pitch of logits/dlogits in elements.
+// Smooth: the target is (1 - eps) * onehot + eps / V over the V real classes, as in
+// F.cross_entropy(label_smoothing=eps): loss = lse - (1 - eps) l_y - (eps / V) sum_j l_j, written
+// relative to the row maximum, and dlogits = (softmax - (1 - eps) onehot - eps / V) * scale.  The
+// sum of the logits is reduced next to the exponential sum (one pass over the row).
 template <typename T>
 __device__ __forceinline__ float ld_logit(const T* p);
 template <>
@@ -464,11 +468,11 @@ __device__ __forceinline__ float ld_logit<__nv_bfloat16>(const __nv_bfloat16* p)
   return __bfloat162float(*p);
 }
 
-template <typename T>
+template <typename T, bool Smooth>
 __global__ void __launch_bounds__(128)
 softmax_xent_kernel(const T* __restrict__ logits, const int* __restrict__ labels,
                     __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
-                    int V, int ld, int ldd, float scale) {
+                    int V, int ld, int ldd, float scale, float eps) {
   const long long row = blockIdx.x;
   const T* l = logits + row * ld;
   __shared__ float red[4];
@@ -491,24 +495,48 @@ softmax_xent_kernel(const T* __restrict__ logits, const int* __restrict__ labels
     if (red[w] > mx || (red[w] == mx && redi[w] < amax)) mx = red[w], amax = redi[w];
   __syncthreads();
   float se = 0.f;
-  for (int j = threadIdx.x; j < V; j += blockDim.x) se += __expf(ld_logit(l + j) - mx);
+  [[maybe_unused]] float sd = 0.f;   // Smooth: sum_j (l_j - max)
+  for (int j = threadIdx.x; j < V; j += blockDim.x) {
+    const float v = ld_logit(l + j) - mx;
+    se += __expf(v);
+    if constexpr (Smooth) sd += v;
+  }
   for (int o = 16; o >= 1; o >>= 1) se += __shfl_xor_sync(0xffffffff, se, o);
+  if constexpr (Smooth) {
+    for (int o = 16; o >= 1; o >>= 1) sd += __shfl_xor_sync(0xffffffff, sd, o);
+    // redi is free again: every thread read it before the barrier above
+    if ((threadIdx.x & 31) == 0) redi[threadIdx.x >> 5] = __float_as_int(sd);
+  }
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = se;
   __syncthreads();
   se = red[0] + red[1] + red[2] + red[3];
+  if constexpr (Smooth)
+    sd = __int_as_float(redi[0]) + __int_as_float(redi[1]) + __int_as_float(redi[2]) +
+         __int_as_float(redi[3]);
   const int label = labels[row];
   const float inv = 1.f / se;
   if (dlogits != nullptr) {
     __nv_bfloat16* d = dlogits + row * ldd;
+    [[maybe_unused]] const float off = eps / static_cast<float>(V), on = 1.f - eps + off;
     for (int j = threadIdx.x; j < ldd; j += blockDim.x) {
       float g = 0.f;
-      if (j < V) g = (__expf(ld_logit(l + j) - mx) * inv - (j == label ? 1.f : 0.f)) * scale;
+      if constexpr (Smooth) {
+        if (j < V) g = (__expf(ld_logit(l + j) - mx) * inv - (j == label ? on : off)) * scale;
+      } else {
+        if (j < V) g = (__expf(ld_logit(l + j) - mx) * inv - (j == label ? 1.f : 0.f)) * scale;
+      }
       d[j] = __float2bfloat16_rn(g);
     }
   }
   if (threadIdx.x == 0) {
-    const float lp = ld_logit(l + label) - mx - __logf(se);
-    atomicAdd(loss_sum, -lp * scale);
+    if constexpr (Smooth) {
+      const float loss = __logf(se) - (1.f - eps) * (ld_logit(l + label) - mx) -
+                         eps / static_cast<float>(V) * sd;
+      atomicAdd(loss_sum, loss * scale);
+    } else {
+      const float lp = ld_logit(l + label) - mx - __logf(se);
+      atomicAdd(loss_sum, -lp * scale);
+    }
     if (correct_sum != nullptr && amax == label) atomicAdd(correct_sum, 1.f);
   }
 }
@@ -914,15 +942,22 @@ cudaError_t avgpool_bwd(const void* dy, void* dx, int N, int HW, int C, cudaStre
 }
 cudaError_t softmax_xent(const void* logits, int logits_fp32, const int* labels, void* dlogits,
                          float* loss_sum, float* correct_sum, long long rows, int V, int ld,
-                         int ldd, float scale, cudaStream_t s) {
-  if (logits_fp32)
-    softmax_xent_kernel<float><<<static_cast<unsigned>(rows), 128, 0, s>>>(
-        static_cast<const float*>(logits), labels, static_cast<__nv_bfloat16*>(dlogits), loss_sum,
-        correct_sum, V, ld, ldd, scale);
-  else
-    softmax_xent_kernel<__nv_bfloat16><<<static_cast<unsigned>(rows), 128, 0, s>>>(
-        static_cast<const __nv_bfloat16*>(logits), labels, static_cast<__nv_bfloat16*>(dlogits),
-        loss_sum, correct_sum, V, ld, ldd, scale);
+                         int ldd, float scale, float label_smoothing, cudaStream_t s) {
+  auto launch = [&](auto kernel, auto* l) {
+    kernel<<<static_cast<unsigned>(rows), 128, 0, s>>>(
+        l, labels, static_cast<__nv_bfloat16*>(dlogits), loss_sum, correct_sum, V, ld, ldd, scale,
+        label_smoothing);
+  };
+  const bool smooth = label_smoothing != 0.f;
+  if (logits_fp32) {
+    const float* l = static_cast<const float*>(logits);
+    if (smooth) launch(softmax_xent_kernel<float, true>, l);
+    else launch(softmax_xent_kernel<float, false>, l);
+  } else {
+    const __nv_bfloat16* l = static_cast<const __nv_bfloat16*>(logits);
+    if (smooth) launch(softmax_xent_kernel<__nv_bfloat16, true>, l);
+    else launch(softmax_xent_kernel<__nv_bfloat16, false>, l);
+  }
   TFOS_RET();
 }
 cudaError_t decode_normalize(const uint8_t* in, void* out, int N, int H, int W, int C, int Wp,

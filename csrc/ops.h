@@ -60,9 +60,12 @@ cudaError_t maxpool_bwd(const void* dy, const uint8_t* idx, void* dx, int N, int
                         int OH, int OW, int k, int stride, int pad, cudaStream_t s);
 cudaError_t avgpool_fwd(const void* x, void* y, int N, int HW, int C, cudaStream_t s);
 cudaError_t avgpool_bwd(const void* dy, void* dx, int N, int HW, int C, cudaStream_t s);
+// softmax_xent: label_smoothing = 0 runs the plain cross-entropy instance; in (0, 1] the smoothed
+// one (target (1 - eps) onehot + eps / V over the V real classes).  Columns [V, ldd) of dlogits
+// are written as 0.
 cudaError_t softmax_xent(const void* logits, int logits_fp32, const int* labels, void* dlogits,
                          float* loss_sum, float* correct_sum, long long rows, int V, int ld,
-                         int ldd, float scale, cudaStream_t s);
+                         int ldd, float scale, float label_smoothing, cudaStream_t s);
 cudaError_t decode_normalize(const uint8_t* in, void* out, int N, int H, int W, int C, int Wp,
                              int Cp, int wofs, const float* mean3, const float* istd3,
                              cudaStream_t s);

@@ -39,6 +39,9 @@ def define_flags():
                  help="fused_p2p: all-reduce + momentum-SGD in one kernel over NVLink peer memory")
   p.add_argument("--num_packs", type=int, default=1, help="gradient buckets overlapped with backward")
   p.add_argument("--no_graph", action="store_true", help="do not capture the step in a CUDA graph")
+  p.add_argument("--label_smoothing", type=float, default=0.0,
+                 help="eps of the training loss's label smoothing, in [0, 1] (evaluation reports "
+                      "the plain cross-entropy)")
   return p
 
 
@@ -77,8 +80,9 @@ def main_fun(argv, ctx):
   comm = ctx.gradient_comm() if world > 1 else None
   B = args.batch_size
   from tensorflowonspark_b200.utils import fault
+  smooth = {"label_smoothing": args.label_smoothing} if args.label_smoothing else {}
   net = resnet.CifarResNetTrainer(depth=args.resnet_size, batch=B, device=dev, comm=comm,
-                                  lr=resnet.piecewise_lr(0, B * world))
+                                  lr=resnet.piecewise_lr(0, B * world), **smooth)
   if comm is not None:
     comm.broadcast("weights", root=0)   # the chief's initial variables win
     comm.broadcast("aux32", root=0)

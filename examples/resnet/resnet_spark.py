@@ -19,6 +19,13 @@ Held-out evaluation: ``--eval_steps N`` scores N synthetic ImageNet-shaped batch
 last step (``K = 0``: only after the last step), through the trainer's folded forward pass on its
 own buffers (``ResNetTrainer.evaluate``).  The totals are summed over all ranks; the eval fields
 go to the JSONL metrics, TensorBoard and the Prometheus exporter next to the training fields.
+
+Own label sets: ``--num_classes V`` (any V >= 1), ``--label_smoothing 0.1`` (the published
+large-batch ResNet-50 recipes), and ``--init_checkpoint DIR`` to fine-tune from another run's
+backbone (``ResNetTrainer.load_backbone``: a fresh head, the optimizer state starts at zero):
+
+  python examples/resnet/resnet_spark.py --num_classes 37 --label_smoothing 0.1 \
+      --init_checkpoint /ckpt/imagenet --model_dir /ckpt/pets
 """
 import argparse
 import os
@@ -53,6 +60,14 @@ def parse(argv):
                  help="evaluate every K steps (0: only after the last step)")
   p.add_argument("--metrics_port", type=int, default=None,
                  help="serve the same fields on a Prometheus /metrics endpoint (port + rank; 0: any free port)")
+  p.add_argument("--num_classes", type=int, default=None,
+                 help="classes of the head, any count >= 1 (default: 1000; resnet56: 10)")
+  p.add_argument("--label_smoothing", type=float, default=0.0,
+                 help="eps of the training loss's label smoothing, in [0, 1]")
+  p.add_argument("--init_checkpoint", default=None,
+                 help="model_dir of an earlier run of the same model, any class count: start from "
+                      "the backbone of its newest checkpoint with a new head (only when --model_dir "
+                      "has nothing to resume from)")
   return p.parse_args(argv)
 
 
@@ -72,6 +87,10 @@ def main_fun(argv, ctx):
   else:
     base_lr = args.base_lr if args.base_lr is not None else 0.1 * B * ctx.world_size / 256.0
   opt = dict(optimizer=args.optimizer, trust_coefficient=args.trust_coefficient) if lars else {}
+  if args.num_classes is not None:
+    opt["num_classes"] = args.num_classes
+  if args.label_smoothing:
+    opt["label_smoothing"] = args.label_smoothing
   if args.model == "resnet56":
     net = resnet.CifarResNetTrainer(depth=56, batch=B, device="cuda:0", comm=comm, lr=base_lr, **opt)
   else:
@@ -81,13 +100,19 @@ def main_fun(argv, ctx):
   if comm is not None:
     comm.broadcast("weights", root=0)   # the chief's initial variables win
     comm.broadcast("aux32", root=0)
-  start = 0
+  start, state = 0, None
   if args.model_dir:
     start, state = checkpoint.load(ctx.absolute_path(args.model_dir))
     if state is not None:
       net.load_state_dict(state["params"])      # parameters + batch-norm running statistics
       net.optim.load_state_dict(state["optim"])
       print("resumed from step", start)
+  if args.init_checkpoint and state is None:
+    init_step, init = checkpoint.load(ctx.absolute_path(args.init_checkpoint))
+    if init is None:
+      raise ValueError("--init_checkpoint {}: no checkpoint there".format(args.init_checkpoint))
+    net.load_backbone(init["params"])           # every parameter but the head + running statistics
+    print("backbone from {} (step {})".format(args.init_checkpoint, init_step))
   x, y = net.synthetic_batch(seed=ctx.rank)
   net.set_input(x, y)
   net.train_step()

@@ -8,6 +8,7 @@ Keras model (examples/resnet/resnet_cifar_dist.py:208, momentum SGD with a
 piecewise schedule :35-66); BASELINE.json names ResNet-50/ImageNet-shaped data
 as the headline config.  Both are provided here.
 """
+import numbers
 import os
 
 import torch
@@ -33,6 +34,33 @@ class _Block(object):
 
 def _buf(shape, device, dtype=torch.bfloat16):
   return torch.zeros(shape, dtype=dtype, device=device)
+
+
+def _check_head_args(num_classes, label_smoothing):
+  """(num_classes, label_smoothing) as (int, float); ValueError unless num_classes is an int >= 1
+  and label_smoothing a real number in [0, 1].  The trainers call it before they allocate."""
+  if isinstance(num_classes, bool) or not isinstance(num_classes, numbers.Integral) \
+      or num_classes < 1:
+    raise ValueError("num_classes must be an int >= 1, got {!r}".format(num_classes))
+  if isinstance(label_smoothing, bool) or not isinstance(label_smoothing, numbers.Real) \
+      or not 0.0 <= float(label_smoothing) <= 1.0:     # NaN fails the comparison too
+    raise ValueError("label_smoothing must be a real number in [0, 1], got {!r}".format(
+        label_smoothing))
+  return int(num_classes), float(label_smoothing)
+
+
+def _padded_head_init(V, std=0.01):
+  """Initialiser of a classifier weight padded to ceil(V / 8) * 8 rows: the V real rows are drawn
+  as ``normal(std)`` draws an unpadded [V, K] weight, the padding rows are zero.  Their logits are
+  then 0 and their gradient, momentum and share of LARS's ||w|| stay exactly zero."""
+  def init(shape, gen):
+    w = torch.zeros(shape)
+    w[:V] = torch.randn((V,) + tuple(shape[1:]), generator=gen) * std
+    return w
+  return init
+
+
+_HEAD = ("fc.w", "fc.b")   # the classifier: what load_backbone leaves out
 
 
 # columns of the bn_fold table (csrc/ops.h kFold*)
@@ -165,9 +193,16 @@ class ResNetTrainer(object):
 
   def __init__(self, depth=50, batch=256, image=224, num_classes=1000, device="cuda:0",
                lr=0.1, momentum=0.9, weight_decay=1e-4, comm=None, training=True, seed=1234,
-               optimizer="momentum", trust_coefficient=0.001):
+               optimizer="momentum", trust_coefficient=0.001, label_smoothing=0.0):
     """``optimizer``: sgd | momentum | adam | lars (``trust_coefficient`` is LARS's eta; see
-    parallel/fused_optim.py)."""
+    parallel/fused_optim.py).
+
+    ``num_classes``: any int >= 1.  The head has ``VP = ceil(num_classes / 8) * 8`` rows; the
+    padding rows start at zero and stay zero, and the loss, evaluation and serving read only the
+    first ``num_classes`` logits.  ``label_smoothing`` (eps in [0, 1]): the training loss is the
+    cross-entropy against (1 - eps) * onehot + eps / num_classes, as
+    ``F.cross_entropy(label_smoothing=eps)``; evaluation reports the plain cross-entropy."""
+    num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     assert depth in self.CFG, "bottleneck depths: 50/101/152"
     self.device = torch.device(device)
     self.B, self.image, self.num_classes, self.depth = batch, image, num_classes, depth
@@ -195,7 +230,9 @@ class ResNetTrainer(object):
         b.stride, b.cin, b.width, b.name = stride, cin, width, name
         self.blocks.append(b)
         cin = width * 4
-    self.fc = Dense(st, "fc", cin, num_classes, bias=True, init=normal(0.01))
+    VP = self.VP = (num_classes + 7) // 8 * 8
+    self.fc = Dense(st, "fc", cin, VP, bias=True,
+                    init=normal(0.01) if VP == num_classes else _padded_head_init(num_classes))
     self.feat = cin
 
     alloc = comm.alloc if comm is not None else None
@@ -280,16 +317,13 @@ class ResNetTrainer(object):
     self.last = x
     self.g_last = gx
     self.avg = _buf((B, self.feat), dev)
-    self.logits = _buf((B, num_classes), dev, torch.float32)
-    self.ldd = (num_classes + 7) // 8 * 8
-    self.dlogits = _buf((B, self.ldd), dev) if tr else None
+    self.logits = _buf((B, VP), dev, torch.float32)
+    self.ldd = VP
+    self.dlogits = _buf((B, VP), dev) if tr else None
     self.g_avg = _buf((B, self.feat), dev) if tr else None
     self.loss_sum = torch.zeros(1, dtype=torch.float32, device=dev)
     self.correct = torch.zeros(1, dtype=torch.float32, device=dev)
-    dl = self.dlogits[:, :num_classes] if (tr and self.ldd == num_classes) else None
-    if tr and dl is None:
-      raise ValueError("num_classes must be a multiple of 8 (pad the head)")
-    self.fc.build(self.avg, self.logits, dl, self.g_avg, training=tr)
+    self.fc.build(self.avg, self.logits, self.dlogits, self.g_avg, training=tr)
 
     self.optim = None
     if tr:
@@ -436,7 +470,8 @@ class ResNetTrainer(object):
     self.loss_sum.zero_()
     self.correct.zero_()
     ops.K.softmax_xent(self.logits, self.labels, self.dlogits if with_grad else None,
-                       self.loss_sum, self.correct, self.num_classes, 1.0 / self.B)
+                       self.loss_sum, self.correct, self.num_classes, 1.0 / self.B,
+                       label_smoothing=self.label_smoothing)
 
   # -------------------------------------------------------------- backward
   def _backward(self):
@@ -618,8 +653,10 @@ class ResNetTrainer(object):
 
   def eval_end(self):
     """Totals summed over all ranks (identical on every rank): {"count", "loss", "top1", "top5"};
-    the last three are means over ``count`` (NaN when it is 0).  Raises ValueError on every rank
-    when any rank saw a label outside [0, num_classes)."""
+    the last three are means over ``count`` (NaN when it is 0).  ``loss`` is the plain
+    cross-entropy whatever the trainer's ``label_smoothing``, so that scores of runs with different
+    smoothing compare.  Raises ValueError on every rank when any rank saw a label outside
+    [0, num_classes)."""
     return self._eval_state().end()
 
   def evaluate(self, batches):
@@ -661,6 +698,29 @@ class ResNetTrainer(object):
     if running is not None:
       self.running.tensor().copy_(running.to(self.device))
 
+  def load_backbone(self, state):
+    """Start from a trained backbone: ``state`` is the ``state_dict()`` of a trainer of the same
+    depth with any class count.  Loads every parameter except the classifier (``fc.w``, ``fc.b``)
+    and the batch-norm running statistics (``__running__``), like ``load_state_dict``; the head
+    keeps its seeded initialisation and the optimizer state is untouched.  Every tensor is checked
+    before anything is copied: a missing, unexpected or wrongly shaped one raises ValueError and
+    leaves the trainer as it was."""
+    want = {s["name"]: s["shape"] for s in self.store.order if s["name"] not in _HEAD}
+    want["__running__"] = tuple(self.running.tensor().shape)
+    extra = sorted(set(state) - set(want) - set(_HEAD))
+    if extra:
+      raise ValueError("load_backbone: {} is not a tensor of this trainer (another depth?)".format(
+          extra[0]))
+    for name, shape in want.items():
+      if name not in state:
+        raise ValueError("load_backbone: {} {} is missing from the state (another depth?)".format(
+            name, shape))
+      got = tuple(state[name].shape)
+      if got != shape:
+        raise ValueError("load_backbone: {} has shape {} in the state, {} in this trainer".format(
+            name, got, shape))
+    self.load_state_dict({k: v for k, v in state.items() if k not in _HEAD})
+
 
 class ServedResNet(serving.Replica):
   """Inference callable behind ``pipeline.TFModel`` / ``TFParallel``: one bf16 replica on the
@@ -699,11 +759,13 @@ def build_served(state, depth=50, image=224, num_classes=1000, batch=None, **_):
 class CifarResNetTrainer(object):
   """ResNet-20/32/56 for 32x32 inputs (basic blocks, 16/32/64 channels) - the network the
   reference example actually trains (examples/resnet/resnet_cifar_dist.py:208, ``resnet56``,
-  momentum SGD, batch 128, weight decay 2e-4)."""
+  momentum SGD, batch 128, weight decay 2e-4).  ``num_classes`` and ``label_smoothing`` as in
+  ResNetTrainer."""
 
   def __init__(self, depth=56, batch=128, num_classes=10, device="cuda:0", lr=0.1, momentum=0.9,
                weight_decay=2e-4, comm=None, seed=1234, optimizer="momentum",
-               trust_coefficient=0.001):
+               trust_coefficient=0.001, label_smoothing=0.0):
+    num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     assert (depth - 2) % 6 == 0
     n = (depth - 2) // 6
     self.device = dev = torch.device(device)
@@ -774,6 +836,7 @@ class CifarResNetTrainer(object):
   synthetic_batch = ResNetTrainer.synthetic_batch
   state_dict = ResNetTrainer.state_dict
   load_state_dict = ResNetTrainer.load_state_dict
+  load_backbone = ResNetTrainer.load_backbone
   set_input = ResNetTrainer.set_input
   capture = ResNetTrainer.capture
   train_step = ResNetTrainer.train_step
@@ -835,7 +898,7 @@ class CifarResNetTrainer(object):
     self.loss_sum.zero_()
     self.correct.zero_()
     K.softmax_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
-                   self.num_classes, 1.0 / self.B)
+                   self.num_classes, 1.0 / self.B, label_smoothing=self.label_smoothing)
     self.optim.zero_grads()
     self.fc.backward()
     K.avgpool_bwd(self.g_avg, self.g_last)

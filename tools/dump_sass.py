@@ -43,6 +43,8 @@ KERNELS = [
     ("seg_eval_metrics", r"seg_eval_metrics_kernel<false>("),
     ("seg_eval_wide_g4", r"seg_eval_wide_kernel<4, false>"),
     ("seg_eval_wide_g32", r"seg_eval_wide_kernel<32, false>"),
+    ("softmax_xent", r"softmax_xent_kernel<float, false>("),
+    ("softmax_xent_smooth", r"softmax_xent_kernel<float, true>("),
 ]
 KEY = ("HGMMA", "UTMALDG", "WARPGROUP", "LDGMC", "SYNCS", "HMMA", "RED", "ATOM", "ST.E", "STG", "LDG")
 
