@@ -781,6 +781,8 @@ void allreduce_opt(const py::dict& d) {
   a.lars_t0 = geti<int>(d, "lars_t0", 0);
   a.lars_nt = geti<int>(d, "lars_nt", 0);
   a.lars_T = geti<int>(d, "lars_T", 0);
+  // weight average: selects the averaging instances; hyper must then hold tfos::kHyperEma floats
+  a.ema = reinterpret_cast<float*>(geti<uint64_t>(d, "ema", 0));
   const int opt = geti<int>(d, "opt", 0);
   const int grid = geti<int>(d, "grid", 32);
   check(tfos::allreduce_opt(a, opt, grid, cur_stream(), geti<int>(d, "phase", 0)), "allreduce_opt");

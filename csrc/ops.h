@@ -136,9 +136,16 @@ struct AllreduceOptArgs {
   const long long* lars_off;
   const float* lars_norms;
   int lars_t0, lars_nt, lars_T;
+  // Weight average (optional; last so that the fields above keep their parameter offsets).
+  // fp32, indexed shard-locally like state1; hyper then has kHyperEma slots: [8] = decay d,
+  // [9] = updates since the average was reset, counted before the launch.  After update 1 the
+  // average is the master, after each later one d * avg + (1 - d) * master.
+  float* ema;
 };
+constexpr int kHyper = 8, kHyperEma = 10;
 // phase: 0 = fused; 1 = intra-host reduce-scatter only; 2 = update + all-gather only (optim_comm.cu)
 // kOptLars with world > 1 runs as phase 1 -> lars_norms -> phase 2 (phase 0 is refused)
+// a.ema != nullptr selects the averaging instances of phases 0 and 2 (phase 1 does not update)
 cudaError_t allreduce_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStream_t s, int phase = 0);
 
 // LARS per-tensor norms of one rank's shard of one bucket (deterministic: no float atomics).

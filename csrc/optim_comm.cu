@@ -111,10 +111,13 @@ __device__ __forceinline__ float lars_update(float w, float g, float& v, const f
 // the rank's OWN gradient buffer - peers only ever read the other shards of it); 2 = update +
 // all-gather only (the gradient comes from the own buffer, which by then holds the sum over all
 // hosts; new weights go to every local peer).  0 = both in one pass (one host).
-template <int OPT, bool MULTIMEM, int PHASE = 0>
+// EMA: also fold the updated master into the shard's weight average (AllreduceOptArgs::ema) while
+// it is in registers - one extra fp32 load and store per element.
+template <int OPT, bool MULTIMEM, int PHASE = 0, bool EMA = false>
 __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOptArgs a) {
-  __shared__ float h[8];
-  if (threadIdx.x < 8) h[threadIdx.x] = a.hyper[threadIdx.x];
+  constexpr int kH = EMA ? kHyperEma : kHyper;
+  __shared__ float h[kH];
+  if (threadIdx.x < kH) h[threadIdx.x] = a.hyper[threadIdx.x];
   const int world = a.world, rank = a.rank;
   uint32_t e = 0;
   if (world > 1) {
@@ -157,8 +160,9 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
   const long long hi = a.begin + min(n, chunk * (rank + 1));
 
   // NVLS: a thread keeps kU x 2 = 16 multimem.ld_reduce (16 bytes each, reduced in the switch) in
-  // flight; the peer-to-peer path already has 2 x world loads per element group in flight
-  constexpr int kU = MULTIMEM ? 8 : 1;
+  // flight; the peer-to-peer path already has 2 x world loads per element group in flight.  With
+  // the weight average 8 (the average's registers would otherwise spill at the 128-register bound)
+  constexpr int kU = MULTIMEM ? (EMA ? 4 : 8) : 1;
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x * 8;
   for (long long i0 = lo + (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 8;
        i0 < hi; i0 += stride * kU) {
@@ -295,6 +299,24 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
             st_relaxed_sys_v4(dst + 4, hi4);
           }
         }
+    }
+    if constexpr (EMA) {
+      // Keras's rule: the first update after a reset copies the master, each later one decays
+      float av[8];
+      if (h[9] > 1.5f) {
+        const float4 a0 = *reinterpret_cast<const float4*>(a.ema + li);
+        const float4 a1 = *reinterpret_cast<const float4*>(a.ema + li + 4);
+        av[0] = a0.x, av[1] = a0.y, av[2] = a0.z, av[3] = a0.w;
+        av[4] = a1.x, av[5] = a1.y, av[6] = a1.z, av[7] = a1.w;
+        const float d = h[8], om = 1.f - h[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) av[j] = fmaf(d, av[j], om * w[j]);
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) av[j] = w[j];
+      }
+      *reinterpret_cast<float4*>(a.ema + li) = make_float4(av[0], av[1], av[2], av[3]);
+      *reinterpret_cast<float4*>(a.ema + li + 4) = make_float4(av[4], av[5], av[6], av[7]);
     }
     if (a.zero_grads && world == 1) {
       *reinterpret_cast<float4*>(a.grads[0] + i) = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -687,21 +709,22 @@ __global__ void __launch_bounds__(512) ps_pull_model_kernel(const PsPullArgs a) 
   }
 }
 
-template <int OPT>
+template <int OPT, bool EMA>
 cudaError_t launch_ar(const AllreduceOptArgs& a, int grid, cudaStream_t s, int phase) {
   if (phase == 1)   // (the reduce-scatter half does not depend on the optimizer)
     allreduce_opt_kernel<kOptSgd, false, 1><<<grid, 512, 0, s>>>(a);
   else if (phase == 2)
-    allreduce_opt_kernel<OPT, false, 2><<<grid, 512, 0, s>>>(a);
+    allreduce_opt_kernel<OPT, false, 2, EMA><<<grid, 512, 0, s>>>(a);
   else if (a.grads_mc != nullptr && a.weights_mc != nullptr && a.world > 1)
-    allreduce_opt_kernel<OPT, true><<<grid, 512, 0, s>>>(a);
+    allreduce_opt_kernel<OPT, true, 0, EMA><<<grid, 512, 0, s>>>(a);
   else
-    allreduce_opt_kernel<OPT, false><<<grid, 512, 0, s>>>(a);
+    allreduce_opt_kernel<OPT, false, 0, EMA><<<grid, 512, 0, s>>>(a);
   return cudaGetLastError();
 }
 
 // LARS needs whole-tensor norms of the reduced gradient between the two halves, so with peers it
 // always runs split; on a one-host NVLS communicator both halves use the multicast paths
+template <bool EMA>
 cudaError_t launch_lars(const AllreduceOptArgs& a, int grid, cudaStream_t s, int phase) {
   if (a.lars_nt < 0 || a.lars_nt > kLarsMaxTensors) return cudaErrorInvalidValue;
   if (a.lars_nt > 0 && (a.lars_off == nullptr || a.lars_norms == nullptr))
@@ -714,15 +737,26 @@ cudaError_t launch_lars(const AllreduceOptArgs& a, int grid, cudaStream_t s, int
       allreduce_opt_kernel<kOptSgd, false, 1><<<grid, 512, 0, s>>>(a);
   } else if (phase == 2) {
     if (nvls)
-      allreduce_opt_kernel<kOptLars, true, 2><<<grid, 512, 0, s>>>(a);
+      allreduce_opt_kernel<kOptLars, true, 2, EMA><<<grid, 512, 0, s>>>(a);
     else
-      allreduce_opt_kernel<kOptLars, false, 2><<<grid, 512, 0, s>>>(a);
+      allreduce_opt_kernel<kOptLars, false, 2, EMA><<<grid, 512, 0, s>>>(a);
   } else if (a.world == 1) {
-    allreduce_opt_kernel<kOptLars, false><<<grid, 512, 0, s>>>(a);
+    allreduce_opt_kernel<kOptLars, false, 0, EMA><<<grid, 512, 0, s>>>(a);
   } else {
     return cudaErrorInvalidValue;
   }
   return cudaGetLastError();
+}
+
+template <bool EMA>
+cudaError_t launch_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStream_t s, int phase) {
+  switch (opt) {
+    case kOptSgd: return launch_ar<kOptSgd, EMA>(a, grid, s, phase);
+    case kOptMomentum: return launch_ar<kOptMomentum, EMA>(a, grid, s, phase);
+    case kOptAdam: return launch_ar<kOptAdam, EMA>(a, grid, s, phase);
+    case kOptLars: return launch_lars<EMA>(a, grid, s, phase);
+    default: return cudaErrorInvalidValue;
+  }
 }
 
 }  // namespace
@@ -730,13 +764,8 @@ cudaError_t launch_lars(const AllreduceOptArgs& a, int grid, cudaStream_t s, int
 cudaError_t allreduce_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStream_t s, int phase) {
   if (a.world < 1 || a.world > kMaxRanks) return cudaErrorInvalidValue;
   if ((a.begin & 7) != 0 || phase < 0 || phase > 2) return cudaErrorInvalidValue;
-  switch (opt) {
-    case kOptSgd: return launch_ar<kOptSgd>(a, grid, s, phase);
-    case kOptMomentum: return launch_ar<kOptMomentum>(a, grid, s, phase);
-    case kOptAdam: return launch_ar<kOptAdam>(a, grid, s, phase);
-    case kOptLars: return launch_lars(a, grid, s, phase);
-    default: return cudaErrorInvalidValue;
-  }
+  return a.ema != nullptr ? launch_opt<true>(a, opt, grid, s, phase)
+                          : launch_opt<false>(a, opt, grid, s, phase);
 }
 cudaError_t lars_norms(const LarsNormArgs& a, cudaStream_t s) {
   if (a.world < 1 || a.world > kMaxRanks || a.nseg < 0 || a.nt < 0) return cudaErrorInvalidValue;

@@ -42,6 +42,10 @@ def define_flags():
   p.add_argument("--label_smoothing", type=float, default=0.0,
                  help="eps of the training loss's label smoothing, in [0, 1] (evaluation reports "
                       "the plain cross-entropy)")
+  p.add_argument("--ema_decay", type=float, default=None,
+                 help="keep a moving average of the weights with this decay in [0, 1) and also "
+                      "evaluate it (avg_*); checkpoints keep the live weights and carry the "
+                      "average in the optimizer state")
   return p
 
 
@@ -81,6 +85,8 @@ def main_fun(argv, ctx):
   B = args.batch_size
   from tensorflowonspark_b200.utils import fault
   smooth = {"label_smoothing": args.label_smoothing} if args.label_smoothing else {}
+  if args.ema_decay is not None:
+    smooth["ema_decay"] = args.ema_decay
   net = resnet.CifarResNetTrainer(depth=args.resnet_size, batch=B, device=dev, comm=comm,
                                   lr=resnet.piecewise_lr(0, B * world), **smooth)
   if comm is not None:
@@ -127,9 +133,15 @@ def main_fun(argv, ctx):
     if ctx.is_chief:
       print("eval: epoch {} loss {:.4f} top1 {:.4f} top5 {:.4f} ({} images)".format(
           epoch, res["loss"], res["top1"], res["top5"], res["count"]))
+    scalars = {"loss": res["loss"], "accuracy": res["top1"], "top5_accuracy": res["top5"]}
+    if args.ema_decay is not None:   # the weight average on the same batches
+      avg = net.evaluate(eval_set, averaged=True)
+      if ctx.is_chief:
+        print("eval: epoch {} avg loss {:.4f} avg top1 {:.4f} avg top5 {:.4f}".format(
+            epoch, avg["loss"], avg["top1"], avg["top5"]))
+      scalars.update(avg_loss=avg["loss"], avg_accuracy=avg["top1"], avg_top5_accuracy=avg["top5"])
     if eval_events:
-      eval_events.add_scalars({"loss": res["loss"], "accuracy": res["top1"],
-                               "top5_accuracy": res["top5"]}, step)
+      eval_events.add_scalars(scalars, step)
       eval_events.flush()
 
   every = steps_per_epoch * max(1, args.epochs_between_evals)

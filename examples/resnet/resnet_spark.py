@@ -26,6 +26,11 @@ backbone (``ResNetTrainer.load_backbone``: a fresh head, the optimizer state sta
 
   python examples/resnet/resnet_spark.py --num_classes 37 --label_smoothing 0.1 \
       --init_checkpoint /ckpt/imagenet --model_dir /ckpt/pets
+
+Weight averaging: ``--ema_decay d`` also keeps an exponential moving average of the weights
+(Keras's ``use_ema``), fused into the optimizer kernels.  Every evaluation then also scores the
+average (``eval_avg_loss``, ``eval_avg_top1``, ...), and checkpoints carry it in the optimizer
+state.
 """
 import argparse
 import os
@@ -68,6 +73,11 @@ def parse(argv):
                  help="model_dir of an earlier run of the same model, any class count: start from "
                       "the backbone of its newest checkpoint with a new head (only when --model_dir "
                       "has nothing to resume from)")
+  p.add_argument("--ema_decay", type=float, default=None,
+                 help="keep a moving average of the weights with this decay in [0, 1) and also "
+                      "evaluate it (eval_avg_*); checkpoints keep the live weights (the average "
+                      "rides in the optimizer state), so serving from model_dir serves the live "
+                      "weights")
   return p.parse_args(argv)
 
 
@@ -91,6 +101,8 @@ def main_fun(argv, ctx):
     opt["num_classes"] = args.num_classes
   if args.label_smoothing:
     opt["label_smoothing"] = args.label_smoothing
+  if args.ema_decay is not None:
+    opt["ema_decay"] = args.ema_decay
   if args.model == "resnet56":
     net = resnet.CifarResNetTrainer(depth=56, batch=B, device="cuda:0", comm=comm, lr=base_lr, **opt)
   else:
@@ -139,6 +151,13 @@ def main_fun(argv, ctx):
           step, res["loss"], res["top1"], res["top5"], res["count"]))
     fields = {"eval_loss": res["loss"], "eval_top1": res["top1"], "eval_top5": res["top5"],
               "eval_count": res["count"]}
+    if args.ema_decay is not None:   # the weight average on the same batches
+      avg = net.evaluate(eval_batches, averaged=True)
+      if ctx.is_chief:
+        print("eval: step {} avg loss {:.4f} avg top1 {:.4f} avg top5 {:.4f}".format(
+            step, avg["loss"], avg["top1"], avg["top5"]))
+      fields.update(eval_avg_loss=avg["loss"], eval_avg_top1=avg["top1"],
+                    eval_avg_top5=avg["top5"])
     if log:
       log.log(step=step, **fields)
     if events:

@@ -8,6 +8,8 @@ in PASCAL VOC, Cityscapes and COCO-Stuff); ``--class_weights w0,w1,...`` weighs 
 pixels in the cross-entropy (one weight per class).
 ``--encoder_trainable_from k`` fine-tunes the encoder's blocks block_k..block_16 as well (0: the
 stem and every block), e.g. after a frozen run, resuming from its checkpoint.
+``--ema_decay d`` also keeps an exponential moving average of the weights (Keras's ``use_ema``):
+every evaluation scores it too (``val_avg_*``) and ``--export_dir`` exports it.
 Checkpoints every epoch (the reference's ModelCheckpoint callback) and evaluates every epoch on
 ``--eval_steps`` held-out synthetic batches per rank (the reference's ``validation_data``):
 validation loss, pixel accuracy and mean IoU.
@@ -43,6 +45,11 @@ def define_flags():
   p.add_argument("--encoder_trainable_from", type=int, default=None,
                  help="fine-tune the encoder too: 0 trains the stem and every block, k in 1..16 "
                       "blocks block_k..block_16 (default: frozen encoder)")
+  p.add_argument("--ema_decay", type=float, default=None,
+                 help="keep a moving average of the weights with this decay in [0, 1): each "
+                      "evaluation also scores it (val_avg_*) and --export_dir exports it; the "
+                      "checkpoints in --model_dir keep the live weights (and the average in the "
+                      "optimizer state), so serving straight from model_dir serves the live weights")
   return p
 
 
@@ -53,8 +60,8 @@ def class_weights(text):
 
 def trainer_kwargs(args):
   """Keyword arguments the trainer gets from the flags beyond the common ones: only those of the
-  options that are set (encoder fine-tuning, ignore_index, class_weights)."""
-  names = ("encoder_trainable_from", "ignore_index", "class_weights")
+  options that are set (encoder fine-tuning, ignore_index, class_weights, the weight average)."""
+  names = ("encoder_trainable_from", "ignore_index", "class_weights", "ema_decay")
   return {n: getattr(args, n) for n in names if getattr(args, n, None) is not None}
 
 
@@ -121,15 +128,24 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
     torch.cuda.synchronize()
     rate = args.steps_per_epoch * B * world / (time.time() - t0)
     res = net.evaluate([(x, labels_of(x, V)) for x in held_out]) if held_out else None  # collective
+    avg = None
+    if held_out and "ema_decay" in extra:   # the weight average's scores, also collective
+      avg = net.evaluate([(x, labels_of(x, V)) for x in held_out], averaged=True)
     if is_chief:
       line = "epoch {} loss {:.4f}".format(epoch + 1, float(loss))
       if res is not None:
         line += " val_loss {:.4f} val_accuracy {:.4f} val_mean_iou {:.4f}".format(
             res["loss"], res["accuracy"], res["mean_iou"])
+      if avg is not None:
+        line += " val_avg_loss {:.4f} val_avg_accuracy {:.4f} val_avg_mean_iou {:.4f}".format(
+            avg["loss"], avg["accuracy"], avg["mean_iou"])
       print(line + "  {:.0f} images/s".format(rate))
       if eval_events is not None:
-        eval_events.add_scalars({"loss": res["loss"], "accuracy": res["accuracy"],
-                                 "mean_iou": res["mean_iou"]}, step)
+        scalars = {"loss": res["loss"], "accuracy": res["accuracy"], "mean_iou": res["mean_iou"]}
+        if avg is not None:
+          scalars.update({"avg_loss": avg["loss"], "avg_accuracy": avg["accuracy"],
+                          "avg_mean_iou": avg["mean_iou"]})
+        eval_events.add_scalars(scalars, step)
         eval_events.flush()
       if args.model_dir:
         checkpoint.save(args.model_dir, step,
@@ -137,7 +153,8 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
   if eval_events is not None:
     eval_events.close()
   if args.export_dir and is_chief:   # servable: the artefact names unet.build_served
-    checkpoint.export_model(net, args.export_dir)
+    # with --ema_decay the average, as Keras exports after finalize_variable_values()
+    checkpoint.export_model(net.averaged() if "ema_decay" in extra else net, args.export_dir)
   return net
 
 

@@ -17,6 +17,11 @@ After the last step the chief checkpoints into ``--model_dir`` and exports into 
 (both optional); either one serves through ``pipeline.TFModel`` (``unet.ServedUNet``), see
 segmentation_inference.py.
 
+``--ema_decay d`` also keeps an exponential moving average of the weights (Keras's ``use_ema``):
+every evaluation scores it too (``val_avg_*``), and ``--export_dir`` exports the average.  The
+``--model_dir`` checkpoint holds the live parameters only (no optimizer state), so it carries
+neither the optimizer state nor the average.
+
   python examples/segmentation/segmentation_spark.py --cluster_size 8 --batch_size 64 --steps 100
 """
 import argparse
@@ -53,7 +58,8 @@ def main_fun(args, ctx):
   comm = ctx.gradient_comm() if ctx.world_size > 1 else None   # one host: P2P/NVLS kernels; several: NCCL
   B = args.batch_size
   # None: frozen encoder (as the reference), no ignored label, unweighted loss
-  extra = {n: getattr(args, n) for n in ("encoder_trainable_from", "ignore_index", "class_weights")
+  extra = {n: getattr(args, n) for n in ("encoder_trainable_from", "ignore_index", "class_weights",
+                                         "ema_decay")
            if getattr(args, n, None) is not None}
   V = getattr(args, "classes", 3)
   net = unet.UNetTrainer(batch=B, image=IMG, classes=V, device="cuda:0", lr=args.learning_rate,
@@ -71,10 +77,14 @@ def main_fun(args, ctx):
         x, _ = net.synthetic_batch(seed=EVAL_SEED + i * ctx.world_size + ctx.rank)
         held_out.append((x, unet.synthetic_labels(x, V).to(torch.uint8)))
     res = net.evaluate(held_out)   # collective: every rank evaluates
+    avg = net.evaluate(held_out, averaged=True) if "ema_decay" in extra else None
     evaluated[0] = step
     if ctx.is_chief:
       print("eval: step {} val_loss={:.4f} val_accuracy={:.4f} val_mean_iou={:.4f} ({} images)".format(
           step, res["loss"], res["accuracy"], res["mean_iou"], res["images"]), flush=True)
+      if avg is not None:
+        print("eval: step {} val_avg_loss={:.4f} val_avg_accuracy={:.4f} val_avg_mean_iou={:.4f}"
+              .format(step, avg["loss"], avg["accuracy"], avg["mean_iou"]), flush=True)
 
   def after_step(done):
     if eval_steps and eval_every and done % eval_every == 0:
@@ -153,17 +163,16 @@ def main_fun(args, ctx):
       if model_dir:
         checkpoint.save(ctx.absolute_path(model_dir), done, net.state_dict(), model=net)
       if export_dir:
-        checkpoint.export_model(net, ctx.absolute_path(export_dir))
+        # with --ema_decay the average, as Keras exports after finalize_variable_values()
+        checkpoint.export_model(net.averaged() if "ema_decay" in extra else net,
+                                ctx.absolute_path(export_dir))
     if comm is not None:
       # the chief's state_dict() reads the peers' parameter shards: they stay until it is done
       comm.barrier()
       torch.cuda.synchronize()
 
 
-if __name__ == "__main__":
-  from tensorflowonspark_b200 import TFCluster
-  from tensorflowonspark_b200._spark import SparkConf, SparkContext
-
+def define_flags():
   parser = argparse.ArgumentParser()
   parser.add_argument("--batch_size", type=int, default=64)
   parser.add_argument("--cluster_size", type=int, default=1)
@@ -190,7 +199,20 @@ if __name__ == "__main__":
   parser.add_argument("--encoder_trainable_from", type=int, default=None,
                       help="fine-tune the encoder too: 0 trains the stem and every block, k in "
                            "1..16 blocks block_k..block_16 (default: frozen encoder)")
-  args = parser.parse_args()
+  parser.add_argument("--ema_decay", type=float, default=None,
+                      help="keep a moving average of the weights with this decay in [0, 1): each "
+                           "evaluation also scores it (val_avg_*) and --export_dir exports it; "
+                           "the --model_dir checkpoint holds the live weights only (no optimizer "
+                           "state, so not the average): serving from model_dir serves the live "
+                           "weights")
+  return parser
+
+
+if __name__ == "__main__":
+  from tensorflowonspark_b200 import TFCluster
+  from tensorflowonspark_b200._spark import SparkConf, SparkContext
+
+  args = define_flags().parse_args()
   conf = SparkConf().setAppName("segmentation_spark") \
       .set("spark.executor.instances", str(args.cluster_size)) \
       .set("spark.executor.resource.gpu.amount", "1").set("spark.task.resource.gpu.amount", "1")

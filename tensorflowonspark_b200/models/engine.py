@@ -102,6 +102,43 @@ class ParamStore(object):
     self.aux32[:self.total - self.decay_end].copy_(self.master[self.decay_end:])
 
 
+class AveragedModel(object):
+  """Exportable snapshot of a trainer's weight average (``trainer.averaged()``): ``state_dict()``
+  is in the trainer's own format with every parameter replaced by its average, and the trainer's
+  export attributes come along, so ``checkpoint.export_model(view, dir)`` writes an artefact the
+  trainer's serving class loads and ``load_state_dict`` accepts."""
+
+  def __init__(self, state, trainer):
+    self._state = state
+    # (the CIFAR trainer has no serving class: like the trainer, its view exports bare state)
+    self.export_builder = getattr(trainer, "export_builder", None)
+    self.export_builder_args = dict(getattr(trainer, "export_builder_args", {}))
+    self.export_signatures = getattr(trainer, "export_signatures", None)
+
+  def state_dict(self):
+    return dict(self._state)
+
+
+def averaged_params(store, optim):
+  """({name: fp32 host tensor}, fp32 device vector) of the store's parameters taken from
+  ``optim``'s complete weight average (the current parameters before the first update after a
+  reset).  RuntimeError when there is no average."""
+  if optim is None or getattr(optim, "ema", None) is None:
+    raise RuntimeError("this trainer keeps no weight average: build it with ema_decay=d")
+  avg = optim.average_master()
+  return {s["name"]: store._view(avg, s).detach().cpu().clone() for s in store.order}, avg
+
+
+def check_ema_decay(d, training=True):
+  """Validated ``ema_decay`` of a trainer: None, or a float in [0, 1) (ValueError otherwise, and
+  for any value with ``training=False``: an inference-only trainer has no optimizer)."""
+  from ..parallel.fused_optim import check_ema_decay as check
+  d = check(d)
+  if d is not None and not training:
+    raise ValueError("ema_decay needs training=True (an inference-only trainer has no optimizer)")
+  return d
+
+
 def he_normal(fan_in):
   std = math.sqrt(2.0 / fan_in)
   return lambda shape, gen: torch.randn(shape, generator=gen) * std

@@ -126,22 +126,49 @@ class _Evaluator(object):
     else:
       self.running = comm.alloc("eval_running", net.running.used, torch.float32)
     self.rank_sum = evaluation.RankSum(comm, "eval_totals", 8)
-    self._forward = net._eval_forward(lambda spec: st._view(self.wf, spec), bias, self.u8)
-    self.graph, self.calls = None, 0
+    self._wv, self._bias = (lambda spec: st._view(self.wf, spec)), bias
+    # one forward (and graph) per model: "live" reads the head from the store, "averaged" (built
+    # on the first averaged evaluation) from a copy of the averaged head in wf / head_b
+    self._modes = {False: {"forward": net._eval_forward(self._wv, bias, self.u8), "graph": None,
+                           "calls": 0}}
+    self.averaged = False
     self.staging = evaluation.HostStaging(dev, net.B, self.u8.shape[1:], ())
 
-  def begin(self):
+  @property
+  def graph(self):
+    """The captured evaluation of the live model (None before its second batch)."""
+    return self._modes[False]["graph"]
+
+  def _averaged_mode(self):
+    net, st, fc = self.net, self.net.store, self.net.fc
+    if True not in self._modes:
+      self.head_b = torch.zeros(fc.cout, dtype=torch.float32, device=net.device)
+      head = igemm.gemm(net.avg, st._view(self.wf, fc.sw), net.logits, "nk", bias=self.head_b)
+      self._modes[True] = {"forward": net._eval_forward(self._wv, self._bias, self.u8, head.run),
+                           "graph": None, "calls": 0}
+    return fc
+
+  def begin(self, averaged=False):
+    """``averaged``: fold from the weight average (FusedOptimizer.averaged_weights(): complete
+    and identical on every rank) instead of the live weights, with the same running statistics;
+    the classifier then also runs on the averaged head."""
     net, comm = self.net, self.comm
+    st = net.store
+    weights, aux32 = net.optim.averaged_weights() if averaged else (st.weights, st.aux32)
+    self.averaged = bool(averaged)
     self.acc.zero_()
     if comm is not None:
       self.running.copy_(net.running.tensor())
       comm.broadcast("eval_running", 0)
-    st = net.store
-    ops.K.bn_fold(self.tab, self.eps, self.row0, self.rows, st.weights, st.aux32, self.running,
+    ops.K.bn_fold(self.tab, self.eps, self.row0, self.rows, weights, aux32, self.running,
                   self.wf, self.bf)
+    if averaged:   # (bn_fold writes only the convolution filters of wf: the head's rows are free)
+      fc = self._averaged_mode()
+      st._view(self.wf, fc.sw).copy_(st._view(weights, fc.sw))
+      self.head_b.copy_(st._view(aux32, fc.sbias, st.decay_end))
 
   def _run(self):
-    self._forward()
+    self._modes[self.averaged]["forward"]()
     ops.K.eval_metrics(self.net.logits, self.labels, self.n_valid, self.acc, self.V)
 
   def step(self, images_u8, labels):
@@ -153,13 +180,14 @@ class _Evaluator(object):
       self.u8[:n].copy_(x.reshape((n,) + tuple(self.u8.shape[1:])), non_blocking=True)
       self.labels[:n].copy_(torch.as_tensor(labels).reshape(n), non_blocking=True)
     self.n_valid.fill_(n)
-    if self.graph is None and self.calls >= 1:
-      self._capture()
-    if self.graph is not None:
-      self.graph.replay()
+    m = self._modes[self.averaged]
+    if m["graph"] is None and m["calls"] >= 1:
+      m["graph"] = self._capture()
+    if m["graph"] is not None:
+      m["graph"].replay()
     else:
       self._run()
-    self.calls += 1
+    m["calls"] += 1
 
   def _capture(self):
     """The evaluation forward + metric as one CUDA graph (after one eager call, like
@@ -169,7 +197,7 @@ class _Evaluator(object):
     mode = "thread_local" if getattr(self.net.optim, "group_mode", False) else "global"
     with torch.cuda.graph(g, capture_error_mode=mode):
       self._run()
-    self.graph = g
+    return g
 
   def run(self, batches):
     """eval_step over (images, labels) pairs; host batches are staged in page-locked memory one
@@ -193,9 +221,14 @@ class ResNetTrainer(object):
 
   def __init__(self, depth=50, batch=256, image=224, num_classes=1000, device="cuda:0",
                lr=0.1, momentum=0.9, weight_decay=1e-4, comm=None, training=True, seed=1234,
-               optimizer="momentum", trust_coefficient=0.001, label_smoothing=0.0):
+               optimizer="momentum", trust_coefficient=0.001, label_smoothing=0.0,
+               ema_decay=None):
     """``optimizer``: sgd | momentum | adam | lars (``trust_coefficient`` is LARS's eta; see
     parallel/fused_optim.py).
+
+    ``ema_decay``: None, or d in [0, 1): the optimizer also keeps an exponential moving average
+    of the weights (Keras's ``use_ema``), fused into its update kernels; training is unchanged.
+    ``averaged()`` exports it and ``evaluate(..., averaged=True)`` scores it.
 
     ``num_classes``: any int >= 1.  The head has ``VP = ceil(num_classes / 8) * 8`` rows; the
     padding rows start at zero and stay zero, and the loss, evaluation and serving read only the
@@ -203,6 +236,7 @@ class ResNetTrainer(object):
     cross-entropy against (1 - eps) * onehot + eps / num_classes, as
     ``F.cross_entropy(label_smoothing=eps)``; evaluation reports the plain cross-entropy."""
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
+    self.ema_decay = engine.check_ema_decay(ema_decay, training)
     assert depth in self.CFG, "bottleneck depths: 50/101/152"
     self.device = torch.device(device)
     self.B, self.image, self.num_classes, self.depth = batch, image, num_classes, depth
@@ -331,7 +365,7 @@ class ResNetTrainer(object):
       buckets = self._comm_buckets() if (comm is not None and comm.world > 1) else None
       self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, momentum=momentum,
                                   weight_decay=weight_decay, buckets=buckets,
-                                  trust_coefficient=trust_coefficient)
+                                  trust_coefficient=trust_coefficient, ema_decay=self.ema_decay)
     self.graph = None
     self.mean = [0.485, 0.456, 0.406]
     self.std = [0.229, 0.224, 0.225]
@@ -598,9 +632,10 @@ class ResNetTrainer(object):
       cur = target
     return plans, cur
 
-  def _eval_forward(self, wv, bias, u8):
+  def _eval_forward(self, wv, bias, u8, head=None):
     """Evaluation forward pass on this trainer's activation buffers (see _Evaluator): the stem
-    writes ``stem_raw``, which a training trainer has too."""
+    writes ``stem_raw``, which a training trainer has too.  ``head``: what runs the classifier
+    (default ``fc.forward``, on the store's head)."""
     plans, last = self._folded_plans(wv, bias, self.stem_raw)
     K = ops.K
 
@@ -611,7 +646,7 @@ class ResNetTrainer(object):
       for p in plans[1:]:
         p.run()
       K.avgpool_fwd(last, self.avg)
-      self.fc.forward()
+      (head or self.fc.forward)()
     return run
 
   def fold_batch_norms(self):
@@ -637,13 +672,17 @@ class ResNetTrainer(object):
     return self.logits
 
   # ------------------------------------------------------- held-out evaluation
-  def eval_begin(self):
+  def eval_begin(self, averaged=False):
     """Start an evaluation pass: zero the totals, take rank 0's running statistics and fold every
     batch norm into a copy of the current bf16 filters (one launch).  Stream-ordered after the
-    last ``train_step``; the first call allocates the evaluation buffers and plans."""
+    last ``train_step``; the first call allocates the evaluation buffers and plans.
+    ``averaged=True`` folds the weight average instead (``ema_decay``; RuntimeError without it):
+    the model ``averaged()`` exports, with the live running statistics."""
+    if averaged:
+      self._check_average()
     if getattr(self, "_evaluator", None) is None:
       self._evaluator = _Evaluator(self)
-    self._evaluator.begin()
+    self._evaluator.begin(averaged)
 
   def eval_step(self, images_u8, labels):
     """Add the top-1 / top-5 / loss totals of n <= B images (host or device, uint8 NHWC) and their
@@ -659,12 +698,26 @@ class ResNetTrainer(object):
     [0, num_classes)."""
     return self._eval_state().end()
 
-  def evaluate(self, batches):
-    """eval_begin + eval_step over ``(images, labels)`` pairs + eval_end.  Host batches go through
-    page-locked staging: the copy of batch i + 1 overlaps the forward pass of batch i."""
-    self.eval_begin()
+  def evaluate(self, batches, averaged=False):
+    """eval_begin(averaged) + eval_step over ``(images, labels)`` pairs + eval_end.  Host batches
+    go through page-locked staging: the copy of batch i + 1 overlaps the forward pass of batch i."""
+    self.eval_begin(averaged)
     self._evaluator.run(batches)
     return self.eval_end()
+
+  def _check_average(self):
+    if getattr(self.optim, "ema", None) is None:
+      raise RuntimeError("this trainer keeps no weight average: build it with ema_decay=d")
+
+  def averaged(self):
+    """Snapshot of the weight average as an exportable model (engine.AveragedModel): its
+    ``state_dict()`` is this trainer's with every parameter replaced by its average and the live
+    running statistics, so ``checkpoint.export_model(net.averaged(), dir)`` exports the average as
+    Keras does after ``finalize_variable_values()``.  RuntimeError without ``ema_decay``."""
+    self._check_average()
+    sd, _ = engine.averaged_params(self.store, self.optim)
+    sd["__running__"] = self.running.tensor().detach().cpu().clone()
+    return engine.AveragedModel(sd, self)
 
   def _eval_state(self):
     if getattr(self, "_evaluator", None) is None:
@@ -692,11 +745,15 @@ class ResNetTrainer(object):
     return sd
 
   def load_state_dict(self, sd):
+    """Parameters and running statistics of ``state_dict()``; resets the weight average (the
+    optimizer's ``load_state_dict`` restores a saved one)."""
     sd = dict(sd)
     running = sd.pop("__running__", None)
     self.store.load_state_dict(sd)
     if running is not None:
       self.running.tensor().copy_(running.to(self.device))
+    if self.optim is not None:
+      self.optim.reset_average()
 
   def load_backbone(self, state):
     """Start from a trained backbone: ``state`` is the ``state_dict()`` of a trainer of the same
@@ -704,7 +761,7 @@ class ResNetTrainer(object):
     and the batch-norm running statistics (``__running__``), like ``load_state_dict``; the head
     keeps its seeded initialisation and the optimizer state is untouched.  Every tensor is checked
     before anything is copied: a missing, unexpected or wrongly shaped one raises ValueError and
-    leaves the trainer as it was."""
+    leaves the trainer as it was.  Resets the weight average."""
     want = {s["name"]: s["shape"] for s in self.store.order if s["name"] not in _HEAD}
     want["__running__"] = tuple(self.running.tensor().shape)
     extra = sorted(set(state) - set(want) - set(_HEAD))
@@ -759,13 +816,14 @@ def build_served(state, depth=50, image=224, num_classes=1000, batch=None, **_):
 class CifarResNetTrainer(object):
   """ResNet-20/32/56 for 32x32 inputs (basic blocks, 16/32/64 channels) - the network the
   reference example actually trains (examples/resnet/resnet_cifar_dist.py:208, ``resnet56``,
-  momentum SGD, batch 128, weight decay 2e-4).  ``num_classes`` and ``label_smoothing`` as in
-  ResNetTrainer."""
+  momentum SGD, batch 128, weight decay 2e-4).  ``num_classes``, ``label_smoothing`` and
+  ``ema_decay`` as in ResNetTrainer."""
 
   def __init__(self, depth=56, batch=128, num_classes=10, device="cuda:0", lr=0.1, momentum=0.9,
                weight_decay=2e-4, comm=None, seed=1234, optimizer="momentum",
-               trust_coefficient=0.001, label_smoothing=0.0):
+               trust_coefficient=0.001, label_smoothing=0.0, ema_decay=None):
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
+    self.ema_decay = engine.check_ema_decay(ema_decay)
     assert (depth - 2) % 6 == 0
     n = (depth - 2) // 6
     self.device = dev = torch.device(device)
@@ -829,7 +887,8 @@ class CifarResNetTrainer(object):
     self.fc.build(self.avg, self.logits, self.dlogits, self.g_avg)
     from ..parallel.fused_optim import FusedOptimizer
     self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, momentum=momentum,
-                                weight_decay=weight_decay, trust_coefficient=trust_coefficient)
+                                weight_decay=weight_decay, trust_coefficient=trust_coefficient,
+                                ema_decay=self.ema_decay)
     self.graph = None
     self.mean, self.std = [0.4914, 0.4822, 0.4465], [0.2470, 0.2435, 0.2616]
 
@@ -846,6 +905,8 @@ class CifarResNetTrainer(object):
   eval_end = ResNetTrainer.eval_end
   evaluate = ResNetTrainer.evaluate
   _eval_state = ResNetTrainer._eval_state
+  _check_average = ResNetTrainer._check_average
+  averaged = ResNetTrainer.averaged
 
   def _fold_units(self):
     """(filter spec, batch norm) of every convolution followed by a batch norm, stem first."""
@@ -855,10 +916,10 @@ class CifarResNetTrainer(object):
         units.append((u.conv.sw, u.bn))
     return units
 
-  def _eval_forward(self, wv, bias, u8):
+  def _eval_forward(self, wv, bias, u8, head=None):
     """Folded basic-block network on the training buffers (see _Evaluator): bias + ReLU in every
     epilogue, the shortcut into ``out``, conv2 accumulating the residual into ``out`` (projection
-    blocks) or in place into the block input (identity blocks)."""
+    blocks) or in place into the block input (identity blocks).  ``head`` as in ResNetTrainer."""
     conv = lambda x, u, y, **kw: igemm.conv_fprop(  # noqa: E731
         x, wv(u.conv.sw), y, u.conv.stride, u.conv.pad, bias=bias[id(u.bn)], **kw)
     cur = self.stem_act
@@ -877,7 +938,7 @@ class CifarResNetTrainer(object):
       for p in plans:
         p.run()
       K.avgpool_fwd(last, self.avg)
-      self.fc.forward()
+      (head or self.fc.forward)()
     return run
 
   def step_kernels(self):

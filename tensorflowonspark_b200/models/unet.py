@@ -31,6 +31,7 @@ import torch
 from .. import ops
 from ..ops import igemm
 from . import evaluation, serving
+from . import engine
 from .engine import BatchNorm, ParamStore, RunningArena, constant, he_normal
 
 # (expansion t, out channels c, repeats n, stride s) - MobileNetV2, width 1.0
@@ -427,13 +428,20 @@ class UNetTrainer(object):
   averages, as DDP does with a mean-reduced CrossEntropyLoss.  With neither option the step
   launches exactly the kernels it did without them.  ``loss_norm`` (fp64 [3], training only) holds
   the last step's [sum_S w[y], |S|, 1 / sum_S w[y]]: loss_sum is the mean loss and
-  correct / loss_norm[1] the pixel accuracy, without a host sync."""
+  correct / loss_norm[1] the pixel accuracy, without a host sync.
+
+  ``ema_decay``: None, or d in [0, 1) (training only): the Adam update kernels also keep an
+  exponential moving average of every parameter, trainable encoder units included (Keras's
+  ``use_ema``); training is unchanged.  ``averaged()`` exports it, ``evaluate(..., averaged=True)``
+  scores it."""
 
   UP = (512, 256, 128, 64)
 
   def __init__(self, batch=64, image=128, classes=3, device="cuda:0", lr=1e-3, comm=None, seed=1234,
-               training=True, encoder_trainable_from=None, ignore_index=None, class_weights=None):
+               training=True, encoder_trainable_from=None, ignore_index=None, class_weights=None,
+               ema_decay=None):
     classes = _classes(classes)
+    self.ema_decay = engine.check_ema_decay(ema_decay, training)
     k = self.encoder_trainable_from = _trainable_from(encoder_trainable_from, training)
     self.ignore_index = _ignore_index(ignore_index)
     self.class_weights = _class_weights(class_weights, classes)
@@ -510,8 +518,10 @@ class UNetTrainer(object):
     self.in_u8 = _buf((B, image, image, 3), dev, torch.uint8)
     if tr:
       from ..parallel.fused_optim import FusedOptimizer
-      self.optim = FusedOptimizer(st, comm=comm, opt="adam", lr=lr, weight_decay=0.0)
+      self.optim = FusedOptimizer(st, comm=comm, opt="adam", lr=lr, weight_decay=0.0,
+                                  ema_decay=self.ema_decay)
     self.graph = None
+    self._live = None   # (weights, aux32) saved while an averaged evaluation has the average in
 
   # ------------------------------------------------------------------ data
   def synthetic_batch(self, seed=0):
@@ -588,6 +598,9 @@ class UNetTrainer(object):
     self.graph = g
 
   def train_step(self, images_u8=None, labels=None):
+    if self._swapped_in():
+      raise RuntimeError("an averaged evaluation holds the weight average in the weights: call "
+                         "eval_end() before training")
     if images_u8 is not None:
       self.set_input(images_u8, labels)
     if self.graph is not None:
@@ -645,6 +658,8 @@ class UNetTrainer(object):
     self.store.load_state_dict(sd)
     if running is not None:
       self.running.tensor().copy_(running.to(self.device))
+    if self.optim is not None:    # (the optimizer's load_state_dict restores a saved average)
+      self.optim.reset_average()
 
   def _encoder_convs(self):
     return [c for c in self.encoder.layers if not isinstance(c, _Residual)]
@@ -660,11 +675,56 @@ class UNetTrainer(object):
   def export_builder_args(self):
     return {"image": self.image, "classes": self.classes}
 
+  def averaged(self):
+    """Snapshot of the weight average as an exportable model (engine.AveragedModel): its
+    ``state_dict()`` is this trainer's with every parameter replaced by its average, the live
+    running statistics, and ``__encoder__`` with the averaged trainable units (the filter rounded
+    to bf16 to nearest even, as the update kernel rounds masters).  ``checkpoint.export_model(
+    net.averaged(), dir)`` exports the average for ServedUNet.  RuntimeError without
+    ``ema_decay``."""
+    sd, avg = engine.averaged_params(self.store, self.optim)
+    st = self.store
+    sd["__running__"] = self.running.tensor().detach().cpu().clone()
+    sd["__encoder__"] = [
+        (st._view(avg, c.sw).to(torch.bfloat16).cpu(), st._view(avg, c.sb).detach().cpu().clone())
+        if c.trainable else (c.w.detach().cpu().clone(), c.bias.detach().cpu().clone())
+        for c in self._encoder_convs()]
+    return engine.AveragedModel(sd, self)
+
+  def _swapped_in(self):
+    return self._live is not None and self._live[2]
+
+  def _swap_average(self, on):
+    """Put the weight average into ``weights`` / ``aux32`` (the evaluation forward and the
+    trainable encoder units read them), saving the live values; ``on=False`` puts those back,
+    bit for bit.  The masters and optimizer state are never touched."""
+    st = self.store
+    if on:
+      w, aux = self.optim.averaged_weights()    # RuntimeError without an average
+      if not self._swapped_in():
+        if self._live is None:
+          self._live = [torch.empty_like(st.weights), torch.empty_like(st.aux32), False]
+        self._live[0].copy_(st.weights)
+        self._live[1].copy_(st.aux32)
+        self._live[2] = True
+      st.weights.copy_(w)
+      st.aux32.copy_(aux)
+    elif self._swapped_in():
+      st.weights.copy_(self._live[0])
+      st.aux32.copy_(self._live[1])
+      self._live[2] = False
+
   # ------------------------------------------------------- held-out evaluation
-  def eval_begin(self):
+  def eval_begin(self, averaged=False):
     """Start an evaluation pass: zero the totals and take rank 0's running statistics.
     Stream-ordered after the last ``train_step``; the first call allocates the evaluation
-    buffers."""
+    buffers.  ``averaged=True`` scores the weight average (``ema_decay``; RuntimeError without
+    it) with the live running statistics: the average is swapped into ``weights`` / ``aux32``
+    until ``eval_end()``, which restores the live values; ``train_step`` raises RuntimeError in
+    between."""
+    if averaged and (self.optim is None or self.optim.ema is None):
+      raise RuntimeError("this trainer keeps no weight average: build it with ema_decay=d")
+    self._swap_average(averaged)
     if getattr(self, "_evaluator", None) is None:
       self._evaluator = _SegEvaluator(self)
     self._evaluator.begin()
@@ -681,14 +741,23 @@ class UNetTrainer(object):
     """Totals summed over all ranks (identical on every rank), see seg_eval_result.  Raises
     ValueError on every rank when any rank saw a mask value outside [0, classes) that is not
     ``ignore_index``.  With ``ignore_index`` the result also has ``"ignored"``: the pixels left
-    out.  With ``class_weights`` the loss is the weighted mean."""
-    return self._eval_state().end()
+    out.  With ``class_weights`` the loss is the weighted mean.  Ends an averaged evaluation:
+    the live weights are back afterwards, also when the totals raise."""
+    try:
+      return self._eval_state().end()
+    finally:
+      self._swap_average(False)
 
-  def evaluate(self, batches):
-    """eval_begin + eval_step over ``(images, masks)`` pairs + eval_end.  Host batches go through
-    page-locked staging: the copy of batch i + 1 overlaps the forward pass of batch i."""
-    self.eval_begin()
-    self._evaluator.run(batches)
+  def evaluate(self, batches, averaged=False):
+    """eval_begin(averaged) + eval_step over ``(images, masks)`` pairs + eval_end.  Host batches
+    go through page-locked staging: the copy of batch i + 1 overlaps the forward pass of batch i.
+    The live weights are restored even when a batch raises."""
+    self.eval_begin(averaged)
+    try:
+      self._evaluator.run(batches)
+    except BaseException:
+      self._swap_average(False)
+      raise
     return self.eval_end()
 
   def _eval_state(self):

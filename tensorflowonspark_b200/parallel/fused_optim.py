@@ -30,8 +30,18 @@ does not continue under LARS).  The norms need the whole reduced tensor, so ever
 separate, deterministic norm pass (csrc/optim_comm.cu ``lars_norms``) between the reduce-scatter
 and the update: ``[PHASE 1 ->] norms (+ exchange of per-tensor partials among the local peers)
 -> update [+ all-gather]``.  A bucket bound must not cut an adapted tensor.
+
+Weight average (``ema_decay=d``): the update kernels also keep an exponential moving average of
+every parameter, ``ema``, placed and sharded like ``state1``.  The first update after a reset
+(construction, ``reset_average()``, loading a state without it) copies the new master, each later
+one applies ``avg = d avg + (1 - d) w`` in fp32 to the master just written - the rule of Keras's
+``use_ema`` optimizers.  d and the update count n live in ``hyper[8]`` / ``hyper[9]`` and n
+advances on the device like Adam's step, so a replayed CUDA graph keeps averaging.  Training is
+unchanged bit for bit; ``averaged_weights()`` rounds the average into the layout of the store's
+bf16 weights and fp32 tail for evaluation and export.
 """
 import bisect
+import numbers
 
 import torch
 
@@ -42,6 +52,20 @@ OPTS = {"sgd": 0, "momentum": 1, "adam": 2, "lars": 3}
 LARS_MAX_TENSORS = 256
 # elements per work item of the LARS norm pass (one CTA reduces one segment at a time)
 LARS_SEGMENT = 16384
+
+
+# hyper-parameter slots: lr, momentum, wd, grad scale, beta1 | eta, beta2, eps, Adam step; with a
+# weight average also its decay and update count (csrc/ops.h kHyper / kHyperEma)
+HYPER, HYPER_EMA = 8, 10
+
+
+def check_ema_decay(d):
+  """Validated ``ema_decay``: None, or a real number in [0, 1) as a float (ValueError otherwise)."""
+  if d is None:
+    return None
+  if isinstance(d, bool) or not isinstance(d, numbers.Real) or not 0.0 <= float(d) < 1.0:
+    raise ValueError("ema_decay must be None or a real number in [0, 1), got {!r}".format(d))
+  return float(d)
 
 
 def _shard(b, e, world, rank):
@@ -98,9 +122,12 @@ def lars_tables(bounds, buckets, world, seg_len=LARS_SEGMENT):
 class FusedOptimizer(object):
 
   def __init__(self, store, comm=None, opt="momentum", lr=0.1, momentum=0.9, weight_decay=0.0,
-               beta1=0.9, beta2=0.999, eps=1e-7, buckets=None, trust_coefficient=0.001):
+               beta1=0.9, beta2=0.999, eps=1e-7, buckets=None, trust_coefficient=0.001,
+               ema_decay=None):
     """``trust_coefficient``: LARS eta (``opt="lars"``; it takes the slot of Adam's beta1 in
-    the hyper-parameter vector, which LARS does not use)."""
+    the hyper-parameter vector, which LARS does not use).  ``ema_decay``: None (no average) or
+    the decay d in [0, 1) of the weight average (see the module docstring)."""
+    self.ema_decay = check_ema_decay(ema_decay)
     self.store, self.comm = store, comm
     self.opt = OPTS[opt]
     self.lars = self.opt == OPTS["lars"]
@@ -121,8 +148,10 @@ class FusedOptimizer(object):
     else:
       self.world, self.rank = comm.world, comm.rank
     self.deferred = False
-    self.hyper = torch.tensor([lr, momentum, weight_decay, 1.0 / self.gworld, beta1, beta2, eps, 0.0],
-                              dtype=torch.float32, device=dev)
+    hyper = [lr, momentum, weight_decay, 1.0 / self.gworld, beta1, beta2, eps, 0.0]
+    if self.ema_decay is not None:
+      hyper += [self.ema_decay, 0.0]
+    self.hyper = torch.tensor(hyper, dtype=torch.float32, device=dev)
     # with peers, the optimizer state lives in symmetric memory like the master copy: a rank only
     # ever updates its own shard of each bucket, so whoever saves a checkpoint pulls the other
     # shards over NVLink (assemble())
@@ -134,6 +163,8 @@ class FusedOptimizer(object):
       return torch.zeros_like(store.master)
     self.state1 = _state("state1") if self.opt != 0 else None
     self.state2 = _state("state2") if self.opt == 2 else None
+    self.ema = _state("ema") if self.ema_decay is not None else None
+    self._avg = None   # averaged_weights()'s buffers, allocated on first use
     self.step_count = 0
     # CTAs of the fused kernel: one per SM alone, 64 peer-to-peer, 48 with NVLS (below)
     self.grid = 132 if self.world == 1 else 64
@@ -158,6 +189,8 @@ class FusedOptimizer(object):
           "grid": self.grid, "zero_grads": 0,
           "aux_begin": store.decay_end,
       }
+      if self.ema is not None:
+        d["ema"] = self.ema.data_ptr()
       if comm is None or self.group_mode or (self.hier_mode and self.world == 1):
         d["grads"] = [store.grads.data_ptr()]
         d["weights"] = [store.weights.data_ptr()]
@@ -241,6 +274,50 @@ class FusedOptimizer(object):
     if self.opt == 2:
       self.step_count += 1
       self.hyper[7:8].add_(1.0)
+    if self.ema is not None:
+      self.hyper[9:10].add_(1.0)     # n: the kernels copy the master at n = 1, decay after
+
+  # ------------------------------------------------------------ weight average
+  def reset_average(self):
+    """Restart the average: until the next update it is the current parameters, after that
+    update it equals the new master (n = 0).  No-op without an average."""
+    if self.ema is not None:
+      self.hyper[9:10].zero_()
+
+  def average_count(self):
+    """n, the updates folded into the average since it was last reset (host sync)."""
+    return int(self.hyper[9].item()) if self.ema is not None else 0
+
+  def averaged_weights(self):
+    """The complete weight average on this rank: ``(weights, aux32)``, a bf16 buffer in the
+    layout of ``store.weights`` and an fp32 one in that of ``store.aux32`` - what ``bn_fold``
+    and the U-Net forward read.  bf16 is rounded to nearest even by the ps_pull kernel
+    (``pack_bf16x2``, as the update kernel rounds masters), so these are exactly the weights a
+    trainer loading the exported average derives.  Before the first update after a reset they
+    are the current parameters.  Pulls the peers' shards first (assemble()); stream-ordered
+    between two steps like assemble().  Returns buffers owned by the optimizer, rewritten by the
+    next call."""
+    if self.ema is None:
+      raise RuntimeError("this optimizer keeps no weight average (ema_decay=None)")
+    st = self.store
+    src = self.average_master()
+    if self._avg is None:
+      self._avg = (torch.empty_like(st.weights), torch.zeros_like(st.aux32))
+    w, aux = self._avg
+    ops.K.ps_pull(src.data_ptr(), None, w, st.total)
+    aux[:st.total - st.decay_end].copy_(src[st.decay_end:])
+    return w, aux
+
+  def average_master(self):
+    """fp32 [total] vector of the complete average (the masters themselves while n = 0), after
+    pulling the peers' shards; a view of ``ema`` or ``store.master``, not a copy."""
+    if self.ema is None:
+      raise RuntimeError("this optimizer keeps no weight average (ema_decay=None)")
+    if self.average_count() == 0:
+      self.assemble()
+      return self.store.master
+    self.assemble(("ema",))
+    return self.ema
 
   # ---------------------------------------------------------------- overlap
   def launch(self, tag):
@@ -364,7 +441,7 @@ class FusedOptimizer(object):
     chunk = ((n + self.world - 1) // self.world + 7) // 8 * 8
     return b + min(n, chunk * rank), b + min(n, chunk * (rank + 1))
 
-  def assemble(self):
+  def assemble(self, names=None):
     """Make THIS rank's fp32 master and optimizer state complete.
 
     With world > 1 the fused kernel updates master/state only for the rank's own shard of every
@@ -372,7 +449,9 @@ class FusedOptimizer(object):
     peers' symmetric buffers (plain device copies over NVLink on the current stream).  It is not
     a collective: only the saving rank needs to call it.  It is consistent as long as it is
     stream-ordered between two of this rank's steps - a peer cannot finish its next update
-    before this rank has contributed its gradients (the kernel's entry barrier)."""
+    before this rank has contributed its gradients (the kernel's entry barrier).  The weight
+    average is pulled too; ``names`` restricts the pull to some of master / state1 / state2 /
+    ema."""
     if self.world == 1 or self.comm is None:
       return
     C = ops.C()
@@ -382,7 +461,11 @@ class FusedOptimizer(object):
       bufs.append(("state1", self.state1))
     if self.state2 is not None:
       bufs.append(("state2", self.state2))
+    if self.ema is not None:
+      bufs.append(("ema", self.ema))
     for name, local in bufs:
+      if names is not None and name not in names:
+        continue
       ptrs = self.comm.peer_ptrs(name)
       for r in range(self.world):
         if r == self.rank:
@@ -400,14 +483,26 @@ class FusedOptimizer(object):
       sd["state1"] = self.state1.detach().cpu()
     if self.state2 is not None:
       sd["state2"] = self.state2.detach().cpu()
+    if self.ema is not None:
+      sd["ema"] = self.ema.detach().cpu()
+      sd["ema_count"] = self.average_count()
     sd["hyper"] = self.hyper.detach().cpu()
     return sd
 
   def load_state_dict(self, sd):
+    """Inverse of state_dict().  ``hyper`` may come from an optimizer with or without an average
+    (10 or 8 entries): its first 8 are loaded, the decay stays this optimizer's own.  The average
+    and its count are loaded when ``sd`` has them; otherwise the average is reset."""
     self.step_count = int(sd.get("step", 0))
     if self.state1 is not None and "state1" in sd:
       self.state1.copy_(sd["state1"])
     if self.state2 is not None and "state2" in sd:
       self.state2.copy_(sd["state2"])
     if "hyper" in sd:
-      self.hyper.copy_(sd["hyper"])
+      self.hyper[:HYPER].copy_(torch.as_tensor(sd["hyper"])[:HYPER])
+    if self.ema is not None:
+      if "ema" in sd:
+        self.ema.copy_(sd["ema"])
+        self.hyper[9:10].fill_(float(sd.get("ema_count", 1)))
+      else:
+        self.reset_average()

@@ -23,10 +23,23 @@ KERNELS = [
     ("igemm_wgrad_128", r"igemm_wgrad_kernel<128>"),
     ("igemm_wgrad_256", r"igemm_wgrad_kernel<256>"),
     ("igemm_wgrad_halo", r"igemm_wgrad_halo_kernel"),
-    ("allreduce_opt_momentum_nvls", r"allreduce_opt_kernel<1, true, 0>"),
-    ("allreduce_opt_momentum_p2p", r"allreduce_opt_kernel<1, false, 0>"),
-    ("allreduce_phase1_reduce_scatter", r"allreduce_opt_kernel<0, false, 1>"),
-    ("allreduce_phase2_momentum_update_allgather", r"allreduce_opt_kernel<1, false, 2>"),
+    ("allreduce_opt_momentum_nvls", r"allreduce_opt_kernel<1, true, 0, false>"),
+    ("allreduce_opt_momentum_p2p", r"allreduce_opt_kernel<1, false, 0, false>"),
+    ("allreduce_phase1_reduce_scatter", r"allreduce_opt_kernel<0, false, 1, false>"),
+    ("allreduce_phase2_momentum_update_allgather", r"allreduce_opt_kernel<1, false, 2, false>"),
+    # the weight-average instances (last template argument true), every optimizer and path
+    ("allreduce_opt_sgd_p2p_ema", r"allreduce_opt_kernel<0, false, 0, true>"),
+    ("allreduce_opt_sgd_nvls_ema", r"allreduce_opt_kernel<0, true, 0, true>"),
+    ("allreduce_phase2_sgd_ema", r"allreduce_opt_kernel<0, false, 2, true>"),
+    ("allreduce_opt_momentum_p2p_ema", r"allreduce_opt_kernel<1, false, 0, true>"),
+    ("allreduce_opt_momentum_nvls_ema", r"allreduce_opt_kernel<1, true, 0, true>"),
+    ("allreduce_phase2_momentum_ema", r"allreduce_opt_kernel<1, false, 2, true>"),
+    ("allreduce_opt_adam_p2p_ema", r"allreduce_opt_kernel<2, false, 0, true>"),
+    ("allreduce_opt_adam_nvls_ema", r"allreduce_opt_kernel<2, true, 0, true>"),
+    ("allreduce_phase2_adam_ema", r"allreduce_opt_kernel<2, false, 2, true>"),
+    ("allreduce_opt_lars_one_rank_ema", r"allreduce_opt_kernel<3, false, 0, true>"),
+    ("allreduce_phase2_lars_p2p_ema", r"allreduce_opt_kernel<3, false, 2, true>"),
+    ("allreduce_phase2_lars_nvls_ema", r"allreduce_opt_kernel<3, true, 2, true>"),
     ("ps_apply_momentum", r"ps_apply_kernel<1>"),
     ("ps_push_slot", r"ps_push_slot_kernel"),
     ("ps_pull_model", r"ps_pull_model_kernel"),
