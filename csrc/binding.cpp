@@ -783,6 +783,14 @@ void allreduce_opt(const py::dict& d) {
   a.lars_T = geti<int>(d, "lars_T", 0);
   // weight average: selects the averaging instances; hyper must then hold tfos::kHyperEma floats
   a.ema = reinterpret_cast<float*>(geti<uint64_t>(d, "ema", 0));
+  // gradient clipping's reduce-scatter (phase 3): per-CTA scratch and every peer's norm table
+  if (d.contains("clip_sq")) {
+    fill_ptrs(d["clip_sq"].cast<std::vector<uint64_t>>(), reinterpret_cast<void**>(a.clip_sq),
+              a.world);
+    a.clip_partial = reinterpret_cast<float*>(d["clip_partial"].cast<uint64_t>());
+    a.clip_nb = d["clip_nb"].cast<int>();
+    a.clip_index = d["clip_index"].cast<int>();
+  }
   const int opt = geti<int>(d, "opt", 0);
   const int grid = geti<int>(d, "grid", 32);
   check(tfos::allreduce_opt(a, opt, grid, cur_stream(), geti<int>(d, "phase", 0)), "allreduce_opt");
@@ -812,6 +820,37 @@ void lars_norms(const py::dict& d) {
   }
   a.block_counter = reinterpret_cast<uint32_t*>(d["block_counter"].cast<uint64_t>());
   check(tfos::lars_norms(a, cur_stream()), "lars_norms");
+}
+
+void grad_sumsq(const py::dict& d) {
+  tfos::GradSumsqArgs a;
+  std::memset(&a, 0, sizeof(a));
+  a.grads = reinterpret_cast<const float*>(d["grads"].cast<uint64_t>());
+  a.lo = d["lo"].cast<long long>();
+  a.hi = d["hi"].cast<long long>();
+  a.partial = reinterpret_cast<float*>(d["partial"].cast<uint64_t>());
+  a.block_counter = reinterpret_cast<uint32_t*>(d["block_counter"].cast<uint64_t>());
+  a.nb = d["nb"].cast<int>();
+  a.index = d["index"].cast<int>();
+  a.world = geti<int>(d, "world", 1);
+  a.rank = geti<int>(d, "rank", 0);
+  a.slot = geti<int>(d, "slot", 0);
+  TORCH_CHECK(a.world >= 1 && a.world <= tfos::kMaxRanks, "grad_sumsq: world out of range");
+  fill_ptrs(d["table"].cast<std::vector<uint64_t>>(), reinterpret_cast<void**>(a.table), a.world);
+  if (a.world > 1) {
+    fill_ptrs(d["flags"].cast<std::vector<uint64_t>>(), reinterpret_cast<void**>(a.flags), a.world);
+    a.epoch = reinterpret_cast<uint32_t*>(d["epoch"].cast<uint64_t>());
+  }
+  check(tfos::grad_sumsq(a, cur_stream()), "grad_sumsq");
+}
+
+void clip_finalize(uint64_t table, int world, int nb, uint64_t hyper, int nh, double clip,
+                   uint64_t hyper_out, uint64_t grad_norm) {
+  check(tfos::clip_finalize(reinterpret_cast<const float*>(table), world, nb,
+                            reinterpret_cast<const float*>(hyper), nh, clip,
+                            reinterpret_cast<float*>(hyper_out), reinterpret_cast<float*>(grad_norm),
+                            cur_stream()),
+        "clip_finalize");
 }
 
 tfos::BcastArgs parse_bcast(const py::dict& d) {
@@ -1018,6 +1057,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("norm") = py::none());
   m.def("allreduce_opt", &allreduce_opt);
   m.def("lars_norms", &lars_norms);
+  m.def("grad_sumsq", &grad_sumsq);
+  m.def("clip_finalize", &clip_finalize);
   m.def("bcast_pull", &bcast_pull);
   m.def("flag_barrier", &flag_barrier);
   m.def("set_flag_timeout_ms", &set_flag_timeout_ms);

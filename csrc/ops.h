@@ -141,12 +141,43 @@ struct AllreduceOptArgs {
   // [9] = updates since the average was reset, counted before the launch.  After update 1 the
   // average is the master, after each later one d * avg + (1 - d) * master.
   float* ema;
+  // Gradient clipping, phase 3 only (after the fields above for the same reason).  Each CTA
+  // stores the sum of squares of the reduced gradients it visited in clip_partial[blockIdx.x]
+  // (at least gridDim.x floats); the last CTA sums them in CTA order and stores
+  // {sum, 0, 0, 0} at entry (rank, clip_index) of every local peer's [world][clip_nb][4] table
+  // clip_sq before the exit barrier.
+  float* clip_partial;
+  float* clip_sq[kMaxRanks];
+  int clip_nb, clip_index;
 };
 constexpr int kHyper = 8, kHyperEma = 10;
-// phase: 0 = fused; 1 = intra-host reduce-scatter only; 2 = update + all-gather only (optim_comm.cu)
-// kOptLars with world > 1 runs as phase 1 -> lars_norms -> phase 2 (phase 0 is refused)
-// a.ema != nullptr selects the averaging instances of phases 0 and 2 (phase 1 does not update)
+// phase: 0 = fused; 1 = intra-host reduce-scatter only; 2 = update + all-gather only; 3 = phase 1
+// that also publishes the sum of squares of the rank's reduced shard (clip_*, world > 1 only)
+// kOptLars with world > 1 runs as phase 1 | 3 -> lars_norms -> phase 2 (phase 0 is refused)
+// a.ema != nullptr selects the averaging instances of phases 0 and 2 (phases 1, 3 do not update)
 cudaError_t allreduce_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStream_t s, int phase = 0);
+
+// Gradient clipping by global norm.  grad_sumsq: sum of squares of grads[lo, hi) (an unscaled,
+// fully reduced gradient), reduced in a fixed thread -> element mapping and a fixed tree, stored
+// as {sum, 0, 0, 0} at entry (rank, index) of every local peer's [world][nb][4] table; with
+// world > 1 the same exit barrier as lars_norms on flag slot `slot`.
+struct GradSumsqArgs {
+  const float* grads;
+  long long lo, hi;         // multiples of 8
+  float* partial;           // [kSmCount] scratch
+  uint32_t* block_counter;  // back at 0 when the kernel completes
+  float* table[kMaxRanks];
+  int nb, index;
+  int world, rank, slot;
+  uint32_t* flags[kMaxRanks];
+  uint32_t* epoch;
+};
+cudaError_t grad_sumsq(const GradSumsqArgs& a, cudaStream_t s);
+// One thread: N = |hyper[3]| * sqrt(sum of the table, rank after rank, bucket after bucket),
+// coef = clip / (N + 1e-6) clamped to at most 1 (NaN stays NaN), all in double.  Writes
+// grad_norm = fl(N) and hyper_out = hyper[0, nh) with slot 3 replaced by fl(hyper[3] * coef).
+cudaError_t clip_finalize(const float* table, int world, int nb, const float* hyper, int nh,
+                          double clip, float* hyper_out, float* grad_norm, cudaStream_t s);
 
 // LARS per-tensor norms of one rank's shard of one bucket (deterministic: no float atomics).
 // seg[2 s], seg[2 s + 1] bound segment s; the segments of local tensor j are

@@ -41,6 +41,9 @@ namespace {
 // driver exception, TFSparkNode.py): runtime knob, TFOS_FLAG_TIMEOUT_MS (parallel/symm.py)
 __device__ unsigned long long g_flag_timeout_ns = TFOS_FLAG_TIMEOUT_NS;
 
+// kReport = false: trap without the message, whose printf argument buffer would be the kernel's
+// only stack frame (the gradient-clipping kernels)
+template <bool kReport = true>
 __device__ __forceinline__ void wait_flag(const uint32_t* p, uint32_t target) {
   if (static_cast<int32_t>(ld_acquire_sys(p) - target) >= 0) return;
   const uint64_t t0 = globaltimer_ns();
@@ -49,8 +52,9 @@ __device__ __forceinline__ void wait_flag(const uint32_t* p, uint32_t target) {
     if ((++spins & 0xff) == 0) {
       __nanosleep(64);
       if (globaltimer_ns() - t0 > g_flag_timeout_ns) {
-        printf("tfos: peer flag timeout (block %d, want %u, have %u)\n", blockIdx.x, target,
-               ld_acquire_sys(p));
+        if (kReport)
+          printf("tfos: peer flag timeout (block %d, want %u, have %u)\n", blockIdx.x, target,
+                 ld_acquire_sys(p));
         __trap();
       }
     }
@@ -70,6 +74,19 @@ __device__ __forceinline__ void multimem_st_b32x4(void* mc, uint4 v) {
                "f"(__uint_as_float(v.x)), "f"(__uint_as_float(v.y)), "f"(__uint_as_float(v.z)),
                "f"(__uint_as_float(v.w))
                : "memory");
+}
+
+// Sum of v over the CTA, valid on thread 0: a fixed shuffle tree per warp, then the warps in order.
+// red holds one float per warp.  Every thread of the CTA must call it.
+__device__ __forceinline__ float block_sum_thread0(float v, float* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float s = 0.f;
+  if (threadIdx.x == 0)
+    for (int k = 0; k < static_cast<int>(blockDim.x >> 5); ++k) s += red[k];
+  return s;
 }
 
 // hyper[]: 0 lr, 1 momentum, 2 weight_decay, 3 grad_scale (1/world * loss scale),
@@ -112,7 +129,10 @@ __device__ __forceinline__ float lars_update(float w, float g, float& v, const f
 // all-gather only (the gradient comes from the own buffer, which by then holds the sum over all
 // hosts; new weights go to every local peer).  0 = both in one pass (one host).
 // EMA: also fold the updated master into the shard's weight average (AllreduceOptArgs::ema) while
-// it is in registers - one extra fp32 load and store per element.
+// it is in registers - one extra fp32 load and store per element.  PHASE 3 = PHASE 1 that also
+// sums the squares of the reduced shard in registers for gradient clipping (AllreduceOptArgs::
+// clip_*): per-CTA partials, summed in CTA order by the last CTA, which publishes the rank's
+// total to every peer's table before the exit barrier.
 template <int OPT, bool MULTIMEM, int PHASE = 0, bool EMA = false>
 __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOptArgs a) {
   constexpr int kH = EMA ? kHyperEma : kHyper;
@@ -125,7 +145,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
     uint32_t* my = a.flags[rank] + a.slot * 32;
     if (blockIdx.x == 0 && threadIdx.x < world)
       st_release_sys(a.flags[threadIdx.x] + a.slot * 32 + rank, e);
-    if (threadIdx.x < world) wait_flag(my + threadIdx.x, e);
+    if (threadIdx.x < world) wait_flag<PHASE != 3>(my + threadIdx.x, e);
   }
   // LARS: start offsets and trust ratios of the shard's adapted tensors.  Every rank sums the
   // rows of the norms table in rank order, so ranks whose shards split one tensor derive the
@@ -164,6 +184,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
   // the weight average 8 (the average's registers would otherwise spill at the 128-register bound)
   constexpr int kU = MULTIMEM ? (EMA ? 4 : 8) : 1;
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x * 8;
+  float sq = 0.f;   // PHASE 3: this thread's sum of squares, elements in visiting order
   for (long long i0 = lo + (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 8;
        i0 < hi; i0 += stride * kU) {
    float4 mg0[kU], mg1[kU];
@@ -213,7 +234,11 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
           g[6] += __uint_as_float(v1[p].z), g[7] += __uint_as_float(v1[p].w);
         }
     }
-    if (PHASE == 1) {
+    if (PHASE == 1 || PHASE == 3) {
+      if (PHASE == 3) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) sq = fmaf(g[j], g[j], sq);
+      }
       *reinterpret_cast<float4*>(a.grads[rank] + i) = make_float4(g[0], g[1], g[2], g[3]);
       *reinterpret_cast<float4*>(a.grads[rank] + i + 4) = make_float4(g[4], g[5], g[6], g[7]);
       continue;
@@ -324,6 +349,11 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
     }
    }
   }
+  if constexpr (PHASE == 3) {
+    __shared__ float red[16];   // 512 threads = 16 warps
+    const float cta = block_sum_thread0(sq, red);
+    if (threadIdx.x == 0) a.clip_partial[blockIdx.x] = cta;
+  }
 
   if (world > 1) {
     // completion: the last block to finish publishes "rank done" to every peer
@@ -339,9 +369,23 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
     }
     __syncthreads();
     if (is_last) {
+      if constexpr (PHASE == 3) {
+        if (threadIdx.x == 0) {
+          __threadfence();
+          double t = 0.0;
+          for (int b = 0; b < static_cast<int>(gridDim.x); ++b) t += __ldcg(a.clip_partial + b);
+          const uint4 v = make_uint4(__float_as_uint(static_cast<float>(t)), 0u, 0u, 0u);
+          const long long off = (static_cast<long long>(rank) * a.clip_nb + a.clip_index) * 4;
+#pragma unroll
+          for (int p = 0; p < kMaxRanks; ++p)
+            if (p < world) st_relaxed_sys_v4(a.clip_sq[(rank + p) % world] + off, v);
+          __threadfence_system();
+        }
+        __syncthreads();
+      }
       if (threadIdx.x < world) {
         st_release_sys(a.flags[threadIdx.x] + a.slot * 32 + 16 + rank, e);
-        wait_flag(a.flags[rank] + a.slot * 32 + 16 + threadIdx.x, e);
+        wait_flag<PHASE != 3>(a.flags[rank] + a.slot * 32 + 16 + threadIdx.x, e);
       }
       __syncthreads();
       if (threadIdx.x == 0) {
@@ -501,6 +545,78 @@ __global__ void __launch_bounds__(kLarsNormThreads) lars_norms_kernel(const Lars
     if (threadIdx.x == 0) *a.epoch = e;
   }
   if (threadIdx.x == 0) *a.block_counter = 0;
+}
+
+// Gradient clipping: sum of squares of a reduced gradient range (see GradSumsqArgs in ops.h).  The
+// thread -> element mapping depends only on the range and the grid, which grad_sumsq() derives
+// from the length, so replicas that see the same gradients get the same bits.
+constexpr int kSumsqThreads = 256;
+__global__ void __launch_bounds__(kSumsqThreads) grad_sumsq_kernel(const GradSumsqArgs a) {
+  __shared__ float red[kSumsqThreads / 32];
+  float sq = 0.f;
+  for (long long i = a.lo + (static_cast<long long>(blockIdx.x) * kSumsqThreads + threadIdx.x) * 8;
+       i < a.hi; i += static_cast<long long>(gridDim.x) * kSumsqThreads * 8) {
+    const float4 g0 = *reinterpret_cast<const float4*>(a.grads + i);
+    const float4 g1 = *reinterpret_cast<const float4*>(a.grads + i + 4);
+    sq = fmaf(g0.x, g0.x, sq), sq = fmaf(g0.y, g0.y, sq);
+    sq = fmaf(g0.z, g0.z, sq), sq = fmaf(g0.w, g0.w, sq);
+    sq = fmaf(g1.x, g1.x, sq), sq = fmaf(g1.y, g1.y, sq);
+    sq = fmaf(g1.z, g1.z, sq), sq = fmaf(g1.w, g1.w, sq);
+  }
+  const float cta = block_sum_thread0(sq, red);
+  __shared__ uint32_t is_last;
+  if (threadIdx.x == 0) {
+    a.partial[blockIdx.x] = cta;
+    __threadfence();
+    is_last = (atomicAdd(a.block_counter, 1u) == gridDim.x - 1) ? 1u : 0u;
+  }
+  __syncthreads();
+  if (!is_last) return;
+  const int world = a.world, rank = a.rank;
+  if (threadIdx.x == 0) {
+    __threadfence();
+    double t = 0.0;
+    for (int b = 0; b < static_cast<int>(gridDim.x); ++b) t += __ldcg(a.partial + b);
+    const uint4 v = make_uint4(__float_as_uint(static_cast<float>(t)), 0u, 0u, 0u);
+    const long long off = (static_cast<long long>(rank) * a.nb + a.index) * 4;
+    if (world == 1) {
+      *reinterpret_cast<uint4*>(a.table[0] + off) = v;
+    } else {
+#pragma unroll
+      for (int p = 0; p < kMaxRanks; ++p)
+        if (p < world) st_relaxed_sys_v4(a.table[(rank + p) % world] + off, v);
+    }
+  }
+  if (world > 1) {
+    // exit barrier: when this kernel completes on a rank, every peer's entry is visible there
+    const uint32_t e = *a.epoch + 1;
+    __threadfence_system();
+    __syncthreads();
+    if (threadIdx.x < world) {
+      st_release_sys(a.flags[threadIdx.x] + a.slot * 32 + 16 + rank, e);
+      wait_flag<false>(a.flags[rank] + a.slot * 32 + 16 + threadIdx.x, e);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) *a.epoch = e;
+  }
+  if (threadIdx.x == 0) *a.block_counter = 0;
+}
+
+// One thread.  fminf(1, NaN) is 1, so the clamp is a comparison that lets a NaN quotient through:
+// a NaN norm gives a NaN coefficient and an infinite one 0, as torch.nn.utils.clip_grad_norm_.
+__global__ void clip_finalize_kernel(const float* __restrict__ table, int world, int nb,
+                                     const float* __restrict__ hyper, int nh, double clip,
+                                     float* __restrict__ hyper_out, float* __restrict__ grad_norm) {
+  double t = 0.0;
+  for (int r = 0; r < world; ++r)
+    for (int b = 0; b < nb; ++b) t += table[(static_cast<long long>(r) * nb + b) * 4];
+  const double s = hyper[3];
+  const double norm = sqrt(t) * fabs(s);
+  const double q = clip / (norm + 1e-6);
+  const double coef = q >= 1.0 ? 1.0 : q;
+  *grad_norm = static_cast<float>(norm);
+  for (int k = 0; k < nh; ++k) hyper_out[k] = hyper[k];
+  hyper_out[3] = static_cast<float>(s * coef);
 }
 
 // ------------------------------------------------------- parameter server
@@ -709,8 +825,22 @@ __global__ void __launch_bounds__(512) ps_pull_model_kernel(const PsPullArgs a) 
   }
 }
 
+// gradient clipping's reduce-scatter (phase 3): peers only, through the switch on NVLS
+cudaError_t launch_rs_sumsq(const AllreduceOptArgs& a, int grid, cudaStream_t s) {
+  if (a.world < 2 || a.clip_partial == nullptr || a.clip_nb < 1 || a.clip_index < 0 ||
+      a.clip_index >= a.clip_nb || grid > kSmCount)
+    return cudaErrorInvalidValue;
+  if (a.grads_mc != nullptr && a.weights_mc != nullptr)
+    allreduce_opt_kernel<kOptSgd, true, 3><<<grid, 512, 0, s>>>(a);
+  else
+    allreduce_opt_kernel<kOptSgd, false, 3><<<grid, 512, 0, s>>>(a);
+  return cudaGetLastError();
+}
+
 template <int OPT, bool EMA>
 cudaError_t launch_ar(const AllreduceOptArgs& a, int grid, cudaStream_t s, int phase) {
+  if (phase == 3)
+    return launch_rs_sumsq(a, grid, s);
   if (phase == 1)   // (the reduce-scatter half does not depend on the optimizer)
     allreduce_opt_kernel<kOptSgd, false, 1><<<grid, 512, 0, s>>>(a);
   else if (phase == 2)
@@ -730,6 +860,7 @@ cudaError_t launch_lars(const AllreduceOptArgs& a, int grid, cudaStream_t s, int
   if (a.lars_nt > 0 && (a.lars_off == nullptr || a.lars_norms == nullptr))
     return cudaErrorInvalidValue;
   const bool nvls = a.grads_mc != nullptr && a.weights_mc != nullptr && a.world > 1;
+  if (phase == 3) return launch_rs_sumsq(a, grid, s);
   if (phase == 1) {
     if (nvls)
       allreduce_opt_kernel<kOptSgd, true, 1><<<grid, 512, 0, s>>>(a);
@@ -763,7 +894,7 @@ cudaError_t launch_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStream_
 
 cudaError_t allreduce_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStream_t s, int phase) {
   if (a.world < 1 || a.world > kMaxRanks) return cudaErrorInvalidValue;
-  if ((a.begin & 7) != 0 || phase < 0 || phase > 2) return cudaErrorInvalidValue;
+  if ((a.begin & 7) != 0 || phase < 0 || phase > 3) return cudaErrorInvalidValue;
   return a.ema != nullptr ? launch_opt<true>(a, opt, grid, s, phase)
                           : launch_opt<false>(a, opt, grid, s, phase);
 }
@@ -772,6 +903,24 @@ cudaError_t lars_norms(const LarsNormArgs& a, cudaStream_t s) {
   int grid = a.nseg < kSmCount * 4 ? a.nseg : kSmCount * 4;
   if (grid < 1) grid = 1;
   lars_norms_kernel<<<grid, kLarsNormThreads, 0, s>>>(a);
+  return cudaGetLastError();
+}
+cudaError_t grad_sumsq(const GradSumsqArgs& a, cudaStream_t s) {
+  if (a.world < 1 || a.world > kMaxRanks || ((a.lo | a.hi) & 7) != 0 || a.nb < 1 || a.index < 0 ||
+      a.index >= a.nb)
+    return cudaErrorInvalidValue;
+  const long long n = a.hi > a.lo ? a.hi - a.lo : 0;
+  long long grid = (n + kSumsqThreads * 8 * 4 - 1) / (kSumsqThreads * 8 * 4);
+  if (grid > kSmCount) grid = kSmCount;
+  if (grid < 1) grid = 1;
+  grad_sumsq_kernel<<<static_cast<unsigned>(grid), kSumsqThreads, 0, s>>>(a);
+  return cudaGetLastError();
+}
+cudaError_t clip_finalize(const float* table, int world, int nb, const float* hyper, int nh,
+                          double clip, float* hyper_out, float* grad_norm, cudaStream_t s) {
+  if (world < 1 || world > kMaxRanks || nb < 1 || nh < 4 || nh > kHyperEma)
+    return cudaErrorInvalidValue;
+  clip_finalize_kernel<<<1, 1, 0, s>>>(table, world, nb, hyper, nh, clip, hyper_out, grad_norm);
   return cudaGetLastError();
 }
 cudaError_t set_flag_timeout_ns(unsigned long long ns) {

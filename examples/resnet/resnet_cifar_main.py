@@ -46,6 +46,9 @@ def define_flags():
                  help="keep a moving average of the weights with this decay in [0, 1) and also "
                       "evaluate it (avg_*); checkpoints keep the live weights and carry the "
                       "average in the optimizer state")
+  p.add_argument("--clip_norm", type=float, default=None,
+                 help="clip the averaged gradient to this global L2 norm (> 0; inf: only measure "
+                      "it) and print grad_norm next to the loss")
   return p
 
 
@@ -87,6 +90,8 @@ def main_fun(argv, ctx):
   smooth = {"label_smoothing": args.label_smoothing} if args.label_smoothing else {}
   if args.ema_decay is not None:
     smooth["ema_decay"] = args.ema_decay
+  if args.clip_norm is not None:
+    smooth["clip_norm"] = args.clip_norm
   net = resnet.CifarResNetTrainer(depth=args.resnet_size, batch=B, device=dev, comm=comm,
                                   lr=resnet.piecewise_lr(0, B * world), **smooth)
   if comm is not None:
@@ -166,8 +171,9 @@ def main_fun(argv, ctx):
     if (step + 1) % 100 == 0 or step + 1 == total:
       torch.cuda.synchronize()
       if ctx.is_chief:
-        print("epoch {:3d} step {:6d} loss {:.4f} lr {:.4f}  {:.0f} images/s".format(
-            epoch, step + 1, float(loss), resnet.piecewise_lr(epoch, B * world),
+        norm = "" if args.clip_norm is None else "  grad_norm {:.4f}".format(float(net.grad_norm))
+        print("epoch {:3d} step {:6d} loss {:.4f}{} lr {:.4f}  {:.0f} images/s".format(
+            epoch, step + 1, float(loss), norm, resnet.piecewise_lr(epoch, B * world),
             seen / (time.time() - t0)))
       t0, seen = time.time(), 0
     if args.model_dir and ctx.is_chief and (step + 1) % (steps_per_epoch * max(

@@ -31,6 +31,11 @@ Weight averaging: ``--ema_decay d`` also keeps an exponential moving average of 
 (Keras's ``use_ema``), fused into the optimizer kernels.  Every evaluation then also scores the
 average (``eval_avg_loss``, ``eval_avg_top1``, ...), and checkpoints carry it in the optimizer
 state.
+
+Gradient clipping: ``--clip_norm c`` clips the averaged gradient to global norm c before each
+update (Keras's ``global_clipnorm``, ``torch.nn.utils.clip_grad_norm_``), inside the fused optimizer
+kernels; the step log then also reports the gradient's norm (``grad_norm``, before clipping).
+``--clip_norm inf`` only measures it.
 """
 import argparse
 import os
@@ -78,6 +83,9 @@ def parse(argv):
                       "evaluate it (eval_avg_*); checkpoints keep the live weights (the average "
                       "rides in the optimizer state), so serving from model_dir serves the live "
                       "weights")
+  p.add_argument("--clip_norm", type=float, default=None,
+                 help="clip the averaged gradient to this global L2 norm (> 0; inf: only measure "
+                      "it) and log grad_norm")
   return p.parse_args(argv)
 
 
@@ -103,6 +111,8 @@ def main_fun(argv, ctx):
     opt["label_smoothing"] = args.label_smoothing
   if args.ema_decay is not None:
     opt["ema_decay"] = args.ema_decay
+  if args.clip_norm is not None:
+    opt["clip_norm"] = args.clip_norm
   if args.model == "resnet56":
     net = resnet.CifarResNetTrainer(depth=56, batch=B, device="cuda:0", comm=comm, lr=base_lr, **opt)
   else:
@@ -179,10 +189,13 @@ def main_fun(argv, ctx):
       torch.cuda.synchronize()
       dt = time.time() - t0
       rate = 10 * B * ctx.world_size / dt
+      norm = {} if args.clip_norm is None else {"grad_norm": float(net.grad_norm)}
       if ctx.is_chief:
-        print("step {:5d} loss {:.4f}  {:.0f} images/s".format(step + 1, float(loss), rate))
+        print("step {:5d} loss {:.4f}{}  {:.0f} images/s".format(
+            step + 1, float(loss), "".join("  grad_norm {:.4f}".format(v) for v in norm.values()),
+            rate))
       if log:
-        log.log(step=step + 1, loss=float(loss), images_per_s=rate, step_ms=dt * 100)
+        log.log(step=step + 1, loss=float(loss), images_per_s=rate, step_ms=dt * 100, **norm)
       if events:
         events.add_scalars({"loss": float(loss), "images_per_s": rate}, step + 1)
       if exporter and not log:

@@ -10,6 +10,9 @@ pixels in the cross-entropy (one weight per class).
 stem and every block), e.g. after a frozen run, resuming from its checkpoint.
 ``--ema_decay d`` also keeps an exponential moving average of the weights (Keras's ``use_ema``):
 every evaluation scores it too (``val_avg_*``) and ``--export_dir`` exports it.
+``--clip_norm c`` clips the averaged gradient to global norm c before each Adam update (Keras's
+``global_clipnorm``) and prints the last step's ``grad_norm`` next to the loss (``inf``: only
+measure it).
 Checkpoints every epoch (the reference's ModelCheckpoint callback) and evaluates every epoch on
 ``--eval_steps`` held-out synthetic batches per rank (the reference's ``validation_data``):
 validation loss, pixel accuracy and mean IoU.
@@ -50,6 +53,9 @@ def define_flags():
                       "evaluation also scores it (val_avg_*) and --export_dir exports it; the "
                       "checkpoints in --model_dir keep the live weights (and the average in the "
                       "optimizer state), so serving straight from model_dir serves the live weights")
+  p.add_argument("--clip_norm", type=float, default=None,
+                 help="clip the averaged gradient to this global L2 norm (> 0; inf: only measure "
+                      "it) and print grad_norm next to the loss")
   return p
 
 
@@ -60,8 +66,9 @@ def class_weights(text):
 
 def trainer_kwargs(args):
   """Keyword arguments the trainer gets from the flags beyond the common ones: only those of the
-  options that are set (encoder fine-tuning, ignore_index, class_weights, the weight average)."""
-  names = ("encoder_trainable_from", "ignore_index", "class_weights", "ema_decay")
+  options that are set (encoder fine-tuning, ignore_index, class_weights, the weight average,
+  gradient clipping)."""
+  names = ("encoder_trainable_from", "ignore_index", "class_weights", "ema_decay", "clip_norm")
   return {n: getattr(args, n) for n in names if getattr(args, n, None) is not None}
 
 
@@ -133,6 +140,8 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
       avg = net.evaluate([(x, labels_of(x, V)) for x in held_out], averaged=True)
     if is_chief:
       line = "epoch {} loss {:.4f}".format(epoch + 1, float(loss))
+      if "clip_norm" in extra:
+        line += " grad_norm {:.4f}".format(float(net.grad_norm))
       if res is not None:
         line += " val_loss {:.4f} val_accuracy {:.4f} val_mean_iou {:.4f}".format(
             res["loss"], res["accuracy"], res["mean_iou"])

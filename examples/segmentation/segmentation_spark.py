@@ -22,6 +22,9 @@ every evaluation scores it too (``val_avg_*``), and ``--export_dir`` exports the
 ``--model_dir`` checkpoint holds the live parameters only (no optimizer state), so it carries
 neither the optimizer state nor the average.
 
+``--clip_norm c`` clips the averaged gradient to global norm c before each Adam update (Keras's
+``global_clipnorm``) and prints the step's ``grad_norm`` next to the loss (``inf``: only measure it).
+
   python examples/segmentation/segmentation_spark.py --cluster_size 8 --batch_size 64 --steps 100
 """
 import argparse
@@ -47,6 +50,11 @@ def synth_rows(n, seed, classes=3):
   return [(imgs[i % pool], masks[i % pool]) for i in range(n)]
 
 
+def grad_norm_text(net, extra):
+  """" grad_norm N" of the last step with --clip_norm, "" without."""
+  return " grad_norm {:.4f}".format(float(net.grad_norm)) if "clip_norm" in extra else ""
+
+
 def main_fun(args, ctx):
   import time
   import numpy as np
@@ -59,7 +67,7 @@ def main_fun(args, ctx):
   B = args.batch_size
   # None: frozen encoder (as the reference), no ignored label, unweighted loss
   extra = {n: getattr(args, n) for n in ("encoder_trainable_from", "ignore_index", "class_weights",
-                                         "ema_decay")
+                                         "ema_decay", "clip_norm")
            if getattr(args, n, None) is not None}
   V = getattr(args, "classes", 3)
   net = unet.UNetTrainer(batch=B, image=IMG, classes=V, device="cuda:0", lr=args.learning_rate,
@@ -126,8 +134,9 @@ def main_fun(args, ctx):
       seen += B
       if (step + 1) % 10 == 0 and ctx.is_chief:
         torch.cuda.synchronize()
-        print("step {:4d} loss {:.4f} {:.0f} images/s".format(
-            step + 1, float(loss), seen * ctx.num_workers / (time.time() - t0)))
+        print("step {:4d} loss {:.4f}{} {:.0f} images/s".format(
+            step + 1, float(loss), grad_norm_text(net, extra),
+            seen * ctx.num_workers / (time.time() - t0)))
       after_step(done)
     print("rank {} ran {} steps ({} rows); host ms/step: feed {:.2f} staging {:.2f} hand-over {:.2f} "
           "launch {:.2f}; H2D tensors straight from the ring {} / staged {}".format(
@@ -148,8 +157,9 @@ def main_fun(args, ctx):
       done += 1
       if (step + 1) % 10 == 0 and ctx.is_chief:
         torch.cuda.synchronize()
-        print("step {:4d} loss {:.4f} {:.0f} images/s".format(
-            step + 1, float(loss), (step + 1) * B * ctx.world_size / (time.time() - t0)))
+        print("step {:4d} loss {:.4f}{} {:.0f} images/s".format(
+            step + 1, float(loss), grad_norm_text(net, extra),
+            (step + 1) * B * ctx.world_size / (time.time() - t0)))
       after_step(done)
   if eval_steps and evaluated[0] != done:
     evaluate(done)
@@ -205,6 +215,9 @@ def define_flags():
                            "the --model_dir checkpoint holds the live weights only (no optimizer "
                            "state, so not the average): serving from model_dir serves the live "
                            "weights")
+  parser.add_argument("--clip_norm", type=float, default=None,
+                      help="clip the averaged gradient to this global L2 norm (> 0; inf: only "
+                           "measure it) and print grad_norm next to the loss")
   return parser
 
 

@@ -139,6 +139,17 @@ def check_ema_decay(d, training=True):
   return d
 
 
+def check_clip_norm(c, training=True):
+  """Validated ``clip_norm`` of a trainer: None, or a float > 0, inf allowed (ValueError
+  otherwise, and for any value with ``training=False``: an inference-only trainer has no
+  optimizer)."""
+  from ..parallel.fused_optim import check_clip_norm as check
+  c = check(c)
+  if c is not None and not training:
+    raise ValueError("clip_norm needs training=True (an inference-only trainer has no optimizer)")
+  return c
+
+
 def he_normal(fan_in):
   std = math.sqrt(2.0 / fan_in)
   return lambda shape, gen: torch.randn(shape, generator=gen) * std

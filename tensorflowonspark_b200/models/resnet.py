@@ -222,9 +222,14 @@ class ResNetTrainer(object):
   def __init__(self, depth=50, batch=256, image=224, num_classes=1000, device="cuda:0",
                lr=0.1, momentum=0.9, weight_decay=1e-4, comm=None, training=True, seed=1234,
                optimizer="momentum", trust_coefficient=0.001, label_smoothing=0.0,
-               ema_decay=None):
+               ema_decay=None, clip_norm=None):
     """``optimizer``: sgd | momentum | adam | lars (``trust_coefficient`` is LARS's eta; see
     parallel/fused_optim.py).
+
+    ``clip_norm``: None, or c > 0 (inf allowed): the averaged gradient is clipped to global norm
+    c before the update, as ``torch.nn.utils.clip_grad_norm_`` (Keras's ``global_clipnorm``),
+    inside the fused optimizer kernels; ``grad_norm`` holds the norm of each step, and
+    ``clip_norm=float("inf")`` only measures it.
 
     ``ema_decay``: None, or d in [0, 1): the optimizer also keeps an exponential moving average
     of the weights (Keras's ``use_ema``), fused into its update kernels; training is unchanged.
@@ -237,6 +242,7 @@ class ResNetTrainer(object):
     ``F.cross_entropy(label_smoothing=eps)``; evaluation reports the plain cross-entropy."""
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     self.ema_decay = engine.check_ema_decay(ema_decay, training)
+    self.clip_norm = engine.check_clip_norm(clip_norm, training)
     assert depth in self.CFG, "bottleneck depths: 50/101/152"
     self.device = torch.device(device)
     self.B, self.image, self.num_classes, self.depth = batch, image, num_classes, depth
@@ -365,7 +371,8 @@ class ResNetTrainer(object):
       buckets = self._comm_buckets() if (comm is not None and comm.world > 1) else None
       self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, momentum=momentum,
                                   weight_decay=weight_decay, buckets=buckets,
-                                  trust_coefficient=trust_coefficient, ema_decay=self.ema_decay)
+                                  trust_coefficient=trust_coefficient, ema_decay=self.ema_decay,
+                                  clip_norm=self.clip_norm)
     self.graph = None
     self.mean = [0.485, 0.456, 0.406]
     self.std = [0.229, 0.224, 0.225]
@@ -709,6 +716,12 @@ class ResNetTrainer(object):
     if getattr(self.optim, "ema", None) is None:
       raise RuntimeError("this trainer keeps no weight average: build it with ema_decay=d")
 
+  @property
+  def grad_norm(self):
+    """Device fp32 [1]: the global norm N of the last step's averaged gradient, before clipping
+    (updated by every replay of the captured step); None without ``clip_norm``."""
+    return self.optim.grad_norm if self.optim is not None else None
+
   def averaged(self):
     """Snapshot of the weight average as an exportable model (engine.AveragedModel): its
     ``state_dict()`` is this trainer's with every parameter replaced by its average and the live
@@ -816,14 +829,15 @@ def build_served(state, depth=50, image=224, num_classes=1000, batch=None, **_):
 class CifarResNetTrainer(object):
   """ResNet-20/32/56 for 32x32 inputs (basic blocks, 16/32/64 channels) - the network the
   reference example actually trains (examples/resnet/resnet_cifar_dist.py:208, ``resnet56``,
-  momentum SGD, batch 128, weight decay 2e-4).  ``num_classes``, ``label_smoothing`` and
-  ``ema_decay`` as in ResNetTrainer."""
+  momentum SGD, batch 128, weight decay 2e-4).  ``num_classes``, ``label_smoothing``,
+  ``ema_decay`` and ``clip_norm`` as in ResNetTrainer."""
 
   def __init__(self, depth=56, batch=128, num_classes=10, device="cuda:0", lr=0.1, momentum=0.9,
                weight_decay=2e-4, comm=None, seed=1234, optimizer="momentum",
-               trust_coefficient=0.001, label_smoothing=0.0, ema_decay=None):
+               trust_coefficient=0.001, label_smoothing=0.0, ema_decay=None, clip_norm=None):
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     self.ema_decay = engine.check_ema_decay(ema_decay)
+    self.clip_norm = engine.check_clip_norm(clip_norm)
     assert (depth - 2) % 6 == 0
     n = (depth - 2) // 6
     self.device = dev = torch.device(device)
@@ -888,7 +902,7 @@ class CifarResNetTrainer(object):
     from ..parallel.fused_optim import FusedOptimizer
     self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, momentum=momentum,
                                 weight_decay=weight_decay, trust_coefficient=trust_coefficient,
-                                ema_decay=self.ema_decay)
+                                ema_decay=self.ema_decay, clip_norm=self.clip_norm)
     self.graph = None
     self.mean, self.std = [0.4914, 0.4822, 0.4465], [0.2470, 0.2435, 0.2616]
 
@@ -907,6 +921,7 @@ class CifarResNetTrainer(object):
   _eval_state = ResNetTrainer._eval_state
   _check_average = ResNetTrainer._check_average
   averaged = ResNetTrainer.averaged
+  grad_norm = ResNetTrainer.grad_norm
 
   def _fold_units(self):
     """(filter spec, batch norm) of every convolution followed by a batch norm, stem first."""

@@ -433,15 +433,20 @@ class UNetTrainer(object):
   ``ema_decay``: None, or d in [0, 1) (training only): the Adam update kernels also keep an
   exponential moving average of every parameter, trainable encoder units included (Keras's
   ``use_ema``); training is unchanged.  ``averaged()`` exports it, ``evaluate(..., averaged=True)``
-  scores it."""
+  scores it.
+
+  ``clip_norm``: None, or c > 0, inf allowed (training only): the averaged gradient is clipped to
+  global norm c before the Adam update, as ``torch.nn.utils.clip_grad_norm_``; ``grad_norm`` holds
+  the norm of each step (``clip_norm=float("inf")`` only measures it)."""
 
   UP = (512, 256, 128, 64)
 
   def __init__(self, batch=64, image=128, classes=3, device="cuda:0", lr=1e-3, comm=None, seed=1234,
                training=True, encoder_trainable_from=None, ignore_index=None, class_weights=None,
-               ema_decay=None):
+               ema_decay=None, clip_norm=None):
     classes = _classes(classes)
     self.ema_decay = engine.check_ema_decay(ema_decay, training)
+    self.clip_norm = engine.check_clip_norm(clip_norm, training)
     k = self.encoder_trainable_from = _trainable_from(encoder_trainable_from, training)
     self.ignore_index = _ignore_index(ignore_index)
     self.class_weights = _class_weights(class_weights, classes)
@@ -519,7 +524,7 @@ class UNetTrainer(object):
     if tr:
       from ..parallel.fused_optim import FusedOptimizer
       self.optim = FusedOptimizer(st, comm=comm, opt="adam", lr=lr, weight_decay=0.0,
-                                  ema_decay=self.ema_decay)
+                                  ema_decay=self.ema_decay, clip_norm=self.clip_norm)
     self.graph = None
     self._live = None   # (weights, aux32) saved while an averaged evaluation has the average in
 
@@ -674,6 +679,12 @@ class UNetTrainer(object):
   @property
   def export_builder_args(self):
     return {"image": self.image, "classes": self.classes}
+
+  @property
+  def grad_norm(self):
+    """Device fp32 [1]: the global norm N of the last step's averaged gradient, before clipping
+    (updated by every replay of the captured step); None without ``clip_norm``."""
+    return self.optim.grad_norm if self.optim is not None else None
 
   def averaged(self):
     """Snapshot of the weight average as an exportable model (engine.AveragedModel): its

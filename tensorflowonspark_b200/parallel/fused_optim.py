@@ -39,6 +39,27 @@ one applies ``avg = d avg + (1 - d) w`` in fp32 to the master just written - the
 advances on the device like Adam's step, so a replayed CUDA graph keeps averaging.  Training is
 unchanged bit for bit; ``averaged_weights()`` rounds the average into the layout of the store's
 bf16 weights and fp32 tail for evaluation and export.
+
+Gradient clipping by global norm (``clip_norm=c``): ``torch.nn.utils.clip_grad_norm_(max_norm=c)``
+applied to the averaged gradient ``g = hyper[3] * sum_r g_r`` before the update.  The averaged
+gradient only exists inside the fused kernels, so they compute its norm N over the whole vector
+(every bucket, decayed head and fp32 tail) in a fixed order, without float atomics:
+``N = |hyper[3]| sqrt(sum of per-rank, per-bucket sums of squares)``.  ``coef = c / (N + 1e-6)``
+clamped to at most 1 (a NaN norm gives NaN, an infinite one 0, as in torch) is folded into the
+scale: the update kernels read a per-step copy of ``hyper``, ``hyper_step``, whose slot 3 is
+``fl(hyper[3] * coef)``, so every optimizer (and LARS's trust ratio) sees the clipped gradient and
+weight decay is added after clipping.  When ``c / (N + 1e-6) >= 1`` (``c = inf`` included) the step
+is bitwise the unclipped one.  No bucket may update before every bucket is reduced, so a bucket's
+``launch(tag)`` runs only its reduction and sum of squares; ``finish()`` (or ``after_replay()``)
+finalises N into ``grad_norm`` and runs every bucket's update:
+
+  no peers / GroupComm : [NCCL all-reduce ->] grad_sumsq of the bucket
+  one host, P2P / NVLS : PHASE 3 (reduce-scatter + sum of squares of the shard, published to
+                         every peer's table before the exit barrier)
+  HierComm             : [PHASE 1 ->] NCCL all-reduce of the shard -> grad_sumsq of the shard
+                         (+ exchange among the local peers)
+  LARS                 : any of the above, then the bucket's lars_norms
+  then, once           : clip_finalize -> every bucket's update (PHASE 0 or 2) reading hyper_step
 """
 import bisect
 import numbers
@@ -66,6 +87,16 @@ def check_ema_decay(d):
   if isinstance(d, bool) or not isinstance(d, numbers.Real) or not 0.0 <= float(d) < 1.0:
     raise ValueError("ema_decay must be None or a real number in [0, 1), got {!r}".format(d))
   return float(d)
+
+
+def check_clip_norm(c):
+  """Validated ``clip_norm``: None, or a real number > 0 (inf allowed) as a float (ValueError
+  otherwise: bools, NaN, zero, negative numbers and non-numbers)."""
+  if c is None:
+    return None
+  if isinstance(c, bool) or not isinstance(c, numbers.Real) or not float(c) > 0.0:
+    raise ValueError("clip_norm must be None or a real number > 0 (inf allowed), got {!r}".format(c))
+  return float(c)
 
 
 def _shard(b, e, world, rank):
@@ -123,11 +154,14 @@ class FusedOptimizer(object):
 
   def __init__(self, store, comm=None, opt="momentum", lr=0.1, momentum=0.9, weight_decay=0.0,
                beta1=0.9, beta2=0.999, eps=1e-7, buckets=None, trust_coefficient=0.001,
-               ema_decay=None):
+               ema_decay=None, clip_norm=None):
     """``trust_coefficient``: LARS eta (``opt="lars"``; it takes the slot of Adam's beta1 in
     the hyper-parameter vector, which LARS does not use).  ``ema_decay``: None (no average) or
-    the decay d in [0, 1) of the weight average (see the module docstring)."""
+    the decay d in [0, 1) of the weight average.  ``clip_norm``: None or the global-norm
+    threshold c > 0 (inf: measure only); ``grad_norm`` then holds N of the last step (see the
+    module docstring)."""
     self.ema_decay = check_ema_decay(ema_decay)
+    self.clip_norm = check_clip_norm(clip_norm)
     self.store, self.comm = store, comm
     self.opt = OPTS[opt]
     self.lars = self.opt == OPTS["lars"]
@@ -214,6 +248,9 @@ class FusedOptimizer(object):
     self.nvls = bool(self._args and self._args[0].get("grads_mc"))
     if self.lars:
       self._build_lars(store, comm)
+    self.grad_norm = None
+    if self.clip_norm is not None:
+      self._build_clip(store, comm)
     self._by_tag = {}
     for i, (_, _, tag) in enumerate(self.buckets):
       self._by_tag.setdefault(tag, []).append(i)
@@ -261,6 +298,46 @@ class FusedOptimizer(object):
         nd.update(flags=d["flags"], epoch=d["epoch"])
       self._lars_args.append(nd)
       self._lars_phase.append((dict(d, phase=1), dict(d, phase=2)))
+
+  def _build_clip(self, store, comm):
+    """Gradient clipping's buffers and launch arguments.  ``clip_sq``: ``world`` rows of one
+    {sum g^2, 0, 0, 0} entry per bucket, row r written by rank r (symmetric with peers)."""
+    dev, nb = self.device, len(self.buckets)
+    if comm is not None and self.world > 1:
+      self.clip_sq = comm.alloc("clip_sq", self.world * nb * 4, torch.float32)
+      self.clip_sq.zero_()
+      table = comm.peer_ptrs("clip_sq")
+    else:
+      self.clip_sq = torch.zeros(self.world * nb * 4, dtype=torch.float32, device=dev)
+      table = [self.clip_sq.data_ptr()]
+    self.grad_norm = torch.zeros(1, dtype=torch.float32, device=dev)
+    self.hyper_step = torch.zeros_like(self.hyper)
+    grid = 132   # >= every grid of the sum-of-squares passes (csrc/ptx.cuh kSmCount)
+    self._clip_partial = torch.zeros(nb * grid, dtype=torch.float32, device=dev)
+    self._clip_counter = torch.zeros(nb, dtype=torch.int32, device=dev)
+    self._clip_phase1, self._clip_reduce, self._clip_update = [], [], []
+    hs = self.hyper_step.data_ptr()
+    for i, d in enumerate(self._args):
+      if self.lars:
+        phase1, phase2 = self._lars_phase[i]
+        one = self._args[i]
+      else:
+        phase1, phase2, one = dict(d, phase=1), dict(d, phase=2), d
+      partial = self._clip_partial.data_ptr() + 4 * grid * i
+      if self.world > 1 and not self.hier_mode:
+        red = dict(phase1, phase=3, clip_sq=table, clip_partial=partial, clip_nb=nb, clip_index=i)
+      else:
+        lo, hi = self.shard_bounds(i, self.rank)
+        red = {"grads": store.grads.data_ptr(), "lo": lo, "hi": hi, "partial": partial,
+               "block_counter": self._clip_counter.data_ptr() + 4 * i, "table": table, "nb": nb,
+               "index": i, "world": self.world, "rank": self.rank, "slot": i}
+        if self.world > 1:
+          red.update(flags=d["flags"], epoch=d["epoch"])
+      self._clip_phase1.append(phase1)
+      self._clip_reduce.append(red)
+      self._clip_update.append(dict(phase2 if (self.world > 1 or self.hier_mode) else one,
+                                    hyper=hs))
+    self._clip_pending = False
 
   def set_lr(self, lr):
     self.hyper[0:1].fill_(float(lr))
@@ -334,8 +411,20 @@ class FusedOptimizer(object):
       self._ev_ready[i].record(main)
       self.comm_stream.wait_event(self._ev_ready[i])
       with torch.cuda.stream(self.comm_stream):
-        self._run_bucket(i)
+        if self.clip_norm is not None:
+          self._reduce_bucket(i)     # the update waits for every bucket's norm: _launch_all()
+        else:
+          self._run_bucket(i)
       self._launched.add(i)
+
+  def _launch_all(self):
+    """launch() every tag, then (clipping) the norm and every bucket's update on the
+    communication stream."""
+    for tag in list(self._by_tag):
+      self.launch(tag)
+    if self.clip_norm is not None:
+      with torch.cuda.stream(self.comm_stream):
+        self._update_all()
 
   def finish(self):
     """Launch whatever has not been launched and make the current stream wait for all of it."""
@@ -344,8 +433,7 @@ class FusedOptimizer(object):
       return
     if not self.overlap:
       return self.step()
-    for tag in list(self._by_tag):
-      self.launch(tag)
+    self._launch_all()
     main = torch.cuda.current_stream(self.device)
     timing = not torch.cuda.is_current_stream_capturing()  # timed events cannot be captured
     if timing:
@@ -370,8 +458,15 @@ class FusedOptimizer(object):
     if self._capturing_group():
       self.deferred = True      # see finish()
       return
+    if self.clip_norm is not None and bucket is not None and len(self.buckets) > 1:
+      raise ValueError("clip_norm: the norm covers every bucket, step() them all at once")
     self._bump_step()
     todo = range(len(self.buckets)) if bucket is None else [bucket]
+    if self.clip_norm is not None:
+      for i in todo:
+        self._reduce_bucket(i)
+      self._update_all()
+      return
     for i in todo:
       self._run_bucket(i)
 
@@ -416,6 +511,39 @@ class FusedOptimizer(object):
       ops.K.lars_norms(self._lars_args[i])
       ops.K.allreduce_opt(self._args[i])
 
+  def _reduce_bucket(self, i):
+    """Clipping, first half of bucket i: its gradient fully reduced and the sum of squares of
+    this rank's share of it in the norm table (+ LARS norms); no update."""
+    if self.hier_mode:
+      if self.world > 1:
+        ops.K.allreduce_opt(self._clip_phase1[i])
+      lo, hi = self.shard_bounds(i, self.rank)
+      if hi > lo:
+        self.comm.all_reduce_inter(self.store.grads[lo:hi])
+      ops.K.grad_sumsq(self._clip_reduce[i])
+    elif self.world > 1:
+      ops.K.allreduce_opt(self._clip_reduce[i])      # PHASE 3
+    else:
+      if self.group_mode:
+        b, e, _ = self.buckets[i]
+        self.comm.all_reduce(self.store.grads[b:e])
+      ops.K.grad_sumsq(self._clip_reduce[i])
+    if self.lars:
+      ops.K.lars_norms(self._lars_args[i])
+    self._clip_pending = True
+
+  def _update_all(self):
+    """Clipping, second half: N into grad_norm, the clipped scale into hyper_step, then every
+    bucket's update.  Runs once per set of reductions."""
+    if not self._clip_pending:
+      return
+    ops.K.clip_finalize(self.clip_sq.data_ptr(), self.world, len(self.buckets),
+                        self.hyper.data_ptr(), self.hyper.numel(), self.clip_norm,
+                        self.hyper_step.data_ptr(), self.grad_norm.data_ptr())
+    for d in self._clip_update:
+      ops.K.allreduce_opt(d)
+    self._clip_pending = False
+
   def _capturing_group(self):
     return ((self.group_mode or self.hier_mode) and self.device.type == "cuda"
             and torch.cuda.is_current_stream_capturing())
@@ -426,8 +554,7 @@ class FusedOptimizer(object):
     if self.deferred:
       self._launched = set()
       if self.overlap:
-        for tag in list(self._by_tag):
-          self.launch(tag)
+        self._launch_all()
         torch.cuda.current_stream(self.device).wait_stream(self.comm_stream)
       else:
         self.step()

@@ -40,6 +40,11 @@ KERNELS = [
     ("allreduce_opt_lars_one_rank_ema", r"allreduce_opt_kernel<3, false, 0, true>"),
     ("allreduce_phase2_lars_p2p_ema", r"allreduce_opt_kernel<3, false, 2, true>"),
     ("allreduce_phase2_lars_nvls_ema", r"allreduce_opt_kernel<3, true, 2, true>"),
+    # gradient clipping: reduce-scatter + sum of squares, the standalone sum, the finaliser
+    ("allreduce_phase3_sumsq_p2p", r"allreduce_opt_kernel<0, false, 3, false>"),
+    ("allreduce_phase3_sumsq_nvls", r"allreduce_opt_kernel<0, true, 3, false>"),
+    ("grad_sumsq", r"grad_sumsq_kernel"),
+    ("clip_finalize", r"clip_finalize_kernel"),
     ("ps_apply_momentum", r"ps_apply_kernel<1>"),
     ("ps_push_slot", r"ps_push_slot_kernel"),
     ("ps_pull_model", r"ps_pull_model_kernel"),
