@@ -38,6 +38,65 @@ inline const void* optptr(const c10::optional<Tensor>& t) {
 inline float* optf(const c10::optional<Tensor>& t) {
   return t.has_value() && t->defined() ? t->data_ptr<float>() : nullptr;
 }
+// Argument errors with numbers in the message.  The message is put together with std::to_string
+// rather than an ostream: inserting a number into a stream of the extension's libstdc++ is not
+// safe next to the one torch was built with.
+inline std::string msg_part(const char* s) { return s; }
+inline std::string msg_part(const std::string& s) { return s; }
+template <typename T>
+std::string msg_part(T v) { return std::to_string(v); }
+inline std::string shape_str(const Tensor& t) {
+  std::string s = "[";
+  for (int64_t d = 0; d < t.dim(); ++d) s += (d ? ", " : "") + std::to_string(t.size(d));
+  return s + "]";
+}
+template <typename... A>
+[[noreturn]] void refuse(const A&... a) {
+  std::string m;
+  ((m += msg_part(a)), ...);
+  throw py::value_error(m);
+}
+#define TFOS_REQUIRE(cond, ...)       \
+  do {                                \
+    if (!(cond)) refuse(__VA_ARGS__); \
+  } while (0)
+// kernels that move 8 bf16 channels (or 8 arg-max bytes) as one vector need aligned pointers
+inline void need_aligned(const Tensor& t, int bytes, const char* name) {
+  TFOS_REQUIRE(reinterpret_cast<uintptr_t>(t.data_ptr()) % bytes == 0, name, " must be ", bytes,
+               "-byte aligned");
+}
+inline void need_numel(const Tensor& t, int64_t n, const char* what, const char* name) {
+  TFOS_REQUIRE(t.numel() == n, what, ": ", name, " must hold ", n, " elements, got ", t.numel());
+}
+// NHWC max pooling: `in` [N, H, W, C] and `out` [N, OH, OW, C] bf16 with OH = (H + 2 pad - k) /
+// stride + 1 (PyTorch's floor mode), C a multiple of 8 (one 16-byte vector per 8 channels), and
+// the uint8 arg-max taps `idx` one per output element.  k <= 15 keeps every tap below 255, the
+// "no window" sentinel of the 3x3/2 backward.
+void check_maxpool(const Tensor& in, const Tensor& out, const Tensor* idx, int k, int stride,
+                   int pad, const char* in_name, const char* out_name, const char* what) {
+  need(in, torch::kBFloat16, in_name);
+  need(out, torch::kBFloat16, out_name);
+  TFOS_REQUIRE(in.dim() == 4 && out.dim() == 4, what, ": ", in_name, " and ", out_name,
+               " must be 4-D NHWC");
+  const int64_t N = in.size(0), H = in.size(1), W = in.size(2), C = in.size(3);
+  TFOS_REQUIRE(C > 0 && C % 8 == 0, what, ": C must be a positive multiple of 8, got ", C);
+  TFOS_REQUIRE(k >= 1 && k <= 15 && stride >= 1 && pad >= 0 && 2 * pad <= k, what,
+               ": need 1 <= k <= 15, stride >= 1 and 0 <= pad <= k / 2, got k=", k, " stride=",
+               stride, " pad=", pad);
+  TFOS_REQUIRE(H + 2 * pad >= k && W + 2 * pad >= k, what, ": the ", k, "x", k,
+               " window does not fit the padded ", H, "x", W, " input");
+  const int64_t OH = (H + 2 * pad - k) / stride + 1, OW = (W + 2 * pad - k) / stride + 1;
+  TFOS_REQUIRE(out.size(0) == N && out.size(1) == OH && out.size(2) == OW && out.size(3) == C,
+               what, ": ", out_name, " must be [", N, ", ", OH, ", ", OW, ", ", C, "], got ",
+               shape_str(out));
+  need_aligned(in, 16, in_name);
+  need_aligned(out, 16, out_name);
+  if (idx != nullptr) {
+    need(*idx, torch::kUInt8, "idx");
+    need_numel(*idx, out.numel(), what, "idx");
+    need_aligned(*idx, 8, "idx");
+  }
+}
 
 int num_sms() {
   static int n = 0;
@@ -337,9 +396,13 @@ void stem_bn_relu_pool_fwd(const Tensor& x, Tensor y, Tensor idx, const Tensor& 
                            const Tensor& sumsq, const Tensor& gamma, const Tensor& beta,
                            Tensor running_mean, Tensor running_var, Tensor mean, Tensor invstd,
                            Tensor scale, Tensor shift, double count, double eps, double momentum) {
-  need(x, torch::kBFloat16, "x");
-  need(y, torch::kBFloat16, "y");
-  TORCH_CHECK(x.dim() == 4 && y.dim() == 4 && idx.numel() == y.numel(), "stem_bn_relu_pool_fwd: shapes");
+  const char* what = "stem_bn_relu_pool_fwd";
+  check_maxpool(x, y, &idx, 3, 2, 1, "x", "y", what);
+  const int64_t C = x.size(3);
+  const std::initializer_list<const Tensor*> vectors = {
+      &sum, &sumsq, &gamma, &beta, &running_mean, &running_var, &mean, &invstd, &scale, &shift};
+  for (const Tensor* t : vectors)
+    need_numel(*t, C, what, "per-channel vector");
   tfos::BnFinalize f;
   f.sum = sum.data_ptr<float>();
   f.sumsq = sumsq.data_ptr<float>();
@@ -362,10 +425,19 @@ void stem_bn_relu_pool_fwd(const Tensor& x, Tensor y, Tensor idx, const Tensor& 
 void stem_pool_bn_bwd(const Tensor& dy_pool, const Tensor& idx, const Tensor& x, const Tensor& gamma,
                       const Tensor& mean, const Tensor& invstd, const Tensor& scale,
                       const Tensor& shift, Tensor dgamma, Tensor dbeta, Tensor dx) {
-  need(dy_pool, torch::kBFloat16, "dy_pool");
-  need(x, torch::kBFloat16, "x");
+  const char* what = "stem_pool_bn_bwd";
+  check_maxpool(x, dy_pool, &idx, 3, 2, 1, "x", "dy_pool", what);
   need(dx, torch::kBFloat16, "dx");
-  TORCH_CHECK(x.dim() == 4 && dy_pool.dim() == 4 && dx.numel() == x.numel(), "stem_pool_bn_bwd: shapes");
+  TFOS_REQUIRE(dx.sizes() == x.sizes(), what, ": dx must have x's shape ", shape_str(x), ", got ",
+               shape_str(dx));
+  need_aligned(dx, 16, "dx");
+  const int64_t C = x.size(3);
+  // a thread keeps one channel group across its grid-stride loop: 256 threads hold whole sets
+  TFOS_REQUIRE(256 % (C / 8) == 0, what, ": C / 8 must divide 256, got C=", C);
+  const std::initializer_list<const Tensor*> vectors = {&gamma, &mean, &invstd, &scale,
+                                                         &shift, &dgamma, &dbeta};
+  for (const Tensor* t : vectors)
+    need_numel(*t, C, what, "per-channel vector");
   check(tfos::stem_pool_bn_bwd(dy_pool.data_ptr(), idx.data_ptr<uint8_t>(), x.data_ptr(),
                                gamma.data_ptr<float>(), mean.data_ptr<float>(),
                                invstd.data_ptr<float>(), scale.data_ptr<float>(),
@@ -394,7 +466,7 @@ void colsum(const Tensor& x, Tensor out) {
         "colsum");
 }
 void maxpool_fwd(const Tensor& x, Tensor y, c10::optional<Tensor> idx, int k, int stride, int pad) {
-  need(x, torch::kBFloat16, "x");
+  check_maxpool(x, y, idx.has_value() ? &*idx : nullptr, k, stride, pad, "x", "y", "maxpool_fwd");
   check(tfos::maxpool_fwd(x.data_ptr(), y.data_ptr(),
                           idx.has_value() ? idx->data_ptr<uint8_t>() : nullptr, x.size(0),
                           x.size(1), x.size(2), x.size(3), y.size(1), y.size(2), k, stride, pad,
@@ -402,18 +474,32 @@ void maxpool_fwd(const Tensor& x, Tensor y, c10::optional<Tensor> idx, int k, in
         "maxpool_fwd");
 }
 void maxpool_bwd(const Tensor& dy, const Tensor& idx, Tensor dx, int k, int stride, int pad) {
+  check_maxpool(dx, dy, &idx, k, stride, pad, "dx", "dy", "maxpool_bwd");
   check(tfos::maxpool_bwd(dy.data_ptr(), idx.data_ptr<uint8_t>(), dx.data_ptr(), dx.size(0),
                           dx.size(1), dx.size(2), dx.size(3), dy.size(1), dy.size(2), k, stride,
                           pad, cur_stream()),
         "maxpool_bwd");
 }
+// global average pool: x [N, ..., C] (HW pixels per image) -> y [N, C], both bf16, C % 8 == 0
+void check_avgpool(const Tensor& x, const Tensor& y, const char* x_name, const char* y_name,
+                   const char* what) {
+  need(x, torch::kBFloat16, x_name);
+  need(y, torch::kBFloat16, y_name);
+  TFOS_REQUIRE(x.dim() >= 2 && x.numel() > 0, what, ": ", x_name, " must be [N, ..., C]");
+  const int64_t N = x.size(0), C = x.size(-1);
+  TFOS_REQUIRE(C % 8 == 0, what, ": C must be a multiple of 8, got ", C);
+  need_numel(y, N * C, what, y_name);
+  need_aligned(x, 16, x_name);
+  need_aligned(y, 16, y_name);
+}
 void avgpool_fwd(const Tensor& x, Tensor y) {
-  need(x, torch::kBFloat16, "x");
+  check_avgpool(x, y, "x", "y", "avgpool_fwd");
   const int N = x.size(0), C = x.size(-1);
   check(tfos::avgpool_fwd(x.data_ptr(), y.data_ptr(), N, x.numel() / N / C, C, cur_stream()),
         "avgpool_fwd");
 }
 void avgpool_bwd(const Tensor& dy, Tensor dx) {
+  check_avgpool(dx, dy, "dx", "dy", "avgpool_bwd");
   const int N = dx.size(0), C = dx.size(-1);
   check(tfos::avgpool_bwd(dy.data_ptr(), dx.data_ptr(), N, dx.numel() / N / C, C, cur_stream()),
         "avgpool_bwd");
@@ -444,8 +530,20 @@ void softmax_xent(const Tensor& logits, const Tensor& labels, c10::optional<Tens
 }
 void decode_normalize(const Tensor& in, Tensor out, int wofs, std::vector<double> mean,
                       std::vector<double> stdv) {
+  // in [N, H, W, C] uint8 -> out [N, H, Wp, Cp] bf16: pixel w lands at column wofs + w, channels
+  // C..Cp and the columns outside [wofs, wofs + W) are zero
+  const char* what = "decode_normalize";
   need(in, torch::kUInt8, "in");
   need(out, torch::kBFloat16, "out");
+  TFOS_REQUIRE(in.dim() == 4 && out.dim() == 4, what, ": in and out must be 4-D NHWC");
+  TFOS_REQUIRE(!mean.empty() && !stdv.empty(), what, ": mean and std need at least one value");
+  const int64_t W = in.size(2), C = in.size(3), Wp = out.size(2), Cp = out.size(3);
+  TFOS_REQUIRE(out.size(0) == in.size(0) && out.size(1) == in.size(1), what,
+               ": out must have in's N and H, got in ", shape_str(in), " out ", shape_str(out));
+  TFOS_REQUIRE(C >= 1 && C <= Cp, what, ": need 1 <= C <= Cp, got C=", C, " Cp=", Cp);
+  TFOS_REQUIRE(wofs >= 0 && wofs + W <= Wp, what, ": need 0 <= wofs and wofs + W <= Wp, got wofs=",
+               wofs, " W=", W, " Wp=", Wp);
+  if (Cp % 8 == 0) need_aligned(out, 16, "out");
   float m[3], is[3];
   for (int i = 0; i < 3; ++i) {
     m[i] = mean[i % mean.size()];

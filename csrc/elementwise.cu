@@ -183,7 +183,9 @@ colsum_kernel(const __nv_bfloat16* __restrict__ x, long long P, int C, float* ou
 
 // ----------------------------------------------------------------- pooling
 // max pool k x k, stride s, pad p over NHWC; records the argmax tap so the
-// backward routes the gradient to exactly one input (PyTorch semantics).
+// backward routes the gradient to exactly one input.  Selection as in PyTorch's max_pool2d:
+// a value replaces the running maximum when it is larger or NaN, so ties keep the first tap in
+// row-major window order and a window holding NaN yields NaN with its last NaN tap.
 // K > 0: window known at compile time - the K*K 16-byte loads of a thread are all in flight
 // at once (ResNet's 3x3/2 pool); K == 0: run-time window.
 template <int K, int S, int PAD>
@@ -224,7 +226,7 @@ maxpool_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restric
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float f = __uint_as_float((j & 1) ? (wd[j >> 1] & 0xffff0000u) : (wd[j >> 1] << 16));
-          if (f > best[j]) best[j] = f, bi[j] = t;
+          if (f > best[j] || f != f) best[j] = f, bi[j] = t;
         }
       }
     } else {
@@ -238,7 +240,7 @@ maxpool_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restric
           load8(x + ((static_cast<long long>(n) * H + h) * W + w) * C + g * 8, f);
 #pragma unroll
           for (int j = 0; j < 8; ++j)
-            if (f[j] > best[j]) best[j] = f[j], bi[j] = kh * k + kw;
+            if (f[j] > best[j] || f[j] != f[j]) best[j] = f[j], bi[j] = kh * k + kw;
         }
       }
     }
@@ -291,7 +293,7 @@ maxpool_fwd_3x3s2_tiled_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat1
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const float f = __uint_as_float((j & 1) ? (wd[j >> 1] & 0xffff0000u) : (wd[j >> 1] << 16));
-      if (f > best[j]) best[j] = f, bi[j] = k;
+      if (f > best[j] || f != f) best[j] = f, bi[j] = k;
     }
   }
   const long long o = ((static_cast<long long>(n) * OH + oh) * OW + ow) * C + g * 8;
