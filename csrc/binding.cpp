@@ -917,7 +917,14 @@ void lars_norms(const py::dict& d) {
     a.epoch = reinterpret_cast<uint32_t*>(d["epoch"].cast<uint64_t>());
   }
   a.block_counter = reinterpret_cast<uint32_t*>(d["block_counter"].cast<uint64_t>());
-  check(tfos::lars_norms(a, cur_stream()), "lars_norms");
+  // LAMB: the norms of the update direction, from the hyper vector and the moments
+  const bool lamb = geti<int>(d, "lamb", 0) != 0;
+  if (lamb) {
+    a.hyper = reinterpret_cast<const float*>(d["hyper"].cast<uint64_t>());
+    a.state1 = reinterpret_cast<const float*>(d["state1"].cast<uint64_t>());
+    a.state2 = reinterpret_cast<const float*>(d["state2"].cast<uint64_t>());
+  }
+  check(tfos::lars_norms(a, cur_stream(), lamb), "lars_norms");
 }
 
 void grad_sumsq(const py::dict& d) {

@@ -105,7 +105,8 @@ cudaError_t pixel_xent(const void* logits, const int* labels, void* dlogits, flo
 
 // ---- optim_comm.cu
 constexpr int kMaxRanks = 8;
-constexpr int kOptSgd = 0, kOptMomentum = 1, kOptAdam = 2, kOptLars = 3;
+constexpr int kOptSgd = 0, kOptMomentum = 1, kOptAdam = 2, kOptLars = 3, kOptAdamW = 4,
+              kOptLamb = 5;
 // LARS: most adapted tensors one shard of a bucket may intersect (the update kernel keeps their
 // start offsets and trust ratios in shared memory); ResNet-152 has 156 adapted tensors
 constexpr int kLarsMaxTensors = 256;
@@ -129,10 +130,10 @@ struct AllreduceOptArgs {
   float* aux32_mc;
   uint32_t* epoch;          // local, one word per slot
   uint32_t* block_counter;  // local, one word per slot
-  // LARS only.  The adapted tensors (the decayed head) tile [0, decay_end): tensor t is
+  // LARS and LAMB only.  The adapted tensors (the decayed head) tile [0, decay_end): tensor t is
   // [lars_off[t], lars_off[t + 1]).  This rank's shard intersects [lars_t0, lars_t0 + lars_nt).
-  // lars_norms is the local [world][lars_T] table of {sum g^2, sum w^2, 0, 0} that
-  // lars_norms() filled, row r with rank r's partial sums.
+  // lars_norms is the local [world][lars_T] table of {sum g^2 | sum r^2 (LAMB), sum w^2, 0, 0}
+  // that lars_norms() filled, row r with rank r's partial sums.
   const long long* lars_off;
   const float* lars_norms;
   int lars_t0, lars_nt, lars_T;
@@ -153,7 +154,9 @@ struct AllreduceOptArgs {
 constexpr int kHyper = 8, kHyperEma = 10;
 // phase: 0 = fused; 1 = intra-host reduce-scatter only; 2 = update + all-gather only; 3 = phase 1
 // that also publishes the sum of squares of the rank's reduced shard (clip_*, world > 1 only)
-// kOptLars with world > 1 runs as phase 1 | 3 -> lars_norms -> phase 2 (phase 0 is refused)
+// kOptLars with world > 1 runs as phase 1 | 3 -> lars_norms -> phase 2 (phase 0 is refused);
+// kOptLamb likewise, with the LAMB norm pass (lars_norms(..., lamb = true)) and the same tables.
+// kOptAdamW / kOptLamb keep Adam's state (state1 = m, state2 = v) and hyper layout.
 // a.ema != nullptr selects the averaging instances of phases 0 and 2 (phases 1, 3 do not update)
 cudaError_t allreduce_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStream_t s, int phase = 0);
 
@@ -198,8 +201,16 @@ struct LarsNormArgs {
   uint32_t* flags[kMaxRanks];
   uint32_t* epoch;
   uint32_t* block_counter;  // back at 0 when the kernel completes
+  // LAMB only (after the fields above so that they keep their parameter offsets): the hyper
+  // vector the update reads (hyper_step with clipping) and the moments before the step.  The pass
+  // recomputes the step's m', v' and r = m'/c1 / (sqrt(v'/c2) + eps) + wd w in registers and
+  // stores {sum r^2, sum w^2} instead of {sum g^2, sum w^2}; it writes no state.
+  const float* hyper;
+  const float* state1;
+  const float* state2;
 };
-cudaError_t lars_norms(const LarsNormArgs& a, cudaStream_t s);
+// lamb: run the LAMB instance (hyper, state1, state2 must be set)
+cudaError_t lars_norms(const LarsNormArgs& a, cudaStream_t s, bool lamb = false);
 
 struct BcastArgs {
   int world, rank, root, slot;

@@ -14,8 +14,8 @@
 //                   updated bf16 weights into every rank's weight buffer - the
 //                   "all-gather" half of the all-reduce carries the new
 //                   parameters instead of the reduced gradients.
-//   lars_norms    : LARS per-tensor norms of a rank's reduced shard, exchanged among the local
-//                   peers between the reduce-scatter and update halves of allreduce_opt.
+//   lars_norms    : LARS (and LAMB) per-tensor norms of a rank's reduced shard, exchanged among
+//                   the local peers between the reduce-scatter and update halves of allreduce_opt.
 //   bcast_pull    : startup broadcast, every rank pulls the root's parameters.
 //   ps_*          : asynchronous parameter server: workers apply gradients to
 //                   PS-resident weights with remote red.add (no barrier) and
@@ -90,15 +90,18 @@ __device__ __forceinline__ float block_sum_thread0(float v, float* red) {
 }
 
 // hyper[]: 0 lr, 1 momentum, 2 weight_decay, 3 grad_scale (1/world * loss scale),
-//          4 beta1 (Adam) | trust coefficient eta (LARS), 5 beta2, 6 eps, 7 step (Adam bias
-//          correction)
+//          4 beta1 (Adam, AdamW, LAMB) | trust coefficient eta (LARS), 5 beta2, 6 eps, 7 step
+//          (bias correction)
 template <int OPT>
 __device__ __forceinline__ float opt_update(float w, float g, float& s1, float& s2,
                                             const float* h, bool decay) {
   g *= h[3];
-  if (OPT == kOptAdam) {
-    // decoupled-from-nothing: classic Adam with L2 folded into the gradient
-    if (decay) g += h[2] * w;
+  if (OPT == kOptAdam || OPT == kOptAdamW) {
+    // kOptAdam: classic Adam with L2 folded into the gradient.  kOptAdamW: decoupled decay
+    // (torch.optim.AdamW), a multiply by 1 - lr wd, so wd = 0 leaves w and the step bit for bit
+    // Adam's
+    if (OPT == kOptAdam && decay) g += h[2] * w;
+    if (OPT == kOptAdamW && decay) w *= 1.f - h[0] * h[2];
     s1 = h[4] * s1 + (1.f - h[4]) * g;
     s2 = h[5] * s2 + (1.f - h[5]) * g * g;
     const float c1 = 1.f - __powf(h[4], h[7]);
@@ -123,6 +126,22 @@ __device__ __forceinline__ float lars_update(float w, float g, float& v, const f
   return w - v;
 }
 
+// LAMB's update direction, shared by the norm pass and the update so that both see the same
+// arithmetic: advances the moments s1 = m, s2 = v with the scaled gradient (Adam's rule) and
+// returns r = (m / c1) / (sqrt(v / c2) + eps) + wd w (wd w on decayed elements only).
+__device__ __forceinline__ float lamb_dir(float w, float g, float& s1, float& s2, const float* h,
+                                          bool decay) {
+  g *= h[3];
+  s1 = h[4] * s1 + (1.f - h[4]) * g;
+  s2 = h[5] * s2 + (1.f - h[5]) * g * g;
+  const float c1 = 1.f - __powf(h[4], h[7]);
+  const float c2 = 1.f - __powf(h[5], h[7]);
+  const float r = (s1 / c1) / (sqrtf(s2 / c2) + h[6]);
+  return decay ? r + h[2] * w : r;
+}
+
+constexpr bool has_state2(int opt) { return opt == kOptAdam || opt == kOptAdamW || opt == kOptLamb; }
+
 // PHASE splits the kernel for the hierarchical (several hosts) all-reduce: 1 = intra-host
 // reduce-scatter only (the sum over the local peers of this rank's shard replaces that shard of
 // the rank's OWN gradient buffer - peers only ever read the other shards of it); 2 = update +
@@ -136,6 +155,9 @@ __device__ __forceinline__ float lars_update(float w, float g, float& v, const f
 template <int OPT, bool MULTIMEM, int PHASE = 0, bool EMA = false>
 __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOptArgs a) {
   constexpr int kH = EMA ? kHyperEma : kHyper;
+  // the clipping reduce-scatter and the AdamW / LAMB instances wait without the timeout message,
+  // whose printf argument buffer would be their only stack frame
+  constexpr bool kReport = PHASE != 3 && OPT != kOptAdamW && OPT != kOptLamb;
   __shared__ float h[kH];
   if (threadIdx.x < kH) h[threadIdx.x] = a.hyper[threadIdx.x];
   const int world = a.world, rank = a.rank;
@@ -145,14 +167,15 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
     uint32_t* my = a.flags[rank] + a.slot * 32;
     if (blockIdx.x == 0 && threadIdx.x < world)
       st_release_sys(a.flags[threadIdx.x] + a.slot * 32 + rank, e);
-    if (threadIdx.x < world) wait_flag<PHASE != 3>(my + threadIdx.x, e);
+    if (threadIdx.x < world) wait_flag<kReport>(my + threadIdx.x, e);
   }
   // LARS: start offsets and trust ratios of the shard's adapted tensors.  Every rank sums the
   // rows of the norms table in rank order, so ranks whose shards split one tensor derive the
   // same ratio bit for bit.
   const long long* t_off = nullptr;
   const float* t_trust = nullptr;
-  if constexpr (OPT == kOptLars) {
+  // LAMB: the same tables, the ratio |w| / |r| of the step's update direction r (lamb_dir).
+  if constexpr (OPT == kOptLars || OPT == kOptLamb) {
     __shared__ long long s_off[kLarsMaxTensors + 1];
     __shared__ float s_trust[kLarsMaxTensors];
     for (int j = threadIdx.x; j <= a.lars_nt; j += blockDim.x) s_off[j] = a.lars_off[a.lars_t0 + j];
@@ -164,8 +187,13 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
         g2 += __uint_as_float(v.x);
         w2 += __uint_as_float(v.y);
       }
-      const float gn = sqrtf(g2) * fabsf(a.hyper[3]), wn = sqrtf(w2);
-      s_trust[j] = (wn > 0.f && gn > 0.f) ? a.hyper[4] * wn / (gn + a.hyper[2] * wn) : 1.f;
+      if constexpr (OPT == kOptLamb) {
+        const float rn = sqrtf(g2), wn = sqrtf(w2);   // (r already carries the scale)
+        s_trust[j] = (wn > 0.f && rn > 0.f) ? wn / rn : 1.f;
+      } else {
+        const float gn = sqrtf(g2) * fabsf(a.hyper[3]), wn = sqrtf(w2);
+        s_trust[j] = (wn > 0.f && gn > 0.f) ? a.hyper[4] * wn / (gn + a.hyper[2] * wn) : 1.f;
+      }
     }
     t_off = s_off;
     t_trust = s_trust;
@@ -181,8 +209,9 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
 
   // NVLS: a thread keeps kU x 2 = 16 multimem.ld_reduce (16 bytes each, reduced in the switch) in
   // flight; the peer-to-peer path already has 2 x world loads per element group in flight.  With
-  // the weight average 8 (the average's registers would otherwise spill at the 128-register bound)
-  constexpr int kU = MULTIMEM ? (EMA ? 4 : 8) : 1;
+  // the weight average 8 (the average's registers would otherwise spill at the 128-register bound),
+  // as AdamW's (its decay factor is one register too many at kU = 8)
+  constexpr int kU = MULTIMEM ? ((EMA || OPT == kOptAdamW) ? 4 : 8) : 1;
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x * 8;
   float sq = 0.f;   // PHASE 3: this thread's sum of squares, elements in visiting order
   for (long long i0 = lo + (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 8;
@@ -257,7 +286,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
       s1[0] = m0.x, s1[1] = m0.y, s1[2] = m0.z, s1[3] = m0.w;
       s1[4] = m1.x, s1[5] = m1.y, s1[6] = m1.z, s1[7] = m1.w;
     }
-    if (OPT == kOptAdam) {
+    if (has_state2(OPT)) {
       const float4 m0 = *reinterpret_cast<const float4*>(a.state2 + li);
       const float4 m1 = *reinterpret_cast<const float4*>(a.state2 + li + 4);
       s2[0] = m0.x, s2[1] = m0.y, s2[2] = m0.z, s2[3] = m0.w;
@@ -273,6 +302,16 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
       }
 #pragma unroll
       for (int j = 0; j < 8; ++j) w[j] = lars_update(w[j], g[j], s1[j], h, adapted, lrt);
+    } else if constexpr (OPT == kOptLamb) {
+      // adapted = decayed: lr * ratio of the element's tensor; the tail takes lr, no decay
+      const bool adapted = i < a.decay_end;
+      float lrt = h[0];
+      if (adapted) {
+        while (tj + 1 < a.lars_nt && t_off[tj + 1] <= i) ++tj;
+        lrt = h[0] * t_trust[tj];
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) w[j] -= lrt * lamb_dir(w[j], g[j], s1[j], s2[j], h, adapted);
     } else {
 #pragma unroll
     for (int j = 0; j < 8; ++j) w[j] = opt_update<OPT>(w[j], g[j], s1[j], s2[j], h, i + j < a.decay_end);
@@ -283,7 +322,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
       *reinterpret_cast<float4*>(a.state1 + li) = make_float4(s1[0], s1[1], s1[2], s1[3]);
       *reinterpret_cast<float4*>(a.state1 + li + 4) = make_float4(s1[4], s1[5], s1[6], s1[7]);
     }
-    if (OPT == kOptAdam) {
+    if (has_state2(OPT)) {
       *reinterpret_cast<float4*>(a.state2 + li) = make_float4(s2[0], s2[1], s2[2], s2[3]);
       *reinterpret_cast<float4*>(a.state2 + li + 4) = make_float4(s2[4], s2[5], s2[6], s2[7]);
     }
@@ -385,7 +424,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_opt_kernel(const AllreduceOp
       }
       if (threadIdx.x < world) {
         st_release_sys(a.flags[threadIdx.x] + a.slot * 32 + 16 + rank, e);
-        wait_flag<PHASE != 3>(a.flags[rank] + a.slot * 32 + 16 + threadIdx.x, e);
+        wait_flag<kReport>(a.flags[rank] + a.slot * 32 + 16 + threadIdx.x, e);
       }
       __syncthreads();
       if (threadIdx.x == 0) {
@@ -462,10 +501,20 @@ __global__ void flag_barrier_kernel(const BcastArgs a) {
 // LARS norm pass (see LarsNormArgs in ops.h).  Segments are reduced in a fixed thread -> element
 // mapping and a fixed tree, tensors sum their segments in order: the result does not depend on
 // which CTA takes which segment, and replicas that see the same gradients get the same bits.
+// LAMB: the first sum is of r = lamb_dir(...) instead of g, from the moments before the step (every
+// segment lies in the decayed head); the pass writes no state, the update advances it once.
 constexpr int kLarsNormThreads = 256;
+template <bool LAMB>
 __global__ void __launch_bounds__(kLarsNormThreads) lars_norms_kernel(const LarsNormArgs a) {
   __shared__ float red[2][kLarsNormThreads / 32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float* h = nullptr;
+  if constexpr (LAMB) {
+    __shared__ float s_h[kHyper];
+    if (threadIdx.x < kHyper) s_h[threadIdx.x] = a.hyper[threadIdx.x];
+    __syncthreads();
+    h = s_h;
+  }
   for (int s = blockIdx.x; s < a.nseg; s += gridDim.x) {
     const long long lo = a.seg[2 * s], hi = a.seg[2 * s + 1];
     float g2 = 0.f, w2 = 0.f;
@@ -474,10 +523,27 @@ __global__ void __launch_bounds__(kLarsNormThreads) lars_norms_kernel(const Lars
       const float4 g1 = *reinterpret_cast<const float4*>(a.grads + i + 4);
       const float4 w0 = *reinterpret_cast<const float4*>(a.master + i);
       const float4 w1 = *reinterpret_cast<const float4*>(a.master + i + 4);
-      g2 += g0.x * g0.x + g0.y * g0.y + g0.z * g0.z + g0.w * g0.w;
-      g2 += g1.x * g1.x + g1.y * g1.y + g1.z * g1.z + g1.w * g1.w;
-      w2 += w0.x * w0.x + w0.y * w0.y + w0.z * w0.z + w0.w * w0.w;
-      w2 += w1.x * w1.x + w1.y * w1.y + w1.z * w1.z + w1.w * w1.w;
+      if constexpr (LAMB) {
+        const float4 m0 = *reinterpret_cast<const float4*>(a.state1 + i);
+        const float4 m1 = *reinterpret_cast<const float4*>(a.state1 + i + 4);
+        const float4 v0 = *reinterpret_cast<const float4*>(a.state2 + i);
+        const float4 v1 = *reinterpret_cast<const float4*>(a.state2 + i + 4);
+        const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+        const float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+        float m[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
+        float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float r = lamb_dir(w[j], g[j], m[j], v[j], h, true);
+          g2 = fmaf(r, r, g2);
+          w2 = fmaf(w[j], w[j], w2);
+        }
+      } else {
+        g2 += g0.x * g0.x + g0.y * g0.y + g0.z * g0.z + g0.w * g0.w;
+        g2 += g1.x * g1.x + g1.y * g1.y + g1.z * g1.z + g1.w * g1.w;
+        w2 += w0.x * w0.x + w0.y * w0.y + w0.z * w0.z + w0.w * w0.w;
+        w2 += w1.x * w1.x + w1.y * w1.y + w1.z * w1.z + w1.w * w1.w;
+      }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -539,7 +605,7 @@ __global__ void __launch_bounds__(kLarsNormThreads) lars_norms_kernel(const Lars
     __syncthreads();
     if (threadIdx.x < world) {
       st_release_sys(a.flags[threadIdx.x] + a.slot * 32 + 16 + rank, e);
-      wait_flag(a.flags[rank] + a.slot * 32 + 16 + threadIdx.x, e);
+      wait_flag<!LAMB>(a.flags[rank] + a.slot * 32 + 16 + threadIdx.x, e);
     }
     __syncthreads();
     if (threadIdx.x == 0) *a.epoch = e;
@@ -852,9 +918,9 @@ cudaError_t launch_ar(const AllreduceOptArgs& a, int grid, cudaStream_t s, int p
   return cudaGetLastError();
 }
 
-// LARS needs whole-tensor norms of the reduced gradient between the two halves, so with peers it
-// always runs split; on a one-host NVLS communicator both halves use the multicast paths
-template <bool EMA>
+// LARS (and LAMB) need whole-tensor norms of the reduced gradient between the two halves, so with
+// peers they always run split; on a one-host NVLS communicator both halves use the multicast paths
+template <int OPT, bool EMA>
 cudaError_t launch_lars(const AllreduceOptArgs& a, int grid, cudaStream_t s, int phase) {
   if (a.lars_nt < 0 || a.lars_nt > kLarsMaxTensors) return cudaErrorInvalidValue;
   if (a.lars_nt > 0 && (a.lars_off == nullptr || a.lars_norms == nullptr))
@@ -868,11 +934,11 @@ cudaError_t launch_lars(const AllreduceOptArgs& a, int grid, cudaStream_t s, int
       allreduce_opt_kernel<kOptSgd, false, 1><<<grid, 512, 0, s>>>(a);
   } else if (phase == 2) {
     if (nvls)
-      allreduce_opt_kernel<kOptLars, true, 2, EMA><<<grid, 512, 0, s>>>(a);
+      allreduce_opt_kernel<OPT, true, 2, EMA><<<grid, 512, 0, s>>>(a);
     else
-      allreduce_opt_kernel<kOptLars, false, 2, EMA><<<grid, 512, 0, s>>>(a);
+      allreduce_opt_kernel<OPT, false, 2, EMA><<<grid, 512, 0, s>>>(a);
   } else if (a.world == 1) {
-    allreduce_opt_kernel<kOptLars, false, 0, EMA><<<grid, 512, 0, s>>>(a);
+    allreduce_opt_kernel<OPT, false, 0, EMA><<<grid, 512, 0, s>>>(a);
   } else {
     return cudaErrorInvalidValue;
   }
@@ -885,7 +951,9 @@ cudaError_t launch_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStream_
     case kOptSgd: return launch_ar<kOptSgd, EMA>(a, grid, s, phase);
     case kOptMomentum: return launch_ar<kOptMomentum, EMA>(a, grid, s, phase);
     case kOptAdam: return launch_ar<kOptAdam, EMA>(a, grid, s, phase);
-    case kOptLars: return launch_lars<EMA>(a, grid, s, phase);
+    case kOptLars: return launch_lars<kOptLars, EMA>(a, grid, s, phase);
+    case kOptAdamW: return launch_ar<kOptAdamW, EMA>(a, grid, s, phase);
+    case kOptLamb: return launch_lars<kOptLamb, EMA>(a, grid, s, phase);
     default: return cudaErrorInvalidValue;
   }
 }
@@ -898,11 +966,16 @@ cudaError_t allreduce_opt(const AllreduceOptArgs& a, int opt, int grid, cudaStre
   return a.ema != nullptr ? launch_opt<true>(a, opt, grid, s, phase)
                           : launch_opt<false>(a, opt, grid, s, phase);
 }
-cudaError_t lars_norms(const LarsNormArgs& a, cudaStream_t s) {
+cudaError_t lars_norms(const LarsNormArgs& a, cudaStream_t s, bool lamb) {
   if (a.world < 1 || a.world > kMaxRanks || a.nseg < 0 || a.nt < 0) return cudaErrorInvalidValue;
+  if (lamb && (a.hyper == nullptr || a.state1 == nullptr || a.state2 == nullptr))
+    return cudaErrorInvalidValue;
   int grid = a.nseg < kSmCount * 4 ? a.nseg : kSmCount * 4;
   if (grid < 1) grid = 1;
-  lars_norms_kernel<<<grid, kLarsNormThreads, 0, s>>>(a);
+  if (lamb)
+    lars_norms_kernel<true><<<grid, kLarsNormThreads, 0, s>>>(a);
+  else
+    lars_norms_kernel<false><<<grid, kLarsNormThreads, 0, s>>>(a);
   return cudaGetLastError();
 }
 cudaError_t grad_sumsq(const GradSumsqArgs& a, cudaStream_t s) {

@@ -12,7 +12,10 @@ CIFAR-10 network the reference actually trains.
 Large global batches: ``--optimizer lars`` (per-layer trust ratios, parallel/fused_optim.py) with
 a linear warm-up over ``--warmup_steps`` and polynomial decay to 0 at the last step
 (``resnet.poly_warmup_lr``), peaking at ``--base_lr`` (default: the linear-scaling rule
-0.1 * global batch / 256).
+0.1 * global batch / 256).  ``--optimizer lamb`` is LARS's Adam-style counterpart (layer-wise
+adaptive Adam) and takes the same schedule; ``--optimizer adamw`` is Adam with decoupled weight
+decay (``torch.optim.AdamW``).  Both want a smaller ``--base_lr`` than momentum.  ``--weight_decay``,
+``--beta1``, ``--beta2`` and ``--epsilon`` override the trainer's defaults.
 
 Held-out evaluation: ``--eval_steps N`` scores N synthetic ImageNet-shaped batches per rank
 (drawn from seeds disjoint from the training batch) every ``--eval_every K`` steps and after the
@@ -59,11 +62,16 @@ def parse(argv):
   p.add_argument("--no_graph", action="store_true")
   p.add_argument("--tensorboard", action="store_true")
   p.add_argument("--metrics", default=None, help="JSONL file for per-step metrics")
-  p.add_argument("--optimizer", default="momentum", choices=["momentum", "lars"])
+  p.add_argument("--optimizer", default="momentum", choices=["momentum", "adamw", "lars", "lamb"])
   p.add_argument("--base_lr", type=float, default=None,
                  help="peak learning rate (default: 0.1 * global batch / 256; resnet56: piecewise_lr)")
-  p.add_argument("--warmup_steps", type=int, default=0, help="lars: linear warm-up steps")
+  p.add_argument("--warmup_steps", type=int, default=0, help="lars, lamb: linear warm-up steps")
   p.add_argument("--trust_coefficient", type=float, default=0.001, help="lars: eta")
+  p.add_argument("--weight_decay", type=float, default=None,
+                 help="weight decay of the conv and dense weights (default: the trainer's)")
+  p.add_argument("--beta1", type=float, default=None, help="adamw, lamb: beta1 (default 0.9)")
+  p.add_argument("--beta2", type=float, default=None, help="adamw, lamb: beta2 (default 0.999)")
+  p.add_argument("--epsilon", type=float, default=None, help="adamw, lamb: epsilon (default 1e-7)")
   p.add_argument("--eval_steps", type=int, default=0,
                  help="synthetic held-out batches per rank and evaluation (0: no evaluation)")
   p.add_argument("--eval_every", type=int, default=0,
@@ -100,11 +108,17 @@ def main_fun(argv, ctx):
   comm = ctx.gradient_comm() if ctx.world_size > 1 else None   # one host: P2P/NVLS kernels; several: NCCL
   B = args.batch_size
   lars = args.optimizer == "lars"
+  poly = args.optimizer in ("lars", "lamb")   # the large-batch schedule
   if args.model == "resnet56":
     base_lr = args.base_lr if args.base_lr is not None else resnet.piecewise_lr(0, B * ctx.world_size)
   else:
     base_lr = args.base_lr if args.base_lr is not None else 0.1 * B * ctx.world_size / 256.0
   opt = dict(optimizer=args.optimizer, trust_coefficient=args.trust_coefficient) if lars else {}
+  if args.optimizer in ("adamw", "lamb"):
+    opt["optimizer"] = args.optimizer
+  for name in ("weight_decay", "beta1", "beta2", "epsilon"):
+    if getattr(args, name) is not None:
+      opt[name] = getattr(args, name)
   if args.num_classes is not None:
     opt["num_classes"] = args.num_classes
   if args.label_smoothing:
@@ -179,7 +193,7 @@ def main_fun(argv, ctx):
   t0 = time.time()
   total_steps = start + args.train_steps
   for step in range(start, total_steps):
-    if lars:   # hyper-parameters live in device memory: this works under graph replay
+    if poly:   # hyper-parameters live in device memory: this works under graph replay
       net.set_lr(resnet.poly_warmup_lr(step, total_steps, base_lr, args.warmup_steps))
     elif args.epochs_per_step:
       net.set_lr(resnet.piecewise_lr(int(step * args.epochs_per_step), B * ctx.world_size))

@@ -13,6 +13,8 @@ every evaluation scores it too (``val_avg_*``) and ``--export_dir`` exports it.
 ``--clip_norm c`` clips the averaged gradient to global norm c before each Adam update (Keras's
 ``global_clipnorm``) and prints the last step's ``grad_norm`` next to the loss (``inf``: only
 measure it).
+``--optimizer adamw | lamb`` replaces Adam by AdamW (decoupled weight decay) or LAMB (layer-wise
+adaptive Adam); ``--weight_decay`` decays the filters (with any of the three).
 Checkpoints every epoch (the reference's ModelCheckpoint callback) and evaluates every epoch on
 ``--eval_steps`` held-out synthetic batches per rank (the reference's ``validation_data``):
 validation loss, pixel accuracy and mean IoU.
@@ -53,6 +55,10 @@ def define_flags():
                       "evaluation also scores it (val_avg_*) and --export_dir exports it; the "
                       "checkpoints in --model_dir keep the live weights (and the average in the "
                       "optimizer state), so serving straight from model_dir serves the live weights")
+  p.add_argument("--optimizer", default=None, choices=["adam", "adamw", "lamb"],
+                 help="adam (default), adamw (decoupled weight decay) or lamb (layer-wise adaptive)")
+  p.add_argument("--weight_decay", type=float, default=None,
+                 help="weight decay of the filters, >= 0 (default 0)")
   p.add_argument("--clip_norm", type=float, default=None,
                  help="clip the averaged gradient to this global L2 norm (> 0; inf: only measure "
                       "it) and print grad_norm next to the loss")
@@ -67,8 +73,9 @@ def class_weights(text):
 def trainer_kwargs(args):
   """Keyword arguments the trainer gets from the flags beyond the common ones: only those of the
   options that are set (encoder fine-tuning, ignore_index, class_weights, the weight average,
-  gradient clipping)."""
-  names = ("encoder_trainable_from", "ignore_index", "class_weights", "ema_decay", "clip_norm")
+  gradient clipping, the optimizer and its weight decay)."""
+  names = ("encoder_trainable_from", "ignore_index", "class_weights", "ema_decay", "clip_norm",
+           "optimizer", "weight_decay")
   return {n: getattr(args, n) for n in names if getattr(args, n, None) is not None}
 
 

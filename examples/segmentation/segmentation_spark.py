@@ -24,6 +24,8 @@ neither the optimizer state nor the average.
 
 ``--clip_norm c`` clips the averaged gradient to global norm c before each Adam update (Keras's
 ``global_clipnorm``) and prints the step's ``grad_norm`` next to the loss (``inf``: only measure it).
+``--optimizer adamw | lamb`` replaces Adam by AdamW (decoupled weight decay) or LAMB (layer-wise
+adaptive Adam); ``--weight_decay`` decays the filters (with any of the three).
 
   python examples/segmentation/segmentation_spark.py --cluster_size 8 --batch_size 64 --steps 100
 """
@@ -67,7 +69,7 @@ def main_fun(args, ctx):
   B = args.batch_size
   # None: frozen encoder (as the reference), no ignored label, unweighted loss
   extra = {n: getattr(args, n) for n in ("encoder_trainable_from", "ignore_index", "class_weights",
-                                         "ema_decay", "clip_norm")
+                                         "ema_decay", "clip_norm", "optimizer", "weight_decay")
            if getattr(args, n, None) is not None}
   V = getattr(args, "classes", 3)
   net = unet.UNetTrainer(batch=B, image=IMG, classes=V, device="cuda:0", lr=args.learning_rate,
@@ -215,6 +217,10 @@ def define_flags():
                            "the --model_dir checkpoint holds the live weights only (no optimizer "
                            "state, so not the average): serving from model_dir serves the live "
                            "weights")
+  parser.add_argument("--optimizer", default=None, choices=["adam", "adamw", "lamb"],
+                      help="adam (default), adamw (decoupled weight decay) or lamb (layer-wise adaptive)")
+  parser.add_argument("--weight_decay", type=float, default=None,
+                      help="weight decay of the filters, >= 0 (default 0)")
   parser.add_argument("--clip_norm", type=float, default=None,
                       help="clip the averaged gradient to this global L2 norm (> 0; inf: only "
                            "measure it) and print grad_norm next to the loss")

@@ -150,6 +150,13 @@ def check_clip_norm(c, training=True):
   return c
 
 
+def check_adam_args(beta1, beta2, epsilon):
+  """Validated ``(beta1, beta2, epsilon)`` of a trainer (fused_optim.check_adam_args: ValueError
+  before anything is allocated)."""
+  from ..parallel.fused_optim import check_adam_args as check
+  return check(beta1, beta2, epsilon)
+
+
 def he_normal(fan_in):
   std = math.sqrt(2.0 / fan_in)
   return lambda shape, gen: torch.randn(shape, generator=gen) * std

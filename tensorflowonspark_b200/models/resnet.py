@@ -222,9 +222,11 @@ class ResNetTrainer(object):
   def __init__(self, depth=50, batch=256, image=224, num_classes=1000, device="cuda:0",
                lr=0.1, momentum=0.9, weight_decay=1e-4, comm=None, training=True, seed=1234,
                optimizer="momentum", trust_coefficient=0.001, label_smoothing=0.0,
-               ema_decay=None, clip_norm=None):
-    """``optimizer``: sgd | momentum | adam | lars (``trust_coefficient`` is LARS's eta; see
-    parallel/fused_optim.py).
+               ema_decay=None, clip_norm=None, beta1=0.9, beta2=0.999, epsilon=1e-7):
+    """``optimizer``: sgd | momentum | adam | adamw | lars | lamb (``trust_coefficient`` is LARS's
+    eta; see parallel/fused_optim.py).  adam folds ``weight_decay`` into the gradient (L2), adamw
+    decouples it (``torch.optim.AdamW``), lamb is layer-wise adaptive Adam (apex ``FusedLAMB``).
+    ``beta1``, ``beta2`` in [0, 1) and ``epsilon`` > 0 are the Adam family's (Keras's defaults).
 
     ``clip_norm``: None, or c > 0 (inf allowed): the averaged gradient is clipped to global norm
     c before the update, as ``torch.nn.utils.clip_grad_norm_`` (Keras's ``global_clipnorm``),
@@ -243,6 +245,7 @@ class ResNetTrainer(object):
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     self.ema_decay = engine.check_ema_decay(ema_decay, training)
     self.clip_norm = engine.check_clip_norm(clip_norm, training)
+    beta1, beta2, epsilon = engine.check_adam_args(beta1, beta2, epsilon)
     assert depth in self.CFG, "bottleneck depths: 50/101/152"
     self.device = torch.device(device)
     self.B, self.image, self.num_classes, self.depth = batch, image, num_classes, depth
@@ -372,7 +375,7 @@ class ResNetTrainer(object):
       self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, momentum=momentum,
                                   weight_decay=weight_decay, buckets=buckets,
                                   trust_coefficient=trust_coefficient, ema_decay=self.ema_decay,
-                                  clip_norm=self.clip_norm)
+                                  clip_norm=self.clip_norm, beta1=beta1, beta2=beta2, eps=epsilon)
     self.graph = None
     self.mean = [0.485, 0.456, 0.406]
     self.std = [0.229, 0.224, 0.225]
@@ -829,15 +832,18 @@ def build_served(state, depth=50, image=224, num_classes=1000, batch=None, **_):
 class CifarResNetTrainer(object):
   """ResNet-20/32/56 for 32x32 inputs (basic blocks, 16/32/64 channels) - the network the
   reference example actually trains (examples/resnet/resnet_cifar_dist.py:208, ``resnet56``,
-  momentum SGD, batch 128, weight decay 2e-4).  ``num_classes``, ``label_smoothing``,
-  ``ema_decay`` and ``clip_norm`` as in ResNetTrainer."""
+  momentum SGD, batch 128, weight decay 2e-4).  ``optimizer``, ``num_classes``,
+  ``label_smoothing``, ``ema_decay``, ``clip_norm``, ``beta1``, ``beta2`` and ``epsilon`` as in
+  ResNetTrainer."""
 
   def __init__(self, depth=56, batch=128, num_classes=10, device="cuda:0", lr=0.1, momentum=0.9,
                weight_decay=2e-4, comm=None, seed=1234, optimizer="momentum",
-               trust_coefficient=0.001, label_smoothing=0.0, ema_decay=None, clip_norm=None):
+               trust_coefficient=0.001, label_smoothing=0.0, ema_decay=None, clip_norm=None,
+               beta1=0.9, beta2=0.999, epsilon=1e-7):
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     self.ema_decay = engine.check_ema_decay(ema_decay)
     self.clip_norm = engine.check_clip_norm(clip_norm)
+    beta1, beta2, epsilon = engine.check_adam_args(beta1, beta2, epsilon)
     assert (depth - 2) % 6 == 0
     n = (depth - 2) // 6
     self.device = dev = torch.device(device)
@@ -902,7 +908,8 @@ class CifarResNetTrainer(object):
     from ..parallel.fused_optim import FusedOptimizer
     self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, momentum=momentum,
                                 weight_decay=weight_decay, trust_coefficient=trust_coefficient,
-                                ema_decay=self.ema_decay, clip_norm=self.clip_norm)
+                                ema_decay=self.ema_decay, clip_norm=self.clip_norm, beta1=beta1,
+                                beta2=beta2, eps=epsilon)
     self.graph = None
     self.mean, self.std = [0.4914, 0.4822, 0.4465], [0.2470, 0.2435, 0.2616]
 

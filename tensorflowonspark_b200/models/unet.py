@@ -331,6 +331,24 @@ def _trainable_from(k, training):
   return int(k)
 
 
+def _optimizer_args(optimizer, weight_decay, beta1, beta2, epsilon, training, defaults):
+  """Validated ``(optimizer, weight_decay, beta1, beta2, epsilon)``: optimizer one of adam | adamw
+  | lamb, weight_decay finite >= 0, the Adam family's betas and epsilon; any value other than the
+  default needs training=True (ValueError otherwise)."""
+  from ..parallel.fused_optim import check_weight_decay
+  if optimizer not in ("adam", "adamw", "lamb"):
+    raise ValueError("optimizer must be one of adam | adamw | lamb, got {!r}".format(optimizer))
+  weight_decay = check_weight_decay(weight_decay)
+  beta1, beta2, epsilon = engine.check_adam_args(beta1, beta2, epsilon)
+  args = (optimizer, weight_decay, beta1, beta2, epsilon)
+  if not training:
+    for name, v, d in zip(("optimizer", "weight_decay", "beta1", "beta2", "epsilon"), args, defaults):
+      if v != d:
+        raise ValueError("{} needs training=True (an inference-only U-Net has no optimizer)"
+                         .format(name))
+  return args
+
+
 #: most classes a U-Net can have: its masks (served output, DataFeed wire format) are uint8
 MAX_CLASSES = 256
 
@@ -437,16 +455,29 @@ class UNetTrainer(object):
 
   ``clip_norm``: None, or c > 0, inf allowed (training only): the averaged gradient is clipped to
   global norm c before the Adam update, as ``torch.nn.utils.clip_grad_norm_``; ``grad_norm`` holds
-  the norm of each step (``clip_norm=float("inf")`` only measures it)."""
+  the norm of each step (``clip_norm=float("inf")`` only measures it).
+
+  ``optimizer`` (training only): adam (default; L2 ``weight_decay`` folded into the gradient),
+  adamw (decoupled decay, ``torch.optim.AdamW``) or lamb (layer-wise adaptive Adam, apex
+  ``FusedLAMB``); see parallel/fused_optim.py.  ``weight_decay``: a finite real >= 0, applied to
+  the filters (conv weights, trainable encoder filters included), never to biases.  ``beta1``,
+  ``beta2`` in [0, 1) and ``epsilon`` > 0 as Keras's Adam.  With ``training=False`` each of these
+  must keep its default."""
 
   UP = (512, 256, 128, 64)
+  # optimizer, weight_decay, beta1, beta2, epsilon: the defaults (the U-Net's Adam before they
+  # were options)
+  OPT_DEFAULTS = ("adam", 0.0, 0.9, 0.999, 1e-7)
 
   def __init__(self, batch=64, image=128, classes=3, device="cuda:0", lr=1e-3, comm=None, seed=1234,
                training=True, encoder_trainable_from=None, ignore_index=None, class_weights=None,
-               ema_decay=None, clip_norm=None):
+               ema_decay=None, clip_norm=None, optimizer="adam", weight_decay=0.0, beta1=0.9,
+               beta2=0.999, epsilon=1e-7):
     classes = _classes(classes)
     self.ema_decay = engine.check_ema_decay(ema_decay, training)
     self.clip_norm = engine.check_clip_norm(clip_norm, training)
+    opt_args = _optimizer_args(optimizer, weight_decay, beta1, beta2, epsilon, training,
+                               self.OPT_DEFAULTS)
     k = self.encoder_trainable_from = _trainable_from(encoder_trainable_from, training)
     self.ignore_index = _ignore_index(ignore_index)
     self.class_weights = _class_weights(class_weights, classes)
@@ -523,8 +554,10 @@ class UNetTrainer(object):
     self.in_u8 = _buf((B, image, image, 3), dev, torch.uint8)
     if tr:
       from ..parallel.fused_optim import FusedOptimizer
-      self.optim = FusedOptimizer(st, comm=comm, opt="adam", lr=lr, weight_decay=0.0,
-                                  ema_decay=self.ema_decay, clip_norm=self.clip_norm)
+      optimizer, weight_decay, beta1, beta2, epsilon = opt_args
+      self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, weight_decay=weight_decay,
+                                  ema_decay=self.ema_decay, clip_norm=self.clip_norm, beta1=beta1,
+                                  beta2=beta2, eps=epsilon)
     self.graph = None
     self._live = None   # (weights, aux32) saved while an averaged evaluation has the average in
 

@@ -6,7 +6,8 @@ examples/mnist/keras/mnist_spark.py:11,55-66; TFoS itself only provides the
 cluster spec, tensorflowonspark/TFSparkNode.py:373-384) *and* the Keras
 optimizer update that follows it: one kernel per gradient bucket pulls the peer
 shards over NVLink, averages, applies SGD / momentum / Adam to the fp32 master
-shard and stores the new bf16 weights into every rank's weight buffer.
+shard and stores the new bf16 weights into every rank's weight buffer (also AdamW, LARS and
+LAMB, below).
 
 Buckets are contiguous ranges of the flat parameter vector.  A model may pass
 ``buckets=[(begin, end, tag), ...]`` and call ``launch(tag)`` from inside its
@@ -31,6 +32,20 @@ separate, deterministic norm pass (csrc/optim_comm.cu ``lars_norms``) between th
 and the update: ``[PHASE 1 ->] norms (+ exchange of per-tensor partials among the local peers)
 -> update [+ all-gather]``.  A bucket bound must not cut an adapted tensor.
 
+AdamW (``opt="adamw"``) is ``torch.optim.AdamW`` / Keras's ``AdamW``: decoupled weight decay on the
+decayed head, ``w = w (1 - lr wd)``, then Adam's step ``w = w - lr (m / c1) / (sqrt(v / c2) + eps)``
+(``opt="adam"`` folds ``wd w`` into the gradient instead).  With ``wd = 0`` it is bitwise Adam.
+
+LAMB (``opt="lamb"``, the LAMB paper's Algorithm 2 as in apex ``FusedLAMB`` / TF Addons ``LAMB``)
+is to Adam what LARS is to momentum: ``r = (m / c1) / (sqrt(v / c2) + eps) + wd w`` and, for each
+adapted tensor, ``w = w - lr ratio r`` with ``ratio = |w| / |r|`` (1 if a norm is 0) from the fp32
+master before the step and the step's new moments; the tail takes ``w = w - lr r`` without decay.
+``trust_coefficient`` is not used.  It runs in LARS's shape: the same tables and bucket rules, and
+a norm pass between the reduce-scatter and the update that recomputes m', v' and r in registers
+(it writes no state, so the update alone advances it, once per step).  adam, adamw and lamb share
+their state (``state1 = m``, ``state2 = v``, ``hyper[7] = t``) and hyper layout, so a checkpoint of
+one continues under the others.
+
 Weight average (``ema_decay=d``): the update kernels also keep an exponential moving average of
 every parameter, ``ema``, placed and sharded like ``state1``.  The first update after a reset
 (construction, ``reset_average()``, loading a state without it) copies the new master, each later
@@ -48,9 +63,11 @@ gradient only exists inside the fused kernels, so they compute its norm N over t
 clamped to at most 1 (a NaN norm gives NaN, an infinite one 0, as in torch) is folded into the
 scale: the update kernels read a per-step copy of ``hyper``, ``hyper_step``, whose slot 3 is
 ``fl(hyper[3] * coef)``, so every optimizer (and LARS's trust ratio) sees the clipped gradient and
-weight decay is added after clipping.  When ``c / (N + 1e-6) >= 1`` (``c = inf`` included) the step
-is bitwise the unclipped one.  No bucket may update before every bucket is reduced, so a bucket's
-``launch(tag)`` runs only its reduction and sum of squares; ``finish()`` (or ``after_replay()``)
+weight decay is added after clipping.  LAMB's ratio is not linear in the gradient, so its norm pass
+must see the clipped one: with clipping it runs after ``clip_finalize``, reading ``hyper_step``.
+When ``c / (N + 1e-6) >= 1`` (``c = inf`` included) the step is bitwise the unclipped one.  No
+bucket may update before every bucket is reduced, so a bucket's ``launch(tag)`` runs only its
+reduction and sum of squares; ``finish()`` (or ``after_replay()``)
 finalises N into ``grad_norm`` and runs every bucket's update:
 
   no peers / GroupComm : [NCCL all-reduce ->] grad_sumsq of the bucket
@@ -59,16 +76,23 @@ finalises N into ``grad_norm`` and runs every bucket's update:
   HierComm             : [PHASE 1 ->] NCCL all-reduce of the shard -> grad_sumsq of the shard
                          (+ exchange among the local peers)
   LARS                 : any of the above, then the bucket's lars_norms
-  then, once           : clip_finalize -> every bucket's update (PHASE 0 or 2) reading hyper_step
+  then, once           : clip_finalize -> every bucket's [LAMB norm pass ->] update (PHASE 0 or 2),
+                         both reading hyper_step
 """
 import bisect
+import math
 import numbers
 
 import torch
 
 from .. import ops
 
+# kernel codes (csrc/ops.h kOpt*).  OPTS keeps the four it has always had (code that enumerates it
+# sees the same set); OPTIMIZERS is every optimizer FusedOptimizer runs.
 OPTS = {"sgd": 0, "momentum": 1, "adam": 2, "lars": 3}
+OPTIMIZERS = dict(OPTS, adamw=4, lamb=5)
+# the optimizers with Adam's state: state1 = m, state2 = v, hyper[7] = step
+ADAM_STATE = (OPTIMIZERS["adam"], OPTIMIZERS["adamw"], OPTIMIZERS["lamb"])
 # csrc/ops.h kLarsMaxTensors: adapted tensors one shard of a bucket may intersect
 LARS_MAX_TENSORS = 256
 # elements per work item of the LARS norm pass (one CTA reduces one segment at a time)
@@ -97,6 +121,26 @@ def check_clip_norm(c):
   if isinstance(c, bool) or not isinstance(c, numbers.Real) or not float(c) > 0.0:
     raise ValueError("clip_norm must be None or a real number > 0 (inf allowed), got {!r}".format(c))
   return float(c)
+
+
+def check_adam_args(beta1, beta2, epsilon):
+  """Validated ``(beta1, beta2, epsilon)`` of the Adam family as floats: each beta a real number in
+  [0, 1), epsilon a finite real number > 0 (ValueError otherwise, bools included)."""
+  for name, b in (("beta1", beta1), ("beta2", beta2)):
+    if isinstance(b, bool) or not isinstance(b, numbers.Real) or not 0.0 <= float(b) < 1.0:
+      raise ValueError("{} must be a real number in [0, 1), got {!r}".format(name, b))
+  if (isinstance(epsilon, bool) or not isinstance(epsilon, numbers.Real)
+      or not (math.isfinite(float(epsilon)) and float(epsilon) > 0.0)):
+    raise ValueError("epsilon must be a finite real number > 0, got {!r}".format(epsilon))
+  return float(beta1), float(beta2), float(epsilon)
+
+
+def check_weight_decay(wd):
+  """Validated ``weight_decay``: a finite real number >= 0 as a float (ValueError otherwise)."""
+  if (isinstance(wd, bool) or not isinstance(wd, numbers.Real)
+      or not (math.isfinite(float(wd)) and float(wd) >= 0.0)):
+    raise ValueError("weight_decay must be a finite real number >= 0, got {!r}".format(wd))
+  return float(wd)
 
 
 def _shard(b, e, world, rank):
@@ -163,8 +207,9 @@ class FusedOptimizer(object):
     self.ema_decay = check_ema_decay(ema_decay)
     self.clip_norm = check_clip_norm(clip_norm)
     self.store, self.comm = store, comm
-    self.opt = OPTS[opt]
-    self.lars = self.opt == OPTS["lars"]
+    self.opt = OPTIMIZERS[opt]
+    self.lars = self.opt == OPTIMIZERS["lars"]
+    self.lamb = self.opt == OPTIMIZERS["lamb"]
     if self.lars:
       beta1 = trust_coefficient
     dev = store.master.device
@@ -196,7 +241,7 @@ class FusedOptimizer(object):
         return t
       return torch.zeros_like(store.master)
     self.state1 = _state("state1") if self.opt != 0 else None
-    self.state2 = _state("state2") if self.opt == 2 else None
+    self.state2 = _state("state2") if self.opt in ADAM_STATE else None
     self.ema = _state("ema") if self.ema_decay is not None else None
     self._avg = None   # averaged_weights()'s buffers, allocated on first use
     self.step_count = 0
@@ -208,7 +253,7 @@ class FusedOptimizer(object):
     for b, e, _ in buckets:
       assert b % 8 == 0 and b < e <= n, "bucket bounds must be multiples of 8 inside the vector"
     self.buckets = list(buckets)
-    if self.lars:   # (validates the buckets before anything is allocated)
+    if self.lars or self.lamb:   # (validates the buckets before anything is allocated)
       self._lars_bounds = [s["offset"] for s in store.order if s["decay"]] + [store.decay_end]
       self._lars_tab = lars_tables(self._lars_bounds, self.buckets, self.world)
     self._args = []
@@ -246,7 +291,7 @@ class FusedOptimizer(object):
           d["grid"] = 48
       self._args.append(d)
     self.nvls = bool(self._args and self._args[0].get("grads_mc"))
-    if self.lars:
+    if self.lars or self.lamb:
       self._build_lars(store, comm)
     self.grad_norm = None
     if self.clip_norm is not None:
@@ -265,8 +310,9 @@ class FusedOptimizer(object):
 
   def _build_lars(self, store, comm):
     """Device tables of the norm pass and the norms table: ``world`` rows of ``T`` entries
-    {sum g^2, sum w^2, 0, 0}, row r written by rank r (symmetric with peers, multicast on NVLS).
-    Entries of tensors outside a rank's shards stay 0, so every rank may sum all rows."""
+    {sum g^2 (LAMB: sum r^2), sum w^2, 0, 0}, row r written by rank r (symmetric with peers,
+    multicast on NVLS).  Entries of tensors outside a rank's shards stay 0, so every rank may sum
+    all rows."""
     dev = self.device
     T = len(self._lars_bounds) - 1
     n_norms = self.world * max(1, T) * 4
@@ -296,6 +342,8 @@ class FusedOptimizer(object):
             "norms_mc": norms_mc, "block_counter": counter.data_ptr()}
       if self.world > 1:
         nd.update(flags=d["flags"], epoch=d["epoch"])
+      if self.lamb:
+        nd.update(lamb=1, hyper=d["hyper"], state1=d["state1"], state2=d["state2"])
       self._lars_args.append(nd)
       self._lars_phase.append((dict(d, phase=1), dict(d, phase=2)))
 
@@ -318,7 +366,7 @@ class FusedOptimizer(object):
     self._clip_phase1, self._clip_reduce, self._clip_update = [], [], []
     hs = self.hyper_step.data_ptr()
     for i, d in enumerate(self._args):
-      if self.lars:
+      if self.lars or self.lamb:
         phase1, phase2 = self._lars_phase[i]
         one = self._args[i]
       else:
@@ -337,6 +385,8 @@ class FusedOptimizer(object):
       self._clip_reduce.append(red)
       self._clip_update.append(dict(phase2 if (self.world > 1 or self.hier_mode) else one,
                                     hyper=hs))
+    # LAMB: the norm pass of the clipped step, run by _update_all() after clip_finalize
+    self._clip_lamb_norms = [dict(nd, hyper=hs) for nd in self._lars_args] if self.lamb else None
     self._clip_pending = False
 
   def set_lr(self, lr):
@@ -348,7 +398,7 @@ class FusedOptimizer(object):
     self._launched = set()
 
   def _bump_step(self):
-    if self.opt == 2:
+    if self.opt in ADAM_STATE:
       self.step_count += 1
       self.hyper[7:8].add_(1.0)
     if self.ema is not None:
@@ -471,7 +521,7 @@ class FusedOptimizer(object):
       self._run_bucket(i)
 
   def _run_bucket(self, i):
-    if self.lars:
+    if self.lars or self.lamb:
       return self._run_bucket_lars(i)
     if self.hier_mode:
       d = self._args[i]
@@ -489,7 +539,8 @@ class FusedOptimizer(object):
 
   def _run_bucket_lars(self, i):
     """reduce-scatter -> per-tensor norms (+ exchange among the local peers) -> update +
-    all-gather, all on the bucket's flag slot.  Without peers: norms -> one-pass update."""
+    all-gather, all on the bucket's flag slot.  Without peers: norms -> one-pass update.  LARS and
+    LAMB (its norm pass reads the hyper vector and the moments, see _build_lars)."""
     phase1, phase2 = self._lars_phase[i]
     if self.hier_mode:
       if self.world > 1:
@@ -513,7 +564,8 @@ class FusedOptimizer(object):
 
   def _reduce_bucket(self, i):
     """Clipping, first half of bucket i: its gradient fully reduced and the sum of squares of
-    this rank's share of it in the norm table (+ LARS norms); no update."""
+    this rank's share of it in the norm table (+ LARS norms; LAMB's wait for the clipped scale,
+    _update_all()); no update."""
     if self.hier_mode:
       if self.world > 1:
         ops.K.allreduce_opt(self._clip_phase1[i])
@@ -540,7 +592,9 @@ class FusedOptimizer(object):
     ops.K.clip_finalize(self.clip_sq.data_ptr(), self.world, len(self.buckets),
                         self.hyper.data_ptr(), self.hyper.numel(), self.clip_norm,
                         self.hyper_step.data_ptr(), self.grad_norm.data_ptr())
-    for d in self._clip_update:
+    for i, d in enumerate(self._clip_update):
+      if self.lamb:
+        ops.K.lars_norms(self._clip_lamb_norms[i])
       ops.K.allreduce_opt(d)
     self._clip_pending = False
 

@@ -45,6 +45,21 @@ KERNELS = [
     ("allreduce_phase3_sumsq_nvls", r"allreduce_opt_kernel<0, true, 3, false>"),
     ("grad_sumsq", r"grad_sumsq_kernel"),
     ("clip_finalize", r"clip_finalize_kernel"),
+    # AdamW (opt 4) and LAMB (opt 5, LARS's shape) with and without the weight average, and the
+    # LAMB norm pass
+    ("allreduce_opt_adamw_p2p", r"allreduce_opt_kernel<4, false, 0, false>"),
+    ("allreduce_opt_adamw_nvls", r"allreduce_opt_kernel<4, true, 0, false>"),
+    ("allreduce_phase2_adamw", r"allreduce_opt_kernel<4, false, 2, false>"),
+    ("allreduce_opt_adamw_p2p_ema", r"allreduce_opt_kernel<4, false, 0, true>"),
+    ("allreduce_opt_adamw_nvls_ema", r"allreduce_opt_kernel<4, true, 0, true>"),
+    ("allreduce_phase2_adamw_ema", r"allreduce_opt_kernel<4, false, 2, true>"),
+    ("allreduce_opt_lamb_one_rank", r"allreduce_opt_kernel<5, false, 0, false>"),
+    ("allreduce_phase2_lamb_p2p", r"allreduce_opt_kernel<5, false, 2, false>"),
+    ("allreduce_phase2_lamb_nvls", r"allreduce_opt_kernel<5, true, 2, false>"),
+    ("allreduce_opt_lamb_one_rank_ema", r"allreduce_opt_kernel<5, false, 0, true>"),
+    ("allreduce_phase2_lamb_p2p_ema", r"allreduce_opt_kernel<5, false, 2, true>"),
+    ("allreduce_phase2_lamb_nvls_ema", r"allreduce_opt_kernel<5, true, 2, true>"),
+    ("lamb_norms", r"lars_norms_kernel<true>"),
     ("ps_apply_momentum", r"ps_apply_kernel<1>"),
     ("ps_push_slot", r"ps_push_slot_kernel"),
     ("ps_pull_model", r"ps_pull_model_kernel"),
