@@ -383,13 +383,24 @@ void bn_bwd_apply(const Tensor& dy, const Tensor& x, c10::optional<Tensor> y, co
                   const Tensor& mean, const Tensor& invstd, const Tensor& dgamma,
                   const Tensor& dbeta, Tensor dx, c10::optional<Tensor> dres, int relu,
                   c10::optional<Tensor> fscale, c10::optional<Tensor> fshift,
-                  c10::optional<Tensor> sum_g, c10::optional<Tensor> sum_gx) {
+                  c10::optional<Tensor> sum_g, c10::optional<Tensor> sum_gx,
+                  c10::optional<Tensor> acc_dgamma, c10::optional<Tensor> acc_dbeta) {
   const int C = x.size(-1);
+  const bool acc = acc_dgamma.has_value() && acc_dgamma->defined();
+  TORCH_CHECK(acc == (acc_dbeta.has_value() && acc_dbeta->defined()),
+              "bn_bwd_apply: acc_dgamma and acc_dbeta go together");
+  if (acc) {
+    need(*acc_dgamma, torch::kFloat32, "acc_dgamma");
+    need(*acc_dbeta, torch::kFloat32, "acc_dbeta");
+    need_numel(*acc_dgamma, C, "bn_bwd_apply", "acc_dgamma");
+    need_numel(*acc_dbeta, C, "bn_bwd_apply", "acc_dbeta");
+  }
   check(tfos::bn_bwd_apply(dy.data_ptr(), x.data_ptr(), optptr(y), gamma.data_ptr<float>(),
                            mean.data_ptr<float>(), invstd.data_ptr<float>(),
                            dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), optf(fscale),
                            optf(fshift), dx.data_ptr(), const_cast<void*>(optptr(dres)),
-                           x.numel() / C, C, relu, optf(sum_g), optf(sum_gx), cur_stream()),
+                           x.numel() / C, C, relu, optf(sum_g), optf(sum_gx), cur_stream(),
+                           optf(acc_dgamma), optf(acc_dbeta)),
         "bn_bwd_apply");
 }
 void stem_bn_relu_pool_fwd(const Tensor& x, Tensor y, Tensor idx, const Tensor& sum,
@@ -424,8 +435,12 @@ void stem_bn_relu_pool_fwd(const Tensor& x, Tensor y, Tensor idx, const Tensor& 
 }
 void stem_pool_bn_bwd(const Tensor& dy_pool, const Tensor& idx, const Tensor& x, const Tensor& gamma,
                       const Tensor& mean, const Tensor& invstd, const Tensor& scale,
-                      const Tensor& shift, Tensor dgamma, Tensor dbeta, Tensor dx) {
+                      const Tensor& shift, Tensor dgamma, Tensor dbeta, Tensor dx,
+                      c10::optional<Tensor> acc_dgamma, c10::optional<Tensor> acc_dbeta) {
   const char* what = "stem_pool_bn_bwd";
+  const bool acc = acc_dgamma.has_value() && acc_dgamma->defined();
+  TFOS_REQUIRE(acc == (acc_dbeta.has_value() && acc_dbeta->defined()), what,
+               ": acc_dgamma and acc_dbeta go together");
   check_maxpool(x, dy_pool, &idx, 3, 2, 1, "x", "dy_pool", what);
   need(dx, torch::kBFloat16, "dx");
   TFOS_REQUIRE(dx.sizes() == x.sizes(), what, ": dx must have x's shape ", shape_str(x), ", got ",
@@ -438,12 +453,20 @@ void stem_pool_bn_bwd(const Tensor& dy_pool, const Tensor& idx, const Tensor& x,
                                                          &shift, &dgamma, &dbeta};
   for (const Tensor* t : vectors)
     need_numel(*t, C, what, "per-channel vector");
+  if (acc) {
+    need(*acc_dgamma, torch::kFloat32, "acc_dgamma");
+    need(*acc_dbeta, torch::kFloat32, "acc_dbeta");
+    need_numel(*acc_dgamma, C, what, "per-channel vector");
+    need_numel(*acc_dbeta, C, what, "per-channel vector");
+  }
   check(tfos::stem_pool_bn_bwd(dy_pool.data_ptr(), idx.data_ptr<uint8_t>(), x.data_ptr(),
                                gamma.data_ptr<float>(), mean.data_ptr<float>(),
                                invstd.data_ptr<float>(), scale.data_ptr<float>(),
                                shift.data_ptr<float>(), dgamma.data_ptr<float>(),
                                dbeta.data_ptr<float>(), dx.data_ptr(), x.size(0), x.size(1),
-                               x.size(2), x.size(3), dy_pool.size(1), dy_pool.size(2), cur_stream()),
+                               x.size(2), x.size(3), dy_pool.size(1), dy_pool.size(2), cur_stream(),
+                               acc ? acc_dgamma->data_ptr<float>() : nullptr,
+                               acc ? acc_dbeta->data_ptr<float>() : nullptr),
         "stem_pool_bn_bwd");
 }
 void add_act(const Tensor& a, c10::optional<Tensor> b, Tensor out, int act) {
@@ -740,7 +763,7 @@ inline bool aligned16(const Tensor& t) {
 }
 void depthwise3x3_bwd(const Tensor& x, const Tensor& w, const Tensor& y, const Tensor& dy,
                       c10::optional<Tensor> add, int64_t add_off, Tensor dx, Tensor dw, Tensor dbias,
-                      Tensor dbias_in, Tensor scratch, int64_t stride) {
+                      Tensor dbias_in, Tensor scratch, int64_t stride, bool accumulate) {
   need(x, torch::kBFloat16, "x");
   need(w, torch::kBFloat16, "w");
   need(y, torch::kBFloat16, "y");
@@ -791,7 +814,7 @@ void depthwise3x3_bwd(const Tensor& x, const Tensor& w, const Tensor& y, const T
   check(tfos::depthwise3x3_bwd(x.data_ptr(), w.data_ptr(), y.data_ptr(), dy.data_ptr(), ap, ld,
                                dx.data_ptr(), dw.data_ptr<float>(), dbias.data_ptr<float>(),
                                dbias_in.data_ptr<float>(), scratch.data_ptr<float>(), N, H, W, C,
-                               stride, cur_stream()),
+                               stride, cur_stream(), accumulate),
         "depthwise3x3_bwd");
 }
 void copy_channels(const Tensor& src, Tensor dst, int C, int src_off, int dst_off) {
@@ -1121,9 +1144,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("bn_bwd_apply", &bn_bwd_apply, py::arg("dy"), py::arg("x"), py::arg("y"), py::arg("gamma"),
         py::arg("mean"), py::arg("invstd"), py::arg("dgamma"), py::arg("dbeta"), py::arg("dx"),
         py::arg("dres"), py::arg("relu"), py::arg("fscale"), py::arg("fshift"),
-        py::arg("sum_g") = py::none(), py::arg("sum_gx") = py::none());
+        py::arg("sum_g") = py::none(), py::arg("sum_gx") = py::none(),
+        py::arg("acc_dgamma") = py::none(), py::arg("acc_dbeta") = py::none());
   m.def("stem_bn_relu_pool_fwd", &stem_bn_relu_pool_fwd);
-  m.def("stem_pool_bn_bwd", &stem_pool_bn_bwd);
+  m.def("stem_pool_bn_bwd", &stem_pool_bn_bwd, py::arg("dy_pool"), py::arg("idx"), py::arg("x"),
+        py::arg("gamma"), py::arg("mean"), py::arg("invstd"), py::arg("scale"), py::arg("shift"),
+        py::arg("dgamma"), py::arg("dbeta"), py::arg("dx"), py::arg("acc_dgamma") = py::none(),
+        py::arg("acc_dbeta") = py::none());
   m.def("add_act", &add_act);
   m.def("relu_bwd", &relu_bwd);
   m.def("colsum", &colsum);
@@ -1154,7 +1181,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("C"), py::arg("stride"));
   m.def("depthwise3x3_bwd", &depthwise3x3_bwd, py::arg("x"), py::arg("w"), py::arg("y"),
         py::arg("dy"), py::arg("add"), py::arg("add_off"), py::arg("dx"), py::arg("dw"),
-        py::arg("dbias"), py::arg("dbias_in"), py::arg("scratch"), py::arg("stride"));
+        py::arg("dbias"), py::arg("dbias_in"), py::arg("scratch"), py::arg("stride"),
+        py::arg("accumulate") = false);
   m.def("copy_channels", &copy_channels);
   m.def("pixel_xent", &pixel_xent, py::arg("logits"), py::arg("labels"), py::arg("dlogits"),
         py::arg("loss_sum"), py::arg("correct"), py::arg("V"), py::arg("scale"),

@@ -150,15 +150,22 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
 // dx = A*g + B*x + K with per-channel A = gamma*invstd, B = -A*invstd*dgamma/M,
 // K = -A*dbeta/M - B*mean.  Optionally also stores the masked g (gradient of the residual
 // branch); dres may alias dy (same element read before it is written by the same thread).
-__global__ void __launch_bounds__(kThreads, 2)
-bn_bwd_apply_kernel(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x,
-                    const __nv_bfloat16* __restrict__ y, const float* __restrict__ gamma,
-                    const float* __restrict__ mean, const float* __restrict__ invstd,
-                    float* dgamma, float* dbeta,
-                    const float* __restrict__ fscale, const float* __restrict__ fshift,
-                    __nv_bfloat16* __restrict__ dx, __nv_bfloat16* dres, long long P, int C,
-                    int relu, float inv_count, const int rev,
-                    const float* __restrict__ sum_g, const float* __restrict__ sum_gx) {
+//
+// ACC (gradient accumulation over micro-batches): dgamma / dbeta hold THIS micro-batch's values
+// (per-step scratch written by the reduce; not read on the fused path), dx is formed from them, and
+// the thread that publishes on the fused path adds them to the parameter gradient acc_dgamma /
+// acc_dbeta, which holds the running sum of the earlier micro-batches.
+template <bool ACC>
+__device__ __forceinline__ void
+bn_bwd_apply_body(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x,
+                  const __nv_bfloat16* __restrict__ y, const float* __restrict__ gamma,
+                  const float* __restrict__ mean, const float* __restrict__ invstd,
+                  float* dgamma, float* dbeta,
+                  const float* __restrict__ fscale, const float* __restrict__ fshift,
+                  __nv_bfloat16* __restrict__ dx, __nv_bfloat16* dres, long long P, int C,
+                  int relu, float inv_count, const int rev,
+                  const float* __restrict__ sum_g, const float* __restrict__ sum_gx,
+                  float* acc_dgamma, float* acc_dbeta) {
   const Geo G = geo(C);
   if (G.r_in >= G.rl) return;
   const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
@@ -180,13 +187,17 @@ bn_bwd_apply_kernel(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x
           // sum(g) and sum(g x) arrive raw; one thread per channel publishes dgamma / dbeta
           db = sum_g[ch];
           dg = is * (sum_gx[ch] - mean[ch] * db);
-          if (blockIdx.x == 0 && G.r_in == 0) {
+          if (!ACC && blockIdx.x == 0 && G.r_in == 0) {
             dgamma[ch] = dg;
             dbeta[ch] = db;
           }
         } else {
           dg = dgamma[ch];
           db = dbeta[ch];
+        }
+        if (ACC && blockIdx.x == 0 && G.r_in == 0) {   // one thread per channel: no atomics
+          acc_dgamma[ch] += dg;
+          acc_dbeta[ch] += db;
         }
         a[h] = gamma[ch] * is;
         b[h] = -a[h] * is * dg * inv_count;
@@ -238,6 +249,33 @@ bn_bwd_apply_kernel(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(kThreads, 2)
+bn_bwd_apply_kernel(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x,
+                    const __nv_bfloat16* __restrict__ y, const float* __restrict__ gamma,
+                    const float* __restrict__ mean, const float* __restrict__ invstd,
+                    float* dgamma, float* dbeta,
+                    const float* __restrict__ fscale, const float* __restrict__ fshift,
+                    __nv_bfloat16* __restrict__ dx, __nv_bfloat16* dres, long long P, int C,
+                    int relu, float inv_count, const int rev,
+                    const float* __restrict__ sum_g, const float* __restrict__ sum_gx) {
+  bn_bwd_apply_body<false>(dy, x, y, gamma, mean, invstd, dgamma, dbeta, fscale, fshift, dx, dres,
+                           P, C, relu, inv_count, rev, sum_g, sum_gx, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(kThreads, 2)
+bn_bwd_apply_acc_kernel(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x,
+                        const __nv_bfloat16* __restrict__ y, const float* __restrict__ gamma,
+                        const float* __restrict__ mean, const float* __restrict__ invstd,
+                        float* dgamma, float* dbeta,
+                        const float* __restrict__ fscale, const float* __restrict__ fshift,
+                        __nv_bfloat16* __restrict__ dx, __nv_bfloat16* dres, long long P, int C,
+                        int relu, float inv_count, const int rev,
+                        const float* __restrict__ sum_g, const float* __restrict__ sum_gx,
+                        float* acc_dgamma, float* acc_dbeta) {
+  bn_bwd_apply_body<true>(dy, x, y, gamma, mean, invstd, dgamma, dbeta, fscale, fshift, dx, dres,
+                          P, C, relu, inv_count, rev, sum_g, sum_gx, acc_dgamma, acc_dbeta);
 }
 
 // Forward apply: y = act(x * scale[c] + shift[c] (+ residual)); act 0 none, 1 relu, 2 relu6.
@@ -394,7 +432,17 @@ cudaError_t bn_bwd_apply(const void* dy, const void* x, const void* y, const flo
                          const float* mean, const float* invstd, float* dgamma,
                          float* dbeta, const float* fscale, const float* fshift, void* dx,
                          void* dres, long long P, int C, int relu, const float* sum_g,
-                         const float* sum_gx, cudaStream_t s) {
+                         const float* sum_gx, cudaStream_t s, float* acc_dgamma,
+                         float* acc_dbeta) {
+  if ((acc_dgamma == nullptr) != (acc_dbeta == nullptr)) return cudaErrorInvalidValue;
+  if (acc_dgamma != nullptr) {
+    bn_bwd_apply_acc_kernel<<<red_grid(P, C, kWavesApply), kThreads, 0, s>>>(
+        static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x),
+        static_cast<const __nv_bfloat16*>(y), gamma, mean, invstd, dgamma, dbeta, fscale, fshift,
+        static_cast<__nv_bfloat16*>(dx), static_cast<__nv_bfloat16*>(dres), P, C, relu,
+        1.f / static_cast<float>(P), g_row_reverse, sum_g, sum_gx, acc_dgamma, acc_dbeta);
+    return cudaGetLastError();
+  }
   bn_bwd_apply_kernel<<<red_grid(P, C, kWavesApply), kThreads, 0, s>>>(
       static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x),
       static_cast<const __nv_bfloat16*>(y), gamma, mean, invstd, dgamma, dbeta, fscale, fshift,

@@ -50,7 +50,8 @@ cudaError_t bn_bwd_apply(const void* dy, const void* x, const void* y, const flo
                          const float* mean, const float* invstd, float* dgamma,
                          float* dbeta, const float* fscale, const float* fshift, void* dx,
                          void* dres, long long P, int C, int relu, const float* sum_g,
-                         const float* sum_gx, cudaStream_t s);
+                         const float* sum_gx, cudaStream_t s, float* acc_dgamma = nullptr,
+                         float* acc_dbeta = nullptr);
 cudaError_t add_act(const void* a, const void* b, void* out, long long n, int act, cudaStream_t s);
 cudaError_t relu_bwd(const void* dy, const void* y, void* dx, long long n, cudaStream_t s);
 cudaError_t colsum(const void* x, long long P, int C, float* out, cudaStream_t s);
@@ -236,7 +237,8 @@ cudaError_t stem_bn_relu_pool_fwd(const void* x, void* y, uint8_t* idx, int N, i
 cudaError_t stem_pool_bn_bwd(const void* dy_pool, const uint8_t* idx, const void* x,
                              const float* gamma, const float* mean, const float* invstd,
                              const float* fscale, const float* fshift, float* dgamma, float* dbeta,
-                             void* dx, int N, int H, int W, int C, int OH, int OW, cudaStream_t s);
+                             void* dx, int N, int H, int W, int C, int OH, int OW, cudaStream_t s,
+                             float* acc_dgamma = nullptr, float* acc_dbeta = nullptr);
 
 // parameter server with resident optimizer state ("slot mode", parallel/ps.py)
 struct PsApplyArgs {          // server side, all pointers local to the PS GPU
@@ -287,7 +289,7 @@ cudaError_t depthwise3x3_fwd(const void* x, const void* w, const float* bias, vo
                              int H, int W, int C, int stride, int act, cudaStream_t s);
 // Backward of a depthwise 3x3 (pad 1, stride 1 or 2) whose output y and input x are both ReLU6
 // outputs, r(v) = [0 < v < 6] on the stored bf16 values, g = dy * r(y):
-//   dw[t, c] = sum g * x_tap, dbias[c] = sum g        (fp32, written)
+//   dw[t, c] = sum g * x_tap, dbias[c] = sum g        (fp32, written; added with accumulate)
 //   dx = bf16((sum over taps of g * w + add) * r(x)), dbias_in[c] = sum of the stored dx (fp32)
 // add (may be null): channel slice of a [N, H, W, add_ld] tensor, already offset to its first
 // channel.  scratch: depthwise3x3_bwd_scratch() floats, zero before the first launch; the kernel
@@ -296,7 +298,7 @@ long long depthwise3x3_bwd_scratch(int N, int H, int C, int stride);
 cudaError_t depthwise3x3_bwd(const void* x, const void* w, const void* y, const void* dy,
                              const void* add, int add_ld, void* dx, float* dw, float* dbias,
                              float* dbias_in, float* scratch, int N, int H, int W, int C,
-                             int stride, cudaStream_t s);
+                             int stride, cudaStream_t s, bool accumulate = false);
 
 // ---- held-out evaluation (eval.cu)
 // bn_fold: row u of tab [units][kFoldCols] describes one convolution + batch norm.  Offsets are

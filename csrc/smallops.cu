@@ -217,16 +217,18 @@ __device__ __forceinline__ void relu6_grad(const uint4 dyv, const uint4 yv, floa
   for (int e = 0; e < 8; ++e) g[e] = relu6_pass(yy[e]) ? d[e] : 0.f;
 }
 
-template <int GC>
-__global__ void __launch_bounds__(kDwThreads)
-depthwise3x3_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w,
-                        const __nv_bfloat16* __restrict__ y, const __nv_bfloat16* __restrict__ dy,
-                        const __nv_bfloat16* __restrict__ add, int add_ld,
-                        __nv_bfloat16* __restrict__ dx, float* __restrict__ dw,
-                        float* __restrict__ dbias, float* __restrict__ dbias_in,
-                        float* __restrict__ partial, unsigned int* __restrict__ counters, int N,
-                        int H, int W, int C, int OH, int OW, int stride, int rows_per,
-                        int chunks, int slabs) {
+// ACC (gradient accumulation over micro-batches): the last CTA of a chunk adds its totals to dw,
+// dbias and dbias_in instead of storing them - the same fixed-order sums, one thread per output.
+template <int GC, bool ACC>
+__device__ __forceinline__ void
+depthwise3x3_bwd_body(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w,
+                      const __nv_bfloat16* __restrict__ y, const __nv_bfloat16* __restrict__ dy,
+                      const __nv_bfloat16* __restrict__ add, int add_ld,
+                      __nv_bfloat16* __restrict__ dx, float* __restrict__ dw,
+                      float* __restrict__ dbias, float* __restrict__ dbias_in,
+                      float* __restrict__ partial, unsigned int* __restrict__ counters, int N,
+                      int H, int W, int C, int OH, int OW, int stride, int rows_per,
+                      int chunks, int slabs) {
   constexpr int kSubs = 32 / GC;              // pixel lanes of a warp
   constexpr int kLanes = kDwWarps * kSubs;    // pixel lanes of the CTA
   constexpr int kOut = kDwVals * GC * 8;      // per-CTA partial values, value-major
@@ -371,7 +373,9 @@ depthwise3x3_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16
       if (s + k < slabs) t[k] += __ldcg(col + (s + k) * step);
     const float total = (t[0] + t[1]) + (t[2] + t[3]);
     const int k = u / (GC * 8), c = chunk * GC * 8 + u % (GC * 8);
-    if (k < 9)
+    if (ACC)
+      *(k < 9 ? dw + k * C + c : (k == 9 ? dbias + c : dbias_in + c)) += total;
+    else if (k < 9)
       dw[k * C + c] = total;
     else if (k == 9)
       dbias[c] = total;
@@ -380,6 +384,28 @@ depthwise3x3_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16
   }
   if (threadIdx.x == 0) counters[chunk] = 0;  // ready for the next launch or graph replay
 }
+
+#define TFOS_DW_BWD_PARAMS                                                                         \
+  const __nv_bfloat16 *__restrict__ x, const __nv_bfloat16 *__restrict__ w,                       \
+      const __nv_bfloat16 *__restrict__ y, const __nv_bfloat16 *__restrict__ dy,                  \
+      const __nv_bfloat16 *__restrict__ add, int add_ld, __nv_bfloat16 *__restrict__ dx,          \
+      float *__restrict__ dw, float *__restrict__ dbias, float *__restrict__ dbias_in,            \
+      float *__restrict__ partial, unsigned int *__restrict__ counters, int N, int H, int W,      \
+      int C, int OH, int OW, int stride, int rows_per, int chunks, int slabs
+#define TFOS_DW_BWD_ARGS                                                                           \
+  x, w, y, dy, add, add_ld, dx, dw, dbias, dbias_in, partial, counters, N, H, W, C, OH, OW, stride, \
+      rows_per, chunks, slabs
+
+template <int GC>
+__global__ void __launch_bounds__(kDwThreads) depthwise3x3_bwd_kernel(TFOS_DW_BWD_PARAMS) {
+  depthwise3x3_bwd_body<GC, false>(TFOS_DW_BWD_ARGS);
+}
+template <int GC>
+__global__ void __launch_bounds__(kDwThreads) depthwise3x3_bwd_acc_kernel(TFOS_DW_BWD_PARAMS) {
+  depthwise3x3_bwd_body<GC, true>(TFOS_DW_BWD_ARGS);
+}
+#undef TFOS_DW_BWD_PARAMS
+#undef TFOS_DW_BWD_ARGS
 
 }  // namespace
 
@@ -419,7 +445,7 @@ long long depthwise3x3_bwd_scratch(int N, int H, int C, int stride) {
 cudaError_t depthwise3x3_bwd(const void* x, const void* w, const void* y, const void* dy,
                              const void* add, int add_ld, void* dx, float* dw, float* dbias,
                              float* dbias_in, float* scratch, int N, int H, int W, int C,
-                             int stride, cudaStream_t s) {
+                             int stride, cudaStream_t s, bool accumulate) {
   const DwBwdGrid g = dw_bwd_grid(N, H, C, stride);
   const int OH = (H - 1) / stride + 1, OW = (W - 1) / stride + 1;
   float* partial = scratch;
@@ -433,7 +459,8 @@ cudaError_t depthwise3x3_bwd(const void* x, const void* w, const void* y, const 
   auto* dxb = static_cast<__nv_bfloat16*>(dx);
   const int grid = g.slabs * g.chunks;
 #define TFOS_DW_BWD(GC)                                                                        \
-  depthwise3x3_bwd_kernel<GC><<<grid, kDwThreads, 0, s>>>(                                     \
+  (accumulate ? depthwise3x3_bwd_acc_kernel<GC> : depthwise3x3_bwd_kernel<GC>)                \
+      <<<grid, kDwThreads, 0, s>>>(                                                            \
       xb, wb, yb, dyb, ab, add_ld, dxb, dw, dbias, dbias_in, partial, counters, N, H, W, C, OH, \
       OW, stride, g.rows_per, g.chunks, g.slabs)
   if (g.gc == 4)

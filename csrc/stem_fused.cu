@@ -246,14 +246,17 @@ stem_pool_bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, const uint8
 }
 
 // apply: dx = A g + B x + K  (A = gamma invstd, B = -A invstd dgamma / M, K = -A dbeta / M - B mean)
-__global__ void __launch_bounds__(256)
-stem_pool_bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, const uint8_t* __restrict__ idx,
-                              const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma,
-                              const float* __restrict__ mean, const float* __restrict__ invstd,
-                              const float* __restrict__ dgamma, const float* __restrict__ dbeta,
-                              const float* __restrict__ fscale, const float* __restrict__ fshift,
-                              __nv_bfloat16* __restrict__ dx, int N, int H, int W, int C, int OH,
-                              int OW, float inv_count) {
+// ACC (gradient accumulation): dgamma / dbeta are this micro-batch's values (per-step scratch the
+// reduce wrote); thread t < C / 8 of block 0 (channel group t) adds them to acc_dgamma / acc_dbeta.
+template <bool ACC>
+__device__ __forceinline__ void
+stem_pool_bn_bwd_apply_body(const __nv_bfloat16* __restrict__ dy, const uint8_t* __restrict__ idx,
+                            const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma,
+                            const float* __restrict__ mean, const float* __restrict__ invstd,
+                            const float* __restrict__ dgamma, const float* __restrict__ dbeta,
+                            const float* __restrict__ fscale, const float* __restrict__ fshift,
+                            __nv_bfloat16* __restrict__ dx, int N, int H, int W, int C, int OH,
+                            int OW, float inv_count, float* acc_dgamma, float* acc_dbeta) {
   const int groups = C >> 3;
   const int BH = (H + 1) >> 1, BW = (W + 1) >> 1;
   const int tiles_w = (BW + 7) >> 3, tiles_h = (BH + 3) >> 2;
@@ -268,6 +271,13 @@ stem_pool_bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, const uint8_
     cB[j] = -cA[j] * is * dgamma[ch] * inv_count;
     cK[j] = -cA[j] * dbeta[ch] * inv_count - cB[j] * mean[ch];
     fs[j] = fscale[ch], fh[j] = fshift[ch];
+  }
+  if (ACC && blockIdx.x == 0 && threadIdx.x < groups) {   // g == threadIdx.x: one thread per group
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      acc_dgamma[g * 8 + j] += dgamma[g * 8 + j];
+      acc_dbeta[g * 8 + j] += dbeta[g * 8 + j];
+    }
   }
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -300,6 +310,32 @@ stem_pool_bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, const uint8_
   }
 }
 
+__global__ void __launch_bounds__(256)
+stem_pool_bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, const uint8_t* __restrict__ idx,
+                              const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma,
+                              const float* __restrict__ mean, const float* __restrict__ invstd,
+                              const float* __restrict__ dgamma, const float* __restrict__ dbeta,
+                              const float* __restrict__ fscale, const float* __restrict__ fshift,
+                              __nv_bfloat16* __restrict__ dx, int N, int H, int W, int C, int OH,
+                              int OW, float inv_count) {
+  stem_pool_bn_bwd_apply_body<false>(dy, idx, x, gamma, mean, invstd, dgamma, dbeta, fscale, fshift,
+                                     dx, N, H, W, C, OH, OW, inv_count, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(256)
+stem_pool_bn_bwd_apply_acc_kernel(const __nv_bfloat16* __restrict__ dy,
+                                  const uint8_t* __restrict__ idx,
+                                  const __nv_bfloat16* __restrict__ x,
+                                  const float* __restrict__ gamma, const float* __restrict__ mean,
+                                  const float* __restrict__ invstd, const float* __restrict__ dgamma,
+                                  const float* __restrict__ dbeta, const float* __restrict__ fscale,
+                                  const float* __restrict__ fshift, __nv_bfloat16* __restrict__ dx,
+                                  int N, int H, int W, int C, int OH, int OW, float inv_count,
+                                  float* __restrict__ acc_dgamma, float* __restrict__ acc_dbeta) {
+  stem_pool_bn_bwd_apply_body<true>(dy, idx, x, gamma, mean, invstd, dgamma, dbeta, fscale, fshift,
+                                    dx, N, H, W, C, OH, OW, inv_count, acc_dgamma, acc_dbeta);
+}
+
 inline unsigned grid_blocks(long long threads) {
   long long b = (threads + 255) / 256;
   const long long cap = static_cast<long long>(kSmCount) * 8;
@@ -323,9 +359,11 @@ cudaError_t stem_bn_relu_pool_fwd(const void* x, void* y, uint8_t* idx, int N, i
 cudaError_t stem_pool_bn_bwd(const void* dy_pool, const uint8_t* idx, const void* x,
                              const float* gamma, const float* mean, const float* invstd,
                              const float* fscale, const float* fshift, float* dgamma, float* dbeta,
-                             void* dx, int N, int H, int W, int C, int OH, int OW, cudaStream_t s) {
+                             void* dx, int N, int H, int W, int C, int OH, int OW, cudaStream_t s,
+                             float* acc_dgamma, float* acc_dbeta) {
   // 256 threads per block must hold whole sets of channel groups (a thread keeps its group)
   if (C % 8 != 0 || 256 % (C / 8) != 0) return cudaErrorInvalidValue;
+  if ((acc_dgamma == nullptr) != (acc_dbeta == nullptr)) return cudaErrorInvalidValue;
   const int groups = C / 8;
   const long long threads =
       static_cast<long long>(N) * (((H + 1) / 2 + 3) / 4) * (((W + 1) / 2 + 7) / 8) * 32 * groups;
@@ -333,6 +371,13 @@ cudaError_t stem_pool_bn_bwd(const void* dy_pool, const uint8_t* idx, const void
   stem_pool_bn_bwd_reduce_kernel<8><<<grid, 256, 0, s>>>(
       static_cast<const __nv_bfloat16*>(dy_pool), idx, static_cast<const __nv_bfloat16*>(x), mean,
       invstd, fscale, fshift, dgamma, dbeta, N, H, W, C, OH, OW);
+  if (acc_dgamma != nullptr) {
+    stem_pool_bn_bwd_apply_acc_kernel<<<grid, 256, 0, s>>>(
+        static_cast<const __nv_bfloat16*>(dy_pool), idx, static_cast<const __nv_bfloat16*>(x),
+        gamma, mean, invstd, dgamma, dbeta, fscale, fshift, static_cast<__nv_bfloat16*>(dx), N, H,
+        W, C, OH, OW, 1.f / (static_cast<float>(N) * H * W), acc_dgamma, acc_dbeta);
+    return cudaGetLastError();
+  }
   stem_pool_bn_bwd_apply_kernel<<<grid, 256, 0, s>>>(
       static_cast<const __nv_bfloat16*>(dy_pool), idx, static_cast<const __nv_bfloat16*>(x), gamma,
       mean, invstd, dgamma, dbeta, fscale, fshift, static_cast<__nv_bfloat16*>(dx), N, H, W, C, OH,

@@ -39,6 +39,11 @@ Gradient clipping: ``--clip_norm c`` clips the averaged gradient to global norm 
 update (Keras's ``global_clipnorm``, ``torch.nn.utils.clip_grad_norm_``), inside the fused optimizer
 kernels; the step log then also reports the gradient's norm (``grad_norm``, before clipping).
 ``--clip_norm inf`` only measures it.
+
+Gradient accumulation: ``--gradient_accumulation_steps k`` updates the parameters once every k
+micro-batches of ``--batch_size`` with their mean gradient (Keras's
+``gradient_accumulation_steps``), for an effective global batch of k * batch_size * workers.
+``--train_steps``, ``--save_steps``, ``--eval_every`` and the warm-up schedule count updates.
 """
 import argparse
 import os
@@ -94,6 +99,8 @@ def parse(argv):
   p.add_argument("--clip_norm", type=float, default=None,
                  help="clip the averaged gradient to this global L2 norm (> 0; inf: only measure "
                       "it) and log grad_norm")
+  p.add_argument("--gradient_accumulation_steps", type=int, default=1,
+                 help="micro-batches per update (k >= 1): the step counts above count updates")
   return p.parse_args(argv)
 
 
@@ -127,6 +134,9 @@ def main_fun(argv, ctx):
     opt["ema_decay"] = args.ema_decay
   if args.clip_norm is not None:
     opt["clip_norm"] = args.clip_norm
+  k = args.gradient_accumulation_steps
+  if k != 1:
+    opt["gradient_accumulation_steps"] = k
   if args.model == "resnet56":
     net = resnet.CifarResNetTrainer(depth=56, batch=B, device="cuda:0", comm=comm, lr=base_lr, **opt)
   else:
@@ -154,6 +164,9 @@ def main_fun(argv, ctx):
   net.train_step()
   if not args.no_graph:
     net.capture()
+  if k != 1:
+    while net.micro_step:   # the warm-up ends mid-window: finish it, updates start aligned
+      net.train_step()
   exporter = None
   if args.metrics_port is not None and metrics.Exporter.available():
     exporter = metrics.Exporter(rank=ctx.rank, port=args.metrics_port + ctx.rank if args.metrics_port else 0)
@@ -198,11 +211,12 @@ def main_fun(argv, ctx):
     elif args.epochs_per_step:
       net.set_lr(resnet.piecewise_lr(int(step * args.epochs_per_step), B * ctx.world_size))
     fault.maybe_inject(ctx.rank, step)      # TFOS_FAULT_INJECT (resilience tests), no-op otherwise
-    loss = net.train_step()
+    for _ in range(k):   # one update: k micro-batches
+      loss = net.train_step()
     if (step + 1) % 10 == 0:
       torch.cuda.synchronize()
       dt = time.time() - t0
-      rate = 10 * B * ctx.world_size / dt
+      rate = 10 * k * B * ctx.world_size / dt
       norm = {} if args.clip_norm is None else {"grad_norm": float(net.grad_norm)}
       if ctx.is_chief:
         print("step {:5d} loss {:.4f}{}  {:.0f} images/s".format(

@@ -62,6 +62,9 @@ def define_flags():
   p.add_argument("--clip_norm", type=float, default=None,
                  help="clip the averaged gradient to this global L2 norm (> 0; inf: only measure "
                       "it) and print grad_norm next to the loss")
+  p.add_argument("--gradient_accumulation_steps", type=int, default=None,
+                 help="micro-batches per update (k >= 1, default 1): each step of "
+                      "--steps_per_epoch is one update over k batches")
   return p
 
 
@@ -73,9 +76,9 @@ def class_weights(text):
 def trainer_kwargs(args):
   """Keyword arguments the trainer gets from the flags beyond the common ones: only those of the
   options that are set (encoder fine-tuning, ignore_index, class_weights, the weight average,
-  gradient clipping, the optimizer and its weight decay)."""
+  gradient clipping, the optimizer and its weight decay, gradient accumulation)."""
   names = ("encoder_trainable_from", "ignore_index", "class_weights", "ema_decay", "clip_norm",
-           "optimizer", "weight_decay")
+           "optimizer", "weight_decay", "gradient_accumulation_steps")
   return {n: getattr(args, n) for n in names if getattr(args, n, None) is not None}
 
 
@@ -132,15 +135,17 @@ def train(args, rank=0, world=1, comm=None, device="cuda:0", is_chief=True):
     from tensorflowonspark_b200.utils import summary
     eval_events = summary.SummaryWriter(os.path.join(args.model_dir, "eval"))
   step = start
+  k = extra.get("gradient_accumulation_steps", 1)
   for epoch in range(args.epochs):
     t0 = time.time()
     for i in range(args.steps_per_epoch):
-      x = batches[i % len(batches)]
-      net.set_input(x, labels_of(x, V))
-      loss = net.train_step()
+      for j in range(k):   # one update: k micro-batches
+        x = batches[(i * k + j) % len(batches)]
+        net.set_input(x, labels_of(x, V))
+        loss = net.train_step()
       step += 1
     torch.cuda.synchronize()
-    rate = args.steps_per_epoch * B * world / (time.time() - t0)
+    rate = args.steps_per_epoch * k * B * world / (time.time() - t0)
     res = net.evaluate([(x, labels_of(x, V)) for x in held_out]) if held_out else None  # collective
     avg = None
     if held_out and "ema_decay" in extra:   # the weight average's scores, also collective

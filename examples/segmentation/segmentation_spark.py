@@ -26,6 +26,8 @@ neither the optimizer state nor the average.
 ``global_clipnorm``) and prints the step's ``grad_norm`` next to the loss (``inf``: only measure it).
 ``--optimizer adamw | lamb`` replaces Adam by AdamW (decoupled weight decay) or LAMB (layer-wise
 adaptive Adam); ``--weight_decay`` decays the filters (with any of the three).
+``--gradient_accumulation_steps k`` updates once every k feed batches with their mean gradient;
+``--steps`` and ``--eval_every`` then count updates.
 
   python examples/segmentation/segmentation_spark.py --cluster_size 8 --batch_size 64 --steps 100
 """
@@ -69,8 +71,10 @@ def main_fun(args, ctx):
   B = args.batch_size
   # None: frozen encoder (as the reference), no ignored label, unweighted loss
   extra = {n: getattr(args, n) for n in ("encoder_trainable_from", "ignore_index", "class_weights",
-                                         "ema_decay", "clip_norm", "optimizer", "weight_decay")
+                                         "ema_decay", "clip_norm", "optimizer", "weight_decay",
+                                         "gradient_accumulation_steps")
            if getattr(args, n, None) is not None}
+  k = extra.get("gradient_accumulation_steps", 1)
   V = getattr(args, "classes", 3)
   net = unet.UNetTrainer(batch=B, image=IMG, classes=V, device="cuda:0", lr=args.learning_rate,
                          comm=comm, **extra)
@@ -126,18 +130,23 @@ def main_fun(args, ctx):
       fault.maybe_inject(ctx.rank, step)   # TFOS_FAULT_INJECT (resilience tests), no-op otherwise
       loss = net.train_step()
       h4 = time.time()
-      for k, d in enumerate((h1 - h0, h2 - h1, h3 - h2, h4 - h3)):
-        host[k] += d
-      done += 1
+      for i, d in enumerate((h1 - h0, h2 - h1, h3 - h2, h4 - h3)):
+        host[i] += d
       if step == 0:
         net.capture()          # static buffers: later steps replay one CUDA graph
+        if k != 1:
+          while net.micro_step:   # the warm-up ends mid-window: finish it on this batch
+            net.train_step()
         torch.cuda.synchronize()
         t0, seen = time.time(), -B   # steady-state rate: the clock starts after the capture
       seen += B
-      if (step + 1) % 10 == 0 and ctx.is_chief:
+      if k != 1 and net.micro_step:
+        continue   # mid-window: the counts below are of updates
+      done += 1
+      if done % 10 == 0 and ctx.is_chief:
         torch.cuda.synchronize()
         print("step {:4d} loss {:.4f}{} {:.0f} images/s".format(
-            step + 1, float(loss), grad_norm_text(net, extra),
+            done, float(loss), grad_norm_text(net, extra),
             seen * ctx.num_workers / (time.time() - t0)))
       after_step(done)
     print("rank {} ran {} steps ({} rows); host ms/step: feed {:.2f} staging {:.2f} hand-over {:.2f} "
@@ -151,17 +160,21 @@ def main_fun(args, ctx):
     net.set_input(x, unet.synthetic_labels(x, V))
     net.train_step()
     net.capture()
+    if k != 1:
+      while net.micro_step:   # the warm-up ends mid-window: finish it, updates start aligned
+        net.train_step()
     torch.cuda.synchronize()
     t0 = time.time()          # steady-state rate: the clock starts after the capture
     for step in range(args.steps):
       fault.maybe_inject(ctx.rank, step)
-      loss = net.train_step()
+      for _ in range(k):   # one update: k micro-batches
+        loss = net.train_step()
       done += 1
       if (step + 1) % 10 == 0 and ctx.is_chief:
         torch.cuda.synchronize()
         print("step {:4d} loss {:.4f}{} {:.0f} images/s".format(
             step + 1, float(loss), grad_norm_text(net, extra),
-            (step + 1) * B * ctx.world_size / (time.time() - t0)))
+            (step + 1) * k * B * ctx.world_size / (time.time() - t0)))
       after_step(done)
   if eval_steps and evaluated[0] != done:
     evaluate(done)
@@ -224,6 +237,9 @@ def define_flags():
   parser.add_argument("--clip_norm", type=float, default=None,
                       help="clip the averaged gradient to this global L2 norm (> 0; inf: only "
                            "measure it) and print grad_norm next to the loss")
+  parser.add_argument("--gradient_accumulation_steps", type=int, default=None,
+                      help="feed batches per update (k >= 1, default 1): --steps and --eval_every "
+                           "count updates")
   return parser
 
 

@@ -13,6 +13,7 @@ tf.distribute in its example programs (e.g. examples/mnist/keras/mnist_spark.py:
 11-66, examples/resnet/resnet_cifar_dist.py:196-257).
 """
 import math
+import numbers
 
 import torch
 
@@ -157,6 +158,87 @@ def check_adam_args(beta1, beta2, epsilon):
   return check(beta1, beta2, epsilon)
 
 
+def check_gradient_accumulation_steps(k, training=True):
+  """Validated ``gradient_accumulation_steps`` of a trainer: an int k >= 1 (ValueError for bools,
+  other types and k < 1, and for k != 1 with ``training=False``: an inference-only trainer takes
+  no gradients)."""
+  if isinstance(k, bool) or not isinstance(k, numbers.Integral):
+    raise ValueError("gradient_accumulation_steps must be an int >= 1, not {!r}".format(k))
+  if k < 1:
+    raise ValueError("gradient_accumulation_steps must be >= 1, got {}".format(k))
+  if k != 1 and not training:
+    raise ValueError("gradient_accumulation_steps needs training=True (an inference-only trainer "
+                     "takes no gradients)")
+  return int(k)
+
+
+class GradAccumulation(object):
+  """The update window of a trainer with ``gradient_accumulation_steps`` k (Keras's
+  ``gradient_accumulation_steps``): ``train_step`` call i of a window is micro-step
+  ``micro_step = i`` (0 .. k-1).  Micro-step 0 zeroes the fp32 gradients, every micro-step's
+  backward adds into them, and only micro-step k-1 runs the fused all-reduce + update, with the
+  optimizer's gradient scale ``hyper[3] = 1 / (world k)``: the update sees the mean of the k
+  micro-batches' gradients over all ranks.  With k = 1 every step is both first and last, which is
+  the step the trainers always ran."""
+
+  def __init__(self, k):
+    self.k = k
+    self.micro_step = 0
+
+  def phase(self, micro_step=None):
+    """(zero the gradients first, run the all-reduce + update last) of a micro-step."""
+    i = self.micro_step if micro_step is None else micro_step
+    return i == 0, i == self.k - 1
+
+  def advance(self):
+    self.micro_step = (self.micro_step + 1) % self.k
+
+  def restart(self, optim):
+    """Start a new window: the partial sums are dropped (``optim`` zeroes the gradients), the next
+    call is micro-step 0.  No-op with k = 1, whose every step zeroes the gradients itself."""
+    if self.k > 1:
+      self.micro_step = 0
+      optim.zero_grads()
+
+  def capture(self, device, step_kernels, mode):
+    """CUDA graphs of the micro-steps, one per distinct phase ({phase: graph}): warm-up runs
+    max(2, k) micro-steps eagerly on a side stream (two steps with k = 1, as before accumulation;
+    with k > 1 every position of the window once), then each phase is captured."""
+    s = torch.cuda.Stream(device=device)
+    s.wait_stream(torch.cuda.current_stream(device))
+    with torch.cuda.stream(s):
+      for _ in range(max(2, self.k)):
+        step_kernels()
+        self.advance()
+    torch.cuda.current_stream(device).wait_stream(s)
+    torch.cuda.synchronize(device)
+    graphs, at = {}, self.micro_step
+    for i in range(self.k):
+      ph = self.phase(i)
+      if ph in graphs:
+        continue
+      self.micro_step = i
+      g = torch.cuda.CUDAGraph()
+      with torch.cuda.graph(g, capture_error_mode=mode):
+        step_kernels()
+      graphs[ph] = g
+    self.micro_step = at
+    return graphs
+
+  def run(self, graphs, step_kernels, optim):
+    """One ``train_step``: replay this micro-step's graph (``optim.after_replay()`` after the
+    final one: a cross-host communicator's all-reduce + update run outside the graph) or run it
+    eagerly."""
+    ph = self.phase()
+    if graphs:
+      graphs[ph].replay()
+      if ph[1]:
+        optim.after_replay()
+    else:
+      step_kernels()
+    self.advance()
+
+
 def he_normal(fan_in):
   std = math.sqrt(2.0 / fan_in)
   return lambda shape, gen: torch.randn(shape, generator=gen) * std
@@ -256,6 +338,21 @@ class BatchNorm(object):
       self.running_var = torch.ones(self.C, dtype=torch.float32, device=device)
     self.gamma, self.beta = self.store.f32(self.sg), self.store.f32(self.sb)
     self.dgamma, self.dbeta = self.store.g(self.sg), self.store.g(self.sb)
+    self.acc = None
+
+  def accumulate_grads(self, scratch):
+    """Gradient accumulation: from now on the backward ADDS this micro-batch's dgamma / dbeta to
+    the parameter gradient.  The apply kernel forms dx from this micro-batch's values, so they are
+    kept apart: in ``red_gx`` / ``red_g`` (arena slots zeroed every step, unused when the
+    reduction is not fused) or in 2C floats of ``scratch``, a StatsArena the trainer zeroes every
+    step.  A fused reduction needs no scratch: the apply kernel finishes the sums in registers.
+    Call after the convolutions are built (``fused_reduce`` is final then)."""
+    if self.fused_reduce:
+      self.acc = (self.dgamma, self.dbeta)   # not read: the apply kernel works from red_g / red_gx
+    elif self.red_g is not None:
+      self.acc = (self.red_gx, self.red_g)
+    else:
+      self.acc = (scratch.take(self.C), scratch.take(self.C))
 
   @property
   def stats(self):
@@ -310,23 +407,26 @@ class BatchNorm(object):
       mode, ysrc = 3, mask
     elif relu and getattr(self, "mask", None) is not None:
       mode, ysrc = 3, self.mask   # bit mask written by forward(): 1/16 of y's bytes
+    # accumulation (accumulate_grads): dgamma / dbeta of this micro-batch go to scratch, the
+    # apply kernel adds them to the parameter gradient
+    dg, db = self.acc if self.acc is not None else (self.dgamma, self.dbeta)
+    acc = {} if self.acc is None else {"acc_dgamma": self.dgamma, "acc_dbeta": self.dbeta}
     if getattr(self, "fused_reduce", False):
       # sum(g), sum(g x) were accumulated by the epilogue of the data gradient that wrote dy
       # (ops/igemm.conv_dgrad(bn_reduce=...)): no reduction pass, the apply kernel finishes them
       ops.C().bn_set_row_reverse(bool(rev[1]))
-      ops.K.bn_bwd_apply(dy, x_raw, ysrc, self.gamma, self.mean, self.invstd, self.dgamma,
-                         self.dbeta, dx, dres, mode, self.scale, self.shift, self.red_g,
-                         self.red_gx)
+      ops.K.bn_bwd_apply(dy, x_raw, ysrc, self.gamma, self.mean, self.invstd, dg, db, dx, dres,
+                         mode, self.scale, self.shift, self.red_g, self.red_gx, **acc)
       ops.C().bn_set_row_reverse(False)
       return
     # rev = (reduce, apply) row order: each kernel starts at the end where the previous one
     # stopped, so that what it reads first is still in L2 (ResNetTrainer assigns the directions)
     ops.C().bn_set_row_reverse(bool(rev[0]))
-    ops.K.bn_bwd_reduce(dy, x_raw, ysrc, self.mean, self.invstd, self.dgamma, self.dbeta, mode,
-                        self.scale, self.shift)
+    ops.K.bn_bwd_reduce(dy, x_raw, ysrc, self.mean, self.invstd, dg, db, mode, self.scale,
+                        self.shift)
     ops.C().bn_set_row_reverse(bool(rev[1]))
-    ops.K.bn_bwd_apply(dy, x_raw, ysrc, self.gamma, self.mean, self.invstd, self.dgamma,
-                       self.dbeta, dx, dres, mode, self.scale, self.shift)
+    ops.K.bn_bwd_apply(dy, x_raw, ysrc, self.gamma, self.mean, self.invstd, dg, db, dx, dres,
+                       mode, self.scale, self.shift, **acc)
     ops.C().bn_set_row_reverse(False)
 
 

@@ -222,7 +222,8 @@ class ResNetTrainer(object):
   def __init__(self, depth=50, batch=256, image=224, num_classes=1000, device="cuda:0",
                lr=0.1, momentum=0.9, weight_decay=1e-4, comm=None, training=True, seed=1234,
                optimizer="momentum", trust_coefficient=0.001, label_smoothing=0.0,
-               ema_decay=None, clip_norm=None, beta1=0.9, beta2=0.999, epsilon=1e-7):
+               ema_decay=None, clip_norm=None, beta1=0.9, beta2=0.999, epsilon=1e-7,
+               gradient_accumulation_steps=1):
     """``optimizer``: sgd | momentum | adam | adamw | lars | lamb (``trust_coefficient`` is LARS's
     eta; see parallel/fused_optim.py).  adam folds ``weight_decay`` into the gradient (L2), adamw
     decouples it (``torch.optim.AdamW``), lamb is layer-wise adaptive Adam (apex ``FusedLAMB``).
@@ -241,8 +242,19 @@ class ResNetTrainer(object):
     padding rows start at zero and stay zero, and the loss, evaluation and serving read only the
     first ``num_classes`` logits.  ``label_smoothing`` (eps in [0, 1]): the training loss is the
     cross-entropy against (1 - eps) * onehot + eps / num_classes, as
-    ``F.cross_entropy(label_smoothing=eps)``; evaluation reports the plain cross-entropy."""
+    ``F.cross_entropy(label_smoothing=eps)``; evaluation reports the plain cross-entropy.
+
+    ``gradient_accumulation_steps`` (k, an int >= 1; training only): the parameters are updated
+    every k ``train_step`` calls with the mean of the gradients since the last update (Keras's
+    ``gradient_accumulation_steps``).  Calls 1 .. k-1 of a window run forward, loss and backward
+    and add into the gradient buffer, with no optimizer kernel and no communication; call k also
+    runs the fused all-reduce + update.  Each micro-batch's loss is its own mean (``loss_sum`` is
+    the micro-batch's), label smoothing applies per micro-batch, and the batch-norm batch and
+    running statistics are per micro-batch, as in Keras and PyTorch.  Clipping, the LARS / LAMB
+    norms, weight decay, the weight average and Adam's step advance once per update.
+    ``micro_step`` is the position of the next call in its window (0 .. k-1)."""
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
+    k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps, training)
     self.ema_decay = engine.check_ema_decay(ema_decay, training)
     self.clip_norm = engine.check_clip_norm(clip_norm, training)
     beta1, beta2, epsilon = engine.check_adam_args(beta1, beta2, epsilon)
@@ -293,8 +305,11 @@ class ResNetTrainer(object):
     tr = training
     # all batch-norm statistics accumulators live in one arena that is zeroed once per step;
     # finalisation is folded into the apply kernels (engine.BatchNorm.build)
-    self.stats_arena = engine.StatsArena(dev) if tr else None
-    self.running = engine.RunningArena(dev)   # all BN running statistics, one flat buffer
+    # (sized from the model: ResNet-101 / 152 need more than the arenas' default capacity)
+    c8 = sum((bn.C + 7) // 8 * 8 for bn in self._batch_norms())
+    self.stats_arena = engine.StatsArena(dev, capacity=max(4 * c8, 1 << 17)) if tr else None
+    # all BN running statistics, one flat buffer
+    self.running = engine.RunningArena(dev, capacity=max(2 * c8, 1 << 17))
     self.stem_bn.build(dev, self.stats_arena, self.running)
     # training fuses the stem's BN + ReLU + max pool (_forward): the activation is never stored
     self.stem_act = None if tr else _buf((B, OH, OW, 64), dev)
@@ -376,10 +391,30 @@ class ResNetTrainer(object):
                                   weight_decay=weight_decay, buckets=buckets,
                                   trust_coefficient=trust_coefficient, ema_decay=self.ema_decay,
                                   clip_norm=self.clip_norm, beta1=beta1, beta2=beta2, eps=epsilon)
+      if k_acc > 1:
+        self.optim.set_accumulation(k_acc)
+        for bn in self._batch_norms():
+          bn.accumulate_grads(None)   # every one has its arena slots or a fused reduction
+    self.accum = engine.GradAccumulation(k_acc)
     self.graph = None
+    self.graphs = None
     self.mean = [0.485, 0.456, 0.406]
     self.std = [0.229, 0.224, 0.225]
     self._assign_directions()
+
+  def _batch_norms(self):
+    return [self.stem_bn] + [u.bn for b in self.blocks
+                             for u in (b.u1, b.u2, b.u3) + ((b.ds,) if b.ds is not None else ())]
+
+  @property
+  def gradient_accumulation_steps(self):
+    return self.accum.k
+
+  @property
+  def micro_step(self):
+    """Position (0 .. k-1) of the next ``train_step`` in its accumulation window: the next call
+    updates the parameters when ``micro_step == gradient_accumulation_steps - 1``."""
+    return self.accum.micro_step
 
   def _assign_directions(self):
     """L2 hand-over ("serpentine") schedule.
@@ -460,7 +495,9 @@ class ResNetTrainer(object):
   def first_step_fused_broadcast(self):
     """First training step after start-up: the root's variables win (reference semantics of
     entering strategy.scope(), examples/mnist/keras/mnist_spark.py:55-56) without a separate
-    broadcast phase in front of the first forward pass."""
+    broadcast phase in front of the first forward pass.  It is a ``train_step``: with
+    ``gradient_accumulation_steps`` > 1 it is the first micro-step of a window (broadcast and
+    accumulate, no update)."""
     comm = self.comm
     comm.broadcast("aux32", self._root)  # BN scale/offset + biases: tiny, consumed in fp32
     comm.barrier()                        # root's weights are final and visible
@@ -472,8 +509,11 @@ class ResNetTrainer(object):
     self._forward(True, remote=True)            # forward consumes the root's tiles over NVLink
     main.wait_stream(self._side)
     self._loss(True)
-    self._backward()
-    self.optim.finish()
+    zero, update = self.accum.phase()
+    self._backward(zero, update)
+    if update:
+      self.optim.finish()
+    self.accum.advance()
     return self.loss_sum
 
   # --------------------------------------------------------------- forward
@@ -518,9 +558,12 @@ class ResNetTrainer(object):
                        label_smoothing=self.label_smoothing)
 
   # -------------------------------------------------------------- backward
-  def _backward(self):
+  def _backward(self, zero=True, update=True):
+    """``zero``: zero the gradients first; ``update``: start each bucket's all-reduce + update as
+    soon as its gradients are final (gradient accumulation: only the window's last micro-step)."""
     K = ops.K
-    self.optim.zero_grads()
+    if zero:
+      self.optim.zero_grads()
     self.fc.backward()
     K.avgpool_bwd(self.g_avg, self.g_last)
     for bi in reversed(range(len(self.blocks))):
@@ -536,51 +579,53 @@ class ResNetTrainer(object):
       if b.ds is not None:
         b.ds.bn.backward(b.g_out, b.rd, None, b.g_rd, relu=True, mask=b.u3.bn.mask, rev=b.ds.rev)
         b.ds.conv.backward()  # accumulates into g_x
-      self.optim.launch(bi)   # buckets that became final start their all-reduce now
+      if update:
+        self.optim.launch(bi)   # buckets that became final start their all-reduce now
     # max-pool backward recomputed inside the BN reduction and the BN apply: the gradient of the
     # stem activation (411 MB) is never written or read
     bn = self.stem_bn
-    K.stem_pool_bn_bwd(self.g_pool, self.pool_idx, self.stem_raw, bn.gamma, bn.mean, bn.invstd,
-                       bn.scale, bn.shift, bn.dgamma, bn.dbeta, self.g_stem_raw)
+    if bn.acc is None:
+      K.stem_pool_bn_bwd(self.g_pool, self.pool_idx, self.stem_raw, bn.gamma, bn.mean, bn.invstd,
+                         bn.scale, bn.shift, bn.dgamma, bn.dbeta, self.g_stem_raw)
+    else:   # this micro-batch's dgamma / dbeta in scratch, added to the gradient by the apply
+      K.stem_pool_bn_bwd(self.g_pool, self.pool_idx, self.stem_raw, bn.gamma, bn.mean, bn.invstd,
+                         bn.scale, bn.shift, bn.acc[0], bn.acc[1], self.g_stem_raw,
+                         acc_dgamma=bn.dgamma, acc_dbeta=bn.dbeta)
     ops.count()   # two launches
     self.p_stem_wgrad.run()
 
   # ------------------------------------------------------------------ API
   def step_kernels(self):
-    """Forward + loss + backward + optimizer on the static buffers (capturable)."""
+    """Forward + loss + backward + optimizer on the static buffers (capturable): the micro-step
+    ``micro_step`` of the accumulation window, which it does not advance (``train_step`` does)."""
+    zero, update = self.accum.phase()
     self._forward(True)
     self._loss(True)
-    self._backward()
-    self.optim.finish()
+    self._backward(zero, update)
+    if update:
+      self.optim.finish()
 
   def capture(self):
-    """Capture one training step into a CUDA graph (launch-bound inner loop -> one launch)."""
-    s = torch.cuda.Stream(device=self.device)
-    s.wait_stream(torch.cuda.current_stream(self.device))
-    with torch.cuda.stream(s):
-      for _ in range(2):
-        self.step_kernels()
-    torch.cuda.current_stream(self.device).wait_stream(s)
-    torch.cuda.synchronize(self.device)
-    g = torch.cuda.CUDAGraph()
+    """Capture the training step into CUDA graphs (launch-bound inner loop -> one launch): one
+    graph without accumulation; with ``gradient_accumulation_steps`` k > 1 one per kind of
+    micro-step (first, middle when k > 2, last), each replayed by ``train_step`` at its position.
+    The warm-up trains eagerly: two steps without accumulation, k micro-steps with it.  Returns
+    the graph of the updating step."""
     # cross-host communicator: its collectives stay outside the graph (FusedOptimizer.finish()
     # defers them), but the process group's watchdog thread may still poll events of the warm-up
     # collectives - thread-local capture keeps that from invalidating the capture
     mode = "thread_local" if getattr(self.optim, "group_mode", False) else "global"
-    with torch.cuda.graph(g, capture_error_mode=mode):
-      self.step_kernels()
-    self.graph = g
-    return g
+    self.graphs = self.accum.capture(self.device, self.step_kernels, mode)
+    self.graph = self.graphs[(self.accum.k == 1, True)]
+    return self.graph
 
   def train_step(self, images_u8=None, labels=None):
     if images_u8 is not None:
       self.set_input(images_u8, labels)
-    if self.graph is not None:
-      self.graph.replay()
-      self.optim.after_replay()   # cross-host communicator: all-reduce + update outside the graph
-    else:
-      self.step_kernels()
-    return self.loss_sum  # device scalar: mean loss of the step
+    # a captured step replays its graph; after the updating one a cross-host communicator runs
+    # its all-reduce + update outside the graph (after_replay)
+    self.accum.run(self.graphs if self.graph is not None else None, self.step_kernels, self.optim)
+    return self.loss_sum  # device scalar: mean loss of the step (micro-batch)
 
   def forward_only(self, images_u8=None):
     if images_u8 is not None:
@@ -762,7 +807,9 @@ class ResNetTrainer(object):
 
   def load_state_dict(self, sd):
     """Parameters and running statistics of ``state_dict()``; resets the weight average (the
-    optimizer's ``load_state_dict`` restores a saved one)."""
+    optimizer's ``load_state_dict`` restores a saved one) and restarts the accumulation window
+    (partial sums dropped, ``micro_step = 0``).  ``state_dict()`` may be taken mid-window; it
+    holds no partial sums."""
     sd = dict(sd)
     running = sd.pop("__running__", None)
     self.store.load_state_dict(sd)
@@ -770,6 +817,7 @@ class ResNetTrainer(object):
       self.running.tensor().copy_(running.to(self.device))
     if self.optim is not None:
       self.optim.reset_average()
+      self.accum.restart(self.optim)
 
   def load_backbone(self, state):
     """Start from a trained backbone: ``state`` is the ``state_dict()`` of a trainer of the same
@@ -833,14 +881,15 @@ class CifarResNetTrainer(object):
   """ResNet-20/32/56 for 32x32 inputs (basic blocks, 16/32/64 channels) - the network the
   reference example actually trains (examples/resnet/resnet_cifar_dist.py:208, ``resnet56``,
   momentum SGD, batch 128, weight decay 2e-4).  ``optimizer``, ``num_classes``,
-  ``label_smoothing``, ``ema_decay``, ``clip_norm``, ``beta1``, ``beta2`` and ``epsilon`` as in
-  ResNetTrainer."""
+  ``label_smoothing``, ``ema_decay``, ``clip_norm``, ``beta1``, ``beta2``, ``epsilon`` and
+  ``gradient_accumulation_steps`` as in ResNetTrainer."""
 
   def __init__(self, depth=56, batch=128, num_classes=10, device="cuda:0", lr=0.1, momentum=0.9,
                weight_decay=2e-4, comm=None, seed=1234, optimizer="momentum",
                trust_coefficient=0.001, label_smoothing=0.0, ema_decay=None, clip_norm=None,
-               beta1=0.9, beta2=0.999, epsilon=1e-7):
+               beta1=0.9, beta2=0.999, epsilon=1e-7, gradient_accumulation_steps=1):
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
+    k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps)
     self.ema_decay = engine.check_ema_decay(ema_decay)
     self.clip_norm = engine.check_clip_norm(clip_norm)
     beta1, beta2, epsilon = engine.check_adam_args(beta1, beta2, epsilon)
@@ -910,7 +959,17 @@ class CifarResNetTrainer(object):
                                 weight_decay=weight_decay, trust_coefficient=trust_coefficient,
                                 ema_decay=self.ema_decay, clip_norm=self.clip_norm, beta1=beta1,
                                 beta2=beta2, eps=epsilon)
+    # accumulation: the batch norms have no statistics arena; their per-micro-batch dgamma /
+    # dbeta live in one of their own, zeroed once per micro-step
+    self.grad_scratch = None
+    if k_acc > 1:
+      self.optim.set_accumulation(k_acc)
+      self.grad_scratch = engine.StatsArena(dev)
+      for _, bn in self._fold_units():
+        bn.accumulate_grads(self.grad_scratch)
+    self.accum = engine.GradAccumulation(k_acc)
     self.graph = None
+    self.graphs = None
     self.mean, self.std = [0.4914, 0.4822, 0.4465], [0.2470, 0.2435, 0.2616]
 
   synthetic_batch = ResNetTrainer.synthetic_batch
@@ -929,6 +988,8 @@ class CifarResNetTrainer(object):
   _check_average = ResNetTrainer._check_average
   averaged = ResNetTrainer.averaged
   grad_norm = ResNetTrainer.grad_norm
+  gradient_accumulation_steps = ResNetTrainer.gradient_accumulation_steps
+  micro_step = ResNetTrainer.micro_step
 
   def _fold_units(self):
     """(filter spec, batch norm) of every convolution followed by a batch norm, stem first."""
@@ -965,6 +1026,7 @@ class CifarResNetTrainer(object):
 
   def step_kernels(self):
     K = ops.K
+    zero, update = self.accum.phase()
     K.decode_normalize(self.in_u8, self.x8, 0, self.mean, self.std)
     self.stem.conv.forward()
     self.stem.bn.forward(self.stem_raw, self.stem_act, None, 1, True)
@@ -982,7 +1044,10 @@ class CifarResNetTrainer(object):
     self.correct.zero_()
     K.softmax_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
                    self.num_classes, 1.0 / self.B, label_smoothing=self.label_smoothing)
-    self.optim.zero_grads()
+    if zero:
+      self.optim.zero_grads()
+    if self.grad_scratch is not None:
+      self.grad_scratch.zero()
     self.fc.backward()
     K.avgpool_bwd(self.g_avg, self.g_last)
     for b in reversed(self.blocks):
@@ -995,7 +1060,8 @@ class CifarResNetTrainer(object):
         b.ds.conv.backward()
     self.stem.bn.backward(self.g_stem_act, self.stem_raw, self.stem_act, self.g_stem_raw, relu=True)
     self.stem.conv.backward()
-    self.optim.step()
+    if update:
+      self.optim.step()
 
 
 def piecewise_lr(epoch, batch_size, base=0.1, boundaries=(91, 136, 182), factors=(0.1, 0.01, 0.001)):

@@ -212,14 +212,16 @@ class MobileNetV2Encoder(object):
       u.bind(store)
     self._build_forward()
 
-  def build_backward(self, store, g_top, skip_grads):
+  def build_backward(self, store, g_top, skip_grads, accumulate=False):
     """Plan the backward of the trainable blocks, top down.  ``g_top``: gradient of block_16's
     project output (written by the decoder); ``skip_grads``: {block index: (tensor, channel
     offset)} - the slice of an up-block's concatenation gradient that belongs to that block's
     expand output.  Per block: project wgrad + bias colsum + dgrad, the fused depthwise backward
     (both ReLU6 derivatives, the skip gradient, the producer's bias gradient), expand wgrad and,
     above the lowest trainable block, expand dgrad into the block input's gradient - accumulated
-    when the block is residual, whose input and output share one gradient buffer."""
+    when the block is residual, whose input and output share one gradient buffer.
+    ``accumulate`` (gradient accumulation): the depthwise backward adds its filter and bias
+    gradients instead of storing them (every other producer here adds anyway)."""
     st, dev, K = store, self.dev, ops.K
     lowest = self.trainable_from
     run = self.backward_ops
@@ -239,7 +241,8 @@ class MobileNetV2Encoder(object):
       scratch = torch.zeros(ops.C().depthwise3x3_bwd_scratch(N, H, C, d.stride),
                             dtype=torch.float32, device=dev)
       run.append(functools.partial(K.depthwise3x3_bwd, d.x, d.w, d.y, g_d, add, add_off, g_x,
-                                   st.g(d.sw), st.g(d.sb), st.g(producer.sb), scratch, d.stride))
+                                   st.g(d.sw), st.g(d.sb), st.g(producer.sb), scratch, d.stride,
+                                   accumulate=accumulate))
       if e is None:   # block 0: its input is the stem's output
         run.append(igemm.conv_wgrad(g_x, self.x, st.g(self.stem.sw), 2, 1).run)
         continue
@@ -462,7 +465,17 @@ class UNetTrainer(object):
   ``FusedLAMB``); see parallel/fused_optim.py.  ``weight_decay``: a finite real >= 0, applied to
   the filters (conv weights, trainable encoder filters included), never to biases.  ``beta1``,
   ``beta2`` in [0, 1) and ``epsilon`` > 0 as Keras's Adam.  With ``training=False`` each of these
-  must keep its default."""
+  must keep its default.
+
+  ``gradient_accumulation_steps`` (k, an int >= 1; k != 1 needs training=True): the parameters are
+  updated every k ``train_step`` calls with the mean of the gradients since the last update
+  (Keras's ``gradient_accumulation_steps``).  Calls 1 .. k-1 of a window add into the gradient
+  buffer and launch no optimizer kernel and no communication; call k also runs the all-reduce +
+  update.  Each micro-batch's loss is its own mean; ``ignore_index`` / ``class_weights``
+  normalise each micro-batch by its own denominator (``loss_norm``), as each rank does under data
+  parallelism; the decoder batch norms' batch and running statistics are per micro-batch, as in
+  Keras and PyTorch.  Clipping, weight decay, the weight average and Adam's step advance once
+  per update.  ``micro_step`` is the position of the next call in its window (0 .. k-1)."""
 
   UP = (512, 256, 128, 64)
   # optimizer, weight_decay, beta1, beta2, epsilon: the defaults (the U-Net's Adam before they
@@ -472,8 +485,9 @@ class UNetTrainer(object):
   def __init__(self, batch=64, image=128, classes=3, device="cuda:0", lr=1e-3, comm=None, seed=1234,
                training=True, encoder_trainable_from=None, ignore_index=None, class_weights=None,
                ema_decay=None, clip_norm=None, optimizer="adam", weight_decay=0.0, beta1=0.9,
-               beta2=0.999, epsilon=1e-7):
+               beta2=0.999, epsilon=1e-7, gradient_accumulation_steps=1):
     classes = _classes(classes)
+    k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps, training)
     self.ema_decay = engine.check_ema_decay(ema_decay, training)
     self.clip_norm = engine.check_clip_norm(clip_norm, training)
     opt_args = _optimizer_args(optimizer, weight_decay, beta1, beta2, epsilon, training,
@@ -533,7 +547,7 @@ class UNetTrainer(object):
     if k is not None:
       # up-block i concatenates skips[-2 - i], the expand output of SKIP_BLOCKS[-1 - i]
       skip_grads = {SKIP_BLOCKS[-1 - i]: (g_cat, f) for i, (g_cat, _, f) in enumerate(self.g_cats)}
-      self.encoder.build_backward(st, self.g_top, skip_grads)
+      self.encoder.build_backward(st, self.g_top, skip_grads, accumulate=k_acc > 1)
     self.loss_sum = torch.zeros(1, dtype=torch.float32, device=dev)
     self.correct = torch.zeros(1, dtype=torch.float32, device=dev)
     # the loss options' device state: weights [VP] (zero in the padding channels), the
@@ -558,7 +572,16 @@ class UNetTrainer(object):
       self.optim = FusedOptimizer(st, comm=comm, opt=optimizer, lr=lr, weight_decay=weight_decay,
                                   ema_decay=self.ema_decay, clip_norm=self.clip_norm, beta1=beta1,
                                   beta2=beta2, eps=epsilon)
+    # accumulation: the decoder batch norms' per-micro-batch dgamma / dbeta, zeroed every step
+    self.grad_scratch = None
+    if k_acc > 1:
+      self.optim.set_accumulation(k_acc)
+      self.grad_scratch = engine.StatsArena(dev, capacity=2 * sum(self.UP))
+      for up in self.ups:
+        up.bn.accumulate_grads(self.grad_scratch)
+    self.accum = engine.GradAccumulation(k_acc)
     self.graph = None
+    self.graphs = None
     self._live = None   # (weights, aux32) saved while an averaged evaluation has the average in
 
   # ------------------------------------------------------------------ data
@@ -593,10 +616,21 @@ class UNetTrainer(object):
       K.copy_channels(skip, cat, skip.shape[-1], 0, f)
     self.p_last.run()
 
+  @property
+  def gradient_accumulation_steps(self):
+    return self.accum.k
+
+  @property
+  def micro_step(self):
+    """Position (0 .. k-1) of the next ``train_step`` in its accumulation window."""
+    return self.accum.micro_step
+
   def step_kernels(self):
+    """Micro-step ``micro_step`` of the accumulation window (not advanced: ``train_step`` does)."""
     if not self.training:
       raise RuntimeError("this UNetTrainer was built with training=False: it cannot train")
     K = ops.K
+    zero, update = self.accum.phase()
     self._forward(True)
     self.loss_sum.zero_()
     self.correct.zero_()
@@ -608,7 +642,10 @@ class UNetTrainer(object):
     K.pixel_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
                  self.classes, 1.0 / npix, self.ignore_index, self.weights,
                  self.loss_norm if self.loss_opts else None)
-    self.optim.zero_grads()
+    if zero:
+      self.optim.zero_grads()
+    if self.grad_scratch is not None:
+      self.grad_scratch.zero()
     self.p_last_wgrad.run()
     K.colsum(self.dlogits, self.store.g(self.s_last_b))
     self.p_last_dgrad.run()
@@ -616,24 +653,18 @@ class UNetTrainer(object):
       K.copy_channels(g_cat, g_act, f, 0, 0)  # gradient of the decoder half of the concat
       up.backward()
     self.encoder.backward()   # fine-tuning only: nothing to run on a frozen encoder
-    self.optim.step()
+    if update:
+      self.optim.step()
 
   def capture(self):
-    s = torch.cuda.Stream(device=self.device)
-    s.wait_stream(torch.cuda.current_stream(self.device))
-    with torch.cuda.stream(s):
-      for _ in range(2):
-        self.step_kernels()
-    torch.cuda.current_stream(self.device).wait_stream(s)
-    torch.cuda.synchronize(self.device)
-    g = torch.cuda.CUDAGraph()
+    """CUDA graphs of the training step: one, or with accumulation one per kind of micro-step
+    (see ResNetTrainer.capture); the warm-up trains eagerly."""
     # cross-host communicator: its collectives stay outside the graph (FusedOptimizer.finish()
     # defers them), but the process group's watchdog thread may still poll events of the warm-up
     # collectives - thread-local capture keeps that from invalidating the capture
     mode = "thread_local" if getattr(self.optim, "group_mode", False) else "global"
-    with torch.cuda.graph(g, capture_error_mode=mode):
-      self.step_kernels()
-    self.graph = g
+    self.graphs = self.accum.capture(self.device, self.step_kernels, mode)
+    self.graph = self.graphs[(self.accum.k == 1, True)]
 
   def train_step(self, images_u8=None, labels=None):
     if self._swapped_in():
@@ -641,11 +672,8 @@ class UNetTrainer(object):
                          "eval_end() before training")
     if images_u8 is not None:
       self.set_input(images_u8, labels)
-    if self.graph is not None:
-      self.graph.replay()
-      self.optim.after_replay()   # cross-host communicator: all-reduce + update outside the graph
-    else:
-      self.step_kernels()
+    # after the updating graph a cross-host communicator runs all-reduce + update outside it
+    self.accum.run(self.graphs if self.graph is not None else None, self.step_kernels, self.optim)
     return self.loss_sum
 
   def predict(self, images_u8=None):
@@ -675,7 +703,9 @@ class UNetTrainer(object):
     statistics, one without ``__encoder__`` (checkpoints written before the encoder was part of
     the state) keeps the seeded encoder.  ``__encoder__`` is applied first, then any ``encoder.*``
     fp32 masters: a frozen run's checkpoint starts fine-tuning from its encoder, a fine-tuning
-    checkpoint resumes with exact masters, and a frozen trainer ignores ``encoder.*``."""
+    checkpoint resumes with exact masters, and a frozen trainer ignores ``encoder.*``.  Restarts
+    the accumulation window (partial sums dropped, ``micro_step = 0``); ``state_dict()`` may be
+    taken mid-window and holds no partial sums."""
     sd = dict(sd)
     running = sd.pop("__running__", None)
     encoder = sd.pop("__encoder__", None)
@@ -698,6 +728,7 @@ class UNetTrainer(object):
       self.running.tensor().copy_(running.to(self.device))
     if self.optim is not None:    # (the optimizer's load_state_dict restores a saved average)
       self.optim.reset_average()
+      self.accum.restart(self.optim)
 
   def _encoder_convs(self):
     return [c for c in self.encoder.layers if not isinstance(c, _Residual)]

@@ -392,6 +392,14 @@ class FusedOptimizer(object):
   def set_lr(self, lr):
     self.hyper[0:1].fill_(float(lr))
 
+  def set_accumulation(self, k):
+    """Gradient accumulation over k micro-batches (the trainers' ``gradient_accumulation_steps``):
+    the gradient buffer holds the sum of k micro-batches, so the grad scale ``hyper[3]`` becomes
+    fp32(1 / (world k)).  state_dict() still saves the k-free 1 / world, and load_state_dict()
+    keeps this optimizer's own k, so a checkpoint loads under any k."""
+    self.accumulation = int(k)
+    self.hyper[3:4].fill_(1.0 / (self.gworld * self.accumulation))
+
   def zero_grads(self):
     self.store.grads.zero_()
     ops.count()
@@ -668,6 +676,9 @@ class FusedOptimizer(object):
       sd["ema"] = self.ema.detach().cpu()
       sd["ema_count"] = self.average_count()
     sd["hyper"] = self.hyper.detach().cpu()
+    if getattr(self, "accumulation", 1) != 1:
+      sd["hyper"] = sd["hyper"].clone()
+      sd["hyper"][3] = 1.0 / self.gworld
     return sd
 
   def load_state_dict(self, sd):
@@ -681,6 +692,8 @@ class FusedOptimizer(object):
       self.state2.copy_(sd["state2"])
     if "hyper" in sd:
       self.hyper[:HYPER].copy_(torch.as_tensor(sd["hyper"])[:HYPER])
+      if getattr(self, "accumulation", 1) != 1:
+        self.set_accumulation(self.accumulation)
     if self.ema is not None:
       if "ema" in sd:
         self.ema.copy_(sd["ema"])

@@ -70,6 +70,11 @@ KERNELS = [
     ("bn_fwd_apply_finalize", r"bn_fwd_apply_kernel<true>"),
     ("bn_bwd_apply", r"bn_bwd_apply_kernel"),
     ("bn_bwd_reduce", r"bn_bwd_reduce_kernel"),
+    # gradient accumulation: the applies that add this micro-batch's dgamma / dbeta, and the
+    # depthwise backward that adds its filter and bias gradients
+    ("bn_bwd_apply_acc", r"bn_bwd_apply_acc_kernel"),
+    ("stem_pool_bn_bwd_apply_acc", r"stem_pool_bn_bwd_apply_acc_kernel"),
+    ("depthwise3x3_bwd_acc_g4", r"depthwise3x3_bwd_acc_kernel<4>"),
     ("pixel_xent", r"pixel_xent_kernel<false>("),
     ("pixel_xent_wide_g4", r"pixel_xent_wide_kernel<4, false>"),
     ("pixel_xent_wide_g32", r"pixel_xent_wide_kernel<32, false>"),
