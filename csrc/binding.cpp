@@ -859,6 +859,89 @@ void pixel_xent(const Tensor& logits, const Tensor& labels, c10::optional<Tensor
                          static_cast<float>(scale), opt ? &o : nullptr, cur_stream()),
         "pixel_xent");
 }
+int64_t seg_dice_scratch(int64_t VP) {
+  TORCH_CHECK(VP >= 8 && VP <= 256 && VP % 8 == 0, "seg_dice_scratch: VP a multiple of 8 in [8, 256]");
+  return tfos::seg_dice_scratch(static_cast<int>(VP));
+}
+// coef [2, VP] fp32 = the Dice gradient coefficients; loss_sum += the Dice loss
+void seg_dice_stats(const Tensor& logits, const Tensor& labels, Tensor coef, Tensor loss_sum,
+                    Tensor scratch, int64_t V, double smooth, c10::optional<int64_t> ignore_index,
+                    c10::optional<Tensor> weights) {
+  need(logits, torch::kBFloat16, "logits");
+  need(labels, torch::kInt32, "labels");
+  need(coef, torch::kFloat32, "coef");
+  need(loss_sum, torch::kFloat32, "loss_sum");
+  need(scratch, torch::kFloat32, "scratch");
+  TORCH_CHECK(seg_channels_match(logits, V), "seg_dice_stats: logits [B, ..., VP] with V in [1, 256] "
+              "and VP = 8 for V <= 8, ceil(V / 8) * 8 above");
+  const int64_t VP = logits.size(-1);
+  const int64_t P = logits.numel() / VP;
+  TORCH_CHECK(P > 0, "seg_dice_stats: no pixels");
+  TORCH_CHECK(labels.numel() == P, "seg_dice_stats: one label per pixel");
+  TORCH_CHECK(coef.numel() == 2 * VP, "seg_dice_stats: coef needs 2 * VP entries");
+  TORCH_CHECK(loss_sum.numel() >= 1, "seg_dice_stats: loss_sum needs 1 slot");
+  TORCH_CHECK(scratch.numel() >= seg_dice_scratch(VP),
+              "seg_dice_stats: scratch needs seg_dice_scratch(VP) words");
+  TORCH_CHECK(std::isfinite(smooth) && smooth > 0.0, "seg_dice_stats: smooth must be finite and > 0");
+  for (const Tensor& t : {labels, coef, loss_sum, scratch})
+    TORCH_CHECK(t.device() == logits.device(), "seg_dice_stats: tensors on different devices");
+  const tfos::SegLossOpts o = seg_loss_opts(logits, ignore_index, weights, V, "seg_dice_stats");
+  check(tfos::seg_dice_stats(logits.data_ptr(), labels.data_ptr<int>(), P, static_cast<int>(VP),
+                             static_cast<int>(V), o, static_cast<float>(smooth),
+                             coef.data_ptr<float>(), loss_sum.data_ptr<float>(),
+                             scratch.data_ptr<float>(), cur_stream()),
+        "seg_dice_stats");
+}
+// pixel_xent's arguments plus the loss terms: focal_gamma (not None: the focal factor on the
+// cross-entropy), cross_entropy (false: no cross-entropy term, Dice only) and dice_coef
+// (seg_dice_stats' coef of the same logits and labels)
+void seg_loss_grad(const Tensor& logits, const Tensor& labels, Tensor dlogits, Tensor loss_sum,
+                   c10::optional<Tensor> correct, int64_t V, double scale,
+                   c10::optional<int64_t> ignore_index, c10::optional<Tensor> weights,
+                   c10::optional<Tensor> norm, c10::optional<double> focal_gamma,
+                   bool cross_entropy, c10::optional<Tensor> dice_coef) {
+  need(logits, torch::kBFloat16, "logits");
+  need(labels, torch::kInt32, "labels");
+  need(dlogits, torch::kBFloat16, "dlogits");
+  need(loss_sum, torch::kFloat32, "loss_sum");
+  TORCH_CHECK(seg_channels_match(logits, V), "seg_loss_grad: logits [B, ..., VP] with V in [1, 256] "
+              "and VP = 8 for V <= 8, ceil(V / 8) * 8 above");
+  const int64_t VP = logits.size(-1);
+  const int64_t P = logits.numel() / VP;
+  TORCH_CHECK(labels.numel() == P, "seg_loss_grad: one label per pixel");
+  TORCH_CHECK(dlogits.sizes() == logits.sizes(), "seg_loss_grad: dlogits must have the shape of logits");
+  for (const Tensor& t : {labels, dlogits, loss_sum})
+    TORCH_CHECK(t.device() == logits.device(), "seg_loss_grad: tensors on different devices");
+  tfos::SegLossTerms t{nullptr, 0.f, 0, cross_entropy ? 1 : 0};
+  if (focal_gamma.has_value()) {
+    TORCH_CHECK(cross_entropy, "seg_loss_grad: focal_gamma needs the cross-entropy term");
+    TORCH_CHECK(std::isfinite(*focal_gamma) && *focal_gamma >= 0.0,
+                "seg_loss_grad: focal_gamma must be finite and >= 0");
+    t.gamma = static_cast<float>(*focal_gamma);
+    t.focal = 1;
+  }
+  if (dice_coef.has_value() && dice_coef->defined()) {
+    need(*dice_coef, torch::kFloat32, "dice_coef");
+    TORCH_CHECK(dice_coef->numel() == 2 * VP, "seg_loss_grad: dice_coef needs 2 * VP entries");
+    TORCH_CHECK(dice_coef->device() == logits.device(), "seg_loss_grad: tensors on different devices");
+    t.dice = dice_coef->data_ptr<float>();
+  }
+  TORCH_CHECK(cross_entropy || t.dice != nullptr, "seg_loss_grad: no loss term");
+  tfos::SegLossOpts o = seg_loss_opts(logits, ignore_index, weights, V, "seg_loss_grad");
+  const bool opt = o.has_ignore || o.weights || (norm.has_value() && norm->defined());
+  if (opt) {
+    TORCH_CHECK(norm.has_value() && norm->defined(), "seg_loss_grad: the loss options need norm");
+    need(*norm, torch::kFloat64, "norm");
+    TORCH_CHECK(norm->numel() >= 3, "seg_loss_grad: norm needs 3 slots");
+    TORCH_CHECK(norm->device() == logits.device(), "seg_loss_grad: tensors on different devices");
+    o.norm = norm->data_ptr<double>();
+  }
+  check(tfos::seg_loss_grad(logits.data_ptr(), labels.data_ptr<int>(), dlogits.data_ptr(),
+                            loss_sum.data_ptr<float>(), optf(correct), P, static_cast<int>(VP),
+                            static_cast<int>(V), static_cast<float>(scale), opt ? &o : nullptr, t,
+                            cur_stream()),
+        "seg_loss_grad");
+}
 
 // --------------------------------------------------- collectives / optimizer
 void fill_ptrs(const std::vector<uint64_t>& v, void** dst, int world) {
@@ -1188,6 +1271,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("loss_sum"), py::arg("correct"), py::arg("V"), py::arg("scale"),
         py::arg("ignore_index") = py::none(), py::arg("weights") = py::none(),
         py::arg("norm") = py::none());
+  m.def("seg_dice_scratch", &seg_dice_scratch);
+  m.def("seg_dice_stats", &seg_dice_stats, py::arg("logits"), py::arg("labels"), py::arg("coef"),
+        py::arg("loss_sum"), py::arg("scratch"), py::arg("V"), py::arg("smooth"),
+        py::arg("ignore_index") = py::none(), py::arg("weights") = py::none());
+  m.def("seg_loss_grad", &seg_loss_grad, py::arg("logits"), py::arg("labels"), py::arg("dlogits"),
+        py::arg("loss_sum"), py::arg("correct"), py::arg("V"), py::arg("scale"),
+        py::arg("ignore_index") = py::none(), py::arg("weights") = py::none(),
+        py::arg("norm") = py::none(), py::arg("focal_gamma") = py::none(),
+        py::arg("cross_entropy") = true, py::arg("dice_coef") = py::none());
   m.def("allreduce_opt", &allreduce_opt);
   m.def("lars_norms", &lars_norms);
   m.def("grad_sumsq", &grad_sumsq);

@@ -831,6 +831,238 @@ seg_label_norm_kernel(const int* __restrict__ labels, long long P, int V, const 
   }
 }
 
+// ---- focal and Dice losses (ops.h seg_dice_stats / seg_loss_grad).  G = 1 is the 8-channel
+// layout (one thread per pixel, seg_argmax), G = 2..32 the wide one (seg_argmax_wide); both walk
+// the pixels as pixel_xent does, so G = 1 visits them in pixel_xent_kernel's order and G > 1 in
+// pixel_xent_wide_kernel's.
+
+// One pixel's softmax numerators e (zero in channels >= V) in this lane's channels and their sum
+// over the pixel, shifted by the arg-max of seg_wide.cuh exactly as pixel_xent shifts them.
+template <int G>
+__device__ __forceinline__ int seg_softmax_terms(const float (&l)[8], const int c0, const int V,
+                                                 float& mx, float (&e)[8], float& se) {
+  int am;
+  if constexpr (G == 1) am = seg_argmax(l, V, mx);
+  else am = seg_argmax_wide<G>(l, c0, V, mx);
+  se = 0.f;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    e[k] = c0 + k < V ? __expf(l[k] - mx) : 0.f;
+    se += e[k];
+  }
+  se = seg_group_sum<G>(se);
+  return am;
+}
+
+// seg_dice_stats: P_c, I_c, Y_c of the non-ignored pixels, each lane summing its own channels in
+// registers over a grid-stride loop, then a fixed combine: xor-shuffles across the lanes that hold
+// the same channels, the warps in order, the CTAs' partials (scratch) in order in fp64 by the last
+// CTA (ticket), which writes the coefficients, adds the loss and resets the ticket.
+constexpr int kDiceThreads = 256;
+constexpr int kDiceWarps = kDiceThreads / 32;
+static_assert(kSegDiceBlocks == 4 * kSmCount, "ops.h kSegDiceBlocks: four CTAs per SM");
+
+template <int G>
+__global__ void __launch_bounds__(kDiceThreads)
+seg_dice_stats_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                      long long P, int VP, int V, const SegLossOpts o, float smooth,
+                      float* __restrict__ coef, float* loss_sum, float* __restrict__ scratch) {
+  __shared__ float part[kDiceWarps][3][256];
+  __shared__ double red[kDiceWarps];
+  __shared__ unsigned int is_last;
+  constexpr int kPix = 32 / G;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, sub = lane & (G - 1), c0 = sub * 8;
+  const long long nw = static_cast<long long>(gridDim.x) * kDiceWarps;
+  float sp[8], si[8], sy[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) sp[k] = si[k] = sy[k] = 0.f;
+  for (long long t = static_cast<long long>(blockIdx.x) * kDiceWarps + warp; t * kPix < P;
+       t += nw) {
+    const long long p = t * kPix + lane / G;
+    const bool in = p < P;
+    float l[8];
+    if (in && c0 < VP) {
+      load8(logits + p * VP + c0, l);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) l[k] = 0.f;
+    }
+    float mx, e[8], se;
+    seg_softmax_terms<G>(l, c0, V, mx, e, se);
+    const int y = in ? labels[p] : -1;
+    if (in && !seg_ignored(o, y)) {
+      const float inv = 1.f / se;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float pk = e[k] * inv;
+        sp[k] += pk;
+        if (c0 + k < V && c0 + k == y) si[k] += pk, sy[k] += 1.f;
+      }
+    }
+  }
+#pragma unroll
+  for (int off = 16; off >= G; off >>= 1) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      sp[k] += __shfl_xor_sync(0xffffffffu, sp[k], off);
+      si[k] += __shfl_xor_sync(0xffffffffu, si[k], off);
+      sy[k] += __shfl_xor_sync(0xffffffffu, sy[k], off);
+    }
+  }
+  if (lane < G && c0 < VP) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      part[warp][0][c0 + k] = sp[k], part[warp][1][c0 + k] = si[k], part[warp][2][c0 + k] = sy[k];
+  }
+  __syncthreads();
+  float* mine = scratch + static_cast<long long>(blockIdx.x) * 3 * VP;
+  for (int i = threadIdx.x; i < 3 * VP; i += kDiceThreads) {
+    const int s = i / VP, c = i - s * VP;
+    float v = 0.f;
+    for (int w = 0; w < kDiceWarps; ++w) v += part[w][s][c];
+    mine[i] = v;
+  }
+  __threadfence();
+  __syncthreads();
+  unsigned int* counter = reinterpret_cast<unsigned int*>(scratch + kSegDiceBlocks * 3 * VP);
+  if (threadIdx.x == 0) is_last = (atomicAdd(counter, 1u) == gridDim.x - 1) ? 1u : 0u;
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  // thread c owns class c (kDiceThreads >= 256 >= VP): fp64 sums over the CTAs in order
+  const int c = threadIdx.x;
+  double Pc = 0.0, Ic = 0.0, Yc = 0.0;
+  if (c < VP) {
+    for (unsigned int b = 0; b < gridDim.x; ++b) {
+      const float* q = scratch + static_cast<long long>(b) * 3 * VP + c;
+      Pc += __ldcg(q);
+      Ic += __ldcg(q + VP);
+      Yc += __ldcg(q + 2 * VP);
+    }
+  }
+  const double w = c < V ? static_cast<double>(seg_weight(o, c, V)) : 0.0;
+  // a fixed-order CTA sum: xor-shuffles inside each warp, then the warps in order
+  auto cta_sum = [&](double v) {
+#pragma unroll
+    for (int k = 16; k >= 1; k >>= 1) v += __shfl_xor_sync(0xffffffffu, v, k);
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    double sum = 0.0;
+    for (int k = 0; k < kDiceWarps; ++k) sum += red[k];
+    __syncthreads();
+    return sum;
+  };
+  const double omega = w / cta_sum(w);
+  const double s = static_cast<double>(smooth), den = Pc + Yc + s, dice = (2.0 * Ic + s) / den;
+  if (c < VP) {
+    coef[c] = c < V ? static_cast<float>(-2.0 * omega / den) : 0.f;
+    coef[VP + c] = c < V ? static_cast<float>(omega * dice / den) : 0.f;
+  }
+  const double loss = cta_sum(c < V ? omega * (1.0 - dice) : 0.0);
+  if (threadIdx.x == 0) {
+    *loss_sum += static_cast<float>(loss);
+    *counter = 0u;
+  }
+}
+
+// seg_loss_grad: pixel_xent's pass (one read of each pixel's logits, one write of its dlogits)
+// with the focal factor and the Dice coefficients, chosen by the uniform terms t.  Per channel
+// k < V: dz_k = ce ? (p_k - [k = y]) s F : 0, plus p_k (g_k - sum_j p_j g_j) with
+// g_j = B_j + [j = y] A_j on a non-ignored pixel when t.dice; channels >= V get exactly 0.
+// F = 1 without focal; with it F = q^gamma (1 + gamma p_y r), r = -log(p_y) / q, taken as
+// -log1p(-q) / q for small q (1 at q = 0) and from the loss term otherwise; q = sum over j != y of
+// e_j / sum e_j, never 1 - p_y.  A label outside [0, V) keeps F = 1 (pixel_xent's loss and
+// gradient), and so does gamma = 0: the gradient is then pixel_xent's, bit for bit.
+template <int G, bool kOpt>
+__global__ void __launch_bounds__(256)
+seg_loss_grad_kernel(const __nv_bfloat16* __restrict__ logits, const int* __restrict__ labels,
+                     __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
+                     long long P, int VP, int V, float scale, const SegLossOpts o,
+                     const SegLossTerms t) {
+  if (kOpt) scale = static_cast<float>(o.norm[2]);
+  constexpr int kPix = 32 / G;
+  const int lane = threadIdx.x & 31, sub = lane & (G - 1), c0 = sub * 8;
+  const long long nw = static_cast<long long>(gridDim.x) * (256 / 32);
+  float A[8], B[8];   // this lane's Dice coefficients
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const bool d = t.dice != nullptr && c0 < VP;
+    A[k] = d ? __ldg(t.dice + c0 + k) : 0.f;
+    B[k] = d ? __ldg(t.dice + VP + c0 + k) : 0.f;
+  }
+  float local = 0.f, hits = 0.f;
+  for (long long tile = static_cast<long long>(blockIdx.x) * (256 / 32) + (threadIdx.x >> 5);
+       tile * kPix < P; tile += nw) {
+    const long long p = tile * kPix + lane / G;
+    const bool in = p < P, live = in && c0 < VP;
+    float l[8];
+    if (live) {
+      load8(logits + p * VP + c0, l);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) l[k] = 0.f;
+    }
+    float mx, e[8], se;
+    const int am = seg_softmax_terms<G>(l, c0, V, mx, e, se);
+    const int y = in ? labels[p] : -1;
+    const bool scored = in && (!kOpt || !seg_ignored(o, y));
+    const float s = kOpt ? (scored ? seg_weight(o, y, V) * scale : 0.f) : scale;
+    const bool weighed = !kOpt || s != 0.f;
+    // l_y: the 8-channel kernel reads a label in [V, 8) from its padding channel, as pixel_xent
+    float ly = 0.f, ey = 0.f, en = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      if ((G == 1 || c0 + k < V) && c0 + k == y) ly = l[k];
+      if (c0 + k == y) ey = e[k];
+      else en += e[k];
+    }
+    ly = seg_group_sum<G>(ly);
+    const float inv = 1.f / se;
+    const float lp = ly - mx - __logf(se);   // log p_y
+    float F = 1.f, fl = 1.f;                 // focal factors of the gradient and of the loss
+    if (t.focal) {                           // uniform: the group sums stay convergent
+      ey = seg_group_sum<G>(ey);
+      en = seg_group_sum<G>(en);
+      if (y >= 0 && y < V) {
+        const float py = ey * inv, q = en * inv;
+        const float r = q < 0.25f ? (q > 0.f ? -log1pf(-q) / q : 1.f) : -lp / q;
+        fl = t.gamma == 0.f ? 1.f : (q > 0.f ? __powf(q, t.gamma) : 0.f);
+        F = fl * (1.f + t.gamma * py * r);
+      }
+    }
+    float gbar = 0.f;   // sum_j p_j g_j of the Dice gradient
+    if (t.dice != nullptr) {
+      float dot = 0.f;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) dot += e[k] * inv * (B[k] + (c0 + k == y ? A[k] : 0.f));
+      gbar = seg_group_sum<G>(dot);
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      float g = 0.f;
+      if (c0 + k < V) {
+        if (t.ce && weighed) g = (e[k] * inv - (c0 + k == y ? 1.f : 0.f)) * s * F;
+        if (t.dice != nullptr && scored)
+          g += e[k] * inv * (B[k] + (c0 + k == y ? A[k] : 0.f) - gbar);
+      }
+      e[k] = g;
+    }
+    if (live) store8(dlogits + p * VP + c0, e);
+    if (in && sub == 0) {
+      if (t.ce && weighed) local += -lp * s * fl;
+      hits += (scored && am == y) ? 1.f : 0.f;
+    }
+  }
+  for (int off = 16; off >= 1; off >>= 1) {
+    local += __shfl_xor_sync(0xffffffff, local, off);
+    hits += __shfl_xor_sync(0xffffffff, hits, off);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(loss_sum, local);
+    if (correct_sum != nullptr) atomicAdd(correct_sum, hits);
+  }
+}
+
 inline int grid_for(long long work, int threads, int max_blocks) {
   long long b = (work + threads - 1) / threads;
   if (b < 1) b = 1;
@@ -1019,6 +1251,51 @@ cudaError_t seg_label_norm(const int* labels, long long P, int V, SegLossOpts o,
   seg_label_norm_kernel<<<grid_for(P, kNormThreads * kNormUnroll, kSmCount), kNormThreads, 0, s>>>(
       labels, P, V, o, norm, scratch);
   TFOS_RET();
+}
+cudaError_t seg_dice_stats(const void* logits, const int* labels, long long P, int VP, int V,
+                           SegLossOpts o, float smooth, float* coef, float* loss_sum,
+                           float* scratch, cudaStream_t s) {
+  const auto* l = static_cast<const __nv_bfloat16*>(logits);
+  if (VP == 8) {
+    seg_dice_stats_kernel<1><<<grid_for(P, kDiceThreads, kSegDiceBlocks), kDiceThreads, 0, s>>>(
+        l, labels, P, VP, V, o, smooth, coef, loss_sum, scratch);
+    TFOS_RET();
+  }
+  return seg_wide_dispatch(VP, [&](auto g) {
+    constexpr int G = decltype(g)::value;
+    seg_dice_stats_kernel<G><<<grid_for(P * G, kDiceThreads, kSegDiceBlocks), kDiceThreads, 0,
+                               s>>>(l, labels, P, VP, V, o, smooth, coef, loss_sum, scratch);
+    TFOS_RET();
+  });
+}
+template <bool kOpt>
+static cudaError_t launch_seg_loss_grad(const __nv_bfloat16* logits, const int* labels,
+                                        __nv_bfloat16* dlogits, float* loss_sum,
+                                        float* correct_sum, long long P, int VP, int V,
+                                        float scale, const SegLossOpts& o, const SegLossTerms& t,
+                                        cudaStream_t s) {
+  if (VP == 8) {
+    seg_loss_grad_kernel<1, kOpt><<<grid_for(P, 256, kMaxBlocks), 256, 0, s>>>(
+        logits, labels, dlogits, loss_sum, correct_sum, P, VP, V, scale, o, t);
+    TFOS_RET();
+  }
+  return seg_wide_dispatch(VP, [&](auto g) {
+    constexpr int G = decltype(g)::value;
+    seg_loss_grad_kernel<G, kOpt><<<grid_for(P * G, 256, kMaxBlocks), 256, 0, s>>>(
+        logits, labels, dlogits, loss_sum, correct_sum, P, VP, V, scale, o, t);
+    TFOS_RET();
+  });
+}
+cudaError_t seg_loss_grad(const void* logits, const int* labels, void* dlogits, float* loss_sum,
+                          float* correct_sum, long long P, int VP, int V, float scale,
+                          const SegLossOpts* opts, SegLossTerms t, cudaStream_t s) {
+  const auto* l = static_cast<const __nv_bfloat16*>(logits);
+  auto* d = static_cast<__nv_bfloat16*>(dlogits);
+  if (opts != nullptr)
+    return launch_seg_loss_grad<true>(l, labels, d, loss_sum, correct_sum, P, VP, V, scale, *opts,
+                                      t, s);
+  return launch_seg_loss_grad<false>(l, labels, d, loss_sum, correct_sum, P, VP, V, scale,
+                                     SegLossOpts{}, t, s);
 }
 cudaError_t cast_f32_bf16(const float* in, void* out, long long n, cudaStream_t s) {
   cast_f32_bf16_kernel<<<grid_for(n, 256, kMaxBlocks), 256, 0, s>>>(

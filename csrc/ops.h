@@ -103,6 +103,40 @@ cudaError_t seg_label_norm(const int* labels, long long P, int V, SegLossOpts o,
 cudaError_t pixel_xent(const void* logits, const int* labels, void* dlogits, float* loss_sum,
                        float* correct_sum, long long P, int VP, int V, float scale,
                        const SegLossOpts* opts, cudaStream_t s);
+// Focal and soft Dice losses of the segmentation U-Net, on the logits and labels of pixel_xent.
+// seg_dice_stats: one pass over the non-ignored pixels S (opts: seg_label_norm's rules) forms
+// I_c = sum_S p_c [y = c], P_c = sum_S p_c and Y_c = |{y = c}| for c < V (a label outside [0, V)
+// adds to P_c only), then with w_c = opts' weight of class c, omega_c = w_c / sum_{c<V} w_c,
+// Den_c = P_c + Y_c + smooth, D_c = (2 I_c + smooth) / Den_c:
+//   loss_sum += sum_c omega_c (1 - D_c),
+//   coef [2, VP] fp32 = [A_c = -2 omega_c / Den_c, B_c = omega_c D_c / Den_c], 0 for c >= V.
+// Per-lane register sums and a fixed-order combine (per-CTA partials in scratch, summed in fp64
+// by the last CTA): bitwise reproducible.  scratch: seg_dice_scratch(VP) zeroed fp32 words (the
+// last is the CTA ticket), left with the ticket at zero, so it replays in a CUDA graph with no
+// reset.  A CTA's class counts are exact in fp32 up to 2^24 pixels per CTA.
+constexpr int kSegDiceBlocks = 528;   // CTAs of seg_dice_stats at most: four per H100 SM
+inline long long seg_dice_scratch(int VP) { return 3LL * kSegDiceBlocks * VP + 1; }
+cudaError_t seg_dice_stats(const void* logits, const int* labels, long long P, int VP, int V,
+                           SegLossOpts o, float smooth, float* coef, float* loss_sum,
+                           float* scratch, cudaStream_t s);
+// The terms seg_loss_grad adds per pixel, uniform over the launch: ce the (optioned) softmax
+// cross-entropy of pixel_xent, times the focal factor when focal (exponent gamma >= 0); dice,
+// when not null, seg_dice_stats' coef.
+struct SegLossTerms {
+  const float* dice;
+  float gamma;
+  int focal;
+  int ce;
+};
+// seg_loss_grad: pixel_xent's pass (scale / opts as there) with the terms t:
+//   loss_sum += sum over the pixels of s_p (1 - p_y)^gamma (-log p_y) when t.ce (the Dice loss
+//   comes from seg_dice_stats), correct_sum += the hits as pixel_xent counts them,
+//   dlogits_k = [t.ce] s_p (p_k - [k = y]) F_p + [t.dice, pixel not ignored] p_k (g_k - sum_j p_j g_j)
+// with F_p the focal factor (1 without focal, and for a label outside [0, V)) and
+// g_j = B_j + [j = y] A_j.  Exactly 0 in channels >= V and on ignored pixels.
+cudaError_t seg_loss_grad(const void* logits, const int* labels, void* dlogits, float* loss_sum,
+                          float* correct_sum, long long P, int VP, int V, float scale,
+                          const SegLossOpts* opts, SegLossTerms t, cudaStream_t s);
 
 // ---- optim_comm.cu
 constexpr int kMaxRanks = 8;

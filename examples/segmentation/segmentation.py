@@ -15,6 +15,8 @@ every evaluation scores it too (``val_avg_*``) and ``--export_dir`` exports it.
 measure it).
 ``--optimizer adamw | lamb`` replaces Adam by AdamW (decoupled weight decay) or LAMB (layer-wise
 adaptive Adam); ``--weight_decay`` decays the filters (with any of the three).
+``--loss focal | dice | dice_ce`` trains with the focal loss (exponent ``--focal_gamma``), the soft
+Dice loss or Dice + cross-entropy (smoothing ``--dice_smooth``) instead of the cross-entropy.
 Checkpoints every epoch (the reference's ModelCheckpoint callback) and evaluates every epoch on
 ``--eval_steps`` held-out synthetic batches per rank (the reference's ``validation_data``):
 validation loss, pixel accuracy and mean IoU.
@@ -65,7 +67,18 @@ def define_flags():
   p.add_argument("--gradient_accumulation_steps", type=int, default=None,
                  help="micro-batches per update (k >= 1, default 1): each step of "
                       "--steps_per_epoch is one update over k batches")
+  add_loss_flags(p)
   return p
+
+
+def add_loss_flags(p):
+  """--loss, --focal_gamma and --dice_smooth (UNetTrainer's loss, focal_gamma, dice_smooth)."""
+  p.add_argument("--loss", default=None, choices=["cross_entropy", "focal", "dice", "dice_ce"],
+                 help="training loss (default cross_entropy); evaluation reports the cross-entropy")
+  p.add_argument("--focal_gamma", type=float, default=None,
+                 help="focal loss exponent, >= 0 (default 2; needs --loss focal)")
+  p.add_argument("--dice_smooth", type=float, default=None,
+                 help="Dice smoothing, > 0 (default 1e-5; needs --loss dice or dice_ce)")
 
 
 def class_weights(text):
@@ -76,9 +89,10 @@ def class_weights(text):
 def trainer_kwargs(args):
   """Keyword arguments the trainer gets from the flags beyond the common ones: only those of the
   options that are set (encoder fine-tuning, ignore_index, class_weights, the weight average,
-  gradient clipping, the optimizer and its weight decay, gradient accumulation)."""
+  gradient clipping, the optimizer and its weight decay, gradient accumulation, the loss)."""
   names = ("encoder_trainable_from", "ignore_index", "class_weights", "ema_decay", "clip_norm",
-           "optimizer", "weight_decay", "gradient_accumulation_steps")
+           "optimizer", "weight_decay", "gradient_accumulation_steps", "loss", "focal_gamma",
+           "dice_smooth")
   return {n: getattr(args, n) for n in names if getattr(args, n, None) is not None}
 
 

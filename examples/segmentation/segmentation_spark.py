@@ -28,6 +28,9 @@ neither the optimizer state nor the average.
 adaptive Adam); ``--weight_decay`` decays the filters (with any of the three).
 ``--gradient_accumulation_steps k`` updates once every k feed batches with their mean gradient;
 ``--steps`` and ``--eval_every`` then count updates.
+``--loss focal | dice | dice_ce`` trains with the focal loss (exponent ``--focal_gamma``), the soft
+Dice loss or Dice + cross-entropy (smoothing ``--dice_smooth``; the Dice statistics are each
+rank's own) instead of the cross-entropy.
 
   python examples/segmentation/segmentation_spark.py --cluster_size 8 --batch_size 64 --steps 100
 """
@@ -72,7 +75,8 @@ def main_fun(args, ctx):
   # None: frozen encoder (as the reference), no ignored label, unweighted loss
   extra = {n: getattr(args, n) for n in ("encoder_trainable_from", "ignore_index", "class_weights",
                                          "ema_decay", "clip_norm", "optimizer", "weight_decay",
-                                         "gradient_accumulation_steps")
+                                         "gradient_accumulation_steps", "loss", "focal_gamma",
+                                         "dice_smooth")
            if getattr(args, n, None) is not None}
   k = extra.get("gradient_accumulation_steps", 1)
   V = getattr(args, "classes", 3)
@@ -240,6 +244,13 @@ def define_flags():
   parser.add_argument("--gradient_accumulation_steps", type=int, default=None,
                       help="feed batches per update (k >= 1, default 1): --steps and --eval_every "
                            "count updates")
+  parser.add_argument("--loss", default=None, choices=["cross_entropy", "focal", "dice", "dice_ce"],
+                      help="training loss (default cross_entropy); evaluation reports the "
+                           "cross-entropy")
+  parser.add_argument("--focal_gamma", type=float, default=None,
+                      help="focal loss exponent, >= 0 (default 2; needs --loss focal)")
+  parser.add_argument("--dice_smooth", type=float, default=None,
+                      help="Dice smoothing, > 0 (default 1e-5; needs --loss dice or dice_ce)")
   return parser
 
 

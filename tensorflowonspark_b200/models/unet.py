@@ -352,6 +352,37 @@ def _optimizer_args(optimizer, weight_decay, beta1, beta2, epsilon, training, de
   return args
 
 
+#: the training losses of UNetTrainer(loss=...)
+LOSSES = ("cross_entropy", "focal", "dice", "dice_ce")
+
+
+def _loss_args(loss, focal_gamma, dice_smooth, training, defaults):
+  """Validated ``(loss, focal_gamma, dice_smooth)``: loss one of LOSSES, focal_gamma a finite
+  real >= 0, dice_smooth a finite real > 0.  A value other than its default needs training=True,
+  a non-default focal_gamma the focal loss and a non-default dice_smooth a loss with Dice
+  (ValueError otherwise)."""
+  if not isinstance(loss, str) or loss not in LOSSES:
+    raise ValueError("loss must be one of {}, got {!r}".format(" | ".join(LOSSES), loss))
+
+  def real(name, v, ok, what):
+    if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v) or not ok(v):
+      raise ValueError("{} must be a finite real {}, got {!r}".format(name, what, v))
+    return float(v)
+  focal_gamma = real("focal_gamma", focal_gamma, lambda v: v >= 0, ">= 0")
+  dice_smooth = real("dice_smooth", dice_smooth, lambda v: v > 0, "> 0")
+  args = (loss, focal_gamma, dice_smooth)
+  names = ("loss", "focal_gamma", "dice_smooth")
+  if not training:
+    for name, v, d in zip(names, args, defaults):
+      if v != d:
+        raise ValueError("{} needs training=True (an inference-only U-Net has no loss)".format(name))
+  if focal_gamma != defaults[1] and loss != "focal":
+    raise ValueError("focal_gamma needs loss='focal', not {!r}".format(loss))
+  if dice_smooth != defaults[2] and loss not in ("dice", "dice_ce"):
+    raise ValueError("dice_smooth needs loss='dice' or 'dice_ce', not {!r}".format(loss))
+  return args
+
+
 #: most classes a U-Net can have: its masks (served output, DataFeed wire format) are uint8
 MAX_CLASSES = 256
 
@@ -475,18 +506,47 @@ class UNetTrainer(object):
   normalise each micro-batch by its own denominator (``loss_norm``), as each rank does under data
   parallelism; the decoder batch norms' batch and running statistics are per micro-batch, as in
   Keras and PyTorch.  Clipping, weight decay, the weight average and Adam's step advance once
-  per update.  ``micro_step`` is the position of the next call in its window (0 .. k-1)."""
+  per update.  ``micro_step`` is the position of the next call in its window (0 .. k-1).
+
+  ``loss`` (training only): ``"cross_entropy"`` (default), ``"focal"``, ``"dice"`` or
+  ``"dice_ce"``.  With S the non-ignored pixels of the micro-batch, w the class weights (1
+  without them) and p the softmax over the ``classes`` real channels:
+    * focal (Lin et al.; Keras ``CategoricalFocalCrossentropy`` with ``alpha`` per class given by
+      ``class_weights``), exponent ``focal_gamma`` (a finite real >= 0, default 2):
+      FL_p = -(1 - p_y)^gamma log p_y, normalised as the cross-entropy is,
+      loss = sum_S w[y] FL_p / sum_S w[y].  gamma = 0 is the cross-entropy: the same gradient, bit
+      for bit.  A label outside [0, classes) that is not ignored keeps its cross-entropy terms.
+    * dice (MONAI ``DiceLoss(softmax=True, to_onehot_y=True, batch=True)``), smoothing
+      ``dice_smooth`` (a finite real > 0, default 1e-5) in numerator and denominator: per class c,
+      I_c = sum_S p_c [y = c], P_c = sum_S p_c, Y_c = |{y = c}| and
+      D_c = (2 I_c + smooth) / (P_c + Y_c + smooth); loss = sum_c w_c (1 - D_c) / sum_c w_c, so the
+      class weights average the classes rather than weigh pixels.  A label outside [0, classes)
+      adds to P_c only; an empty S gives loss 0 and a zero gradient.
+    * dice_ce: the (optioned) cross-entropy plus the Dice loss, weight 1 each (MONAI
+      ``DiceCELoss``).
+  The Dice statistics are those of each micro-batch on each rank (like the batch-norm
+  statistics): under gradient accumulation each micro-batch has its own Dice loss, and under data
+  parallelism each rank its own, averaged by the gradient all-reduce.  The Dice losses launch one
+  more kernel per step (the statistics pass, seg_dice_stats); focal launches as many as the
+  cross-entropy.  Evaluation keeps reporting the (optioned) cross-entropy; the per-class Dice
+  coefficient of the evaluation's masks is 2 IoU / (1 + IoU) of its ``iou``.  A non-default
+  ``focal_gamma`` needs ``loss="focal"``, a non-default ``dice_smooth`` a Dice loss."""
 
   UP = (512, 256, 128, 64)
   # optimizer, weight_decay, beta1, beta2, epsilon: the defaults (the U-Net's Adam before they
   # were options)
   OPT_DEFAULTS = ("adam", 0.0, 0.9, 0.999, 1e-7)
+  # loss, focal_gamma, dice_smooth
+  LOSS_DEFAULTS = ("cross_entropy", 2.0, 1e-5)
 
   def __init__(self, batch=64, image=128, classes=3, device="cuda:0", lr=1e-3, comm=None, seed=1234,
                training=True, encoder_trainable_from=None, ignore_index=None, class_weights=None,
                ema_decay=None, clip_norm=None, optimizer="adam", weight_decay=0.0, beta1=0.9,
-               beta2=0.999, epsilon=1e-7, gradient_accumulation_steps=1):
+               beta2=0.999, epsilon=1e-7, gradient_accumulation_steps=1, loss="cross_entropy",
+               focal_gamma=2.0, dice_smooth=1e-5):
     classes = _classes(classes)
+    self.loss, self.focal_gamma, self.dice_smooth = _loss_args(
+        loss, focal_gamma, dice_smooth, training, self.LOSS_DEFAULTS)
     k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps, training)
     self.ema_decay = engine.check_ema_decay(ema_decay, training)
     self.clip_norm = engine.check_clip_norm(clip_norm, training)
@@ -565,6 +625,12 @@ class UNetTrainer(object):
       if self.loss_opts:
         self._norm_scratch = torch.zeros(ops.C().seg_label_norm_scratch(classes),
                                          dtype=torch.int64, device=dev)
+    # the Dice losses: seg_dice_stats' gradient coefficients [A; B] and scratch
+    self.dice_coef = self._dice_scratch = None
+    if self.loss in ("dice", "dice_ce"):
+      self.dice_coef = torch.zeros(2, VP, dtype=torch.float32, device=dev)
+      self._dice_scratch = torch.zeros(ops.C().seg_dice_scratch(VP), dtype=torch.float32,
+                                       device=dev)
     self.in_u8 = _buf((B, image, image, 3), dev, torch.uint8)
     if tr:
       from ..parallel.fused_optim import FusedOptimizer
@@ -634,14 +700,7 @@ class UNetTrainer(object):
     self._forward(True)
     self.loss_sum.zero_()
     self.correct.zero_()
-    npix = self.labels.numel()
-    if self.loss_opts:   # the denominator sum_S w[y] of this batch's labels, on the device
-      K.seg_label_norm(self.labels, self.loss_norm, self._norm_scratch, self.classes,
-                       self.ignore_index, self.weights)
-    # without options ignore_index and weights are None and the scale is the host's 1 / npix
-    K.pixel_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
-                 self.classes, 1.0 / npix, self.ignore_index, self.weights,
-                 self.loss_norm if self.loss_opts else None)
+    self._loss()
     if zero:
       self.optim.zero_grads()
     if self.grad_scratch is not None:
@@ -655,6 +714,28 @@ class UNetTrainer(object):
     self.encoder.backward()   # fine-tuning only: nothing to run on a frozen encoder
     if update:
       self.optim.step()
+
+  def _loss(self):
+    """The loss kernels of a step on ``logits`` and ``labels``: loss_sum and correct add this
+    micro-batch's loss and hits (they are not zeroed here), dlogits is overwritten."""
+    K = ops.K
+    npix = self.labels.numel()
+    if self.loss_opts:   # the denominator sum_S w[y] of this batch's labels, on the device
+      K.seg_label_norm(self.labels, self.loss_norm, self._norm_scratch, self.classes,
+                       self.ignore_index, self.weights)
+    # without options ignore_index and weights are None and the scale is the host's 1 / npix
+    norm = self.loss_norm if self.loss_opts else None
+    if self.loss == "cross_entropy":
+      K.pixel_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
+                   self.classes, 1.0 / npix, self.ignore_index, self.weights, norm)
+      return
+    if self.dice_coef is not None:   # this micro-batch's Dice statistics, before the gradient
+      K.seg_dice_stats(self.logits, self.labels, self.dice_coef, self.loss_sum, self._dice_scratch,
+                       self.classes, self.dice_smooth, self.ignore_index, self.weights)
+    K.seg_loss_grad(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
+                    self.classes, 1.0 / npix, self.ignore_index, self.weights, norm,
+                    focal_gamma=self.focal_gamma if self.loss == "focal" else None,
+                    cross_entropy=self.loss != "dice", dice_coef=self.dice_coef)
 
   def capture(self):
     """CUDA graphs of the training step: one, or with accumulation one per kind of micro-step

@@ -78,6 +78,15 @@ KERNELS = [
     ("pixel_xent", r"pixel_xent_kernel<false>("),
     ("pixel_xent_wide_g4", r"pixel_xent_wide_kernel<4, false>"),
     ("pixel_xent_wide_g32", r"pixel_xent_wide_kernel<32, false>"),
+    # the focal / Dice losses: the statistics pass and the gradient (G = 1: 8 channels)
+    ("seg_dice_stats", r"seg_dice_stats_kernel<1>"),
+    ("seg_dice_stats_g4", r"seg_dice_stats_kernel<4>"),
+    ("seg_dice_stats_g32", r"seg_dice_stats_kernel<32>"),
+    ("seg_loss_grad", r"seg_loss_grad_kernel<1, false>"),
+    ("seg_loss_grad_opt", r"seg_loss_grad_kernel<1, true>"),
+    ("seg_loss_grad_g4", r"seg_loss_grad_kernel<4, false>"),
+    ("seg_loss_grad_g4_opt", r"seg_loss_grad_kernel<4, true>"),
+    ("seg_loss_grad_g32", r"seg_loss_grad_kernel<32, false>"),
     ("seg_eval_metrics", r"seg_eval_metrics_kernel<false>("),
     ("seg_eval_wide_g4", r"seg_eval_wide_kernel<4, false>"),
     ("seg_eval_wide_g32", r"seg_eval_wide_kernel<32, false>"),
