@@ -551,6 +551,57 @@ void softmax_xent(const Tensor& logits, const Tensor& labels, c10::optional<Tens
                            static_cast<float>(label_smoothing), cur_stream()),
         "softmax_xent");
 }
+// The multi-label kernels' shapes: logits [rows, ld] with 1 <= V <= ld, targets [rows, V].
+void check_multilabel(const Tensor& logits, const Tensor& targets, int64_t V, const char* what) {
+  TFOS_REQUIRE(logits.dim() == 2, what, ": logits must be [rows, ld], got ", shape_str(logits));
+  TFOS_REQUIRE(V >= 1 && V <= logits.size(1), what, ": need 1 <= V <= ld, got V=", V, " ld=",
+               logits.size(1));
+  TFOS_REQUIRE(targets.dim() == 2 && targets.size(0) == logits.size(0) && targets.size(1) == V,
+               what, ": targets must be [rows, V] = [", logits.size(0), ", ", V, "], got ",
+               shape_str(targets));
+}
+void sigmoid_bce(const Tensor& logits, const Tensor& targets, c10::optional<Tensor> dlogits,
+                 Tensor loss_sum, c10::optional<Tensor> correct, int64_t V, double scale,
+                 double label_smoothing, c10::optional<Tensor> pos_weight) {
+  const char* what = "sigmoid_bce";
+  TFOS_REQUIRE(std::isfinite(label_smoothing) && label_smoothing >= 0.0 && label_smoothing <= 1.0,
+               what, ": label_smoothing must be in [0, 1], got ", label_smoothing);
+  check_multilabel(logits, targets, V, what);
+  const bool has_d = dlogits.has_value() && dlogits->defined();
+  const bool has_w = pos_weight.has_value() && pos_weight->defined();
+  if (has_d)
+    TFOS_REQUIRE(dlogits->dim() == 2 && dlogits->size(0) == logits.size(0) &&
+                     dlogits->size(1) >= V,
+                 what, ": dlogits must be [rows, ldd] with ldd >= V, got ", shape_str(*dlogits));
+  if (has_w)
+    TFOS_REQUIRE(pos_weight->numel() == V, what, ": pos_weight must hold V = ", V,
+                 " values, got ", pos_weight->numel());
+  need(logits, torch::kFloat32, "logits");
+  need(targets, torch::kUInt8, "targets");
+  need(loss_sum, torch::kFloat32, "loss_sum");
+  std::vector<Tensor> same = {targets, loss_sum};
+  if (has_d) {
+    need(*dlogits, torch::kBFloat16, "dlogits");
+    same.push_back(*dlogits);
+  }
+  if (correct.has_value() && correct->defined()) {
+    need(*correct, torch::kFloat32, "correct");
+    same.push_back(*correct);
+  }
+  if (has_w) {
+    need(*pos_weight, torch::kFloat32, "pos_weight");
+    same.push_back(*pos_weight);
+  }
+  for (const Tensor& t : same)
+    TORCH_CHECK(t.device() == logits.device(), "sigmoid_bce: tensors on different devices");
+  check(tfos::sigmoid_bce(logits.data_ptr<float>(), targets.data_ptr<uint8_t>(),
+                          has_d ? dlogits->data_ptr() : nullptr, loss_sum.data_ptr<float>(),
+                          optf(correct), logits.size(0), static_cast<int>(V), logits.size(1),
+                          has_d ? dlogits->size(1) : 0, scale,
+                          static_cast<float>(label_smoothing),
+                          has_w ? pos_weight->data_ptr<float>() : nullptr, cur_stream()),
+        what);
+}
 void decode_normalize(const Tensor& in, Tensor out, int wofs, std::vector<double> mean,
                       std::vector<double> stdv) {
   // in [N, H, W, C] uint8 -> out [N, H, Wp, Cp] bf16: pixel w lands at column wofs + w, channels
@@ -612,6 +663,25 @@ void eval_metrics(const Tensor& logits, const Tensor& labels, const Tensor& n_va
                            n_valid.data_ptr<int>(), acc.data_ptr<double>(), logits.size(0),
                            logits.size(1), V, cur_stream()),
         "eval_metrics");
+}
+int64_t multilabel_eval_slots(int64_t V) { return tfos::kMlEvalSlots + 3 * V; }
+void multilabel_eval_metrics(const Tensor& logits, const Tensor& targets, const Tensor& n_valid,
+                             Tensor acc, int64_t V) {
+  const char* what = "multilabel_eval_metrics";
+  check_multilabel(logits, targets, V, what);
+  TFOS_REQUIRE(acc.numel() >= multilabel_eval_slots(V), what, ": acc needs 8 + 3 V = ",
+               multilabel_eval_slots(V), " slots, got ", acc.numel());
+  need(logits, torch::kFloat32, "logits");
+  need(targets, torch::kUInt8, "targets");
+  need(n_valid, torch::kInt32, "n_valid");
+  need(acc, torch::kFloat64, "acc");
+  for (const Tensor& t : {targets, n_valid, acc})
+    TORCH_CHECK(t.device() == logits.device(), "multilabel_eval_metrics: tensors on different devices");
+  check(tfos::multilabel_eval_metrics(logits.data_ptr<float>(), targets.data_ptr<uint8_t>(),
+                                      n_valid.data_ptr<int>(), acc.data_ptr<double>(),
+                                      logits.size(0), logits.size(1), static_cast<int>(V),
+                                      cur_stream()),
+        what);
 }
 // The logits' padded channel count picks the kernel: 8 -> the one-load-per-pixel kernels
 // (V <= 8), 16..256 -> the wide kernels (seg_wide.cuh) with VP = ceil(V / 8) * 8.
@@ -1248,6 +1318,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("cast_f32_bf16", &cast_f32_bf16);
   m.def("bn_fold", &bn_fold);
   m.def("eval_metrics", &eval_metrics);
+  m.def("sigmoid_bce", &sigmoid_bce, py::arg("logits"), py::arg("targets"), py::arg("dlogits"),
+        py::arg("loss_sum"), py::arg("correct"), py::arg("V"), py::arg("scale"),
+        py::arg("label_smoothing") = 0.0, py::arg("pos_weight") = py::none());
+  m.def("multilabel_eval_slots", &multilabel_eval_slots);
+  m.def("multilabel_eval_metrics", &multilabel_eval_metrics);
   m.def("seg_eval_scratch", &seg_eval_scratch, py::arg("pixels"), py::arg("classes") = 8);
   m.def("seg_eval_slots", &seg_eval_slots);
   m.def("seg_eval_metrics", &seg_eval_metrics, py::arg("logits"), py::arg("labels"),

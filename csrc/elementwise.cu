@@ -543,6 +543,58 @@ softmax_xent_kernel(const T* __restrict__ logits, const int* __restrict__ labels
   }
 }
 
+// Multi-label binary cross-entropy with logits: one warp per row, one pass over the row.  Element
+// (i, j < V) with target byte y (nonzero = positive), t = y (Smooth: y (1 - eps) + eps / 2) and
+// p = pos_weight[j] (Weighted; 1 otherwise):
+//   loss = p t softplus(-l) + (1 - t) softplus(l),  softplus(x) = max(x, 0) + log1p(exp(-|x|))
+//   dlogits = (sigmoid(l) (p t + 1 - t) - p t) * scale, exactly 0 in columns [V, ldd)
+// loss_sum += the row's loss * scale; correct_sum += 1 when (l_j > 0) == y for every j < V.
+// exp(-|l|) never overflows, so logits of any finite size give a finite loss and gradient.
+constexpr int kBceThreads = 256;
+constexpr int kBceRows = kBceThreads / 32;
+
+template <bool Smooth, bool Weighted>
+__global__ void __launch_bounds__(kBceThreads)
+sigmoid_bce_kernel(const float* __restrict__ logits, const uint8_t* __restrict__ targets,
+                   __nv_bfloat16* __restrict__ dlogits, float* loss_sum, float* correct_sum,
+                   const float* __restrict__ pos_weight, long long rows, int V, int ld, int ldd,
+                   float scale, float eps) {
+  const long long row = static_cast<long long>(blockIdx.x) * kBceRows + (threadIdx.x >> 5);
+  if (row >= rows) return;   // whole warps leave: the shuffles below see full warps
+  const int lane = threadIdx.x & 31;
+  const float* l = logits + row * ld;
+  const uint8_t* y = targets + row * V;
+  __nv_bfloat16* d = dlogits != nullptr ? dlogits + row * ldd : nullptr;
+  [[maybe_unused]] const float t_on = 1.f - 0.5f * eps, t_off = 0.5f * eps;
+  float loss = 0.f;
+  bool miss = false;
+  for (int j = lane; j < V; j += 32) {
+    const float v = l[j];
+    const bool pos = y[j] != 0;
+    float t = pos ? 1.f : 0.f;
+    if constexpr (Smooth) t = pos ? t_on : t_off;
+    float pt = t;
+    if constexpr (Weighted) pt = pos_weight[j] * t;
+    const float e = __expf(-fabsf(v));
+    const float a = log1pf(e);
+    loss += pt * (fmaxf(-v, 0.f) + a) + (1.f - t) * (fmaxf(v, 0.f) + a);
+    miss |= (v > 0.f) != pos;
+    if (d != nullptr) {
+      const float r = 1.f / (1.f + e);
+      const float sig = v >= 0.f ? r : e * r;
+      d[j] = __float2bfloat16_rn((sig * (pt + 1.f - t) - pt) * scale);
+    }
+  }
+  if (d != nullptr)
+    for (int j = V + lane; j < ldd; j += 32) d[j] = __float2bfloat16_rn(0.f);
+  for (int o = 16; o >= 1; o >>= 1) loss += __shfl_xor_sync(0xffffffff, loss, o);
+  const bool any_miss = __any_sync(0xffffffff, miss);
+  if (lane == 0) {
+    atomicAdd(loss_sum, loss * scale);
+    if (correct_sum != nullptr && !any_miss) atomicAdd(correct_sum, 1.f);
+  }
+}
+
 // -------------------------------------------------------------- input decode
 // uint8 NHWC image -> normalised bf16 with Cp (>= C) channels and an optional
 // zero border in W (the stem convolution's TMA window layout wants one).
@@ -1191,6 +1243,26 @@ cudaError_t softmax_xent(const void* logits, int logits_fp32, const int* labels,
     const __nv_bfloat16* l = static_cast<const __nv_bfloat16*>(logits);
     if (smooth) launch(softmax_xent_kernel<__nv_bfloat16, true>, l);
     else launch(softmax_xent_kernel<__nv_bfloat16, false>, l);
+  }
+  TFOS_RET();
+}
+cudaError_t sigmoid_bce(const float* logits, const uint8_t* targets, void* dlogits,
+                        float* loss_sum, float* correct_sum, long long rows, int V, int ld,
+                        int ldd, float scale, float label_smoothing, const float* pos_weight,
+                        cudaStream_t s) {
+  if (rows <= 0) return cudaSuccess;
+  auto launch = [&](auto kernel) {
+    kernel<<<static_cast<unsigned>((rows + kBceRows - 1) / kBceRows), kBceThreads, 0, s>>>(
+        logits, targets, static_cast<__nv_bfloat16*>(dlogits), loss_sum, correct_sum, pos_weight,
+        rows, V, ld, ldd, scale, label_smoothing);
+  };
+  const bool smooth = label_smoothing != 0.f;
+  if (pos_weight != nullptr) {
+    if (smooth) launch(sigmoid_bce_kernel<true, true>);
+    else launch(sigmoid_bce_kernel<false, true>);
+  } else {
+    if (smooth) launch(sigmoid_bce_kernel<true, false>);
+    else launch(sigmoid_bce_kernel<false, false>);
   }
   TFOS_RET();
 }

@@ -7,6 +7,8 @@
 //                   added to an fp64 accumulator by ONE CTA with a fixed row-to-warp assignment
 //                   and a fixed-order reduction: no floating-point atomics, so the totals are
 //                   bitwise reproducible across runs and graph replays.
+//  * multilabel_eval_metrics : the same contract for multi-hot uint8 targets: rows scored and
+//                   invalid, BCE, correct elements, exact-match rows and per-class TP / FP / FN.
 //  * seg_eval_metrics : the same for the U-Net's per-pixel bf16 logits (models/unet.py): count,
 //                   correct, invalid labels, loss and the V x V confusion matrix of every pixel of
 //                   the valid images.  Many CTAs, each over a fixed contiguous pixel range; the
@@ -113,6 +115,91 @@ eval_metrics_kernel(const float* __restrict__ logits, const int* __restrict__ la
   }
   __syncthreads();
   if (threadIdx.x < kEvalUsedSlots) {
+    double s = 0;
+    for (int w = 0; w < kMetricWarps; ++w) s += part[w][threadIdx.x];
+    acc[threadIdx.x] += s;
+  }
+}
+
+// Multi-label rows [0, n_valid) in chunks of kMlChunk.  Row pass: warp r % kMetricWarps scores
+// row r (a byte > 1 makes the row invalid: counted, not scored) and keeps its totals in fp64; the
+// row's validity goes to shared memory.  Class pass: thread j % kMetricThreads owns class j and
+// counts its TP / FP / FN over the chunk's valid rows in integers, added into its own slots of
+// acc.  prediction = l > 0 (a NaN logit predicts negative); loss = the unweighted, unsmoothed BCE
+// y softplus(-l) + (1 - y) softplus(l).  No floating-point atomics and fixed orders throughout.
+constexpr int kMlChunk = 1024;
+
+__global__ void __launch_bounds__(kMetricThreads, 1)
+multilabel_eval_metrics_kernel(const float* __restrict__ logits,
+                               const uint8_t* __restrict__ targets,
+                               const int* __restrict__ n_valid, double* __restrict__ acc, int rows,
+                               int ld, int V) {
+  __shared__ double part[kMetricWarps][kMlEvalUsedSlots];
+  __shared__ uint8_t valid[kMlChunk];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int n = *n_valid;
+  n = n < 0 ? 0 : (n > rows ? rows : n);
+  double cnt = 0, bad = 0, loss = 0, hits = 0, exact = 0;
+  double* tp = acc + kMlEvalSlots;
+  double* fp = tp + V;
+  double* fn = fp + V;
+  for (int r0 = 0; r0 < n; r0 += kMlChunk) {
+    const int m = n - r0 < kMlChunk ? n - r0 : kMlChunk;
+    for (int i = warp; i < m; i += kMetricWarps) {
+      const long long r = r0 + i;
+      const float* l = logits + r * ld;
+      const uint8_t* y = targets + r * V;
+      float ls = 0.f;
+      int ok = 0, over = 0;
+      for (int j = lane; j < V; j += 32) {
+        const float v = l[j];
+        const int t = y[j];
+        over |= t > 1;
+        ok += (v > 0.f) == (t != 0) ? 1 : 0;
+        ls += (t != 0 ? fmaxf(-v, 0.f) : fmaxf(v, 0.f)) + log1pf(__expf(-fabsf(v)));
+      }
+      for (int o = 16; o >= 1; o >>= 1) {
+        ls += __shfl_xor_sync(0xffffffff, ls, o);
+        ok += __shfl_xor_sync(0xffffffff, ok, o);
+      }
+      const bool invalid = __any_sync(0xffffffff, over != 0);
+      if (lane == 0) valid[i] = invalid ? 0 : 1;
+      if (invalid) {
+        bad += 1;
+        continue;
+      }
+      cnt += 1;
+      loss += static_cast<double>(ls);
+      hits += ok;
+      exact += ok == V ? 1 : 0;
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < V; j += kMetricThreads) {
+      long long a = 0, b = 0, c = 0;
+#pragma unroll 4   // several rows' loads in flight: this loop is latency-bound
+      for (int i = 0; i < m; ++i) {
+        if (!valid[i]) continue;
+        const long long r = r0 + i;
+        const bool pred = logits[r * ld + j] > 0.f, pos = targets[r * V + j] != 0;
+        a += pred && pos;
+        b += pred && !pos;
+        c += !pred && pos;
+      }
+      tp[j] += static_cast<double>(a);
+      fp[j] += static_cast<double>(b);
+      fn[j] += static_cast<double>(c);
+    }
+    __syncthreads();   // valid[] is rewritten by the next chunk
+  }
+  if (lane == 0) {
+    part[warp][kMlEvalCount] = cnt;
+    part[warp][kMlEvalInvalid] = bad;
+    part[warp][kMlEvalLoss] = loss;
+    part[warp][kMlEvalCorrect] = hits;
+    part[warp][kMlEvalExact] = exact;
+  }
+  __syncthreads();
+  if (threadIdx.x < kMlEvalUsedSlots) {
     double s = 0;
     for (int w = 0; w < kMetricWarps; ++w) s += part[w][threadIdx.x];
     acc[threadIdx.x] += s;
@@ -596,6 +683,14 @@ cudaError_t bn_fold(const long long* tab, const float* eps, const long long* row
 cudaError_t eval_metrics(const float* logits, const int* labels, const int* n_valid, double* acc,
                          int rows, int ld, int V, cudaStream_t s) {
   eval_metrics_kernel<<<1, kMetricThreads, 0, s>>>(logits, labels, n_valid, acc, rows, ld, V);
+  return cudaGetLastError();
+}
+
+cudaError_t multilabel_eval_metrics(const float* logits, const uint8_t* targets,
+                                    const int* n_valid, double* acc, int rows, int ld, int V,
+                                    cudaStream_t s) {
+  multilabel_eval_metrics_kernel<<<1, kMetricThreads, 0, s>>>(logits, targets, n_valid, acc, rows,
+                                                              ld, V);
   return cudaGetLastError();
 }
 

@@ -67,6 +67,18 @@ cudaError_t avgpool_bwd(const void* dy, void* dx, int N, int HW, int C, cudaStre
 cudaError_t softmax_xent(const void* logits, int logits_fp32, const int* labels, void* dlogits,
                          float* loss_sum, float* correct_sum, long long rows, int V, int ld,
                          int ldd, float scale, float label_smoothing, cudaStream_t s);
+// sigmoid_bce: multi-label binary cross-entropy with logits of fp32 logits [rows, ld] against
+// uint8 targets [rows, V] (nonzero = positive), columns [0, V) of the logits only.  With
+// t = y (1 - eps) + eps / 2 (eps = label_smoothing; t = y at 0) and p = pos_weight[j] (1 when
+// pos_weight is null; the null instance reads no weight vector):
+//   loss_sum += scale * sum_j [p t softplus(-l) + (1 - t) softplus(l)]     (stable softplus)
+//   dlogits (bf16 [rows, ldd], when not null) = (sigmoid(l) (p t + 1 - t) - p t) * scale,
+//   exactly 0 in columns [V, ldd); correct_sum (when not null) += rows with (l_j > 0) == y_j for
+//   every j < V.
+cudaError_t sigmoid_bce(const float* logits, const uint8_t* targets, void* dlogits,
+                        float* loss_sum, float* correct_sum, long long rows, int V, int ld,
+                        int ldd, float scale, float label_smoothing, const float* pos_weight,
+                        cudaStream_t s);
 cudaError_t decode_normalize(const uint8_t* in, void* out, int N, int H, int W, int C, int Wp,
                              int Cp, int wofs, const float* mean3, const float* istd3,
                              cudaStream_t s);
@@ -351,6 +363,18 @@ constexpr int kEvalCount = 0, kEvalTop1 = 1, kEvalTop5 = 2, kEvalInvalid = 3, kE
               kEvalUsedSlots = 5, kEvalSlots = 8;
 cudaError_t eval_metrics(const float* logits, const int* labels, const int* n_valid, double* acc,
                          int rows, int ld, int V, cudaStream_t s);
+// multilabel_eval_metrics: acc += totals of rows [0, *n_valid) of fp32 logits [rows, ld] (columns
+// [0, V)) against uint8 targets [rows, V].  A row with any byte > 1 is invalid: counted in
+// kMlEvalInvalid and not scored.  For the scored rows: kMlEvalCount rows, kMlEvalLoss the
+// unweighted, unsmoothed BCE sum, kMlEvalCorrect elements with (l > 0) == y, kMlEvalExact rows
+// with every element correct, and from slot kMlEvalSlots the per-class TP [V], FP [V], FN [V]
+// (kMlEvalSlots + 3 V slots).  A NaN logit predicts negative.  Deterministic: one CTA, fixed row
+// and class assignments, integer class counts, fixed-order fp64 sums.
+constexpr int kMlEvalCount = 0, kMlEvalInvalid = 1, kMlEvalLoss = 2, kMlEvalCorrect = 3,
+              kMlEvalExact = 4, kMlEvalUsedSlots = 5, kMlEvalSlots = 8;
+cudaError_t multilabel_eval_metrics(const float* logits, const uint8_t* targets,
+                                    const int* n_valid, double* acc, int rows, int ld, int V,
+                                    cudaStream_t s);
 // seg_eval_metrics: acc += totals of the pixels of images [0, *n_valid) of bf16 logits
 // [images * ppi, VP] (channels [0, V) only; VP as for pixel_xent) and int32 labels [images * ppi].
 // counter is one zeroed uint32 that the kernel leaves at zero.

@@ -40,6 +40,10 @@ update (Keras's ``global_clipnorm``, ``torch.nn.utils.clip_grad_norm_``), inside
 kernels; the step log then also reports the gradient's norm (``grad_norm``, before clipping).
 ``--clip_norm inf`` only measures it.
 
+Multi-label tagging: ``--multi_label`` trains the head with the binary cross-entropy on
+synthetic multi-hot labels (``ResNetTrainer(multi_label=True)``); the evaluation then reports
+``binary_accuracy``, ``exact_match``, ``f1`` and ``macro_f1`` in place of top-1 / top-5.
+
 Gradient accumulation: ``--gradient_accumulation_steps k`` updates the parameters once every k
 micro-batches of ``--batch_size`` with their mean gradient (Keras's
 ``gradient_accumulation_steps``), for an effective global batch of k * batch_size * workers.
@@ -101,6 +105,9 @@ def parse(argv):
                       "it) and log grad_norm")
   p.add_argument("--gradient_accumulation_steps", type=int, default=1,
                  help="micro-batches per update (k >= 1): the step counts above count updates")
+  p.add_argument("--multi_label", action="store_true",
+                 help="multi-hot labels and the binary cross-entropy; evaluation reports "
+                      "binary_accuracy, exact_match, f1 and macro_f1")
   return p.parse_args(argv)
 
 
@@ -137,6 +144,8 @@ def main_fun(argv, ctx):
   k = args.gradient_accumulation_steps
   if k != 1:
     opt["gradient_accumulation_steps"] = k
+  if args.multi_label:
+    opt["multi_label"] = True
   if args.model == "resnet56":
     net = resnet.CifarResNetTrainer(depth=56, batch=B, device="cuda:0", comm=comm, lr=base_lr, **opt)
   else:
@@ -182,19 +191,20 @@ def main_fun(argv, ctx):
     if not eval_batches:   # seeds disjoint from the training batch's (seed = rank)
       eval_batches.extend(net.synthetic_batch(seed=EVAL_SEED + ctx.rank * args.eval_steps + i)
                           for i in range(args.eval_steps))
+    keys = ("binary_accuracy", "exact_match", "f1", "macro_f1") if args.multi_label else \
+        ("top1", "top5")
     res = net.evaluate(eval_batches)
     if ctx.is_chief:
-      print("eval: step {} loss {:.4f} top1 {:.4f} top5 {:.4f} ({} images)".format(
-          step, res["loss"], res["top1"], res["top5"], res["count"]))
-    fields = {"eval_loss": res["loss"], "eval_top1": res["top1"], "eval_top5": res["top5"],
-              "eval_count": res["count"]}
+      print("eval: step {} loss {:.4f} {} ({} images)".format(
+          step, res["loss"], " ".join("{} {:.4f}".format(k_, res[k_]) for k_ in keys),
+          res["count"]))
+    fields = dict({"eval_" + k_: res[k_] for k_ in ("loss",) + keys}, eval_count=res["count"])
     if args.ema_decay is not None:   # the weight average on the same batches
       avg = net.evaluate(eval_batches, averaged=True)
       if ctx.is_chief:
-        print("eval: step {} avg loss {:.4f} avg top1 {:.4f} avg top5 {:.4f}".format(
-            step, avg["loss"], avg["top1"], avg["top5"]))
-      fields.update(eval_avg_loss=avg["loss"], eval_avg_top1=avg["top1"],
-                    eval_avg_top5=avg["top5"])
+        print("eval: step {} avg loss {:.4f} {}".format(
+            step, avg["loss"], " ".join("avg {} {:.4f}".format(k_, avg[k_]) for k_ in keys)))
+      fields.update({"eval_avg_" + k_: avg[k_] for k_ in ("loss",) + keys})
     if log:
       log.log(step=step, **fields)
     if events:

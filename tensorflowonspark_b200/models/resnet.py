@@ -8,6 +8,7 @@ Keras model (examples/resnet/resnet_cifar_dist.py:208, momentum SGD with a
 piecewise schedule :35-66); BASELINE.json names ResNet-50/ImageNet-shaped data
 as the headline config.  Both are provided here.
 """
+import math
 import numbers
 import os
 
@@ -47,6 +48,40 @@ def _check_head_args(num_classes, label_smoothing):
     raise ValueError("label_smoothing must be a real number in [0, 1], got {!r}".format(
         label_smoothing))
   return int(num_classes), float(label_smoothing)
+
+
+def _check_multilabel_args(multi_label, pos_weight, num_classes, training=True):
+  """(multi_label, pos_weight as a tuple of floats or None); ValueError unless multi_label is a
+  bool and pos_weight is None or, on a multi-label training trainer, ``num_classes`` finite
+  numbers >= 0.  The trainers call it before they allocate."""
+  if not isinstance(multi_label, bool):
+    raise ValueError("multi_label must be a bool, got {!r}".format(multi_label))
+  if pos_weight is None:
+    return multi_label, None
+  if not multi_label:
+    raise ValueError("pos_weight weighs the positives of the multi-label loss: it needs "
+                     "multi_label=True")
+  if not training:
+    raise ValueError("pos_weight is a training loss option: not on a training=False trainer")
+  try:
+    w = tuple(float(v) for v in pos_weight)
+  except (TypeError, ValueError):
+    raise ValueError("pos_weight must be a sequence of {} numbers, got {!r}".format(
+        num_classes, pos_weight))
+  if len(w) != num_classes:
+    raise ValueError("pos_weight must hold one value per class ({}), got {}".format(
+        num_classes, len(w)))
+  bad = [v for v in w if not (math.isfinite(v) and v >= 0.0)]
+  if bad:
+    raise ValueError("pos_weight values must be finite and >= 0, got {!r}".format(bad[0]))
+  return multi_label, w
+
+
+def _labels_buffer(B, V, multi_label, device):
+  """Training labels: int32 class indices [B], or uint8 multi-hot targets [B, V]."""
+  if multi_label:
+    return torch.zeros((B, V), dtype=torch.uint8, device=device)
+  return torch.zeros(B, dtype=torch.int32, device=device)
 
 
 def _padded_head_init(V, std=0.01):
@@ -92,6 +127,28 @@ def fold_table(store, units, running):
           torch.tensor(row0, dtype=torch.int64), boff)
 
 
+def multilabel_totals(h, V):
+  """``eval_end()`` of a multi-label trainer from the summed multilabel_eval_metrics accumulator
+  ``h`` (8 + 3 V values: rows scored, invalid rows, BCE sum, correct elements, exact-match rows,
+  3 unused, then per-class TP [V], FP [V], FN [V]).  Precision, recall and F1 are micro averages of
+  the summed counts, F1 = 2 TP / (2 TP + FP + FN); a ratio whose denominator is 0 is NaN.  A class
+  with TP + FP + FN = 0 has F1 NaN and is left out of ``macro_f1`` (Keras's ``F1Score`` counts it
+  as 0).  Raises ValueError when any row held a label byte other than 0 or 1."""
+  if h[1] > 0:
+    raise ValueError("evaluation saw {} row(s) with a label byte other than 0 or 1".format(
+        int(h[1])))
+  ratio = lambda a, b: a / b if b else float("nan")   # noqa: E731
+  count = int(h[0])
+  tp, fp, fn = h[8:8 + V], h[8 + V:8 + 2 * V], h[8 + 2 * V:8 + 3 * V]
+  TP, FP, FN = sum(tp), sum(fp), sum(fn)
+  per_class = [ratio(2 * a, 2 * a + b + c) for a, b, c in zip(tp, fp, fn)]
+  present = [f for f in per_class if f == f]
+  return {"count": count, "loss": ratio(h[2], count * V), "binary_accuracy": ratio(h[3], count * V),
+          "exact_match": ratio(h[4], count), "precision": ratio(TP, TP + FP),
+          "recall": ratio(TP, TP + FN), "f1": ratio(2 * TP, 2 * TP + FP + FN),
+          "macro_f1": ratio(sum(present), len(present)), "f1_per_class": per_class}
+
+
 class _Evaluator(object):
   """Held-out evaluation on a trainer's own buffers (``eval_begin`` / ``eval_step`` /
   ``eval_end`` of both ResNet trainers).
@@ -119,20 +176,23 @@ class _Evaluator(object):
     self.u8 = torch.zeros_like(net.in_u8)         # never in_u8: drivers stage a batch and replay
     self.labels = torch.zeros_like(net.labels)
     self.n_valid = torch.zeros(1, dtype=torch.int32, device=dev)
-    self.acc = torch.zeros(8, dtype=torch.float64, device=dev)
     self.V = net.num_classes
+    self.multi_label = net.multi_label
+    # multilabel_eval_metrics: 8 totals, then per-class TP / FP / FN (csrc/ops.h kMlEval*)
+    slots = ops.C().multilabel_eval_slots(self.V) if self.multi_label else 8
+    self.acc = torch.zeros(slots, dtype=torch.float64, device=dev)
     if comm is None:
       self.running = net.running.tensor()
     else:
       self.running = comm.alloc("eval_running", net.running.used, torch.float32)
-    self.rank_sum = evaluation.RankSum(comm, "eval_totals", 8)
+    self.rank_sum = evaluation.RankSum(comm, "eval_totals", slots)
     self._wv, self._bias = (lambda spec: st._view(self.wf, spec)), bias
     # one forward (and graph) per model: "live" reads the head from the store, "averaged" (built
     # on the first averaged evaluation) from a copy of the averaged head in wf / head_b
     self._modes = {False: {"forward": net._eval_forward(self._wv, bias, self.u8), "graph": None,
                            "calls": 0}}
     self.averaged = False
-    self.staging = evaluation.HostStaging(dev, net.B, self.u8.shape[1:], ())
+    self.staging = evaluation.HostStaging(dev, net.B, self.u8.shape[1:], self.labels.shape[1:])
 
   @property
   def graph(self):
@@ -169,7 +229,10 @@ class _Evaluator(object):
 
   def _run(self):
     self._modes[self.averaged]["forward"]()
-    ops.K.eval_metrics(self.net.logits, self.labels, self.n_valid, self.acc, self.V)
+    if self.multi_label:
+      ops.K.multilabel_eval_metrics(self.net.logits, self.labels, self.n_valid, self.acc, self.V)
+    else:
+      ops.K.eval_metrics(self.net.logits, self.labels, self.n_valid, self.acc, self.V)
 
   def step(self, images_u8, labels):
     n = len(images_u8)
@@ -178,7 +241,8 @@ class _Evaluator(object):
     if n:
       x = torch.as_tensor(images_u8)
       self.u8[:n].copy_(x.reshape((n,) + tuple(self.u8.shape[1:])), non_blocking=True)
-      self.labels[:n].copy_(torch.as_tensor(labels).reshape(n), non_blocking=True)
+      self.labels[:n].copy_(torch.as_tensor(labels).reshape((n,) + tuple(self.labels.shape[1:])),
+                            non_blocking=True)
     self.n_valid.fill_(n)
     m = self._modes[self.averaged]
     if m["graph"] is None and m["calls"] >= 1:
@@ -202,10 +266,15 @@ class _Evaluator(object):
   def run(self, batches):
     """eval_step over (images, labels) pairs; host batches are staged in page-locked memory one
     batch ahead of the forward pass."""
-    self.staging.run(self.step, batches)
+    if self.multi_label:   # bool or uint8 host targets are staged as uint8 bytes
+      self.staging.run(self.step, batches, label_dtype=lambda y: torch.uint8)
+    else:
+      self.staging.run(self.step, batches)
 
   def end(self):
     h = self.rank_sum(self.acc)
+    if self.multi_label:
+      return multilabel_totals(h, self.V)
     if h[3] > 0:
       raise ValueError("evaluation saw {} label(s) outside [0, {})".format(int(h[3]), self.V))
     count = int(h[0])
@@ -223,7 +292,7 @@ class ResNetTrainer(object):
                lr=0.1, momentum=0.9, weight_decay=1e-4, comm=None, training=True, seed=1234,
                optimizer="momentum", trust_coefficient=0.001, label_smoothing=0.0,
                ema_decay=None, clip_norm=None, beta1=0.9, beta2=0.999, epsilon=1e-7,
-               gradient_accumulation_steps=1):
+               gradient_accumulation_steps=1, multi_label=False, pos_weight=None):
     """``optimizer``: sgd | momentum | adam | adamw | lars | lamb (``trust_coefficient`` is LARS's
     eta; see parallel/fused_optim.py).  adam folds ``weight_decay`` into the gradient (L2), adamw
     decouples it (``torch.optim.AdamW``), lamb is layer-wise adaptive Adam (apex ``FusedLAMB``).
@@ -252,8 +321,22 @@ class ResNetTrainer(object):
     the micro-batch's), label smoothing applies per micro-batch, and the batch-norm batch and
     running statistics are per micro-batch, as in Keras and PyTorch.  Clipping, the LARS / LAMB
     norms, weight decay, the weight average and Adam's step advance once per update.
-    ``micro_step`` is the position of the next call in its window (0 .. k-1)."""
+    ``micro_step`` is the position of the next call in its window (0 .. k-1).
+
+    ``multi_label`` (bool): each image has a multi-hot target of ``num_classes`` entries, and the
+    labels are uint8 (or bool) [n, num_classes], 0 = negative, 1 = positive (training counts any
+    nonzero byte as positive).  The training loss is the mean over the B x V elements of the binary
+    cross-entropy with logits (``torch.nn.BCEWithLogitsLoss``, Keras's
+    ``BinaryCrossentropy(from_logits=True)``); ``label_smoothing`` eps then smooths the targets to
+    y (1 - eps) + eps / 2, as Keras does.  ``pos_weight`` (training only): None or num_classes
+    finite numbers >= 0, torch's ``pos_weight``: element (i, j) costs
+    -[p_j t log sigmoid(l) + (1 - t) log(1 - sigmoid(l))].  ``train_step`` returns the mean loss
+    and ``correct`` counts the rows whose prediction (logit > 0 per class) equals the target
+    exactly; ``eval_end`` reports binary accuracy, exact match and micro / macro F1
+    (``multilabel_totals``); serving returns a multi-hot ``prediction``."""
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
+    self.multi_label, pos_weight = _check_multilabel_args(multi_label, pos_weight, num_classes,
+                                                          training)
     k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps, training)
     self.ema_decay = engine.check_ema_decay(ema_decay, training)
     self.clip_norm = engine.check_clip_norm(clip_norm, training)
@@ -297,7 +380,9 @@ class ResNetTrainer(object):
     OH, OW, Wp = igemm.stem_geometry(image, image)
     self.in_u8 = _buf((B, image, image, 3), dev, torch.uint8)
     self.xp = _buf((B, image, Wp, 8), dev)
-    self.labels = torch.zeros(B, dtype=torch.int32, device=dev)
+    self.labels = _labels_buffer(B, num_classes, self.multi_label, dev)
+    self.pos_weight = None if pos_weight is None else torch.tensor(pos_weight, dtype=torch.float32,
+                                                                   device=dev)
     self.stem_raw = _buf((B, OH, OW, 64), dev)
     PH, PW = (OH + 2 - 3) // 2 + 1, (OW + 2 - 3) // 2 + 1
     self.pool = _buf((B, PH, PW, 64), dev)
@@ -466,7 +551,10 @@ class ResNetTrainer(object):
     g = torch.Generator(device="cpu")
     g.manual_seed(seed)
     x = torch.randint(0, 256, (self.B, self.image, self.image, 3), dtype=torch.uint8, generator=g)
-    y = torch.randint(0, self.num_classes, (self.B,), dtype=torch.int32, generator=g)
+    if self.multi_label:   # each class present with probability 1/2
+      y = torch.randint(0, 2, (self.B, self.num_classes), dtype=torch.uint8, generator=g)
+    else:
+      y = torch.randint(0, self.num_classes, (self.B,), dtype=torch.int32, generator=g)
     return x.to(self.device), y.to(self.device)
 
   def set_input(self, images_u8, labels=None):
@@ -553,6 +641,12 @@ class ResNetTrainer(object):
   def _loss(self, with_grad):
     self.loss_sum.zero_()
     self.correct.zero_()
+    if self.multi_label:
+      ops.K.sigmoid_bce(self.logits, self.labels, self.dlogits if with_grad else None,
+                        self.loss_sum, self.correct, self.num_classes,
+                        1.0 / (self.B * self.num_classes), label_smoothing=self.label_smoothing,
+                        pos_weight=self.pos_weight)
+      return
     ops.K.softmax_xent(self.logits, self.labels, self.dlogits if with_grad else None,
                        self.loss_sum, self.correct, self.num_classes, 1.0 / self.B,
                        label_smoothing=self.label_smoothing)
@@ -741,8 +835,9 @@ class ResNetTrainer(object):
 
   def eval_step(self, images_u8, labels):
     """Add the top-1 / top-5 / loss totals of n <= B images (host or device, uint8 NHWC) and their
-    labels.  Runs the folded network on the training buffers, leaving ``in_u8`` / ``labels`` and
-    the training state untouched; ``logits`` then holds the batch's logits.  No host sync."""
+    labels (``multi_label``: bool or uint8 [n, V] targets and the multi-label totals).  Runs the
+    folded network on the training buffers, leaving ``in_u8`` / ``labels`` and the training state
+    untouched; ``logits`` then holds the batch's logits.  No host sync."""
     self._eval_state().step(images_u8, labels)
 
   def eval_end(self):
@@ -750,7 +845,9 @@ class ResNetTrainer(object):
     the last three are means over ``count`` (NaN when it is 0).  ``loss`` is the plain
     cross-entropy whatever the trainer's ``label_smoothing``, so that scores of runs with different
     smoothing compare.  Raises ValueError on every rank when any rank saw a label outside
-    [0, num_classes)."""
+    [0, num_classes).  With ``multi_label``: {"count", "loss", "binary_accuracy", "exact_match",
+    "precision", "recall", "f1", "macro_f1", "f1_per_class"} (``multilabel_totals``; the loss is
+    the plain BCE, a mean over count * V), and the ValueError is for a label byte other than 0 / 1."""
     return self._eval_state().end()
 
   def evaluate(self, batches, averaged=False):
@@ -790,13 +887,26 @@ class ResNetTrainer(object):
 
   # ------------------------------------------------- checkpoints / serving
   export_builder = "tensorflowonspark_b200.models.resnet:build_served"
-  export_signatures = {"serving_default": {
-      "inputs": {"image": "image"}, "outputs": {"logits": "logits", "prediction": "prediction"},
-      "input_dtypes": {"image": "uint8"}}}
+
+  @property
+  def export_signatures(self):
+    """logits [n, V] fp32 and prediction: the arg-max class (int64 [n]), or with ``multi_label``
+    the multi-hot uint8 [n, V] of logit > 0, one bytes cell of V values per row (as the U-Net's
+    mask)."""
+    sig = {"inputs": {"image": "image"}, "outputs": {"logits": "logits", "prediction": "prediction"},
+           "input_dtypes": {"image": "uint8"}}
+    if self.multi_label:
+      sig["output_dtypes"] = {"prediction": "uint8"}
+      sig["output_shapes"] = {"logits": [-1, self.num_classes],
+                              "prediction": [-1, self.num_classes]}
+    return {"serving_default": sig}
 
   @property
   def export_builder_args(self):
-    return {"depth": self.depth, "image": self.image, "num_classes": self.num_classes}
+    args = {"depth": self.depth, "image": self.image, "num_classes": self.num_classes}
+    if self.multi_label:   # an export without the key serves as softmax
+      args["multi_label"] = True
+    return args
 
   def state_dict(self):
     """Parameters (fp32 masters, assembled across ranks when sharded) + the batch-norm running
@@ -848,19 +958,24 @@ class ServedResNet(serving.Replica):
   executor's GPU.  ``submit(inputs)`` stages a uint8 NHWC batch in page-locked memory, copies it
   on the copy stream and enqueues the forward pass (~165 launches) + arg-max and an async
   read-back of ``logits`` and ``prediction``; ``collect()`` returns the oldest submitted batch
-  (models/serving.Replica)."""
+  (models/serving.Replica).  ``multi_label``: ``prediction`` is the multi-hot uint8 [n, V] of
+  logit > 0 instead of the arg-max."""
 
-  def __init__(self, state, depth=50, image=224, num_classes=1000, batch=256, device="cuda:0"):
+  def __init__(self, state, depth=50, image=224, num_classes=1000, batch=256, device="cuda:0",
+               multi_label=False):
     torch.cuda.set_device(torch.device(device))
     self.net = ResNetTrainer(depth=depth, batch=batch, image=image, num_classes=num_classes,
-                             device=device, training=False)
+                             device=device, training=False, multi_label=multi_label)
     self.net.load_state_dict(state)
     self.folded = os.environ.get("TFOS_SERVE_FOLD_BN", "1") == "1"
     if self.folded:
       self.net.build_folded_inference()
     self._fwd = self.net.forward_folded if self.folded else (lambda: self.net._forward(False))
-    self.image, self.V = image, num_classes
-    self.pred_dev = torch.zeros(batch, dtype=torch.int64, device=self.net.device)
+    self.image, self.V, self.multi_label = image, num_classes, multi_label
+    if multi_label:
+      self.pred_dev = torch.zeros((batch, num_classes), dtype=torch.uint8, device=self.net.device)
+    else:
+      self.pred_dev = torch.zeros(batch, dtype=torch.int64, device=self.net.device)
     super(ServedResNet, self).__init__(
         self.net.device, batch, (image, image, 3),
         {"logits": self.net.logits[:, :num_classes], "prediction": self.pred_dev},
@@ -868,27 +983,33 @@ class ServedResNet(serving.Replica):
 
   def _run(self):
     self._fwd()
-    self.pred_dev.copy_(self.net.logits[:, :self.V].argmax(1))
+    if self.multi_label:
+      self.pred_dev.copy_(self.net.logits[:, :self.V] > 0)
+    else:
+      self.pred_dev.copy_(self.net.logits[:, :self.V].argmax(1))
 
 
-def build_served(state, depth=50, image=224, num_classes=1000, batch=None, **_):
-  """Export builder (utils/checkpoint.py): rebuilds the replica on the executor's GPU."""
+def build_served(state, depth=50, image=224, num_classes=1000, batch=None, multi_label=False, **_):
+  """Export builder (utils/checkpoint.py): rebuilds the replica on the executor's GPU.  An export
+  written before multi-label heads existed has no ``multi_label`` and serves as softmax."""
   return ServedResNet(state, depth=depth, image=image, num_classes=num_classes,
-                      batch=serving.serve_batch(batch))
+                      batch=serving.serve_batch(batch), multi_label=bool(multi_label))
 
 
 class CifarResNetTrainer(object):
   """ResNet-20/32/56 for 32x32 inputs (basic blocks, 16/32/64 channels) - the network the
   reference example actually trains (examples/resnet/resnet_cifar_dist.py:208, ``resnet56``,
   momentum SGD, batch 128, weight decay 2e-4).  ``optimizer``, ``num_classes``,
-  ``label_smoothing``, ``ema_decay``, ``clip_norm``, ``beta1``, ``beta2``, ``epsilon`` and
-  ``gradient_accumulation_steps`` as in ResNetTrainer."""
+  ``label_smoothing``, ``ema_decay``, ``clip_norm``, ``beta1``, ``beta2``, ``epsilon``,
+  ``gradient_accumulation_steps``, ``multi_label`` and ``pos_weight`` as in ResNetTrainer."""
 
   def __init__(self, depth=56, batch=128, num_classes=10, device="cuda:0", lr=0.1, momentum=0.9,
                weight_decay=2e-4, comm=None, seed=1234, optimizer="momentum",
                trust_coefficient=0.001, label_smoothing=0.0, ema_decay=None, clip_norm=None,
-               beta1=0.9, beta2=0.999, epsilon=1e-7, gradient_accumulation_steps=1):
+               beta1=0.9, beta2=0.999, epsilon=1e-7, gradient_accumulation_steps=1,
+               multi_label=False, pos_weight=None):
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
+    self.multi_label, pos_weight = _check_multilabel_args(multi_label, pos_weight, num_classes)
     k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps)
     self.ema_decay = engine.check_ema_decay(ema_decay)
     self.clip_norm = engine.check_clip_norm(clip_norm)
@@ -920,7 +1041,9 @@ class CifarResNetTrainer(object):
 
     self.in_u8 = _buf((B, 32, 32, 3), dev, torch.uint8)
     self.x8 = _buf((B, 32, 32, 8), dev)
-    self.labels = torch.zeros(B, dtype=torch.int32, device=dev)
+    self.labels = _labels_buffer(B, num_classes, self.multi_label, dev)
+    self.pos_weight = None if pos_weight is None else torch.tensor(pos_weight, dtype=torch.float32,
+                                                                   device=dev)
     self.stem_raw, self.stem_act = _buf((B, 32, 32, 16), dev), _buf((B, 32, 32, 16), dev)
     self.g_stem_raw = _buf((B, 32, 32, 16), dev)
     self.running = engine.RunningArena(dev)
@@ -977,6 +1100,7 @@ class CifarResNetTrainer(object):
   load_state_dict = ResNetTrainer.load_state_dict
   load_backbone = ResNetTrainer.load_backbone
   set_input = ResNetTrainer.set_input
+  _loss = ResNetTrainer._loss
   capture = ResNetTrainer.capture
   train_step = ResNetTrainer.train_step
   set_lr = ResNetTrainer.set_lr
@@ -1040,10 +1164,7 @@ class CifarResNetTrainer(object):
       b.u2.bn.forward(b.r2, b.out, b.idn if b.ds is not None else b.x, 1, True)
     K.avgpool_fwd(self.last, self.avg)
     self.fc.forward()
-    self.loss_sum.zero_()
-    self.correct.zero_()
-    K.softmax_xent(self.logits, self.labels, self.dlogits, self.loss_sum, self.correct,
-                   self.num_classes, 1.0 / self.B, label_smoothing=self.label_smoothing)
+    self._loss(True)
     if zero:
       self.optim.zero_grads()
     if self.grad_scratch is not None:

@@ -92,6 +92,12 @@ KERNELS = [
     ("seg_eval_wide_g32", r"seg_eval_wide_kernel<32, false>"),
     ("softmax_xent", r"softmax_xent_kernel<float, false>("),
     ("softmax_xent_smooth", r"softmax_xent_kernel<float, true>("),
+    # multi-label heads: the BCE loss (plain, smoothed, pos_weight, both) and its evaluation
+    ("sigmoid_bce", r"sigmoid_bce_kernel<false, false>"),
+    ("sigmoid_bce_smooth", r"sigmoid_bce_kernel<true, false>"),
+    ("sigmoid_bce_pos_weight", r"sigmoid_bce_kernel<false, true>"),
+    ("sigmoid_bce_smooth_pos_weight", r"sigmoid_bce_kernel<true, true>"),
+    ("multilabel_eval_metrics", r"multilabel_eval_metrics_kernel"),
 ]
 KEY = ("HGMMA", "UTMALDG", "WARPGROUP", "LDGMC", "SYNCS", "HMMA", "RED", "ATOM", "ST.E", "STG", "LDG")
 
