@@ -1158,22 +1158,55 @@ void set_flag_timeout_ms(double ms) {
 void flag_barrier(const py::dict& d) {
   check(tfos::flag_barrier(parse_bcast(d), cur_stream()), "flag_barrier");
 }
+// hyper[0] (lr) and hyper[3] (gradient scale) are read on the device
+void need_ps_hyper(const Tensor& hyper, const char* what) {
+  need(hyper, torch::kFloat32, "hyper");
+  TFOS_REQUIRE(hyper.numel() >= 4, what, ": hyper must hold at least 4 values, got ",
+               hyper.numel());
+}
 void ps_push_dense(uint64_t w_ps, const Tensor& g, const Tensor& hyper) {
   need(g, torch::kFloat32, "g");
+  need_ps_hyper(hyper, "ps_push_dense");
+  TFOS_REQUIRE(w_ps != 0 || g.numel() == 0, "ps_push_dense: w_ps is null");
   check(tfos::ps_push_dense(reinterpret_cast<float*>(w_ps), g.data_ptr<float>(), g.numel(),
                             hyper.data_ptr<float>(), cur_stream()),
         "ps_push_dense");
 }
+// The indices are not range-checked (that would need a device sync): every idx must name a row
+// of the table at w_ps.
 void ps_push_sparse(uint64_t w_ps, const Tensor& g_rows, const Tensor& idx, const Tensor& hyper) {
   need(g_rows, torch::kFloat32, "g_rows");
   need(idx, torch::kInt32, "idx");
+  need_ps_hyper(hyper, "ps_push_sparse");
+  TFOS_REQUIRE(g_rows.dim() == 2, "ps_push_sparse: g_rows must be [rows, width], got ",
+               shape_str(g_rows));
+  TFOS_REQUIRE(idx.dim() == 1, "ps_push_sparse: idx must be 1-D, got ", shape_str(idx));
+  need_numel(idx, g_rows.size(0), "ps_push_sparse", "idx (one index per row of g_rows)");
+  TFOS_REQUIRE(g_rows.size(0) <= INT32_MAX && g_rows.size(1) <= INT32_MAX,
+               "ps_push_sparse: g_rows is too large, got ", shape_str(g_rows));
+  TFOS_REQUIRE(w_ps != 0 || g_rows.numel() == 0, "ps_push_sparse: w_ps is null");
   check(tfos::ps_push_sparse(reinterpret_cast<float*>(w_ps), g_rows.data_ptr<float>(),
                              idx.data_ptr<int>(), g_rows.size(0), g_rows.size(1),
                              hyper.data_ptr<float>(), cur_stream()),
         "ps_push_sparse");
 }
+// The 16-byte vector path needs w_ps and w_local 16-byte aligned and w_bf16 8-byte aligned;
+// misaligned pointers are refused (every caller passes slices that start on multiples of 8).
 void ps_pull(uint64_t w_ps, c10::optional<Tensor> w_local, c10::optional<Tensor> w_bf16,
              long long n) {
+  TFOS_REQUIRE(n >= 0, "ps_pull: n must be >= 0, got ", n);
+  TFOS_REQUIRE(w_ps != 0 || n == 0, "ps_pull: w_ps is null");
+  TFOS_REQUIRE(w_ps % 16 == 0, "ps_pull: w_ps must be 16-byte aligned");
+  if (w_local.has_value() && w_local->defined()) {
+    need(*w_local, torch::kFloat32, "w_local");
+    need_numel(*w_local, n, "ps_pull", "w_local");
+    need_aligned(*w_local, 16, "w_local");
+  }
+  if (w_bf16.has_value() && w_bf16->defined()) {
+    need(*w_bf16, torch::kBFloat16, "w_bf16");
+    need_numel(*w_bf16, n, "ps_pull", "w_bf16");
+    need_aligned(*w_bf16, 8, "w_bf16");
+  }
   check(tfos::ps_pull(reinterpret_cast<const float*>(w_ps), optf(w_local),
                       const_cast<void*>(optptr(w_bf16)), n, cur_stream()),
         "ps_pull");

@@ -799,6 +799,8 @@ __global__ void __launch_bounds__(512) ps_apply_kernel(const PsApplyArgs a) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) w[j] -= g[j];
     } else {
+      // a group may straddle ema_begin (any value is accepted): the tail test is per element, as
+      // the decay test is; the state of a tail element is stored back unchanged
       float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
       if (OPT != kOptSgd) {
         const float4 m = *reinterpret_cast<const float4*>(a.state1 + i);
@@ -810,7 +812,8 @@ __global__ void __launch_bounds__(512) ps_apply_kernel(const PsApplyArgs a) {
       }
 #pragma unroll
       for (int j = 0; j < 4; ++j)
-        w[j] = opt_update<OPT>(w[j], g[j], s1[j], s2[j], h, gi + j < a.decay_end);
+        w[j] = gi + j < a.ema_begin ? opt_update<OPT>(w[j], g[j], s1[j], s2[j], h, gi + j < a.decay_end)
+                                    : w[j] - g[j];
       if (OPT != kOptSgd)
         *reinterpret_cast<float4*>(a.state1 + i) = make_float4(s1[0], s1[1], s1[2], s1[3]);
       if (OPT == kOptAdam)
@@ -1026,6 +1029,12 @@ cudaError_t ps_push_sparse(float* w_ps, const float* g_rows, const int* idx, int
 }
 cudaError_t ps_apply(const PsApplyArgs& a, int opt, cudaStream_t s) {
   if ((a.n & 7) != 0 || (a.lo & 7) != 0) return cudaErrorInvalidValue;
+  if (a.n < 0 || a.lo < 0 || a.hyper == nullptr || a.applied_flag == nullptr ||
+      a.block_counter == nullptr)
+    return cudaErrorInvalidValue;
+  if (a.n > 0 && (a.master == nullptr || a.wbf16 == nullptr || a.slot == nullptr ||
+                  (opt != kOptSgd && a.state1 == nullptr) || (opt == kOptAdam && a.state2 == nullptr)))
+    return cudaErrorInvalidValue;
   const int grid = kSmCount * 2;
   switch (opt) {
     case kOptSgd: ps_apply_kernel<kOptSgd><<<grid, 512, 0, s>>>(a); break;
@@ -1035,18 +1044,43 @@ cudaError_t ps_apply(const PsApplyArgs& a, int opt, cudaStream_t s) {
   }
   return cudaGetLastError();
 }
+// The slot kernels read or write each source and destination only where the slice needs it: the
+// gradients for elements below total, aux32 for [decay_end, total), the running statistics at and
+// past total.  A slice that needs one the caller left null is refused before the launch.
 cudaError_t ps_push_slot(const PsPushArgs& a, int grid, cudaStream_t s) {
   if ((a.n & 7) != 0 || (a.lo & 7) != 0 || (a.total & 7) != 0) return cudaErrorInvalidValue;
+  if (a.n < 0 || a.lo < 0 || grid < 1 || a.applied_flag == nullptr || a.ready_flag == nullptr ||
+      a.block_counter == nullptr)
+    return cudaErrorInvalidValue;
+  if (a.n > 0 && (a.slot == nullptr || (a.lo < a.total && a.grads == nullptr)))
+    return cudaErrorInvalidValue;
+  if (a.lo + a.n > a.total && (a.running == nullptr || a.running_pulled == nullptr))
+    return cudaErrorInvalidValue;
   ps_push_slot_kernel<<<grid, 512, 0, s>>>(a);
   return cudaGetLastError();
 }
 cudaError_t ps_pull_model(const PsPullArgs& a, int grid, cudaStream_t s) {
   if ((a.n & 7) != 0 || (a.lo & 7) != 0 || (a.total & 7) != 0 || (a.decay_end & 7) != 0)
     return cudaErrorInvalidValue;
+  if (a.n < 0 || a.lo < 0 || grid < 1 || a.decay_end < 0 || a.decay_end > a.total)
+    return cudaErrorInvalidValue;
+  if (a.n > 0 && (a.wbf16 == nullptr || a.master == nullptr)) return cudaErrorInvalidValue;
+  const long long hi = a.lo + a.n;
+  if (a.lo < a.total && hi > a.lo && a.weights == nullptr) return cudaErrorInvalidValue;
+  if ((a.lo > a.decay_end ? a.lo : a.decay_end) < (hi < a.total ? hi : a.total) &&
+      a.aux32 == nullptr)
+    return cudaErrorInvalidValue;
+  if (hi > a.total && (a.running == nullptr || a.running_pulled == nullptr))
+    return cudaErrorInvalidValue;
   ps_pull_model_kernel<<<grid, 512, 0, s>>>(a);
   return cudaGetLastError();
 }
 cudaError_t ps_pull(const float* w_ps, float* w_local, void* w_bf16, long long n, cudaStream_t s) {
+  // the vector path moves 16 bytes of fp32 and 8 of bf16 at every multiple of 4 elements
+  if (n < 0 || (n > 0 && w_ps == nullptr) ||
+      ((reinterpret_cast<uintptr_t>(w_ps) | reinterpret_cast<uintptr_t>(w_local)) & 15) != 0 ||
+      (reinterpret_cast<uintptr_t>(w_bf16) & 7) != 0)
+    return cudaErrorInvalidValue;
   long long blocks = (n / 4 + 255) / 256;
   if (blocks > kSmCount * 4) blocks = kSmCount * 4;
   if (blocks < 1) blocks = 1;

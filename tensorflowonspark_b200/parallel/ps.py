@@ -67,6 +67,62 @@ def _slices(numel, num_ps):
   return [(min(numel, i * per), min(numel, (i + 1) * per)) for i in range(num_ps)]
 
 
+def _sparse_plan(lo, hi, base, width):
+  """How a server owning flat elements [lo, hi) applies a row-sparse push to a [rows, width] table
+  at flat offset ``base``: ``(r0, r1, cuts)``.  Rows r0 <= r < r1 lie wholly inside the slice (the
+  sparse kernel); ``cuts`` lists ``(r, a, b)`` for each row the slice cuts, whose owned elements
+  are [a, b) (the dense kernel).  Every row appears at most once, in one of the two: a row wider
+  than the slice can be cut at both of its edges."""
+  if hi <= max(lo, base):
+    return 0, 0, []
+  first = max(lo - base, 0) // width        # rows overlapping the slice: first .. last
+  last = (hi - 1 - base) // width
+  r0 = first + int(base + first * width < lo)
+  r1 = last + 1 - int(base + (last + 1) * width > hi)
+  cuts = []
+  for r in sorted({first, last}):
+    s = base + r * width
+    if s < lo or s + width > hi:
+      cuts.append((r, max(s, lo), min(s + width, hi)))
+  return r0, max(r0, r1), cuts
+
+
+def _check_pull_model(numel, total, decay_end, weights, aux32, running):
+  """Refuse, before any launch, a GPU ``pull_model`` whose destinations cannot hold what the
+  servers send: the bf16 weights [total], the fp32 copy of [decay_end, total) and the running
+  statistics [total, numel)."""
+  if weights is None or weights.numel() < total:
+    raise ValueError("pull_model needs bf16 weights of at least total = {} elements".format(total))
+  if not 0 <= decay_end <= total:
+    raise ValueError("pull_model needs 0 <= decay_end <= total, got {} and {}".format(
+        decay_end, total))
+  if decay_end < total and (aux32 is None or aux32.numel() < total - decay_end):
+    raise ValueError("pull_model needs aux32 of at least total - decay_end = {} elements".format(
+        total - decay_end))
+  if total > numel:
+    raise ValueError("total {} exceeds the {} parameters the servers hold".format(total, numel))
+  if numel > total and (running is None or running.numel() != numel - total):
+    raise ValueError("the servers hold {} running statistics past total: pull_model needs "
+                     "running of that length".format(numel - total))
+
+
+def _check_push_grads(numel, total, grads, running, running_pulled):
+  """Refuse, before any launch, a GPU ``push_grads`` whose sources do not cover the servers'
+  slices: the gradients [total] and, past total, the running statistics together with the
+  snapshot ``pull_model`` took of them."""
+  if total > numel:
+    raise ValueError("total {} exceeds the {} parameters the servers hold".format(total, numel))
+  if total > 0 and (grads is None or grads.numel() < total):
+    raise ValueError("push_grads needs gradients of at least total = {} elements".format(total))
+  if numel > total:
+    if running is None or running.numel() != numel - total:
+      raise ValueError("the servers hold {} running statistics past total: push_grads needs "
+                       "running of that length".format(numel - total))
+    if running_pulled is None or running_pulled.numel() != running.numel():
+      raise ValueError("push_grads with running statistics needs a pull_model(..., running) "
+                       "first: their deltas are taken against what it pulled")
+
+
 OPTS = {"sgd": 0, "momentum": 1, "adam": 2}
 NSLOTS = 2   # gradient slots per worker on each server (push i+1 overlaps the apply of push i)
 
@@ -375,9 +431,13 @@ class PSClient(object):
     if not self.cuda:
       return np.concatenate([a for a in self.arrays]) if len(self.arrays) > 1 \
           else self.arrays[0].copy()
+    if weights is None:
+      raise ValueError("pull_model on a GPU needs the bf16 weights buffer")
+    total = int(total if total is not None else weights.numel())
+    decay_end = int(decay_end if decay_end is not None else total)
+    _check_pull_model(self.numel, total, decay_end, weights, aux32, running)
     import torch
     from .. import ops
-    total = int(total if total is not None else weights.numel())
     if running is not None and (self._running_pulled is None
                                 or self._running_pulled.numel() != running.numel()):
       self._running_pulled = torch.zeros_like(running)
@@ -387,19 +447,21 @@ class PSClient(object):
           "weights": weights.data_ptr(), "aux32": aux32.data_ptr() if aux32 is not None else 0,
           "running": running.data_ptr() if running is not None else 0,
           "running_pulled": self._running_pulled.data_ptr() if running is not None else 0,
-          "n": p["hi"] - p["lo"], "lo": p["lo"], "total": total,
-          "decay_end": int(decay_end if decay_end is not None else total), "grid": 64})
+          "n": p["hi"] - p["lo"], "lo": p["lo"], "total": total, "decay_end": decay_end,
+          "grid": 64})
 
   def push_grads(self, grads, running=None, total=None):
     """Slot mode: hand this step's gradients (flat fp32, length ``total``) to the servers.  The
     non-trainable tail, if any, is sent as (pulled - current) running statistics."""
+    if self.cuda:
+      total = int(total if total is not None else grads.numel())
+      _check_push_grads(self.numel, total, grads, running, self._running_pulled)
     self.pushes += 1
     seq, slot = self.pushes, self.pushes % NSLOTS
     need = max(0, seq - NSLOTS)        # what must have been applied before the slot is reused
     k = self.client_id * NSLOTS + slot
     if self.cuda:
       from .. import ops
-      total = int(total if total is not None else grads.numel())
       for p, ptr, lay in zip(self.parts, self.ptrs, self.layouts):
         n = p["hi"] - p["lo"]
         ops.K.ps_push_slot({
@@ -472,7 +534,7 @@ class PSClient(object):
       idx = indices.to(torch.int32)
       for p, ptr in zip(self.parts, self.ptrs):
         lo, hi = p["lo"], p["hi"]
-        r0, r1 = max(0, (lo - base + width - 1) // width), max(0, (hi - base) // width)
+        r0, r1, cuts = _sparse_plan(lo, hi, base, width)
         sel = (idx >= r0) & (idx < r1)
         if r1 > r0 and bool(sel.any()):
           rows = grad_rows[sel].contiguous()
@@ -480,12 +542,8 @@ class PSClient(object):
           off = base + r0 * width - lo
           ops.K.ps_push_sparse(ptr + 4 * off, rows, local, self.hyper)
         # rows cut by this server's boundaries: the owned element range goes through the dense kernel
-        for edge in (lo, hi):
-          r = (edge - base) // width
+        for r, a, b in cuts:
           s0 = base + r * width
-          if edge <= base or s0 == edge or s0 + width <= lo or s0 >= hi:
-            continue
-          a, b = max(s0, lo), min(s0 + width, hi)
           for k in torch.nonzero(idx == r).flatten().tolist():
             seg = grad_rows[k].reshape(-1)[a - s0:b - s0].to(torch.float32).contiguous()
             ops.K.ps_push_dense(ptr + 4 * (a - lo), seg, self.hyper)

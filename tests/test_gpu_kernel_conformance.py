@@ -73,6 +73,18 @@ COVERED_ELSEWHERE = {
     "grad_sumsq": "test_gpu_grad_clip.py::test_clipped_steps_match_float64",
     "clip_finalize": "test_gpu_grad_clip.py::test_clipped_steps_match_float64",
     "lars_norms": "test_gpu_lars.py::test_lars_steps_match_float64_reference",
+    "igemm_run": "test_gpu_plan_conformance.py::test_gemm_plans_match_float64",
+    "sigmoid_bce": "test_gpu_multilabel.py::test_sigmoid_bce_against_float64",
+    "multilabel_eval_metrics":
+        "test_gpu_multilabel.py::test_multilabel_eval_metrics_against_reference",
+    "seg_loss_grad": "test_gpu_seg_losses.py::test_focal_against_float64",
+    "seg_dice_stats": "test_gpu_seg_losses.py::test_dice_against_float64",
+    "ps_push_dense": "test_gpu_ps_kernels.py::test_push_dense_is_bit_exact",
+    "ps_push_sparse": "test_gpu_ps_kernels.py::test_push_sparse_against_float64",
+    "ps_pull": "test_gpu_ps_kernels.py::test_pull_copies_bitwise",
+    "ps_apply": "test_gpu_ps_kernels.py::test_apply_against_float64",
+    "ps_push_slot": "test_gpu_ps_kernels.py::test_push_slot_is_bitwise",
+    "ps_pull_model": "test_gpu_ps_kernels.py::test_pull_model_is_bitwise",
 }
 
 

@@ -1221,6 +1221,9 @@ def ps_net_gpu():
         grads = torch.randn(total, device="cuda")
         running += 0.1 * torch.randn(R, device="cuda")
         c.push_grads(grads, running, total=total)
+        # push_grads returns before the servers apply it, and the next client pulls over its own
+        # connection: wait for the acknowledgement, so the applies happen in the reference's order
+        c.applies()
         gg = grads.double() * 0.5
         gg[:decay_end] += 1e-2 * w[:decay_end]
         if opt == "momentum":
