@@ -57,28 +57,46 @@ UNWRITTEN_U8 = 0xEE   # no tap of a k <= 15 window
 
 KERNEL_OPS = ("stem_bn_relu_pool_fwd", "stem_pool_bn_bwd", "maxpool_fwd", "maxpool_bwd",
               "avgpool_fwd", "avgpool_bwd", "decode_normalize", "copy_channels", "relu_bwd",
-              "conv3x3_c1_fwd", "conv3x3_c1_wgrad", "bn_finalize")
-# entry points checked against float64 elsewhere: entry -> the test that does it
+              "conv3x3_c1_fwd", "conv3x3_c1_wgrad", "bn_finalize", "bn_fold")
+# entry points checked against float64 elsewhere: entry -> the test that does it.  A key
+# "entry[kw1,kw2]" names the launches that switch on exactly those optional arguments
+# (tests/test_gpu_option_conformance.py's variant()), "entry[*]" every variant; a bare "entry"
+# covers the launch with no option switched on.
 COVERED_ELSEWHERE = {
     "softmax_xent": "test_gpu_resnet_head.py::test_softmax_xent_against_float64",
+    "softmax_xent[label_smoothing]": "test_gpu_resnet_head.py::test_softmax_xent_against_float64",
     "pixel_xent": "test_gpu_unet_loss_options.py::test_optioned_pixel_xent_against_float64",
+    "pixel_xent[ignore_index,norm,weights]":
+        "test_gpu_unet_loss_options.py::test_optioned_pixel_xent_against_float64",
+    "pixel_xent[ignore_index,norm]":
+        "test_gpu_unet_loss_options.py::test_optioned_pixel_xent_against_float64",
+    "pixel_xent[norm,weights]":
+        "test_gpu_unet_loss_options.py::test_optioned_pixel_xent_against_float64",
     "seg_label_norm":
         "test_gpu_unet_loss_options.py::test_label_prepass_is_exact_and_bitwise_reproducible",
+    "seg_label_norm[*]":
+        "test_gpu_unet_loss_options.py::test_label_prepass_is_exact_and_bitwise_reproducible",
     "seg_eval_metrics": "test_gpu_seg_eval.py::test_seg_eval_metrics_against_float64",
+    "seg_eval_metrics[*]":
+        "test_gpu_unet_loss_options.py::test_optioned_seg_eval_metrics_against_numpy",
     "seg_predict": "test_gpu_serve_unet.py::test_seg_predict_against_host_reference",
     "depthwise3x3_bwd": "test_gpu_unet_finetune.py::test_depthwise_bwd_against_float64",
     "eval_metrics": "test_gpu_eval.py::test_eval_metrics_against_float64",
-    "bn_fold": "test_gpu_eval.py::test_resnet50_eval_logits_and_totals",
     "allreduce_opt": "test_gpu_grad_clip.py::test_clipped_steps_match_float64",
     "grad_sumsq": "test_gpu_grad_clip.py::test_clipped_steps_match_float64",
     "clip_finalize": "test_gpu_grad_clip.py::test_clipped_steps_match_float64",
     "lars_norms": "test_gpu_lars.py::test_lars_steps_match_float64_reference",
     "igemm_run": "test_gpu_plan_conformance.py::test_gemm_plans_match_float64",
     "sigmoid_bce": "test_gpu_multilabel.py::test_sigmoid_bce_against_float64",
+    "sigmoid_bce[*]": "test_gpu_multilabel.py::test_sigmoid_bce_against_float64",
     "multilabel_eval_metrics":
         "test_gpu_multilabel.py::test_multilabel_eval_metrics_against_reference",
     "seg_loss_grad": "test_gpu_seg_losses.py::test_focal_against_float64",
+    "seg_loss_grad[*]": "test_gpu_seg_losses.py::test_focal_against_float64",
+    "seg_loss_grad[cross_entropy,dice_coef]": "test_gpu_seg_losses.py::test_dice_against_float64",
+    "seg_loss_grad[dice_coef]": "test_gpu_seg_losses.py::test_dice_against_float64",
     "seg_dice_stats": "test_gpu_seg_losses.py::test_dice_against_float64",
+    "seg_dice_stats[*]": "test_gpu_seg_losses.py::test_dice_against_float64",
     "ps_push_dense": "test_gpu_ps_kernels.py::test_push_dense_is_bit_exact",
     "ps_push_sparse": "test_gpu_ps_kernels.py::test_push_sparse_against_float64",
     "ps_pull": "test_gpu_ps_kernels.py::test_pull_copies_bitwise",
@@ -94,73 +112,38 @@ def _mod():
 
 
 # ----------------------------------------------------------------------------- recording
-def _record_models(calls, names):
-  import torch
-  from tensorflowonspark_b200 import ops
-  from tensorflowonspark_b200.models import mnist, resnet, unet
-  mod = _mod()
-  with pytest.MonkeyPatch.context() as mp:
-    for name in dir(mod):
-      fn = getattr(mod, name)
-      if name.startswith("_") or isinstance(fn, type) or not callable(fn):
-        continue
+def _resnet50_train_and_evaluate():
+  from tensorflowonspark_b200.models import resnet
+  net = resnet.ResNetTrainer(50, batch=256, image=224)
+  net.train_step(*net.synthetic_batch())
+  net.evaluate([net.synthetic_batch(seed=1)])
 
-      def wrap(*a, _fn=fn, _name=name, **k):
-        names.add(_name)
-        if _name in KERNEL_OPS:
-          alias = tuple((j, i) for i in range(1, len(a)) for j in range(i)
-                        if isinstance(a[i], torch.Tensor) and isinstance(a[j], torch.Tensor)
-                        and a[i].data_ptr() == a[j].data_ptr())
-          calls.append((_name, _plans._spec_of(tuple(a)), alias))
-        return _fn(*a, **k)
-      mp.setattr(ops.K, name, wrap, raising=False)
 
-    def free():   # after the last reference to a trainer is gone
-      torch.cuda.synchronize()
-      gc.collect()
-      torch.cuda.empty_cache()
+def _cifar_and_evaluate():
+  from tensorflowonspark_b200.models import resnet
+  net = resnet.CifarResNetTrainer(20, batch=128)
+  net.step_kernels()
+  net.evaluate([net.synthetic_batch(seed=1)])
 
-    net = resnet.ResNetTrainer(50, batch=256, image=224)
-    net.train_step(*net.synthetic_batch())
-    net.evaluate([net.synthetic_batch(seed=1)])
-    del net
-    free()
-    net = resnet.ResNetTrainer(50, batch=256, image=224, training=False)
-    net.forward_only()
-    net.build_folded_inference()
-    net.forward_folded()
-    del net
-    free()
-    net = resnet.ResNetTrainer(50, batch=8, image=64)
-    net.train_step(*net.synthetic_batch())
-    del net
-    free()
-    net = resnet.CifarResNetTrainer(20, batch=128)
-    net.step_kernels()
-    net.evaluate([net.synthetic_batch(seed=1)])
-    del net
-    free()
-    net = unet.UNetTrainer(batch=64, image=128, training=True)
-    net.train_step(*net.synthetic_batch())
-    del net
-    free()
-    net = unet.UNetTrainer(batch=64, image=128, training=False)
-    net.predict(net.synthetic_batch()[0])
-    del net
-    free()
-    net = mnist.MnistTrainer(batch=64)
-    net.train_step()
-    del net
-    free()
+
+MODELS = (_resnet50_train_and_evaluate, _plans._resnet50_serving, _plans._resnet50_small,
+          _cifar_and_evaluate, _plans._unet_train, _plans._unet_predict, _plans._mnist)
+
+
+def signatures(rec):
+  """The distinct (op, positional spec, keyword spec, aliases) of the entry points this file
+  replays, and the names of every entry point launched, from a plan suite recorder."""
+  calls = pc.dedup((op, spec, kw, alias) for op, spec, kw, _, alias in rec.k if op in KERNEL_OPS)
+  return {"calls": calls, "names": {c[0] for c in rec.k}}
 
 
 @pytest.fixture(scope="module")
 def recorded():
   import torch
   torch.cuda.set_device(0)
-  calls, names = [], set()
-  _record_models(calls, names)
-  return {"calls": pc.dedup(calls), "names": names}
+  rec = _plans._Recorder()
+  _plans._record_models(rec, MODELS)
+  return signatures(rec)
 
 
 # ----------------------------------------------------------------------------- tensors
@@ -365,7 +348,10 @@ def check_stem_fwd(N, H, W, C, what, eps=1e-3, mom=0.01, compare_unfused=True):
   return int(amb.sum())
 
 
-def check_stem_bwd(N, H, W, C, what, runs=2):
+def check_stem_bwd(N, H, W, C, what, runs=2, accumulate=False):
+  """``accumulate``: the trainer's accumulating launch - dgamma / dbeta reduce into zeroed scratch
+  (checked as the writing variant's outputs) and the scratch is added to the parameter gradient,
+  prefilled with A: it must end as fl(A + scratch) bit for bit."""
   import torch
   gen = _Gen(what)
   OH, OW = kc.pool_out(H, 3, 2, 1), kc.pool_out(W, 3, 2, 1)
@@ -404,9 +390,17 @@ def check_stem_bwd(N, H, W, C, what, runs=2):
     dgam, dgb = _guarded_copy(torch.zeros(C, device=DEV))
     dbet, dbb = _guarded_copy(torch.zeros(C, device=DEV))
     dx, dxb = _out((N, H, W, C), torch.bfloat16)
-    _mod().stem_pool_bn_bwd(dy, idx, x, gam, mean, invstd, fs, fh, dgam, dbet, dx)
+    kw, accs, prefill = {}, [], []
+    if accumulate:
+      prefill = [gen.randn((C,), 1.0, 0.0, torch.float32) for _ in range(2)]
+      accs = [_guarded_copy(t) for t in prefill]
+      kw = {"acc_dgamma": accs[0][0], "acc_dbeta": accs[1][0]}
+    _mod().stem_pool_bn_bwd(dy, idx, x, gam, mean, invstd, fs, fh, dgam, dbet, dx, **kw)
     _sync()
     w = "{} run{}".format(what, r)
+    for (t, bk), a0, v, name in zip(accs, prefill, (dgam, dbet), ("acc_dgamma", "acc_dbeta")):
+      kc.check_accumulated(t, a0, v, w + " " + name)
+      assert pc.guard_intact(t, bk), w + ": " + name + " guard band"
     pc.check_close(dgam, dg_ref, dg_bnd, w + " dgamma")
     pc.check_close(dbet, db_ref, db_bnd, w + " dbeta")
     dg, db = _f64(dgam), _f64(dbet)
@@ -561,15 +555,43 @@ def check_bn_finalize(C, rows, what, eps=1e-3, mom=0.01):
   assert all(pc.guard_intact(v, b) for v, b in outs + [(sv, sb), (qv, qb)]), what + ": guard band"
 
 
+def check_bn_fold(tab, row0, rows, wshape, aux_n, run_n, what):
+  """bn_fold over a recorded table (tab, row0: the trainer's values) on fresh seeded filters,
+  gamma / beta and running statistics, with variances from 1e-6 to 1e3 (log-uniform) so that eps
+  matters for some channels and is negligible for others, and guarded outputs prefilled with
+  random values: the elements no unit covers must keep them (kc.check_bn_fold)."""
+  import torch
+  gen = _Gen(what)
+  tab_t = torch.tensor(tab, dtype=torch.int64).reshape(-1, kc.FOLD_COLS)
+  row0_t = torch.tensor(row0, dtype=torch.int64)
+  eps = torch.full((tab_t.shape[0],), 1e-5, dtype=torch.float32)
+  w = gen.randn(wshape, 0.05)
+  aux32 = gen.randn((aux_n,), 1.0, 0.0, torch.float32)
+  running = gen.randn((run_n,), 0.5, 0.0, torch.float32)
+  for wo, cout, per, go, bo, mo, vo, fo in tab_t.tolist():
+    running[vo:vo + cout] = torch.pow(10.0, torch.rand(cout, generator=gen.g, device=DEV) * 9 - 6)
+  nb = max(r[7] + (r[1] + 7) // 8 * 8 for r in tab_t.tolist())
+  wf, wfb = _guarded_copy(gen.randn(wshape))
+  bias, bb = _guarded_copy(gen.randn((nb,), 1.0, 0.0, torch.float32))
+  wf0, bias0 = wf.clone(), bias.clone()
+  _mod().bn_fold(tab_t.to(DEV), eps.to(DEV), row0_t.to(DEV), rows, w, aux32, running, wf, bias)
+  _sync()
+  kc.check_bn_fold(wf, bias, wf0, bias0, tab_t, eps, row0_t, w, aux32, running, what)
+  assert pc.guard_intact(wf, wfb) and pc.guard_intact(bias, bb), what + ": guard band"
+
+
 # -------------------------------------------------------------------- recorded signatures
 def _shape(s):
   assert isinstance(s, tuple) and s and s[0] == "T", s
   return tuple(s[1])
 
 
-def replay(op, spec, alias, what):
-  """Run the checker of a recorded call with the recorded shapes and scalar arguments."""
+def replay(op, spec, kwspec, alias, what):
+  """Run the checker of a recorded call with the recorded shapes, scalar and keyword arguments."""
   a = list(spec)
+  kw = dict(kwspec)
+  if kw and not (op == "stem_pool_bn_bwd" and sorted(kw) == ["acc_dbeta", "acc_dgamma"]):
+    raise AssertionError("{}: no float64 replay for keywords {}".format(what, sorted(kw)))
   if op == "maxpool_fwd":
     N, H, W, C = _shape(a[0])
     k, s, p = a[3:6]
@@ -580,7 +602,7 @@ def replay(op, spec, alias, what):
   elif op == "stem_bn_relu_pool_fwd":
     check_stem_fwd(*_shape(a[0]), what, eps=a[14], mom=a[15])
   elif op == "stem_pool_bn_bwd":
-    check_stem_bwd(*_shape(a[2]), what, runs=1)
+    check_stem_bwd(*_shape(a[2]), what, runs=1, accumulate=bool(kw))
   elif op == "avgpool_fwd":
     check_avgpool_fwd(_shape(a[0]), what)
   elif op == "avgpool_bwd":
@@ -598,6 +620,8 @@ def replay(op, spec, alias, what):
   elif op == "bn_finalize":
     C = _shape(a[0])[0]
     check_bn_finalize(C, 4096, what, eps=a[11], mom=a[12])
+  elif op == "bn_fold":
+    check_bn_fold(a[0][3], a[2][3], a[3], _shape(a[4]), _shape(a[5])[0], _shape(a[6])[0], what)
   else:
     raise AssertionError(op)
 
@@ -605,10 +629,10 @@ def replay(op, spec, alias, what):
 def test_recorded_launches_match_float64(recorded):
   import torch
   failures = []
-  for i, (op, spec, alias) in enumerate(recorded["calls"]):
+  for i, (op, spec, kw, alias) in enumerate(recorded["calls"]):
     what = "{}#{}".format(op, i)
     try:
-      replay(op, spec, alias, what)
+      replay(op, spec, kw, alias, what)
     except AssertionError as e:
       failures.append(str(e))
     gc.collect()
@@ -616,13 +640,13 @@ def test_recorded_launches_match_float64(recorded):
   print("replayed {} recorded pooling / stem / decode / MNIST signatures".format(
       len(recorded["calls"])))
   assert not failures, "\n".join(failures[:20])
-  seen = {op for op, _, _ in recorded["calls"]}
+  seen = {c[0] for c in recorded["calls"]}
   assert seen == set(KERNEL_OPS), "entry points never recorded: {}".format(set(KERNEL_OPS) - seen)
 
 
 def test_every_launched_entry_point_has_a_float64_check(recorded):
   """A new ops.K launch in any model must be added to one of the float64 suites."""
-  covered = set(KERNEL_OPS) | set(_plans.K_OPS) | set(COVERED_ELSEWHERE)
+  covered = set(KERNEL_OPS) | set(_plans.K_OPS) | {k.split("[")[0] for k in COVERED_ELSEWHERE}
   missing = sorted(recorded["names"] - covered)
   assert not missing, "ops.K entry points without a float64 check: {}".format(missing)
   for op, test in COVERED_ELSEWHERE.items():

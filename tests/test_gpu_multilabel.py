@@ -16,6 +16,19 @@ from test_gpu_eval import _rel_l2  # noqa: E402
 from test_gpu_resnet_head import _head_padding_is_zero  # noqa: E402
 from test_multilabel_host import ref_bce, ref_exact_rows, ref_multilabel_acc  # noqa: E402
 
+
+def _load_pc():
+  import importlib.util
+  spec = importlib.util.spec_from_file_location(
+      "plan_conformance", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
+                                       "tools", "plan_conformance.py"))
+  m = importlib.util.module_from_spec(spec)
+  spec.loader.exec_module(m)
+  return m
+
+
+pc = _load_pc()
+
 pytestmark = pytest.mark.gpu
 
 KEYS = {"count", "loss", "binary_accuracy", "exact_match", "precision", "recall", "f1",
@@ -103,7 +116,11 @@ def test_sigmoid_bce_replays_bitwise_under_a_cuda_graph():
       if rows == 1:    # one atomic add onto 0: bitwise too
         assert torch.equal(loss, eager[1])
       else:
-        assert abs(float(loss) - float(eager[1])) <= 1e-6 * abs(float(eager[1]))
+        # the same rows' losses (each >= 0, so their sum bounds the magnitudes) added with one
+        # float atomic per row in any order: each total is within gamma_prob(rows - 1) of the
+        # exact sum, so two totals within twice that
+        bound = 2 * pc.gamma_prob(rows - 1) * abs(float(eager[1])) * (1 + 2.0 ** -20)
+        assert abs(float(loss) - float(eager[1])) <= bound, (float(loss), float(eager[1]), bound)
 
 
 # --------------------------------------------------------------------------- evaluation kernel

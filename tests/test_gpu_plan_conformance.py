@@ -34,6 +34,11 @@ _spec = importlib.util.spec_from_file_location(
                                      "tools", "plan_conformance.py"))
 pc = importlib.util.module_from_spec(_spec)
 _spec.loader.exec_module(pc)
+_spec = importlib.util.spec_from_file_location(
+    "kernel_conformance", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
+                                       "tools", "kernel_conformance.py"))
+kc = importlib.util.module_from_spec(_spec)
+_spec.loader.exec_module(kc)
 
 GEMM_BUILDERS = ("gemm", "gemm_wgrad", "conv_fprop", "conv_dgrad", "conv_wgrad", "stem_fprop",
                  "stem_wgrad")
@@ -45,11 +50,17 @@ K_OPS = ("bn_apply", "bn_apply_finalize", "bn_bwd_reduce", "bn_bwd_apply", "dept
 
 
 def _spec_of(v):
+  """The signature of one argument: a tensor's shape and dtype (and the values of an int64 index
+  table: they decide what a launch does), scalars as they are."""
   import torch
   if isinstance(v, torch.Tensor):
+    if v.dtype == torch.int64 and v.numel() <= 4096:
+      return ("T", tuple(v.shape), "int64", tuple(v.reshape(-1).tolist()))
     return ("T", tuple(v.shape), str(v.dtype).replace("torch.", ""))
   if isinstance(v, (tuple, list)):
     return tuple(_spec_of(x) for x in v)
+  if isinstance(v, dict):
+    return tuple(sorted((k, _spec_of(x)) for k, x in v.items()))
   if isinstance(v, float):
     return round(v, 6)
   return v
@@ -59,16 +70,82 @@ class _Recorder(object):
 
   def __init__(self):
     self.gemm = []    # [op, frozen args, infos (list of dicts, mutable for set_reverse)]
-    self.k = []       # (op, frozen args, row reverse, aliases)
+    # every ops.K launch: (op, positional spec, sorted keyword spec, row reverse, aliases); the
+    # aliases index the positional arguments followed by the keyword arguments in sorted order
+    self.k = []
     self.row_reverse = False
     self._depth = 0
 
 
-def _record_models(rec):
+def _free():
+  """After the last reference to a trainer is gone."""
+  import torch
+  torch.cuda.synchronize()
+  gc.collect()
+  torch.cuda.empty_cache()
+
+
+def _resnet50_train():
+  from tensorflowonspark_b200.models import resnet
+  net = resnet.ResNetTrainer(50, batch=256, image=224)
+  net.train_step(*net.synthetic_batch())
+
+
+def _resnet50_serving():
+  # batch norms folded into the filters, residual accumulate + ReLU epilogues
+  from tensorflowonspark_b200.models import resnet
+  net = resnet.ResNetTrainer(50, batch=256, image=224, training=False)
+  net.forward_only()
+  net.build_folded_inference()
+  net.forward_folded()
+
+
+def _resnet50_small():
+  from tensorflowonspark_b200.models import resnet
+  net = resnet.ResNetTrainer(50, batch=8, image=64)
+  net.train_step(*net.synthetic_batch())
+
+
+def _cifar():
+  from tensorflowonspark_b200.models import resnet
+  resnet.CifarResNetTrainer(20, batch=128).step_kernels()
+
+
+def _unet_train():
+  from tensorflowonspark_b200.models import unet
+  net = unet.UNetTrainer(batch=64, image=128, training=True)
+  net.train_step(*net.synthetic_batch())
+
+
+def _unet_predict():
+  from tensorflowonspark_b200.models import unet
+  net = unet.UNetTrainer(batch=64, image=128, training=False)
+  net.predict(net.synthetic_batch()[0])
+
+
+def _mnist():
+  from tensorflowonspark_b200.models import mnist
+  mnist.MnistTrainer(batch=64).train_step()
+
+
+DEFAULT_MODELS = (_resnet50_train, _resnet50_serving, _resnet50_small, _cifar, _unet_train,
+                  _unet_predict, _mnist)
+
+
+def _alias_pairs(vals):
+  import torch
+  return tuple((j, i) for i in range(1, len(vals)) for j in range(i)
+               if isinstance(vals[i], torch.Tensor) and isinstance(vals[j], torch.Tensor)
+               and vals[i].data_ptr() == vals[j].data_ptr() and vals[i].dtype == vals[j].dtype)
+
+
+def _record_models(rec, models=DEFAULT_MODELS):
+  """Run each callable of ``models`` (it builds a trainer, runs it and drops it) while the igemm
+  builders, ``Plan.set_reverse``, ``bn_set_row_reverse`` and every ``ops.K`` entry point are
+  wrapped, freeing the GPU memory after each."""
   import torch
   from tensorflowonspark_b200 import _build, ops
   from tensorflowonspark_b200.ops import igemm
-  from tensorflowonspark_b200.models import mnist, resnet, unet
   mod = _build.load(required=True)
   with pytest.MonkeyPatch.context() as mp:
     for name in GEMM_BUILDERS:
@@ -106,57 +183,21 @@ def _record_models(rec):
       rec.row_reverse = bool(flag)
       orig_rowrev(flag)
     mp.setattr(mod, "bn_set_row_reverse", row_rev)
-    for name in K_OPS:
+    for name in dir(mod):
       fn = getattr(mod, name)
+      if name.startswith("_") or isinstance(fn, type) or not callable(fn):
+        continue
 
-      def wrapk(*a, _fn=fn, _name=name):
-        alias_pairs = tuple((j, i) for i in range(1, len(a)) for j in range(i)
-                            if isinstance(a[i], torch.Tensor) and isinstance(a[j], torch.Tensor)
-                            and a[i].data_ptr() == a[j].data_ptr()
-                            and a[i].dtype == a[j].dtype)
-        rec.k.append((_name, _spec_of(tuple(a)), rec.row_reverse, alias_pairs))
-        return _fn(*a)
-      mp.setattr(ops.K, name, wrapk)
-
-    def free():   # after the last reference to a trainer is gone
-      torch.cuda.synchronize()
-      gc.collect()
-      torch.cuda.empty_cache()
-
-    net = resnet.ResNetTrainer(50, batch=256, image=224)
-    net.train_step(*net.synthetic_batch())
-    del net
-    free()
-    # the serving path: batch norms folded into the filters, residual accumulate + ReLU epilogues
-    net = resnet.ResNetTrainer(50, batch=256, image=224, training=False)
-    net.forward_only()
-    net.build_folded_inference()
-    net.forward_folded()
-    del net
-    free()
-    net = resnet.ResNetTrainer(50, batch=8, image=64)
-    net.train_step(*net.synthetic_batch())
-    del net
-    free()
-    net = resnet.CifarResNetTrainer(20, batch=128)
-    net.step_kernels()
-    del net
-    free()
-    net = unet.UNetTrainer(batch=64, image=128, training=True)
-    net.train_step(*net.synthetic_batch())
-    del net
-    free()
-    net = unet.UNetTrainer(batch=64, image=128, training=False)
-    net.predict(net.synthetic_batch()[0])
-    del net
-    free()
-    net = mnist.MnistTrainer(batch=64)
-    net.train_step()
-    del net
-    free()
-  gc.collect()
-  torch.cuda.synchronize()
-  torch.cuda.empty_cache()
+      def wrapk(*a, _fn=fn, _name=name, **k):
+        kw = sorted(k.items())
+        rec.k.append((_name, _spec_of(tuple(a)), _spec_of(tuple(kw)), rec.row_reverse,
+                      _alias_pairs(list(a) + [v for _, v in kw])))
+        return _fn(*a, **k)
+      mp.setattr(ops.K, name, wrapk, raising=False)
+    for model in models:
+      model()
+      _free()
+  _free()
 
 
 @pytest.fixture(scope="module")
@@ -166,12 +207,15 @@ def recorded():
   torch.cuda.reset_peak_memory_stats()
   rec = _Recorder()
   _record_models(rec)
+  return {"gemm": distinct_plans(rec), "k": pc.dedup(c for c in rec.k if c[0] in K_OPS)}
+
+
+def distinct_plans(rec):
+  """The recorded igemm plans without repeats: (op, args, infos)."""
   gemm = {}
   for op, args, infos in rec.gemm:
-    key = (op, args, pc.freeze(infos))
-    gemm.setdefault(key, (op, args, infos))
-  kops = pc.dedup(rec.k)
-  return {"gemm": list(gemm.values()), "k": kops}
+    gemm.setdefault((op, args, pc.freeze(infos)), (op, args, infos))
+  return list(gemm.values())
 
 
 # ----------------------------------------------------------------------------- synthetic cases
@@ -758,7 +802,7 @@ def test_dispatch_coverage(recorded):
 
 # --------------------------------------------------------------- batch norm and elementwise ops
 def _bn_tensors(spec, gen, alias):
-  """Fresh tensors for a recorded ops.K call (positional specs)."""
+  """Fresh tensors for a recorded ops.K call (positional specs, then keyword specs)."""
   import torch
   out = []
   for i, s in enumerate(spec):
@@ -790,13 +834,13 @@ def _guard_out(t, unwritten=True):
   return v, b
 
 
-def _run_k(op, a, rev):
+def _run_k(op, a, rev, kw=None):
   import torch
   from tensorflowonspark_b200 import _build
   C = _build.load(required=True)
   C.bn_set_row_reverse(rev)
   try:
-    getattr(C, op)(*a)
+    getattr(C, op)(*a, **(kw or {}))
   finally:
     C.bn_set_row_reverse(False)
   torch.cuda.synchronize()
@@ -813,10 +857,15 @@ def _bits_of(mask, P, Cn):
   return ((mask.reshape(-1)[e >> 3].to(torch.int64) >> (e & 7)) & 1).reshape(P, Cn).bool()
 
 
-def _check_k(op, spec, rev, alias, what):
+def _check_k(op, spec, kwspec, rev, alias, what):
+  """Replay one recorded ops.K call.  Keyword arguments: only the accumulating bn_bwd_apply
+  (acc_dgamma / acc_dbeta) is checked here; any other keyword fails the replay."""
   import torch
   gen = _Gen(zlib.crc32(what.encode()))
-  a = _bn_tensors(spec, gen, alias)
+  vals = _bn_tensors(tuple(spec) + tuple(v for _, v in kwspec), gen, alias)
+  a, kwv = vals[:len(spec)], dict(zip((n for n, _ in kwspec), vals[len(spec):]))
+  if kwv and not (op == "bn_bwd_apply" and sorted(kwv) == ["acc_dbeta", "acc_dgamma"]):
+    raise AssertionError("{}: no float64 replay for keywords {}".format(what, sorted(kwv)))
   u = pc.U_FP32
   if op in ("bn_apply", "bn_apply_finalize"):
     if op == "bn_apply":
@@ -941,6 +990,24 @@ def _check_k(op, spec, rev, alias, what):
       del namb
       assert pc.guard_intact(dgv, dgb) and pc.guard_intact(dbv, dbb), what + ": guard band"
       return
+    acc = None
+    if kwv:
+      # the accumulating variant: this micro-batch's (dgamma, dbeta) v go to dx and are added to
+      # the parameter gradient, prefilled with A.  Unfused, v is the scratch the apply reads; on
+      # the fused path only the writing variant publishes v, so it runs first on the same inputs
+      # (without dres, which may alias dy)
+      acc = [gen.randn((Cn,), torch.float32) for _ in range(2)]
+      accv = [_guard_out(t, False) for t in acc]
+      if sum_g is not None:
+        vg, vgb = _guard_out(dgam)
+        vb, vbb = _guard_out(dbet)
+        w = list(a)
+        w[6], w[7], w[8], w[9] = vg, vb, torch.empty_like(dx), None
+        _run_k(op, w, rev)
+        assert pc.guard_intact(vg, vgb) and pc.guard_intact(vb, vbb), what + ": v guard band"
+        dgam, dbet = vg, vb
+        a[6], a[7] = accv[0][0], accv[1][0]   # as the trainer passes them: not read
+      kwv = {"acc_dgamma": accv[0][0], "acc_dbeta": accv[1][0]}
     dxv, dxb = _guard_out(dx)
     a[8] = dxv
     dresv = None
@@ -951,7 +1018,7 @@ def _check_k(op, spec, rev, alias, what):
         dresv, dresb = _guard_out(dres)
         a[9] = dresv
     saved = [t.clone() if isinstance(t, torch.Tensor) else t for t in a]
-    _run_k(op, a, rev)
+    _run_k(op, a, rev, kwv)
     if sum_g is not None:
       db = _f64(sum_g)
       assert torch.equal(dbet, sum_g), what + ": dbeta differs from sum_g"
@@ -962,6 +1029,13 @@ def _check_k(op, spec, rev, alias, what):
       dg = _f64(dgam)
     else:
       dg, db = _f64(dgam), _f64(dbet)
+    if acc is not None:
+      if sum_g is None:
+        assert torch.equal(dgam, saved[6]) and torch.equal(dbet, saved[7]), \
+            what + ": the micro-batch's dgamma / dbeta changed"
+      for (t, bk), a0, v, name in zip(accv, acc, (dgam, dbet), ("acc_dgamma", "acc_dbeta")):
+        kc.check_accumulated(t, a0, v, what + " " + name)
+        assert pc.guard_intact(t, bk), what + ": " + name + " guard band"
     A = _f64(gam) * is64
     ref = A * (g - db / P - xm * is64 * dg / P)
     Mv = (A * g).abs() + (A * is64 * dg / P).abs() * (x64.abs() + _f64(mean).abs()) + \
@@ -982,7 +1056,15 @@ def _check_k(op, spec, rev, alias, what):
       if dresv is dy:
         b[0] = dy
         dy.copy_(saved[0])
-    _run_k(op, b, not rev)
+    if acc is not None:
+      for (t, _), a0 in zip(accv, acc):
+        t.copy_(a0)
+      if sum_g is not None:
+        b[6], b[7] = accv[0][0], accv[1][0]
+    _run_k(op, b, not rev, kwv)
+    if acc is not None:
+      for (t, _), a0, v in zip(accv, acc, (dgam, dbet)):
+        kc.check_accumulated(t, a0, v, what + ": row order")
     assert torch.equal(first[0].view(torch.int16), dxv.view(torch.int16)), \
         what + ": row order changes dx"
     if dresv is not None:
@@ -1063,11 +1145,11 @@ def test_bn_and_elementwise_launches_match_float64(recorded):
   import torch
   failures = []
   ops_seen = set()
-  for idx, (op, spec, rev, alias) in enumerate(recorded["k"]):
+  for idx, (op, spec, kw, rev, alias) in enumerate(recorded["k"]):
     ops_seen.add(op)
     what = "{}#{} rev{}".format(op, idx, int(rev))
     try:
-      _check_k(op, list(spec), rev, alias, what)
+      _check_k(op, spec, kw, rev, alias, what)
     except AssertionError as e:
       failures.append(str(e))
     torch.cuda.empty_cache()

@@ -1,7 +1,7 @@
 """The segmentation U-Net beyond eight classes (9..256): the wide-logit kernels pixel_xent,
 seg_eval_metrics and seg_predict (csrc/seg_wide.cuh) against float64, and a 21-class trainer end
-to end - its new GEMM plans, logits, last-layer gradients, learning, checkpoints, serving and
-fine-tuning."""
+to end - its logits, last-layer gradients, learning, checkpoints, serving and fine-tuning (its new
+GEMM plans are replayed against float64 by tests/test_gpu_option_conformance.py)."""
 import argparse
 import importlib.util
 import os
@@ -224,38 +224,6 @@ def test_wide_kernels_reject_mismatched_channels():
 def _labels_of(x, V):
   from tensorflowonspark_b200.models import unet
   return unet.synthetic_labels(x, V)
-
-
-def test_new_plans_match_float64():
-  """Every GEMM plan a 21- or 150-class trainer builds and a 3-class one does not, replayed
-  against float64 (the checks of tests/test_gpu_plan_conformance.py)."""
-  from tensorflowonspark_b200.models import unet
-  ft = _load("unet_finetune_plans", os.path.join("tests", "test_gpu_unet_finetune.py"))
-  conf = _load("plan_conformance_replay", os.path.join("tests", "test_gpu_plan_conformance.py"))
-  base = ft._record_plans(lambda: unet.UNetTrainer(batch=64, image=128, classes=3))
-  old = {(op, args) for op, args, _ in base}
-  new, keys = [], set()
-  for V in (21, 150):
-    for op, args, infos in ft._record_plans(lambda: unet.UNetTrainer(batch=64, image=128,
-                                                                      classes=V)):
-      if (op, args) not in old and (op, args) not in keys:
-        keys.add((op, args))
-        new.append((op, args, infos))
-  print("{} new plans: {}".format(len(new), sorted(op for op, _, _ in new)))
-  assert len(new) >= 6, "p_last, p_last_wgrad and p_last_dgrad at two class counts"
-  failures = []
-  for op, args, infos in new:
-    what = "{} {}".format(op, [v[1] for v in dict(args).values()
-                               if isinstance(v, tuple) and v and v[0] == "T"])
-    try:
-      if op in ("gemm_wgrad", "conv_wgrad"):
-        conf._replay_wgrad(op, args, infos, what)
-      else:
-        conf._replay_fwd(op, args, infos, what)
-    except AssertionError as e:
-      failures.append(str(e))
-    torch.cuda.empty_cache()
-  assert not failures, "\n".join(failures[:20])
 
 
 def test_21_class_logits_and_last_layer_gradients():

@@ -6,12 +6,12 @@
 * a trainer with ``encoder_trainable_from=0`` starts as exactly the frozen network of its seed;
 * every encoder parameter's gradient against fp32 PyTorch autograd (k = 0 and k = 13);
 * partial fine-tuning leaves the frozen units untouched; the stem's padding channels stay zero;
-* training on the example's synthetic trimap task; checkpoints, resume, serving and evaluation;
-* the implicit-GEMM plans only fine-tuning builds, replayed against float64
-  (tools/plan_conformance.py, through tests/test_gpu_plan_conformance.py's replay)."""
+* training on the example's synthetic trimap task; checkpoints, resume, serving and evaluation.
+
+The implicit-GEMM plans only fine-tuning builds are replayed against float64 by
+tests/test_gpu_option_conformance.py."""
 import gc
 import importlib.util
-import inspect
 import os
 
 import pytest
@@ -447,80 +447,3 @@ def test_checkpoints_resume_serving_and_evaluation():
   assert (mask == ref).all()
   res = tuned.evaluate([(x, _masks(x))])
   assert res["images"] == B and res["loss"] == res["loss"]
-
-
-# ----------------------------------------------------------------------------- new igemm plans
-_GEMM = ("gemm", "gemm_wgrad", "conv_fprop", "conv_dgrad", "conv_wgrad")
-
-
-def _record_plans(build):
-  from tensorflowonspark_b200.ops import igemm
-  seen = []
-  depth = [0]
-  with pytest.MonkeyPatch.context() as mp:
-    for name in _GEMM:
-      fn = getattr(igemm, name)
-      sig = inspect.signature(fn)
-
-      def wrap(*a, _fn=fn, _sig=sig, _name=name, **k):
-        depth[0] += 1
-        try:
-          plan = _fn(*a, **k)
-        finally:
-          depth[0] -= 1
-        if depth[0] == 0:
-          b = _sig.bind(*a, **k)
-          b.apply_defaults()
-          args = pc.freeze({n: _spec_of(v) for n, v in b.arguments.items()})
-          seen.append((_name, args, plan.info()))
-        return plan
-      mp.setattr(igemm, name, wrap)
-    net = build()
-    del net
-  gc.collect()
-  torch.cuda.synchronize()
-  torch.cuda.empty_cache()
-  return seen
-
-
-def _spec_of(v):
-  if isinstance(v, torch.Tensor):
-    return ("T", tuple(v.shape), str(v.dtype).replace("torch.", ""))
-  if isinstance(v, (tuple, list)):
-    return tuple(_spec_of(x) for x in v)
-  if isinstance(v, float):
-    return round(v, 6)
-  return v
-
-
-def test_fine_tuning_plans_match_float64():
-  from tensorflowonspark_b200.models import unet
-  conf = _load("plan_conformance_replay", os.path.join("tests", "test_gpu_plan_conformance.py"))
-  frozen = _record_plans(lambda: unet.UNetTrainer(batch=64, image=128))
-  tuned = _record_plans(lambda: unet.UNetTrainer(batch=64, image=128, encoder_trainable_from=0))
-  old = {(op, args) for op, args, _ in frozen}
-  new, keys = [], set()
-  for op, args, infos in tuned:
-    if (op, args) not in old and (op, args) not in keys:
-      keys.add((op, args))
-      new.append((op, args, infos))
-  print("{} new plans: {}".format(len(new), sorted({op for op, _, _ in new})))
-  # 1x1 data and weight gradients, the stem's 3x3/s2 weight gradient with 8 input channels and
-  # up-block 0's data gradient into block_16's output
-  assert any(op == "conv_wgrad" and dict(a)["dw"][1][1:3] == (1, 1) for op, a, _ in new)
-  assert any(op == "conv_dgrad" and dict(a)["w"][1][1:3] == (1, 1) for op, a, _ in new)
-  assert any(op == "conv_wgrad" and dict(a)["dw"][1] == (32, 3, 3, 8) for op, a, _ in new)
-  assert any(op == "conv_fprop" and dict(a)["y"][1][1:] == (4, 4, 320) for op, a, _ in new)
-  failures = []
-  for op, args, infos in new:
-    what = "{} {}".format(op, [v[1] for v in dict(args).values()
-                               if isinstance(v, tuple) and v and v[0] == "T"])
-    try:
-      if op in ("gemm_wgrad", "conv_wgrad"):
-        conf._replay_wgrad(op, args, infos, what)
-      else:
-        conf._replay_fwd(op, args, infos, what)
-    except AssertionError as e:
-      failures.append(str(e))
-    torch.cuda.empty_cache()
-  assert not failures, "\n".join(failures[:20])

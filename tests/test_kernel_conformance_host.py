@@ -157,3 +157,95 @@ def test_conv3x3_c1_refs_are_conv2d_and_autograd():
   assert torch.allclose(dw, wr.grad, rtol=1e-12, atol=1e-12)
   assert torch.allclose(db, br.grad, rtol=1e-12, atol=1e-12)
   assert bool((dwm >= dw.abs()).all() and (dbm >= db.abs()).all())
+
+
+# ------------------------------------------------------------------ gradient accumulation
+def test_accumulated_check_rejects_overwrite_and_double_add():
+  g = torch.Generator().manual_seed(3)
+  A, v = torch.randn(200, generator=g), torch.randn(200, generator=g)
+  kc.check_accumulated(A + v, A, v, "fl(A + v)")
+  for wrong, name in ((v.clone(), "overwrites"), (A + v + v, "adds twice"),
+                      ((A.double() + v.double()).float().nextafter(torch.tensor(float("inf"))),
+                       "one ulp off")):
+    with pytest.raises(AssertionError, match="not fl"):
+      kc.check_accumulated(wrong, A, v, name)
+
+
+# ------------------------------------------------------------------ batch-norm folding
+def _fold_problem(seed=0, eps=1e-3):
+  """Three folded units followed by a 10-row head the fold must not touch, as fold_table lays
+  them out: (tab, eps, row0, w, aux32, running).  The variances span 1e-6 .. 1e3, so eps matters
+  for some channels and var + eps is far above eps for others."""
+  g = torch.Generator().manual_seed(seed)
+  units = [(16, 8), (24, 16), (8, 72)]
+  rows, woff, aoff, roff, boff = [], 0, 0, 0, 0
+  for cout, per in units:
+    rows.append([woff, cout, per, aoff, aoff + cout, roff, roff + cout, boff])
+    woff += cout * per
+    aoff += 2 * cout
+    roff += 2 * cout
+    boff += (cout + 7) // 8 * 8
+  w = torch.randn(woff + 10 * 16, generator=g).to(torch.bfloat16)
+  aux32 = torch.randn(aoff, generator=g)
+  running = torch.randn(roff, generator=g)
+  for r in rows:   # variances: positive, log-uniform
+    running[r[6]:r[6] + r[1]] = torch.pow(10.0, torch.rand(r[1], generator=g) * 9 - 6)
+  tab = torch.tensor(rows, dtype=torch.int64)
+  row0 = torch.tensor([0, 16, 40, 48], dtype=torch.int64)
+  return tab, torch.full((3,), eps, dtype=torch.float32), row0, w, aux32, running
+
+
+def _fold_like_the_kernel(tab, eps, row0, w, aux32, running, drop_eps=False, mean_as_var=False,
+                          extra_row=False):
+  """fp32 s = gamma * rsqrt(var + eps), bf16(fp32(w s)), fp32 beta - mean s; and the faults."""
+  wf = torch.randn(w.shape, generator=torch.Generator().manual_seed(9)).to(torch.bfloat16)
+  nb = 48
+  bias = torch.randn(nb + 8, generator=torch.Generator().manual_seed(10))
+  wf0, bias0 = wf.clone(), bias.clone()
+  for u, (wo, cout, per, go, bo, mo, vo, fo) in enumerate(tab.tolist()):
+    var = running[mo:mo + cout] if mean_as_var else running[vo:vo + cout]
+    s = aux32[go:go + cout] * torch.rsqrt(var if drop_eps else var + eps[u])
+    wf[wo:wo + cout * per] = (w[wo:wo + cout * per].float().view(cout, per) * s[:, None]) \
+        .to(torch.bfloat16).view(-1)
+    bias[fo:fo + cout] = aux32[bo:bo + cout] - running[mo:mo + cout] * s
+    if extra_row and u == len(tab) - 1:   # one row past the unit: the head's first row
+      e = wo + cout * per
+      wf[e:e + per] = (w[e:e + per].float() * s[-1]).to(torch.bfloat16)
+  return wf, bias, wf0, bias0
+
+
+def test_fold_ref_is_eval_batch_norm_after_the_layer():
+  tab, eps, row0, w, aux32, running = _fold_problem()
+  s, wf, bias, wmask, bmask = kc.fold_ref(tab, eps, row0, w, aux32, running)
+  x = torch.randn(5, 72, generator=torch.Generator().manual_seed(1), dtype=torch.float64)
+  for (wo, cout, per, go, bo, mo, vo, fo), e in zip(tab.tolist(), eps.tolist()):
+    W = w[wo:wo + cout * per].double().view(cout, per)
+    ref = F.batch_norm(x[:, :per] @ W.t(), running[mo:mo + cout].double(),
+                       running[vo:vo + cout].double(), aux32[go:go + cout].double(),
+                       aux32[bo:bo + cout].double(), False, 0.0, e)
+    got = x[:, :per] @ wf[wo:wo + cout * per].view(cout, per).t() + bias[fo:fo + cout]
+    torch.testing.assert_close(got, ref, rtol=1e-12, atol=1e-12)
+  assert int(wmask.sum()) == 16 * 8 + 24 * 16 + 8 * 72 and not bool(wmask[-160:].any())
+  assert int(bmask.sum()) == 48
+
+
+def test_check_bn_fold_accepts_the_kernels_rounding():
+  for seed in range(3):
+    p = _fold_problem(seed)
+    kc.check_bn_fold(*_fold_like_the_kernel(*p), *p, "fold")
+
+
+@pytest.mark.parametrize("fault", ["drop_eps", "mean_as_var", "extra_row"])
+def test_check_bn_fold_rejects_a_wrong_fold(fault):
+  p = _fold_problem(1)
+  with pytest.raises(AssertionError):
+    kc.check_bn_fold(*_fold_like_the_kernel(*p, **{fault: True}), *p, fault)
+
+
+def test_check_bn_fold_rejects_one_bf16_step():
+  p = _fold_problem(2)
+  wf, bias, wf0, bias0 = _fold_like_the_kernel(*p)
+  i = 200   # a filter element of the second unit
+  wf.view(torch.int16)[i] += 1
+  with pytest.raises(AssertionError, match="folded filter"):
+    kc.check_bn_fold(wf, bias, wf0, bias0, *p, "one step")

@@ -1,7 +1,9 @@
-"""Float64 references for the pooling, fused-stem, input-decode and small MNIST kernels.
+"""Float64 references for the pooling, fused-stem, input-decode and small MNIST kernels, the
+batch-norm fold of evaluation and serving, and the accumulators of gradient accumulation.
 
-Shared by tests/test_gpu_kernel_conformance.py (replays what the models launch) and
-tests/test_kernel_conformance_host.py (checks these references against PyTorch on the CPU).
+Shared by tests/test_gpu_kernel_conformance.py and tests/test_gpu_option_conformance.py (replay
+what the models launch) and tests/test_kernel_conformance_host.py (checks these references against
+PyTorch on the CPU, and the checkers against deliberately wrong results).
 Everything works on torch tensors of any device, NHWC, float64.
 
 Max pool selection (maxpool_fwd, PyTorch's max_pool2d): the taps of a window are visited in
@@ -163,3 +165,110 @@ def conv3x3_c1_wgrad_ref(x, dy):
   cols = torch.stack([x[:, kh:kh + H - 2, kw:kw + W - 2] for kh in range(3) for kw in range(3)], -1)
   cols, g = cols.reshape(-1, 9), dy.reshape(-1, Cout)
   return g.t() @ cols, g.abs().t() @ cols.abs(), g.sum(0), g.abs().sum(0)
+
+
+# ------------------------------------------------------------------ gradient accumulation
+def check_accumulated(acc, prefill, v, what):
+  """An accumulating kernel's parameter gradient: exactly one fp32 round-to-nearest addition of
+  this micro-batch's value ``v`` to the ``prefill`` A, fl(A + v), bit for bit."""
+  want = (prefill.to(torch.float32) + v.to(torch.float32)).contiguous().view(torch.int32)
+  got = acc.to(torch.float32).contiguous().view(torch.int32)
+  bad = got != want
+  if bool(bad.any()):
+    i = int(bad.reshape(-1).nonzero()[0])
+    raise AssertionError("{}: {} of {} accumulated elements are not fl(A + v); first at {}: "
+                         "got {!r}"
+                         " A {!r} v {!r}".format(what, int(bad.sum()), bad.numel(), i,
+                                                 float(acc.reshape(-1)[i]),
+                                                 float(prefill.reshape(-1)[i]),
+                                                 float(v.reshape(-1)[i])))
+
+
+# ------------------------------------------------------------------ batch-norm folding
+# bn_fold (csrc/eval.cu) per output channel c of a unit: s = gamma * rsqrtf(var + eps) in fp32,
+# wf = bf16(fp32(w * s)), bias = beta - mean * s.  The sum var + eps is one rounding (half an ulp
+# of the result after the square root), rsqrtf is within 2 ulp (CUDA Programming Guide, the
+# --use_fast_math table) and the product with gamma one rounding: |s - s64| <= FOLD_S_REL |s64|.
+FOLD_S_REL = 7 * 2.0 ** -24
+FOLD_COLS = 8   # kFold*: weight, cout, per_channel, gamma, beta, mean, var, bias
+
+
+def fold_ref(tab, eps, row0, w, aux32, running):
+  """float64 s = gamma / sqrt(var + eps) [rows], the folded filter w * s and bias beta - mean * s
+  (flat, in the layouts of w and of the bias vector), and boolean masks of the filter / bias
+  elements some unit writes.  Inputs: the host table, its fp32 eps and row0, the bf16 filters,
+  aux32 (gamma, beta) and the running-statistics buffer."""
+  f64 = lambda t: t.to(torch.float64)  # noqa: E731
+  tab, row0 = tab.cpu().tolist(), row0.cpu().tolist()
+  eps = f64(eps.cpu())
+  wflat = w.reshape(-1)
+  wf = torch.zeros(wflat.shape, dtype=torch.float64, device=w.device)
+  wmask = torch.zeros(wflat.shape, dtype=torch.bool, device=w.device)
+  nb = max(r[7] + (r[1] + 7) // 8 * 8 for r in tab)
+  bias = torch.zeros(nb, dtype=torch.float64, device=w.device)
+  bmask = torch.zeros(nb, dtype=torch.bool, device=w.device)
+  s_all = torch.zeros(row0[-1], dtype=torch.float64, device=w.device)
+  for u, (wo, cout, per, go, bo, mo, vo, fo) in enumerate(tab):
+    gam, bet = f64(aux32[go:go + cout]), f64(aux32[bo:bo + cout])
+    mean, var = f64(running[mo:mo + cout]), f64(running[vo:vo + cout])
+    # var + eps with eps as the fp32 value the kernel adds
+    s = gam / torch.sqrt(var + float(eps[u]))
+    s_all[row0[u]:row0[u] + cout] = s
+    sl = slice(wo, wo + cout * per)
+    wf[sl] = (f64(wflat[sl]).reshape(cout, per) * s[:, None]).reshape(-1)
+    wmask[sl] = True
+    bias[fo:fo + cout] = bet - mean * s
+    bmask[fo:fo + cout] = True
+  return s_all, wf, bias, wmask, bmask
+
+
+def check_bn_fold(wf, bias, wf0, bias0, tab, eps, row0, w, aux32, running, what):
+  """bn_fold's outputs ``wf`` (bf16, layout of w) and ``bias`` (fp32) against float64, given what
+  they held before the launch (``wf0``, ``bias0``):
+    * wf: the float64 product t = w s64 rounded to bf16, exactly, unless t lies within the error
+      of the fp32 product (FOLD_S_REL + one rounding) of a bf16 rounding boundary; there either
+      neighbour (rounding is monotone, so wf must lie in [bf16(t - e), bf16(t + e)]);
+    * bias: within fp32 bounds of beta - mean s64: the scale's error on mean s and two roundings;
+    * every element no unit covers (the head's rows, the bias padding) exactly as it was."""
+  u = 2.0 ** -24
+  s64, t, b64, wmask, bmask = fold_ref(tab, eps, row0, w, aux32, running)
+  e = (FOLD_S_REL + 2 * u) * t.abs()
+  rne = lambda v: v.to(torch.float32).to(torch.bfloat16).to(torch.float64)  # noqa: E731
+  lo, hi = rne(t - e), rne(t + e)
+  got = wf.reshape(-1).to(torch.float64)
+  bad = wmask & ~((got >= lo) & (got <= hi))
+  if bool(bad.any()):
+    i = int(bad.nonzero()[0])
+    raise AssertionError("{}: {} of {} folded filter elements wrong; first at {}: got {!r} "
+                         "float64 {!r}".format(what, int(bad.sum()), int(wmask.sum()), i,
+                                               float(got[i]), float(t[i])))
+  b = bias.reshape(-1)[:b64.numel()].to(torch.float64)
+  ms = (b64 - _fold_beta(tab, aux32, b64)).abs()   # |mean s64|
+  bound = (FOLD_S_REL + 2 * u) * ms + 2 * u * b64.abs()
+  err = (b - b64).abs()
+  badb = bmask & ~(err <= bound)
+  if bool(badb.any()):
+    i = int(badb.nonzero()[0])
+    raise AssertionError("{}: {} of {} folded biases out of bound; first at {}: got {!r} float64 "
+                         "{!r} bound {!r}".format(what, int(badb.sum()), int(bmask.sum()), i,
+                                                  float(b[i]), float(b64[i]), float(bound[i])))
+  keep = ~wmask
+  assert _same_bits(wf.reshape(-1)[keep], wf0.reshape(-1)[keep]), \
+      what + ": filter elements of no folded unit changed"
+  bk = torch.ones(bias.numel(), dtype=torch.bool, device=bias.device)
+  bk[:bmask.numel()] = ~bmask
+  assert _same_bits(bias.reshape(-1)[bk], bias0.reshape(-1)[bk]), \
+      what + ": bias elements of no folded unit changed"
+
+
+def _same_bits(a, b):
+  iv = {torch.bfloat16: torch.int16, torch.float32: torch.int32}
+  return torch.equal(a.contiguous().view(iv[a.dtype]), b.contiguous().view(iv[b.dtype]))
+
+
+def _fold_beta(tab, aux32, like):
+  """beta of every bias slot the table covers, in the bias vector's layout (0 elsewhere)."""
+  out = torch.zeros_like(like)
+  for wo, cout, per, go, bo, mo, vo, fo in tab.cpu().tolist():
+    out[fo:fo + cout] = aux32[bo:bo + cout].to(torch.float64)
+  return out
