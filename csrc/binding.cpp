@@ -68,6 +68,21 @@ inline void need_aligned(const Tensor& t, int bytes, const char* name) {
 inline void need_numel(const Tensor& t, int64_t n, const char* what, const char* name) {
   TFOS_REQUIRE(t.numel() == n, what, ": ", name, " must hold ", n, " elements, got ", t.numel());
 }
+// The staged Mixup / CutMix draw of a training step (csrc/mix.cu): fp32 [kMixSlots] on the device
+// of `like`.  Refused with ValueError before anything else is looked at, so that no launch reads a
+// wrong vector.
+const float* check_mix(const c10::optional<Tensor>& mix, const Tensor& like, const char* what) {
+  if (!mix.has_value() || !mix->defined()) return nullptr;
+  TFOS_REQUIRE(mix->scalar_type() == torch::kFloat32, what, ": mix must be float32, got ",
+               std::string(c10::toString(mix->scalar_type())));
+  TFOS_REQUIRE(mix->numel() == tfos::kMixSlots && mix->is_contiguous(), what,
+               ": mix must be a contiguous vector of ", tfos::kMixSlots, " values, got ",
+               shape_str(*mix));
+  TFOS_REQUIRE(mix->is_cuda() && mix->device() == like.device(), what,
+               ": mix must be on the CUDA device of the batch (", like.device().str(), "), got ",
+               mix->device().str());
+  return mix->data_ptr<float>();
+}
 // NHWC max pooling: `in` [N, H, W, C] and `out` [N, OH, OW, C] bf16 with OH = (H + 2 pad - k) /
 // stride + 1 (PyTorch's floor mode), C a multiple of 8 (one 16-byte vector per 8 channels), and
 // the uint8 arg-max taps `idx` one per output element.  k <= 15 keeps every tap below 255, the
@@ -529,7 +544,14 @@ void avgpool_bwd(const Tensor& dy, Tensor dx) {
 }
 void softmax_xent(const Tensor& logits, const Tensor& labels, c10::optional<Tensor> dlogits,
                   Tensor loss_sum, c10::optional<Tensor> correct, int V, double scale,
-                  double label_smoothing) {
+                  double label_smoothing, c10::optional<Tensor> mix) {
+  if (mix.has_value() && mix->defined()) {
+    TFOS_REQUIRE(logits.scalar_type() == torch::kFloat32, "softmax_xent: mix needs fp32 logits");
+    TFOS_REQUIRE(logits.dim() == 2 && labels.numel() == logits.size(0),
+                 "softmax_xent: mix pairs the rows of logits [rows, ld] and needs one label per "
+                 "row, got logits ", shape_str(logits), " and ", labels.numel(), " labels");
+  }
+  const float* mixp = check_mix(mix, logits, "softmax_xent");
   if (!(std::isfinite(label_smoothing) && label_smoothing >= 0.0 && label_smoothing <= 1.0))
     throw py::value_error("softmax_xent: label_smoothing must be in [0, 1], got " +
                           std::to_string(label_smoothing));
@@ -548,7 +570,7 @@ void softmax_xent(const Tensor& logits, const Tensor& labels, c10::optional<Tens
   }
   check(tfos::softmax_xent(logits.data_ptr(), fp32 ? 1 : 0, labels.data_ptr<int>(), dl,
                            loss_sum.data_ptr<float>(), optf(correct), rows, V, ld, ldd, scale,
-                           static_cast<float>(label_smoothing), cur_stream()),
+                           static_cast<float>(label_smoothing), cur_stream(), mixp),
         "softmax_xent");
 }
 // The multi-label kernels' shapes: logits [rows, ld] with 1 <= V <= ld, targets [rows, V].
@@ -562,8 +584,10 @@ void check_multilabel(const Tensor& logits, const Tensor& targets, int64_t V, co
 }
 void sigmoid_bce(const Tensor& logits, const Tensor& targets, c10::optional<Tensor> dlogits,
                  Tensor loss_sum, c10::optional<Tensor> correct, int64_t V, double scale,
-                 double label_smoothing, c10::optional<Tensor> pos_weight) {
+                 double label_smoothing, c10::optional<Tensor> pos_weight,
+                 c10::optional<Tensor> mix) {
   const char* what = "sigmoid_bce";
+  const float* mixp = check_mix(mix, logits, what);
   TFOS_REQUIRE(std::isfinite(label_smoothing) && label_smoothing >= 0.0 && label_smoothing <= 1.0,
                what, ": label_smoothing must be in [0, 1], got ", label_smoothing);
   check_multilabel(logits, targets, V, what);
@@ -599,14 +623,19 @@ void sigmoid_bce(const Tensor& logits, const Tensor& targets, c10::optional<Tens
                           optf(correct), logits.size(0), static_cast<int>(V), logits.size(1),
                           has_d ? dlogits->size(1) : 0, scale,
                           static_cast<float>(label_smoothing),
-                          has_w ? pos_weight->data_ptr<float>() : nullptr, cur_stream()),
+                          has_w ? pos_weight->data_ptr<float>() : nullptr, cur_stream(), mixp),
         what);
 }
 void decode_normalize(const Tensor& in, Tensor out, int wofs, std::vector<double> mean,
-                      std::vector<double> stdv) {
+                      std::vector<double> stdv, c10::optional<Tensor> mix) {
   // in [N, H, W, C] uint8 -> out [N, H, Wp, Cp] bf16: pixel w lands at column wofs + w, channels
   // C..Cp and the columns outside [wofs, wofs + W) are zero
   const char* what = "decode_normalize";
+  if (mix.has_value() && mix->defined())
+    TFOS_REQUIRE(in.dim() == 4 && out.dim() == 4 && in.size(3) == 3 && out.size(3) == 8, what,
+                 ": mix decodes RGB into 8 channels only, got in ", shape_str(in), " out ",
+                 shape_str(out));
+  const float* mixp = check_mix(mix, in, what);
   need(in, torch::kUInt8, "in");
   need(out, torch::kBFloat16, "out");
   TFOS_REQUIRE(in.dim() == 4 && out.dim() == 4, what, ": in and out must be 4-D NHWC");
@@ -625,7 +654,7 @@ void decode_normalize(const Tensor& in, Tensor out, int wofs, std::vector<double
   }
   check(tfos::decode_normalize(in.data_ptr<uint8_t>(), out.data_ptr(), in.size(0), in.size(1),
                                in.size(2), in.size(3), out.size(2), out.size(3), wofs, m, is,
-                               cur_stream()),
+                               cur_stream(), mixp),
         "decode_normalize");
 }
 void bn_fold(const Tensor& tab, const Tensor& eps, const Tensor& row0, int64_t rows, const Tensor& w,
@@ -1346,14 +1375,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("avgpool_bwd", &avgpool_bwd);
   m.def("softmax_xent", &softmax_xent, py::arg("logits"), py::arg("labels"), py::arg("dlogits"),
         py::arg("loss_sum"), py::arg("correct"), py::arg("V"), py::arg("scale"),
-        py::arg("label_smoothing") = 0.0);
-  m.def("decode_normalize", &decode_normalize);
+        py::arg("label_smoothing") = 0.0, py::arg("mix") = py::none());
+  m.def("decode_normalize", &decode_normalize, py::arg("in"), py::arg("out"), py::arg("wofs"),
+        py::arg("mean"), py::arg("std"), py::arg("mix") = py::none());
   m.def("cast_f32_bf16", &cast_f32_bf16);
   m.def("bn_fold", &bn_fold);
   m.def("eval_metrics", &eval_metrics);
   m.def("sigmoid_bce", &sigmoid_bce, py::arg("logits"), py::arg("targets"), py::arg("dlogits"),
         py::arg("loss_sum"), py::arg("correct"), py::arg("V"), py::arg("scale"),
-        py::arg("label_smoothing") = 0.0, py::arg("pos_weight") = py::none());
+        py::arg("label_smoothing") = 0.0, py::arg("pos_weight") = py::none(),
+        py::arg("mix") = py::none());
   m.def("multilabel_eval_slots", &multilabel_eval_slots);
   m.def("multilabel_eval_metrics", &multilabel_eval_metrics);
   m.def("seg_eval_scratch", &seg_eval_scratch, py::arg("pixels"), py::arg("classes") = 8);

@@ -1228,7 +1228,13 @@ cudaError_t avgpool_bwd(const void* dy, void* dx, int N, int HW, int C, cudaStre
 }
 cudaError_t softmax_xent(const void* logits, int logits_fp32, const int* labels, void* dlogits,
                          float* loss_sum, float* correct_sum, long long rows, int V, int ld,
-                         int ldd, float scale, float label_smoothing, cudaStream_t s) {
+                         int ldd, float scale, float label_smoothing, cudaStream_t s,
+                         const float* mix) {
+  if (mix != nullptr) {
+    if (!logits_fp32) return cudaErrorInvalidValue;   // the mixed-target kernel reads fp32 logits
+    return mixed_target_xent(static_cast<const float*>(logits), labels, dlogits, loss_sum,
+                             correct_sum, rows, V, ld, ldd, scale, label_smoothing, mix, s);
+  }
   auto launch = [&](auto kernel, auto* l) {
     kernel<<<static_cast<unsigned>(rows), 128, 0, s>>>(
         l, labels, static_cast<__nv_bfloat16*>(dlogits), loss_sum, correct_sum, V, ld, ldd, scale,
@@ -1249,7 +1255,10 @@ cudaError_t softmax_xent(const void* logits, int logits_fp32, const int* labels,
 cudaError_t sigmoid_bce(const float* logits, const uint8_t* targets, void* dlogits,
                         float* loss_sum, float* correct_sum, long long rows, int V, int ld,
                         int ldd, float scale, float label_smoothing, const float* pos_weight,
-                        cudaStream_t s) {
+                        cudaStream_t s, const float* mix) {
+  if (mix != nullptr)
+    return mixed_target_bce(logits, targets, dlogits, loss_sum, correct_sum, rows, V, ld, ldd,
+                            scale, label_smoothing, pos_weight, mix, s);
   if (rows <= 0) return cudaSuccess;
   auto launch = [&](auto kernel) {
     kernel<<<static_cast<unsigned>((rows + kBceRows - 1) / kBceRows), kBceThreads, 0, s>>>(
@@ -1268,7 +1277,11 @@ cudaError_t sigmoid_bce(const float* logits, const uint8_t* targets, void* dlogi
 }
 cudaError_t decode_normalize(const uint8_t* in, void* out, int N, int H, int W, int C, int Wp,
                              int Cp, int wofs, const float* mean3, const float* istd3,
-                             cudaStream_t s) {
+                             cudaStream_t s, const float* mix) {
+  if (mix != nullptr) {
+    if (C != 3 || Cp != 8) return cudaErrorInvalidValue;
+    return mix_decode_rgb8(in, out, N, H, W, Wp, wofs, mean3, istd3, mix, s);
+  }
   if (C == 3 && Cp == 8) {
     const long long rows = static_cast<long long>(N) * H;
     decode_rgb8_kernel<<<grid_for(rows * ((Wp + 3) / 4), 256, kMaxBlocks * 4), 256, 0, s>>>(

@@ -64,9 +64,12 @@ cudaError_t avgpool_bwd(const void* dy, void* dx, int N, int HW, int C, cudaStre
 // softmax_xent: label_smoothing = 0 runs the plain cross-entropy instance; in (0, 1] the smoothed
 // one (target (1 - eps) onehot + eps / V over the V real classes).  Columns [V, ldd) of dlogits
 // are written as 0.
+// mix (optional, fp32 logits only): the staged Mixup / CutMix draw (mix.cu); the mixed-target
+// instance then runs in place of the plain one.
 cudaError_t softmax_xent(const void* logits, int logits_fp32, const int* labels, void* dlogits,
                          float* loss_sum, float* correct_sum, long long rows, int V, int ld,
-                         int ldd, float scale, float label_smoothing, cudaStream_t s);
+                         int ldd, float scale, float label_smoothing, cudaStream_t s,
+                         const float* mix = nullptr);
 // sigmoid_bce: multi-label binary cross-entropy with logits of fp32 logits [rows, ld] against
 // uint8 targets [rows, V] (nonzero = positive), columns [0, V) of the logits only.  With
 // t = y (1 - eps) + eps / 2 (eps = label_smoothing; t = y at 0) and p = pos_weight[j] (1 when
@@ -78,10 +81,11 @@ cudaError_t softmax_xent(const void* logits, int logits_fp32, const int* labels,
 cudaError_t sigmoid_bce(const float* logits, const uint8_t* targets, void* dlogits,
                         float* loss_sum, float* correct_sum, long long rows, int V, int ld,
                         int ldd, float scale, float label_smoothing, const float* pos_weight,
-                        cudaStream_t s);
+                        cudaStream_t s, const float* mix = nullptr);
+// mix (optional, C = 3 and Cp = 8 only): decode a Mixup / CutMix of the batch (mix.cu).
 cudaError_t decode_normalize(const uint8_t* in, void* out, int N, int H, int W, int C, int Wp,
                              int Cp, int wofs, const float* mean3, const float* istd3,
-                             cudaStream_t s);
+                             cudaStream_t s, const float* mix = nullptr);
 cudaError_t cast_f32_bf16(const float* in, void* out, long long n, cudaStream_t s);
 cudaError_t copy_channels(const void* src, void* dst, long long P, int C, int src_ld, int src_off,
                           int dst_ld, int dst_off, cudaStream_t s);
@@ -407,5 +411,33 @@ cudaError_t seg_eval_metrics(const void* logits, const int* labels, const int* n
 // channel j < V.  One pass; any pixel count; mask and out must be 16-byte aligned.
 cudaError_t seg_predict(const void* logits, uint8_t* mask, float* out, long long pixels, int VP,
                         int V, cudaStream_t s);
+
+// ---- mix.cu: Mixup / CutMix of a training batch (timm's "batch" mode, one draw per step).
+// mix[kMixSlots] is a device fp32 vector [mode, lam, y0, y1, x0, x1, 0, 0] staged by the host before
+// each step: mode kMixNone / kMixMixup / kMixCutmix (any other value is none), lam the weight of
+// a row's own sample, [y0, y1) x [x0, x1) the CutMix box of the uint8 image (clamped to it).  Row i
+// of the rows-row batch is paired with row rows - 1 - i.  Mode none gives the plain kernels'
+// results bit for bit (the loss sum within its rounding).
+constexpr int kMixSlots = 8;
+constexpr int kMixNone = 0;
+constexpr int kMixMixup = 1;
+constexpr int kMixCutmix = 2;
+// RGB uint8 [N, H, W, 3] -> bf16 [N, H, Wp, 8] as decode_normalize's RGB kernel lays it out; mixup
+// x = lam n(u_i) + (1 - lam) n(u_p) in fp32, one bf16 rounding; cutmix n(u_p) inside the box.
+cudaError_t mix_decode_rgb8(const uint8_t* in, void* out, int N, int H, int W, int Wp, int wofs,
+                            const float* mean3, const float* istd3, const float* mix,
+                            cudaStream_t s);
+// softmax_xent of fp32 logits against t = lam s(y_i) + (1 - lam) s(y_p), s the smoothed one-hot;
+// correct_sum counts arg-max == the dominant label (y_i when lam >= 0.5, else y_p).
+cudaError_t mixed_target_xent(const float* logits, const int* labels, void* dlogits,
+                              float* loss_sum, float* correct_sum, long long rows, int V, int ld,
+                              int ldd, float scale, float label_smoothing, const float* mix,
+                              cudaStream_t s);
+// sigmoid_bce against t = lam s(y_i) + (1 - lam) s(y_p), s(y) = y (1 - eps) + eps / 2; correct_sum
+// counts rows whose prediction equals the dominant row's multi-hot target.
+cudaError_t mixed_target_bce(const float* logits, const uint8_t* targets, void* dlogits,
+                             float* loss_sum, float* correct_sum, long long rows, int V, int ld,
+                             int ldd, float scale, float label_smoothing, const float* pos_weight,
+                             const float* mix, cudaStream_t s);
 
 }  // namespace tfos

@@ -49,6 +49,14 @@ def define_flags():
   p.add_argument("--clip_norm", type=float, default=None,
                  help="clip the averaged gradient to this global L2 norm (> 0; inf: only measure "
                       "it) and print grad_norm next to the loss")
+  p.add_argument("--mixup_alpha", type=float, default=0.0,
+                 help="Mixup: lam ~ Beta(alpha, alpha) per step (0: off)")
+  p.add_argument("--cutmix_alpha", type=float, default=0.0,
+                 help="CutMix: lam ~ Beta(alpha, alpha) per step (0: off)")
+  p.add_argument("--mix_prob", type=float, default=1.0,
+                 help="probability that a step mixes at all, in [0, 1]")
+  p.add_argument("--mix_switch_prob", type=float, default=0.5,
+                 help="with both alphas > 0: probability that a mixing step is CutMix")
   return p
 
 
@@ -92,6 +100,10 @@ def main_fun(argv, ctx):
     smooth["ema_decay"] = args.ema_decay
   if args.clip_norm is not None:
     smooth["clip_norm"] = args.clip_norm
+  for name, default in (("mixup_alpha", 0.0), ("cutmix_alpha", 0.0), ("mix_prob", 1.0),
+                        ("mix_switch_prob", 0.5)):
+    if getattr(args, name) != default:
+      smooth[name] = getattr(args, name)
   net = resnet.CifarResNetTrainer(depth=args.resnet_size, batch=B, device=dev, comm=comm,
                                   lr=resnet.piecewise_lr(0, B * world), **smooth)
   if comm is not None:

@@ -105,6 +105,14 @@ def parse(argv):
                       "it) and log grad_norm")
   p.add_argument("--gradient_accumulation_steps", type=int, default=1,
                  help="micro-batches per update (k >= 1): the step counts above count updates")
+  p.add_argument("--mixup_alpha", type=float, default=0.0,
+                 help="Mixup: lam ~ Beta(alpha, alpha) per step (0: off)")
+  p.add_argument("--cutmix_alpha", type=float, default=0.0,
+                 help="CutMix: lam ~ Beta(alpha, alpha) per step (0: off)")
+  p.add_argument("--mix_prob", type=float, default=1.0,
+                 help="probability that a step mixes at all, in [0, 1]")
+  p.add_argument("--mix_switch_prob", type=float, default=0.5,
+                 help="with both alphas > 0: probability that a mixing step is CutMix")
   p.add_argument("--multi_label", action="store_true",
                  help="multi-hot labels and the binary cross-entropy; evaluation reports "
                       "binary_accuracy, exact_match, f1 and macro_f1")
@@ -146,6 +154,10 @@ def main_fun(argv, ctx):
     opt["gradient_accumulation_steps"] = k
   if args.multi_label:
     opt["multi_label"] = True
+  for name, default in (("mixup_alpha", 0.0), ("cutmix_alpha", 0.0), ("mix_prob", 1.0),
+                        ("mix_switch_prob", 0.5)):
+    if getattr(args, name) != default:
+      opt[name] = getattr(args, name)
   if args.model == "resnet56":
     net = resnet.CifarResNetTrainer(depth=56, batch=B, device="cuda:0", comm=comm, lr=base_lr, **opt)
   else:

@@ -15,6 +15,7 @@ tf.distribute in its example programs (e.g. examples/mnist/keras/mnist_spark.py:
 import math
 import numbers
 
+import numpy as np
 import torch
 
 from .. import ops
@@ -172,6 +173,75 @@ def check_gradient_accumulation_steps(k, training=True):
   return int(k)
 
 
+def check_mix_args(mixup_alpha=0.0, cutmix_alpha=0.0, mix_prob=1.0, mix_switch_prob=0.5,
+                   training=True):
+  """Validated ``(mixup_alpha, cutmix_alpha, mix_prob, mix_switch_prob)`` of a trainer as floats:
+  the alphas finite and >= 0, the probabilities in [0, 1] (ValueError otherwise, and for any value
+  other than the default with ``training=False``: an inference-only trainer has no training
+  batch to mix)."""
+  vals = {}
+  for name, v, lo, hi in (("mixup_alpha", mixup_alpha, 0.0, math.inf),
+                          ("cutmix_alpha", cutmix_alpha, 0.0, math.inf),
+                          ("mix_prob", mix_prob, 0.0, 1.0),
+                          ("mix_switch_prob", mix_switch_prob, 0.0, 1.0)):
+    if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(float(v)) \
+        or not lo <= float(v) <= hi:
+      rng = "finite and >= 0" if hi == math.inf else "in [0, 1]"
+      raise ValueError("{} must be a real number {}, got {!r}".format(name, rng, v))
+    vals[name] = float(v)
+  if not training and (vals["mixup_alpha"] or vals["cutmix_alpha"] or vals["mix_prob"] != 1.0 or
+                       vals["mix_switch_prob"] != 0.5):
+    raise ValueError("mixup_alpha, cutmix_alpha, mix_prob and mix_switch_prob need training=True "
+                     "(an inference-only trainer has no training batch to mix)")
+  return (vals["mixup_alpha"], vals["cutmix_alpha"], vals["mix_prob"], vals["mix_switch_prob"])
+
+
+MIX_MODES = ("none", "mixup", "cutmix")   # index = the mode code of the staged vector (kMix*)
+MIX_SLOTS = 8                             # csrc/ops.h kMixSlots
+
+
+class MixDraws(object):
+  """The per-step Mixup / CutMix draw of a trainer: timm's ``Mixup`` in "batch" mode with
+  ``correct_lam=True``, from a ``numpy.random.Generator`` seeded with ``(seed, rank)``.
+
+  ``draw(H, W)`` returns ``(mode, lam, box)``: with probability ``1 - mix_prob`` the step does not
+  mix (``("none", 1.0, (0, 0, 0, 0))``); otherwise the mode is cutmix with probability
+  ``mix_switch_prob`` when both alphas are > 0 (else the one whose alpha is > 0) and
+  lam ~ Beta(alpha, alpha) of that mode.  A CutMix box ``(y0, y1, x0, x1)`` (rows [y0, y1), columns
+  [x0, x1) of the H x W image) is centred on a uniform pixel with sides int(H r), int(W r),
+  r = sqrt(1 - lam), clipped to the image, and lam becomes 1 - box area / (H W)."""
+
+  def __init__(self, mixup_alpha, cutmix_alpha, mix_prob=1.0, mix_switch_prob=0.5, seed=0, rank=0):
+    self.mixup_alpha, self.cutmix_alpha = float(mixup_alpha), float(cutmix_alpha)
+    self.mix_prob, self.mix_switch_prob = float(mix_prob), float(mix_switch_prob)
+    self.rng = np.random.default_rng([int(seed), int(rank)])
+
+  def draw(self, H, W):
+    rng = self.rng
+    if not rng.random() < self.mix_prob:
+      return "none", 1.0, (0, 0, 0, 0)
+    if self.mixup_alpha > 0 and self.cutmix_alpha > 0:
+      cut = bool(rng.random() < self.mix_switch_prob)
+    else:
+      cut = self.cutmix_alpha > 0
+    a = self.cutmix_alpha if cut else self.mixup_alpha
+    lam = float(rng.beta(a, a))
+    if not cut:
+      return "mixup", lam, (0, 0, 0, 0)
+    r = math.sqrt(1.0 - lam)
+    ch, cw = int(H * r), int(W * r)
+    cy, cx = int(rng.integers(0, H)), int(rng.integers(0, W))
+    y0, y1 = min(max(cy - ch // 2, 0), H), min(max(cy + ch // 2, 0), H)
+    x0, x1 = min(max(cx - cw // 2, 0), W), min(max(cx + cw // 2, 0), W)
+    return "cutmix", 1.0 - (y1 - y0) * (x1 - x0) / float(H * W), (y0, y1, x0, x1)
+
+  @staticmethod
+  def vector(draw):
+    """The draw as the kernels read it: [mode, lam, y0, y1, x0, x1, 0, 0] (fp32 on the device)."""
+    mode, lam, box = draw
+    return [float(MIX_MODES.index(mode)), float(lam)] + [float(v) for v in box] + [0.0, 0.0]
+
+
 class GradAccumulation(object):
   """The update window of a trainer with ``gradient_accumulation_steps`` k (Keras's
   ``gradient_accumulation_steps``): ``train_step`` call i of a window is micro-step
@@ -200,14 +270,18 @@ class GradAccumulation(object):
       self.micro_step = 0
       optim.zero_grads()
 
-  def capture(self, device, step_kernels, mode):
+  def capture(self, device, step_kernels, mode, before_step=None):
     """CUDA graphs of the micro-steps, one per distinct phase ({phase: graph}): warm-up runs
     max(2, k) micro-steps eagerly on a side stream (two steps with k = 1, as before accumulation;
-    with k > 1 every position of the window once), then each phase is captured."""
+    with k > 1 every position of the window once), then each phase is captured.
+    ``before_step``: called on the side stream before each warm-up step, as ``train_step`` does
+    before a step (the Mixup / CutMix draw and its staging); never inside a capture."""
     s = torch.cuda.Stream(device=device)
     s.wait_stream(torch.cuda.current_stream(device))
     with torch.cuda.stream(s):
       for _ in range(max(2, self.k)):
+        if before_step is not None:
+          before_step()
         step_kernels()
         self.advance()
     torch.cuda.current_stream(device).wait_stream(s)

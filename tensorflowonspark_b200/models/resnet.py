@@ -292,7 +292,8 @@ class ResNetTrainer(object):
                lr=0.1, momentum=0.9, weight_decay=1e-4, comm=None, training=True, seed=1234,
                optimizer="momentum", trust_coefficient=0.001, label_smoothing=0.0,
                ema_decay=None, clip_norm=None, beta1=0.9, beta2=0.999, epsilon=1e-7,
-               gradient_accumulation_steps=1, multi_label=False, pos_weight=None):
+               gradient_accumulation_steps=1, multi_label=False, pos_weight=None,
+               mixup_alpha=0.0, cutmix_alpha=0.0, mix_prob=1.0, mix_switch_prob=0.5):
     """``optimizer``: sgd | momentum | adam | adamw | lars | lamb (``trust_coefficient`` is LARS's
     eta; see parallel/fused_optim.py).  adam folds ``weight_decay`` into the gradient (L2), adamw
     decouples it (``torch.optim.AdamW``), lamb is layer-wise adaptive Adam (apex ``FusedLAMB``).
@@ -333,10 +334,24 @@ class ResNetTrainer(object):
     -[p_j t log sigmoid(l) + (1 - t) log(1 - sigmoid(l))].  ``train_step`` returns the mean loss
     and ``correct`` counts the rows whose prediction (logit > 0 per class) equals the target
     exactly; ``eval_end`` reports binary accuracy, exact match and micro / macro F1
-    (``multilabel_totals``); serving returns a multi-hot ``prediction``."""
+    (``multilabel_totals``); serving returns a multi-hot ``prediction``.
+
+    ``mixup_alpha``, ``cutmix_alpha`` (finite, >= 0; training only): Mixup and CutMix as timm's
+    ``Mixup`` in "batch" mode with ``correct_lam=True``.  Each ``train_step`` call (each
+    micro-step, each warm-up step of ``capture()``) draws one (mode, lam, box) on the host
+    (engine.MixDraws, seeded with (``seed``, rank)); ``last_mix`` holds the last draw.  Row i of the
+    local batch of B rows is paired with row B - 1 - i: Mixup trains on lam x_i + (1 - lam) x_p,
+    CutMix pastes row p's pixels into a box of row i, and the target is lam s(y_i) + (1 - lam)
+    s(y_p) with s the smoothed target above (one-hot or multi-hot).  ``mix_prob`` (in [0, 1]): the
+    probability that a step mixes at all; ``mix_switch_prob`` (in [0, 1]): with both alphas > 0,
+    the probability that a mixing step is CutMix.  ``correct`` then counts hits against the
+    dominant sample (the row's own label when lam >= 0.5, its partner's otherwise).  Evaluation,
+    serving and exports never mix."""
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     self.multi_label, pos_weight = _check_multilabel_args(multi_label, pos_weight, num_classes,
                                                           training)
+    mix_args = engine.check_mix_args(mixup_alpha, cutmix_alpha, mix_prob, mix_switch_prob,
+                                     training)
     k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps, training)
     self.ema_decay = engine.check_ema_decay(ema_decay, training)
     self.clip_norm = engine.check_clip_norm(clip_norm, training)
@@ -481,11 +496,39 @@ class ResNetTrainer(object):
         for bn in self._batch_norms():
           bn.accumulate_grads(None)   # every one has its arena slots or a fused reduction
     self.accum = engine.GradAccumulation(k_acc)
+    self._build_mix(mix_args, seed)
     self.graph = None
     self.graphs = None
     self.mean = [0.485, 0.456, 0.406]
     self.std = [0.229, 0.224, 0.225]
     self._assign_directions()
+
+  def _build_mix(self, mix_args, seed):
+    """Mixup / CutMix state: the host draws (engine.MixDraws) and the device vector each step's
+    draw is staged into; neither exists when both alphas are 0."""
+    (self.mixup_alpha, self.cutmix_alpha, self.mix_prob, self.mix_switch_prob) = mix_args
+    self.mixer = self.mix = self.last_mix = None
+    if self.mixup_alpha > 0 or self.cutmix_alpha > 0:
+      rank = self.comm.rank if self.comm is not None else 0
+      self.mixer = engine.MixDraws(self.mixup_alpha, self.cutmix_alpha, self.mix_prob,
+                                   self.mix_switch_prob, seed=seed, rank=rank)
+      self.mix = torch.zeros(engine.MIX_SLOTS, dtype=torch.float32, device=self.device)
+
+  def _stage_mix(self):
+    """Draw this step's mix on the host and copy it into ``mix`` on the current stream, ahead of
+    the step's kernels (never inside a graph capture).  The source is a fresh pageable tensor: the
+    copy takes the values before it returns, so the host never waits and never overwrites what a
+    queued copy still reads."""
+    if self.mixer is None:
+      return
+    self.last_mix = self.mixer.draw(self.image, self.image)
+    self.mix.copy_(torch.tensor(engine.MixDraws.vector(self.last_mix), dtype=torch.float32),
+                   non_blocking=True)
+
+  def _mix_arg(self):
+    """The ``mix`` keyword of the training decode and loss: none when the trainer does not mix,
+    so such a trainer launches exactly what it did before mixing existed."""
+    return {} if self.mix is None else {"mix": self.mix}
 
   def _batch_norms(self):
     return [self.stem_bn] + [u.bn for b in self.blocks
@@ -587,6 +630,7 @@ class ResNetTrainer(object):
     ``gradient_accumulation_steps`` > 1 it is the first micro-step of a window (broadcast and
     accumulate, no update)."""
     comm = self.comm
+    self._stage_mix()
     comm.broadcast("aux32", self._root)  # BN scale/offset + biases: tiny, consumed in fp32
     comm.barrier()                        # root's weights are final and visible
     main = torch.cuda.current_stream(self.device)
@@ -610,7 +654,8 @@ class ResNetTrainer(object):
     run = (lambda c: c.forward_remote()) if remote else (lambda c: c.forward())
     if self.stats_arena is not None:
       self.stats_arena.zero()   # the fused conv epilogues accumulate from zero every pass
-    K.decode_normalize(self.in_u8, self.xp, igemm.STEM_PAD, self.mean, self.std)
+    K.decode_normalize(self.in_u8, self.xp, igemm.STEM_PAD, self.mean, self.std,
+                       **(self._mix_arg() if training else {}))
     (self.p_stem_remote if remote else self.p_stem).run()
     if training:
       # BN + ReLU + max pool in one pass over the raw conv output (csrc/stem_fused.cu): the
@@ -641,15 +686,16 @@ class ResNetTrainer(object):
   def _loss(self, with_grad):
     self.loss_sum.zero_()
     self.correct.zero_()
+    mix = self._mix_arg() if with_grad else {}
     if self.multi_label:
       ops.K.sigmoid_bce(self.logits, self.labels, self.dlogits if with_grad else None,
                         self.loss_sum, self.correct, self.num_classes,
                         1.0 / (self.B * self.num_classes), label_smoothing=self.label_smoothing,
-                        pos_weight=self.pos_weight)
+                        pos_weight=self.pos_weight, **mix)
       return
     ops.K.softmax_xent(self.logits, self.labels, self.dlogits if with_grad else None,
                        self.loss_sum, self.correct, self.num_classes, 1.0 / self.B,
-                       label_smoothing=self.label_smoothing)
+                       label_smoothing=self.label_smoothing, **mix)
 
   # -------------------------------------------------------------- backward
   def _backward(self, zero=True, update=True):
@@ -709,13 +755,16 @@ class ResNetTrainer(object):
     # defers them), but the process group's watchdog thread may still poll events of the warm-up
     # collectives - thread-local capture keeps that from invalidating the capture
     mode = "thread_local" if getattr(self.optim, "group_mode", False) else "global"
-    self.graphs = self.accum.capture(self.device, self.step_kernels, mode)
+    # the warm-up steps draw and stage their mix as train_step does; the graphs read ``mix``
+    self.graphs = self.accum.capture(self.device, self.step_kernels, mode,
+                                     before_step=self._stage_mix if self.mixer else None)
     self.graph = self.graphs[(self.accum.k == 1, True)]
     return self.graph
 
   def train_step(self, images_u8=None, labels=None):
     if images_u8 is not None:
       self.set_input(images_u8, labels)
+    self._stage_mix()
     # a captured step replays its graph; after the updating one a cross-host communicator runs
     # its all-reduce + update outside the graph (after_replay)
     self.accum.run(self.graphs if self.graph is not None else None, self.step_kernels, self.optim)
@@ -1001,15 +1050,19 @@ class CifarResNetTrainer(object):
   reference example actually trains (examples/resnet/resnet_cifar_dist.py:208, ``resnet56``,
   momentum SGD, batch 128, weight decay 2e-4).  ``optimizer``, ``num_classes``,
   ``label_smoothing``, ``ema_decay``, ``clip_norm``, ``beta1``, ``beta2``, ``epsilon``,
-  ``gradient_accumulation_steps``, ``multi_label`` and ``pos_weight`` as in ResNetTrainer."""
+  ``gradient_accumulation_steps``, ``multi_label``, ``pos_weight``, ``mixup_alpha``,
+  ``cutmix_alpha``, ``mix_prob`` and ``mix_switch_prob`` as in ResNetTrainer (the CutMix box is
+  drawn on the 32 x 32 image)."""
 
   def __init__(self, depth=56, batch=128, num_classes=10, device="cuda:0", lr=0.1, momentum=0.9,
                weight_decay=2e-4, comm=None, seed=1234, optimizer="momentum",
                trust_coefficient=0.001, label_smoothing=0.0, ema_decay=None, clip_norm=None,
                beta1=0.9, beta2=0.999, epsilon=1e-7, gradient_accumulation_steps=1,
-               multi_label=False, pos_weight=None):
+               multi_label=False, pos_weight=None, mixup_alpha=0.0, cutmix_alpha=0.0, mix_prob=1.0,
+               mix_switch_prob=0.5):
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     self.multi_label, pos_weight = _check_multilabel_args(multi_label, pos_weight, num_classes)
+    mix_args = engine.check_mix_args(mixup_alpha, cutmix_alpha, mix_prob, mix_switch_prob)
     k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps)
     self.ema_decay = engine.check_ema_decay(ema_decay)
     self.clip_norm = engine.check_clip_norm(clip_norm)
@@ -1091,6 +1144,7 @@ class CifarResNetTrainer(object):
       for _, bn in self._fold_units():
         bn.accumulate_grads(self.grad_scratch)
     self.accum = engine.GradAccumulation(k_acc)
+    self._build_mix(mix_args, seed)
     self.graph = None
     self.graphs = None
     self.mean, self.std = [0.4914, 0.4822, 0.4465], [0.2470, 0.2435, 0.2616]
@@ -1114,6 +1168,9 @@ class CifarResNetTrainer(object):
   grad_norm = ResNetTrainer.grad_norm
   gradient_accumulation_steps = ResNetTrainer.gradient_accumulation_steps
   micro_step = ResNetTrainer.micro_step
+  _build_mix = ResNetTrainer._build_mix
+  _stage_mix = ResNetTrainer._stage_mix
+  _mix_arg = ResNetTrainer._mix_arg
 
   def _fold_units(self):
     """(filter spec, batch norm) of every convolution followed by a batch norm, stem first."""
@@ -1151,7 +1208,7 @@ class CifarResNetTrainer(object):
   def step_kernels(self):
     K = ops.K
     zero, update = self.accum.phase()
-    K.decode_normalize(self.in_u8, self.x8, 0, self.mean, self.std)
+    K.decode_normalize(self.in_u8, self.x8, 0, self.mean, self.std, **self._mix_arg())
     self.stem.conv.forward()
     self.stem.bn.forward(self.stem_raw, self.stem_act, None, 1, True)
     for b in self.blocks:
