@@ -83,6 +83,29 @@ const float* check_mix(const c10::optional<Tensor>& mix, const Tensor& like, con
                mix->device().str());
   return mix->data_ptr<float>();
 }
+// Stochastic depth's per-sample factors of a residual branch's last batch norm (bn_bwd.cu): fp32
+// [N], contiguous, on the device of the NHWC batch x [N, H, W, C] (fewer than 2^31 rows).  Refused
+// with ValueError before anything else is looked at, so that no launch reads a wrong vector.
+tfos::SampleScale check_sample_scale(const c10::optional<Tensor>& ss, const Tensor& x,
+                                     const char* what) {
+  tfos::SampleScale out;
+  if (!ss.has_value() || !ss->defined()) return out;
+  TFOS_REQUIRE(ss->scalar_type() == torch::kFloat32, what, ": sample_scale must be float32, got ",
+               std::string(c10::toString(ss->scalar_type())));
+  TFOS_REQUIRE(ss->is_contiguous(), what, ": sample_scale must be contiguous");
+  TFOS_REQUIRE(x.dim() == 4, what, ": sample_scale needs a 4-D NHWC x, got ", shape_str(x));
+  TFOS_REQUIRE(ss->dim() == 1 && ss->numel() == x.size(0), what,
+               ": sample_scale must hold one value per sample of x ", shape_str(x), ", got ",
+               shape_str(*ss));
+  TFOS_REQUIRE(ss->is_cuda() && ss->device() == x.device(), what,
+               ": sample_scale must be on the CUDA device of x (", x.device().str(), "), got ",
+               ss->device().str());
+  TFOS_REQUIRE(x.size(0) * x.size(1) * x.size(2) < (int64_t{1} << 31), what,
+               ": sample_scale needs fewer than 2^31 rows, got ", shape_str(x));
+  out.scale = ss->data_ptr<float>();
+  out.rows_per_sample = static_cast<unsigned>(x.size(1) * x.size(2));
+  return out;
+}
 // NHWC max pooling: `in` [N, H, W, C] and `out` [N, OH, OW, C] bf16 with OH = (H + 2 pad - k) /
 // stride + 1 (PyTorch's floor mode), C a multiple of 8 (one 16-byte vector per 8 channels), and
 // the uint8 arg-max taps `idx` one per output element.  k <= 15 keeps every tap below 255, the
@@ -339,7 +362,9 @@ void bn_inference_coeffs(const Tensor& gamma, const Tensor& beta, const Tensor& 
         "bn_inference_coeffs");
 }
 void bn_apply(const Tensor& x, c10::optional<Tensor> residual, const Tensor& scale,
-              const Tensor& shift, Tensor y, int act, c10::optional<Tensor> mask) {
+              const Tensor& shift, Tensor y, int act, c10::optional<Tensor> mask,
+              c10::optional<Tensor> sample_scale) {
+  const tfos::SampleScale ss = check_sample_scale(sample_scale, x, "bn_apply");
   need(x, torch::kBFloat16, "x");
   need(y, torch::kBFloat16, "y");
   const int C = x.size(-1);
@@ -350,14 +375,16 @@ void bn_apply(const Tensor& x, c10::optional<Tensor> residual, const Tensor& sca
   check(tfos::bn_apply(x.data_ptr(), optptr(residual), scale.data_ptr<float>(),
                        shift.data_ptr<float>(), y.data_ptr(),
                        mask.has_value() ? mask->data_ptr<uint8_t>() : nullptr, x.numel() / C, C,
-                       act, cur_stream()),
+                       act, cur_stream(), ss),
         "bn_apply");
 }
 void bn_apply_finalize(const Tensor& x, c10::optional<Tensor> residual, Tensor y, int act,
                        c10::optional<Tensor> mask, const Tensor& sum, const Tensor& sumsq,
                        const Tensor& gamma, const Tensor& beta, c10::optional<Tensor> running_mean,
                        c10::optional<Tensor> running_var, Tensor mean, Tensor invstd, Tensor scale,
-                       Tensor shift, double count, double eps, double momentum) {
+                       Tensor shift, double count, double eps, double momentum,
+                       c10::optional<Tensor> sample_scale) {
+  const tfos::SampleScale ss = check_sample_scale(sample_scale, x, "bn_apply_finalize");
   need(x, torch::kBFloat16, "x");
   need(y, torch::kBFloat16, "y");
   const int C = x.size(-1);
@@ -378,12 +405,16 @@ void bn_apply_finalize(const Tensor& x, c10::optional<Tensor> residual, Tensor y
   f.momentum = static_cast<float>(momentum);
   check(tfos::bn_apply_finalize(x.data_ptr(), optptr(residual), y.data_ptr(),
                                 mask.has_value() ? mask->data_ptr<uint8_t>() : nullptr,
-                                x.numel() / C, C, act, f, cur_stream()),
+                                x.numel() / C, C, act, f, cur_stream(), ss),
         "bn_apply_finalize");
 }
 void bn_bwd_reduce(const Tensor& dy, const Tensor& x, c10::optional<Tensor> y, const Tensor& mean,
                    const Tensor& invstd, Tensor dgamma, Tensor dbeta, int relu,
-                   c10::optional<Tensor> fscale, c10::optional<Tensor> fshift) {
+                   c10::optional<Tensor> fscale, c10::optional<Tensor> fshift,
+                   c10::optional<Tensor> sample_scale) {
+  TFOS_REQUIRE(!(sample_scale.has_value() && sample_scale->defined()) || relu != 2,
+               "bn_bwd_reduce: sample_scale needs relu 0, 1 or 3 (a residual unit), got 2");
+  const tfos::SampleScale ss = check_sample_scale(sample_scale, x, "bn_bwd_reduce");
   TORCH_CHECK(relu != 1 || (y.has_value() && y->defined()), "bn_bwd_reduce: relu=1 needs y");
   TORCH_CHECK(relu != 2 || (fscale.has_value() && fshift.has_value()), "bn_bwd_reduce: relu=2 needs scale/shift");
   need(dy, torch::kBFloat16, "dy");
@@ -391,7 +422,8 @@ void bn_bwd_reduce(const Tensor& dy, const Tensor& x, c10::optional<Tensor> y, c
   const int C = x.size(-1);
   check(tfos::bn_bwd_reduce(dy.data_ptr(), x.data_ptr(), optptr(y), mean.data_ptr<float>(),
                             invstd.data_ptr<float>(), optf(fscale), optf(fshift), x.numel() / C, C,
-                            relu, dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), cur_stream()),
+                            relu, dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), cur_stream(),
+                            ss),
         "bn_bwd_reduce");
 }
 void bn_bwd_apply(const Tensor& dy, const Tensor& x, c10::optional<Tensor> y, const Tensor& gamma,
@@ -399,7 +431,16 @@ void bn_bwd_apply(const Tensor& dy, const Tensor& x, c10::optional<Tensor> y, co
                   const Tensor& dbeta, Tensor dx, c10::optional<Tensor> dres, int relu,
                   c10::optional<Tensor> fscale, c10::optional<Tensor> fshift,
                   c10::optional<Tensor> sum_g, c10::optional<Tensor> sum_gx,
-                  c10::optional<Tensor> acc_dgamma, c10::optional<Tensor> acc_dbeta) {
+                  c10::optional<Tensor> acc_dgamma, c10::optional<Tensor> acc_dbeta,
+                  c10::optional<Tensor> sample_scale) {
+  if (sample_scale.has_value() && sample_scale->defined()) {
+    TFOS_REQUIRE(!(sum_g.has_value() && sum_g->defined()) &&
+                     !(sum_gx.has_value() && sum_gx->defined()),
+                 "bn_bwd_apply: sample_scale cannot be used with a fused reduction (sum_g / sum_gx)");
+    TFOS_REQUIRE(relu != 2,
+                 "bn_bwd_apply: sample_scale needs relu 0, 1 or 3 (a residual unit), got 2");
+  }
+  const tfos::SampleScale ss = check_sample_scale(sample_scale, x, "bn_bwd_apply");
   const int C = x.size(-1);
   const bool acc = acc_dgamma.has_value() && acc_dgamma->defined();
   TORCH_CHECK(acc == (acc_dbeta.has_value() && acc_dbeta->defined()),
@@ -415,7 +456,7 @@ void bn_bwd_apply(const Tensor& dy, const Tensor& x, c10::optional<Tensor> y, co
                            dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), optf(fscale),
                            optf(fshift), dx.data_ptr(), const_cast<void*>(optptr(dres)),
                            x.numel() / C, C, relu, optf(sum_g), optf(sum_gx), cur_stream(),
-                           optf(acc_dgamma), optf(acc_dbeta)),
+                           optf(acc_dgamma), optf(acc_dbeta), ss),
         "bn_bwd_apply");
 }
 void stem_bn_relu_pool_fwd(const Tensor& x, Tensor y, Tensor idx, const Tensor& sum,
@@ -1353,14 +1394,22 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("bn_finalize", &bn_finalize);
   m.def("bn_inference_coeffs", &bn_inference_coeffs);
   m.def("bn_apply", &bn_apply, py::arg("x"), py::arg("residual"), py::arg("scale"),
-        py::arg("shift"), py::arg("y"), py::arg("act"), py::arg("mask") = py::none());
-  m.def("bn_apply_finalize", &bn_apply_finalize);
-  m.def("bn_bwd_reduce", &bn_bwd_reduce);
+        py::arg("shift"), py::arg("y"), py::arg("act"), py::arg("mask") = py::none(),
+        py::arg("sample_scale") = py::none());
+  m.def("bn_apply_finalize", &bn_apply_finalize, py::arg("x"), py::arg("residual"), py::arg("y"),
+        py::arg("act"), py::arg("mask"), py::arg("sum"), py::arg("sumsq"), py::arg("gamma"),
+        py::arg("beta"), py::arg("running_mean"), py::arg("running_var"), py::arg("mean"),
+        py::arg("invstd"), py::arg("scale"), py::arg("shift"), py::arg("count"), py::arg("eps"),
+        py::arg("momentum"), py::arg("sample_scale") = py::none());
+  m.def("bn_bwd_reduce", &bn_bwd_reduce, py::arg("dy"), py::arg("x"), py::arg("y"),
+        py::arg("mean"), py::arg("invstd"), py::arg("dgamma"), py::arg("dbeta"), py::arg("relu"),
+        py::arg("fscale"), py::arg("fshift"), py::arg("sample_scale") = py::none());
   m.def("bn_bwd_apply", &bn_bwd_apply, py::arg("dy"), py::arg("x"), py::arg("y"), py::arg("gamma"),
         py::arg("mean"), py::arg("invstd"), py::arg("dgamma"), py::arg("dbeta"), py::arg("dx"),
         py::arg("dres"), py::arg("relu"), py::arg("fscale"), py::arg("fshift"),
         py::arg("sum_g") = py::none(), py::arg("sum_gx") = py::none(),
-        py::arg("acc_dgamma") = py::none(), py::arg("acc_dbeta") = py::none());
+        py::arg("acc_dgamma") = py::none(), py::arg("acc_dbeta") = py::none(),
+        py::arg("sample_scale") = py::none());
   m.def("stem_bn_relu_pool_fwd", &stem_bn_relu_pool_fwd);
   m.def("stem_pool_bn_bwd", &stem_pool_bn_bwd, py::arg("dy_pool"), py::arg("idx"), py::arg("x"),
         py::arg("gamma"), py::arg("mean"), py::arg("invstd"), py::arg("scale"), py::arg("shift"),

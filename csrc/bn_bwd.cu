@@ -11,6 +11,13 @@
 // Both kernels are latency bound unless enough bytes are in flight, so every thread owns one
 // 8-channel group (per-channel coefficients live in registers) and issues the 16-byte loads of
 // FOUR rows before touching any of them.
+//
+// Stochastic depth (the *_scaled kernels, template flag SCALE): a residual branch's last batch
+// norm multiplies sample n's output by sample_scale[n] (0 for a dropped sample, 1 / (1 - p) for a
+// kept one) before the shortcut is added.  Row r of the [P, C] tensor belongs to sample
+// r / rows_per_sample (r the memory row, after the row-order mapping).  The forward statistics
+// ignore the scale; the backward forms g = scale * masked dy, which is the gradient of the batch
+// norm's output.  The instances without the flag are the kernels as they were.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -59,12 +66,14 @@ __device__ __forceinline__ Geo geo(int C) {
   return g;
 }
 
-__global__ void __launch_bounds__(kThreads, 2)
-bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
-                     const __nv_bfloat16* __restrict__ y, const float* __restrict__ mean,
-                     const float* __restrict__ invstd, const float* __restrict__ fscale,
-                     const float* __restrict__ fshift, long long P, int C, int relu, float* dgamma,
-                     float* dbeta, const int rev) {
+template <bool SCALE>
+__device__ __forceinline__ void
+bn_bwd_reduce_body(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
+                   const __nv_bfloat16* __restrict__ y, const float* __restrict__ mean,
+                   const float* __restrict__ invstd, const float* __restrict__ fscale,
+                   const float* __restrict__ fshift, long long P, int C, int relu, float* dgamma,
+                   float* dbeta, const int rev, const float* __restrict__ sscale,
+                   unsigned rows_per_sample) {
   const Geo G = geo(C);
   __shared__ float red[2][kThreads][8];
   const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
@@ -89,15 +98,18 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
            p += kRows * stride) {
         uint4 gq[kRows], xq[kRows], yq[kRows];
         uint32_t mq[kRows];
+        float sq[kRows];
 #pragma unroll
         for (int k = 0; k < kRows; ++k) {
           const long long pk = p + k * stride;
           const bool in = pk < P;
-          const long long o = (rev ? P - 1 - pk : pk) * C + c;
+          const long long row = rev ? P - 1 - pk : pk;
+          const long long o = row * C + c;
           gq[k] = in ? ld_nc_v4(dy + o) : zero;
           xq[k] = in ? ld_nc_v4(x + o) : zero;
           yq[k] = (in && relu == 1) ? ld_nc_v4(y + o) : zero;
           mq[k] = (in && relu == 3) ? __ldg(reinterpret_cast<const uint8_t*>(y) + (o >> 3)) : 0u;
+          sq[k] = (SCALE && in) ? __ldg(sscale + static_cast<unsigned>(row) / rows_per_sample) : 0.f;
         }
 #pragma unroll
         for (int k = 0; k < kRows; ++k) {
@@ -107,7 +119,8 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const float2 xv = up2(xw[j]);
-            const float2 gj = masked_g(relu, gw[j], xv, yw[j], mq[k], j, fs[j], fh[j]);
+            float2 gj = masked_g(relu, gw[j], xv, yw[j], mq[k], j, fs[j], fh[j]);
+            if (SCALE) gj = make_float2(__fmul_rn(sq[k], gj.x), __fmul_rn(sq[k], gj.y));
             a0[j] = ffma2_rn(gj, fadd2_rn(xv, nmu[j]), a0[j]);
             a1[j] = fadd2_rn(a1[j], gj);
           }
@@ -147,6 +160,28 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
   }
 }
 
+__global__ void __launch_bounds__(kThreads, 2)
+bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
+                     const __nv_bfloat16* __restrict__ y, const float* __restrict__ mean,
+                     const float* __restrict__ invstd, const float* __restrict__ fscale,
+                     const float* __restrict__ fshift, long long P, int C, int relu, float* dgamma,
+                     float* dbeta, const int rev) {
+  bn_bwd_reduce_body<false>(dy, x, y, mean, invstd, fscale, fshift, P, C, relu, dgamma, dbeta, rev,
+                            nullptr, 1u);
+}
+
+__global__ void __launch_bounds__(kThreads, 2)
+bn_bwd_reduce_scaled_kernel(const __nv_bfloat16* __restrict__ dy,
+                            const __nv_bfloat16* __restrict__ x,
+                            const __nv_bfloat16* __restrict__ y, const float* __restrict__ mean,
+                            const float* __restrict__ invstd, const float* __restrict__ fscale,
+                            const float* __restrict__ fshift, long long P, int C, int relu,
+                            float* dgamma, float* dbeta, const int rev,
+                            const float* __restrict__ sscale, unsigned rows_per_sample) {
+  bn_bwd_reduce_body<true>(dy, x, y, mean, invstd, fscale, fshift, P, C, relu, dgamma, dbeta, rev,
+                           sscale, rows_per_sample);
+}
+
 // dx = A*g + B*x + K with per-channel A = gamma*invstd, B = -A*invstd*dgamma/M,
 // K = -A*dbeta/M - B*mean.  Optionally also stores the masked g (gradient of the residual
 // branch); dres may alias dy (same element read before it is written by the same thread).
@@ -155,7 +190,10 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
 // (per-step scratch written by the reduce; not read on the fused path), dx is formed from them, and
 // the thread that publishes on the fused path adds them to the parameter gradient acc_dgamma /
 // acc_dbeta, which holds the running sum of the earlier micro-batches.
-template <bool ACC>
+//
+// SCALE: dx is formed from sample_scale[n] * g; dres keeps the unscaled masked g (the shortcut's
+// gradient).
+template <bool ACC, bool SCALE>
 __device__ __forceinline__ void
 bn_bwd_apply_body(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x,
                   const __nv_bfloat16* __restrict__ y, const float* __restrict__ gamma,
@@ -165,9 +203,13 @@ bn_bwd_apply_body(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x,
                   __nv_bfloat16* __restrict__ dx, __nv_bfloat16* dres, long long P, int C,
                   int relu, float inv_count, const int rev,
                   const float* __restrict__ sum_g, const float* __restrict__ sum_gx,
-                  float* acc_dgamma, float* acc_dbeta) {
+                  float* acc_dgamma, float* acc_dbeta, const float* __restrict__ sscale,
+                  unsigned rows_per_sample) {
   const Geo G = geo(C);
   if (G.r_in >= G.rl) return;
+  // the scaled instances serve residual units (relu 0, 1, 3): without the recomputed mask, the
+  // scale fits in the registers the forward scale / shift would take
+  if (SCALE) relu = relu == 2 ? 0 : relu;
   const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
   for (int g0 = blockIdx.y * G.cg; g0 < G.groups; g0 += gridDim.y * G.cg) {
     const int g = g0 + G.g_in;
@@ -216,21 +258,25 @@ bn_bwd_apply_body(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x,
          p += kRows * stride) {
       uint4 gq[kRows], xq[kRows], yq[kRows];
       uint32_t mq[kRows];
+      float sq[kRows];
 #pragma unroll
       for (int k = 0; k < kRows; ++k) {
         const long long pk = p + k * stride;
         const bool in = pk < P;
-        const long long o = (rev ? P - 1 - pk : pk) * C + c;
+        const long long row = rev ? P - 1 - pk : pk;
+        const long long o = row * C + c;
         gq[k] = in ? *reinterpret_cast<const uint4*>(dy + o) : zero;  // may alias dres: no .nc
         xq[k] = in ? ld_nc_v4(x + o) : zero;
         yq[k] = (in && relu == 1) ? ld_nc_v4(y + o) : zero;
         mq[k] = (in && relu == 3) ? __ldg(reinterpret_cast<const uint8_t*>(y) + (o >> 3)) : 0u;
+        sq[k] = (SCALE && in) ? __ldg(sscale + static_cast<unsigned>(row) / rows_per_sample) : 0.f;
       }
 #pragma unroll
       for (int k = 0; k < kRows; ++k) {
         const long long pk = p + k * stride;
         if (pk >= P) break;
         const long long o = (rev ? P - 1 - pk : pk) * C + c;
+        const float sk = sq[k];
         const uint32_t gw[4] = {gq[k].x, gq[k].y, gq[k].z, gq[k].w};
         const uint32_t xw[4] = {xq[k].x, xq[k].y, xq[k].z, xq[k].w};
         const uint32_t yw[4] = {yq[k].x, yq[k].y, yq[k].z, yq[k].w};
@@ -239,7 +285,9 @@ bn_bwd_apply_body(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x,
         for (int j = 0; j < 4; ++j) {
           const float2 xv = up2(xw[j]);
           const float2 gj = masked_g(relu, gw[j], xv, yw[j], mq[k], j, fs[j], fh[j]);
-          const float2 ov = ffma2_rn(cA[j], gj, ffma2_rn(cB[j], xv, cK[j]));
+          const float2 gs =
+              SCALE ? make_float2(__fmul_rn(sk, gj.x), __fmul_rn(sk, gj.y)) : gj;
+          const float2 ov = ffma2_rn(cA[j], gs, ffma2_rn(cB[j], xv, cK[j]));
           ow[j] = pack_bf16x2(ov.x, ov.y);
           rw[j] = pack_bf16x2(gj.x, gj.y);
         }
@@ -260,8 +308,9 @@ bn_bwd_apply_kernel(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x
                     __nv_bfloat16* __restrict__ dx, __nv_bfloat16* dres, long long P, int C,
                     int relu, float inv_count, const int rev,
                     const float* __restrict__ sum_g, const float* __restrict__ sum_gx) {
-  bn_bwd_apply_body<false>(dy, x, y, gamma, mean, invstd, dgamma, dbeta, fscale, fshift, dx, dres,
-                           P, C, relu, inv_count, rev, sum_g, sum_gx, nullptr, nullptr);
+  bn_bwd_apply_body<false, false>(dy, x, y, gamma, mean, invstd, dgamma, dbeta, fscale, fshift, dx,
+                                  dres, P, C, relu, inv_count, rev, sum_g, sum_gx, nullptr, nullptr,
+                                  nullptr, 1u);
 }
 
 __global__ void __launch_bounds__(kThreads, 2)
@@ -274,20 +323,59 @@ bn_bwd_apply_acc_kernel(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict
                         int relu, float inv_count, const int rev,
                         const float* __restrict__ sum_g, const float* __restrict__ sum_gx,
                         float* acc_dgamma, float* acc_dbeta) {
-  bn_bwd_apply_body<true>(dy, x, y, gamma, mean, invstd, dgamma, dbeta, fscale, fshift, dx, dres,
-                          P, C, relu, inv_count, rev, sum_g, sum_gx, acc_dgamma, acc_dbeta);
+  bn_bwd_apply_body<true, false>(dy, x, y, gamma, mean, invstd, dgamma, dbeta, fscale, fshift, dx,
+                                 dres, P, C, relu, inv_count, rev, sum_g, sum_gx, acc_dgamma,
+                                 acc_dbeta, nullptr, 1u);
+}
+
+// The stochastic-depth instances (SCALE).  The host passes sum_g = sum_gx = nullptr (the reduction
+// of a scaled gradient is never fused), but as launch arguments, not constants: the per-channel
+// coefficients then compile as in the plain instances, and a scale of ones gives their dx bit for
+// bit.
+__global__ void __launch_bounds__(kThreads, 2)
+bn_bwd_apply_scaled_kernel(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x,
+                           const __nv_bfloat16* __restrict__ y, const float* __restrict__ gamma,
+                           const float* __restrict__ mean, const float* __restrict__ invstd,
+                           float* dgamma, float* dbeta, const float* __restrict__ fscale,
+                           const float* __restrict__ fshift, __nv_bfloat16* __restrict__ dx,
+                           __nv_bfloat16* dres, long long P, int C, int relu, float inv_count,
+                           const int rev, const float* __restrict__ sum_g,
+                           const float* __restrict__ sum_gx, const float* __restrict__ sscale,
+                           unsigned rows_per_sample) {
+  bn_bwd_apply_body<false, true>(dy, x, y, gamma, mean, invstd, dgamma, dbeta, fscale, fshift, dx,
+                                 dres, P, C, relu, inv_count, rev, sum_g, sum_gx, nullptr, nullptr,
+                                 sscale, rows_per_sample);
+}
+
+__global__ void __launch_bounds__(kThreads, 2)
+bn_bwd_apply_acc_scaled_kernel(const __nv_bfloat16* dy, const __nv_bfloat16* __restrict__ x,
+                               const __nv_bfloat16* __restrict__ y,
+                               const float* __restrict__ gamma, const float* __restrict__ mean,
+                               const float* __restrict__ invstd, float* dgamma, float* dbeta,
+                               const float* __restrict__ fscale, const float* __restrict__ fshift,
+                               __nv_bfloat16* __restrict__ dx, __nv_bfloat16* dres, long long P,
+                               int C, int relu, float inv_count, const int rev,
+                               const float* __restrict__ sum_g, const float* __restrict__ sum_gx,
+                               float* acc_dgamma, float* acc_dbeta,
+                               const float* __restrict__ sscale, unsigned rows_per_sample) {
+  bn_bwd_apply_body<true, true>(dy, x, y, gamma, mean, invstd, dgamma, dbeta, fscale, fshift, dx,
+                                dres, P, C, relu, inv_count, rev, sum_g, sum_gx, acc_dgamma,
+                                acc_dbeta, sscale, rows_per_sample);
 }
 
 // Forward apply: y = act(x * scale[c] + shift[c] (+ residual)); act 0 none, 1 relu, 2 relu6.
 // Same thread geometry as the backward kernels (a thread keeps one 8-channel group, so scale /
 // shift are loaded once, and four rows are in flight); the arithmetic runs on the packed
 // fp32x2 pipe.  mask (optional): one bit per element, set where the pre-activation is > 0.
-template <bool FIN>
-__global__ void __launch_bounds__(kThreads, 3)
-bn_fwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ residual,
-                    const float* __restrict__ scale, const float* __restrict__ shift,
-                    __nv_bfloat16* __restrict__ y, uint8_t* __restrict__ mask, long long P, int C,
-                    int act, const BnFinalize fin, const int rev) {
+// SCALE: y = act(sample_scale[n] * (x * scale[c] + shift[c]) (+ residual)), the mask taken from
+// that pre-activation; the FIN statistics do not see the scale.
+template <bool FIN, bool SCALE>
+__device__ __forceinline__ void
+bn_fwd_apply_body(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ residual,
+                  const float* __restrict__ scale, const float* __restrict__ shift,
+                  __nv_bfloat16* __restrict__ y, uint8_t* __restrict__ mask, long long P, int C,
+                  int act, const BnFinalize fin, const int rev, const float* __restrict__ sscale,
+                  unsigned rows_per_sample) {
   const Geo G = geo(C);
   if (G.r_in >= G.rl) return;
   const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
@@ -337,13 +425,16 @@ bn_fwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __
     for (long long p = static_cast<long long>(blockIdx.x) * G.rl + G.r_in; p < P;
          p += kRows * stride) {
       uint4 xq[kRows], rq[kRows];
+      float sq[kRows];
 #pragma unroll
       for (int k = 0; k < kRows; ++k) {
         const long long pk = p + k * stride;
         const bool in = pk < P;
-        const long long o = (rev ? P - 1 - pk : pk) * C + c;
+        const long long row = rev ? P - 1 - pk : pk;
+        const long long o = row * C + c;
         xq[k] = in ? ld_nc_v4(x + o) : zero;
         rq[k] = (in && has_res) ? ld_nc_v4(residual + o) : zero;
+        sq[k] = (SCALE && in) ? __ldg(sscale + static_cast<unsigned>(row) / rows_per_sample) : 0.f;
       }
 #pragma unroll
       for (int k = 0; k < kRows; ++k) {
@@ -358,6 +449,7 @@ bn_fwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __
           float2 v = ffma2_rn(make_float2(__uint_as_float(xw[j] << 16),
                                             __uint_as_float(xw[j] & 0xffff0000u)),
                                 sc[j], sh[j]);
+          if (SCALE) v = make_float2(__fmul_rn(sq[k], v.x), __fmul_rn(sq[k], v.y));
           if (has_res)
             v = fadd2_rn(v, make_float2(__uint_as_float(rw[j] << 16),
                                           __uint_as_float(rw[j] & 0xffff0000u)));
@@ -372,6 +464,29 @@ bn_fwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __
       }
     }
   }
+}
+
+template <bool FIN>
+__global__ void __launch_bounds__(kThreads, 3)
+bn_fwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ residual,
+                    const float* __restrict__ scale, const float* __restrict__ shift,
+                    __nv_bfloat16* __restrict__ y, uint8_t* __restrict__ mask, long long P, int C,
+                    int act, const BnFinalize fin, const int rev) {
+  bn_fwd_apply_body<FIN, false>(x, residual, scale, shift, y, mask, P, C, act, fin, rev, nullptr,
+                                1u);
+}
+
+// (two resident blocks, as the backward kernels: the scale's registers do not fit three)
+template <bool FIN>
+__global__ void __launch_bounds__(kThreads, 2)
+bn_fwd_apply_scaled_kernel(const __nv_bfloat16* __restrict__ x,
+                           const __nv_bfloat16* __restrict__ residual,
+                           const float* __restrict__ scale, const float* __restrict__ shift,
+                           __nv_bfloat16* __restrict__ y, uint8_t* __restrict__ mask, long long P,
+                           int C, int act, const BnFinalize fin, const int rev,
+                           const float* __restrict__ sscale, unsigned rows_per_sample) {
+  bn_fwd_apply_body<FIN, true>(x, residual, scale, shift, y, mask, P, C, act, fin, rev, sscale,
+                               rows_per_sample);
 }
 
 // L2 hand-over hint (see bn_set_row_reverse in ops.h): the next launches walk the rows from the
@@ -396,13 +511,22 @@ inline dim3 red_grid(long long P, int C, int waves) {
 constexpr int kWavesFwd = 3;
 constexpr int kWavesReduce = 2;
 constexpr int kWavesApply = 2;
+constexpr int kWavesFwdScaled = 2;   // bn_fwd_apply_scaled_kernel: launch bounds 2
 
 }  // namespace
 
 void bn_set_row_reverse(int flag) { g_row_reverse = flag ? 1 : 0; }
 
 cudaError_t bn_apply(const void* x, const void* residual, const float* scale, const float* shift,
-                     void* y, uint8_t* mask, long long P, int C, int act, cudaStream_t s) {
+                     void* y, uint8_t* mask, long long P, int C, int act, cudaStream_t s,
+                     const SampleScale& ss) {
+  if (ss.scale != nullptr) {
+    bn_fwd_apply_scaled_kernel<false><<<red_grid(P, C, kWavesFwdScaled), kThreads, 0, s>>>(
+        static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(residual), scale,
+        shift, static_cast<__nv_bfloat16*>(y), mask, P, C, act, BnFinalize(), g_row_reverse,
+        ss.scale, ss.rows_per_sample);
+    return cudaGetLastError();
+  }
   bn_fwd_apply_kernel<false><<<red_grid(P, C, kWavesFwd), kThreads, 0, s>>>(
       static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(residual), scale,
       shift, static_cast<__nv_bfloat16*>(y), mask, P, C, act, BnFinalize(), g_row_reverse);
@@ -410,7 +534,15 @@ cudaError_t bn_apply(const void* x, const void* residual, const float* scale, co
 }
 
 cudaError_t bn_apply_finalize(const void* x, const void* residual, void* y, uint8_t* mask,
-                              long long P, int C, int act, const BnFinalize& fin, cudaStream_t s) {
+                              long long P, int C, int act, const BnFinalize& fin, cudaStream_t s,
+                              const SampleScale& ss) {
+  if (ss.scale != nullptr) {
+    bn_fwd_apply_scaled_kernel<true><<<red_grid(P, C, kWavesFwdScaled), kThreads, 0, s>>>(
+        static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(residual), nullptr,
+        nullptr, static_cast<__nv_bfloat16*>(y), mask, P, C, act, fin, g_row_reverse, ss.scale,
+        ss.rows_per_sample);
+    return cudaGetLastError();
+  }
   bn_fwd_apply_kernel<true><<<red_grid(P, C, kWavesFwd), kThreads, 0, s>>>(
       static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(residual), nullptr,
       nullptr, static_cast<__nv_bfloat16*>(y), mask, P, C, act, fin, g_row_reverse);
@@ -420,7 +552,14 @@ cudaError_t bn_apply_finalize(const void* x, const void* residual, void* y, uint
 cudaError_t bn_bwd_reduce(const void* dy, const void* x, const void* y, const float* mean,
                           const float* invstd, const float* fscale, const float* fshift,
                           long long P, int C, int relu, float* dgamma, float* dbeta,
-                          cudaStream_t s) {
+                          cudaStream_t s, const SampleScale& ss) {
+  if (ss.scale != nullptr) {
+    bn_bwd_reduce_scaled_kernel<<<red_grid(P, C, kWavesReduce), kThreads, 0, s>>>(
+        static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x),
+        static_cast<const __nv_bfloat16*>(y), mean, invstd, fscale, fshift, P, C, relu, dgamma,
+        dbeta, g_row_reverse, ss.scale, ss.rows_per_sample);
+    return cudaGetLastError();
+  }
   bn_bwd_reduce_kernel<<<red_grid(P, C, kWavesReduce), kThreads, 0, s>>>(
       static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x),
       static_cast<const __nv_bfloat16*>(y), mean, invstd, fscale, fshift, P, C, relu, dgamma,
@@ -433,8 +572,28 @@ cudaError_t bn_bwd_apply(const void* dy, const void* x, const void* y, const flo
                          float* dbeta, const float* fscale, const float* fshift, void* dx,
                          void* dres, long long P, int C, int relu, const float* sum_g,
                          const float* sum_gx, cudaStream_t s, float* acc_dgamma,
-                         float* acc_dbeta) {
+                         float* acc_dbeta, const SampleScale& ss) {
   if ((acc_dgamma == nullptr) != (acc_dbeta == nullptr)) return cudaErrorInvalidValue;
+  const float inv_count = 1.f / static_cast<float>(P);
+  if (ss.scale != nullptr) {
+    // the scaled instances take their dgamma / dbeta from bn_bwd_reduce only
+    if (sum_g != nullptr || sum_gx != nullptr) return cudaErrorInvalidValue;
+    if (acc_dgamma != nullptr) {
+      bn_bwd_apply_acc_scaled_kernel<<<red_grid(P, C, kWavesApply), kThreads, 0, s>>>(
+          static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x),
+          static_cast<const __nv_bfloat16*>(y), gamma, mean, invstd, dgamma, dbeta, fscale,
+          fshift, static_cast<__nv_bfloat16*>(dx), static_cast<__nv_bfloat16*>(dres), P, C, relu,
+          inv_count, g_row_reverse, sum_g, sum_gx, acc_dgamma, acc_dbeta, ss.scale,
+          ss.rows_per_sample);
+      return cudaGetLastError();
+    }
+    bn_bwd_apply_scaled_kernel<<<red_grid(P, C, kWavesApply), kThreads, 0, s>>>(
+        static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x),
+        static_cast<const __nv_bfloat16*>(y), gamma, mean, invstd, dgamma, dbeta, fscale, fshift,
+        static_cast<__nv_bfloat16*>(dx), static_cast<__nv_bfloat16*>(dres), P, C, relu, inv_count,
+        g_row_reverse, sum_g, sum_gx, ss.scale, ss.rows_per_sample);
+    return cudaGetLastError();
+  }
   if (acc_dgamma != nullptr) {
     bn_bwd_apply_acc_kernel<<<red_grid(P, C, kWavesApply), kThreads, 0, s>>>(
         static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x),

@@ -20,8 +20,19 @@ cudaError_t bn_inference_coeffs(const float* gamma, const float* beta, const flo
 // mask (optional): one bit per element, set where the pre-activation value is > 0
 // row order of the following bn_apply / bn_apply_finalize / bn_bwd_* launches: 1 = last row first
 void bn_set_row_reverse(int flag);
+// Stochastic depth (bn_bwd.cu): per-sample factors of a residual branch's last batch norm, fp32
+// scale[N] on the device; row r of the [P, C] tensor is sample r / rows_per_sample (= H * W, and
+// P < 2^31).  scale == nullptr: the plain kernels.  bn_apply / bn_apply_finalize then store
+// act(scale[n] * bn(x) (+ residual)) with the batch statistics of bn(x); bn_bwd_reduce / bn_bwd_apply
+// take g = scale[n] * masked dy as the batch norm's output gradient, and dres (when given) receives
+// the unscaled masked dy.  Not with a fused reduction (sum_g / sum_gx).
+struct SampleScale {
+  const float* scale = nullptr;
+  unsigned rows_per_sample = 1;
+};
 cudaError_t bn_apply(const void* x, const void* residual, const float* scale, const float* shift,
-                     void* y, uint8_t* mask, long long P, int C, int act, cudaStream_t s);
+                     void* y, uint8_t* mask, long long P, int C, int act, cudaStream_t s,
+                     const SampleScale& ss = SampleScale());
 // Same, with the statistics finalisation folded in: every thread derives scale / shift of its
 // channel group from the accumulated (sum, sumsq); one designated thread per group also stores
 // mean / invstd / scale / shift (the backward kernels read them) and updates the running
@@ -41,17 +52,18 @@ struct BnFinalize {
   float count, eps, momentum;
 };
 cudaError_t bn_apply_finalize(const void* x, const void* residual, void* y, uint8_t* mask,
-                              long long P, int C, int act, const BnFinalize& fin, cudaStream_t s);
+                              long long P, int C, int act, const BnFinalize& fin, cudaStream_t s,
+                              const SampleScale& ss = SampleScale());
 cudaError_t bn_bwd_reduce(const void* dy, const void* x, const void* y, const float* mean,
                           const float* invstd, const float* fscale, const float* fshift,
                           long long P, int C, int relu, float* dgamma, float* dbeta,
-                          cudaStream_t s);
+                          cudaStream_t s, const SampleScale& ss = SampleScale());
 cudaError_t bn_bwd_apply(const void* dy, const void* x, const void* y, const float* gamma,
                          const float* mean, const float* invstd, float* dgamma,
                          float* dbeta, const float* fscale, const float* fshift, void* dx,
                          void* dres, long long P, int C, int relu, const float* sum_g,
                          const float* sum_gx, cudaStream_t s, float* acc_dgamma = nullptr,
-                         float* acc_dbeta = nullptr);
+                         float* acc_dbeta = nullptr, const SampleScale& ss = SampleScale());
 cudaError_t add_act(const void* a, const void* b, void* out, long long n, int act, cudaStream_t s);
 cudaError_t relu_bwd(const void* dy, const void* y, void* dx, long long n, cudaStream_t s);
 cudaError_t colsum(const void* x, long long P, int C, float* out, cudaStream_t s);

@@ -57,6 +57,9 @@ def define_flags():
                  help="probability that a step mixes at all, in [0, 1]")
   p.add_argument("--mix_switch_prob", type=float, default=0.5,
                  help="with both alphas > 0: probability that a mixing step is CutMix")
+  p.add_argument("--drop_path_rate", type=float, default=0.0,
+                 help="stochastic depth: the last residual block drops with this rate, block i of "
+                      "N with rate * i / (N - 1) (0: off)")
   return p
 
 
@@ -101,7 +104,7 @@ def main_fun(argv, ctx):
   if args.clip_norm is not None:
     smooth["clip_norm"] = args.clip_norm
   for name, default in (("mixup_alpha", 0.0), ("cutmix_alpha", 0.0), ("mix_prob", 1.0),
-                        ("mix_switch_prob", 0.5)):
+                        ("mix_switch_prob", 0.5), ("drop_path_rate", 0.0)):
     if getattr(args, name) != default:
       smooth[name] = getattr(args, name)
   net = resnet.CifarResNetTrainer(depth=args.resnet_size, batch=B, device=dev, comm=comm,

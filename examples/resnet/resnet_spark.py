@@ -113,6 +113,9 @@ def parse(argv):
                  help="probability that a step mixes at all, in [0, 1]")
   p.add_argument("--mix_switch_prob", type=float, default=0.5,
                  help="with both alphas > 0: probability that a mixing step is CutMix")
+  p.add_argument("--drop_path_rate", type=float, default=0.0,
+                 help="stochastic depth: the last residual block drops with this rate, block i of "
+                      "N with rate * i / (N - 1) (0: off)")
   p.add_argument("--multi_label", action="store_true",
                  help="multi-hot labels and the binary cross-entropy; evaluation reports "
                       "binary_accuracy, exact_match, f1 and macro_f1")
@@ -155,7 +158,7 @@ def main_fun(argv, ctx):
   if args.multi_label:
     opt["multi_label"] = True
   for name, default in (("mixup_alpha", 0.0), ("cutmix_alpha", 0.0), ("mix_prob", 1.0),
-                        ("mix_switch_prob", 0.5)):
+                        ("mix_switch_prob", 0.5), ("drop_path_rate", 0.0)):
     if getattr(args, name) != default:
       opt[name] = getattr(args, name)
   if args.model == "resnet56":

@@ -242,6 +242,50 @@ class MixDraws(object):
     return [float(MIX_MODES.index(mode)), float(lam)] + [float(v) for v in box] + [0.0, 0.0]
 
 
+def check_drop_path_rate(r=0.0, training=True):
+  """Validated ``drop_path_rate`` of a trainer as a float: a real, finite r with 0 <= r < 1
+  (ValueError otherwise, for bools, and for r != 0 with ``training=False``: an inference-only
+  trainer never drops)."""
+  if isinstance(r, bool) or not isinstance(r, numbers.Real) or not math.isfinite(float(r)) \
+      or not 0.0 <= float(r) < 1.0:
+    raise ValueError("drop_path_rate must be a real number in [0, 1), got {!r}".format(r))
+  if float(r) and not training:
+    raise ValueError("drop_path_rate needs training=True (an inference-only trainer never drops)")
+  return float(r)
+
+
+def drop_path_rates(r, n_blocks):
+  """timm's linear decay of the stochastic-depth rate over the residual blocks of a network:
+  block i of N (0-based) drops with p_i = r * i / (N - 1), so block 0 never drops and the last one
+  drops at r.  (Huang et al. use p_l = r * l / L with l from 1, which drops the first block too.)"""
+  if n_blocks < 2:
+    return (0.0,) * n_blocks
+  return tuple(r * i / (n_blocks - 1) for i in range(n_blocks))
+
+
+class DropPathDraws(object):
+  """The per-step stochastic-depth draw of a trainer (timm's ``DropPath(scale_by_keep=True)``),
+  from its own ``numpy.random.Generator`` seeded with ``(seed, rank, 1)``: a stream apart from
+  MixDraws' ``(seed, rank)``, so that turning drop path on leaves a mixing trainer's mix draws as
+  they were.
+
+  ``draw()`` returns float32 [n_blocks, B]: row i holds each sample's factor s_b for block i,
+  ``keep_b / (1 - p_i)`` with keep_b ~ Bernoulli(1 - p_i) (0, or 1 / (1 - p_i) rounded to fp32).
+  Rows of blocks with p_i = 0 are all ones and draw nothing."""
+
+  def __init__(self, rates, B, seed=0, rank=0):
+    self.rates, self.B = tuple(float(p) for p in rates), int(B)
+    self.rng = np.random.default_rng([int(seed), int(rank), 1])
+
+  def draw(self):
+    out = np.ones((len(self.rates), self.B), dtype=np.float32)
+    for i, p in enumerate(self.rates):
+      if p > 0:
+        keep = self.rng.random(self.B) < 1.0 - p
+        out[i] = np.where(keep, np.float32(1.0 / (1.0 - p)), np.float32(0.0))
+    return out
+
+
 class GradAccumulation(object):
   """The update window of a trainer with ``gradient_accumulation_steps`` k (Keras's
   ``gradient_accumulation_steps``): ``train_step`` call i of a window is micro-step
@@ -275,7 +319,8 @@ class GradAccumulation(object):
     max(2, k) micro-steps eagerly on a side stream (two steps with k = 1, as before accumulation;
     with k > 1 every position of the window once), then each phase is captured.
     ``before_step``: called on the side stream before each warm-up step, as ``train_step`` does
-    before a step (the Mixup / CutMix draw and its staging); never inside a capture."""
+    before a step (the Mixup / CutMix and drop-path draws and their staging); never inside a
+    capture."""
     s = torch.cuda.Stream(device=device)
     s.wait_stream(torch.cuda.current_stream(device))
     with torch.cuda.stream(s):
@@ -432,10 +477,13 @@ class BatchNorm(object):
   def stats(self):
     return (self.sum, self.sumsq)
 
-  def forward(self, x_raw, y, residual=None, act=1, training=True, rev=False):
+  def forward(self, x_raw, y, residual=None, act=1, training=True, rev=False, sample_scale=None):
     """``rev``: walk the rows last-to-first.  The convolution that produced ``x_raw`` wrote its
     tiles first-to-last, so the END of the tensor is what the 50 MB L2 still holds; the apply
-    kernel then finishes at the START of ``y``, which is where the next convolution begins."""
+    kernel then finishes at the START of ``y``, which is where the next convolution begins.
+    ``sample_scale`` (stochastic depth; fp32 [N] on the device): y = act(s[n] bn(x) (+ residual)),
+    with the batch and running statistics of bn(x) over the whole batch."""
+    ss = {} if sample_scale is None else {"sample_scale": sample_scale}
     count = x_raw.numel() // self.C
     ops.C().bn_set_row_reverse(bool(rev))
     # a residual unit's ReLU mask depends on the sum, not on x alone: keep it as one bit per
@@ -451,7 +499,7 @@ class BatchNorm(object):
       ops.K.bn_apply_finalize(x_raw, residual, y, act, self.mask, self.sum, self.sumsq, self.gamma,
                               self.beta, self.running_mean, self.running_var, self.mean,
                               self.invstd, self.scale, self.shift, float(count), self.eps,
-                              self.momentum)
+                              self.momentum, **ss)
       return
     if training:
       ops.K.bn_finalize(self.sum, self.sumsq, self.gamma, self.beta, self.running_mean,
@@ -460,7 +508,7 @@ class BatchNorm(object):
     else:
       ops.K.bn_inference_coeffs(self.gamma, self.beta, self.running_mean, self.running_var,
                                 self.scale, self.shift, self.eps)
-    ops.K.bn_apply(x_raw, residual, self.scale, self.shift, y, act, self.mask)
+    ops.K.bn_apply(x_raw, residual, self.scale, self.shift, y, act, self.mask, **ss)
 
   def ensure_mask(self, numel, device):
     """The unit's ReLU bit mask buffer (numel / 8 bytes), allocated once."""
@@ -470,11 +518,15 @@ class BatchNorm(object):
     return buf
 
   def backward(self, dy, x_raw, y, dx, dres=None, relu=True, residual=False, mask=None,
-               rev=(False, False)):
+               rev=(False, False), sample_scale=None):
     """relu mask: recomputed from x_raw with the forward scale/shift when the unit has no
     residual input (saves reading y: 2 of 6-8 bytes per element); from the stored y otherwise;
     ``mask``: another unit's bit mask (a projection shortcut's BN sees the gradient of the block
-    output, i.e. the ReLU that followed the *sum*)."""
+    output, i.e. the ReLU that followed the *sum*).  ``sample_scale``: the forward's stochastic-depth
+    factors; the batch norm's output gradient is then s[n] * the masked dy (``dres`` still gets
+    the unscaled one), and the reduction runs as its own pass - it cannot be fused into a data
+    gradient's epilogue."""
+    ss = {} if sample_scale is None else {"sample_scale": sample_scale}
     mode = 0 if not relu else (1 if (residual or dres is not None) else 2)
     ysrc = y if mode == 1 else None
     if mask is not None and relu:
@@ -486,6 +538,9 @@ class BatchNorm(object):
     dg, db = self.acc if self.acc is not None else (self.dgamma, self.dbeta)
     acc = {} if self.acc is None else {"acc_dgamma": self.dgamma, "acc_dbeta": self.dbeta}
     if getattr(self, "fused_reduce", False):
+      if ss:
+        raise ValueError("{}: sample_scale needs the unfused backward reduction (build the data "
+                         "gradient that writes dy without dx_bn_reduce)".format(self.name))
       # sum(g), sum(g x) were accumulated by the epilogue of the data gradient that wrote dy
       # (ops/igemm.conv_dgrad(bn_reduce=...)): no reduction pass, the apply kernel finishes them
       ops.C().bn_set_row_reverse(bool(rev[1]))
@@ -497,10 +552,10 @@ class BatchNorm(object):
     # stopped, so that what it reads first is still in L2 (ResNetTrainer assigns the directions)
     ops.C().bn_set_row_reverse(bool(rev[0]))
     ops.K.bn_bwd_reduce(dy, x_raw, ysrc, self.mean, self.invstd, dg, db, mode, self.scale,
-                        self.shift)
+                        self.shift, **ss)
     ops.C().bn_set_row_reverse(bool(rev[1]))
     ops.K.bn_bwd_apply(dy, x_raw, ysrc, self.gamma, self.mean, self.invstd, dg, db, dx, dres,
-                       mode, self.scale, self.shift, **acc)
+                       mode, self.scale, self.shift, **acc, **ss)
     ops.C().bn_set_row_reverse(False)
 
 

@@ -293,7 +293,8 @@ class ResNetTrainer(object):
                optimizer="momentum", trust_coefficient=0.001, label_smoothing=0.0,
                ema_decay=None, clip_norm=None, beta1=0.9, beta2=0.999, epsilon=1e-7,
                gradient_accumulation_steps=1, multi_label=False, pos_weight=None,
-               mixup_alpha=0.0, cutmix_alpha=0.0, mix_prob=1.0, mix_switch_prob=0.5):
+               mixup_alpha=0.0, cutmix_alpha=0.0, mix_prob=1.0, mix_switch_prob=0.5,
+               drop_path_rate=0.0):
     """``optimizer``: sgd | momentum | adam | adamw | lars | lamb (``trust_coefficient`` is LARS's
     eta; see parallel/fused_optim.py).  adam folds ``weight_decay`` into the gradient (L2), adamw
     decouples it (``torch.optim.AdamW``), lamb is layer-wise adaptive Adam (apex ``FusedLAMB``).
@@ -346,12 +347,25 @@ class ResNetTrainer(object):
     probability that a step mixes at all; ``mix_switch_prob`` (in [0, 1]): with both alphas > 0,
     the probability that a mixing step is CutMix.  ``correct`` then counts hits against the
     dominant sample (the row's own label when lam >= 0.5, its partner's otherwise).  Evaluation,
-    serving and exports never mix."""
+    serving and exports never mix.
+
+    ``drop_path_rate`` (r in [0, 1); training only): stochastic depth as timm's
+    ``DropPath(scale_by_keep=True)`` in its ``Bottleneck``: block i of the N residual blocks
+    drops with p_i = r * i / (N - 1) (timm's linear decay; ``drop_path_rates`` holds them), and
+    each sample's residual branch output is multiplied by s_b = keep_b / (1 - p_i),
+    keep_b ~ Bernoulli(1 - p_i), before the shortcut is added: out = relu(s_b bn3(conv3(..)) +
+    shortcut).  bn3's batch and running statistics are those of the whole batch, the shortcut
+    (identity or projection) is never dropped, and the branch's gradient is s_b times the block
+    output's.  Each ``train_step`` call (each micro-step, each warm-up step of ``capture()``)
+    draws the factors of every block on the host (engine.DropPathDraws, seeded with (``seed``,
+    rank, 1)); ``last_drop_path`` holds the last draw.  Evaluation, serving, ``averaged()`` and
+    exports never drop."""
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     self.multi_label, pos_weight = _check_multilabel_args(multi_label, pos_weight, num_classes,
                                                           training)
     mix_args = engine.check_mix_args(mixup_alpha, cutmix_alpha, mix_prob, mix_switch_prob,
                                      training)
+    self.drop_path_rate = engine.check_drop_path_rate(drop_path_rate, training)
     k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps, training)
     self.ema_decay = engine.check_ema_decay(ema_decay, training)
     self.clip_norm = engine.check_clip_norm(clip_norm, training)
@@ -387,6 +401,7 @@ class ResNetTrainer(object):
     self.fc = Dense(st, "fc", cin, VP, bias=True,
                     init=normal(0.01) if VP == num_classes else _padded_head_init(num_classes))
     self.feat = cin
+    self.drop_path_rates = engine.drop_path_rates(self.drop_path_rate, len(self.blocks))
 
     alloc = comm.alloc if comm is not None else None
     st.finalize(dev, alloc=alloc, seed=seed)
@@ -423,7 +438,8 @@ class ResNetTrainer(object):
     prev_block = None
     gx = _buf(x.shape, dev) if tr else None  # gradient wrt the block input
     self.g_pool = gx
-    for b in self.blocks:
+    for b, p in zip(self.blocks, self.drop_path_rates):
+      b.drop_path = p
       s = b.stride
       H2, W2 = (H - 1) // s + 1, (W - 1) // s + 1
       w, c4 = b.width, b.width * 4
@@ -454,7 +470,8 @@ class ResNetTrainer(object):
       red1 = (b.u1.bn, b.r1, b.u1.bn.ensure_mask(b.a1.numel(), dev)) if tr else None
       red2 = (b.u2.bn, b.r2, b.u2.bn.ensure_mask(b.a2.numel(), dev)) if tr else None
       redp = None
-      if tr and ident and prev_block is not None:
+      # (a block that drops scales its bn3's gradient per sample: that reduction stays unfused)
+      if tr and ident and prev_block is not None and not prev_block.drop_path:
         redp = (prev_block.u3.bn, prev_block.r3, prev_block.u3.bn.ensure_mask(
             prev_block.out.numel(), dev))
       b.u1.conv.build(x, b.r1, b.g_r1, b.g_x, stats=b.u1.bn.stats, dx_accumulate=ident,
@@ -497,6 +514,7 @@ class ResNetTrainer(object):
           bn.accumulate_grads(None)   # every one has its arena slots or a fused reduction
     self.accum = engine.GradAccumulation(k_acc)
     self._build_mix(mix_args, seed)
+    self._build_drop_path(seed)
     self.graph = None
     self.graphs = None
     self.mean = [0.485, 0.456, 0.406]
@@ -529,6 +547,34 @@ class ResNetTrainer(object):
     """The ``mix`` keyword of the training decode and loss: none when the trainer does not mix,
     so such a trainer launches exactly what it did before mixing existed."""
     return {} if self.mix is None else {"mix": self.mix}
+
+  def _build_drop_path(self, seed):
+    """Stochastic-depth state: the host draws (engine.DropPathDraws) and the device tensor
+    ``drop_scale`` [n_blocks, B] each step's factors are staged into; neither exists when
+    ``drop_path_rate`` is 0."""
+    self.dropper = self.drop_scale = self.last_drop_path = None
+    if self.drop_path_rate > 0:
+      rank = self.comm.rank if self.comm is not None else 0
+      self.dropper = engine.DropPathDraws(self.drop_path_rates, self.B, seed=seed, rank=rank)
+      self.drop_scale = torch.ones((len(self.blocks), self.B), dtype=torch.float32,
+                                   device=self.device)
+
+  def _stage_draws(self):
+    """Draw this step's mix and drop-path factors on the host and copy them into ``mix`` and
+    ``drop_scale`` on the current stream, ahead of the step's kernels (never inside a graph
+    capture).  Each source is a fresh pageable tensor: the copy takes the values before it
+    returns, so the host never waits and never overwrites what a queued copy still reads."""
+    self._stage_mix()
+    if self.dropper is not None:
+      self.last_drop_path = self.dropper.draw()
+      self.drop_scale.copy_(torch.from_numpy(self.last_drop_path.copy()), non_blocking=True)
+
+  def _drop_arg(self, i):
+    """The ``sample_scale`` keyword of block i's last batch norm: none when the block never
+    drops, so a trainer without drop path launches exactly what it did before."""
+    if self.drop_scale is None or not self.drop_path_rates[i]:
+      return {}
+    return {"sample_scale": self.drop_scale[i]}
 
   def _batch_norms(self):
     return [self.stem_bn] + [u.bn for b in self.blocks
@@ -630,7 +676,7 @@ class ResNetTrainer(object):
     ``gradient_accumulation_steps`` > 1 it is the first micro-step of a window (broadcast and
     accumulate, no update)."""
     comm = self.comm
-    self._stage_mix()
+    self._stage_draws()
     comm.broadcast("aux32", self._root)  # BN scale/offset + biases: tiny, consumed in fp32
     comm.barrier()                        # root's weights are final and visible
     main = torch.cuda.current_stream(self.device)
@@ -668,7 +714,7 @@ class ResNetTrainer(object):
     else:
       self.stem_bn.forward(self.stem_raw, self.stem_act, None, 1, training)
       K.maxpool_fwd(self.stem_act, self.pool, self.pool_idx, 3, 2, 1)
-    for b in self.blocks:
+    for bi, b in enumerate(self.blocks):
       for u, raw, act in ((b.u1, b.r1, b.a1), (b.u2, b.r2, b.a2)):
         run(u.conv)
         u.bn.forward(raw, act, None, 1, training, rev=True)
@@ -679,7 +725,8 @@ class ResNetTrainer(object):
         idn = b.idn
       else:
         idn = b.x
-      b.u3.bn.forward(b.r3, b.out, idn, 1, training, rev=True)
+      b.u3.bn.forward(b.r3, b.out, idn, 1, training, rev=True,
+                      **(self._drop_arg(bi) if training else {}))
     K.avgpool_fwd(self.last, self.avg)
     run(self.fc)
 
@@ -710,7 +757,9 @@ class ResNetTrainer(object):
       b = self.blocks[bi]
       # out = relu(bn3(r3) + idn): the masked gradient goes to both branches; the mask is applied
       # where g_out is consumed (here, in conv1's accumulate epilogue, in the shortcut's BN)
-      b.u3.bn.backward(b.g_out, b.r3, b.out, b.g_r3, relu=True, residual=True, rev=b.u3.rev)
+      # stochastic depth: bn3 sees s_b * the masked gradient, the shortcut the unscaled one
+      b.u3.bn.backward(b.g_out, b.r3, b.out, b.g_r3, relu=True, residual=True, rev=b.u3.rev,
+                       **self._drop_arg(bi))
       b.u3.conv.backward()
       b.u2.bn.backward(b.g_a2, b.r2, b.a2, b.g_r2, relu=True, rev=b.u2.rev)
       b.u2.conv.backward()
@@ -755,16 +804,18 @@ class ResNetTrainer(object):
     # defers them), but the process group's watchdog thread may still poll events of the warm-up
     # collectives - thread-local capture keeps that from invalidating the capture
     mode = "thread_local" if getattr(self.optim, "group_mode", False) else "global"
-    # the warm-up steps draw and stage their mix as train_step does; the graphs read ``mix``
+    # the warm-up steps draw and stage their mix and drop-path factors as train_step does; the
+    # graphs read ``mix`` and ``drop_scale``
+    draws = self.mixer is not None or self.dropper is not None
     self.graphs = self.accum.capture(self.device, self.step_kernels, mode,
-                                     before_step=self._stage_mix if self.mixer else None)
+                                     before_step=self._stage_draws if draws else None)
     self.graph = self.graphs[(self.accum.k == 1, True)]
     return self.graph
 
   def train_step(self, images_u8=None, labels=None):
     if images_u8 is not None:
       self.set_input(images_u8, labels)
-    self._stage_mix()
+    self._stage_draws()
     # a captured step replays its graph; after the updating one a cross-host communicator runs
     # its all-reduce + update outside the graph (after_replay)
     self.accum.run(self.graphs if self.graph is not None else None, self.step_kernels, self.optim)
@@ -1051,18 +1102,20 @@ class CifarResNetTrainer(object):
   momentum SGD, batch 128, weight decay 2e-4).  ``optimizer``, ``num_classes``,
   ``label_smoothing``, ``ema_decay``, ``clip_norm``, ``beta1``, ``beta2``, ``epsilon``,
   ``gradient_accumulation_steps``, ``multi_label``, ``pos_weight``, ``mixup_alpha``,
-  ``cutmix_alpha``, ``mix_prob`` and ``mix_switch_prob`` as in ResNetTrainer (the CutMix box is
-  drawn on the 32 x 32 image)."""
+  ``cutmix_alpha``, ``mix_prob``, ``mix_switch_prob`` and ``drop_path_rate`` as in ResNetTrainer
+  (the CutMix box is drawn on the 32 x 32 image; stochastic depth scales the output of each basic
+  block's second batch norm, as in timm's ``BasicBlock``)."""
 
   def __init__(self, depth=56, batch=128, num_classes=10, device="cuda:0", lr=0.1, momentum=0.9,
                weight_decay=2e-4, comm=None, seed=1234, optimizer="momentum",
                trust_coefficient=0.001, label_smoothing=0.0, ema_decay=None, clip_norm=None,
                beta1=0.9, beta2=0.999, epsilon=1e-7, gradient_accumulation_steps=1,
                multi_label=False, pos_weight=None, mixup_alpha=0.0, cutmix_alpha=0.0, mix_prob=1.0,
-               mix_switch_prob=0.5):
+               mix_switch_prob=0.5, drop_path_rate=0.0):
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     self.multi_label, pos_weight = _check_multilabel_args(multi_label, pos_weight, num_classes)
     mix_args = engine.check_mix_args(mixup_alpha, cutmix_alpha, mix_prob, mix_switch_prob)
+    self.drop_path_rate = engine.check_drop_path_rate(drop_path_rate)
     k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps)
     self.ema_decay = engine.check_ema_decay(ema_decay)
     self.clip_norm = engine.check_clip_norm(clip_norm)
@@ -1090,6 +1143,7 @@ class CifarResNetTrainer(object):
         self.blocks.append(b)
         cin = width
     self.fc = Dense(st, "fc", 64, self.VP, bias=True, init=normal(0.01))
+    self.drop_path_rates = engine.drop_path_rates(self.drop_path_rate, len(self.blocks))
     st.finalize(dev, alloc=comm.alloc if comm is not None else None, seed=seed)
 
     self.in_u8 = _buf((B, 32, 32, 3), dev, torch.uint8)
@@ -1145,6 +1199,7 @@ class CifarResNetTrainer(object):
         bn.accumulate_grads(self.grad_scratch)
     self.accum = engine.GradAccumulation(k_acc)
     self._build_mix(mix_args, seed)
+    self._build_drop_path(seed)
     self.graph = None
     self.graphs = None
     self.mean, self.std = [0.4914, 0.4822, 0.4465], [0.2470, 0.2435, 0.2616]
@@ -1171,6 +1226,9 @@ class CifarResNetTrainer(object):
   _build_mix = ResNetTrainer._build_mix
   _stage_mix = ResNetTrainer._stage_mix
   _mix_arg = ResNetTrainer._mix_arg
+  _build_drop_path = ResNetTrainer._build_drop_path
+  _stage_draws = ResNetTrainer._stage_draws
+  _drop_arg = ResNetTrainer._drop_arg
 
   def _fold_units(self):
     """(filter spec, batch norm) of every convolution followed by a batch norm, stem first."""
@@ -1211,14 +1269,15 @@ class CifarResNetTrainer(object):
     K.decode_normalize(self.in_u8, self.x8, 0, self.mean, self.std, **self._mix_arg())
     self.stem.conv.forward()
     self.stem.bn.forward(self.stem_raw, self.stem_act, None, 1, True)
-    for b in self.blocks:
+    for bi, b in enumerate(self.blocks):
       b.u1.conv.forward()
       b.u1.bn.forward(b.r1, b.a1, None, 1, True)
       b.u2.conv.forward()
       if b.ds is not None:
         b.ds.conv.forward()
         b.ds.bn.forward(b.rd, b.idn, None, 0, True)
-      b.u2.bn.forward(b.r2, b.out, b.idn if b.ds is not None else b.x, 1, True)
+      b.u2.bn.forward(b.r2, b.out, b.idn if b.ds is not None else b.x, 1, True,
+                      **self._drop_arg(bi))
     K.avgpool_fwd(self.last, self.avg)
     self.fc.forward()
     self._loss(True)
@@ -1228,8 +1287,11 @@ class CifarResNetTrainer(object):
       self.grad_scratch.zero()
     self.fc.backward()
     K.avgpool_bwd(self.g_avg, self.g_last)
-    for b in reversed(self.blocks):
-      b.u2.bn.backward(b.g_out, b.r2, b.out, b.g_r2, dres=b.g_out, relu=True)
+    for bi in reversed(range(len(self.blocks))):
+      b = self.blocks[bi]
+      # stochastic depth: u2's dx is formed from s_b * the masked gradient; dres (the shortcut's,
+      # written in place into g_out) stays unscaled
+      b.u2.bn.backward(b.g_out, b.r2, b.out, b.g_r2, dres=b.g_out, relu=True, **self._drop_arg(bi))
       b.u2.conv.backward()
       b.u1.bn.backward(b.g_a1, b.r1, b.a1, b.g_r1, relu=True)
       b.u1.conv.backward()
