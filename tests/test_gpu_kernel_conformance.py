@@ -279,28 +279,11 @@ def _stats_inputs(gen, x, C):
 def _check_finalize(s_sum, s_sq, gam, bet, rm0, rv0, rm, rv, mean, invstd, scale, shift, cnt,
                     eps, mom, what):
   """The bounds of the plan conformance suite's bn_apply_finalize check."""
-  import torch
-  m64 = _f64(s_sum) / cnt
-  ex2 = _f64(s_sq) / cnt
-  var = (ex2 - m64 * m64).clamp_min(0)
-  is64 = 1.0 / torch.sqrt(var + eps)
-  e_var = pc.gamma(10, U) * (ex2 + m64 * m64)
-  rel_is = 0.5 * e_var / (var + eps) + 5 * U
-  pc.check_close(mean, m64, 4 * U * m64.abs(), what + " mean")
-  pc.check_close(invstd, is64, rel_is * is64, what + " invstd")
-  sc64 = _f64(gam) * is64
-  pc.check_close(scale, sc64, (rel_is + 2 * U) * sc64.abs(), what + " scale")
-  sh64 = _f64(bet) - m64 * sc64
-  pc.check_close(shift, sh64, (rel_is + 8 * U) * (m64 * sc64).abs() + 2 * U * sh64.abs(),
-                 what + " shift")
-  rm0, rv0 = _f64(rm0), _f64(rv0)
-  pc.check_close(rm, (1 - mom) * rm0 + mom * m64,
-                 pc.gamma(8, U) * ((1 - mom) * rm0.abs() + mom * m64.abs()), what + " running_mean")
-  unb = var * cnt / (cnt - 1) if cnt > 1 else var
-  fac = cnt / (cnt - 1) if cnt > 1 else 1.0
-  pc.check_close(rv, (1 - mom) * rv0 + mom * unb,
-                 pc.gamma(10, U) * ((1 - mom) * rv0.abs() + mom * unb) +
-                 mom * (e_var + U * var) * fac, what + " running_var")
+  refs = pc.bn_finalize_refs(_f64(s_sum), _f64(s_sq), _f64(gam), _f64(bet), _f64(rm0),
+                             _f64(rv0), cnt, eps, mom, U)
+  for name, got in (("mean", mean), ("invstd", invstd), ("scale", scale), ("shift", shift),
+                    ("running_mean", rm), ("running_var", rv)):
+    pc.check_close(got, refs[name][0], refs[name][1], what + " " + name)
 
 
 def check_stem_fwd(N, H, W, C, what, eps=1e-3, mom=0.01, compare_unfused=True):
@@ -373,13 +356,7 @@ def check_stem_bwd(N, H, W, C, what, runs=2, accumulate=False):
   xm = x64 - _f64(mean)
   is64 = _f64(invstd)
   P = N * H * W
-  # a thread's chain: 4 pixels per grid-stride iteration (each pixel up to 4 routed terms), the
-  # block's threads of one channel group in shared memory, one atomic per block
-  groups = C // 8
-  threads = N * (((H + 1) // 2 + 3) // 4) * (((W + 1) // 2 + 7) // 8) * 32 * groups
-  grid = max(1, min(-(-threads // 256), SMS * 8))
-  depth = 4 * -(-threads // (grid * 256)) + 4 + 256 // groups + grid + 3
-  gp = pc.gamma_prob(depth)
+  gp = pc.gamma_prob(kc.stem_bwd_depth(N, H, W, C, SMS))
   dg_ref = (g * xm).reshape(-1, C).sum(0) * is64
   dg_bnd = gp * (gm * xm.abs()).reshape(-1, C).sum(0) * is64 + \
       (gmag * amb * xm.abs()).reshape(-1, C).sum(0) * is64

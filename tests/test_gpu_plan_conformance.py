@@ -887,48 +887,20 @@ def _check_k(op, spec, kwspec, rev, alias, what):
     saved = [t.clone() if isinstance(t, torch.Tensor) else t for t in a]
     _run_k(op, a, rev)
     if op == "bn_apply_finalize":
-      cnt = count
-      m64 = _f64(s_sum) / cnt
-      ex2 = _f64(s_sq) / cnt
-      var = (ex2 - m64 * m64).clamp_min(0)
-      is64 = 1.0 / torch.sqrt(var + eps)
-      # the extension is built with --use_fast_math: an fp32 division is within 2 ulp (4 u), a
-      # multiply or add within u, rsqrtf within 2 ulp
-      e_var = pc.gamma(10, u) * (ex2 + m64 * m64)
-      rel_is = 0.5 * e_var / (var + eps) + 5 * u
-      pc.check_close(mean, m64, 4 * u * m64.abs(), what + " mean")
-      pc.check_close(invstd, is64, rel_is * is64, what + " invstd")
-      sc64 = _f64(gam) * is64
-      pc.check_close(scale, sc64, (rel_is + 2 * u) * sc64.abs(), what + " scale")
-      sh64 = _f64(bet) - m64 * sc64
-      pc.check_close(shift, sh64, (rel_is + 8 * u) * (m64 * sc64).abs() + 2 * u * sh64.abs(),
-                     what + " shift")
-      rm0, rv0 = _f64(saved[9]), _f64(saved[10])
-      pc.check_close(rm, (1 - mom) * rm0 + mom * m64,
-                     pc.gamma(8, u) * ((1 - mom) * rm0.abs() + mom * m64.abs()),
-                     what + " running_mean")
-      unb = var * cnt / (cnt - 1)
-      pc.check_close(rv, (1 - mom) * rv0 + mom * unb,
-                     pc.gamma(10, u) * ((1 - mom) * rv0.abs() + mom * unb) +
-                     mom * (e_var + u * var) * cnt / (cnt - 1), what + " running_var")
+      refs = pc.bn_finalize_refs(_f64(s_sum), _f64(s_sq), _f64(gam), _f64(bet), _f64(saved[9]),
+                                 _f64(saved[10]), count, eps, mom)
+      for name, got in (("mean", mean), ("invstd", invstd), ("scale", scale), ("shift", shift),
+                        ("running_mean", rm), ("running_var", rv)):
+        pc.check_close(got, refs[name][0], refs[name][1], what + " " + name)
     Cn = x.shape[-1]
-    sc, sh = _f64(scale), _f64(shift)
-    xs = _f64(x).reshape(-1, Cn) * sc
-    pre = xs + sh
-    Mv = xs.abs() + sh.abs()
-    if res is not None:
-      r64 = _f64(res).reshape(-1, Cn)
-      pre = pre + r64
-      Mv = Mv + r64.abs()
-    ref = _act(pre, act)
-    # one fma and one add in fp32, then the bf16 rounding
-    bound = pc.U_BF16 * ref.abs() + (1 + pc.U_BF16) * pc.gamma(2, u) * Mv
+    ref, bound, pre, amb = pc.bn_apply_ref(_f64(x).reshape(-1, Cn), _f64(scale), _f64(shift),
+                                           _f64(res).reshape(-1, Cn) if res is not None else None,
+                                           act)
     pc.check_close(yv.reshape(-1, Cn), ref, bound, what + " y")
     assert pc.guard_intact(yv, yb), what + ": y guard band"
     if mask is not None:
       assert pc.guard_intact(mv, mb), what + ": mask guard band"
       bits = _bits_of(mv, pre.shape[0], Cn)
-      amb = pre.abs() <= pc.gamma(2, u) * Mv
       bad = (bits != (pre > 0)) & ~amb
       assert not bool(bad.any()), "{}: {} mask bits wrong".format(what, int(bad.sum()))
     outs = [yv.clone()] + ([mv.clone()] if mask is not None else [])
@@ -977,17 +949,12 @@ def _check_k(op, spec, kwspec, rev, alias, what):
       a[5], a[6] = dgv, dbv
       d0, b0 = _f64(dgam), _f64(dbet)
       _run_k(op, a, rev)
-      namb = g.abs() * amb
-      ref_g = d0 + (g * xm).sum(0) * is64
       # fp32 round-to-nearest along bn_bwd_reduce_kernel's tree, plus x - mean and the invstd
       # product for dgamma
-      depth = pc.red_grid_depth(P, Cn, 2)
-      bnd = pc.gamma_prob(depth + 2) * (d0.abs() + (g.abs() * xm.abs()).sum(0) * is64) + \
-          (dy64.abs() * amb * xm.abs()).sum(0) * is64
-      pc.check_close(dgv, ref_g, bnd, what + " dgamma")
-      pc.check_close(dbv, b0 + g.sum(0), pc.gamma_prob(depth) * (b0.abs() + g.abs().sum(0)) +
-                     (dy64.abs() * amb).sum(0), what + " dbeta")
-      del namb
+      (ref_g, bnd_g), (ref_b, bnd_b) = pc.bn_bwd_reduce_refs(
+          g, xm, is64, pc.red_grid_depth(P, Cn, 2), d0, b0, amb_mag=dy64.abs() * amb)
+      pc.check_close(dgv, ref_g, bnd_g, what + " dgamma")
+      pc.check_close(dbv, ref_b, bnd_b, what + " dbeta")
       assert pc.guard_intact(dgv, dgb) and pc.guard_intact(dbv, dbb), what + ": guard band"
       return
     acc = None
@@ -1022,10 +989,8 @@ def _check_k(op, spec, kwspec, rev, alias, what):
     if sum_g is not None:
       db = _f64(sum_g)
       assert torch.equal(dbet, sum_g), what + ": dbeta differs from sum_g"
-      dg_ref = is64 * (_f64(sum_gx) - _f64(mean) * db)
-      pc.check_close(dgam, dg_ref, pc.gamma(3, u) * is64 * (_f64(sum_gx).abs() +
-                                                            (_f64(mean) * db).abs()),
-                     what + " dgamma")
+      dg_ref, dg_bnd = pc.bn_bwd_fused_dgamma_ref(db, _f64(sum_gx), _f64(mean), is64)
+      pc.check_close(dgam, dg_ref, dg_bnd, what + " dgamma")
       dg = _f64(dgam)
     else:
       dg, db = _f64(dgam), _f64(dbet)
@@ -1036,12 +1001,7 @@ def _check_k(op, spec, kwspec, rev, alias, what):
       for (t, bk), a0, v, name in zip(accv, acc, (dgam, dbet), ("acc_dgamma", "acc_dbeta")):
         kc.check_accumulated(t, a0, v, what + " " + name)
         assert pc.guard_intact(t, bk), what + ": " + name + " guard band"
-    A = _f64(gam) * is64
-    ref = A * (g - db / P - xm * is64 * dg / P)
-    Mv = (A * g).abs() + (A * is64 * dg / P).abs() * (x64.abs() + _f64(mean).abs()) + \
-        (A * db / P).abs()
-    bound = pc.U_BF16 * ref.abs() + (1 + pc.U_BF16) * pc.gamma(10, u) * Mv
-    bound = torch.where(amb, torch.full_like(bound, float("inf")), bound)
+    ref, bound = pc.bn_bwd_dx_ref(g, x64, _f64(gam), _f64(mean), is64, dg, db, amb)
     pc.check_close(dxv.reshape(-1, Cn), ref, bound, what + " dx")
     assert pc.guard_intact(dxv, dxb), what + ": dx guard band"
     if dresv is not None:

@@ -120,6 +120,17 @@ def relu_mask(x, scale, shift, u=2.0 ** -24):
   return pre > 0, pre.abs() <= 2 * u * (xs.abs() + shift.abs())
 
 
+def stem_bwd_depth(N, H, W, C, sms=132):
+  """Roundings of one pixel's term in stem_pool_bn_bwd's dgamma / dbeta sums over an N x H x W
+  x C stem output: a thread's chain of 4 pixels per grid-stride iteration (each pixel up to 4
+  routed terms), the block's threads of one channel group in shared memory, one atomic per
+  block (the grid is capped at 8 blocks per SM)."""
+  groups = C // 8
+  threads = N * (((H + 1) // 2 + 3) // 4) * (((W + 1) // 2 + 7) // 8) * 32 * groups
+  grid = max(1, min(-(-threads // 256), sms * 8))
+  return 4 * -(-threads // (grid * 256)) + 4 + 256 // groups + grid + 3
+
+
 def avgpool_ref(x):
   """(mean over the pixels, mean of magnitudes) of x [N, HW..., C] per image and channel."""
   N, C = x.shape[0], x.shape[-1]

@@ -199,6 +199,104 @@ def check_no_bias(out, ref, M, n, what, u_out=U_BF16, tol=0.25):
   return mean, cnt
 
 
+# ------------------------------------------------------------------ batch norm
+# Bounds of the batch-norm kernels (csrc/bn_bwd.cu, csrc/elementwise.cu), shared by the plan
+# suite's replays and the step suite (tools/step_conformance.py).  Everything is float64; per-
+# channel vectors are [C], per-element tensors [P, C].  The extension is built with
+# --use_fast_math: an fp32 division is within 2 ulp (4 u), a multiply or add within u, rsqrtf
+# within 2 ulp.
+def bn_finalize_refs(s_sum, s_sq, gam, bet, rm0, rv0, cnt, eps, mom, u=U_FP32):
+  """{output: (float64 reference, bound)} of the statistics finalisation (bn_apply_finalize,
+  bn_finalize, the fused stem) from the fp32 sums it read, the parameters and the running
+  statistics before the launch."""
+  m64 = s_sum / cnt
+  ex2 = s_sq / cnt
+  var = (ex2 - m64 * m64).clamp_min(0)
+  is64 = 1.0 / torch.sqrt(var + eps)
+  e_var = gamma(10, u) * (ex2 + m64 * m64)
+  rel_is = 0.5 * e_var / (var + eps) + 5 * u
+  sc64 = gam * is64
+  sh64 = bet - m64 * sc64
+  unb = var * cnt / (cnt - 1) if cnt > 1 else var
+  fac = cnt / (cnt - 1) if cnt > 1 else 1.0
+  return {
+      "mean": (m64, 4 * u * m64.abs()),
+      "invstd": (is64, rel_is * is64),
+      "scale": (sc64, (rel_is + 2 * u) * sc64.abs()),
+      "shift": (sh64, (rel_is + 8 * u) * (m64 * sc64).abs() + 2 * u * sh64.abs()),
+      "running_mean": ((1 - mom) * rm0 + mom * m64,
+                       gamma(8, u) * ((1 - mom) * rm0.abs() + mom * m64.abs())),
+      "running_var": ((1 - mom) * rv0 + mom * unb,
+                      gamma(10, u) * ((1 - mom) * rv0.abs() + mom * unb) +
+                      mom * (e_var + u * var) * fac),
+  }
+
+
+def bn_apply_ref(x, scale, shift, res=None, act=1, u=U_FP32, sample_scale=None):
+  """(y reference, bound, pre-activation, ambiguous) of the apply y = bf16(act(x scale + shift
+  (+ res))): one fma and one add in fp32, then the bf16 rounding.  ``ambiguous``: elements whose
+  pre-activation lies within those roundings of 0, where the ReLU mask bit is not decided.
+  ``sample_scale`` (stochastic depth; per row, broadcast against x): y = act(s (x scale + shift)
+  (+ res)), one more fp32 multiply."""
+  xs = x * scale
+  pre = xs + shift
+  Mv = xs.abs() + shift.abs()
+  n = 2
+  if sample_scale is not None:
+    pre = pre * sample_scale
+    Mv = Mv * sample_scale.abs()
+    n = 3
+  if res is not None:
+    pre = pre + res
+    Mv = Mv + res.abs()
+  ref = pre.clamp_min(0.0) if act else pre
+  if act == 2:
+    ref = ref.clamp_max(6.0)
+  bound = U_BF16 * ref.abs() + (1 + U_BF16) * gamma(n, u) * Mv
+  return ref, bound, pre, pre.abs() <= gamma(n, u) * Mv
+
+
+def bn_bwd_reduce_refs(g, xm, invstd, depth, d0=0.0, b0=0.0, amb_mag=None):
+  """((dgamma ref, bound), (dbeta ref, bound)) of bn_bwd_reduce: column sums of the masked
+  gradient g and of g (x - mean) invstd added to d0 / b0, fp32 round-to-nearest along a tree of
+  ``depth`` roundings (red_grid_depth), plus x - mean and the invstd product for dgamma.
+  ``amb_mag``: |dy| where the recomputed mask is ambiguous (either bit is right there)."""
+  d0 = torch.as_tensor(d0, dtype=torch.float64, device=g.device)
+  b0 = torch.as_tensor(b0, dtype=torch.float64, device=g.device)
+  ref_g = d0 + (g * xm).sum(0) * invstd
+  bnd_g = gamma_prob(depth + 2) * (d0.abs() + (g.abs() * xm.abs()).sum(0) * invstd)
+  ref_b = b0 + g.sum(0)
+  bnd_b = gamma_prob(depth) * (b0.abs() + g.abs().sum(0))
+  if amb_mag is not None:
+    bnd_g = bnd_g + (amb_mag * xm.abs()).sum(0) * invstd
+    bnd_b = bnd_b + amb_mag.sum(0)
+  return (ref_g, bnd_g), (ref_b, bnd_b)
+
+
+def bn_bwd_fused_dgamma_ref(sum_g, sum_gx, mean, invstd, u=U_FP32):
+  """(dgamma reference, bound) of the apply kernel that finishes a reduction fused into a data
+  gradient's epilogue: invstd (sum(g x) - mean sum(g)), three fp32 roundings."""
+  return invstd * (sum_gx - mean * sum_g), gamma(3, u) * invstd * (sum_gx.abs() +
+                                                                  (mean * sum_g).abs())
+
+
+def bn_bwd_dx_ref(g, x, gam, mean, invstd, dg, db, amb=None, gmag=None, u=U_FP32, roundings=10):
+  """(dx reference, bound) of bn_bwd_apply: dx = gamma invstd (g - dbeta / P - (x - mean) invstd
+  dgamma / P) from the dgamma / dbeta the kernel read, ten fp32 roundings, then bf16; infinite
+  where ``amb`` (the mask bit is not decided).  ``gmag``: sum of the magnitudes behind g, where g
+  is itself a sum (the stem's routed max-pool gradient); |g| otherwise.  ``roundings``: 11 where
+  g is itself an fp32 product (the stochastic-depth factor times the masked gradient)."""
+  P = x.shape[0]
+  A = gam * invstd
+  ref = A * (g - db / P - (x - mean) * invstd * dg / P)
+  Mv = (A * (g.abs() if gmag is None else gmag)).abs() + \
+      (A * invstd * dg / P).abs() * (x.abs() + mean.abs()) + (A * db / P).abs()
+  bound = U_BF16 * ref.abs() + (1 + U_BF16) * gamma(roundings, u) * Mv
+  if amb is not None:
+    bound = torch.where(amb, torch.full_like(bound, float("inf")), bound)
+  return ref, bound
+
+
 # ------------------------------------------------------------------ row sampling
 def sample_box_rows(box_index, rows, valid):
   """Rows of M box ``box_index`` (``rows`` rows, ``valid(r)``: row r maps to a pixel inside the
