@@ -612,31 +612,49 @@ igemm_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-    // the per-column sums meet in shared memory for as long as the CTA stays on one n tile
+    // The per-column sums stay in registers for as long as the CTA stays on one n tile.  Then the
+    // lanes of a warp that share a chunk combine theirs with shuffles, each consumer warp leaves
+    // its partial in the (drained) epilogue stages, and one thread per column adds the eight warp
+    // partials and the direct path's shared-memory sums.  A float add on shared memory is a
+    // compare-and-swap loop on sm_90 (ATOMS.CAST.SPIN): a red.shared.add flush with 16 threads per
+    // column cost 14 to 32 us per launch on an H100 SXM at 700 W (DESIGN.md section 4).
     const int next_tile = tile + tstep;
     if ((do_stats || red_on) && (next_tile >= total_tiles || next_tile % a.n_tiles != nt)) {
+      float2* const wpart = reinterpret_cast<float2*>(smem + Cfg::kRing);   // [8 warps][BN]
+      static_assert(8 * BN * 8 <= 2 * Cfg::kOutWgBytes, "warp partials fit in the stages");
+      consumer_sync();   // both stages drained
 #pragma unroll
       for (int p = 0; p < kPasses; ++p)
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          const int c = p * kOutCols + ochunk * 8 + j;
-          if (csum[p][j] != 0.f || csq[p][j] != 0.f) {
-            red_shared_add(stat_smem + c * 2 + 0, csum[p][j]);
-            red_shared_add(stat_smem + c * 2 + 1, csq[p][j]);
+          float su = csum[p][j], sq = csq[p][j];
+#pragma unroll
+          for (int o = kChunks; o < 32; o *= 2) {
+            su += __shfl_xor_sync(0xffffffffu, su, o);
+            sq += __shfl_xor_sync(0xffffffffu, sq, o);
           }
+          if (lane < kChunks)   // lane == ochunk
+            wpart[(warp - 4) * BN + p * kOutCols + ochunk * 8 + j] = make_float2(su, sq);
           csum[p][j] = csq[p][j] = 0.f;
         }
       consumer_sync();
       for (int c = threadIdx.x - 128; c < BN; c += kConsumerThreads) {
+        float su = stat_smem[c * 2 + 0], sq = stat_smem[c * 2 + 1];
+#pragma unroll
+        for (int w = 0; w < 8; ++w) {
+          const float2 v = wpart[w * BN + c];
+          su += v.x;
+          sq += v.y;
+        }
         const int col = nt * BN + c;
         if (col < a.n_valid) {
-          atomicAdd(a.col_sum + col, stat_smem[c * 2 + 0]);
-          atomicAdd(a.col_sumsq + col, stat_smem[c * 2 + 1]);
+          atomicAdd(a.col_sum + col, su);
+          atomicAdd(a.col_sumsq + col, sq);
         }
         stat_smem[c * 2 + 0] = 0.f;
         stat_smem[c * 2 + 1] = 0.f;
       }
-      consumer_sync();
+      consumer_sync();   // the stages and stat_smem may be reused
     }
     org = next_org;
   }

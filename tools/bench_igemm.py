@@ -22,13 +22,19 @@ B = 256
 # name, kind, (H, W, Cin, Cout, k, stride)
 CASES = [
     ("l1c1", "fprop", (56, 56, 256, 64, 1, 1)),
+    ("l1c1b0", "fprop", (56, 56, 64, 64, 1, 1)),      # b0: the first block of the layer
     ("l1c2", "fprop", (56, 56, 64, 64, 3, 1)),
     ("l1c3", "fprop", (56, 56, 64, 256, 1, 1)),
+    ("l2c1b0", "fprop", (56, 56, 256, 128, 1, 1)),
+    ("l2c1", "fprop", (28, 28, 512, 128, 1, 1)),
     ("l2c2", "fprop", (28, 28, 128, 128, 3, 1)),
     ("l2c3", "fprop", (28, 28, 128, 512, 1, 1)),
+    ("l3c1b0", "fprop", (28, 28, 512, 256, 1, 1)),
     ("l3c1", "fprop", (14, 14, 1024, 256, 1, 1)),
     ("l3c2", "fprop", (14, 14, 256, 256, 3, 1)),
     ("l3c3", "fprop", (14, 14, 256, 1024, 1, 1)),
+    ("l4c1b0", "fprop", (14, 14, 1024, 512, 1, 1)),
+    ("l4c1", "fprop", (7, 7, 2048, 512, 1, 1)),
     ("l4c2", "fprop", (7, 7, 512, 512, 3, 1)),
     ("l4c3", "fprop", (7, 7, 512, 2048, 1, 1)),
     ("l2c2s2", "fprop", (56, 56, 128, 128, 3, 2)),
