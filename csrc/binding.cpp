@@ -5,6 +5,7 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
+#include <cfloat>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -613,6 +614,87 @@ void softmax_xent(const Tensor& logits, const Tensor& labels, c10::optional<Tens
                            loss_sum.data_ptr<float>(), optf(correct), rows, V, ld, ldd, scale,
                            static_cast<float>(label_smoothing), cur_stream(), mixp),
         "softmax_xent");
+}
+// Knowledge distillation loss (distill.cu): every argument is checked, with ValueError, before the
+// launch.  Shapes and dtypes first, then the scalars and the mix vector, then the devices.
+void distill_xent(const Tensor& logits, const Tensor& teacher_logits, const Tensor& labels,
+                  c10::optional<Tensor> dlogits, Tensor loss_sum, c10::optional<Tensor> correct,
+                  int64_t V, double scale, double label_smoothing, double alpha,
+                  double temperature, c10::optional<Tensor> mix) {
+  const char* what = "distill_xent";
+  TFOS_REQUIRE(logits.scalar_type() == torch::kFloat32 && logits.dim() == 2 &&
+                   logits.is_contiguous(),
+               what, ": logits must be contiguous fp32 [rows, ld], got ",
+               std::string(c10::toString(logits.scalar_type())), " ", shape_str(logits));
+  TFOS_REQUIRE(teacher_logits.scalar_type() == torch::kFloat32, what,
+               ": teacher_logits must be fp32, got ",
+               std::string(c10::toString(teacher_logits.scalar_type())));
+  TFOS_REQUIRE(teacher_logits.dim() == 2 && teacher_logits.is_contiguous(), what,
+               ": teacher_logits must be contiguous [rows, ldt], got ", shape_str(teacher_logits));
+  const int64_t rows = logits.size(0), ld = logits.size(1), ldt = teacher_logits.size(1);
+  TFOS_REQUIRE(teacher_logits.size(0) == rows, what, ": teacher_logits must have the student's ",
+               rows, " rows, got ", teacher_logits.size(0));
+  TFOS_REQUIRE(V >= 1 && V <= ld, what, ": need 1 <= V <= ld, got V=", V, " ld=", ld);
+  TFOS_REQUIRE(ldt >= V, what, ": teacher_logits need ldt >= V, got ldt=", ldt, " V=", V);
+  TFOS_REQUIRE(labels.scalar_type() == torch::kInt32 && labels.is_contiguous() &&
+                   labels.numel() == rows,
+               what, ": labels must be contiguous int32 with one label per row (", rows,
+               "), got ", std::string(c10::toString(labels.scalar_type())), " ",
+               shape_str(labels));
+  const bool has_dl = dlogits.has_value() && dlogits->defined();
+  if (has_dl)
+    TFOS_REQUIRE(dlogits->scalar_type() == torch::kBFloat16 && dlogits->dim() == 2 &&
+                     dlogits->is_contiguous() && dlogits->size(0) == rows &&
+                     dlogits->size(1) >= V,
+                 what, ": dlogits must be contiguous bf16 [", rows, ", >= V], got ",
+                 std::string(c10::toString(dlogits->scalar_type())), " ", shape_str(*dlogits));
+  TFOS_REQUIRE(loss_sum.scalar_type() == torch::kFloat32 && loss_sum.numel() >= 1, what,
+               ": loss_sum must be an fp32 scalar");
+  const bool has_c = correct.has_value() && correct->defined();
+  if (has_c)
+    TFOS_REQUIRE(correct->scalar_type() == torch::kFloat32 && correct->numel() >= 1, what,
+                 ": correct must be an fp32 scalar");
+  TFOS_REQUIRE(std::isfinite(label_smoothing) && label_smoothing >= 0.0 && label_smoothing <= 1.0,
+               what, ": label_smoothing must be in [0, 1], got ", label_smoothing);
+  TFOS_REQUIRE(alpha > 0.0 && alpha <= 1.0, what, ": alpha must be in (0, 1], got ", alpha);
+  // checked as the kernel gets it: an fp32 T that is finite and at least FLT_MIN, so that 1 / T
+  // is finite too (a T such as 1e-50 would round to 0 in fp32)
+  const float tf = static_cast<float>(temperature);
+  TFOS_REQUIRE(std::isfinite(temperature) && std::isfinite(tf) && tf >= FLT_MIN, what,
+               ": temperature must be finite and > 0 in fp32 (>= 1.18e-38), got ", temperature);
+  TFOS_REQUIRE(std::isfinite(scale), what, ": scale must be finite, got ", scale);
+  const float* mixp = check_mix(mix, logits, what);
+  TFOS_REQUIRE(logits.is_cuda(), what, ": logits must be a CUDA tensor");
+  const auto dev = logits.device();
+  auto same = [&](const Tensor& t, const char* name) {
+    TFOS_REQUIRE(t.device() == dev, what, ": ", name, " must be on the device of logits (",
+                 dev.str(), "), got ", t.device().str());
+  };
+  same(teacher_logits, "teacher_logits");
+  same(labels, "labels");
+  same(loss_sum, "loss_sum");
+  if (has_dl) same(*dlogits, "dlogits");
+  if (has_c) same(*correct, "correct");
+  TFOS_REQUIRE(rows < (int64_t{1} << 31), what, ": too many rows: ", rows);
+  const c10::cuda::CUDAGuard guard(dev);
+  check(tfos::distill_xent(logits.data_ptr<float>(), teacher_logits.data_ptr<float>(),
+                           labels.data_ptr<int>(), has_dl ? dlogits->data_ptr() : nullptr,
+                           loss_sum.data_ptr<float>(), optf(correct), rows, static_cast<int>(V),
+                           static_cast<int>(ld), static_cast<int>(ldt),
+                           has_dl ? static_cast<int>(dlogits->size(1)) : 0,
+                           static_cast<float>(scale), static_cast<float>(label_smoothing),
+                           static_cast<float>(alpha), static_cast<float>(temperature), mixp,
+                           cur_stream()),
+        what);
+}
+// The distillation loss registers through its own function: its float64 check and its coverage
+// entry live with the feature's tests (tests/test_gpu_distill.py CHECKED_HERE), and
+// tests/test_distill_host.py requires one for every entry point registered here.
+void bind_distill(py::module_& mod) {
+  mod.def("distill_xent", &distill_xent, py::arg("logits"), py::arg("teacher_logits"),
+          py::arg("labels"), py::arg("dlogits"), py::arg("loss_sum"), py::arg("correct"),
+          py::arg("V"), py::arg("scale"), py::arg("label_smoothing") = 0.0,
+          py::arg("alpha") = 0.5, py::arg("temperature") = 1.0, py::arg("mix") = py::none());
 }
 // The multi-label kernels' shapes: logits [rows, ld] with 1 <= V <= ld, targets [rows, V].
 void check_multilabel(const Tensor& logits, const Tensor& targets, int64_t V, const char* what) {
@@ -1487,6 +1569,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("symm_free", &symm_free);
   m.def("tensor_from_ptr", &tensor_from_ptr);
   m.def("num_sms", &num_sms);
+  // Not an m.def of this list: the registry test of tests/test_ps_kernels_host.py, which scans
+  // it, cannot name the entry point.  tests/test_distill_host.py holds the same guard for every
+  // entry point bind_distill registers (each needs a float64 check in tests/test_gpu_distill.py).
+  bind_distill(m);
   tfos::bind_feed(m);
   tfos::bind_tfrecord(m);
   tfos::bind_vmm(m);

@@ -452,4 +452,16 @@ cudaError_t mixed_target_bce(const float* logits, const uint8_t* targets, void* 
                              int ldd, float scale, float label_smoothing, const float* pos_weight,
                              const float* mix, cudaStream_t s);
 
+// ---- distill.cu: knowledge distillation loss of fp32 student logits [rows, ld] against the hard
+// target of mixed_target_xent (mix null: softmax_xent's) and fp32 teacher logits [rows, ldt], both
+// read in columns [0, V):
+//   l = (1 - alpha) CE(s, t) + alpha T^2 KL(softmax(z / T) || softmax(s / T)),  loss_sum += l scale
+//   dlogits (bf16 [rows, ldd], when not null) = [(1 - alpha)(softmax(s) - t) + alpha T
+//   (softmax(s / T) - softmax(z / T))] scale, exactly 0 in columns [V, ldd); correct_sum (when not
+//   null) counts the student's lowest-index arg-max == the dominant label.
+cudaError_t distill_xent(const float* logits, const float* teacher_logits, const int* labels,
+                         void* dlogits, float* loss_sum, float* correct_sum, long long rows, int V,
+                         int ld, int ldt, int ldd, float scale, float label_smoothing, float alpha,
+                         float temperature, const float* mix, cudaStream_t s);
+
 }  // namespace tfos

@@ -60,6 +60,15 @@ def define_flags():
   p.add_argument("--drop_path_rate", type=float, default=0.0,
                  help="stochastic depth: the last residual block drops with this rate, block i of "
                       "N with rate * i / (N - 1) (0: off)")
+  p.add_argument("--teacher", default=None,
+                 help="knowledge distillation: model_dir of an earlier CIFAR ResNet run with the "
+                      "same class count; the params of its newest checkpoint are the frozen teacher")
+  p.add_argument("--teacher_depth", type=int, default=None,
+                 help="depth of the --teacher model (default: --resnet_size)")
+  p.add_argument("--distill_alpha", type=float, default=None,
+                 help="weight of the distillation term, in (0, 1] (default 0.5)")
+  p.add_argument("--distill_temperature", type=float, default=None,
+                 help="softmax temperature of the distillation term, > 0 (default 1)")
   return p
 
 
@@ -106,6 +115,15 @@ def main_fun(argv, ctx):
   for name, default in (("mixup_alpha", 0.0), ("cutmix_alpha", 0.0), ("mix_prob", 1.0),
                         ("mix_switch_prob", 0.5), ("drop_path_rate", 0.0)):
     if getattr(args, name) != default:
+      smooth[name] = getattr(args, name)
+  if args.teacher:   # read as resnet_spark.py reads --init_checkpoint
+    t_step, t_state = checkpoint.load(ctx.absolute_path(args.teacher))
+    if t_state is None:
+      raise ValueError("--teacher {}: no checkpoint there".format(args.teacher))
+    smooth["teacher"] = t_state["params"]
+    print("teacher from {} (step {})".format(args.teacher, t_step))
+  for name in ("teacher_depth", "distill_alpha", "distill_temperature"):
+    if getattr(args, name) is not None:
       smooth[name] = getattr(args, name)
   net = resnet.CifarResNetTrainer(depth=args.resnet_size, batch=B, device=dev, comm=comm,
                                   lr=resnet.piecewise_lr(0, B * world), **smooth)

@@ -116,10 +116,38 @@ def parse(argv):
   p.add_argument("--drop_path_rate", type=float, default=0.0,
                  help="stochastic depth: the last residual block drops with this rate, block i of "
                       "N with rate * i / (N - 1) (0: off)")
+  p.add_argument("--teacher", default=None,
+                 help="knowledge distillation: model_dir of an earlier run of this model family with "
+                      "the same class count; the params of its newest checkpoint are the frozen "
+                      "teacher")
+  p.add_argument("--teacher_depth", type=int, default=None,
+                 help="depth of the --teacher model (default: the student's)")
+  p.add_argument("--distill_alpha", type=float, default=None,
+                 help="weight of the distillation term, in (0, 1] (default 0.5)")
+  p.add_argument("--distill_temperature", type=float, default=None,
+                 help="softmax temperature of the distillation term, > 0 (default 1)")
   p.add_argument("--multi_label", action="store_true",
                  help="multi-hot labels and the binary cross-entropy; evaluation reports "
                       "binary_accuracy, exact_match, f1 and macro_f1")
   return p.parse_args(argv)
+
+
+def distill_options(args, ctx):
+  """The trainer's distillation keywords from --teacher, --teacher_depth, --distill_alpha and
+  --distill_temperature: only the flags that were set.  --teacher is read as --init_checkpoint
+  is: the ``params`` of the newest checkpoint under that model_dir."""
+  from tensorflowonspark_b200.utils import checkpoint
+  opt = {}
+  if args.teacher:
+    step, state = checkpoint.load(ctx.absolute_path(args.teacher))
+    if state is None:
+      raise ValueError("--teacher {}: no checkpoint there".format(args.teacher))
+    opt["teacher"] = state["params"]
+    print("teacher from {} (step {})".format(args.teacher, step))
+  for name in ("teacher_depth", "distill_alpha", "distill_temperature"):
+    if getattr(args, name) is not None:
+      opt[name] = getattr(args, name)
+  return opt
 
 
 def main_fun(argv, ctx):
@@ -161,6 +189,7 @@ def main_fun(argv, ctx):
                         ("mix_switch_prob", 0.5), ("drop_path_rate", 0.0)):
     if getattr(args, name) != default:
       opt[name] = getattr(args, name)
+  opt.update(distill_options(args, ctx))
   if args.model == "resnet56":
     net = resnet.CifarResNetTrainer(depth=56, batch=B, device="cuda:0", comm=comm, lr=base_lr, **opt)
   else:

@@ -24,7 +24,8 @@ CSRC_DIR = os.path.join(REPO_DIR, "csrc")
 EXT_DIR = os.path.join(PKG_DIR, "_ext")
 
 SOURCES = ["binding.cpp", "igemm.cu", "igemm_wgrad.cu", "elementwise.cu", "bn_bwd.cu", "stem_fused.cu",
-           "smallops.cu", "eval.cu", "optim_comm.cu", "mix.cu", "feed.cc", "tfrecord.cc", "vmm.cc"]
+           "smallops.cu", "eval.cu", "optim_comm.cu", "mix.cu", "distill.cu", "feed.cc",
+           "tfrecord.cc", "vmm.cc"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--expt-relaxed-constexpr", "--use_fast_math"]
 

@@ -254,6 +254,47 @@ def check_drop_path_rate(r=0.0, training=True):
   return float(r)
 
 
+def check_distill_args(teacher=None, teacher_depth=None, distill_alpha=0.5,
+                       distill_temperature=1.0, training=True, multi_label=False):
+  """Validated ``(teacher_depth, distill_alpha, distill_temperature)`` of a trainer, the last two
+  as floats: ``teacher`` None or a mapping (a ``state_dict()``), ``teacher_depth`` None or an int,
+  alpha a real in (0, 1], T a finite real > 0.  ValueError otherwise, for a non-default alpha, T or
+  ``teacher_depth`` without a teacher, for any of the four with ``training=False`` (an
+  inference-only trainer has no loss to distil into) and for a teacher with ``multi_label``
+  (distillation is of softmax classifiers).  The teacher's tensors are checked by the trainer."""
+  a, t = distill_alpha, distill_temperature
+  if isinstance(a, bool) or not isinstance(a, numbers.Real) or not 0.0 < float(a) <= 1.0:
+    raise ValueError("distill_alpha must be a real number in (0, 1], got {!r}".format(a))
+  # the kernels take T in fp32: it must stay finite and nonzero there (1 / T finite too)
+  ok = not isinstance(t, bool) and isinstance(t, numbers.Real) and math.isfinite(float(t)) \
+      and float(t) > 0.0
+  if ok:
+    with np.errstate(over="ignore"):
+      t32 = np.float32(t)
+    ok = bool(np.isfinite(t32)) and t32 >= np.finfo(np.float32).tiny
+  if not ok:
+    raise ValueError("distill_temperature must be a finite real number > 0 that fp32 holds "
+                     "(>= {:.3g}), got {!r}".format(float(np.finfo(np.float32).tiny), t))
+  if teacher_depth is not None and (isinstance(teacher_depth, bool) or
+                                    not isinstance(teacher_depth, numbers.Integral)):
+    raise ValueError("teacher_depth must be an int, got {!r}".format(teacher_depth))
+  given = teacher is not None or teacher_depth is not None or float(a) != 0.5 or float(t) != 1.0
+  if given and not training:
+    raise ValueError("teacher, teacher_depth, distill_alpha and distill_temperature need "
+                     "training=True (an inference-only trainer has no loss to distil into)")
+  if teacher is None:
+    if given:
+      raise ValueError("teacher_depth, distill_alpha and distill_temperature configure "
+                       "distillation: they need a teacher")
+  else:
+    if not hasattr(teacher, "keys") or not hasattr(teacher, "__getitem__"):
+      raise ValueError("teacher must be a state_dict() (a mapping of tensors), got {}".format(
+          type(teacher).__name__))
+    if multi_label:
+      raise ValueError("a teacher distils a softmax classifier: not with multi_label=True")
+  return (None if teacher_depth is None else int(teacher_depth)), float(a), float(t)
+
+
 def drop_path_rates(r, n_blocks):
   """timm's linear decay of the stochastic-depth rate over the residual blocks of a network:
   block i of N (0-based) drops with p_i = r * i / (N - 1), so block 0 never drops and the last one

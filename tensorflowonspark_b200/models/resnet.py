@@ -98,6 +98,54 @@ def _padded_head_init(V, std=0.01):
 _HEAD = ("fc.w", "fc.b")   # the classifier: what load_backbone leaves out
 
 
+def _state_shapes(cls, depth, num_classes):
+  """{name: shape} of the ``state_dict()`` of a ``cls`` trainer of ``depth`` with ``num_classes``
+  classes, ``__running__`` included, from the parameter registration alone (nothing on a
+  device)."""
+  st = engine.ParamStore()
+  cls._register(st, depth, num_classes)
+  shapes = {s["name"]: s["shape"] for s in st._specs}
+  # RunningArena: mean and var of every batch norm, each padded to 8
+  shapes["__running__"] = (sum(2 * ((s["shape"][0] + 7) // 8 * 8) for s in st._specs
+                               if s["name"].endswith(".gamma")),)
+  return shapes
+
+
+def _check_state_shapes(state, want, what):
+  """ValueError naming the first tensor of ``state`` that is not in ``want`` ({name: shape}), is
+  missing from it or has another shape; nothing is copied."""
+  extra = sorted(set(state) - set(want))
+  if extra:
+    raise ValueError("{}: {} is not a tensor of this model (another depth or family?)".format(
+        what, extra[0]))
+  for name, shape in want.items():
+    if name not in state:
+      raise ValueError("{}: {} {} is missing from the state{}".format(
+          what, name, shape, " (it must include the running statistics)"
+          if name == "__running__" else " (another depth or family?)"))
+    got = tuple(getattr(state[name], "shape", ()))
+    if got != tuple(shape):
+      raise ValueError("{}: {} has shape {} in the state, {} in this model{}".format(
+          what, name, got, tuple(shape), " (a head for another class count?)"
+          if name in _HEAD else ""))
+
+
+def _check_teacher(cls, teacher, teacher_depth, alpha, temperature, depth, num_classes, training,
+                   multi_label):
+  """The distillation options of a ``cls`` trainer (engine.check_distill_args) and its teacher's
+  tensors, checked before anything is allocated.  Returns (the teacher's depth, or None without a
+  teacher; alpha; T)."""
+  td, a, t = engine.check_distill_args(teacher, teacher_depth, alpha, temperature, training,
+                                       multi_label)
+  if teacher is None:
+    return None, a, t
+  td = depth if td is None else td
+  if not cls._valid_depth(td):
+    raise ValueError("teacher_depth {} is not a depth of {}".format(td, cls.__name__))
+  _check_state_shapes(teacher, _state_shapes(cls, td, num_classes), "teacher")
+  return td, a, t
+
+
 # columns of the bn_fold table (csrc/ops.h kFold*)
 FOLD_WEIGHT, FOLD_COUT, FOLD_PER_CHANNEL, FOLD_GAMMA, FOLD_BETA, FOLD_MEAN, FOLD_VAR, FOLD_BIAS = \
     range(8)
@@ -294,7 +342,8 @@ class ResNetTrainer(object):
                ema_decay=None, clip_norm=None, beta1=0.9, beta2=0.999, epsilon=1e-7,
                gradient_accumulation_steps=1, multi_label=False, pos_weight=None,
                mixup_alpha=0.0, cutmix_alpha=0.0, mix_prob=1.0, mix_switch_prob=0.5,
-               drop_path_rate=0.0):
+               drop_path_rate=0.0, teacher=None, teacher_depth=None, distill_alpha=0.5,
+               distill_temperature=1.0):
     """``optimizer``: sgd | momentum | adam | adamw | lars | lamb (``trust_coefficient`` is LARS's
     eta; see parallel/fused_optim.py).  adam folds ``weight_decay`` into the gradient (L2), adamw
     decouples it (``torch.optim.AdamW``), lamb is layer-wise adaptive Adam (apex ``FusedLAMB``).
@@ -359,13 +408,33 @@ class ResNetTrainer(object):
     output's.  Each ``train_step`` call (each micro-step, each warm-up step of ``capture()``)
     draws the factors of every block on the host (engine.DropPathDraws, seeded with (``seed``,
     rank, 1)); ``last_drop_path`` holds the last draw.  Evaluation, serving, ``averaged()`` and
-    exports never drop."""
+    exports never drop.
+
+    ``teacher`` (training only): None, or the ``state_dict()`` of a trained ResNetTrainer of depth
+    ``teacher_depth`` (50, 101 or 152; default: this trainer's depth) with the same
+    ``num_classes``, ``__running__`` included (``net.averaged().state_dict()`` too): knowledge
+    distillation.  Every tensor is checked as ``load_backbone`` checks it, before anything is
+    allocated.  The teacher is a frozen ``training=False`` replica with every batch norm folded
+    into its convolutions (``build_folded_inference``, with its running statistics; it never drops
+    a path and is never updated).  It runs inside every training step, right after the decode, on
+    the student's decoded input (the mixed one under Mixup / CutMix), and the training loss of row
+    i with student logits s, teacher logits z and the hard target t above becomes
+    (1 - a) CE(s, t) + a T^2 KL(softmax(z / T) || softmax(s / T)), a = ``distill_alpha`` in (0, 1],
+    T = ``distill_temperature`` (finite, > 0): ``(1-a) F.cross_entropy(s, y, label_smoothing=eps)
+    + a T^2 F.kl_div(F.log_softmax(s/T), F.log_softmax(z/T), log_target=True,
+    reduction="batchmean")``.  ``correct`` still counts the student's arg-max against the dominant
+    label.  The teacher is not part of ``state_dict()``, checkpoints, the optimizer state,
+    ``averaged()``, exports, evaluation or serving: a resumed run passes it again.  Not with
+    ``multi_label``."""
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     self.multi_label, pos_weight = _check_multilabel_args(multi_label, pos_weight, num_classes,
                                                           training)
     mix_args = engine.check_mix_args(mixup_alpha, cutmix_alpha, mix_prob, mix_switch_prob,
                                      training)
     self.drop_path_rate = engine.check_drop_path_rate(drop_path_rate, training)
+    self.teacher_depth, self.distill_alpha, self.distill_temperature = _check_teacher(
+        type(self), teacher, teacher_depth, distill_alpha, distill_temperature, depth, num_classes,
+        training, self.multi_label)
     k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps, training)
     self.ema_decay = engine.check_ema_decay(ema_decay, training)
     self.clip_norm = engine.check_clip_norm(clip_norm, training)
@@ -380,27 +449,9 @@ class ResNetTrainer(object):
     B = batch
 
     # ---- parameters -----------------------------------------------------
-    self.stem_w = st.register("stem.conv.w", (64, 7, 64), True, self._stem_init)
-    self.stem_bn = BatchNorm(st, "stem.bn", 64)
-    self.blocks = []
-    cin = 64
-    for si, nblocks in enumerate(self.CFG[depth]):
-      width = 64 * (2 ** si)
-      for bi in range(nblocks):
-        stride = 2 if (bi == 0 and si > 0) else 1
-        b = _Block()
-        name = "layer{}.{}".format(si + 1, bi)
-        b.u1 = _Unit(st, name + ".u1", cin, width, 1, 1)
-        b.u2 = _Unit(st, name + ".u2", width, width, 3, stride)
-        b.u3 = _Unit(st, name + ".u3", width, width * 4, 1, 1, zero_gamma=True)
-        b.ds = _Unit(st, name + ".ds", cin, width * 4, 1, stride) if bi == 0 else None
-        b.stride, b.cin, b.width, b.name = stride, cin, width, name
-        self.blocks.append(b)
-        cin = width * 4
+    self.stem_w, self.stem_bn, self.blocks, self.fc, self.feat = self._register(st, depth,
+                                                                                num_classes)
     VP = self.VP = (num_classes + 7) // 8 * 8
-    self.fc = Dense(st, "fc", cin, VP, bias=True,
-                    init=normal(0.01) if VP == num_classes else _padded_head_init(num_classes))
-    self.feat = cin
     self.drop_path_rates = engine.drop_path_rates(self.drop_path_rate, len(self.blocks))
 
     alloc = comm.alloc if comm is not None else None
@@ -520,6 +571,37 @@ class ResNetTrainer(object):
     self.mean = [0.485, 0.456, 0.406]
     self.std = [0.229, 0.224, 0.225]
     self._assign_directions()
+    self.teacher = None if teacher is None else _ResNetTeacher(self, teacher, self.teacher_depth)
+
+  @classmethod
+  def _register(cls, st, depth, num_classes):
+    """Register the parameters of a ResNet-``depth`` with ``num_classes`` classes in ``st`` (host
+    only).  Returns (stem filter spec, stem batch norm, blocks, head, feature width)."""
+    stem_w = st.register("stem.conv.w", (64, 7, 64), True, cls._stem_init)
+    stem_bn = BatchNorm(st, "stem.bn", 64)
+    blocks = []
+    cin = 64
+    for si, nblocks in enumerate(cls.CFG[depth]):
+      width = 64 * (2 ** si)
+      for bi in range(nblocks):
+        stride = 2 if (bi == 0 and si > 0) else 1
+        b = _Block()
+        name = "layer{}.{}".format(si + 1, bi)
+        b.u1 = _Unit(st, name + ".u1", cin, width, 1, 1)
+        b.u2 = _Unit(st, name + ".u2", width, width, 3, stride)
+        b.u3 = _Unit(st, name + ".u3", width, width * 4, 1, 1, zero_gamma=True)
+        b.ds = _Unit(st, name + ".ds", cin, width * 4, 1, stride) if bi == 0 else None
+        b.stride, b.cin, b.width, b.name = stride, cin, width, name
+        blocks.append(b)
+        cin = width * 4
+    VP = (num_classes + 7) // 8 * 8
+    fc = Dense(st, "fc", cin, VP, bias=True,
+               init=normal(0.01) if VP == num_classes else _padded_head_init(num_classes))
+    return stem_w, stem_bn, blocks, fc, cin
+
+  @classmethod
+  def _valid_depth(cls, depth):
+    return depth in cls.CFG
 
   def _build_mix(self, mix_args, seed):
     """Mixup / CutMix state: the host draws (engine.MixDraws) and the device vector each step's
@@ -702,6 +784,8 @@ class ResNetTrainer(object):
       self.stats_arena.zero()   # the fused conv epilogues accumulate from zero every pass
     K.decode_normalize(self.in_u8, self.xp, igemm.STEM_PAD, self.mean, self.std,
                        **(self._mix_arg() if training else {}))
+    if training and self.teacher is not None:
+      self.teacher.run()      # its stem reads xp: the (mixed) input the student trains on
     (self.p_stem_remote if remote else self.p_stem).run()
     if training:
       # BN + ReLU + max pool in one pass over the raw conv output (csrc/stem_fused.cu): the
@@ -739,6 +823,12 @@ class ResNetTrainer(object):
                         self.loss_sum, self.correct, self.num_classes,
                         1.0 / (self.B * self.num_classes), label_smoothing=self.label_smoothing,
                         pos_weight=self.pos_weight, **mix)
+      return
+    if with_grad and self.teacher is not None:
+      ops.K.distill_xent(self.logits, self.teacher.logits, self.labels, self.dlogits,
+                         self.loss_sum, self.correct, self.num_classes, 1.0 / self.B,
+                         label_smoothing=self.label_smoothing, alpha=self.distill_alpha,
+                         temperature=self.distill_temperature, **mix)
       return
     ops.K.softmax_xent(self.logits, self.labels, self.dlogits if with_grad else None,
                        self.loss_sum, self.correct, self.num_classes, 1.0 / self.B,
@@ -828,8 +918,9 @@ class ResNetTrainer(object):
     return self.logits
 
   # ------------------------------------------ inference with folded batch norm
-  def build_folded_inference(self):
-    """Serving path: every batch norm is folded into the convolution in front of it
+  def build_folded_inference(self, x=None):
+    """``x``: the decoded input the stem reads (default ``xp``; a distilling student's ``xp`` for
+    its teacher).  Serving path: every batch norm is folded into the convolution in front of it
     (w' = w * gamma / sqrt(var + eps) per output channel, bias = beta - mean * that scale, from
     the fp32 masters and the running statistics), ReLU and the residual add run in the conv
     epilogues (bias / ReLU / accumulate), identity blocks accumulate IN PLACE into their input.
@@ -847,7 +938,7 @@ class ResNetTrainer(object):
       bias[id(bn)] = self.bf[off:off + bn.C]
       off += (bn.C + 7) // 8 * 8
     self._f_plans, self._f_last = self._folded_plans(lambda spec: st._view(self.wf, spec), bias,
-                                                     self.stem_act)
+                                                     self.stem_act, x)
     self.fold_batch_norms()
 
   def _fold_units(self):
@@ -858,10 +949,12 @@ class ResNetTrainer(object):
         units.append((u.conv.sw, u.bn))
     return units
 
-  def _folded_plans(self, wv, bias, stem_out):
+  def _folded_plans(self, wv, bias, stem_out, x=None):
     """The folded network's convolutions: ``wv(spec)`` is a folded filter, ``bias[id(bn)]`` the
-    folded batch norm's bias; the stem writes ``stem_out``.  Returns (plans, last activation)."""
-    plans = [igemm.stem_fprop(self.xp, wv(self.stem_w), stem_out, bias=bias[id(self.stem_bn)],
+    folded batch norm's bias; the stem reads ``x`` (default ``xp``) and writes ``stem_out``.
+    Returns (plans, last activation)."""
+    x = self.xp if x is None else x
+    plans = [igemm.stem_fprop(x, wv(self.stem_w), stem_out, bias=bias[id(self.stem_bn)],
                               relu=True)]
     cur = self.pool
     for b in self.blocks:
@@ -910,8 +1003,13 @@ class ResNetTrainer(object):
 
   def forward_folded(self):
     """logits of the staged batch through the folded network (capturable)."""
+    ops.K.decode_normalize(self.in_u8, self.xp, igemm.STEM_PAD, self.mean, self.std)
+    return self.run_folded()
+
+  def run_folded(self):
+    """``forward_folded`` without the decode: the folded network on the input its stem was built
+    to read (``build_folded_inference(x)``); returns ``logits`` (capturable)."""
     K = ops.K
-    K.decode_normalize(self.in_u8, self.xp, igemm.STEM_PAD, self.mean, self.std)
     self._f_plans[0].run()
     K.maxpool_fwd(self.stem_act, self.pool, self.pool_idx, 3, 2, 1)
     for p in self._f_plans[1:]:
@@ -1096,53 +1194,97 @@ def build_served(state, depth=50, image=224, num_classes=1000, batch=None, multi
                       batch=serving.serve_batch(batch), multi_label=bool(multi_label))
 
 
+class _ResNetTeacher(object):
+  """Frozen distillation teacher of a ResNetTrainer: a ``training=False`` replica of ``depth``
+  on the student's device and batch, loaded from ``state`` and folded once
+  (``build_folded_inference``), whose stem reads the student's decoded input ``xp``.  ``run()``
+  launches its folded forward pass (convolutions, pools, head); it writes only the replica's own
+  buffers and leaves the teacher's logits in ``logits``."""
+
+  def __init__(self, student, state, depth):
+    self.net = ResNetTrainer(depth=depth, batch=student.B, image=student.image,
+                             num_classes=student.num_classes, device=student.device,
+                             training=False)
+    self.net.load_state_dict(state)
+    self.net.build_folded_inference(x=student.xp)
+    self.logits = self.net.logits
+
+  def run(self):
+    self.net.run_folded()
+
+
+class _CifarTeacher(object):
+  """Frozen distillation teacher of a CifarResNetTrainer: a CifarResNetTrainer of ``depth`` on the
+  student's device and batch, loaded from ``state``, with every batch norm folded once on the host
+  (``ResNetTrainer.fold_batch_norms``: fp32 masters and running statistics) into a copy of its
+  filters.  Its folded plans (``_folded_plans``) read the student's decoded input ``x8``; ``run()``
+  launches them, the average pool and the head, writing only the teacher's own buffers, and
+  leaves the teacher's logits in ``logits``.  Its optimizer is never stepped."""
+
+  def __init__(self, student, state, depth):
+    net = self.net = CifarResNetTrainer(depth=depth, batch=student.B,
+                                        num_classes=student.num_classes, device=student.device)
+    net.load_state_dict(state)
+    st = net.store
+    units = net._fold_units()
+    net.wf = torch.zeros_like(st.weights)
+    net.bf = torch.zeros(sum((bn.C + 7) // 8 * 8 for _, bn in units), dtype=torch.float32,
+                         device=net.device)
+    bias, off = {}, 0
+    for _, bn in units:
+      bias[id(bn)] = net.bf[off:off + bn.C]
+      off += (bn.C + 7) // 8 * 8
+    ResNetTrainer.fold_batch_norms(net)
+    self.plans, self.last = net._folded_plans(lambda spec: st._view(net.wf, spec), bias,
+                                              student.x8)
+    self.logits = net.logits
+
+  def run(self):
+    for p in self.plans:
+      p.run()
+    ops.K.avgpool_fwd(self.last, self.net.avg)
+    self.net.fc.forward()
+
+
 class CifarResNetTrainer(object):
   """ResNet-20/32/56 for 32x32 inputs (basic blocks, 16/32/64 channels) - the network the
   reference example actually trains (examples/resnet/resnet_cifar_dist.py:208, ``resnet56``,
   momentum SGD, batch 128, weight decay 2e-4).  ``optimizer``, ``num_classes``,
   ``label_smoothing``, ``ema_decay``, ``clip_norm``, ``beta1``, ``beta2``, ``epsilon``,
   ``gradient_accumulation_steps``, ``multi_label``, ``pos_weight``, ``mixup_alpha``,
-  ``cutmix_alpha``, ``mix_prob``, ``mix_switch_prob`` and ``drop_path_rate`` as in ResNetTrainer
-  (the CutMix box is drawn on the 32 x 32 image; stochastic depth scales the output of each basic
-  block's second batch norm, as in timm's ``BasicBlock``)."""
+  ``cutmix_alpha``, ``mix_prob``, ``mix_switch_prob``, ``drop_path_rate``, ``teacher``,
+  ``teacher_depth``, ``distill_alpha`` and ``distill_temperature`` as in ResNetTrainer (the CutMix
+  box is drawn on the 32 x 32 image; stochastic depth scales the output of each basic block's
+  second batch norm, as in timm's ``BasicBlock``; the teacher is the ``state_dict()`` of a
+  CifarResNetTrainer of any valid depth, folded once on the host, whose folded convolutions read
+  the student's decoded ``x8``)."""
 
   def __init__(self, depth=56, batch=128, num_classes=10, device="cuda:0", lr=0.1, momentum=0.9,
                weight_decay=2e-4, comm=None, seed=1234, optimizer="momentum",
                trust_coefficient=0.001, label_smoothing=0.0, ema_decay=None, clip_norm=None,
                beta1=0.9, beta2=0.999, epsilon=1e-7, gradient_accumulation_steps=1,
                multi_label=False, pos_weight=None, mixup_alpha=0.0, cutmix_alpha=0.0, mix_prob=1.0,
-               mix_switch_prob=0.5, drop_path_rate=0.0):
+               mix_switch_prob=0.5, drop_path_rate=0.0, teacher=None, teacher_depth=None,
+               distill_alpha=0.5, distill_temperature=1.0):
     num_classes, self.label_smoothing = _check_head_args(num_classes, label_smoothing)
     self.multi_label, pos_weight = _check_multilabel_args(multi_label, pos_weight, num_classes)
     mix_args = engine.check_mix_args(mixup_alpha, cutmix_alpha, mix_prob, mix_switch_prob)
     self.drop_path_rate = engine.check_drop_path_rate(drop_path_rate)
+    self.teacher_depth, self.distill_alpha, self.distill_temperature = _check_teacher(
+        type(self), teacher, teacher_depth, distill_alpha, distill_temperature, depth, num_classes,
+        True, self.multi_label)
     k_acc = engine.check_gradient_accumulation_steps(gradient_accumulation_steps)
     self.ema_decay = engine.check_ema_decay(ema_decay)
     self.clip_norm = engine.check_clip_norm(clip_norm)
     beta1, beta2, epsilon = engine.check_adam_args(beta1, beta2, epsilon)
     assert (depth - 2) % 6 == 0
-    n = (depth - 2) // 6
     self.device = dev = torch.device(device)
     self.B, self.image, self.num_classes = batch, 32, num_classes
     self.comm = comm
     self.VP = (num_classes + 7) // 8 * 8
     B = batch
     st = self.store = ParamStore()
-    self.stem = _Unit(st, "stem", 8, 16, 3, 1)
-    self.blocks = []
-    cin = 16
-    for si, width in enumerate((16, 32, 64)):
-      for bi in range(n):
-        stride = 2 if (bi == 0 and si > 0) else 1
-        b = _Block()
-        name = "stage{}.{}".format(si + 1, bi)
-        b.u1 = _Unit(st, name + ".u1", cin, width, 3, stride)
-        b.u2 = _Unit(st, name + ".u2", width, width, 3, 1, zero_gamma=True)
-        b.ds = _Unit(st, name + ".ds", cin, width, 1, stride) if stride != 1 else None
-        b.stride, b.width = stride, width
-        self.blocks.append(b)
-        cin = width
-    self.fc = Dense(st, "fc", 64, self.VP, bias=True, init=normal(0.01))
+    self.stem, self.blocks, self.fc = self._register(st, depth, num_classes)
     self.drop_path_rates = engine.drop_path_rates(self.drop_path_rate, len(self.blocks))
     st.finalize(dev, alloc=comm.alloc if comm is not None else None, seed=seed)
 
@@ -1203,6 +1345,34 @@ class CifarResNetTrainer(object):
     self.graph = None
     self.graphs = None
     self.mean, self.std = [0.4914, 0.4822, 0.4465], [0.2470, 0.2435, 0.2616]
+    self.teacher = None if teacher is None else _CifarTeacher(self, teacher, self.teacher_depth)
+
+  @staticmethod
+  def _register(st, depth, num_classes):
+    """Register the parameters of a CIFAR ResNet-``depth`` in ``st`` (host only).  Returns (stem
+    unit, blocks, head)."""
+    n = (depth - 2) // 6
+    stem = _Unit(st, "stem", 8, 16, 3, 1)
+    blocks = []
+    cin = 16
+    for si, width in enumerate((16, 32, 64)):
+      for bi in range(n):
+        stride = 2 if (bi == 0 and si > 0) else 1
+        b = _Block()
+        name = "stage{}.{}".format(si + 1, bi)
+        b.u1 = _Unit(st, name + ".u1", cin, width, 3, stride)
+        b.u2 = _Unit(st, name + ".u2", width, width, 3, 1, zero_gamma=True)
+        b.ds = _Unit(st, name + ".ds", cin, width, 1, stride) if stride != 1 else None
+        b.stride, b.width = stride, width
+        blocks.append(b)
+        cin = width
+    fc = Dense(st, "fc", 64, (num_classes + 7) // 8 * 8, bias=True, init=normal(0.01))
+    return stem, blocks, fc
+
+  @staticmethod
+  def _valid_depth(depth):
+    return (isinstance(depth, numbers.Integral) and not isinstance(depth, bool) and depth >= 8 and
+            (depth - 2) % 6 == 0)
 
   synthetic_batch = ResNetTrainer.synthetic_batch
   state_dict = ResNetTrainer.state_dict
@@ -1238,21 +1408,27 @@ class CifarResNetTrainer(object):
         units.append((u.conv.sw, u.bn))
     return units
 
-  def _eval_forward(self, wv, bias, u8, head=None):
-    """Folded basic-block network on the training buffers (see _Evaluator): bias + ReLU in every
-    epilogue, the shortcut into ``out``, conv2 accumulating the residual into ``out`` (projection
-    blocks) or in place into the block input (identity blocks).  ``head`` as in ResNetTrainer."""
+  def _folded_plans(self, wv, bias, x=None):
+    """The folded basic-block network on the training buffers: bias + ReLU in every epilogue, the
+    shortcut into ``out``, conv2 accumulating the residual into ``out`` (projection blocks) or in
+    place into the block input (identity blocks).  The stem reads ``x`` (default ``x8``).
+    Returns (plans, last activation)."""
     conv = lambda x, u, y, **kw: igemm.conv_fprop(  # noqa: E731
         x, wv(u.conv.sw), y, u.conv.stride, u.conv.pad, bias=bias[id(u.bn)], **kw)
     cur = self.stem_act
-    plans = [conv(self.x8, self.stem, cur, relu=True)]
+    plans = [conv(self.x8 if x is None else x, self.stem, cur, relu=True)]
     for b in self.blocks:
       plans.append(conv(cur, b.u1, b.a1, relu=True))
       if b.ds is not None:
         plans.append(conv(cur, b.ds, b.out))
         cur = b.out
       plans.append(conv(b.a1, b.u2, cur, relu=True, accumulate=True))
-    last = cur
+    return plans, cur
+
+  def _eval_forward(self, wv, bias, u8, head=None):
+    """Folded basic-block network (``_folded_plans``) on the training buffers (see _Evaluator).
+    ``head`` as in ResNetTrainer."""
+    plans, last = self._folded_plans(wv, bias)
     K = ops.K
 
     def run():
@@ -1267,6 +1443,8 @@ class CifarResNetTrainer(object):
     K = ops.K
     zero, update = self.accum.phase()
     K.decode_normalize(self.in_u8, self.x8, 0, self.mean, self.std, **self._mix_arg())
+    if self.teacher is not None:
+      self.teacher.run()      # its stem reads x8: the (mixed) input the student trains on
     self.stem.conv.forward()
     self.stem.bn.forward(self.stem_raw, self.stem_act, None, 1, True)
     for bi, b in enumerate(self.blocks):

@@ -34,6 +34,12 @@ with its reference.  Because every reference is linearised at the trainer's own 
 errors do not compound from layer to layer and the per-element bounds are those of the kernel
 suites (tools/plan_conformance.py); a wiring fault shows up as an O(1) miss.
 
+A distilling trainer's step also holds its frozen teacher's folded forward pass, right after the
+decode, and ``distill_xent`` in place of ``softmax_xent``.  ``teacher_buffers`` names the teacher's
+buffers ``teacher.*``; every teacher launch is claimed by a ``teacher.*`` layer check, its
+reference reads the student's decoded ``xp`` by name, and it may write only teacher buffers, so a
+teacher launch that writes a student buffer fails.
+
 The optimizer is checked from the snapshot before its launch: master, momentum and bf16 weights
 against float64 momentum SGD with the weight-decay partition of the network definition (convolution
 and dense weights decayed; batch-norm parameters and biases not, as ``torch.optim.SGD`` parameter
@@ -668,6 +674,8 @@ def check_resnet_step(net, launches, snaps, lr=0.1, momentum=0.9, weight_decay=1
   rep.close("decode", "decode", L, c.a("xp", L), ref,
             pc.U_BF16 * ref.abs() + (1 + pc.U_BF16) * pc.gamma(6, U) * mag, "xp")
   c.owns(L, "decode", "xp")
+  if getattr(net, "teacher", None) is not None:
+    _teacher_forward(c, net.teacher)
   L = c.claims.take("stem.conv", "plan", plan=net.p_stem)
   ref, M = stem_ref(c.b("xp", L), c.w(net.stem_w, L), net.stem_raw.shape[2])
   y = c.a("stem_raw", L)
@@ -721,8 +729,18 @@ def check_resnet_step(net, launches, snaps, lr=0.1, momentum=0.9, weight_decay=1
   rep.close("fc", "head fwd", L, c.a("logits", L), ref, pc.elem_bound(ref, M, fc.cin + 1, U),
             "logits")
   c.owns(L, "fc", "logits")
-  L = c.claims.take("loss", "k", "softmax_xent")
+  if getattr(net, "teacher", None) is not None:
+    _distill_loss(c, net)
+  else:
+    _xent_loss(c, net)
+  _backward_and_update(c, net, zero, update, HW, fc, drop)
+  return rep, c.claims.finish()
+
+
+def _xent_loss(c, net):
+  rep = c.rep
   V, B = net.num_classes, net.B
+  L = c.claims.take("loss", "k", "softmax_xent")
   loss, dl, hits, tie = xent_ref(c.b("logits", L), c.S.before("labels", L), V, 1.0 / B)
   rep.close("loss", "loss", L, c.a("loss_sum", L).reshape(()), loss,
             2e-5 * abs(float(loss)) + 1e-6, "loss_sum")
@@ -736,6 +754,9 @@ def check_resnet_step(net, launches, snaps, lr=0.1, momentum=0.9, weight_decay=1
   # (loss_sum and correct are cleared by torch just before the launch: charged to it)
   c.owns(L, "loss", "dlogits", "loss_sum", "correct")
 
+
+def _backward_and_update(c, net, zero, update, HW, fc, drop):
+  rep, B = c.rep, net.B
   # ---- backward
   if zero:   # the first micro-step of an accumulation window (every step without accumulation)
     L = c.claims.take("grads", "host", "FusedOptimizer.zero_grads")
@@ -799,7 +820,6 @@ def check_resnet_step(net, launches, snaps, lr=0.1, momentum=0.9, weight_decay=1
   c.owns(L, "stem.conv", "grads")
   if update:
     _optimizer(c, 1.0 / net.accum.k)
-  return rep, c.claims.finish()
 
 
 def _stem_bwd(c, net):
@@ -858,3 +878,137 @@ def _optimizer(c, gscale=1.0):
   tail = st.total - st.decay_end
   c.rep.exact("optimizer", "optimizer", L, c.a("aux32", L)[:tail] != m[st.decay_end:], "aux32")
   c.owns(L, "optimizer", "master", "state1", "weights", "aux32")
+
+
+# ----------------------------------------------------------------------------- distillation
+def teacher_buffers(teacher):
+  """(name, tensor) of every buffer of a ResNetTrainer's distillation teacher (models/resnet.py
+  _ResNetTeacher), named ``teacher.*`` after its network definition: the folded filters
+  (``teacher.wf:<filter>``) and biases (``teacher.bf:<batch norm>``), the head's bf16 weight and
+  fp32 bias, its own (never decoded) input buffer and its activations."""
+  t = teacher.net
+  st = t.store
+  out = [("teacher.wf", t.wf), ("teacher.bf", t.bf), ("teacher.weights", st.weights),
+         ("teacher.aux32", st.aux32), ("teacher.in_u8", t.in_u8), ("teacher.xp", t.xp)]
+  off = 0
+  for spec, bn in t._fold_units():
+    out.append(("teacher.wf:" + spec["name"], st._view(t.wf, spec)))
+    out.append(("teacher.bf:" + bn.name, t.bf[off:off + bn.C]))
+    off += (bn.C + 7) // 8 * 8
+  out.append(("teacher.weights:" + t.fc.sw["name"], st.w(t.fc.sw)))
+  out.append(("teacher.aux32:" + t.fc.sbias["name"], st.f32(t.fc.sbias)))
+  for name in ("stem_act", "pool", "pool_idx", "avg", "logits"):
+    out.append(("teacher." + name, getattr(t, name)))
+  for b in t.blocks:
+    for a in ("a1", "a2", "out"):
+      out.append(("teacher.{}.{}".format(b.name, a), getattr(b, a)))
+  return out
+
+
+def _folded_conv(c, layer, plan, xname, wname, bname, yname, stride, pad, relu, accumulate=False):
+  """One folded convolution of the teacher: y = act(conv(x, w') + b' (+ y before, accumulate))."""
+  L = c.claims.take(layer, "plan", plan=plan)
+  x, w, bias = c.b(xname, L), c.b(wname, L), c.b(bname, L)
+  ref, M = conv_ref(x, w, stride, pad)
+  ref, M = ref + bias, M + bias.abs()
+  n = w.shape[1] * w.shape[2] * w.shape[3] + 1
+  # the accumulate epilogue rounds twice, RN(act(RN(conv + bias) + prev)) (plan_conformance)
+  partial, prev = ref, None
+  if accumulate:
+    prev = c.b(yname, L)
+    ref = ref + prev
+  if relu:
+    ref = ref.clamp_min(0.0)
+  bound = pc.elem_bound(ref, M, n, partial=partial if accumulate else None, prev=prev)
+  c.rep.close(layer, "teacher conv", L, c.a(yname, L), ref, bound, "y")
+  c.owns(L, layer, yname)
+
+
+def _teacher_forward(c, teacher):
+  """The teacher's folded forward pass on the student's decoded ``xp``: stem (bias + ReLU), max
+  pool, per block conv1 / conv2 (bias + ReLU), the projection (bias) and conv3 accumulating the
+  shortcut (bias + ReLU), the average pool and the head."""
+  t = teacher.net
+  plans = list(t._f_plans)
+  rep = c.rep
+  L = c.claims.take("teacher.stem.conv", "plan", plan=plans.pop(0))
+  w, bias = c.b("teacher.wf:" + t.stem_w["name"], L), c.b("teacher.bf:" + t.stem_bn.name, L)
+  ref, M = stem_ref(c.b("xp", L), w, t.stem_act.shape[2])
+  ref, M = (ref + bias).clamp_min(0.0), M + bias.abs()
+  rep.close("teacher.stem.conv", "teacher conv", L, c.a("teacher.stem_act", L), ref,
+            pc.elem_bound(ref, M, 7 * 64 + 2), "y")
+  c.owns(L, "teacher.stem.conv", "teacher.stem_act")
+  L = c.claims.take("teacher.maxpool", "k", "maxpool_fwd")
+  ry, ridx = kc.maxpool_ref(c.b("teacher.stem_act", L), 3, 2, 1)
+  rep.exact("teacher.maxpool", "teacher pool", L, (f64(c.a("teacher.pool", L)) != ry) |
+            (c.a("teacher.pool_idx", L).long() != ridx), "pool / idx")
+  c.owns(L, "teacher.maxpool", "teacher.pool", "teacher.pool_idx")
+  cur = "teacher.pool"
+  for b in t.blocks:
+    n = "teacher." + b.name
+    wf = lambda u: "teacher.wf:" + u.conv.sw["name"]   # noqa: E731
+    bf = lambda u: "teacher.bf:" + u.bn.name            # noqa: E731
+    _folded_conv(c, n + ".u1.conv", plans.pop(0), cur, wf(b.u1), bf(b.u1), n + ".a1", 1, 0, True)
+    _folded_conv(c, n + ".u2.conv", plans.pop(0), n + ".a1", wf(b.u2), bf(b.u2), n + ".a2",
+                 b.stride, 1, True)
+    if b.ds is not None:
+      _folded_conv(c, n + ".ds.conv", plans.pop(0), cur, wf(b.ds), bf(b.ds), n + ".out", b.stride,
+                   0, False)
+      cur = n + ".out"
+    # identity blocks accumulate in place into the block input
+    _folded_conv(c, n + ".u3.conv", plans.pop(0), n + ".a2", wf(b.u3), bf(b.u3), cur, 1, 0, True,
+                 accumulate=True)
+  assert not plans, "teacher plans left unclaimed"
+  L = c.claims.take("teacher.avgpool", "k", "avgpool_fwd")
+  ref, mag = kc.avgpool_ref(c.b(cur, L))
+  HW = math.prod(t._f_last.shape[1:3])
+  rep.close("teacher.avgpool", "teacher pool", L, c.a("teacher.avg", L), ref,
+            pc.U_BF16 * ref.abs() + (1 + pc.U_BF16) * pc.gamma(HW + 3, U) * mag, "avg")
+  c.owns(L, "teacher.avgpool", "teacher.avg")
+  fc = t.fc
+  L = c.claims.take("teacher.fc", "plan", plan=fc.fwd)
+  a = c.b("teacher.avg", L)
+  w = c.b("teacher.weights:" + fc.sw["name"], L)
+  bias = c.b("teacher.aux32:" + fc.sbias["name"], L)
+  ref = a @ w.t() + bias
+  M = a.abs() @ w.abs().t() + bias.abs()
+  rep.close("teacher.fc", "teacher head", L, c.a("teacher.logits", L), ref,
+            pc.elem_bound(ref, M, fc.cin + 1, U), "logits")
+  c.owns(L, "teacher.fc", "teacher.logits")
+
+
+def distill_ref(s, z, labels, V, eps, alpha, T, scale):
+  """(summed loss, dlogits [B, V]) of the distillation loss without a mix, float64:
+  (1 - alpha) CE(s, smoothed one-hot) + alpha T^2 KL(softmax(z / T) || softmax(s / T))."""
+  s, z = s[:, :V], z[:, :V]
+  t = F.one_hot(labels.long(), V).to(s.dtype) * (1.0 - eps) + eps / V
+  ls, lsT, lq = torch.log_softmax(s, 1), torch.log_softmax(s / T, 1), torch.log_softmax(z / T, 1)
+  q = lq.exp()
+  loss = ((1 - alpha) * -(t * ls).sum(1) + alpha * T * T * (q * (lq - lsT)).sum(1)).sum() * scale
+  d = ((1 - alpha) * (ls.exp() - t) + alpha * T * (lsT.exp() - q)) * scale
+  return loss, d
+
+
+def _distill_loss(c, net):
+  """distill_xent on the student's logits and the teacher's, as the two layers left them."""
+  rep = c.rep
+  V, B = net.num_classes, net.B
+  L = c.claims.take("loss", "k", "distill_xent")
+  if net.mix is not None:
+    rep.fail(L, "loss", "the step check covers distillation without Mixup / CutMix")
+    return
+  T, alpha = net.distill_temperature, net.distill_alpha
+  s, z = c.b("logits", L), c.b("teacher.logits", L)
+  loss, dl = distill_ref(s, z, c.S.before("labels", L), V, net.label_smoothing, alpha, T, 1.0 / B)
+  rep.close("loss", "distill loss", L, c.a("loss_sum", L).reshape(()), loss,
+            4e-5 * abs(float(loss)) + 1e-6, "loss_sum")
+  got = c.a("dlogits", L)
+  rep.close("loss", "distill loss", L, got[:, :V], dl,
+            pc.U_BF16 * dl.abs() + 1e-5 * (1 + T) / B, "dlogits")
+  if net.VP > V:
+    rep.exact("loss", "distill loss", L, got[:, V:] != 0, "dlogits padding")
+  _, _, hits, tie = xent_ref(s, c.S.before("labels", L), V, 1.0 / B)
+  nh = float(c.a("correct", L))
+  if not int(hits[~tie].sum()) <= nh <= int(hits[~tie].sum()) + int(tie.sum()):
+    rep.fail(L, "loss", "correct {} against {} top-1 hits".format(nh, int(hits.sum())))
+  c.owns(L, "loss", "dlogits", "loss_sum", "correct")
